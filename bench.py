@@ -7,12 +7,18 @@
 `value` (every N): LLaMA-3-8B bf16 paged-KV decode (BASELINE.json configs[1]), bs=16, seq=4096, tensor-parallel
 over the N ranks (column/row shards + all-reduce exactly where chitu/tensor_parallel.py:166 reduces) -> strong scaling.
 The SAME JSON line also carries the north-star configuration (BASELINE.json configs[3]) under the driver's clock:
-    N = 8 : "deepseek_r1_tp8"    DeepSeek-R1 671B FP8 MLA-absorb paged decode, all 61 layers, tp=8, bs=16 and bs=1
-    N = 1 : "deepseek_r1_shard"  ONE rank's tp=8 shard (85 GB of FP8 weights, 61 layers) without collectives
-    N = 2/4: "deepseek_r1_reduced" tp=N with a reduced layer count (SURVEY §8e: the full model only fits at tp=8)
+    N = 1 : "deepseek_r1_shard"  ONE rank's tp=16 shard (42 GB of FP8 weights, 61 layers) without collectives: the
+            smallest tensor-parallel degree at which the FP8 model fits 80 GB H100s (two 8-GPU nodes)
+    N = 2/4/8: "deepseek_r1_reduced" tp=N with a reduced layer count (12 / 24 / 40 of 61 layers) so that one rank's FP8
+            weights stay within ~55-62 GB of an 80 GB H100: the full 61 layers need ~85 GB per rank at tp=8
 each with tokens/s, ms/step, counted distinct experts, algorithmic bytes and the step's fraction of the HBM roofline
-against the MEASURED peak and against the nominal 8 TB/s, and its own clocks record.
-A "step" = one decode step of the whole model for the whole batch.
+against the measured peak (when MEASURED_PEAKS.json exists) or the H100 SXM data sheet's 3.35 TB/s, and its own clocks
+record.  A "step" = one decode step of the whole model for the whole batch.
+
+--dump-outputs DIR writes, after the timed steps, what the last timed step of every engine returned to its caller
+(logits and next tokens, float32 / float64 .npy; logits over 12 MB as a fixed, seeded sample of vocabulary columns; at
+most 64 MB in all; with tensor parallelism rank 0's vocabulary shard of the logits).  Inputs are seeded, so two builds
+given the same arguments can be compared output for output.
 """
 import argparse
 import dataclasses
@@ -27,24 +33,7 @@ sys.path.insert(0, ROOT)
 
 METRIC = "decode tokens/s at bs=16 (LLaMA-3-8B bf16 paged-KV, seq=4096)"
 UNIT = "tokens/s"
-NOMINAL_HBM_GBS = 8000.0
-
-
-def measured_traffic(kernel_name):
-    """DRAM bytes per launch of the roofline kernel from the committed ncu capture (profiles/traffic.json); entries are
-    matched by their `M=.. N=.. K=..` shape."""
-    import re
-    p = os.path.join(ROOT, "profiles", "traffic.json")
-    try:
-        shape = re.search(r"M=\d+ N=\d+ K=\d+", kernel_name).group(0)
-        with open(p) as f:
-            table = json.load(f)
-        for k, e in table.items():
-            if isinstance(e, dict) and shape in k:
-                return int(e["bytes"])
-        return None
-    except Exception:
-        return None
+NOMINAL_HBM_GBS = 3350.0          # H100 SXM data sheet (HBM3)
 
 
 def peaks():
@@ -52,11 +41,11 @@ def peaks():
     if os.path.exists(p):
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return NOMINAL_HBM_GBS, "H100 SXM data sheet (not measured)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md).
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region.
 
     The query loop is started before the warm-up (nvidia-smi needs ~100 ms to initialise); a reader thread
     stamps every sample on arrival and `stop()` keeps the samples that fall into [mark_begin, mark_end].
@@ -142,9 +131,45 @@ def dist_env():
     return world, rank, local
 
 
-def time_engine(eng, B, S, args, world, dev, sampler=None):
+DUMP_BUDGET_BYTES = 64 << 20          # --dump-outputs writes at most this much in all
+DUMP_LOGITS_BYTES = 12 << 20          # per logits array; larger ones are sampled
+
+
+def dump_outputs(args, label, eng, next_tokens):
+    """--dump-outputs: the logits and next tokens of the engine's last timed step -> DIR/<label>_*.npy.  Logits larger
+    than DUMP_LOGITS_BYTES (float32) keep a fixed, seeded sample of vocabulary columns, written beside them as
+    <label>_logits_cols.npy; nothing more is written once DUMP_BUDGET_BYTES is used.  With tensor parallelism the logits
+    are rank 0's vocabulary shard (the next tokens are global)."""
+    import numpy as np
+    import torch
+    if not getattr(args, "dump_outputs", None):
+        return
+    os.makedirs(args.dump_outputs, exist_ok=True)
+    logits = eng.logits.float()
+    rows, cols = logits.shape
+    arrays = {}
+    if rows * cols * 4 > DUMP_LOGITS_BYTES:
+        k = max(1, DUMP_LOGITS_BYTES // (rows * 4))
+        pick = torch.randperm(cols, generator=torch.Generator().manual_seed(0))[:k].sort().values
+        arrays["logits"] = logits[:, pick.to(logits.device)].cpu().numpy()
+        arrays["logits_cols"] = pick.numpy().astype(np.float64)
+    else:
+        arrays["logits"] = logits.cpu().numpy()
+    arrays["next_tokens"] = next_tokens.cpu().numpy().astype(np.float64)
+    used = getattr(args, "_dump_bytes", 0)
+    for name, a in arrays.items():
+        if used + a.nbytes > DUMP_BUDGET_BYTES:
+            print(f"--dump-outputs: {label}_{name} skipped (the {DUMP_BUDGET_BYTES >> 20} MB budget is used)", file=sys.stderr)
+            continue
+        np.save(os.path.join(args.dump_outputs, f"{label}_{name}.npy"), a)
+        used += a.nbytes
+    args._dump_bytes = used
+
+
+def time_engine(eng, B, S, args, world, dev, sampler=None, label=None):
     """W untimed warm-up steps, K device-timed steps (CUDA events between barriers, max over ranks), then K end-to-end
-    steps through the public `decode()` (pinned host tokens in, host tokens out).  Returns ms/step, e2e ms/step, clocks."""
+    steps through the public `decode()` (pinned host tokens in, host tokens out).  Returns ms/step, e2e ms/step, clocks.
+    With --dump-outputs, what the last end-to-end step returned is written under `label`."""
     import torch
     import torch.distributed as dist
 
@@ -153,7 +178,8 @@ def time_engine(eng, B, S, args, world, dev, sampler=None):
             dist.barrier()
         torch.cuda.synchronize()
 
-    tokens_host = torch.randint(100, 1000, (B,), dtype=torch.int64).pin_memory()      # gen_reqs_fake range
+    tokens_host = torch.randint(100, 1000, (B,), dtype=torch.int64,                  # gen_reqs_fake range
+                                generator=torch.Generator().manual_seed(B)).pin_memory()
     eng.tokens.copy_(tokens_host)
     if sampler is not None:
         sampler.start()
@@ -177,9 +203,11 @@ def time_engine(eng, B, S, args, world, dev, sampler=None):
     barrier()
     t0 = time.perf_counter()
     for _ in range(args.steps):
-        eng.decode(tokens_host)          # H2D tokens + graph replay + D2H next tokens (sync)
+        nxt = eng.decode(tokens_host)    # H2D tokens + graph replay + D2H next tokens (sync)
     barrier()
     e2e_ms = (time.perf_counter() - t0) * 1e3
+    if label is not None and args.steps > 0 and int(os.environ.get("RANK", "0")) == 0:
+        dump_outputs(args, label, eng, nxt)
     t = torch.tensor([ms, e2e_ms], dtype=torch.float64, device=dev)
     if world > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -271,7 +299,7 @@ def run_llama(args, world, rank, local, pg):
         eng.set_synthetic_context(S)
         eng.capture()
         sampler = ClockSampler(local) if (B == args.bs and rank == 0) else None
-        ms, e2e_ms, clocks = time_engine(eng, B, S, args, world, dev, sampler)
+        ms, e2e_ms, clocks = time_engine(eng, B, S, args, world, dev, sampler, label=f"llama3_8b_bs{B}")
         results[B] = dict(ms_per_step=ms, e2e_ms_per_step=e2e_ms, launches_per_step=eng.launches_per_step, clocks=clocks)
         if B == args.bs and world == 1:
             results["gemms"] = gemm_table(eng, B, args)
@@ -282,16 +310,16 @@ def run_llama(args, world, rank, local, pg):
 
 def deepseek_variant(world):
     """(label, tp, n_layers, n_dense, note) of the DeepSeek-R1 block reported at this GPU count (SURVEY §8e)."""
-    if world == 8:
-        return "deepseek_r1_tp8", 8, 61, 3, "full model: 61 layers, tp=8, fused NVLink all-reduce where the reference reduces"
     if world == 1:
-        return ("deepseek_r1_shard", 8, 61, 3,
-                "ONE rank's tp=8 shard of the full 61-layer model on one GPU, no collectives (per-rank kernel time of the "
-                "tp=8 configuration; NOT a 1-GPU DeepSeek-R1)")
-    layers = {2: 12, 4: 24}.get(world, 8)
+        return ("deepseek_r1_shard", 16, 61, 3,
+                "ONE rank's tp=16 shard of the full 61-layer model on one GPU, no collectives (per-rank kernel time of the "
+                "tp=16 configuration that fits 80 GB H100s; NOT a 1-GPU DeepSeek-R1)")
+    # per rank: a MoE layer holds 1.42 GB x (8 / tp) of FP8 experts; the layer count keeps the weights within ~62 GB so
+    # that the KV cache and workspaces fit an 80 GB H100 (61 layers at tp=8 would need ~85 GB)
+    layers = {2: 12, 4: 24, 8: 40}.get(world, 8)
     return ("deepseek_r1_reduced", world, layers, 3,
-            f"REDUCED model: {layers} of 61 layers (3 dense + {layers - 3} MoE) at tp={world} — the full model only fits at "
-            "tp=8 (SURVEY §8e); tokens/s of this variant are not comparable with the 61-layer numbers")
+            f"REDUCED model: {layers} of 61 layers (3 dense + {layers - 3} MoE) at tp={world}, sized for 80 GB per GPU — the "
+            "full FP8 model needs tp >= 16 on 80 GB GPUs; tokens/s of this variant are not comparable with the 61-layer numbers")
 
 
 def run_deepseek_block(args, world, rank, local, pg, tp=None, layers=None):
@@ -314,14 +342,14 @@ def run_deepseek_block(args, world, rank, local, pg, tp=None, layers=None):
         eng.set_synthetic_context(S)
         eng.capture()
         sampler = ClockSampler(local) if rank == 0 else None
-        ms, e2e_ms, clocks = time_engine(eng, B, S, args, world, dev, sampler)
+        ms, e2e_ms, clocks = time_engine(eng, B, S, args, world, dev, sampler, label=f"{label}_bs{B}")
         distinct = eng.distinct_experts_per_layer()
         nbytes = eng.algorithmic_bytes(S, distinct)
         gbs = nbytes / (ms * 1e-3) / 1e9
         out[B] = {"tokens_per_s": B / (ms * 1e-3), "ms_per_step": ms, "e2e_tokens_per_s": B / (e2e_ms * 1e-3),
                   "distinct_experts_per_layer": distinct, "algorithmic_bytes_per_rank": nbytes,
                   "achieved_gbs_per_rank": gbs, "step_frac_of_measured_peak": gbs / peak,
-                  "step_frac_of_nominal_8tbs": gbs / NOMINAL_HBM_GBS, "launches_per_step": int(eng.launches_per_step),
+                  "step_frac_of_datasheet_hbm": gbs / NOMINAL_HBM_GBS, "launches_per_step": int(eng.launches_per_step),
                   "clocks": clocks}
         del eng
         torch.cuda.empty_cache()
@@ -370,7 +398,7 @@ def run_cuda(args):
     peak, peak_src = peaks()
     step_gbs = total_bytes / (r["ms_per_step"] * 1e-3) / 1e9
     roof = {"bound": "hbm", "peak": peak, "unit": "GB/s", "peak_source": peak_src,
-            "step_achieved_gbs": step_gbs, "step_frac": step_gbs / peak, "step_frac_of_nominal_8tbs": step_gbs / NOMINAL_HBM_GBS,
+            "step_achieved_gbs": step_gbs, "step_frac": step_gbs / peak, "step_frac_of_datasheet_hbm": step_gbs / NOMINAL_HBM_GBS,
             "step_algorithmic_bytes": total_bytes}
     if "gemms" in results:
         g = results["gemms"]
@@ -378,23 +406,22 @@ def run_cuda(args):
         tot_ms = sum(x["ms"] * x["launches_per_step"] for x in g)
         best = max(g, key=lambda x: x["bytes"] / x["ms"])
         achieved = tot_b / (tot_ms * 1e-3) / 1e9
-        roof.update({"kernel": "tc_gemm_kernel<bf16,16> (tcgen05 swap-AB weight-streaming GEMM), launch-weighted over the "
+        roof.update({"kernel": "tc_gemm_kernel<bf16,16> (wgmma swap-AB weight-streaming GEMM), launch-weighted over the "
                                "four layer shapes x 32 layers (128 of the step's launches)",
                      "achieved": achieved, "frac": achieved / peak, "kernel_ms_per_step": tot_ms,
-                     "kernel_share_of_step": tot_ms / r["ms_per_step"], "traffic": measured_traffic(best["name"]),
-                     "traffic_kernel": best["name"],
+                     "kernel_share_of_step": tot_ms / r["ms_per_step"], "best_kernel": best["name"],
                      "per_shape": [{"name": x["name"], "us": x["ms"] * 1e3, "gbs": x["bytes"] / (x["ms"] * 1e-3) / 1e9,
                                     "frac": x["bytes"] / (x["ms"] * 1e-3) / 1e9 / peak, "bytes": x["bytes"]} for x in g]})
     else:
         roof.update({"kernel": "whole decode step (per-rank algorithmic bytes / step time)", "achieved": step_gbs,
-                     "frac": step_gbs / peak, "traffic": None})
+                     "frac": step_gbs / peak})
     line = {
         "metric": METRIC, "value": B / (r["ms_per_step"] * 1e-3), "unit": UNIT, "n_gpus": world,
         "steps": args.steps, "warmup": args.warmup, "ms_per_step": r["ms_per_step"], "higher_is_better": True,
         "scaling": "strong", "vs_baseline": None, "dtype": "bf16", "data": "synthetic",
         "config": {"workload": f"LLaMA-3-8B bf16 paged-KV decode, bs={B}, seq={S}, page=256, tp={world}",
                    "global_batch": B, "seq_len": S, "parallelism": f"tp{world}",
-                   "l2": "inputs larger than L2: %.1f GB of weights+KV streamed per step vs 126 MB L2" % (total_bytes / 1e9),
+                   "l2": "inputs larger than L2: %.1f GB of weights+KV streamed per step vs 50 MB L2" % (total_bytes / 1e9),
                    "cuda_graph": True, "linear_impl": args.linear_impl,
                    "allreduce": "none" if world == 1 else ("nccl" if args.nccl_allreduce else "fused one-shot NVLink peer-memory all-reduce + residual + RMSNorm")},
         "bs1": {"value": 1 / (results[1]["ms_per_step"] * 1e-3), "ms_per_step": results[1]["ms_per_step"],
@@ -451,7 +478,7 @@ def run_deepseek(args):
         "roofline": {"bound": "hbm", "achieved": r["achieved_gbs_per_rank"], "peak": ds["peak_gbs"], "unit": "GB/s",
                      "frac": r["step_frac_of_measured_peak"], "traffic": None,
                      "kernel": "whole decode step (per-rank algorithmic bytes / step time)", "peak_source": ds["peak_source"],
-                     "step_frac_of_nominal_8tbs": r["step_frac_of_nominal_8tbs"],
+                     "step_frac_of_datasheet_hbm": r["step_frac_of_datasheet_hbm"],
                      "step_algorithmic_bytes": r["algorithmic_bytes_per_rank"]},
     }
     print(json.dumps(line))
@@ -837,7 +864,7 @@ def main():
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--bs", type=int, default=16)
     ap.add_argument("--seq", type=int, default=4096)
-    ap.add_argument("--linear-impl", type=int, default=0, help="0 auto, 1 SIMT, 2 tcgen05")
+    ap.add_argument("--linear-impl", type=int, default=0, help="0 auto, 1 SIMT, 2 wgmma")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-deepseek", action="store_true", help="skip the DeepSeek-R1 block of the default line")
     ap.add_argument("--no-mgpu-check", action="store_true", help="skip the multi-GPU parity preamble (N > 1)")
@@ -845,6 +872,8 @@ def main():
     ap.add_argument("--workload", default="llama3-8b", choices=["llama3-8b", "deepseek-r1", "w8a8-sweep", "mixtral", "ref-kernels"])
     ap.add_argument("--tp", type=int, default=0, help="deepseek-r1: tensor-parallel degree that shapes the shard")
     ap.add_argument("--layers", type=int, default=0, help="deepseek-r1 / sweep: layer count override")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the logits / next tokens of the last timed step of every engine to DIR/<name>.npy")
     ap.add_argument("--short", action="store_true", help="--impl reference: the bounded cpu_baseline sample only (1 warm-up, "
                     "no configs[0] run, no oracle-port leg); used by our own arm's cpu_baseline subprocess")
     args = ap.parse_args()

@@ -1,4 +1,4 @@
-"""chitu_b200 — B200-native (sm_100a) decode operators behind Chitu's plugin surfaces.
+"""chitu_b200 — H100-native (sm_90a) decode operators behind Chitu's plugin surfaces.
 
 Host side mirrors the reference's operator interfaces (same names / argument meaning):
   chitu_b200.ops            <-> chitu.ops

@@ -88,7 +88,7 @@ SIGNATURES = {
 
 
 def build(verbose: bool = False) -> str:
-    """Compile every CUDA source for sm_100a into chitu_b200/libchitu_b200.so (nvcc cross-compiles
+    """Compile every CUDA source for sm_90a into chitu_b200/libchitu_b200.so (nvcc cross-compiles
     without a GPU)."""
     res = subprocess.run(["make", "-C", CSRC_DIR, "-j8"], capture_output=True, text=True)
     if res.returncode != 0:

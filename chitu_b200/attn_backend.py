@@ -36,7 +36,7 @@ class AttnBackend:
 
 
 class B200AttnBackend(AttnBackend):
-    """sm_100a decode attention.  Constructor arguments replace the reference's reads of
+    """sm_90a decode attention.  Constructor arguments replace the reference's reads of
     `get_global_args()` (attn_backend.py:508-511, 691-695) so the class is usable stand-alone;
     `from_global_args(args)` mirrors the reference construction."""
 

@@ -10,7 +10,7 @@
 // Both kernels never read the cache row of the token being appended: the CTA that owns that
 // position takes it from `k_new` directly and split 0 writes it to the cache -> no RAW hazard.
 // The reference fixes NUM_KV_SPLITS = 4 (attn_backend.py:735) -> 4 CTAs at B=1; here the split
-// count is sized from the SM count so 148 SMs are busy at B=1.
+// count is sized from the SM count so the 132 SMs of an H100 are busy at B=1.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -1134,7 +1134,7 @@ __global__ void __launch_bounds__(160, 1) mla_decode_mma_kernel(
 }
 
 inline int pick_splits_1cta(int ctas_without_split, int max_len) {
-  int want = (148 * 3 + ctas_without_split - 1) / ctas_without_split;
+  int want = (132 * 3 + ctas_without_split - 1) / ctas_without_split;
   int by_len = (max_len + 255) / 256;
   int s = want < by_len ? want : by_len;
   if (s > 64) s = 64;
@@ -1159,7 +1159,7 @@ inline int pick_splits_waves(int ctas_without_split, int max_len, int slots) {
 }
 
 inline int pick_splits(int ctas_without_split, int max_len, int min_keys_per_split, int max_splits) {
-  int want = (148 * 4 + ctas_without_split - 1) / ctas_without_split;  // ~4 CTAs per SM
+  int want = (132 * 4 + ctas_without_split - 1) / ctas_without_split;  // ~4 CTAs per SM
   int by_len = (max_len + min_keys_per_split - 1) / min_keys_per_split;
   int s = want < by_len ? want : by_len;
   if (s > max_splits) s = max_splits;
@@ -1229,7 +1229,7 @@ extern "C" int chitu_b200_gqa_paged_decode_rope(const void* q, int64_t q_sb, voi
     const int gqa_cfg = e_cfg ? atoi(e_cfg) : 5;
     if (rope_cos && gqa_cfg < 4) return fail(-2, "gqa_paged_decode_rope: the heads-as-M kernel has no fused rotary");
     const int ctas_per_sm = (gqa_cfg == 2 || gqa_cfg == 6 || gqa_cfg == 8) ? 2 : 1;
-    splits = e_spl ? atoi(e_spl) : pick_splits_waves(B * Hkv, max_len, 148 * ctas_per_sm);
+    splits = e_spl ? atoi(e_spl) : pick_splits_waves(B * Hkv, max_len, 132 * ctas_per_sm);
     if (splits < 1) splits = 1;
     splits = workspace ? splits_that_fit(splits, B, Hq, D, workspace_bytes) : 1;
     lse = o_part ? o_part + (int64_t)B * Hq * splits * D : nullptr;
@@ -1315,11 +1315,11 @@ int mla_decode_tc_launch(const void* q_nope, const void* q_pe, void* kv_cache, c
                          const int32_t* seqlens_excl, const int32_t* block_table, int bt_stride, int B, int H,
                          int num_blocks, int num_splits, float scale, void* out, float* o_part, float* lse,
                          const int32_t* plan, cudaStream_t st);
-// KV splits of the tcgen05 MLA kernel (1 CTA per SM): one wave of CTAs, whole pages, at least two pages per split, and
+// KV splits of the wgmma MLA kernel (1 CTA per SM): one wave of CTAs, whole pages, at least two pages per split, and
 // the partials must fit the workspace.  Deterministic in its arguments: the merging absorb-o kernel recomputes it.
 int mla_tc_num_splits(int B, int H, int max_len, int64_t workspace_bytes) {
   const int hgroups = cdiv(H, 16);
-  int want = 148 / (B * hgroups);
+  int want = 132 / (B * hgroups);
   const int pages = cdiv(max_len, 64);
   int by_len = pages / 2;
   int splits = want < by_len ? want : by_len;
@@ -1348,7 +1348,7 @@ extern "C" int chitu_b200_mla_decode(const void* q_nope, const void* q_pe, void*
   const int hgroups = cdiv(H, 16);
   int max_len = max_seqlen_hint > 0 ? max_seqlen_hint : bt_stride * page_size;
   cudaStream_t st = (cudaStream_t)stream;
-  // implementation (A/B switch CHITU_B200_MLA_IMPL): 0 / unset = tcgen05 kernel (mla_tc.cu), 1 = mma.sync kernel,
+  // implementation (A/B switch CHITU_B200_MLA_IMPL): 0 / unset = wgmma kernel (mla_tc.cu), 1 = mma.sync kernel,
   // 2 = SIMT kernel; pages other than 64 tokens only run on the SIMT kernel
   static const int impl_env = getenv("CHITU_B200_MLA_IMPL") ? atoi(getenv("CHITU_B200_MLA_IMPL"))
                                                             : (getenv("CHITU_B200_MLA_SIMT") ? 2 : 0);
@@ -1371,12 +1371,12 @@ extern "C" int chitu_b200_mla_decode(const void* q_nope, const void* q_pe, void*
     }
     return 0;
   }
-  if (!out) return fail(-1, "mla_decode: out == NULL (deferred merge) needs the tcgen05 kernel (page 64, TMA)");
+  if (!out) return fail(-1, "mla_decode: out == NULL (deferred merge) needs the wgmma kernel (page 64, TMA)");
   int splits;
   float *o_part, *lse;
   if (use_mma) {
     // one CTA per SM (2 x 72 KB page stages): ~2 CTAs per SM in total, whole pages per split
-    int want = (148 * 2 + B * hgroups - 1) / (B * hgroups);
+    int want = (132 * 2 + B * hgroups - 1) / (B * hgroups);
     // at least 4 pages per CTA: a one-page split has no pipeline and makes the merge a long chain of
     // dependent L2 round trips (65 splits at bs=1 cost 14 us in the merge alone)
     int by_len = (max_len + 4 * kMtTile - 1) / (4 * kMtTile);

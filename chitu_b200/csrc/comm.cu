@@ -454,7 +454,7 @@ extern "C" int chitu_b200_comm_create(int rank, int world, int64_t slot_bytes, v
     const char* e = getenv("CHITU_B200_COMM_TIMEOUT_S");
     const double sec = e ? atof(e) : 600.0;
     c->timeout_ns = sec > 0 ? (uint64_t)(sec * 1e9) : 0;
-    int dev = 0, sms = 148, per_sm = 1;
+    int dev = 0, sms = 132, per_sm = 1;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, allreduce_norm_kernel, 256, 0) != cudaSuccess || per_sm < 1) per_sm = 1;

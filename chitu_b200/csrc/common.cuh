@@ -1,4 +1,4 @@
-// Shared helpers for libchitu_b200 (sm_100a only).
+// Shared helpers for libchitu_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -43,8 +43,8 @@ static inline int cdiv(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
 // ---- programmatic dependent launch (PDL) ----------------------------------------------------
 // Every kernel of this library is launched with cudaLaunchAttributeProgrammaticStreamSerialization
 // and starts with pdl_prologue(): `griddepcontrol.launch_dependents` lets the NEXT kernel of the
-// stream be scheduled as soon as SM resources free up (its launch latency, barrier init, TMEM
-// allocation, tensormap prefetch overlap this kernel's tail), `griddepcontrol.wait` blocks until
+// stream be scheduled as soon as SM resources free up (its launch latency, barrier init,
+// tensormap prefetch overlap this kernel's tail), `griddepcontrol.wait` blocks until
 // the PREVIOUS kernel has completed and flushed — so no kernel touches global memory before its
 // predecessor is done.  Inside CUDA graphs this becomes a programmatic dependency edge.
 bool pdl_enabled();

@@ -346,7 +346,7 @@ extern "C" int chitu_b200_attn_plan(const int32_t* seqlens_incl, int B, int head
   CB_ARG(seqlens_incl && workspace && workspace_bytes >= 512 && B >= 0 && heads > 0 && page_size > 0 && max_seqlen_hint > 0);
   if (B == 0) return 0;
   const int hgroups = cb::cdiv(heads, 16);
-  int slots = 148 / hgroups;
+  int slots = 132 / hgroups;                                  // one CTA per H100 SM
   if (slots < 1) slots = 1;
   // the grid the decode kernel will be launched with for this (B, heads, hint): upper bound of a request's splits
   const int max_splits = chitu_b200_mla_num_splits(B, heads, max_seqlen_hint, workspace_bytes);

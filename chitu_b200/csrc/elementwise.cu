@@ -401,7 +401,7 @@ extern "C" int chitu_b200_silu_and_mul(const void* x, void* out, int64_t rows, i
   cudaStream_t st = (cudaStream_t)stream;
   int64_t n = rows * d;
   int blocks = (int)((n + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   if (dtype == CB_BF16)
     cb::launch_k(silu_and_mul_kernel<__nv_bfloat16>, dim3(blocks), dim3(256), 0, st, (const __nv_bfloat16*)x, (__nv_bfloat16*)out, rows, d);
   else if (dtype == CB_F16)
@@ -421,7 +421,7 @@ extern "C" int chitu_b200_silu_and_mul(const void* x, void* out, int64_t rows, i
 //                                                               y = fp8(clamp(x / s, -448, 448))
 // The division x / s is an IEEE fp32 division in both (Triton `/` on fp32 is div.full? no:
 // Triton lowers fp32 `/` to div.full.f32 — ~2 ulp — unless IEEE rounding is requested; the CPU
-// interpreter and this kernel use correctly-rounded division, see DESIGN.md §parity).
+// interpreter and this kernel use correctly-rounded division).
 // ============================================================================================
 template <typename T>
 __global__ void act_quant_fp8_kernel(const T* __restrict__ x, uint8_t* __restrict__ y,
@@ -587,7 +587,7 @@ extern "C" int chitu_b200_add(const void* a, const void* b, void* y, int64_t n, 
   CB_ARG(a && b && y && n >= 0);
   if (n == 0) return 0;
   int blocks = (int)((n + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   cudaStream_t st = (cudaStream_t)stream;
   if (dtype == CB_BF16)
     cb::launch_k(add_kernel<__nv_bfloat16>, dim3(blocks), dim3(256), 0, st, (const __nv_bfloat16*)a, (const __nv_bfloat16*)b, (__nv_bfloat16*)y, n);

@@ -1,22 +1,21 @@
-// tcgen05 + TMA weight-streaming skinny GEMM for decode linears (sm_100a only).
+// wgmma + TMA weight-streaming skinny GEMM for decode linears (sm_90a).
 //
 //   y[M,N] = x[M,K] · W[N,K]^T        M = decode tokens (1..256), N x K = nn.Linear weight
 //
-// Swap-AB mapping (SURVEY §7.3-1): the WEIGHT tile is the 128-row UMMA "A" operand, the tokens
-// are the UMMA "N" dimension (BN = 16/32/64/128), so one `tcgen05.mma.cta_group::1` of shape
-// M=128 x N=BN x K=32 bytes consumes 4 KB of weights however small the batch is; the tensor pipe
-// is <10 % busy and the kernel is a pure HBM stream:
-//   warp 0   : TMA producer   — cp.async.bulk.tensor.2d, 128B-swizzled boxes W[128 rows x 128 B] and
-//              X[BN rows x 128 B] into an S-stage shared-memory ring (mbarrier full/empty), weights
-//              with an L2 evict-first policy (read exactly once), activations evict-last.
-//   warp 1   : MMA issuer     — one elected lane, 4 MMAs per stage, accumulators in TMEM.
-//   warps 2-5: epilogue       — tcgen05.ld the 128 x BN fp32 tile (one output feature per thread),
-//              FP8: per-128-K-block drain with a_s[m,kb]*b_s[n/128,kb] applied to the fp32 partial
-//              product exactly as the reference does (triton_kernels.py:357) — every K block gets
-//              its own TMEM accumulator slot (ring of R slots) so MMA and drain overlap;
-//              bf16 / int8: one accumulator, drained once.
-// Split-K fills the 148 SMs when N/128 tiles are too few: fp32 (int32) partials go to a
-// workspace, the last CTA of a tile (atomic ticket) reduces them in split order -> deterministic.
+// Swap-AB mapping (SURVEY §7.3-1): the WEIGHT tile is the wgmma "A" operand (128 rows = two warpgroups of M = 64), the
+// tokens are the wgmma "N" dimension (BN = 16/32/64/128), so one 128 B stage row of K consumes 16 KB of weights however
+// small the batch is; the tensor pipe is mostly idle and the kernel is a pure HBM stream:
+//   warps 0-7: two consumer warpgroups — warpgroup g multiplies weight rows [64 g, 64 g + 64) of the tile with the
+//              tokens, accumulators in registers (BN / 2 per thread), then runs the epilogue for its rows.
+//              FP8: every 128-K block is multiplied into a fresh accumulator and added with a_s[m,kb]*b_s[n/128,kb]
+//              applied to the fp32 partial product exactly as the reference does (triton_kernels.py:357);
+//              bf16 / int8: one accumulator per work item.
+//   warp 8   : TMA producer — cp.async.bulk.tensor.2d, 128B-swizzled boxes W[128 rows x 128 B] and X[BN rows x 128 B]
+//              into an S-stage shared-memory ring (mbarrier full/empty), weights with an L2 evict-first policy (read
+//              exactly once), activations evict-last.
+//   soft fp8 : 8 more warps convert each fp8 weight stage to bf16 for the bf16 MMA.
+// Split-K fills the SMs when N/128 tiles are too few: fp32 (int32) partials go to a workspace, the last CTA of a tile
+// half (atomic ticket) reduces them in split order -> deterministic.
 //
 // Reference semantics implemented here:
 //   kind 0: F.linear bf16/fp16 (+bias fp32-joined, +residual as a separate rounding)
@@ -27,9 +26,11 @@
 #include <stdlib.h>
 
 #include <mutex>
+#include <type_traits>
 
 #include "common.cuh"
 #include "tc_ptx.cuh"
+#include "wgmma.cuh"
 
 namespace cb {
 
@@ -37,66 +38,12 @@ namespace {
 
 enum { KIND_16 = 0, KIND_FP8 = 1, KIND_I8 = 2, KIND_SOFT = 3 };   // SOFT: fp8 weights -> bf16 in shared memory, bf16 MMA
 
-constexpr int kTileN = 128;        // weight rows per CTA (UMMA M)
+constexpr int kTileN = 128;        // weight rows per CTA tile (two wgmma M = 64 halves)
 constexpr int kStageRowBytes = 128;  // bytes of K per stage row (one 128B swizzle atom)
-constexpr int kBaseThreads = 64;    // warp 0 (TMA producer) + warp 1 (MMA issuer); epilogue warps follow
+constexpr int kMmaThreads = 256;   // two consumer warpgroups; the producer warp and the converter warps follow
 constexpr int kGeomCache = 256;   // grouped mode: tiles whose geometry a CTA stages in shared memory
 
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] * B[smem];  KIND selects .kind::f16 / .kind::f8f6f4 / .kind::i8
-template <int KIND>
-__device__ __forceinline__ void umma(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  if constexpr (KIND == KIND_16 || KIND == KIND_SOFT) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-                 ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-  } else if constexpr (KIND == KIND_FP8) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::f8f6f4 [%0], %1, %2, %3, p;\n\t}\n"
-                 ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-  } else {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n\t}\n"
-                 ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-  }
-}
-// all previously issued MMAs of this thread arrive on `bar` when they complete
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-// 32 lanes x 16 consecutive 32-bit columns -> 16 registers per thread
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld4(uint32_t taddr, uint32_t (&r)[4]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
-               : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// K-major, 128B-swizzled operand tile (rows of 128 B, 8-row groups 1024 B apart):
-// start>>4 | LBO(16 B)>>4 <<16 | SBO(1024 B)>>4 <<32 | version 1 <<46 | SWIZZLE_128B(2) <<61
-__device__ __forceinline__ uint64_t make_kmajor_sw128_desc(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
+__device__ __forceinline__ uint64_t make_kmajor_sw128_desc(uint32_t smem_addr) { return make_sw128_desc(smem_addr, 16, 1024); }
 
 // ---------------------------------------------------------------------------------------------
 // Persistent stream-K schedule.  The global work list is the sequence of pipeline stages
@@ -113,7 +60,6 @@ struct Params {
   int n_tiles, m_chunks;
   int per;                  // stages per CTA (dense mode; grouped mode derives it on the device)
   int kblocks;              // fp8: ceil(K/128) (scale columns)
-  uint32_t idesc;
   int out_dtype;            // CB_BF16 | CB_F16
   int prefetch;             // dense mode: stream weight tiles before griddepcontrol.wait (A/B: CHITU_B200_GEMM_PREFETCH=0)
   int act_pairs;            // kind 0: weight rows (2i, 2i+1) = (gate_i, up_i); out[m, i] = SiluAndMul -> [M, N/2]
@@ -126,7 +72,7 @@ struct Params {
   void* out;                // [M, N]
   float* partial;           // [gridDim.x][2 slots][BN][128] fp32 (int32 bits for i8): a CTA has at most
                             // two partially covered tiles (its first and its last work item)
-  int* tickets;             // [tiles], zero on entry, zero on exit
+  int* tickets;             // [tiles][2 halves], zero on entry, zero on exit
   // ---- grouped (MoE experts) mode: the tile list lives in device memory (g_num_tiles != null) ----
   const int* g_num_tiles;   // number of active (expert, n-tile) tiles
   const int* g_tile_wrow;   // [tiles] first weight row of the tile in the stacked [E*Ng, K] matrix
@@ -146,34 +92,19 @@ struct Cfg {
   static constexpr int kStageX = BN * kStageRowBytes * (kSoft ? 2 : 1);
   static constexpr int kStageBytes = kStageW + kStageX;
   // soft fp8: ring of converted (bf16) weight tiles, [2 atoms][128 rows][128 B] each, between the converter warps and
-  // the MMA issuer
+  // the MMA warpgroups
   static constexpr int kCvtStages = kSoft ? 3 : 0;
   static constexpr int kCvtBytes = 2 * kTileN * kStageRowBytes;               // 32 KB
-  static constexpr int kCvtThreads = kSoft ? 256 : 0;
-  // One CTA per SM with the deepest ring that fits.  A half-SM variant for the decode-sized bf16 GEMMs (5 stages, <= 96
-  // registers, so that the NEXT kernel's CTA can become resident and prefetch during this one's split-K fix-up) was
-  // measured and dropped: every LLaMA shape 0.5-0.6 us slower in a chain, step 5.03 -> 5.13 ms (r2 call 15).
-  static constexpr int kMinCtas = 1;
+  // 3 converter warps: with the producer warp they fill a third warpgroup, so the block stays at 384 threads (registers
+  // are budgeted per 128 threads; more converter threads would cut every consumer thread to 128 registers)
+  static constexpr int kCvtThreads = kSoft ? 96 : 0;
+  static constexpr int kCvtRing = kSoft ? kCvtStages : 1;                     // modulus of the converter ring
+  // one CTA per SM with the deepest ring that fits
   static constexpr int kBudget = 200 * 1024 - kCvtStages * kCvtBytes;
   static constexpr int kStages = (kBudget / kStageBytes) > 10 ? 10 : (kBudget / kStageBytes);
-  // epilogue warp sets (4 warps = 128 TMEM lanes each) that take alternate work items: the drain of a
-  // short-K tile is a latency chain of ~400 dependent instructions, one set could not keep up with the
-  // weight stream of the K = 256 MoE down projection (ncu r1: 1.5 TB/s).  Wide tiles keep one set
-  // (their accumulators need up to 254 registers per thread).
-  // The fp8 BN = 16 kernel (MoE experts at decode batch sizes: thousands of two-stage tiles) runs four sets:
-  // more warps per scheduler is what hides the dependent-issue latency of the drain.
-  static constexpr int kEpiSets = (KIND == KIND_FP8 && BN <= 16) ? 4 : (BN <= 32 ? 2 : 1);
-  static constexpr int kThreads = kBaseThreads + 128 * kEpiSets + kCvtThreads;
-  static constexpr int kCvtWarp0 = (kBaseThreads + 128 * kEpiSets) / 32;      // first converter warp
-  // accumulator ring in TMEM: fp8 drains every stage (ring of up to 8 slots per epilogue set), the other
-  // kinds once per work item (1-2 slots per set).  Every set owns its slots and counts its own groups:
-  // an mbarrier parity wait can only tell adjacent phases apart, so a waiter must never be more than one
-  // phase ahead of the barrier it waits on.
-  static constexpr int kSlotsFp8 = (512 / BN) > 8 * kEpiSets ? 8 * kEpiSets : (512 / BN);
-  static constexpr int kSlots = KIND == KIND_FP8 ? kSlotsFp8 : (kEpiSets > 2 ? kEpiSets : 2);
-  static constexpr int kSetSlots = kSlots / kEpiSets;
-  static constexpr int kTmemColsRaw = BN * kSlots;
-  static constexpr int kTmemCols = kTmemColsRaw <= 32 ? 32 : kTmemColsRaw <= 64 ? 64 : kTmemColsRaw <= 128 ? 128 : kTmemColsRaw <= 256 ? 256 : 512;
+  static constexpr int kProducerWarp = kMmaThreads / 32;
+  static constexpr int kCvtWarp0 = kProducerWarp + 1;                         // first converter warp
+  static constexpr int kThreads = kMmaThreads + 32 + kCvtThreads;
 };
 
 struct WorkItem {
@@ -203,25 +134,37 @@ struct ItemIter {
 };
 
 // Epilogue variants are separate instantiations: folding SiluAndMul / the NVLink push into the plain kernel as run-time
-// branches grew its SASS from 3.9k to 10k instructions and cost EVERY dense GEMM 1.0-1.6 us (same-box A/B, r2 call 8).
+// branches grows the code of every dense GEMM.
 enum { EPI_PLAIN = 0, EPI_PAIRS = 1, EPI_PUSH = 2, EPI_ROWS = 3 };   // ROWS: Params::g_out_rows (grouped mode only)
 
+// one 128 B K slice of a stage: D[64 weight rows x BN tokens] (+)= W[64 x K] . X[BN x K]^T
+// (KIND_16 multiplies fp16 operands when `f16`, bf16 otherwise)
+template <int KIND, int BN, typename Acc>
+__device__ __forceinline__ void mma_k(Acc (&d)[BN / 2], uint64_t a, uint64_t b, int accumulate, bool f16) {
+  if constexpr (KIND == KIND_FP8) WgmmaN<BN>::e4m3(d, a, b, accumulate);
+  else if constexpr (KIND == KIND_I8) WgmmaN<BN>::s8(d, a, b, accumulate);
+  else if constexpr (KIND == KIND_SOFT) WgmmaN<BN>::template bf16<0>(d, a, b, accumulate);
+  else if (f16) WgmmaN<BN>::template f16<0>(d, a, b, accumulate);
+  else WgmmaN<BN>::template bf16<0>(d, a, b, accumulate);
+}
+
 template <int KIND, int BN, int EPI>
-__global__ void __launch_bounds__((Cfg<KIND, BN>::kThreads), (Cfg<KIND, BN>::kMinCtas))
+__global__ void __launch_bounds__((Cfg<KIND, BN>::kThreads), 1)
 tc_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_x, const Params p) {
   using C = Cfg<KIND, BN>;
+  using Acc = typename std::conditional<KIND == KIND_I8, int32_t, float>::type;
   constexpr bool kPairs = EPI == EPI_PAIRS;       // Params::act_pairs
   constexpr bool kPush = EPI == EPI_PUSH;         // Params::has_push
+  constexpr int NR = BN / 2;                      // accumulators per thread
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // dynamic smem base is only guaranteed 16 B aligned: round up to the 1024 B the swizzle needs
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_w = smem;
   uint8_t* smem_x = smem + C::kStages * C::kStageW;
   uint8_t* smem_c = smem_x + C::kStages * C::kStageX;          // soft fp8: converted weight tiles
-  __shared__ __align__(8) uint64_t full_bar[C::kStages], empty_bar[C::kStages], acc_full[C::kSlots], acc_empty[C::kSlots];
+  __shared__ __align__(8) uint64_t full_bar[C::kStages], empty_bar[C::kStages];
   __shared__ __align__(8) uint64_t cvt_full[C::kSoft ? C::kCvtStages : 1], cvt_empty[C::kSoft ? C::kCvtStages : 1];
-  __shared__ uint32_t s_tmem_base;
-  __shared__ int s_is_last[4];
+  __shared__ int s_is_last[2];
   __shared__ int4 s_geom[kGeomCache];             // grouped mode: {wrow, xrow, cnt, out col} of this CTA's first tiles
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -242,9 +185,9 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
   const int g_begin = min((int)blockIdx.x * per, total);
   const int g_end = min(g_begin + per, total);
   constexpr int kElemsPerStage = KIND == KIND_16 ? 64 : 128;   // K elements per pipeline stage
-  // grouped mode: the tile geometry lives in device memory; reading it per tile put an L2 round trip in
-  // front of every tile of the producer and of the epilogue (ncu r1: 122 us for the K = 256 down
-  // projection whose tiles are only two stages long).  Stage this CTA's share once.
+  // grouped mode: the tile geometry lives in device memory; reading it per tile puts an L2 round trip in front of every
+  // tile of the producer and of the epilogue (the K = 256 down projection's tiles are only two stages long).  Stage this
+  // CTA's share once.
   const int geom_t0 = g_begin / S;
   if (grouped && g_end > g_begin) {
     const int nt = min((g_end - 1) / S - geom_t0 + 1, kGeomCache);
@@ -259,27 +202,22 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
   };
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < C::kStages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-    for (int i = 0; i < C::kSlots; ++i) { mbar_init(&acc_full[i], 1); mbar_init(&acc_empty[i], 4); }
+    for (int i = 0; i < C::kStages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 2); }
     if (C::kSoft)
-      for (int i = 0; i < C::kCvtStages; ++i) { mbar_init(&cvt_full[i], 1); mbar_init(&cvt_empty[i], 1); }
+      for (int i = 0; i < C::kCvtStages; ++i) { mbar_init(&cvt_full[i], 1); mbar_init(&cvt_empty[i], 2); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 0 && lane == 0) {
+  if (warp == C::kProducerWarp && lane == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_x) : "memory");
   }
-  if (warp == 1) tmem_alloc(&s_tmem_base, C::kTmemCols);
   pdl_launch_dependents();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = s_tmem_base;
-  // everything above (barrier init, tensormap prefetch, TMEM allocation) overlapped the previous kernel's tail.
-  // The WEIGHTS are never written by a preceding kernel, so the producer also starts streaming them now — up to the
-  // whole ring (10 x 16 KB per SM, 23 MB over the GPU: more than the small decode linears hold) is in flight or landed
-  // before the activations exist; everything else waits here for the previous kernel to complete and flush.
-  if (warp == 0) {
+  // everything above (barrier init, tensormap prefetch) overlapped the previous kernel's tail.  The WEIGHTS are never
+  // written by a preceding kernel, so the producer also starts streaming them now — up to the whole ring (10 x 16 KB per
+  // SM) is in flight or landed before the activations exist; everything else waits here for the previous kernel to
+  // complete and flush.
+  if (warp == C::kProducerWarp) {
     // ================= TMA producer =================
     if (elect_one()) {
       const uint64_t pol_w = l2_policy_evict_first(), pol_x = l2_policy_evict_last();
@@ -320,58 +258,12 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
         }
       }
     }
-  } else if (warp == 1) {
-    // ================= MMA issuer =================
-    pdl_wait();
-    if (elect_one()) {
-      int it = 0, item_idx = 0;
-      int grp_of[4] = {0, 0, 0, 0};     // accumulator groups (fp8: stages, else: work items) handed to each epilogue set
-      for (ItemIter ii(g_begin, g_end, S); ii.valid(); ii.next(), ++item_idx) {
-        const WorkItem w = ii.item();
-        const int set = item_idx % C::kEpiSets;
-        int grp = grp_of[set];
-        for (int st = w.s_lo; st < w.s_hi; ++st, ++it) {
-          const int s = it % C::kStages;
-          const uint32_t ph = (it / C::kStages) & 1;
-          const bool group_first = KIND == KIND_FP8 ? true : (st == w.s_lo);
-          const bool group_last = KIND == KIND_FP8 ? true : (st == w.s_hi - 1);
-          const int slot = set * C::kSetSlots + grp % C::kSetSlots;
-          if (group_first) mbar_wait(&acc_empty[slot], ((grp / C::kSetSlots) & 1) ^ 1);
-          mbar_wait(&full_bar[s], ph);
-          const uint32_t d = tmem_base + slot * BN;
-          if constexpr (C::kSoft) {
-            // A = the bf16 tile the converter warps produced from this stage's fp8 weights (two 64-element atoms)
-            const int c = it % C::kCvtStages;
-            mbar_wait(&cvt_full[c], (it / C::kCvtStages) & 1);
-            tc_fence_after();
-            const uint64_t adesc = make_kmajor_sw128_desc(smem_u32(smem_c + c * C::kCvtBytes));
-            const uint64_t bdesc = make_kmajor_sw128_desc(smem_u32(smem_x + s * C::kStageX));
-#pragma unroll
-            for (int k = 0; k < 8; ++k)
-              umma<KIND>(d, adesc + (k >> 2) * ((kTileN * kStageRowBytes) >> 4) + 2 * (k & 3),
-                         bdesc + (k >> 2) * ((BN * kStageRowBytes) >> 4) + 2 * (k & 3), p.idesc,
-                         (group_first && k == 0) ? 0u : 1u);
-            umma_commit(&cvt_empty[c]);
-          } else {
-            tc_fence_after();
-            const uint64_t adesc = make_kmajor_sw128_desc(smem_u32(smem_w + s * C::kStageW));
-            const uint64_t bdesc = make_kmajor_sw128_desc(smem_u32(smem_x + s * C::kStageX));
-#pragma unroll
-            for (int k = 0; k < 4; ++k)     // 4 x 32 B of K per 128 B stage row; +2 in the (addr>>4) field per step
-              umma<KIND>(d, adesc + 2 * k, bdesc + 2 * k, p.idesc, (group_first && k == 0) ? 0u : 1u);
-          }
-          umma_commit(&empty_bar[s]);
-          if (group_last) { umma_commit(&acc_full[slot]); ++grp; }
-        }
-        grp_of[set] = grp;
-      }
-    }
   } else if (C::kSoft && warp >= C::kCvtWarp0) {
-    // ================= soft fp8: weight converter (8 warps) =================
+    // ================= soft fp8: weight converter (3 warps) =================
     // soft_fp8_gemm_deepseek_v3 (triton_kernels.py:388-508): w_bf16 = bf16(fp8 bits as fp32 * (s * 2^120)) == the value
     // bf16(fp32(fp8) * s) for every finite fp8 weight; the stage's [128 rows x 128 B] fp8 tile (one 128x128 scale block)
-    // becomes two 128B-swizzled bf16 atoms [128 rows x 64 elements].  A thread converts four 16-byte units.
-    const int ct = threadIdx.x - C::kCvtWarp0 * 32;            // 0..255
+    // becomes two 128B-swizzled bf16 atoms [128 rows x 64 elements], 1024 units of 16 fp8 weights.
+    const int ct = threadIdx.x - C::kCvtWarp0 * 32;            // 0..95
     int it = 0;
     for (ItemIter ii(g_begin, g_end, S); ii.valid(); ii.next()) {
       const WorkItem w = ii.item();
@@ -379,16 +271,15 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
       const float* srow = p.b_s + (int64_t)(w_row0 / kTileN) * p.kblocks;
       float sc_next = srow[w.s_lo];
       for (int st = w.s_lo; st < w.s_hi; ++st, ++it) {
-        const int s = it % C::kStages, c = it % C::kCvtStages;
+        const int s = it % C::kStages, c = it % C::kCvtRing;
         const float sc = sc_next;
         if (st + 1 < w.s_hi) sc_next = srow[st + 1];
         mbar_wait(&full_bar[s], (it / C::kStages) & 1);
-        mbar_wait(&cvt_empty[c], ((it / C::kCvtStages) & 1) ^ 1);
+        mbar_wait(&cvt_empty[c], ((it / C::kCvtRing) & 1) ^ 1);
         const uint8_t* src = smem_w + s * C::kStageW;
         uint8_t* dst = smem_c + c * C::kCvtBytes;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const int unit = j * 256 + ct;                          // 1024 units: row = unit / 8, 16 elements each
+#pragma unroll 2
+        for (int unit = ct; unit < 1024; unit += C::kCvtThreads) {   // row = unit / 8, 16 elements each
           const int r = unit >> 3, u = unit & 7;
           const uint4 v = *reinterpret_cast<const uint4*>(src + r * 128 + ((u ^ (r & 7)) << 4));
           const uint32_t vw[4] = {v.x, v.y, v.z, v.w};
@@ -406,22 +297,23 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
           *reinterpret_cast<uint4*>(drow + (((du + 1) ^ (r & 7)) << 4)) = make_uint4(o[4], o[5], o[6], o[7]);
         }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        asm volatile("bar.sync 5, 256;" ::: "memory");
+        asm volatile("bar.sync 5, %0;" ::"n"(C::kCvtThreads) : "memory");
         if (ct == 0) mbar_arrive(&cvt_full[c]);
       }
     }
-  } else {
-    // ================= epilogue: thread <-> output feature (TMEM lane) =================
+  } else if (warp < C::kProducerWarp) {
+    // ================= MMA + epilogue: consumer warpgroup `wg` owns weight rows [64 wg, 64 wg + 64) of every tile ==========
     pdl_wait();
     tl_stamp();
-    const int q = warp & 3;                       // TMEM lane quarter this warp may access
-    const int set = (warp - 2) >> 2;              // epilogue warp set: takes work items set, set + kEpiSets, ...
-    const int row = q * 32 + lane;
-    const uint32_t tbase = tmem_base + ((uint32_t)(q * 32) << 16);
-    int grp = 0;
+    const int wg = warp >> 2;
+    const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);     // tile rows r0 and r0 + 8 (wgmma fragment rows)
+    const int cl = 2 * (lane & 3);                               // token columns 8 nb + cl + {0, 1}
+    const bool signal = (threadIdx.x & 127) == 0;                // arrives on the ring barriers for its warpgroup
+    const bool f16 = KIND == KIND_16 && p.out_dtype == CB_F16;
+    auto row_of = [&](int e) { return r0 + 8 * ((e >> 1) & 1); };
+    auto col_of = [&](int e) { return 8 * (e >> 2) + cl + (e & 1); };
 
-    // final conversion of one element: m = activation / output row, n = output column, ld = row stride;
-    // sn = row index of the per-channel vectors (i8 b_scales / bias)
+    // final conversion of one element: m = activation / output row, n = output column, ld = row stride
     const uint32_t push_calls = kPush ? *p.push.calls : 0u;       // reduces completed so far: slot and epoch of this one
     const int64_t push_off = kPush ? push_area(p.push, push_calls) : 0;
     auto finish = [&](int m, int n, int ld, float v_f, int v_i) {
@@ -470,10 +362,9 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
       }
       return ge;
     };
-    // fp8 block scales of one accumulator group (= one 128-wide K block).  They are fetched ONE GROUP
-    // AHEAD, before waiting for the group's MMAs: loaded after the wait they were an exposed L2 round
-    // trip per K block (~0.5 us each, the whole fp8 GEMM ran at the speed of this chain).  The BN
-    // activation scales are spread over the lanes (token j -> lane j % 32) and broadcast by shuffle.
+    // fp8 block scales of one 128-wide K block, fetched ONE BLOCK AHEAD of the MMA that needs them (loaded after the
+    // wait they are an exposed L2 round trip per K block).  The BN activation scales are spread over the lanes
+    // (token j -> lane j % 32) and broadcast by shuffle.
     constexpr int AV = (BN + 31) / 32;
     auto fetch_scales = [&](const Geo& ge, int kb, float& bsc, float (&av)[AV]) {
       bsc = p.b_s[(int64_t)(ge.w_row0 / kTileN) * p.kblocks + kb];
@@ -485,136 +376,127 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
       }
     };
 
-    ItemIter it_e(g_begin, g_end, S);
-    int item_idx = 0;
-    // advance it_e to the next work item of this set (grp counts this set's own accumulator groups)
-    auto seek = [&]() -> bool {
-      while (it_e.valid()) {
-        if (item_idx % C::kEpiSets == set) return true;
-        it_e.next();
-        ++item_idx;
-      }
-      return false;
-    };
-    bool have = seek();
-    WorkItem w = {0, 0, 0};
-    Geo ge = {0, 0, 0, 0, 0, 0};
+    int it = 0;                                   // pipeline stage counter (same sequence as the producer's)
+    ItemIter ii(g_begin, g_end, S);
     float bsc_n = 0.f, av_n[AV];
 #pragma unroll
     for (int i = 0; i < AV; ++i) av_n[i] = 0.f;
-    if (have) {
-      w = it_e.item();
-      ge = geo_of(w);
-      if (KIND == KIND_FP8) fetch_scales(ge, w.s_lo, bsc_n, av_n);
+    Geo ge = {0, 0, 0, 0, 0, 0};
+    if (ii.valid()) {
+      ge = geo_of(ii.item());
+      if (KIND == KIND_FP8) fetch_scales(ge, ii.item().s_lo, bsc_n, av_n);
     }
-    while (have) {
-      it_e.next();
-      ++item_idx;
-      const bool have_next = seek();
-      WorkItem wn = w;
-      Geo gn = ge;
-      if (have_next) { wn = it_e.item(); gn = geo_of(wn); }
+    while (ii.valid()) {
+      const WorkItem w = ii.item();
+      ii.next();
+      const bool have_next = ii.valid();
+      const Geo gn = have_next ? geo_of(ii.item()) : ge;
       const int m0 = ge.m0, cnt = ge.cnt, ld = ge.ld;
-      const int n = ge.ocol0 + row;                      // output column of this thread
-      const bool n_ok = grouped ? (row < kTileN) : (n < p.N);
-      const bool narrow = cnt <= 4;
-      float acc[BN];
+
+      Acc d[NR];
+      float acc[NR];
 #pragma unroll
-      for (int j = 0; j < BN; ++j) acc[j] = 0.f;
-      const int ngroups = KIND == KIND_FP8 ? (w.s_hi - w.s_lo) : 1;
-      for (int gi = 0; gi < ngroups; ++gi, ++grp) {
-        const int slot = set * C::kSetSlots + grp % C::kSetSlots;
+      for (int e = 0; e < NR; ++e) { d[e] = 0; acc[e] = 0.f; }
+      for (int st = w.s_lo; st < w.s_hi; ++st, ++it) {
+        const int s = it % C::kStages;
         const float bsc = bsc_n;
         float av[AV];
 #pragma unroll
         for (int i = 0; i < AV; ++i) av[i] = av_n[i];
         if (KIND == KIND_FP8) {
-          if (gi + 1 < ngroups) fetch_scales(ge, w.s_lo + gi + 1, bsc_n, av_n);
-          else if (have_next) fetch_scales(gn, wn.s_lo, bsc_n, av_n);
+          if (st + 1 < w.s_hi) fetch_scales(ge, st + 1, bsc_n, av_n);
+          else if (have_next) fetch_scales(gn, ii.item().s_lo, bsc_n, av_n);
         }
-        mbar_wait(&acc_full[slot], (grp / C::kSetSlots) & 1);
-        tc_fence_after();
-        if (narrow) {
-          // <= 4 valid tokens in the tile (MoE experts at decode batch sizes, bs <= 4 linears): drain 4 columns
-          uint32_t r[4];
-          tmem_ld4(tbase + slot * BN, r);
-          tmem_ld_wait();
+        mbar_wait(&full_bar[s], (it / C::kStages) & 1);
+        const int first = KIND == KIND_FP8 || st == w.s_lo;     // fp8: a fresh accumulator per K block
+        wgmma_fence();
+        if constexpr (C::kSoft) {
+          // A = the bf16 tile the converter warps produced from this stage's fp8 weights (two 64-element atoms)
+          const int c = it % C::kCvtRing;
+          mbar_wait(&cvt_full[c], (it / C::kCvtRing) & 1);
+          const uint32_t a0 = smem_u32(smem_c + c * C::kCvtBytes) + wg * 64 * kStageRowBytes;
+          const uint32_t b0 = smem_u32(smem_x + s * C::kStageX);
 #pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            if (KIND == KIND_FP8) {
-              const float as = __shfl_sync(0xffffffffu, av[0], j);
-              acc[j] = fmaf(__uint_as_float(r[j]) * as, bsc, acc[j]);
-            } else {
-              acc[j] = __uint_as_float(r[j]);
-            }
-          }
-        } else
+          for (int k = 0; k < 8; ++k)
+            mma_k<KIND, BN>(d, make_kmajor_sw128_desc(a0 + (k >> 2) * (kTileN * kStageRowBytes) + 32 * (k & 3)),
+                            make_kmajor_sw128_desc(b0 + (k >> 2) * (BN * kStageRowBytes) + 32 * (k & 3)),
+                            (first && k == 0) ? 0 : 1, f16);
+          wgmma_commit();
+          wgmma_wait<0>();
+          if (signal) mbar_arrive(&cvt_empty[c]);
+        } else {
+          const uint32_t a0 = smem_u32(smem_w + s * C::kStageW) + wg * 64 * kStageRowBytes;
+          const uint32_t b0 = smem_u32(smem_x + s * C::kStageX);
 #pragma unroll
-        for (int c = 0; c < BN; c += 16) {
-          uint32_t r[16];
-          tmem_ld16(tbase + slot * BN + c, r);
-          tmem_ld_wait();
+          for (int k = 0; k < 4; ++k)     // 4 x 32 B of K per 128 B stage row
+            mma_k<KIND, BN>(d, make_kmajor_sw128_desc(a0 + 32 * k), make_kmajor_sw128_desc(b0 + 32 * k),
+                            (first && k == 0) ? 0 : 1, f16);
+          wgmma_commit();
+          wgmma_wait<0>();
+        }
+        if (signal) mbar_arrive(&empty_bar[s]);
+        if constexpr (KIND == KIND_FP8) {
 #pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            if (KIND == KIND_FP8) {
-              // (dot * a_s) * b_s as the reference does (triton_kernels.py:357)
-              const float as = __shfl_sync(0xffffffffu, av[(c + j) / 32], (c + j) & 31);
-              acc[c + j] = fmaf(__uint_as_float(r[j]) * as, bsc, acc[c + j]);
-            } else {
-              acc[c + j] = __uint_as_float(r[j]);      // i8: raw int32 bits kept in the float register
-            }
+          for (int e = 0; e < NR; ++e) {
+            // (dot * a_s) * b_s as the reference does (triton_kernels.py:357)
+            const int col = col_of(e);
+            const float as = __shfl_sync(0xffffffffu, av[(e >> 2) >> 2], col & 31);
+            acc[e] = fmaf(d[e] * as, bsc, acc[e]);
           }
         }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&acc_empty[slot]);
+      }
+      float vals[NR];                             // i8: raw int32 bits kept in the float register
+#pragma unroll
+      for (int e = 0; e < NR; ++e) {
+        if constexpr (KIND == KIND_FP8) vals[e] = acc[e];
+        else if constexpr (KIND == KIND_I8) vals[e] = __int_as_float(d[e]);
+        else vals[e] = d[e];
       }
 
       const bool whole = (w.s_lo == 0 && w.s_hi == S);
+      auto n_ok = [&](int e) { return grouped ? true : (ge.ocol0 + row_of(e) < p.N); };
       // SiluAndMul fused into the epilogue (fused_moe.py:24-39; FeedForward gate_up -> silu * mul): with the gate / up rows
-      // of the merged weight interleaved at load time, adjacent TMEM lanes hold g and u of the same output element.  Same
-      // roundings as the two separate launches: g, u -> bf16 (the GEMM's output), silu(g) -> bf16, product -> bf16.
-      auto emit_pairs = [&](const float (&vals)[BN], int ncols) {
+      // of the merged weight interleaved at load time, rows 2i and 2i+1 of the tile (lanes l and l ^ 4) hold g and u of the
+      // same output element.  Same roundings as the two separate launches: g, u -> bf16 (the GEMM's output), silu(g) ->
+      // bf16, product -> bf16.
+      auto emit_pairs = [&](const float (&v)[NR]) {
 #pragma unroll
-        for (int j = 0; j < BN; ++j) {
-          if (j >= ncols) break;                                      // warp-uniform
-          const float other = __shfl_xor_sync(0xffffffffu, vals[j], 1);
-          if (n_ok && (lane & 1) == 0 && j < cnt) {
-            const float g = __bfloat162float(__float2bfloat16_rn(vals[j])), u = __bfloat162float(__float2bfloat16_rn(other));
+        for (int e = 0; e < NR; ++e) {
+          const float other = __shfl_xor_sync(0xffffffffu, v[e], 4);
+          const int n = ge.ocol0 + row_of(e), j = col_of(e);
+          if (n_ok(e) && ((lane >> 2) & 1) == 0 && j < cnt) {
+            const float g = __bfloat162float(__float2bfloat16_rn(v[e])), u = __bfloat162float(__float2bfloat16_rn(other));
             const float sl = __bfloat162float(__float2bfloat16_rn(g / (1.f + expf(-g))));
             reinterpret_cast<__nv_bfloat16*>(p.out)[(int64_t)(m0 + j) * (ld >> 1) + (n >> 1)] = __float2bfloat16_rn(sl * u);
           }
         }
       };
-      // tensor-parallel partial (EPI_PUSH): bf16 pairs (adjacent output features = adjacent TMEM lanes) straight into
+      // tensor-parallel partial (EPI_PUSH): bf16 pairs (adjacent output features = lanes l and l ^ 4) straight into
       // every rank's push area over NVLink, each 8-byte word tagged with the reduce's epoch (comm.cu)
-      auto emit_push = [&](const float (&vals)[BN], int ncols) {
+      auto emit_push = [&](const float (&v)[NR]) {
 #pragma unroll
-        for (int j = 0; j < BN; ++j) {
-          if (j >= ncols) break;                                      // warp-uniform
-          const float other = __shfl_xor_sync(0xffffffffu, vals[j], 1);
-          if (n_ok && (lane & 1) == 0 && j < cnt) {
+        for (int e = 0; e < NR; ++e) {
+          const float other = __shfl_xor_sync(0xffffffffu, v[e], 4);
+          const int n = ge.ocol0 + row_of(e), j = col_of(e);
+          if (n_ok(e) && ((lane >> 2) & 1) == 0 && j < cnt) {
             const __nv_bfloat16* tag = nullptr;
-            push_word(p.push, push_off + ((((int64_t)(m0 + j) * ld + n) >> 1) << 3), pack2(vals[j], other, tag), push_calls + 1u);
+            push_word(p.push, push_off + ((((int64_t)(m0 + j) * ld + n) >> 1) << 3), pack2(v[e], other, tag), push_calls + 1u);
           }
         }
       };
-      if (whole) {
+      auto emit = [&](const float (&v)[NR]) {
         if constexpr (kPairs) {
-          emit_pairs(acc, narrow ? 4 : BN);
+          emit_pairs(v);
         } else if constexpr (kPush) {
-          emit_push(acc, narrow ? 4 : BN);
-        } else if (n_ok) {
-          if (narrow) {
+          emit_push(v);
+        } else {
 #pragma unroll
-            for (int j = 0; j < 4; ++j)
-              if (j < cnt) finish(m0 + j, n, ld, acc[j], __float_as_int(acc[j]));
-          } else {
-#pragma unroll
-            for (int j = 0; j < BN; ++j)
-              if (j < cnt) finish(m0 + j, n, ld, acc[j], __float_as_int(acc[j]));
-          }
+          for (int e = 0; e < NR; ++e)
+            if (n_ok(e) && col_of(e) < cnt) finish(m0 + col_of(e), ge.ocol0 + row_of(e), ld, v[e], __float_as_int(v[e]));
         }
+      };
+      if (whole) {
+        emit(vals);
       } else {
         // contributors of this tile: CTAs whose ranges intersect [tile*S, (tile+1)*S); CTA c keeps the
         // partial of its FIRST work item in slot 0 and of any later (necessarily last) item in slot 1
@@ -624,68 +506,53 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
         const int my_slot = ((int)blockIdx.x * per) / S == w.tile ? 0 : 1;
         float* mine = p.partial + ((int64_t)blockIdx.x * 2 + my_slot) * (BN * kTileN);
 #pragma unroll
-        for (int j = 0; j < BN; ++j) mine[j * kTileN + row] = acc[j];
+        for (int e = 0; e < NR; ++e) mine[col_of(e) * kTileN + row_of(e)] = vals[e];
         __threadfence();
-        // named barrier of this epilogue set (ids 1..4), 128 threads
-        asm volatile("bar.sync %0, 128;" ::"r"(1 + set) : "memory");
-        if (threadIdx.x == kBaseThreads + 128 * set) {
-          const int prev = atomicAdd(&p.tickets[w.tile], 1);
-          s_is_last[set] = (prev == count - 1);
-          if (prev == count - 1) p.tickets[w.tile] = 0;   // self-reset for the next launch / graph replay
+        // named barrier of this warpgroup (ids 1..2), 128 threads; each half of the tile has its own ticket
+        asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+        if (signal) {
+          const int prev = atomicAdd(&p.tickets[w.tile * 2 + wg], 1);
+          s_is_last[wg] = (prev == count - 1);
+          if (prev == count - 1) p.tickets[w.tile * 2 + wg] = 0;   // self-reset for the next launch / graph replay
         }
-        asm volatile("bar.sync %0, 128;" ::"r"(1 + set) : "memory");
-        const bool last = s_is_last[set] != 0;
-        asm volatile("bar.sync %0, 128;" ::"r"(1 + set) : "memory");   // s_is_last may be rewritten by the next item
-        if (last && (n_ok || kPairs || kPush)) {    // pairs / push: every lane takes part in the shuffles
+        asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+        const bool last = s_is_last[wg] != 0;
+        asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");   // s_is_last may be rewritten by the next item
+        if (last) {
           __threadfence();
-          // all BN loads of one contributor are independent -> issued back to back (the serial
-          // version of this loop cost ~20 us per GEMM: every load is an L2 round trip)
-          float tot[BN];
+          // all loads of one contributor are independent -> issued back to back (a serial loop is one L2 round trip
+          // per load)
+          float tot[NR];
 #pragma unroll
-          for (int j = 0; j < BN; ++j) tot[j] = 0.f;
-          // CB contributors per round trip (<= 128 independent loads in flight per thread), summed in
-          // contributor order -> deterministic
+          for (int e = 0; e < NR; ++e) tot[e] = 0.f;
+          // CB contributors per round trip, summed in contributor order -> deterministic
           constexpr int CB = BN <= 16 ? 8 : (BN <= 32 ? 4 : (BN <= 64 ? 2 : 1));
           for (int c0 = c_first; c0 <= c_last; c0 += CB) {
-            float v[CB][BN];
+            float v[CB][NR];
 #pragma unroll
             for (int cc = 0; cc < CB; ++cc) {
               const int c = min(c0 + cc, c_last);
               const int slot = (c * per) / S == w.tile ? 0 : 1;
-              const float* base = p.partial + ((int64_t)c * 2 + slot) * (BN * kTileN) + row;
+              const float* base = p.partial + ((int64_t)c * 2 + slot) * (BN * kTileN);
 #pragma unroll
-              for (int j = 0; j < BN; ++j) v[cc][j] = __ldcg(&base[j * kTileN]);
+              for (int e = 0; e < NR; ++e) v[cc][e] = __ldcg(&base[col_of(e) * kTileN + row_of(e)]);
             }
 #pragma unroll
             for (int cc = 0; cc < CB; ++cc) {
               if (c0 + cc > c_last) break;
 #pragma unroll
-              for (int j = 0; j < BN; ++j) {
-                if (KIND == KIND_I8) tot[j] = __int_as_float(__float_as_int(tot[j]) + __float_as_int(v[cc][j]));
-                else tot[j] += v[cc][j];
+              for (int e = 0; e < NR; ++e) {
+                if (KIND == KIND_I8) tot[e] = __int_as_float(__float_as_int(tot[e]) + __float_as_int(v[cc][e]));
+                else tot[e] += v[cc][e];
               }
             }
           }
-          if constexpr (kPairs) {
-            emit_pairs(tot, BN);
-          } else if constexpr (kPush) {
-            emit_push(tot, BN);
-          } else {
-#pragma unroll
-            for (int j = 0; j < BN; ++j)
-              if (j < cnt) finish(m0 + j, n, ld, tot[j], __float_as_int(tot[j]));
-          }
+          emit(tot);
         }
       }
-      w = wn;
       ge = gn;
-      have = have_next;
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, C::kTmemCols);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -735,7 +602,7 @@ int make_map(CUtensorMap* map, const void* base, int rows, int K, int elem_bytes
 
 int pick_bn(int M) { return M <= 16 ? 16 : M <= 32 ? 32 : M <= 64 ? 64 : 128; }
 
-constexpr int kMaxTickets = 65536;
+constexpr int kMaxTickets = 65536;          // tiles; two tickets (one per 64-row half) each
 int g_num_sms = 0;
 
 int num_sms() {
@@ -744,25 +611,26 @@ int num_sms() {
     if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0)
       g_num_sms = n;
     else
-      g_num_sms = 148;
+      g_num_sms = 132;
   }
   return g_num_sms;
 }
 
 // tickets + two partial slots of [BN][128] fp32 per CTA
-int64_t ws_bytes_for(int grid, int BN) { return (int64_t)kMaxTickets * 4 + (int64_t)grid * 2 * BN * kTileN * 4; }
+constexpr int64_t kTicketBytes = (int64_t)kMaxTickets * 2 * 4;
+int64_t ws_bytes_for(int grid, int BN) { return kTicketBytes + (int64_t)grid * 2 * BN * kTileN * 4; }
 
 template <int KIND, int BN, int EPI>
 int launch_epi(const CUtensorMap& mw, const CUtensorMap& mx, Params& p, int grid, cudaStream_t st) {
   using C = Cfg<KIND, BN>;
   size_t smem = 1024 + (size_t)C::kStages * C::kStageBytes + (size_t)C::kCvtStages * C::kCvtBytes;
-  // opt-in dynamic shared memory: static (barriers) + dynamic must stay within 227 KB
+  // opt-in dynamic shared memory: static (barriers, tile geometry) + dynamic must stay within 227 KB
   static size_t attr_bytes = 0;
   if (smem > attr_bytes) {
     CB_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<KIND, BN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr_bytes = smem;
   }
-  cb::launch_k(tc_gemm_kernel<KIND, BN, EPI>, dim3(grid), dim3(Cfg<KIND, BN>::kThreads), smem, st, mw, mx, p);
+  cb::launch_k(tc_gemm_kernel<KIND, BN, EPI>, dim3(grid), dim3(C::kThreads), smem, st, mw, mx, p);
   CB_LAUNCHED(1);
   return 0;
 }
@@ -825,7 +693,7 @@ int run(int kind, const void* x, const void* w, Params& p, int elem, CUtensorMap
     grid = (int)((total + p.per - 1) / p.per);
   }
   p.tickets = (int*)ws;
-  p.partial = ws ? (float*)((uint8_t*)ws + (int64_t)kMaxTickets * 4) : nullptr;
+  p.partial = ws ? (float*)((uint8_t*)ws + kTicketBytes) : nullptr;
   CUtensorMap mw, mx;
   int rc = make_map(&mw, w, p.N, p.K, elem, dt, kTileN);
   if (rc) return rc;
@@ -835,11 +703,6 @@ int run(int kind, const void* x, const void* w, Params& p, int elem, CUtensorMap
   if (kind == KIND_FP8) return dispatch_bn<KIND_FP8>(BN, mw, mx, p, grid, st);
   if (kind == KIND_SOFT) return dispatch_bn<KIND_SOFT>(BN, mw, mx, p, grid, st);
   return dispatch_bn<KIND_I8>(BN, mw, mx, p, grid, st);
-}
-
-uint32_t make_idesc(int c_fmt, int a_fmt, int b_fmt, int BN) {
-  return ((uint32_t)c_fmt << 4) | ((uint32_t)a_fmt << 7) | ((uint32_t)b_fmt << 10) | ((uint32_t)(BN >> 3) << 17) |
-         ((uint32_t)(kTileN >> 4) << 24);
 }
 
 }  // namespace
@@ -856,12 +719,12 @@ bool tc_supported(int kind, int M, int N, int K) {
 
 int64_t tc_workspace_bytes(int M, int N) {
   (void)N;
-  return ws_bytes_for(148, pick_bn(M));
+  return ws_bytes_for(num_sms(), pick_bn(M));
 }
 
 // Grouped (MoE experts) GEMM: sorted activations xs [rows, K], stacked weights w [E*Ng, K]; tile list in
 // device memory (see Params).  kind: KIND_16 (bf16 x bf16) or KIND_FP8 (block-scaled, a_s [rows, K/128],
-// b_s [E*Ng/128, K/128]).  max_tokens_per_expert bounds UMMA-N.  Output: sorted rows [rows, Ng] bf16.
+// b_s [E*Ng/128, K/128]).  max_tokens_per_expert bounds wgmma N.  Output: sorted rows [rows, Ng] bf16.
 int tc_grouped_gemm(int kind, const void* xs, const float* a_s, const void* w, const float* b_s, void* out, int rows,
                     int E, int Ng, int K, int max_tokens_per_expert, const int* g_num_tiles, const int* g_tile_wrow,
                     const int* g_tile_xrow, const int* g_tile_cnt, const float* row_scale, const int* out_rows, void* ws,
@@ -881,8 +744,7 @@ int tc_grouped_gemm(int kind, const void* xs, const float* a_s, const void* w, c
   const int grid = num_sms();
   if (!ws || ws_bytes < ws_bytes_for(grid, BN)) return fail(-2, "tc_grouped_gemm: workspace too small");
   p.tickets = (int*)ws;
-  p.partial = (float*)((uint8_t*)ws + (int64_t)kMaxTickets * 4);
-  p.idesc = kind == KIND_FP8 ? make_idesc(1, 0, 0, BN) : make_idesc(1, 1, 1, BN);
+  p.partial = (float*)((uint8_t*)ws + kTicketBytes);
   CUtensorMap mw, mx;
   const CUtensorMapDataType wdt = kind == KIND_16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_UINT8;
   const bool x16 = kind != KIND_FP8;                  // bf16 activations (bf16 and soft-fp8 kinds)
@@ -905,8 +767,6 @@ int tc_linear16(const void* x, const void* w, const void* bias, const void* resi
     if (rc) return rc;
     p.has_push = 1;
   }
-  const int fmt = dtype == CB_BF16 ? 1 : 0;
-  p.idesc = make_idesc(1, fmt, fmt, pick_bn(M));
   return run(KIND_16, x, w, p, 2, dtype == CB_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16,
              ws, ws_bytes, st);
 }
@@ -917,7 +777,6 @@ int tc_linear16_silu_pairs(const void* x, const void* w, void* y, int M, int N, 
   Params p{};
   p.M = M; p.N = N; p.K = K;
   p.out_dtype = CB_BF16; p.out = y; p.act_pairs = 1;
-  p.idesc = make_idesc(1, 1, 1, pick_bn(M));
   return run(KIND_16, x, w, p, 2, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, ws, ws_bytes, st);
 }
 
@@ -931,7 +790,6 @@ int tc_fp8_gemm(const void* a, const float* a_s, const void* b, const float* b_s
     if (rc) return rc;
     p.has_push = 1;
   }
-  p.idesc = make_idesc(1, 0, 0, pick_bn(M));
   return run(KIND_FP8, a, b, p, 1, CU_TENSOR_MAP_DATA_TYPE_UINT8, ws, ws_bytes, st);
 }
 
@@ -941,7 +799,6 @@ int tc_soft_fp8_gemm(const void* a, const void* b, const float* b_s, void* c, in
   Params p{};
   p.M = M; p.N = N; p.K = K;
   p.out_dtype = CB_BF16; p.b_s = b_s; p.out = c;
-  p.idesc = make_idesc(1, 1, 1, pick_bn(M));
   return run(KIND_SOFT, a, b, p, 1, CU_TENSOR_MAP_DATA_TYPE_UINT8, ws, ws_bytes, st, 2, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
 }
 
@@ -950,7 +807,6 @@ int tc_w8a8_gemm(void* out, const int8_t* a, const int8_t* b, const float* a_sca
   Params p{};
   p.M = M; p.N = N; p.K = K;
   p.out_dtype = CB_F16; p.a_s = a_scales; p.b_s = b_scales; p.bias = bias; p.out = out;
-  p.idesc = make_idesc(2, 1, 1, pick_bn(M));
   return run(KIND_I8, a, b, p, 1, CU_TENSOR_MAP_DATA_TYPE_UINT8, ws, ws_bytes, st);
 }
 

@@ -4,7 +4,7 @@
 // the 32 lanes stride K with 128-bit `ld.global.nc.L1::no_allocate` loads (each weight byte is
 // read exactly once from HBM), activations are re-read through L1 (they are tiny), fp32
 // accumulation, butterfly reduce.  This path is the small-M / any-shape implementation; the
-// tcgen05 + TMA swap-AB kernel in gemm_tc.cu is the tensor-core implementation of the same
+// wgmma + TMA swap-AB kernel in gemm_tc.cu is the tensor-core implementation of the same
 // entry points (impl = 2) and the default for M > 2.
 #include "common.cuh"
 

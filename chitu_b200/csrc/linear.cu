@@ -1,5 +1,5 @@
 // C-ABI entry points of the decode linears; dispatch between the SIMT weight-streaming path
-// (gemv.cu) and the tcgen05 + TMA swap-AB path (gemm_tc.cu).
+// (gemv.cu) and the wgmma + TMA swap-AB path (gemm_tc.cu).
 #include "common.cuh"
 
 namespace cb {
@@ -32,9 +32,8 @@ using namespace cb;
 
 enum { KIND_16 = 0, KIND_FP8 = 1, KIND_I8 = 2, KIND_SOFT = 3 };
 
-// auto policy: the persistent stream-K tcgen05 kernel wins at every decode batch size on B200
-// (measured: bs=1 LLaMA-3-8B step 3.82 ms vs 4.03 ms with the SIMT GEMV, bs=16 needs tensor cores
-// outright: 16 tokens x 2 flop per weight byte exceeds the FMA pipes); the SIMT path remains for
+// auto policy: the persistent stream-K wgmma kernel (bs=16 needs tensor cores outright: 16 tokens x 2 flop per weight
+// byte exceeds the FMA pipes); the SIMT path remains for
 // shapes TMA cannot address (row pitch not a multiple of 16 B, fp8 K % 128 != 0) and as impl=1.
 static bool use_tc(int impl, int kind, int M, int N, int K, void* ws, int64_t ws_bytes) {
   if (impl == 1) return false;
@@ -54,19 +53,19 @@ extern "C" int chitu_b200_linear_bf16(const void* x, const void* w, const void* 
   cudaStream_t st = (cudaStream_t)stream;
   if (use_tc(impl, KIND_16, M, N, K, workspace, workspace_bytes))
     return tc_linear16(x, w, bias, residual, y, M, N, K, dtype, workspace, workspace_bytes, st);
-  if (impl == 2) return fail(-2, "linear_bf16: tcgen05 path unavailable for M=%d N=%d K=%d (or workspace too small)", M, N, K);
+  if (impl == 2) return fail(-2, "linear_bf16: wgmma path unavailable for M=%d N=%d K=%d (or workspace too small)", M, N, K);
   return simt_linear16(x, w, bias, residual, y, M, N, K, dtype, st);
 }
 
 // FeedForward's gate_up linear + SiluAndMul (models/model_llama.py:139-149, fused_moe.py:24-39) in one launch:
 // w_pairs = the merged [w1 ; w3] weight with its rows interleaved (row 2i = gate_i, row 2i+1 = up_i) at load time;
-// y[M, N/2] = bf16(bf16(silu(bf16 g)) * bf16(u)) — the roundings of the two separate reference ops.  bf16, tcgen05 only.
+// y[M, N/2] = bf16(bf16(silu(bf16 g)) * bf16(u)) — the roundings of the two separate reference ops.  bf16, wgmma only.
 extern "C" int chitu_b200_linear_bf16_silu_pairs(const void* x, const void* w_pairs, void* y, int M, int N, int K,
                                                  void* workspace, int64_t workspace_bytes, void* stream) {
   CB_ARG(x && w_pairs && y && M >= 0 && N > 0 && N % 2 == 0 && K > 0);
   if (M == 0) return 0;
   if (!use_tc(2, KIND_16, M, N, K, workspace, workspace_bytes))
-    return fail(-2, "linear_bf16_silu_pairs: tcgen05 path unavailable for M=%d N=%d K=%d (or workspace too small)", M, N, K);
+    return fail(-2, "linear_bf16_silu_pairs: wgmma path unavailable for M=%d N=%d K=%d (or workspace too small)", M, N, K);
   return tc_linear16_silu_pairs(x, w_pairs, y, M, N, K, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
@@ -78,7 +77,7 @@ extern "C" int chitu_b200_fp8_gemm(const void* a, const float* a_s, const void* 
   cudaStream_t st = (cudaStream_t)stream;
   if (use_tc(impl, KIND_FP8, M, N, K, workspace, workspace_bytes))
     return tc_fp8_gemm(a, a_s, b, b_s, c, M, N, K, residual, workspace, workspace_bytes, st);
-  if (impl == 2) return fail(-2, "fp8_gemm: tcgen05 path unavailable for M=%d N=%d K=%d (or workspace too small)", M, N, K);
+  if (impl == 2) return fail(-2, "fp8_gemm: wgmma path unavailable for M=%d N=%d K=%d (or workspace too small)", M, N, K);
   int rc = simt_fp8_gemm(a, a_s, b, b_s, c, M, N, K, st);
   if (rc || !residual) return rc;
   return chitu_b200_add(c, residual, c, (int64_t)M * N, CB_BF16, stream);
@@ -93,7 +92,7 @@ extern "C" int chitu_b200_fp8_gemm_ar(const void* a, const float* a_s, const voi
   CB_ARG(a && a_s && b && b_s && comm && M > 0 && N > 0 && N % 2 == 0 && K > 0);
   CB_ARG((int64_t)M * N * 2 <= comm_slot_bytes(comm));
   if (!use_tc(2, KIND_FP8, M, N, K, workspace, workspace_bytes))
-    return fail(-2, "fp8_gemm_ar: tcgen05 path unavailable for M=%d N=%d K=%d (or workspace too small)", M, N, K);
+    return fail(-2, "fp8_gemm_ar: wgmma path unavailable for M=%d N=%d K=%d (or workspace too small)", M, N, K);
   return tc_fp8_gemm(a, a_s, b, b_s, nullptr, M, N, K, nullptr, workspace, workspace_bytes, (cudaStream_t)stream, comm);
 }
 
@@ -102,7 +101,7 @@ extern "C" int chitu_b200_linear_bf16_ar(const void* x, const void* w, int M, in
   CB_ARG(x && w && comm && M > 0 && N > 0 && N % 2 == 0 && K > 0);
   CB_ARG((int64_t)M * N * 2 <= comm_slot_bytes(comm));
   if (!use_tc(2, KIND_16, M, N, K, workspace, workspace_bytes))
-    return fail(-2, "linear_bf16_ar: tcgen05 path unavailable for M=%d N=%d K=%d (or workspace too small)", M, N, K);
+    return fail(-2, "linear_bf16_ar: wgmma path unavailable for M=%d N=%d K=%d (or workspace too small)", M, N, K);
   return tc_linear16(x, w, nullptr, nullptr, nullptr, M, N, K, CB_BF16, workspace, workspace_bytes, (cudaStream_t)stream, comm);
 }
 
@@ -111,10 +110,10 @@ extern "C" int chitu_b200_soft_fp8_gemm(const void* a, const void* b, const floa
                                         int64_t workspace_bytes, int impl, void* stream) {
   CB_ARG(a && b && b_s && c && M >= 0 && N > 0 && K > 0);
   if (M == 0) return 0;
-  // tcgen05 path: the fp8 weight tile is converted to bf16 in shared memory between the TMA landing and the bf16 MMA
+  // wgmma path: the fp8 weight tile is converted to bf16 in shared memory between the TMA landing and the bf16 MMA
   if (out_dtype == CB_BF16 && use_tc(impl, KIND_SOFT, M, N, K, workspace, workspace_bytes))
     return tc_soft_fp8_gemm(a, b, b_s, c, M, N, K, workspace, workspace_bytes, (cudaStream_t)stream);
-  if (impl == 2) return fail(-2, "soft_fp8_gemm: tcgen05 path unavailable for M=%d N=%d K=%d (bf16 only, K %% 128 == 0)", M, N, K);
+  if (impl == 2) return fail(-2, "soft_fp8_gemm: wgmma path unavailable for M=%d N=%d K=%d (bf16 only, K %% 128 == 0)", M, N, K);
   return simt_soft_fp8_gemm(a, b, b_s, c, M, N, K, out_dtype, (cudaStream_t)stream);
 }
 
@@ -126,7 +125,7 @@ extern "C" int chitu_b200_w8a8_gemm(void* out, const int8_t* a, const int8_t* b,
   cudaStream_t st = (cudaStream_t)stream;
   if (use_tc(impl, KIND_I8, M, N, K, workspace, workspace_bytes))
     return tc_w8a8_gemm(out, a, b, a_scales, b_scales, bias, M, N, K, workspace, workspace_bytes, st);
-  if (impl == 2) return fail(-2, "w8a8_gemm: tcgen05 path unavailable for M=%d N=%d K=%d (or workspace too small)", M, N, K);
+  if (impl == 2) return fail(-2, "w8a8_gemm: wgmma path unavailable for M=%d N=%d K=%d (or workspace too small)", M, N, K);
   return simt_w8a8_gemm(out, a, b, a_scales, b_scales, bias, M, N, K, st);
 }
 

@@ -1,31 +1,29 @@
-// Absorbed-MLA paged decode on the 5th-generation tensor cores (sm_100a): tcgen05.mma + TMEM + TMA.
+// Absorbed-MLA paged decode on the Hopper tensor cores (sm_90a): wgmma + TMA + mbarrier.
 //
-// Replaces third_party/FlashMLA (sm_90a only, flash_api.cpp:73-75) and triton_decode_attention.py:20-290 behind
+// Replaces third_party/FlashMLA (flash_api.cpp:73-75) and triton_decode_attention.py:20-290 behind
 // AttnBackend.mla_attn_with_kvcache (attn_backend.py:536-572 / 707-774).  Same arithmetic as the reference:
 // scores = (q_nope.k_c + q_pe.k_pe) * scale in fp32, softmax in fp32, P rounded to bf16 before P.V
 // (triton_decode_attention.py:113), V = the first 512 columns of the SAME cache row, split-KV partials merged by LSE.
 //
-// Mapping (one CTA per (KV split, 16-head group, request), 1 CTA / SM, 6 warps):
-//   both products are SWAPPED so that the 16 local heads (tp = 8) are the UMMA N dimension:
-//     S^T[64 keys x 16 heads]  = K[64 x 576] . Q^T       A = staged K chunk, K-major (UMMA M = 128: rows 64..127 read the
-//                                                         next ring slot and land in TMEM lanes nobody reads)
+// Mapping (one CTA per (KV split, 16-head group, request), 1 CTA / SM, 5 warps):
+//   both products are SWAPPED so that the 16 local heads (tp = 8) are the wgmma N dimension:
+//     S^T[64 keys x 16 heads]  = K[64 x 576] . Q^T       A = staged K chunk, K-major (wgmma M = 64 = one page)
 //     O^T[512 dims x 16 heads] += V^T[512 x 64] . P^T     A = the SAME staged chunks read MN-major (dims contiguous),
-//                                                         4 M tiles of 128 dims, B = P[16 heads x 64 keys] K-major
-//   so a cache row is read from HBM exactly once and the tensor pipe does 32 + 4 + 16 tiny MMAs per 64-key page.
-//   warp 0   TMA producer: one page = 9 boxes [64 keys x 128 B] (128B swizzle); the 8 latent chunks go through a ring of
+//                                                         8 M tiles of 64 dims, B = P[16 heads x 64 keys] K-major
+//   so a cache row is read from HBM exactly once and the tensor pipe does 36 + 32 tiny MMAs per 64-key page.
+//   warp 4   TMA producer: one page = 9 boxes [64 keys x 128 B] (128B swizzle); the 8 latent chunks go through a ring of
 //            22 x 8 KB slots (2.75 pages in flight), the rope chunk through its own 3-slot ring (it is released right
 //            after Q.K^T).  KV streaming starts BEFORE griddepcontrol.wait: cache rows are only written by earlier decode
 //            steps and by this kernel, so the stream overlaps the tail of the previous kernel (PDL).
-//   warp 1   MMA issuer (one elected lane): Q.K^T of page i+1 is issued before P.V of page i (two S^T buffers in TMEM), so
-//            the softmax of page i+1 overlaps P.V of page i.
-//   warps 2-5 softmax / epilogue, thread = TMEM lane: a key of S^T (lanes 0..63), a latent dim of an O^T tile (all 128).
-//            Per-head running max through a 16-shuffle butterfly; the O^T rescale (TMEM round trip) only happens when a
-//            head's max moved by more than 2^8 (the exact result is recovered at the end: P, l and O share the same
-//            reference max); row sums are kept per thread and reduced once in the epilogue.
+//   warps 0-3 one warpgroup: Q.K^T (S^T in registers: 2 keys x 4 heads per thread), softmax, P -> shared memory, P.V
+//            (O^T in registers: 8 tiles x 2 dims x 4 heads per thread).  Per-head running max across the 64 keys by
+//            shuffles + one shared-memory exchange between the 4 warps; O^T is only rescaled when a head's max moved
+//            by more than 2^8 (the exact result is recovered at the end: P, l and O share the same reference max).
 #include <cuda.h>
 
 #include "common.cuh"
 #include "tc_ptx.cuh"
+#include "wgmma.cuh"
 
 namespace cb {
 namespace {
@@ -33,66 +31,20 @@ namespace {
 constexpr int kC = 512, kR = 64, kRow = kC + kR;
 constexpr int kTile = 64;                      // keys per tile == page size
 constexpr int kSlot = kTile * 128;             // 8 KB: one TMA box [64 keys x 128 B]
-constexpr int kNSM = 22;                       // main ring slots (even: chunk pairs (2m, 2m+1) stay adjacent)
+constexpr int kNSM = 22;                       // main ring slots
 constexpr int kNSR = 3;                        // rope ring slots
 constexpr int kQBytes = 9 * 16 * 128;          // Q as 9 K-major chunks of [16 heads x 128 B]
 constexpr int kPBytes = 16 * 128;              // P as [16 heads x 64 keys] bf16, K-major
 constexpr int kSmemBytes = kNSM * kSlot + kNSR * kSlot + kQBytes + 2 * kPBytes;
 constexpr float kLog2e = 1.4426950408889634f;
 constexpr float kRescaleThreshold = 8.f;       // log2 domain
+constexpr int kThreads = 160;                  // warpgroup (warps 0-3) + producer warp
 
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t acc) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-               ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(acc) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-        "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
-// shared-memory matrix descriptor, 128B swizzle: start>>4 | LBO>>4 <<16 | SBO>>4 <<32 | version 1 <<46 | SWIZZLE_128B <<61
-//   K-major  operand (rows of 128 B):         LBO unused (16), SBO = 1024 (8-row groups)
-//   MN-major operand (64-element MN chunks):  LBO = stride between 64-element MN chunks, SBO = 1024 (8 k-rows),
-//                                             one UMMA K step (16 k-rows) = 2048 B   (verified on B200: scripts/exp_umma_mn.py)
-__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
 // byte offset of the 16-byte unit `unit` of row `row` in a [rows x 128 B] 128B-swizzled tile
 __device__ __forceinline__ uint32_t sw128(int row, int unit) { return (uint32_t)(row * 128 + ((unit ^ (row & 7)) << 4)); }
 
-// Reduce 16 per-thread values across the 32 lanes of a warp with 16 shuffles (instead of 80): every exchange step halves
-// the number of values a lane keeps.  Returns the reduction of value index `butterfly_index(lane)` over all 32 lanes.
 // dev tool (profiling build only, -DCB_TIMELINE): %globaltimer at fixed points of every CTA, 32 slots per CTA, read by
 // scripts/mla_probe.py.  The product library compiles these to nothing.
 #ifdef CB_TIMELINE
@@ -109,35 +61,26 @@ __device__ __forceinline__ void probe(int idx) {
 __device__ __forceinline__ void probe(int) {}
 #endif
 
-__device__ __forceinline__ int butterfly_index(int lane) { return ((lane >> 4) & 1) * 8 + ((lane >> 3) & 1) * 4 + ((lane >> 2) & 1) * 2 + ((lane >> 1) & 1); }
-template <bool MAX>
-__device__ __forceinline__ float butterfly16(const float (&v)[16], int lane) {
-  auto op = [](float a, float b) { return MAX ? fmaxf(a, b) : a + b; };
-  float w8[8], w4[4], w2[2], w1;
-  const bool b16 = lane & 16, b8 = lane & 8, b4 = lane & 4, b2 = lane & 2;
+// max / sum over the 8 lanes that share lane % 4 (the key rows of one wgmma fragment column)
+__device__ __forceinline__ float rows_max(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 4));
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 8));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 16));
+}
+__device__ __forceinline__ float rows_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 4);
+  v += __shfl_xor_sync(0xffffffffu, v, 8);
+  return v + __shfl_xor_sync(0xffffffffu, v, 16);
+}
+// value h of a 16-entry register array without dynamic register indexing
+__device__ __forceinline__ float pick16(const float (&v)[16], int h) {
+  float r = v[0];
 #pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const float send = b16 ? v[i] : v[i + 8], keep = b16 ? v[i + 8] : v[i];
-    w8[i] = op(keep, __shfl_xor_sync(0xffffffffu, send, 16));
-  }
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const float send = b8 ? w8[i] : w8[i + 4], keep = b8 ? w8[i + 4] : w8[i];
-    w4[i] = op(keep, __shfl_xor_sync(0xffffffffu, send, 8));
-  }
-#pragma unroll
-  for (int i = 0; i < 2; ++i) {
-    const float send = b4 ? w4[i] : w4[i + 2], keep = b4 ? w4[i + 2] : w4[i];
-    w2[i] = op(keep, __shfl_xor_sync(0xffffffffu, send, 4));
-  }
-  {
-    const float send = b2 ? w2[0] : w2[1], keep = b2 ? w2[1] : w2[0];
-    w1 = op(keep, __shfl_xor_sync(0xffffffffu, send, 2));
-  }
-  return op(w1, __shfl_xor_sync(0xffffffffu, w1, 1));
+  for (int i = 1; i < 16; ++i) r = (h == i) ? v[i] : r;
+  return r;
 }
 
-__global__ void __launch_bounds__(192, 1) mla_decode_tc_kernel(
+__global__ void __launch_bounds__(kThreads, 1) mla_decode_tc_kernel(
     const __grid_constant__ CUtensorMap map_kv, const __nv_bfloat16* __restrict__ q_nope,
     const __nv_bfloat16* __restrict__ q_pe, __nv_bfloat16* __restrict__ kv_cache,
     const __nv_bfloat16* __restrict__ new_kv, const int32_t* __restrict__ seqlens_excl,
@@ -150,10 +93,8 @@ __global__ void __launch_bounds__(192, 1) mla_decode_tc_kernel(
   uint8_t* s_rope = s_ring + kNSM * kSlot;                  // [kNSR][64 keys][128 B]   rope chunk
   uint8_t* s_q = s_rope + kNSR * kSlot;                     // [9][16 heads][128 B]
   uint8_t* s_p = s_q + kQBytes;                             // [2][16 heads][128 B]
-  __shared__ __align__(8) uint64_t full_m[kNSM], empty_m[kNSM], full_r[kNSR], empty_r[kNSR], s_full[2], p_ready[2], o_done,
-      raw_bar, q_ready;
-  __shared__ float red_max[2][2][16], red_sum[2][16];
-  __shared__ uint32_t s_tmem;
+  __shared__ __align__(8) uint64_t full_m[kNSM], empty_m[kNSM], full_r[kNSR], empty_r[kNSR], raw_bar;
+  __shared__ float red_max[4][16], red_sum[4][16];
 
   const int split = blockIdx.x, hg = blockIdx.y, b = blockIdx.z;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -163,21 +104,12 @@ __global__ void __launch_bounds__(192, 1) mla_decode_tc_kernel(
     probe(0);
     for (int i = 0; i < kNSM; ++i) { mbar_init(&full_m[i], 1); mbar_init(&empty_m[i], 1); }
     for (int i = 0; i < kNSR; ++i) { mbar_init(&full_r[i], 1); mbar_init(&empty_r[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&s_full[i], 1); mbar_init(&p_ready[i], 1); }
-    mbar_init(&o_done, 1);
     mbar_init(&raw_bar, 1);
-    mbar_init(&q_ready, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_kv) : "memory");
   }
-  if (warp == 1) tmem_alloc(&s_tmem, 128);
   cb::pdl_launch_dependents();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = s_tmem;
-  const uint32_t tm_s = tmem;                                // S^T : 2 buffers x 16 columns
-  const uint32_t tm_o = tmem + 32;                           // O^T : 4 M tiles x 16 columns
 
   // sequence lengths and the block table are written only by kernels that do not trigger dependents early (torch copies,
   // the decode-prepare kernel): they are stable here even before griddepcontrol.wait
@@ -195,7 +127,7 @@ __global__ void __launch_bounds__(192, 1) mla_decode_tc_kernel(
   const int ntiles = end > begin ? (end - begin + kTile - 1) / kTile : 0;
   const int32_t* bt = block_table + (int64_t)b * bt_stride;
 
-  if (warp == 0) {
+  if (warp == 4) {
     // ================= TMA producer (whole warp: lane 0 issues, all lanes patch the tail page) =================
     const uint64_t pol = l2_policy_evict_first();
     uint32_t raw_phase = 0;
@@ -256,71 +188,18 @@ __global__ void __launch_bounds__(192, 1) mla_decode_tc_kernel(
         }
       }
     }
-  } else if (warp == 1) {
-    // ================= MMA issuer =================
-    if (elect_one()) {
-      // c_fmt f32 | a, b bf16 | N = 16 | M = 128 ; P.V adds a_major = MN (bit 15)
-      const uint32_t idesc_qk = (1u << 4) | (1u << 7) | (1u << 10) | ((16u >> 3) << 17) | ((128u >> 4) << 24);
-      const uint32_t idesc_pv = idesc_qk | (1u << 15);
-      const uint32_t ring_a = smem_u32(s_ring), rope_a = smem_u32(s_rope), q_a = smem_u32(s_q), p_a = smem_u32(s_p);
-      mbar_wait(&q_ready, 0);
-      tc_fence_after();
-      probe(31);
-      auto issue_qk = [&](int it) {
-        const uint32_t d = tm_s + (it & 1) * 16;
-        for (int c = 0; c < 8; ++c) {
-          const int g = it * 8 + c, s = g % kNSM;
-          mbar_wait(&full_m[s], (g / kNSM) & 1);
-          tc_fence_after();
-          const uint64_t a = make_desc(ring_a + s * kSlot, 16, 1024);
-          const uint64_t bq = make_desc(q_a + c * 2048, 16, 1024);
-#pragma unroll
-          for (int k = 0; k < 4; ++k) umma_f16(d, a + 2 * k, bq + 2 * k, idesc_qk, (c == 0 && k == 0) ? 0u : 1u);
-        }
-        const int rs = it % kNSR;
-        mbar_wait(&full_r[rs], (it / kNSR) & 1);
-        tc_fence_after();
-        const uint64_t a = make_desc(rope_a + rs * kSlot, 16, 1024);
-        const uint64_t bq = make_desc(q_a + 8 * 2048, 16, 1024);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) umma_f16(d, a + 2 * k, bq + 2 * k, idesc_qk, 1u);
-        umma_commit(&empty_r[rs]);                           // the rope chunk is not needed by P.V
-        umma_commit(&s_full[it & 1]);
-      };
-      if (ntiles > 0) issue_qk(0);
-      for (int it = 0; it < ntiles; ++it) {
-        if (it + 1 < ntiles) issue_qk(it + 1);
-        mbar_wait(&p_ready[it & 1], (it >> 1) & 1);
-        tc_fence_after();
-        const uint64_t bp = make_desc(p_a + (it & 1) * kPBytes, 16, 1024);
-#pragma unroll
-        for (int m = 0; m < 4; ++m) {
-          const int g = it * 8 + 2 * m, s = g % kNSM;        // even position, even ring size: slot s + 1 is adjacent
-#pragma unroll
-          for (int ks = 0; ks < 4; ++ks) {
-            const uint64_t a = make_desc(ring_a + s * kSlot + ks * 2048, kSlot, 1024);
-            umma_f16(tm_o + 16 * m, a, bp + 2 * ks, idesc_pv, (it == 0 && ks == 0) ? 0u : 1u);
-          }
-          umma_commit(&empty_m[s]);
-          umma_commit(&empty_m[s + 1]);
-        }
-        umma_commit(&o_done);
-      }
-    }
   } else {
-    // ================= softmax / epilogue: thread <-> TMEM lane =================
-    const int q = warp & 3;                                  // TMEM lane quarter this warp may access
-    const int row = q * 32 + lane;                           // key row of S^T (q < 2) / dim row of an O^T M tile
-    const bool key_warp = q < 2;
-    const uint32_t lane_base = (uint32_t)(q * 32) << 16;
-    const int t = threadIdx.x - 64;                          // 0..127
+    // ================= warpgroup: Q.K^T, softmax, P.V, epilogue =================
+    const int t = threadIdx.x;                               // 0..127
+    const int krow = warp * 16 + (lane >> 2);                // fragment rows krow, krow + 8: keys of S^T, dims of O^T tiles
+    const int hc = 2 * (lane & 3);                           // fragment columns hc + 8 nb + j: heads
     // ---- Q -> shared memory (K-major, swizzled); rows >= H are zero ----
     cb::pdl_wait();
     cb::tl_stamp();
     if (t == 0) probe(1);
     {
       // 16 heads x 72 units of 16 B = 9 units per thread: all nine global loads are issued before the first shared-memory
-      // store (ncu r2: the load -> store -> load chain of the plain loop was 11 % of the kernel's stall samples)
+      // store
       uint4 v[9];
 #pragma unroll
       for (int j = 0; j < 9; ++j) {
@@ -342,7 +221,7 @@ __global__ void __launch_bounds__(192, 1) mla_decode_tc_kernel(
     }
     fence_async_smem();
     asm volatile("bar.sync 1, 128;" ::: "memory");
-    if (t == 0) { mbar_arrive(&q_ready); probe(2); }
+    if (t == 0) probe(2);
     if (new_kv && split == 0 && hg == 0) {                   // append for the following steps (ops.py:50-91)
       const int page = bt[L_cache / kTile];
       __nv_bfloat16* dst = kv_cache + ((int64_t)page * kTile + L_cache % kTile) * kRow;
@@ -350,35 +229,66 @@ __global__ void __launch_bounds__(192, 1) mla_decode_tc_kernel(
       for (int i = t; i < kRow / 8; i += 128) reinterpret_cast<uint4*>(dst)[i] = reinterpret_cast<const uint4*>(src)[i];
     }
 
+    const uint32_t ring_a = smem_u32(s_ring), rope_a = smem_u32(s_rope), q_a = smem_u32(s_q), p_a = smem_u32(s_p);
     const float sc = scale * kLog2e;
-    const int hsel = butterfly_index(lane);
-    float m_run[16], l_part[16];
+    float m_run[16];                                         // identical in every thread
+    float l_part[4];                                         // this thread's keys, heads hc + 8 (e >> 1) + (e & 1)
+    float o[8][8];                                           // O^T tile m: dims 64 m + krow (+8), heads as S^T
 #pragma unroll
-    for (int h = 0; h < 16; ++h) { m_run[h] = -INFINITY; l_part[h] = 0.f; }
+    for (int h = 0; h < 16; ++h) m_run[h] = -INFINITY;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) l_part[i] = 0.f;
+#pragma unroll
+    for (int m = 0; m < 8; ++m)
+#pragma unroll
+      for (int e = 0; e < 8; ++e) o[m][e] = 0.f;
 
     for (int it = 0; it < ntiles; ++it) {
-      const int buf = it & 1;
-      float s[16];
-      mbar_wait(&s_full[buf], (it >> 1) & 1);
-      tc_fence_after();
-      if (t == 0 && it < 12) probe(3 + 2 * it);
-      if (key_warp) {
-        const bool valid = begin + it * kTile + row < end;
-        uint32_t r[16];
-        tmem_ld16(tm_s + buf * 16 + lane_base, r);
-        tmem_ld_wait();
+      // ---- S^T = K . Q^T over the 8 latent chunks and the rope chunk ----
+      float s[8];
 #pragma unroll
-        for (int h = 0; h < 16; ++h) s[h] = valid ? __uint_as_float(r[h]) * sc : -INFINITY;
-        const float mx = butterfly16<true>(s, lane);
-        if ((lane & 1) == 0) red_max[buf][q][hsel] = mx;
+      for (int e = 0; e < 8; ++e) s[e] = 0.f;
+      wgmma_fence();
+      for (int c = 0; c < 8; ++c) {
+        const int g = it * 8 + c, sl = g % kNSM;
+        mbar_wait(&full_m[sl], (g / kNSM) & 1);
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+          WgmmaN<16>::bf16<0>(s, make_sw128_desc(ring_a + sl * kSlot + 32 * k, 16, 1024),
+                              make_sw128_desc(q_a + c * 2048 + 32 * k, 16, 1024), (c | k) != 0);
+      }
+      const int rs = it % kNSR;
+      mbar_wait(&full_r[rs], (it / kNSR) & 1);
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        WgmmaN<16>::bf16<0>(s, make_sw128_desc(rope_a + rs * kSlot + 32 * k, 16, 1024),
+                            make_sw128_desc(q_a + 8 * 2048 + 32 * k, 16, 1024), 1);
+      wgmma_commit();
+      wgmma_wait<0>();
+      if (t == 0) {
+        mbar_arrive(&empty_r[rs]);                           // the rope chunk is not needed by P.V
+        if (it < 12) probe(3 + 2 * it);
+      }
+
+      // ---- per-head tile maximum over the 64 keys (finite: every tile has a valid key) ----
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        const bool valid = begin + it * kTile + krow + 8 * ((e >> 1) & 1) < end;
+        s[e] = valid ? s[e] * sc : -INFINITY;
+      }
+#pragma unroll
+      for (int x = 0; x < 4; ++x) {                          // x = 2 nb + j
+        const int e = 4 * (x >> 1) + (x & 1);
+        const float mx = rows_max(fmaxf(s[e], s[e + 2]));
+        if (lane < 4) red_max[warp][hc + 8 * (x >> 1) + (x & 1)] = mx;
       }
       asm volatile("bar.sync 1, 128;" ::: "memory");
-      // per-head tile maximum (finite: every tile has a valid key); rescale only when some head moved by > 2^8
+      // rescale only when some head moved by > 2^8
       float mt[16];
       bool need = false;
 #pragma unroll
       for (int h = 0; h < 16; ++h) {
-        mt[h] = fmaxf(red_max[buf][0][h], red_max[buf][1][h]);
+        mt[h] = fmaxf(fmaxf(red_max[0][h], red_max[1][h]), fmaxf(red_max[2][h], red_max[3][h]));
         need |= mt[h] > m_run[h] + kRescaleThreshold;
       }
       float alpha[16];
@@ -390,90 +300,82 @@ __global__ void __launch_bounds__(192, 1) mla_decode_tc_kernel(
           m_run[h] = mn;
         }
       }
-      if (key_warp) {
-        uint8_t* pb = s_p + buf * kPBytes;
+      // ---- P = exp2(S - m) -> bf16 -> shared memory as P[head][key] (K-major, swizzled) ----
+      uint8_t* pb = s_p + (it & 1) * kPBytes;
 #pragma unroll
-        for (int h = 0; h < 16; ++h) {
-          const float p = exp2f(s[h] - m_run[h]);            // 0 for masked keys
-          l_part[h] = (need ? l_part[h] * alpha[h] : l_part[h]) + p;
-          // P^T -> shared memory as P[head][key] (K-major, swizzled): this thread owns key `row` (< 64)
-          *reinterpret_cast<__nv_bfloat16*>(pb + sw128(h, row >> 3) + (row & 7) * 2) = __float2bfloat16_rn(p);
-        }
+      for (int x = 0; x < 4; ++x) {
+        const int h = hc + 8 * (x >> 1) + (x & 1);
+        const float mr = pick16(m_run, h);
+        const int e = 4 * (x >> 1) + (x & 1);
+        const float p0 = exp2f(s[e] - mr), p1 = exp2f(s[e + 2] - mr);       // 0 for masked keys
+        l_part[x] = (need ? l_part[x] * pick16(alpha, h) : l_part[x]) + p0 + p1;
+        *reinterpret_cast<__nv_bfloat16*>(pb + sw128(h, krow >> 3) + (krow & 7) * 2) = __float2bfloat16_rn(p0);
+        *reinterpret_cast<__nv_bfloat16*>(pb + sw128(h, (krow + 8) >> 3) + (krow & 7) * 2) = __float2bfloat16_rn(p1);
       }
-      // The previous tile's P.V (issued right behind this tile's Q.K^T, i.e. finished long before this point) is
-      // observed on EVERY tile, not only when O^T must be rescaled: each phase of o_done then has a waiter
-      // (compute-sanitizer synccheck flagged the conditional version as "missing wait") and the cost is one try_wait.
-      if (it > 0) mbar_wait(&o_done, (it - 1) & 1);
       if (need && it > 0) {
-        // P.V accumulates into O^T: it must have finished before O^T is rescaled
-        tc_fence_after();
+        float al[4];
 #pragma unroll
-        for (int m = 0; m < 4; ++m) {
-          uint32_t o[16];
-          tmem_ld16(tm_o + 16 * m + lane_base, o);
-          tmem_ld_wait();
+        for (int x = 0; x < 4; ++x) al[x] = pick16(alpha, hc + 8 * (x >> 1) + (x & 1));
 #pragma unroll
-          for (int h = 0; h < 16; ++h) o[h] = __float_as_uint(__uint_as_float(o[h]) * alpha[h]);
-          tmem_st16(tm_o + 16 * m + lane_base, o);
-        }
-        tmem_st_wait();
+        for (int m = 0; m < 8; ++m)
+#pragma unroll
+          for (int e = 0; e < 8; ++e) o[m][e] *= al[2 * (e >> 2) + (e & 1)];
       }
       fence_async_smem();
-      tc_fence_before();
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      if (t == 0) {
-        mbar_arrive(&p_ready[buf]);
-        if (it < 12) probe(4 + 2 * it);
+      asm volatile("bar.sync 1, 128;" ::: "memory");          // P complete; red_max free for the next tile
+      if (t == 0 && it < 12) probe(4 + 2 * it);
+
+      // ---- O^T += V^T . P^T: the 8 latent chunks of the page, each a 64-dim M tile read MN-major ----
+      wgmma_fence();
+#pragma unroll
+      for (int m = 0; m < 8; ++m) {
+        const int sl = (it * 8 + m) % kNSM;
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks)                       // 16 keys = two 8-row groups of the chunk
+          WgmmaN<16>::bf16<1>(o[m], make_sw128_desc(ring_a + sl * kSlot + ks * 2048, kSlot, 1024),
+                              make_sw128_desc(p_a + (it & 1) * kPBytes + 32 * ks, 16, 1024), 1);
       }
+      wgmma_commit();
+      wgmma_wait<0>();
+      if (t == 0)
+        for (int m = 0; m < 8; ++m) mbar_arrive(&empty_m[(it * 8 + m) % kNSM]);
     }
 
-    // ---- epilogue: row sums across the 64 key lanes, O^T / l -> out (one split) or normalised partial + log2-sum-exp ----
-    if (key_warp) {
-      const float ls = butterfly16<false>(l_part, lane);
-      if ((lane & 1) == 0) red_sum[q][hsel] = ls;
-    }
-    if (ntiles > 0) {
-      mbar_wait(&o_done, (ntiles - 1) & 1);
-      tc_fence_after();
+    // ---- epilogue: row sums across the 64 keys, O^T / l -> out (one split) or normalised partial + log2-sum-exp ----
+#pragma unroll
+    for (int x = 0; x < 4; ++x) {
+      const float ls = rows_sum(l_part[x]);
+      if (lane < 4) red_sum[warp][hc + 8 * (x >> 1) + (x & 1)] = ls;
     }
     if (t == 0) probe(28);
     asm volatile("bar.sync 1, 128;" ::: "memory");
     const bool direct = num_splits == 1 && out != nullptr;   // out == NULL: partials even for one split (deferred merge)
-    float inv[16];
+    float inv[4];
 #pragma unroll
-    for (int h = 0; h < 16; ++h) {
-      const float l = red_sum[0][h] + red_sum[1][h];
-      inv[h] = (ntiles > 0 && l > 0.f) ? 1.f / l : 0.f;
+    for (int x = 0; x < 4; ++x) {
+      const int h = hc + 8 * (x >> 1) + (x & 1);
+      const float l = (red_sum[0][h] + red_sum[1][h]) + (red_sum[2][h] + red_sum[3][h]);
+      inv[x] = (ntiles > 0 && l > 0.f) ? 1.f / l : 0.f;
     }
 #pragma unroll
-    for (int m = 0; m < 4; ++m) {
-      uint32_t o[16];
-      if (ntiles > 0) {
-        tmem_ld16(tm_o + 16 * m + lane_base, o);
-        tmem_ld_wait();
-      }
-      const int dim = m * 128 + row;
+    for (int m = 0; m < 8; ++m) {
 #pragma unroll
-      for (int h = 0; h < 16; ++h) {
+      for (int e = 0; e < 8; ++e) {
+        const int x = 2 * (e >> 2) + (e & 1);
+        const int h = hc + 8 * (x >> 1) + (x & 1);
+        const int dim = m * 64 + krow + 8 * ((e >> 1) & 1);
         if (h0 + h >= H) continue;
-        const float v = ntiles > 0 ? __uint_as_float(o[h]) * inv[h] : 0.f;
+        const float v = o[m][e] * inv[x];
         if (direct) out[((int64_t)b * H + h0 + h) * kC + dim] = __float2bfloat16_rn(v);
         else o_part[(((int64_t)b * H + h0 + h) * num_splits + split) * kC + dim] = v;
       }
     }
     if (!direct && t < 16 && h0 + t < H) {
-      const float l = red_sum[0][t] + red_sum[1][t];
-      float mr = -INFINITY;                                  // m_run[t] without dynamic register indexing
-#pragma unroll
-      for (int h = 0; h < 16; ++h) mr = (h == t) ? m_run[h] : mr;
-      lse[((int64_t)b * H + h0 + t) * num_splits + split] = (ntiles > 0 && l > 0.f) ? mr + log2f(l) : -INFINITY;
+      const float l = (red_sum[0][t] + red_sum[1][t]) + (red_sum[2][t] + red_sum[3][t]);
+      lse[((int64_t)b * H + h0 + t) * num_splits + split] = (ntiles > 0 && l > 0.f) ? pick16(m_run, t) + log2f(l) : -INFINITY;
     }
     if (t == 0) probe(29);
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem, 128);
 }
 
 }  // namespace
@@ -496,7 +398,7 @@ int mla_decode_tc_launch(const void* q_nope, const void* q_pe, void* kv_cache, c
     attr = true;
   }
   dim3 grid(num_splits, cdiv(H, 16), B);
-  launch_k(mla_decode_tc_kernel, grid, dim3(192), smem, st, map, (const __nv_bfloat16*)q_nope,
+  launch_k(mla_decode_tc_kernel, grid, dim3(kThreads), smem, st, map, (const __nv_bfloat16*)q_nope,
            (const __nv_bfloat16*)q_pe, (__nv_bfloat16*)kv_cache, (const __nv_bfloat16*)new_kv, seqlens_excl, block_table,
            bt_stride, H, scale, num_splits, o_part, lse, (__nv_bfloat16*)out, plan);
   CB_LAUNCHED(1);

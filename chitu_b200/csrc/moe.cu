@@ -6,7 +6,7 @@
 //  * fused_experts  : fused_moe.py:1060-1307 (align -> quant -> GEMM1 -> SiluAndMul -> quant ->
 //                     GEMM2 x routed weight -> sum over top-k).  Decode batches give 1-2 tokens
 //                     per expert, so each (token, slot) pair streams its expert's weight rows once:
-//                     a batched weight-streaming GEMV (the grouped tcgen05 path lives in
+//                     a batched weight-streaming GEMV (the grouped wgmma path lives in
 //                     gemm_tc.cu and is selected for larger token counts per expert).
 #include <stdlib.h>
 #include <string.h>
@@ -171,7 +171,7 @@ __device__ __forceinline__ void moe_plan_large(const IdT* ids, const void* topk_
 
 // Decode-sized plans (P <= 1024 pairs): every phase is parallel over PAIRS or over TILE-LIST ENTRIES instead of one warp
 // per expert.  In-graph probes of the per-expert version at bs = 16 (144 pairs, ~100 active experts): 1.0 us staging, 1.9 us
-// scan, 4.6 - 7 us scatter + tile lists = 10 us after the dependency wait (profiles/r02_moe_plan_probe.log); the same
+// scan, 4.6 - 7 us scatter + tile lists = 10 us after the dependency wait; the same
 // stable order (pairs of an expert keep their pair-index order), so every output array is identical.
 template <typename IdT, int NT>
 __device__ __forceinline__ void moe_plan_small(const IdT* ids, const void* topk_w, int topk_w_f32,
@@ -333,8 +333,8 @@ __device__ __forceinline__ uint32_t ordered_key(float v) {
 
 // Gate logits for a decode batch (T <= 16): logits[t, e] = bf16(sum_k x[t,k] w[e,k]), fp32 accumulation.  One CTA per PAIR of
 // experts streams its two weight rows ONCE (prefetched before griddepcontrol.wait: weights are immutable) against all T
-// rows of x (L2-resident, 2 T dim bytes).  The tcgen05 GEMM it replaces here had only E / 128 = 2 weight tiles to share
-// among 148 CTAs: 74-way split-K and a fix-up of 74 partial tiles — 12 us per layer in the DeepSeek-R1 graph for 3.7 MB.
+// rows of x (L2-resident, 2 T dim bytes).  The tensor-core GEMM would have only E / 128 = 2 weight tiles to share among
+// all SMs: a 66-way split-K and a fix-up of 66 partial tiles for 3.7 MB of weights.
 constexpr int kGateVecIters = 4;      // 256 threads x 4 x 8 elements: dim <= 8192
 template <int TB>
 __global__ void __launch_bounds__(256) gate_logits_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ w,
@@ -422,7 +422,7 @@ __global__ void __launch_bounds__(256) moe_gate_kernel(
   const int t = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
 
   if (logits) {
-    // logits = F.linear(x, W) were produced by the tcgen05 GEMM (bf16, as the reference's are)
+    // logits = F.linear(x, W) were produced by the wgmma GEMM (bf16, as the reference's are)
     for (int e = tid; e < E; e += 256) s_orig[e] = __bfloat162float(logits[(int64_t)t * E + e]);
   } else {
     for (int i = tid; i < dim / 8; i += 256)
@@ -740,7 +740,7 @@ __global__ void moe_sum_kernel(const __nv_bfloat16* __restrict__ c3, __nv_bfloat
 
 // --------------------------------------------------------------------------------------------
 // Grouped-GEMM path of fused_experts (tokens sorted by expert, every distinct expert's weights are
-// streamed ONCE by the tcgen05 stream-K kernel of gemm_tc.cu):
+// streamed ONCE by the wgmma stream-K kernel of gemm_tc.cu):
 //   moe_plan_kernel        counting sort of the (token, slot) pairs by expert (stable, deterministic)
 //                          + the active (expert, n-tile) lists of both GEMMs
 //   moe_gather_quant_kernel  xs[r] = quant(x[pair_sorted[r] / topk])   (per_token_group_quant_fp8)
@@ -989,7 +989,7 @@ static int moe_gate_impl(const void* x, const void* w, const void* bias, int bia
   CB_ARG(bias == nullptr || bias_dtype == CB_F32 || bias_dtype == CB_BF16);
   if (T == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
-  // gate logits: one weight-streaming tcgen05 GEMM over all tokens (the old per-token in-kernel GEMV
+  // gate logits: one weight-streaming wgmma GEMM over all tokens (the old per-token in-kernel GEMV
   // re-read the 3.67 MB gate matrix once per token: 360 us per layer at bs=16)
   const __nv_bfloat16* logits = nullptr;
   if (workspace && workspace_bytes >= chitu_b200_moe_gate_workspace_bytes(T, E) && cb::tc_supported(0, T, E, dim)) {
@@ -1035,7 +1035,7 @@ static int moe_gate_impl(const void* x, const void* w, const void* bias, int bia
 // Blocks of `block_m` entries of sorted_token_ids (moe_align_block_size's output) share expert expert_ids[block];
 // entry r reads A[sorted_ids[r] / top_k] and writes C.view(-1, N)[sorted_ids[r]] (x topk_weights[sorted_ids[r]] when
 // mul_routed_weight); entries >= numel are padding.  Here: gather (+ per_token_group_quant_fp8 for fp8_w8a8) the A rows
-// into sorted order, build the (block, n-tile) list on the device, run the grouped tcgen05 GEMM with an output-row
+// into sorted order, build the (block, n-tile) list on the device, run the grouped wgmma GEMM with an output-row
 // indirection.
 __global__ void moe_blocks_prepare_kernel(const int32_t* __restrict__ sorted_ids, const int32_t* __restrict__ expert_ids,
                                           const int32_t* __restrict__ npp, int EM, int numel, int block_m, int E, int N,
@@ -1175,7 +1175,7 @@ extern "C" int64_t chitu_b200_moe_workspace_bytes(int T, int topk, int E, int N1
   b += align256(P * (N1 / 2));                       // a2_q
   b += align256(P * (N1 / 2 / 128 + 1) * 4);         // a2_s
   b += align256(P * K1 * 2);                         // c3
-  // grouped tcgen05 path (laid out separately; see fused_experts)
+  // grouped wgmma path (laid out separately; see fused_experts)
   int64_t g = align256(cb::tc_workspace_bytes(128, 128));                 // GEMM tickets + partials (zeroed once)
   g += align256((P + P + (E + 1) + 2 + P) * 4);                           // pair_sorted, pos, seg_start, counts, w_sorted
   const int64_t chunks = E + P / 16 + 1;                                  // row chunks of >= 16 sorted rows
@@ -1194,7 +1194,7 @@ static int fused_experts_impl(const void* x, const void* w1, const void* w2, con
                               int K1, int wmode, void* out, const void* residual, void* workspace,
                               int64_t workspace_bytes, void* stream, void* comm, int planned);
 
-// rows per chunk (= UMMA-N of the grouped GEMMs): twice the mean number of routed rows per expert, 16 .. 128
+// rows per chunk (= wgmma N of the grouped GEMMs): twice the mean number of routed rows per expert, 16 .. 128
 static int moe_chunk_rows(int64_t P, int E) {
   int BN = 16;
   while (BN < 128 && BN < 2 * (int)((P + E - 1) / E)) BN *= 2;
@@ -1288,7 +1288,7 @@ static int fused_experts_impl(const void* x, const void* w1, const void* w2, con
   const int N2 = N1 / 2;
   CB_ARG(P <= 65535);
 
-  // ---- grouped tcgen05 path: sort pairs by expert, stream every distinct expert once ----
+  // ---- grouped wgmma path: sort pairs by expert, stream every distinct expert once ----
   static const bool force_pair = getenv("CHITU_B200_MOE_PAIR") != nullptr;
   const int BN = moe_chunk_rows(P, E);
   const int64_t chunks = E + P / 16 + 1;
@@ -1360,7 +1360,7 @@ static int fused_experts_impl(const void* x, const void* w1, const void* w2, con
                              pl.tile2_xrow, pl.tile2_cnt, pl.w_sorted, nullptr, gws, cb::tc_workspace_bytes(128, 128), st);
     if (rc) return rc;
     int cblocks = cdiv((int64_t)T * K1 / 2, 256);
-    if (cblocks > 148 * 8) cblocks = 148 * 8;
+    if (cblocks > 132 * 8) cblocks = 132 * 8;
     PushDev push;
     memset(&push, 0, sizeof(push));
     if (comm) {
@@ -1372,7 +1372,7 @@ static int fused_experts_impl(const void* x, const void* w1, const void* w2, con
     CB_LAUNCHED(1);
     return 0;
   }
-  if (comm) return cb::fail(-2, "fused_experts_ar: only the grouped tcgen05 path pushes (T=%d topk=%d E=%d N1=%d K1=%d)", T, topk, E, N1, K1);
+  if (comm) return cb::fail(-2, "fused_experts_ar: only the grouped wgmma path pushes (T=%d topk=%d E=%d N1=%d K1=%d)", T, topk, E, N1, K1);
 
   // (the first bytes of the workspace hold the grouped path's ticket counters and must stay zero)
   uint8_t* p = (uint8_t*)workspace + align256(cb::tc_workspace_bytes(128, 128));
@@ -1413,7 +1413,7 @@ static int fused_experts_impl(const void* x, const void* w1, const void* w2, con
   }
   CB_LAUNCHED(1);
   int blocks = cdiv((int64_t)T * K1, 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   cb::launch_k(moe_sum_kernel, dim3(blocks), dim3(256), 0, st, c3, (__nv_bfloat16*)out, T, topk, K1);
   CB_LAUNCHED(1);
   if (residual) return chitu_b200_add(out, residual, out, (int64_t)T * K1, CB_BF16, stream);

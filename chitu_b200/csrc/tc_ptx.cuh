@@ -1,4 +1,4 @@
-// PTX wrappers shared by the TMA / mbarrier / tcgen05 kernels (sm_100a).
+// PTX wrappers shared by the TMA / mbarrier kernels (sm_90a).
 #pragma once
 #include <cuda.h>
 

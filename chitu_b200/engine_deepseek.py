@@ -207,15 +207,15 @@ class DeepSeekDecodeEngine:
                                                                      2 * self.F_moe, dim), dtype=torch.uint8, device=dev)
         self.gate_ws = torch.zeros(lib.chitu_b200_moe_gate_workspace_bytes(B, c.n_routed_experts), dtype=torch.uint8, device=dev)
         self.max_seq_len = max_seq_len
-        # the tcgen05 MLA kernel can leave its split-KV partials for the absorb-o kernel to merge (one launch fewer)
+        # the wgmma MLA kernel can leave its split-KV partials for the absorb-o kernel to merge (one launch fewer)
         import os
         self.defer_merge = (page_size == 64 and os.environ.get("CHITU_B200_MLA_IMPL", "0") == "0"
                             and os.environ.get("CHITU_B200_MLA_DEFER_MERGE", "1") != "0"
                             and c.v_head_dim == 128 and self.C == 512)
         self.ar_push = os.environ.get("CHITU_B200_AR_PUSH", "1") != "0"
-        # optional: the gate kernel's last CTA writes the expert plan (chitu_b200_moe_gate_plan, one launch fewer).  Measured
-        # on B200 (r2 call 8, 61-layer tp8 shard): 16.81 ms with it vs 16.44 ms without at bs16, 7.92 vs 7.78 ms at bs1 — the
-        # in-kernel hand-off (fence + ticket + a 256-thread plan) costs more than the PDL launch it saves, so it stays off.
+        # optional: the gate kernel's last CTA writes the expert plan (chitu_b200_moe_gate_plan, one launch fewer); off by
+        # default: the in-kernel hand-off (fence + ticket + a 256-thread plan) is serial work on the critical path where the
+        # separate plan kernel only costs a PDL launch.
         self.gate_plan = os.environ.get("CHITU_B200_GATE_PLAN", "0") == "1" and B * self.topk1 <= 8192
         self.graph = None
         self.launches_per_step = 0

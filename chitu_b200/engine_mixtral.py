@@ -280,7 +280,7 @@ def run_bench(args, time_engine, ClockSampler, peaks):
         eng.set_synthetic_context(S)
         eng.capture()
         sampler = ClockSampler(local) if rank == 0 else None
-        ms, e2e_ms, clocks = time_engine(eng, B, S, args, world, dev, sampler)
+        ms, e2e_ms, clocks = time_engine(eng, B, S, args, world, dev, sampler, label=f"mixtral_bs{B}")
         distinct = eng.distinct_experts_per_layer()
         nbytes = eng.algorithmic_bytes(S, distinct)
         out[B] = dict(ms=ms, e2e_ms=e2e_ms, distinct=distinct, bytes=nbytes, launches=int(eng.launches_per_step), clocks=clocks)
@@ -295,7 +295,7 @@ def run_bench(args, time_engine, ClockSampler, peaks):
             "value": B / (r["ms"] * 1e-3), "unit": "tokens/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
             "ms_per_step": r["ms"], "higher_is_better": True, "scaling": "strong", "vs_baseline": None, "dtype": "bf16",
             "data": "synthetic",
-            "config": {"workload": f"Mixtral-8x7B bf16, softmax top-2 router -> grouped tcgen05 expert GEMMs, bs={B} seq={S} page=256, "
+            "config": {"workload": f"Mixtral-8x7B bf16, softmax top-2 router -> grouped wgmma expert GEMMs, bs={B} seq={S} page=256, "
                                    f"{cfg.n_layers} layers, tp={tp}" + ("" if world > 1 else " (one rank's shard on 1 GPU, no collectives)"),
                        "global_batch": B, "seq_len": S, "parallelism": f"tp{tp}", "cuda_graph": True,
                        "distinct_experts_per_layer": r["distinct"],

@@ -1,6 +1,6 @@
 """Drop-in for the hot-path entry points of `chitu/fused_moe.py`: moe_align_block_size,
 per_token_group_quant_fp8, SiluAndMul, fused_experts (+ the DeepSeek gate as `moe_gate`).
-Reference: /root/reference/chitu/fused_moe.py (file:line cited per function).
+Reference: thu-pacman/chitu, chitu/fused_moe.py (file:line cited per function).
 """
 from __future__ import annotations
 
@@ -95,11 +95,11 @@ def invoke_fused_moe_kernel(A: torch.Tensor, B: torch.Tensor, C: torch.Tensor, A
                             compute_type=None, use_fp8_w8a8: bool = False, use_int8_w8a16: bool = False,
                             use_int4_w4a16: bool = False, block_shape: Optional[List[int]] = None,
                             soft_fp8: bool = False) -> None:
-    """fused_moe.py:796-891 — same signature, writes C in place.  One grouped tcgen05 GEMM over the blocks that
+    """fused_moe.py:796-891 — same signature, writes C in place.  One grouped wgmma GEMM over the blocks that
     `moe_align_block_size(topk_ids, config["BLOCK_SIZE_M"], E)` produced (BLOCK_SIZE_M in {16, 32, 64, 128}; the Triton
     tiling keys BLOCK_SIZE_N / K / GROUP_SIZE_M have no meaning here and are ignored)."""
     if use_int8_w8a16 or use_int4_w4a16 or B_zp is not None:
-        raise NotImplementedError("int8_w8a16 / int4_w4a16 expert weights are outside the B200 hot path")
+        raise NotImplementedError("int8_w8a16 / int4_w4a16 expert weights are outside the hot path of this library")
     assert topk_weights.stride(1) == 1
     assert sorted_token_ids.stride(0) == 1
     assert A.dtype == torch.bfloat16 and A.is_contiguous() and B.is_contiguous() and C.is_contiguous()
@@ -137,7 +137,7 @@ def fused_experts(hidden_states: torch.Tensor, w1: torch.Tensor, w2: torch.Tenso
     """fused_moe.py:1060-1307 — same signature.  Quantisation flags that are outside the
     north-star path are accepted and rejected with NotImplementedError (SURVEY §8b)."""
     if use_int8_w8a16 or use_int4_w4a16:
-        raise NotImplementedError("int8_w8a16 / int4_w4a16 expert weights are outside the B200 hot path")
+        raise NotImplementedError("int8_w8a16 / int4_w4a16 expert weights are outside the hot path of this library")
     if activation != "silu":
         raise ValueError(f"Unsupported FusedMoe activation: {activation}")
     if a1_scale is not None or a2_scale is not None or w1_zp is not None or w2_zp is not None:
@@ -147,7 +147,7 @@ def fused_experts(hidden_states: torch.Tensor, w1: torch.Tensor, w2: torch.Tenso
     assert hidden_states.is_contiguous(), "Hidden_states must be contiguous"
     assert w1.is_contiguous(), "Expert weights1 must be contiguous"
     assert w2.is_contiguous(), "Expert weights2 must be contiguous"
-    assert hidden_states.dtype == torch.bfloat16, "the B200 path computes in bf16"
+    assert hidden_states.dtype == torch.bfloat16, "this path computes in bf16"
     require_cuda(hidden_states, w1, w2, topk_weights, topk_ids)
     T, K1 = hidden_states.shape
     E, N1, _ = w1.shape
@@ -170,7 +170,7 @@ def fused_experts(hidden_states: torch.Tensor, w1: torch.Tensor, w2: torch.Tenso
         tw = tw.float()
     out = hidden_states if inplace else torch.empty_like(hidden_states)
     lib = _lib.load()
-    # (token, slot) pairs per launch: <= 8192 keeps every chunk on the grouped tcgen05 path (each distinct expert streamed
+    # (token, slot) pairs per launch: <= 8192 keeps every chunk on the grouped wgmma path (each distinct expert streamed
     # once per chunk); the C side accepts up to 65535 pairs (SIMT fallback above 8192)
     CHUNK = max(1, 8192 // max(topk, 1))
     for t0 in range(0, T, CHUNK):

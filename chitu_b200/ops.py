@@ -1,7 +1,7 @@
 """Drop-in for `chitu/ops.py`: same function names, argument meaning and error behaviour
-(asserts on non-contiguous inputs), bodies replaced by libchitu_b200 (sm_100a CUDA).
+(asserts on non-contiguous inputs), bodies replaced by libchitu_b200 (sm_90a CUDA).
 
-Reference: /root/reference/chitu/ops.py (file:line cited per function).
+Reference: thu-pacman/chitu, chitu/ops.py (file:line cited per function).
 """
 from __future__ import annotations
 
@@ -27,7 +27,7 @@ __all__ = [
     "sample_top_k_top_p",
 ]
 
-# impl selector for the linears: 0 auto, 1 SIMT, 2 tcgen05 (tests flip this)
+# impl selector for the linears: 0 auto, 1 SIMT, 2 wgmma (tests flip this)
 LINEAR_IMPL = 0
 
 
@@ -186,7 +186,7 @@ def soft_fp8_gemm_deepseek_v3(a: torch.Tensor, b: torch.Tensor, b_s: torch.Tenso
     M = a.numel() // K
     N = b.size(0)
     c = a.new_empty(*a.size()[:-1], N, dtype=a.dtype)
-    # tcgen05 path (bf16, K % 128 == 0): fp8 weight tiles are converted to bf16 in shared memory between TMA and MMA
+    # wgmma path (bf16, K % 128 == 0): fp8 weight tiles are converted to bf16 in shared memory between TMA and MMA
     ws, wsn = _linear_ws(M, N, a.device)
     check(_lib.load().chitu_b200_soft_fp8_gemm(ptr(a), ptr(b), ptr(b_s), ptr(c), M, N, K, dtype_code(a.dtype),
                                                ptr(ws), wsn, LINEAR_IMPL, current_stream()),

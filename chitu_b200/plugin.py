@@ -1,4 +1,4 @@
-"""`install()` patches the B200 operators into an importable reference `chitu` package so that
+"""`install()` patches this library's operators into an importable reference `chitu` package so that
 `chitu.executor` / `cache_manager` / the model files run unchanged (SURVEY.md §8b):
 
   * `sys.modules["chitu_backend"]`      <- chitu_b200.chitu_backend      (csrc/binding.cpp:11-19)

@@ -4,7 +4,7 @@
 What must match the reference so that its checkpoints and its quantizer walk (`quantize/quantizer.py:117-145`)
 work unchanged: the buffer names and dtypes (`weight` int8 [N, K], `scale_channel` fp32 [N], `bias` fp16 [N] or
 None), the constructor / `from_float` parameters, and the dispatch rule of `forward` ([bs <= 4, seq, K] inputs go
-to `w8a8gemv.mv`, everything else to `w8a8gemm.mm`).  The arithmetic runs in the B200 kernels behind those two
+to `w8a8gemv.mv`, everything else to `w8a8gemm.mm`).  The arithmetic runs in the H100 kernels behind those two
 shims and in `chitu_b200_quant_act_int8`."""
 from __future__ import annotations
 

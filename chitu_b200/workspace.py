@@ -9,7 +9,7 @@ allocator while that graph can still be replayed.  Therefore
   * `reserve_decode()` sizes every tag once for the largest decode batch, so that in steady state nothing
     grows at all (B200AttnBackend / plugin.install call it);
   * growing while the current stream is being captured raises: the zero-fill of the new buffer would be
-    recorded into the graph and the ticket counters of the tcgen05 GEMM would be shared with eager calls.
+    recorded into the graph and the ticket counters of the wgmma GEMM would be shared with eager calls.
 """
 from __future__ import annotations
 
@@ -38,7 +38,7 @@ def get(tag: str, nbytes: int, device) -> torch.Tensor:
                 "batch size) before capturing")
         if buf is not None:
             _retired.append(buf)          # a captured graph may still point at it
-        # zero-filled: the split-K ticket counters of the tcgen05 GEMM must start at 0 (they self-reset)
+        # zero-filled: the split-K ticket counters of the wgmma GEMM must start at 0 (they self-reset)
         buf = torch.zeros(_round_up_pow2(nbytes), dtype=torch.uint8, device=dev)
         _ws[key] = buf
     return buf

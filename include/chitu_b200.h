@@ -1,5 +1,5 @@
 /*
- * chitu_b200.h — C ABI of the B200-native decode operator library (libchitu_b200.so).
+ * chitu_b200.h — C ABI of the H100-native (sm_90a) decode operator library (libchitu_b200.so).
  *
  * This is the drop-in boundary for Chitu's decode hot path (SURVEY.md §8b). Every entry
  * point replaces one reference operator; the reference interface it replaces is cited as
@@ -82,7 +82,7 @@ int chitu_b200_moe_gate(const void* x, const void* w, const void* bias, int bias
  * moe_align_block_size, fused_moe.py:599-610, inside fused_experts_impl fused_moe.py:1130-1307) of the fused_experts call
  * that follows, into that call's workspace: the pairs are the [T, out_stride] rows of out_indices / out_weights (engines pre-fill column `topk` with the shared
  * expert).  Follow with chitu_b200_fused_experts_planned(T, topk = out_stride, E_total, N1, K1, moe_workspace).
- * One dependent launch fewer per MoE layer; measured SLOWER than the separate plan kernel on B200 (DESIGN.md 3), so the
+ * One dependent launch fewer per MoE layer; the in-kernel hand-off is serial work on the critical path, so the
  * engines keep it off by default. */
 int chitu_b200_moe_gate_plan(const void* x, const void* w, const void* bias, int bias_dtype, int T, int dim, int E,
                              int n_groups, int topk_groups, int topk, int score_sigmoid, float route_scale,
@@ -151,7 +151,7 @@ int chitu_b200_weight_dequant_fp8(const void* x, const float* s, void* y, int B,
 /* Workspace for split-K partials + ticket counters: chitu_b200_linear_workspace_bytes(M_max, N_max).
  * It must be zero-filled ONCE before its first use; every call leaves the counters at zero again. */
 int64_t chitu_b200_linear_workspace_bytes(int M, int N);
-/* impl: 0 = auto, 1 = SIMT weight-streaming GEMV, 2 = tcgen05/TMA swap-AB GEMM. */
+/* impl: 0 = auto, 1 = SIMT weight-streaming GEMV, 2 = wgmma/TMA swap-AB GEMM. */
 /* F.linear for bf16/fp16 weights (linear_deepseek_v3 element_size()>1 branch,
  * model_deepseek_v3.py:84-85; tensor_parallel.py linear_op default). y = x W^T (+bias) (+residual). */
 int chitu_b200_linear_bf16(const void* x, const void* w, const void* bias, const void* residual,
@@ -159,7 +159,7 @@ int chitu_b200_linear_bf16(const void* x, const void* w, const void* bias, const
                            int64_t workspace_bytes, int impl, void* stream);
 /* FeedForward gate_up linear + SiluAndMul in one launch (models/model_llama.py:139-149 + fused_moe.py:24-39):
  * w_pairs = the merged [w1 ; w3] weight [N, K] with rows interleaved at load time (row 2i = gate_i, row 2i+1 = up_i);
- * y [M, N/2] bf16 with the roundings of the two separate reference ops.  bf16, tcgen05 path only. */
+ * y [M, N/2] bf16 with the roundings of the two separate reference ops.  bf16, wgmma path only. */
 int chitu_b200_linear_bf16_silu_pairs(const void* x, const void* w_pairs, void* y, int M, int N, int K, void* workspace,
                                       int64_t workspace_bytes, void* stream);
 /* fp8_gemm_deepseek_v3 (ops.py:452-483; kernel triton_kernels.py:303-365):
@@ -216,14 +216,14 @@ int chitu_b200_gqa_paged_decode_rope(const void* q, int64_t q_sb, void* k_cache,
  * seqlens_excl:[B] (length before this token) ; attention runs over seqlens_excl+1 keys when
  * new_kv != NULL else over seqlens_excl keys.  out:[B,H,C] (latent space). bf16.
  * num_blocks = kv_cache.shape[0] (bounds the TMA tensor map that stages whole 64-key pages).
- * out == NULL (tcgen05 kernel only: page 64): the split merge is deferred to chitu_b200_mla_absorb_o_merge_quant. */
+ * out == NULL (wgmma kernel only: page 64): the split merge is deferred to chitu_b200_mla_absorb_o_merge_quant. */
 int chitu_b200_mla_decode(const void* q_nope, const void* q_pe, void* kv_cache, const void* new_kv,
                           const int32_t* seqlens_excl, const int32_t* block_table, int bt_stride,
                           int B, int H, int C, int R, int page_size, int num_blocks, int max_seqlen_hint,
                           float softmax_scale, void* out, void* workspace, int64_t workspace_bytes,
                           void* stream);
 
-/* invoke_fused_moe_kernel (fused_moe.py:796-891; Triton kernel :62-307) as ONE grouped tcgen05 GEMM:
+/* invoke_fused_moe_kernel (fused_moe.py:796-891; Triton kernel :62-307) as ONE grouped wgmma GEMM:
  * A bf16 [numel/top_k (GEMM1) or numel (top_k = 1), K]; B stacked expert weights [E, N, K] (bf16 for wmode 0, fp8 +
  * B_scale [E, N/128, K/128] for wmode 1 = fp8_w8a8 — A is quantised per_token_group_quant_fp8 inside, as the reference
  * does at :826 — and wmode 2 = soft_fp8); C bf16 = C.view(-1, N) with `numel` rows; sorted_token_ids int32 [EM],
@@ -265,7 +265,7 @@ int chitu_b200_decode_prepare(int32_t* seq_lens_excl, int32_t* seq_lens_incl, in
  * chitu_b200_mla_decode when the same workspace / workspace_bytes are passed.  No host synchronisation. */
 int chitu_b200_attn_plan(const int32_t* seqlens_incl, int B, int heads, int page_size, int max_seqlen_hint,
                          void* workspace, int64_t workspace_bytes, void* stream);
-/* grid.x (upper bound of KV splits per request) the tcgen05 MLA kernel uses for these arguments */
+/* grid.x (upper bound of KV splits per request) the wgmma MLA kernel uses for these arguments */
 int chitu_b200_mla_num_splits(int B, int H, int max_seqlen_hint, int64_t workspace_bytes);
 
 /* MLA weight absorption = the two torch.einsum around the attention call

@@ -519,3 +519,21 @@ def deepseek_decode_step(layers, embed, norm_w, head, cfg, tokens, kv_caches, se
             y = y + y1
         h = h + y
     return linear(rms_norm(h, norm_w, eps, bf), head).float()
+
+
+def check_kv_append(after, before, ref_after, table, lens, page: int) -> float:
+    """KV-page indexing is bit exact: the step touched exactly one row per request — page table[b, L // page], slot
+    L % page — and nothing else.  The appended VALUES come out of a GEMM (accumulation order differs between two correct
+    implementations), so they are compared with the reference's appended rows within 1e-2 instead of bit for bit.
+    Returns that max relative difference."""
+    nb, pg = after.shape[0], after.shape[1]
+    mask = torch.zeros(nb, pg, dtype=torch.bool, device=after.device)
+    for b, L in enumerate(lens.tolist()):
+        mask[int(table[b, L // page]), L % page] = True
+    flat_a, flat_b = after.view(torch.int16).reshape(nb, pg, -1), before.view(torch.int16).reshape(nb, pg, -1)
+    assert torch.equal(flat_a[~mask], flat_b[~mask]), "a cache row other than the appended ones changed"
+    got = after.reshape(nb, pg, -1)[mask].double()
+    want = ref_after.to(after.device).reshape(nb, pg, -1)[mask].double()
+    rel = ((got - want).abs().max() / want.abs().max().clamp(min=1e-30)).item()
+    assert rel < 1e-2, f"appended rows differ from the reference: max rel {rel}"
+    return rel

@@ -1,6 +1,6 @@
-"""Generate tests/golden/*.npz by running the REAL reference (thu-pacman/chitu @ /root/reference).
+"""Generate tests/golden/*.npz by running the REAL reference (a thu-pacman/chitu checkout at $CHITU_REFERENCE).
 
-Run in the authoring container only (the GPU box has no /root/reference):
+Needs that checkout (CPU only):
     python oracle/gen_golden.py
 The reference's Triton kernels run under TRITON_INTERPRET=1 on CPU (SURVEY.md §8c / Appendix A);
 its torch code runs as is.  bf16 tensors are stored as uint16 bit patterns, fp8 as uint8.
@@ -14,11 +14,13 @@ import types
 os.environ["TRITON_INTERPRET"] = "1"
 os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
 os.environ.setdefault("MASTER_PORT", "29577")
-REF = "/root/reference"
+REF = os.environ.get("CHITU_REFERENCE", "reference")   # checkout of thu-pacman/chitu
 sys.path.insert(0, REF)
 
 import numpy as np
 import torch
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
+from oracle.golden_inputs import compact  # noqa: E402
 
 sys.modules["chitu_backend"] = types.ModuleType("chitu_backend")
 for name in ("w8a8gemm", "w8a8gemv"):
@@ -45,8 +47,10 @@ def bits(t: torch.Tensor) -> np.ndarray:
 
 
 def save(name, **arrs):
-    np.savez_compressed(os.path.join(OUT, name + ".npz"), **{k: (bits(v) if torch.is_tensor(v) else np.asarray(v)) for k, v in arrs.items()})
-    print("wrote", name, {k: tuple(np.asarray(bits(v) if torch.is_tensor(v) else v).shape) for k, v in arrs.items()})
+    """Writes the stored form (oracle/golden_inputs.compact): large seeded inputs as SHA-256, near-copies as deltas."""
+    full = {k: (bits(v) if torch.is_tensor(v) else np.asarray(v)) for k, v in arrs.items()}
+    np.savez_compressed(os.path.join(OUT, name + ".npz"), **compact(name, full))
+    print("wrote", name, {k: tuple(v.shape) for k, v in full.items()})
 
 
 def bf16r(t):

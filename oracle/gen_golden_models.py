@@ -1,4 +1,4 @@
-"""Layer-level golden vectors: run the REAL reference transformer blocks (thu-pacman/chitu @ /root/reference)
+"""Layer-level golden vectors: run the REAL reference transformer blocks (a thu-pacman/chitu checkout at $CHITU_REFERENCE)
 on CPU with small dimensions and record inputs, weights and outputs.
 
     python oracle/gen_golden_models.py            (authoring container only; writes tests/golden/block_*.npz)
@@ -19,12 +19,13 @@ os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
 os.environ.setdefault("MASTER_PORT", "29578")
 os.environ.setdefault("RANK", "0")
 os.environ.setdefault("WORLD_SIZE", "1")
-REF = "/root/reference"
+REF = os.environ.get("CHITU_REFERENCE", "reference")   # checkout of thu-pacman/chitu
 sys.path.insert(0, REF)
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
 
 import numpy as np
 import torch
+from oracle.golden_inputs import compact  # noqa: E402
 
 sys.modules["chitu_backend"] = types.ModuleType("chitu_backend")
 for name in ("w8a8gemm", "w8a8gemv"):
@@ -48,8 +49,10 @@ def bits(t):
 
 
 def save(name, **arrs):
-    np.savez_compressed(os.path.join(OUT, name + ".npz"), **{k: bits(v) for k, v in arrs.items()})
-    print("wrote", name, {k: tuple(bits(v).shape) for k, v in arrs.items()})
+    """Writes the stored form (oracle/golden_inputs.compact): large seeded inputs as SHA-256, near-copies as deltas."""
+    full = {k: bits(v) for k, v in arrs.items()}
+    np.savez_compressed(os.path.join(OUT, name + ".npz"), **compact(name, full))
+    print("wrote", name, {k: tuple(v.shape) for k, v in full.items()})
 
 
 def bootstrap():

@@ -1,10 +1,10 @@
 """Per-kernel microbenchmarks (dev tool): warm CUDA-event timing of the hot kernels at the bench shapes.
 
 Every case rotates over enough distinct copies of its HBM-resident operands (weights / KV pages) that a call never
-finds them in the 126 MB L2 — the honest way to defeat the cache: a memset-style flush leaves dirty lines whose
-write-back is charged to the next kernel (scripts/gqa_sweep.py read 64 us for a kernel ncu times at 46 us).
+finds them in the 50 MB L2 — the honest way to defeat the cache: a memset-style flush leaves dirty lines whose
+write-back is charged to the next kernel.
 
-    python scripts/kernel_bench.py gemm | mla | gqa | moe | all        (needs a B200; use under gpurun)
+    python scripts/kernel_bench.py gemm | mla | gqa | moe | all        (needs an H100)
 """
 import math
 import os

@@ -1,4 +1,4 @@
-"""dev tool: where the tcgen05 MLA decode kernel spends its time INSIDE the decode graph (profiling build of the library,
+"""dev tool: where the wgmma MLA decode kernel spends its time INSIDE the decode graph (profiling build of the library,
 csrc/mla_tc.cu probe()): every CTA records %globaltimer at fixed points; the last layer's launch is what remains.
 
     python scripts/mla_probe.py [bs] [layers]

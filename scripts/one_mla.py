@@ -1,4 +1,4 @@
-"""dev tool: a few tcgen05 MLA decode launches at the bench shape (B=16, S=4096, H=16) for `ncu --set full`"""
+"""dev tool: a few wgmma MLA decode launches at the bench shape (B=16, S=4096, H=16) for `ncu --set full`"""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

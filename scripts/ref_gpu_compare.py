@@ -1,13 +1,12 @@
 """GPU comparator (SURVEY §8d "bar to beat", VERDICT r1 item 9): the UNMODIFIED reference installed under baseline/_ref
-(`python -m pip install --no-index --no-build-isolation --no-deps --target baseline/_ref <copy of the reference>`, see
-DESIGN.md §5) — its Triton fp8 GEMM, Triton MLA decode, Triton fused experts, and flash_attn paged decode, all through the
-reference's own functions / backend classes — timed on the SAME B200 beside this repository's kernels, on the same inputs,
+(`python -m pip install --no-index --no-build-isolation --no-deps --target baseline/_ref <copy of the reference>`) — its Triton fp8 GEMM, Triton MLA decode, Triton fused experts, and flash_attn paged decode, all through the
+reference's own functions / backend classes — timed on the SAME GPU beside this repository's kernels, on the same inputs,
 at the DeepSeek-R1 tp=8 / LLaMA-3-8B decode shapes.  Both sides run inside CUDA graphs over rotating operand sets larger
 than L2 (the reference captures its decode step the same way, models/model.py:537-622), CUDA-event timed.
 
     python scripts/ref_gpu_compare.py [bs]          -> one JSON line (also called by bench.py --workload ref-kernels)
 
-Nothing here is on the product path; the reference is only ever imported from baseline/_ref (never /root/reference)."""
+Nothing here is on the product path; the reference is only ever imported from baseline/_ref (never from a source checkout)."""
 import json
 import os
 import sys

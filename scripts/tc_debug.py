@@ -1,4 +1,4 @@
-"""GPU debugging aid for the tcgen05 GEMM: runs each case in isolation and prints the first error."""
+"""GPU debugging aid for the wgmma GEMM: runs each case in isolation and prints the first error."""
 import sys, os, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

@@ -12,7 +12,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 # the stamps are compiled into a separate profiling build of the library only
 _TL = os.path.join(ROOT, "chitu_b200", "libchitu_b200_tl.so")
-if not os.path.exists(_TL):          # built here (CPU box, `make -C chitu_b200/csrc tl`) and shipped with the snapshot
+if not os.path.exists(_TL):          # `make -C chitu_b200/csrc tl`
     subprocess.run(["make", "-C", os.path.join(ROOT, "chitu_b200", "csrc"), "tl"], check=True, capture_output=True)
 os.environ["CHITU_B200_LIB"] = _TL
 import torch

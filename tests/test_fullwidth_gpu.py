@@ -21,6 +21,7 @@ import torch
 
 import torch_ref as R
 from conftest import cos_diff, max_rel
+from oracle import chitu_oracle as O
 
 pytestmark = pytest.mark.gpu
 BF, F8 = torch.bfloat16, torch.float8_e4m3fn
@@ -32,7 +33,7 @@ def _fp8_weight(gen, *shape, scale=0.02):
     return quantize_fp8_block(torch.randn(*shape, generator=gen, device=DEV) * scale)
 
 
-# ------------------------------------------------------------------ a8: every UMMA-N of the fp8 tcgen05 GEMM
+# ------------------------------------------------------------------ a8: every wgmma N (token tile) of the fp8 GEMM
 @pytest.mark.parametrize("M", [24, 48, 100, 128, 200, 256])
 @pytest.mark.parametrize("N,K", [(4608, 7168), (7168, 2304), (3072, 1536)])
 def test_fp8_gemm_wide_batches(M, N, K):
@@ -97,21 +98,6 @@ def test_fused_experts_deepseek_r1_shape(T):
 
 
 
-def _check_append(after, before, ref_after, table, lens, page):
-    """KV-page indexing is bit exact: the step touched exactly one row per request — page table[b, L // page], slot
-    L % page — and nothing else; the appended VALUES come out of a GEMM (accumulation order differs between two correct
-    implementations), so they are compared with the reference's appended row within 1e-2 instead of bit for bit."""
-    a, b0, r = after.view(torch.int16), before.view(torch.int16), ref_after
-    nb, pg = after.shape[0], after.shape[1]
-    mask = torch.zeros(nb, pg, dtype=torch.bool, device=after.device)
-    ll = lens.tolist()
-    for b in range(len(ll)):
-        mask[table[b, ll[b] // page].long(), ll[b] % page] = True
-    flat_a, flat_b = a.reshape(nb, pg, -1), b0.reshape(nb, pg, -1)
-    assert torch.equal(flat_a[~mask], flat_b[~mask]), "a cache row other than the appended ones changed"
-    got, want = after.reshape(nb, pg, -1)[mask].float(), r.reshape(nb, pg, -1)[mask].float()
-    assert max_rel(got, want) < 1e-2, "appended rows differ from the reference"
-
 # ------------------------------------------------------------------ whole steps at real width
 def _routes_agree(eng, routes, cfg):
     """(all equal, any near-tie).  A differing selection is excused only when the reference's own masked scores of the
@@ -168,7 +154,7 @@ def test_deepseek_r1_tp8_shard_layers_teacher_forced():
         kc, kc2, routes, routes2 = before[li].clone(), before[li].clone(), [], []
         ref = R.deepseek_layer(L, hs[li], kc, ln, eng.block_table, cos, sin, cfg, eng.H, routes)
         ref2 = R.deepseek_layer(L, _ulp_perturb(hs[li], gen), kc2, ln, eng.block_table, cos, sin, cfg, eng.H, routes2)
-        _check_append(eng.kv_cache[li], before[li], kc, eng.block_table, ln, 64)
+        O.check_kv_append(eng.kv_cache[li], before[li], kc, eng.block_table, ln, 64)
         same_routes = True
         if routes:
             idx, sc = routes[0]
@@ -224,8 +210,8 @@ def test_llama3_8b_full_depth_step_logits_within_1e2():
     eng.decode(tokens.pin_memory())
     torch.cuda.synchronize()
     got = eng.logits.float()
-    _check_append(eng.k_cache[0], kc0_before, kc[0], eng.block_table, ln, 256)
-    _check_append(eng.v_cache[0], vc0_before, vc[0], eng.block_table, ln, 256)
+    O.check_kv_append(eng.k_cache[0], kc0_before, kc[0], eng.block_table, ln, 256)
+    O.check_kv_append(eng.v_cache[0], vc0_before, vc[0], eng.block_table, ln, 256)
     mr, cd = max_rel(got, ref), cos_diff(got, ref)
     print(f"llama-3-8b 32 layers: logits max_rel {mr:.3e} (floor {floor_mr:.3e}) cos_diff {cd:.3e} (floor {floor_cd:.3e})")
     assert mr < max(1e-2, 3 * floor_mr) and mr < 0.1
@@ -234,7 +220,7 @@ def test_llama3_8b_full_depth_step_logits_within_1e2():
 
 # ------------------------------------------------------------------ a21: Mixtral sparse-MoE block through fused experts
 def test_mixtral_block_vs_reference_golden():
-    """The GPU path (softmax top-2 renormalised router kernel + grouped bf16 tcgen05 experts) against the output of the
+    """The GPU path (softmax top-2 renormalised router kernel + grouped bf16 wgmma experts) against the output of the
     REAL SparseMoeBlockHFMixtral recorded in tests/golden/block_mixtral_moe.npz (oracle/gen_golden_models.py)."""
     from conftest import Golden
     from chitu_b200 import fused_moe
@@ -253,29 +239,55 @@ def test_mixtral_block_vs_reference_golden():
 
 
 def test_mixtral_engine_step_vs_torch_ref():
-    """4 layers of Mixtral-8x7B at real width, one rank's tp=4 shard (8 q / 2 kv heads, expert dim 3584), bs=16, S=4096."""
+    """Mixtral-8x7B at real width, one rank's tp=4 shard (8 q / 2 kv heads, expert dim 3584), bs=16, S=4096: a 1-layer
+    and a 4-layer step against the bf16 torch restatement.  Routing must be identical.  On synthetic weights the step
+    amplifies rounding with depth: a one-ulp change of the embedding moves the reference itself by mr 0.02-0.04 / cd
+    1.5-2.2e-4 after one layer and mr 0.14 / cd 1.9e-3 after four, and a different split-KV count (summation order only)
+    moves this engine by a similar amount (H100: 4-layer mr 0.045-0.12).  So the logits must agree with the reference at
+    least as well as the reference agrees with itself under that perturbation (factor 1, not 3), the floor is taken
+    only from a perturbation that leaves every layer's routing unchanged (a routing flip is not rounding noise), and at
+    one layer the cosine bound of 1e-4 holds outright."""
     from chitu_b200.engine_mixtral import MixtralConfig, MixtralDecodeEngine
-    cfg = MixtralConfig(n_layers=4)
     B, S = 16, 4096
-    eng = MixtralDecodeEngine(cfg, max_reqs=B, max_seq_len=S + 256, device=DEV, tp_size=4)
-    eng.set_synthetic_context(S)
-    lens = torch.full((B,), S, dtype=torch.int32)
-    lens[1], lens[2], lens[3] = 255, 256, 1000
-    eng.seq_lens.copy_(lens)
-    tokens = torch.randint(100, 1000, (B,), generator=torch.Generator().manual_seed(0))
-    kc = [eng.k_cache[l].clone() for l in range(cfg.n_layers)]
-    vc = [eng.v_cache[l].clone() for l in range(cfg.n_layers)]
-    kc0_before = kc[0].clone()
-    ln = eng.seq_lens.clone()
-    cos, sin = eng.cos_table[ln.long()], eng.sin_table[ln.long()]
-    ref, routes = R.mixtral_decode_step(eng.layers, eng.embed, eng.norm, eng.head, tokens.to(DEV), kc, vc, ln, eng.block_table,
-                                        cos, sin, eng.Hq, eng.Hkv, eng.topk, cfg.norm_eps)
-    eng.decode(tokens.pin_memory())
-    torch.cuda.synchronize()
-    got = eng.logits.float()
-    _check_append(eng.k_cache[0], kc0_before, kc[0], eng.block_table, ln, 256)
-    same = all(torch.equal(eng.gate_i_all[li].sort(dim=-1)[0], r.sort(dim=-1)[0]) for li, r in enumerate(routes))
-    mr, cd = max_rel(got, ref), cos_diff(got, ref)
-    print(f"mixtral tp4 shard, 4 layers: same_routes {same} logits max_rel {mr:.3e} cos_diff {cd:.3e}")
-    if same:
-        assert mr < 1e-2 and cd < 1e-4
+    for n_layers, cap_mr, cap_cd in ((1, 5e-2, 1e-4), (4, 0.15, 2e-3)):
+        cfg = MixtralConfig(n_layers=n_layers)
+        eng = MixtralDecodeEngine(cfg, max_reqs=B, max_seq_len=S + 256, device=DEV, tp_size=4)
+        eng.set_synthetic_context(S)
+        lens = torch.full((B,), S, dtype=torch.int32)
+        lens[1], lens[2], lens[3] = 255, 256, 1000
+        eng.seq_lens.copy_(lens)
+        tokens = torch.randint(100, 1000, (B,), generator=torch.Generator().manual_seed(0))
+        kc0 = [eng.k_cache[l].clone() for l in range(cfg.n_layers)]
+        vc0 = [eng.v_cache[l].clone() for l in range(cfg.n_layers)]
+        ln = eng.seq_lens.clone()
+        cos, sin = eng.cos_table[ln.long()], eng.sin_table[ln.long()]
+
+        def reference(embed):
+            kc, vc = [c.clone() for c in kc0], [c.clone() for c in vc0]
+            out, routes = R.mixtral_decode_step(eng.layers, embed, eng.norm, eng.head, tokens.to(DEV), kc, vc, ln,
+                                                eng.block_table, cos, sin, eng.Hq, eng.Hkv, eng.topk, cfg.norm_eps)
+            return out, routes, kc
+
+        def same_routes(a, b):
+            return all(torch.equal(x.sort(dim=-1)[0], y.sort(dim=-1)[0]) for x, y in zip(a, b))
+
+        ref, routes, kc = reference(eng.embed)
+        floor = None
+        for seed in range(1, 7):
+            ref2, routes2, _ = reference(_ulp_perturb(eng.embed, torch.Generator(device=DEV).manual_seed(seed)))
+            if same_routes(routes2, routes):
+                floor = (max_rel(ref2, ref), cos_diff(ref2, ref))
+                break
+        eng.decode(tokens.pin_memory())
+        torch.cuda.synchronize()
+        got = eng.logits.float()
+        O.check_kv_append(eng.k_cache[0], kc0[0], kc[0], eng.block_table, ln, 256)
+        assert same_routes([eng.gate_i_all[li] for li in range(n_layers)], routes), f"{n_layers} layers: routing differs"
+        mr, cd = max_rel(got, ref), cos_diff(got, ref)
+        floor_mr, floor_cd = floor if floor is not None else (1e-2, 1e-4)   # no routing-preserving perturbation: strict
+        print(f"mixtral tp4 shard, {n_layers} layers: logits max_rel {mr:.3e} (floor {floor_mr:.3e}) "
+              f"cos_diff {cd:.3e} (floor {floor_cd:.3e})")
+        assert mr < max(1e-2, floor_mr) and mr < cap_mr
+        assert cd < max(1e-4, floor_cd) and cd < cap_cd
+        del eng
+        torch.cuda.empty_cache()

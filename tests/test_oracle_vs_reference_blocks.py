@@ -1,5 +1,5 @@
 """Pins the oracle's MODEL-LEVEL restatements against whole transformer blocks of the real reference
-(tests/golden/block_*.npz, written by oracle/gen_golden_models.py from /root/reference).  CPU only."""
+(tests/golden/block_*.npz, written by oracle/gen_golden_models.py from the reference).  CPU only."""
 import numpy as np
 import torch
 

@@ -224,7 +224,7 @@ LINEAR_IMPLS = [1, 2]
 def _need_impl(impl):
     from chitu_b200 import _lib
     if impl == 2 and _lib.load().chitu_b200_linear_workspace_bytes(16, 4096) <= 0:
-        pytest.skip("tcgen05 path not built in this library")
+        pytest.skip("wgmma path not built in this library")
 
 
 @pytest.mark.parametrize("impl", LINEAR_IMPLS)
@@ -280,7 +280,7 @@ def test_fp8_gemm_golden():
 @pytest.mark.parametrize("M,N,K", [(1, 2112, 7168), (16, 1024, 2048), (16, 7168, 2048), (7, 3072, 1536), (48, 4608, 7168),
                                    (200, 7168, 2304)])
 def test_soft_fp8_gemm(impl, M, N, K):
-    """soft_fp8_gemm_deepseek_v3 (ops.py:486-511): impl 2 = tcgen05 (fp8 -> bf16 conversion warps between TMA and the
+    """soft_fp8_gemm_deepseek_v3 (ops.py:486-511): impl 2 = wgmma (fp8 -> bf16 conversion warps between TMA and the
     bf16 MMA, same "weight rounded to bf16 before the MMA" semantics), impl 1 = SIMT."""
     from chitu_b200 import ops
     _need_impl(impl)

@@ -1,5 +1,5 @@
-"""`chitu_b200.install()` against the REAL reference package (authoring container only: skipped where
-/root/reference does not exist): every operator name the reference's model files hold is rebound to the B200
+"""`chitu_b200.install()` against the REAL reference package (a thu-pacman/chitu checkout named by $CHITU_REFERENCE;
+skipped without one): every operator name the reference's model files hold is rebound to this library's
 implementation, and each replacement accepts the reference's parameters (drop-in signature check)."""
 import json
 import os
@@ -9,7 +9,7 @@ import sys
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = "/root/reference"
+REF = os.environ.get("CHITU_REFERENCE", "")
 
 SCRIPT = r"""
 import inspect, json, os, sys, types
@@ -61,7 +61,7 @@ print('RESULT' + json.dumps(res))
 """
 
 
-@pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "chitu")), reason="the reference tree is only present in the authoring container")
+@pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "chitu")), reason="needs a reference checkout ($CHITU_REFERENCE)")
 def test_install_rebinds_every_holder_and_signatures_are_drop_in():
     env = dict(os.environ, TRITON_INTERPRET="1")
     out = subprocess.run([sys.executable, "-c", SCRIPT % {"ref": REF, "root": ROOT}], capture_output=True, text=True,

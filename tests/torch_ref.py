@@ -1,6 +1,6 @@
 """TEST INFRASTRUCTURE — device-agnostic fp32 torch restatements of the oracle's model-level functions, so that
 full-width parity (dim 7168, 257 experts, S = 4096) can be checked ON THE GPU in seconds (SURVEY Appendix A:
-"full-size parity on the B200 box is checked against the torch fp32 restatements running on GPU").
+"full-size parity on the GPU is checked against the torch fp32 restatements running on GPU").
 
 Every function mirrors the function of the same name in oracle/chitu_oracle.py (which cites the reference lines and is
 pinned against the reference's goldens); `tests/test_torch_ref_cpu.py` proves the two agree on CPU at small shapes.
