@@ -1,9 +1,9 @@
 """Drop-in attention backend for `chitu.attn_backend` (reference: chitu/attn_backend.py).
 
 `B200AttnBackend` implements the four methods the models call (SURVEY.md §8b):
-prepare_metadata_for_decode, attn_varlen_func (prefill: out of the decode hot path, delegated to
-the reference-style fp32 formulation on the GPU), attn_with_kvcache (GQA paged decode with
-in-place append) and mla_attn_with_kvcache (absorbed-MLA paged decode with fused append).
+prepare_metadata_for_decode, attn_varlen_func (prefill: the absorbed-MLA form runs the sm_90a
+prefill kernel; GQA prefill stays on flash_attn / torch SDPA), attn_with_kvcache (GQA paged decode
+with in-place append) and mla_attn_with_kvcache (absorbed-MLA paged decode with fused append).
 """
 from __future__ import annotations
 
@@ -18,6 +18,7 @@ from ._lib import check, current_stream, dtype_code, ptr, require_cuda
 __all__ = ["AttnBackend", "B200AttnBackend"]
 
 _MAX_SPLITS = 128
+_MLA_QK, _MLA_V = 576, 512          # absorbed MLA: kv_lora_rank + qk_rope_head_dim, kv_lora_rank
 
 
 class AttnBackend:
@@ -98,12 +99,44 @@ class B200AttnBackend(AttnBackend):
         buf = workspace.get("attn", self._ws_bytes(B, H, DV), device)
         return buf, buf.numel()
 
-    # -- prefill (NOT on the decode hot path; SURVEY §8f n4, §8b "inherit prefill from Ref/flash_attn").
-    # Exactly what the reference's FlashAttnBackend does (attn_backend.py:193-206): flash_attn_varlen_func when the
-    # library is importable; otherwise torch's fused SDPA per sequence (no [H, Tq, Tk] fp32 score tensor, no host loop
-    # over heads).  Both are library calls on a path this repository does not optimise.
+    # -- prefill (SURVEY §8f n4).  attn_backend.py:193-206 (FlashAttnBackend), flash_attn_varlen_func semantics.
     def attn_varlen_func(self, q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k,
                          dropout_p=0.0, causal=False, window_size=(-1, -1), softcap=0.0, softmax_scale=None):
+        """Varlen prefill attention.  The absorbed-MLA form DeepSeek's prefill calls (model_deepseek_v3.py:588-602):
+        bf16 q [Tq, H, 576], k [Tk, 1, 576], v [Tk, 1, 512], no dropout / window / softcap, runs the sm_90a kernel
+        (chitu_b200_mla_prefill): no host synchronisation, capturable in a CUDA graph, deterministic; returns
+        [Tq, H, 512].  softmax_scale=None means 1/sqrt(576).  Every other shape (GQA prefill) takes flash_attn, or
+        torch SDPA per sequence when flash_attn is not installed."""
+        if (q.dtype == k.dtype == v.dtype == torch.bfloat16 and q.dim() == 3 and q.shape[-1] == _MLA_QK
+                and k.dim() == 3 and tuple(k.shape[1:]) == (1, _MLA_QK) and v.dim() == 3
+                and tuple(v.shape[1:]) == (1, _MLA_V) and dropout_p == 0.0 and tuple(window_size) == (-1, -1)
+                and softcap == 0.0):
+            return self._mla_prefill(q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, causal, softmax_scale)
+        return self._attn_varlen_library(q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, dropout_p,
+                                         causal, window_size, softcap, softmax_scale)
+
+    @staticmethod
+    def _mla_prefill(q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, causal, softmax_scale):
+        require_cuda(q, k, v, cu_seqlens_q, cu_seqlens_k)
+        assert q.is_contiguous() and k.stride(-1) == 1 and v.stride(-1) == 1
+        assert cu_seqlens_q.dtype == torch.int32 and cu_seqlens_k.dtype == torch.int32
+        assert cu_seqlens_q.is_contiguous() and cu_seqlens_k.is_contiguous()
+        assert cu_seqlens_q.numel() == cu_seqlens_k.numel() >= 1
+        Tq, H, _ = q.shape
+        out = torch.empty((Tq, H, _MLA_V), dtype=q.dtype, device=q.device)
+        scale = softmax_scale if softmax_scale is not None else 1.0 / math.sqrt(_MLA_QK)
+        check(_lib.load().chitu_b200_mla_prefill(
+            ptr(q), ptr(k), k.stride(0), ptr(v), v.stride(0), ptr(cu_seqlens_q), ptr(cu_seqlens_k),
+            cu_seqlens_q.numel() - 1, H, Tq, k.shape[0], int(max_seqlen_q), int(bool(causal)), float(scale), ptr(out),
+            current_stream()), "mla_prefill")
+        return out
+
+    # Exactly what the reference's FlashAttnBackend does (attn_backend.py:193-206): flash_attn_varlen_func when the
+    # library is importable; otherwise torch's fused SDPA per sequence (no [H, Tq, Tk] fp32 score tensor, no host loop
+    # over heads).  Both are library calls on a path this repository does not optimise (GQA prefill).
+    @staticmethod
+    def _attn_varlen_library(q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k,
+                             dropout_p=0.0, causal=False, window_size=(-1, -1), softcap=0.0, softmax_scale=None):
         assert dropout_p == 0.0
         if q.dtype in (torch.float16, torch.bfloat16) and q.shape[-1] <= 256 and k.shape[-1] == v.shape[-1]:
             try:

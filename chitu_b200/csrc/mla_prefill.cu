@@ -1,0 +1,322 @@
+// Absorbed-MLA prefill attention on the Hopper tensor cores (sm_90a): wgmma + TMA + mbarrier.
+//
+// Replaces the flash_attn / SDPA delegation of AttnBackend.attn_varlen_func (FlashAttnBackend, attn_backend.py:193-206)
+// for the call DeepSeek's prefill makes (model_deepseek_v3.py:588-602): absorbed MLA in MQA form,
+//   q [Tq, H, 576] = [q_nope . W_uk | q_pe],  k [Tk, 1, 576] = [kv_norm(kv) | k_pe],  v [Tk, 1, 512] = kv_norm(kv),
+// ragged batch by cu_seqlens_q / cu_seqlens_k, flash_attn_varlen_func semantics: fp32 scores and softmax, P rounded to
+// bf16 before P.V, causal mask aligned bottom-right (query i sees keys j <= i + Lk - Lq), rows that see no key are 0.
+//
+// Mapping: q is flattened to [Tq * H, 576] rows, token-major (row r of a sequence is token r / H, head r % H), and one
+// CTA owns 64 rows of one sequence.  Both products are SWAPPED, as in the decode kernel (mla_tc.cu), so the 64 rows are
+// the wgmma N dimension:
+//   S^T[64 keys x 64 rows]  = K[64 x 576] . Q^T           A = staged K chunk (K-major), B = staged Q chunk
+//   O^T[512 dims x 64 rows] += V^T[512 x 64] . P^T         A = staged V chunks read MN-major, B = P[64 rows x 64 keys]
+// O^T is 128 fp32 registers per thread for 256 dims, so the dims are split over two warpgroups (256 threads):
+//   WG0 (warps 0-3)  S^T, the online softmax (fp32, log2 domain), P -> shared memory, O^T for dims 0..255
+//   WG1 (warps 4-7)  O^T for dims 256..511: waits for P of the tile, applies WG0's rescale factors, P.V
+// There is no producer warp: with a third warpgroup the launch bound caps every thread at 168 registers, which spills
+// WG0 (O^T + S^T + row sums).  Instead each TMA load is issued by the warpgroup that frees its slot, one tile ahead:
+//   K chunks of tile i+1   by WG1 once P(i) is published (WG0 has finished S(i), so the K slots are free)
+//   V chunks 0-3 / 4-7     by WG0 / WG1 right after their own P.V of tile i
+// so K(i+1) streams in during softmax(i) and P.V(i), and V(i+1) during S(i+1).
+// Shared memory: 17 x 8 KB chunk slots (one 64-key tile: 9 K + 8 V boxes [64 rows x 128 B]) + Q 72 KB + P 8 KB
+// = 216 KB + 1 KB alignment.  The Q tile is reused at the end to stage the bf16 output for 16-byte coalesced stores.
+// Scheduling: a 1-D grid of (row tile, sequence) with the LAST row tiles first: under the causal mask they see the most
+// keys, so the long CTAs start in the first wave and the short ones fill in behind them.
+// Deterministic: every key of a row is reduced by one CTA in a fixed order (no split over keys).
+#include <cuda.h>
+#include <limits.h>
+
+#include "common.cuh"
+#include "tc_ptx.cuh"
+#include "wgmma.cuh"
+
+namespace cb {
+namespace {
+
+constexpr int kC = 512, kR = 64, kRow = kC + kR;
+constexpr int kTile = 64;                      // keys per tile
+constexpr int kRows = 64;                      // query rows (token, head) per CTA
+constexpr int kSlot = 64 * 128;                // 8 KB: one TMA box [64 rows x 128 B]
+constexpr int kKC = kRow / 64, kVC = kC / 64;  // 9 K chunks, 8 V chunks per key tile
+constexpr int kTC = kKC + kVC;                 // chunk c of every tile lives in slot c
+constexpr int kQBytes = kKC * kSlot;           // Q as 9 K-major chunks [64 rows x 128 B]
+constexpr int kPBytes = kRows * 128;           // P as [64 rows x 64 keys] bf16, K-major
+constexpr int kSmemBytes = kTC * kSlot + kQBytes + kPBytes;
+constexpr int kOutPitch = kC * 2 + 16;         // staged output row in bytes (padded: the 4 rows a store touches differ in bank)
+static_assert(kRows * kOutPitch <= kQBytes, "the output tile is staged in the Q buffer");
+constexpr float kLog2e = 1.4426950408889634f;
+constexpr float kRescaleThreshold = 8.f;       // log2 domain
+constexpr int kThreads = 256;
+
+// one 64-key tile's chunks [c_begin, c_end) into their slots (issued by one thread)
+__device__ __forceinline__ void load_chunks(const CUtensorMap* mk, const CUtensorMap* mv, uint8_t* s_ring, uint64_t* full,
+                                            int c_begin, int c_end, int row, uint64_t pol) {
+  for (int c = c_begin; c < c_end; ++c) {
+    mbar_expect_tx(&full[c], kSlot);
+    if (c < kKC) tma_load_2d(s_ring + c * kSlot, mk, &full[c], c * 64, row, pol);
+    else tma_load_2d(s_ring + c * kSlot, mv, &full[c], (c - kKC) * 64, row, pol);
+  }
+}
+
+__global__ void __launch_bounds__(kThreads, 1) mla_prefill_kernel(
+    const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
+    const __grid_constant__ CUtensorMap map_v, const int32_t* __restrict__ cu_q, const int32_t* __restrict__ cu_k, int B,
+    int H, int row_tiles, int causal, float scale, __nv_bfloat16* __restrict__ out) {
+  extern __shared__ __align__(1024) uint8_t mla_prefill_smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(mla_prefill_smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* s_ring = smem;                                   // [kTC][64 rows][128 B]  K / V chunks of one tile
+  uint8_t* s_q = s_ring + kTC * kSlot;                      // [9][64 rows][128 B]; output staging at the end
+  uint8_t* s_p = s_q + kQBytes;                             // [64 rows][128 B]
+  __shared__ __align__(8) uint64_t full_b[kTC], q_bar, p_full, p_empty;
+  __shared__ float red[4][kRows];                           // per-warp row partials: tile max, then the final row sum
+  __shared__ float s_m[kRows];                              // running row max (log2 domain)
+  __shared__ float s_alpha[kRows];                          // O rescale factor of the tile whose P is in s_p
+  __shared__ float s_inv[kRows];                            // 1 / row sum (0 for a row that sees no key)
+
+  const int b = blockIdx.x % B;
+  const int tile = row_tiles - 1 - blockIdx.x / B;          // last row tiles (most causal work) first
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const bool wg0 = __shfl_sync(0xffffffffu, threadIdx.x / 128, 0) == 0;   // warp-uniform for the compiler (wgmma paths)
+
+  cb::pdl_prologue();                                       // q, k, v and the lengths are written by earlier kernels
+  const int q0 = cu_q[b], Lq = cu_q[b + 1] - q0;
+  const int k0 = cu_k[b], Lk = cu_k[b + 1] - k0;
+  const int nrows = Lq * H;
+  const int r0 = tile * kRows;
+  if (r0 >= nrows) return;                                  // uniform over the CTA
+  const int rlast = min(r0 + kRows, nrows) - 1;
+  // keys visible to row r (token r / H) are [0, lim(r)); lim is non-decreasing in r
+  auto lim = [&](int r) { return causal ? max(0, min(Lk, r / H + 1 + Lk - Lq)) : max(Lk, 0); };
+  const int nkeys = lim(rlast);
+  const int all_see = lim(r0);                              // keys below this are visible to every row of the tile
+  const int ntiles = (nkeys + kTile - 1) / kTile;
+  const uint64_t pol_kv = l2_policy_evict_last();           // K / V are re-read by every row tile of the sequence
+
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < kTC; ++i) mbar_init(&full_b[i], 1);
+    mbar_init(&q_bar, 1);
+    mbar_init(&p_full, 1);
+    mbar_init(&p_empty, 4);                                 // one arrival per WG1 warp
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    if (ntiles > 0) {
+      mbar_expect_tx(&q_bar, kQBytes);
+      for (int c = 0; c < kKC; ++c) tma_load_2d(s_q + c * kSlot, &map_q, &q_bar, c * 64, q0 * H + r0, l2_policy_evict_first());
+      load_chunks(&map_k, &map_v, s_ring, full_b, 0, kTC, k0, pol_kv);
+    }
+  }
+  if (threadIdx.x < kRows) s_m[threadIdx.x] = -INFINITY;
+  __syncthreads();
+
+  const int krow = (warp & 3) * 16 + (lane >> 2);           // fragment rows krow, krow + 8: keys of S^T, dims of O^T
+  const int qd = 2 * (lane & 3);                            // fragment columns 8 nb + qd + j: query rows of the tile
+  const uint32_t ring_a = smem_u32(s_ring), q_a = smem_u32(s_q), p_a = smem_u32(s_p);
+  const int vc0 = wg0 ? 0 : 4;                              // this warpgroup's V chunks (64 dims each)
+  float o[4][32];                                           // O^T tile m: dims 64 (vc0 + m) + krow (+8), rows as S^T
+#pragma unroll
+  for (int m = 0; m < 4; ++m)
+#pragma unroll
+    for (int e = 0; e < 32; ++e) o[m][e] = 0.f;
+  float l_part[16];                                         // WG0: this thread's share of the row sums, x = 2 nb + j
+#pragma unroll
+  for (int x = 0; x < 16; ++x) l_part[x] = 0.f;
+
+  if (wg0 && ntiles > 0) mbar_wait(&q_bar, 0);
+  const float sc = scale * kLog2e;
+  for (int it = 0; it < ntiles; ++it) {
+    const uint32_t ph = it & 1;                             // phase of every chunk slot for tile it
+    const bool more = it + 1 < ntiles;
+    const int next_row = k0 + (it + 1) * kTile;             // rows past the sequence are masked; past the tensor, zero
+    if (wg0) {
+      // ---- S^T = K . Q^T over the 9 chunks of 64 dims ----
+      float s[32];
+#pragma unroll
+      for (int e = 0; e < 32; ++e) s[e] = 0.f;
+      wgmma_fence();
+      for (int c = 0; c < kKC; ++c) {
+        mbar_wait(&full_b[c], ph);
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+          WgmmaN<64>::bf16<0>(s, make_sw128_desc(ring_a + c * kSlot + 32 * k, 16, 1024),
+                              make_sw128_desc(q_a + c * kSlot + 32 * k, 16, 1024), (c | k) != 0);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+
+      // ---- scale, mask (only tiles that reach past some row's last visible key), per-row tile max ----
+      const int key0 = it * kTile;
+      if (key0 + kTile > all_see) {
+#pragma unroll
+        for (int x = 0; x < 16; ++x) {
+          const int lr = lim(r0 + 8 * (x >> 1) + qd + (x & 1));
+          const int e = 4 * (x >> 1) + (x & 1);
+          s[e] = key0 + krow < lr ? s[e] * sc : -INFINITY;
+          s[e + 2] = key0 + krow + 8 < lr ? s[e + 2] * sc : -INFINITY;
+        }
+      } else {
+#pragma unroll
+        for (int e = 0; e < 32; ++e) s[e] *= sc;
+      }
+#pragma unroll
+      for (int x = 0; x < 16; ++x) {
+        const int e = 4 * (x >> 1) + (x & 1);
+        const float mx = rows_max(fmaxf(s[e], s[e + 2]));
+        if (lane < 4) red[warp][8 * (x >> 1) + qd + (x & 1)] = mx;
+      }
+      mbar_wait(&p_empty, ph ^ 1);                          // WG1 is done with P / alpha of tile it - 1
+      asm volatile("bar.sync 1, 128;" ::: "memory");
+      // ---- running max: moved only when a row's max grew by more than 2^8 (exact result: P, l, O share it) ----
+      if (threadIdx.x < kRows) {
+        const int r = threadIdx.x;
+        const float mt = fmaxf(fmaxf(red[0][r], red[1][r]), fmaxf(red[2][r], red[3][r]));
+        const float mo = s_m[r];
+        float a = 1.f;
+        if (mt > mo + kRescaleThreshold) {                  // also the first finite max (mo = -inf): a = 0
+          a = exp2f(mo - mt);
+          s_m[r] = mt;
+        }
+        s_alpha[r] = a;
+      }
+      asm volatile("bar.sync 1, 128;" ::: "memory");
+      // ---- P = exp2(S - m) -> bf16 -> shared memory as P[row][key] (K-major, swizzled) ----
+      bool need = false;
+#pragma unroll
+      for (int x = 0; x < 16; ++x) {
+        const int r = 8 * (x >> 1) + qd + (x & 1);
+        const float m = s_m[r];
+        const float mr = m == -INFINITY ? 0.f : m;          // a row with no visible key so far: P = 0
+        const float a = s_alpha[r];
+        need |= a != 1.f;
+        const int e = 4 * (x >> 1) + (x & 1);
+        const float p0 = exp2f(s[e] - mr), p1 = exp2f(s[e + 2] - mr);
+        l_part[x] = l_part[x] * a + p0 + p1;
+        *reinterpret_cast<__nv_bfloat16*>(s_p + sw128(r, krow >> 3) + (krow & 7) * 2) = __float2bfloat16_rn(p0);
+        *reinterpret_cast<__nv_bfloat16*>(s_p + sw128(r, (krow >> 3) + 1) + (krow & 7) * 2) = __float2bfloat16_rn(p1);
+      }
+      if (need) {
+#pragma unroll
+        for (int x = 0; x < 16; ++x) {
+          const float a = s_alpha[8 * (x >> 1) + qd + (x & 1)];
+          const int e = 4 * (x >> 1) + (x & 1);
+#pragma unroll
+          for (int m = 0; m < 4; ++m) { o[m][e] *= a; o[m][e + 2] *= a; }
+        }
+      }
+      fence_async_smem();
+      asm volatile("bar.sync 1, 128;" ::: "memory");       // P complete; red / s_m free for the next tile
+      if (threadIdx.x == 0) mbar_arrive(&p_full);
+    } else {
+      // ---- WG1: the K slots are free once P(it) is published; then the rescale WG0 decided for this tile ----
+      mbar_wait(&p_full, ph);
+      if (more && threadIdx.x == 128) load_chunks(&map_k, &map_v, s_ring, full_b, 0, kKC, next_row, pol_kv);
+      float al[16];
+      bool need = false;
+#pragma unroll
+      for (int x = 0; x < 16; ++x) {
+        al[x] = s_alpha[8 * (x >> 1) + qd + (x & 1)];
+        need |= al[x] != 1.f;
+      }
+      if (need) {
+#pragma unroll
+        for (int x = 0; x < 16; ++x) {
+          const int e = 4 * (x >> 1) + (x & 1);
+#pragma unroll
+          for (int m = 0; m < 4; ++m) { o[m][e] *= al[x]; o[m][e + 2] *= al[x]; }
+        }
+      }
+    }
+    // ---- O^T += V^T . P^T over this warpgroup's 4 V chunks, each a 64-dim M tile read MN-major ----
+    wgmma_fence();
+#pragma unroll
+    for (int m = 0; m < 4; ++m) {
+      const int c = kKC + vc0 + m;
+      mbar_wait(&full_b[c], ph);
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks)                        // 16 keys = two 8-row groups of the chunk
+        WgmmaN<64>::bf16<1>(o[m], make_sw128_desc(ring_a + c * kSlot + ks * 2048, kSlot, 1024),
+                            make_sw128_desc(p_a + 32 * ks, 16, 1024), 1);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    if (!wg0 && lane == 0) mbar_arrive(&p_empty);
+    if (more) {                                             // this warpgroup's V slots are free: load tile it + 1's
+      if (wg0) asm volatile("bar.sync 1, 128;" ::: "memory");
+      else asm volatile("bar.sync 3, 128;" ::: "memory");
+      if ((threadIdx.x & 127) == 0) load_chunks(&map_k, &map_v, s_ring, full_b, kKC + vc0, kKC + vc0 + 4, next_row, pol_kv);
+    }
+  }
+
+  // ---- epilogue: row sums (WG0), O^T / l -> bf16 staged in the Q buffer -> 16-byte coalesced stores ----
+  if (wg0) {
+#pragma unroll
+    for (int x = 0; x < 16; ++x) {
+      const float ls = rows_sum(l_part[x]);
+      if (lane < 4) red[warp][8 * (x >> 1) + qd + (x & 1)] = ls;
+    }
+    asm volatile("bar.sync 1, 128;" ::: "memory");
+    if (threadIdx.x < kRows) {
+      const int r = threadIdx.x;
+      const float l = (red[0][r] + red[1][r]) + (red[2][r] + red[3][r]);
+      s_inv[r] = l > 0.f ? 1.f / l : 0.f;
+    }
+  }
+  __syncthreads();                                          // s_inv ready; Q no longer read by any wgmma
+#pragma unroll
+  for (int x = 0; x < 16; ++x) {
+    const int r = 8 * (x >> 1) + qd + (x & 1);
+    const float inv = s_inv[r];
+    const int e = 4 * (x >> 1) + (x & 1);
+#pragma unroll
+    for (int m = 0; m < 4; ++m) {
+      uint8_t* dst = s_q + r * kOutPitch + (64 * (vc0 + m) + krow) * 2;
+      *reinterpret_cast<__nv_bfloat16*>(dst) = __float2bfloat16_rn(o[m][e] * inv);
+      *reinterpret_cast<__nv_bfloat16*>(dst + 16) = __float2bfloat16_rn(o[m][e + 2] * inv);
+    }
+  }
+  __syncthreads();
+  __nv_bfloat16* orow = out + ((int64_t)q0 * H + r0) * kC;
+  for (int u = threadIdx.x; u < kRows * (kC / 8); u += kThreads) {
+    const int r = u / (kC / 8), cu = u % (kC / 8);
+    if (r0 + r <= rlast)
+      *reinterpret_cast<uint4*>(orow + (int64_t)r * kC + cu * 8) = *reinterpret_cast<const uint4*>(s_q + r * kOutPitch + cu * 16);
+  }
+}
+
+}  // namespace
+}  // namespace cb
+
+// flash_attn_varlen_func for absorbed MLA (include/chitu_b200.h).
+extern "C" int chitu_b200_mla_prefill(const void* q, const void* k, int64_t k_sb, const void* v, int64_t v_sb,
+                                      const int32_t* cu_seqlens_q, const int32_t* cu_seqlens_k, int B, int H,
+                                      int total_q, int total_k, int max_seqlen_q, int causal, float softmax_scale,
+                                      void* out, void* stream) {
+  using namespace cb;
+  CB_ARG(q && k && v && cu_seqlens_q && cu_seqlens_k && out);
+  CB_ARG(B >= 0 && H >= 1 && max_seqlen_q >= 0 && total_q >= 0 && total_k >= 0);
+  CB_ARG(k_sb >= kRow && v_sb >= kC && k_sb % 8 == 0 && v_sb % 8 == 0);          // TMA: 16-byte row strides
+  CB_ARG(((uintptr_t)q | (uintptr_t)k | (uintptr_t)v | (uintptr_t)out) % 16 == 0); // TMA / vector stores: 16-byte bases
+  CB_ARG((int64_t)total_q * H <= INT_MAX && (int64_t)max_seqlen_q * H <= INT_MAX - kRows);   // int32 TMA row coordinates
+  if (B == 0 || total_q == 0 || max_seqlen_q == 0) return 0;
+  const int row_tiles = cdiv((int64_t)max_seqlen_q * H, kRows);
+  if ((int64_t)row_tiles * B > INT_MAX)
+    return fail(-1, "mla_prefill: %d sequences x %d row tiles exceed the grid", B, row_tiles);
+  CUtensorMap mq, mk, mv;
+  // total_k == 0: no sequence has a key, the K / V maps are never read (one row keeps them encodable)
+  const int64_t krows = total_k > 0 ? total_k : 1;
+  int rc = make_tma_map_2d(&mq, q, (int64_t)total_q * H, kRow, 2, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, kRows);
+  if (!rc) rc = make_tma_map_2d(&mk, k, krows, kRow, 2, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, kTile, k_sb);
+  if (!rc) rc = make_tma_map_2d(&mv, v, krows, kC, 2, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, kTile, v_sb);
+  if (rc) return rc;
+  const size_t smem = 1024 + (size_t)kSmemBytes;
+  static bool attr = false;
+  if (!attr) {
+    CB_CUDA(cudaFuncSetAttribute(mla_prefill_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    attr = true;
+  }
+  launch_k(mla_prefill_kernel, dim3(row_tiles * B), dim3(kThreads), smem, (cudaStream_t)stream, mq, mk, mv, cu_seqlens_q,
+           cu_seqlens_k, B, H, row_tiles, causal ? 1 : 0, softmax_scale, (__nv_bfloat16*)out);
+  CB_LAUNCHED(1);
+  return 0;
+}
+
+CB_DEFINE_TL_SETTER(mla_prefill)

@@ -40,11 +40,6 @@ constexpr float kLog2e = 1.4426950408889634f;
 constexpr float kRescaleThreshold = 8.f;       // log2 domain
 constexpr int kThreads = 160;                  // warpgroup (warps 0-3) + producer warp
 
-__device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-
-// byte offset of the 16-byte unit `unit` of row `row` in a [rows x 128 B] 128B-swizzled tile
-__device__ __forceinline__ uint32_t sw128(int row, int unit) { return (uint32_t)(row * 128 + ((unit ^ (row & 7)) << 4)); }
-
 // dev tool (profiling build only, -DCB_TIMELINE): %globaltimer at fixed points of every CTA, 32 slots per CTA, read by
 // scripts/mla_probe.py.  The product library compiles these to nothing.
 #ifdef CB_TIMELINE
@@ -61,17 +56,6 @@ __device__ __forceinline__ void probe(int idx) {
 __device__ __forceinline__ void probe(int) {}
 #endif
 
-// max / sum over the 8 lanes that share lane % 4 (the key rows of one wgmma fragment column)
-__device__ __forceinline__ float rows_max(float v) {
-  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 4));
-  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 8));
-  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 16));
-}
-__device__ __forceinline__ float rows_sum(float v) {
-  v += __shfl_xor_sync(0xffffffffu, v, 4);
-  v += __shfl_xor_sync(0xffffffffu, v, 8);
-  return v + __shfl_xor_sync(0xffffffffu, v, 16);
-}
 // value h of a 16-entry register array without dynamic register indexing
 __device__ __forceinline__ float pick16(const float (&v)[16], int h) {
   float r = v[0];

@@ -8,6 +8,24 @@ namespace cb {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
+// make generic-proxy shared-memory stores visible to the async proxy (wgmma operands, TMA)
+__device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
+// byte offset of the 16-byte unit `unit` of row `row` in a [rows x 128 B] 128B-swizzled tile
+__device__ __forceinline__ uint32_t sw128(int row, int unit) { return (uint32_t)(row * 128 + ((unit ^ (row & 7)) << 4)); }
+
+// max / sum over the 8 lanes that share lane % 4 (the M rows of one wgmma fragment column within a warp)
+__device__ __forceinline__ float rows_max(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 4));
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 8));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 16));
+}
+__device__ __forceinline__ float rows_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 4);
+  v += __shfl_xor_sync(0xffffffffu, v, 8);
+  return v + __shfl_xor_sync(0xffffffffu, v, 16);
+}
+
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile(
@@ -74,9 +92,10 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
 
 
 // 2-D row-major [rows, cols] tensor of `elem_bytes` elements, box = [box_rows, 128 bytes], 128B swizzle,
-// zero fill outside the tensor (host side; the driver entry point is resolved at run time).
+// zero fill outside the tensor (host side; the driver entry point is resolved at run time).  row_stride: elements
+// between rows (0 = dense, cols); a multiple of 16 bytes.
 int make_tma_map_2d(CUtensorMap* map, const void* base, int64_t rows, int64_t cols, int elem_bytes,
-                    CUtensorMapDataType dt, int box_rows);
+                    CUtensorMapDataType dt, int box_rows, int64_t row_stride = 0);
 bool tma_available();
 
 }  // namespace cb

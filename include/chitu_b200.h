@@ -223,6 +223,19 @@ int chitu_b200_mla_decode(const void* q_nope, const void* q_pe, void* kv_cache, 
                           float softmax_scale, void* out, void* workspace, int64_t workspace_bytes,
                           void* stream);
 
+/* FlashAttnBackend.attn_varlen_func (attn_backend.py:193-206) for the absorbed-MLA prefill of DeepSeek
+ * (model_deepseek_v3.py:588-602), with flash_attn_varlen_func semantics: q [total_q, H, 576] contiguous,
+ * k [total_k, 576] (row stride k_sb elements), v [total_k, 512] (row stride v_sb), one KV head shared by the H query
+ * heads; out [total_q, H, 512] contiguous.  bf16; fp32 scores and softmax, P rounded to bf16 before P.V.
+ * cu_seqlens_q / cu_seqlens_k: int32 [B + 1] on the device (zero-length sequences allowed); max_seqlen_q (host) sizes
+ * the grid.  causal != 0: bottom-right aligned mask (query i sees keys j <= i + Lk - Lq); a row that sees no key is 0.
+ * No host synchronisation, no workspace (capturable in a CUDA graph); deterministic (no split over keys).
+ * Bases 16-byte aligned, k_sb / v_sb multiples of 8; total_q * H must fit int32. */
+int chitu_b200_mla_prefill(const void* q, const void* k, int64_t k_sb, const void* v, int64_t v_sb,
+                           const int32_t* cu_seqlens_q, const int32_t* cu_seqlens_k, int B, int H,
+                           int total_q, int total_k, int max_seqlen_q, int causal, float softmax_scale,
+                           void* out, void* stream);
+
 /* invoke_fused_moe_kernel (fused_moe.py:796-891; Triton kernel :62-307) as ONE grouped wgmma GEMM:
  * A bf16 [numel/top_k (GEMM1) or numel (top_k = 1), K]; B stacked expert weights [E, N, K] (bf16 for wmode 0, fp8 +
  * B_scale [E, N/128, K/128] for wmode 1 = fp8_w8a8 — A is quantised per_token_group_quant_fp8 inside, as the reference
