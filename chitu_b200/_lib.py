@@ -33,7 +33,6 @@ SIGNATURES = {
     "chitu_b200_moe_align_block_size": (I, [P, I, L, I, I, P, P, P, P, P]),
     "chitu_b200_moe_gate_workspace_bytes": (L, [I, I]),
     "chitu_b200_moe_gate": (I, [P, P, P, I, I, I, I, I, I, I, I, F, P, P, I, P, L, P]),
-    "chitu_b200_moe_gate_plan": (I, [P, P, P, I, I, I, I, I, I, I, I, F, P, P, I, P, L, I, I, I, P, L, P]),
     "chitu_b200_rotary_interleaved": (I, [P, P, P, P, P, P, I, I, I, I, L, L, L, L, I, P]),
     "chitu_b200_rotary_interleaved_strided": (I, [P, P, P, P, P, P, I, I, I, I, L, L, L, L, L, L, I, P]),
     "chitu_b200_rotary_half": (I, [P, P, P, P, I, I, I, I, P]),
@@ -69,7 +68,6 @@ SIGNATURES = {
     "chitu_b200_mla_prep": (I, [P, P, L, P, P, P, P, P, P, P, I, I, I, I, I, I, F, P]),
     "chitu_b200_moe_workspace_bytes": (L, [I, I, I, I, I]),
     "chitu_b200_fused_experts": (I, [P, P, P, P, P, P, I, P, I, I, I, I, I, I, I, P, P, P, L, P]),
-    "chitu_b200_fused_experts_planned": (I, [P, P, P, P, P, P, I, P, I, I, I, I, I, I, I, P, P, P, L, P]),
     "chitu_b200_moe_grouped_gemm_workspace_bytes": (L, [I, I, I]),
     "chitu_b200_moe_grouped_gemm": (I, [P, P, P, P, P, I, P, P, P, I, I, I, I, I, I, I, I, I, P, L, P]),
     "chitu_b200_comm_create": (I, [I, I, L, P, P]),
@@ -78,7 +76,7 @@ SIGNATURES = {
     "chitu_b200_comm_status": (I, [P]),
     "chitu_b200_fp8_gemm_ar": (I, [P, P, P, P, I, I, I, P, P, L, P]),
     "chitu_b200_linear_bf16_ar": (I, [P, P, I, I, I, P, P, L, P]),
-    "chitu_b200_fused_experts_ar": (I, [P, P, P, P, P, P, I, P, I, I, I, I, I, I, I, P, P, L, I, P]),
+    "chitu_b200_fused_experts_ar": (I, [P, P, P, P, P, P, I, P, I, I, I, I, I, I, I, P, P, L, P]),
     "chitu_b200_allreduce_consume": (I, [P, P, P, P, P, P, P, I, I, F, P]),
     "chitu_b200_allreduce_residual_rmsnorm": (I, [P, P, P, P, P, P, P, P, I, I, F, P]),
     "chitu_b200_sample_top_k_top_p": (I, [P, L, I, I, I, P, P, P, P, P, P, P, P]),

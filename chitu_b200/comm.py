@@ -50,11 +50,11 @@ class FusedAllReduce:
         check(self.lib.chitu_b200_linear_bf16_ar(ptr(x), ptr(w), M, N, K, self.handle, ptr(lin_ws), lin_ws.numel(),
                                                  current_stream()), "linear_bf16_ar")
 
-    def experts_push(self, x, w1, w2, w1_s, w2_s, topk_w, topk_w_code, topk_ids, ids_code, T, topk, E, N1, K1, wmode, moe_ws,
-                     planned: int = 0) -> None:
+    def experts_push(self, x, w1, w2, w1_s, w2_s, topk_w, topk_w_code, topk_ids, ids_code, T, topk, E, N1, K1, wmode,
+                     moe_ws) -> None:
         check(self.lib.chitu_b200_fused_experts_ar(ptr(x), ptr(w1), ptr(w2), ptr(w1_s), ptr(w2_s), ptr(topk_w), topk_w_code,
                                                    ptr(topk_ids), ids_code, T, topk, E, N1, K1, wmode, self.handle, ptr(moe_ws),
-                                                   moe_ws.numel(), int(planned), current_stream()), "fused_experts_ar")
+                                                   moe_ws.numel(), current_stream()), "fused_experts_ar")
 
     def consume(self, residual, h_out, norm_w, y, q, q_scales, rows, dim, eps):
         """reduce the partials every rank pushed (same outputs as __call__)"""

@@ -47,7 +47,6 @@ static inline int cdiv(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
 // tensormap prefetch overlap this kernel's tail), `griddepcontrol.wait` blocks until
 // the PREVIOUS kernel has completed and flushed — so no kernel touches global memory before its
 // predecessor is done.  Inside CUDA graphs this becomes a programmatic dependency edge.
-bool pdl_enabled();
 
 // ---- in-graph timeline (dev tool, off by default) --------------------------------------------------------------
 // chitu_b200_debug_timeline(buf, capacity) arms a device buffer; every kernel then records %globaltimer when the LAST
@@ -98,7 +97,7 @@ inline cudaError_t launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, siz
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
+  cfg.numAttrs = 1;
   return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
 }
 #endif

@@ -1,5 +1,4 @@
 // Error plumbing + the integer / bit-exact operators: paged-KV append, MoE align.
-#include <stdlib.h>
 #include <string.h>
 
 #include "common.cuh"
@@ -33,14 +32,6 @@ void tl_log_launch(const char* entry, int n) {
     g_tl_names[g_tl_len++] = '\n';
     g_tl_names[g_tl_len] = 0;
   }
-}
-bool pdl_enabled() {
-  static int on = -1;
-  if (on < 0) {
-    const char* e = getenv("CHITU_B200_PDL");
-    on = (e && e[0] == '0') ? 0 : 1;
-  }
-  return on != 0;
 }
 
 }  // namespace cb

@@ -104,8 +104,7 @@ extern "C" int chitu_b200_rotary_interleaved_strided(const void* q, const void* 
   cudaStream_t st = (cudaStream_t)stream;
   int total = (hq + hk) * rot_dim / 2;
   // 16-byte path: a thread rotates 4 pairs (one uint4 of 2-byte elements); needs 16 B aligned rows
-  static const bool force_scalar = getenv("CHITU_B200_ROTARY_SCALAR") != nullptr;
-  const bool vec_ok = !force_scalar && (dtype == CB_BF16 || dtype == CB_F16) && rot_dim % 8 == 0 &&
+  const bool vec_ok = (dtype == CB_BF16 || dtype == CB_F16) && rot_dim % 8 == 0 &&
                       q_sb % 8 == 0 && q_sh % 8 == 0 && k_sb % 8 == 0 && k_sh % 8 == 0 && oq_sb % 8 == 0 &&
                       ok_sb % 8 == 0 && aligned16(q) && aligned16(k) && aligned16(out_q) && aligned16(out_k) &&
                       aligned16(cos) && aligned16(sin);

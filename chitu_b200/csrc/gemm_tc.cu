@@ -23,8 +23,6 @@
 //   kind 2: w8a8gemm.mm / w8a8gemv.mv (quantize/w8a8.py:105,120,125)
 #include <cuda.h>
 
-#include <stdlib.h>
-
 #include <mutex>
 #include <type_traits>
 
@@ -61,7 +59,6 @@ struct Params {
   int per;                  // stages per CTA (dense mode; grouped mode derives it on the device)
   int kblocks;              // fp8: ceil(K/128) (scale columns)
   int out_dtype;            // CB_BF16 | CB_F16
-  int prefetch;             // dense mode: stream weight tiles before griddepcontrol.wait (A/B: CHITU_B200_GEMM_PREFETCH=0)
   int act_pairs;            // kind 0: weight rows (2i, 2i+1) = (gate_i, up_i); out[m, i] = SiluAndMul -> [M, N/2]
   int has_push;             // row-parallel linear of a tensor-parallel layer: the bf16 result is stored into every rank's
   PushDev push;             // push area instead of `out`, as epoch-tagged words (comm.cu allreduce_consume_kernel)
@@ -222,7 +219,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
     if (elect_one()) {
       const uint64_t pol_w = l2_policy_evict_first(), pol_x = l2_policy_evict_last();
       int pre = 0;                                  // stages whose weight tile was issued before griddepcontrol.wait
-      if (!grouped && p.prefetch) {
+      if (!grouped) {
         int it = 0;
         for (ItemIter ii(g_begin, g_end, S); ii.valid() && it < C::kStages; ii.next()) {
           const WorkItem w = ii.item();
@@ -664,8 +661,6 @@ int dispatch_bn(int BN, const CUtensorMap& mw, const CUtensorMap& mx, Params& p,
 
 int run(int kind, const void* x, const void* w, Params& p, int elem, CUtensorMapDataType dt, void* ws, int64_t ws_bytes,
         cudaStream_t st, int x_elem = 0, CUtensorMapDataType x_dt = CU_TENSOR_MAP_DATA_TYPE_UINT8) {
-  static const int prefetch_env = getenv("CHITU_B200_GEMM_PREFETCH") ? atoi(getenv("CHITU_B200_GEMM_PREFETCH")) : 1;
-  p.prefetch = prefetch_env;
   const int BN = pick_bn(p.M);
   p.n_tiles = cdiv(p.N, kTileN);
   p.m_chunks = cdiv(p.M, BN);

@@ -8,7 +8,6 @@
 //                     per expert, so each (token, slot) pair streams its expert's weight rows once:
 //                     a batched weight-streaming GEMV (the grouped wgmma path lives in
 //                     gemm_tc.cu and is selected for larger token counts per expert).
-#include <stdlib.h>
 #include <string.h>
 
 #include "common.cuh"
@@ -51,15 +50,15 @@ __device__ __forceinline__ void mprobe(int idx) {
 __device__ __forceinline__ void mprobe(int) {}
 #endif
 
-// The plan itself, for a CTA of NT threads (1024: the stand-alone kernel; 256: the last CTA of the gate kernel).  `sm` needs
-// moe_plan_smem_ints(P, E) ints.  A thread owns EPT = 1024 / NT consecutive experts in the block-wide scans.  ids / topk_w
-// are read with plain (coherent) loads: in the gate kernel they were written by other CTAs of the same grid.
+// The plan itself, run by one CTA of kPlanThreads threads.  `sm` needs moe_plan_smem_ints(P, E) ints.  E <= kPlanThreads:
+// a thread owns one expert in the block-wide scans.
+constexpr int kPlanThreads = 1024;
 __host__ __device__ inline int64_t moe_plan_smem_ints(int64_t P, int E) { return 3 * (int64_t)E + 2 + 2 * P + 2 * (E + P / 16 + 2); }
 
-template <typename IdT, int NT>
+template <typename IdT>
 __device__ __forceinline__ void moe_plan_large(const IdT* ids, const void* topk_w, int topk_w_f32,
                                                int P, int E, int N1, int K1, int BN, const MoePlan& pl, int* sm) {
-  constexpr int EPT = 1024 / NT, NW = NT / 32;
+  constexpr int NT = kPlanThreads, NW = NT / 32;
   int* cnt = sm;              // [E]
   int* start = sm + E;        // [E+1]
   int* act = start + E + 1;   // [E] first row chunk (of BN sorted rows) of the expert among all chunks
@@ -86,16 +85,8 @@ __device__ __forceinline__ void moe_plan_large(const IdT* ids, const void* topk_
   // block-wide exclusive scan of cnt[] and of the row-chunk counts (E <= 1024).  An expert with more than BN routed rows
   // (bs > 128, or the shared expert that every token visits) is cut into chunks of BN rows: each chunk is a tile column
   // of the grouped GEMM (its weight tile is re-read per chunk, mostly from L2).
-  int c[EPT], ch[EPT], csum = 0, asum = 0;
-#pragma unroll
-  for (int i = 0; i < EPT; ++i) {
-    const int e = tid * EPT + i;
-    c[i] = e < E ? cnt[e] : 0;
-    ch[i] = (c[i] + BN - 1) / BN;
-    csum += c[i];
-    asum += ch[i];
-  }
-  int ci = csum, ai = asum;
+  const int c = tid < E ? cnt[tid] : 0, ch = (c + BN - 1) / BN;
+  int ci = c, ai = ch;
 #pragma unroll
   for (int o = 1; o < 32; o <<= 1) {
     const int n1 = __shfl_up_sync(0xffffffffu, ci, o), n2 = __shfl_up_sync(0xffffffffu, ai, o);
@@ -109,17 +100,11 @@ __device__ __forceinline__ void moe_plan_large(const IdT* ids, const void* topk_
     na += s_wact[w];
     tot += s_wsum[w];
   }
-  int run_c = woff + ci - csum, run_a = aoff + ai - asum;      // exclusive prefixes of this thread's first expert
-#pragma unroll
-  for (int i = 0; i < EPT; ++i) {
-    const int e = tid * EPT + i;
-    if (e < E) {
-      start[e] = run_c;
-      act[e] = ch[i] ? run_a : -1;
-      pl.seg_start[e] = run_c;
-    }
-    run_c += c[i];
-    run_a += ch[i];
+  const int run_c = woff + ci - c, run_a = aoff + ai - ch;    // exclusive prefixes of this thread's expert
+  if (tid < E) {
+    start[tid] = run_c;
+    act[tid] = ch ? run_a : -1;
+    pl.seg_start[tid] = run_c;
   }
   if (tid == 0) {
     pl.seg_start[E] = tot;    // pairs with absent experts excluded
@@ -173,10 +158,10 @@ __device__ __forceinline__ void moe_plan_large(const IdT* ids, const void* topk_
 // per expert.  In-graph probes of the per-expert version at bs = 16 (144 pairs, ~100 active experts): 1.0 us staging, 1.9 us
 // scan, 4.6 - 7 us scatter + tile lists = 10 us after the dependency wait; the same
 // stable order (pairs of an expert keep their pair-index order), so every output array is identical.
-template <typename IdT, int NT>
+template <typename IdT>
 __device__ __forceinline__ void moe_plan_small(const IdT* ids, const void* topk_w, int topk_w_f32,
                                                int P, int E, int N1, int K1, int BN, const MoePlan& pl, int* sm) {
-  constexpr int EPT = 1024 / NT, NW = NT / 32, PPT = 1024 / NT;
+  constexpr int NT = kPlanThreads, NW = NT / 32;
   int* cnt = sm;              // [E]
   int* start = sm + E;        // [E+1]
   int* act = start + E + 1;   // [E] first row chunk of the expert among all chunks, -1 = no rows
@@ -194,37 +179,25 @@ __device__ __forceinline__ void moe_plan_small(const IdT* ids, const void* topk_
   }
   __syncthreads();
   mprobe(2);
-  // histogram + the pair's rank among the earlier pairs of the same expert (stable order), one pass over shared memory
-  int my_rank[PPT];
-#pragma unroll
-  for (int k = 0; k < PPT; ++k) {
-    const int p = tid + k * NT;
-    my_rank[k] = -1;
-    if (p < P) {
-      const int e = sid[p];
-      if (e >= 0 && e < E) {
-        atomicAdd(&cnt[e], 1);
-        int r = 0;
-        for (int q = 0; q < p; ++q) r += (sid[q] == e);
-        my_rank[k] = r;
-      } else {
-        pl.pos[p] = -1;       // expert not on this rank (expert_map == -1)
-      }
+  // histogram + the pair's rank among the earlier pairs of the same expert (stable order), one pass over shared memory;
+  // thread p owns pair p
+  int my_rank = -1;
+  if (tid < P) {
+    const int e = sid[tid];
+    if (e >= 0 && e < E) {
+      atomicAdd(&cnt[e], 1);
+      int r = 0;
+      for (int q = 0; q < tid; ++q) r += (sid[q] == e);
+      my_rank = r;
+    } else {
+      pl.pos[tid] = -1;       // expert not on this rank (expert_map == -1)
     }
   }
   __syncthreads();
   mprobe(3);
   // block-wide exclusive scan of the counts and of the row-chunk counts (E <= 1024)
-  int c[EPT], ch[EPT], csum = 0, asum = 0;
-#pragma unroll
-  for (int i = 0; i < EPT; ++i) {
-    const int e = tid * EPT + i;
-    c[i] = e < E ? cnt[e] : 0;
-    ch[i] = (c[i] + BN - 1) / BN;
-    csum += c[i];
-    asum += ch[i];
-  }
-  int ci = csum, ai = asum;
+  const int c = tid < E ? cnt[tid] : 0, ch = (c + BN - 1) / BN;
+  int ci = c, ai = ch;
 #pragma unroll
   for (int o = 1; o < 32; o <<= 1) {
     const int n1 = __shfl_up_sync(0xffffffffu, ci, o), n2 = __shfl_up_sync(0xffffffffu, ai, o);
@@ -242,19 +215,13 @@ __device__ __forceinline__ void moe_plan_small(const IdT* ids, const void* topk_
   }
   const int tot = __shfl_sync(0xffffffffu, wi, 31), na = __shfl_sync(0xffffffffu, aii, 31);
   const int woff = __shfl_sync(0xffffffffu, wi - wt, warp), aoff = __shfl_sync(0xffffffffu, aii - at, warp);
-  int run_c = woff + ci - csum, run_a = aoff + ai - asum;      // exclusive prefixes of this thread's first expert
-#pragma unroll
-  for (int i = 0; i < EPT; ++i) {
-    const int e = tid * EPT + i;
-    if (e < E) {
-      start[e] = run_c;
-      act[e] = ch[i] ? run_a : -1;
-      pl.seg_start[e] = run_c;
+  const int run_c = woff + ci - c, run_a = aoff + ai - ch;    // exclusive prefixes of this thread's expert
+  if (tid < E) {
+    start[tid] = run_c;
+    act[tid] = ch ? run_a : -1;
+    pl.seg_start[tid] = run_c;
 #pragma unroll 1
-      for (int cc = 0; cc < ch[i]; ++cc) { chunk_e[run_a + cc] = e; chunk_c[run_a + cc] = cc; }
-    }
-    run_c += c[i];
-    run_a += ch[i];
+    for (int cc = 0; cc < ch; ++cc) { chunk_e[run_a + cc] = tid; chunk_c[run_a + cc] = cc; }
   }
   if (tid == 0) {
     pl.seg_start[E] = tot;    // pairs with absent experts excluded
@@ -264,15 +231,11 @@ __device__ __forceinline__ void moe_plan_small(const IdT* ids, const void* topk_
   __syncthreads();
   mprobe(4);
   // one thread per pair: its sorted row
-#pragma unroll
-  for (int k = 0; k < PPT; ++k) {
-    const int p = tid + k * NT;
-    if (my_rank[k] >= 0) {
-      const int rr = start[sid[p]] + my_rank[k];
-      pl.pair_sorted[rr] = p;
-      pl.pos[p] = rr;
-      pl.w_sorted[rr] = swt[p];
-    }
+  if (my_rank >= 0) {
+    const int rr = start[sid[tid]] + my_rank;
+    pl.pair_sorted[rr] = tid;
+    pl.pos[tid] = rr;
+    pl.w_sorted[rr] = swt[tid];
   }
   mprobe(5);
   // one thread per tile-list entry of either GEMM
@@ -298,21 +261,6 @@ __device__ __forceinline__ void moe_plan_small(const IdT* ids, const void* topk_
   mprobe(6);
 #endif
 }
-
-template <typename IdT, int NT>
-__device__ __forceinline__ void moe_plan_body(const IdT* ids, const void* topk_w, int topk_w_f32,
-                                              int P, int E, int N1, int K1, int BN, const MoePlan& pl, int* sm) {
-  if (P <= 1024) moe_plan_small<IdT, NT>(ids, topk_w, topk_w_f32, P, E, N1, K1, BN, pl, sm);
-  else moe_plan_large<IdT, NT>(ids, topk_w, topk_w_f32, P, E, N1, K1, BN, pl, sm);
-}
-
-// gate + plan in one launch: the gate kernel's CTAs (one per token) take a ticket when their routing row is written; the
-// LAST one runs the plan over all rows (ids int64 [T, stride] with the shared-expert column pre-filled by the engine).
-struct GatePlanArgs {
-  int enabled, P, E, N1, K1, BN;
-  int* ticket;                // zero on entry, zero on exit
-  MoePlan pl;
-};
 
 // --------------------------------------------------------------------------------------------
 // gate: one CTA (256 threads) per token.
@@ -411,7 +359,7 @@ __global__ void __launch_bounds__(256) moe_gate_kernel(
     const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ w, const void* __restrict__ bias,
     int bias_is_f32, int dim, int E, int n_groups, int topk_groups, int topk, int score_sigmoid,
     float route_scale, __nv_bfloat16* __restrict__ out_w, int64_t* __restrict__ out_idx,
-    const __nv_bfloat16* __restrict__ logits, int out_stride, const GatePlanArgs gp) {
+    const __nv_bfloat16* __restrict__ logits, int out_stride) {
   cb::pdl_prologue();
   extern __shared__ __align__(16) uint8_t smem_raw[];
   __nv_bfloat16* sx = reinterpret_cast<__nv_bfloat16*>(smem_raw);                 // [dim]
@@ -595,23 +543,6 @@ __global__ void __launch_bounds__(256) moe_gate_kernel(
       out_idx[(int64_t)t * out_stride + r] = s_sel[r];
     }
   }
-  if (gp.enabled) {
-    // the last CTA to finish its routing row builds the expert plan of the whole batch (one launch fewer; the plan no
-    // longer waits for a kernel boundary after the slowest gate CTA)
-    __shared__ int s_last;
-    __threadfence();
-    __syncthreads();
-    if (tid == 0) {
-      const int prev = atomicAdd(gp.ticket, 1);
-      s_last = prev == (int)gridDim.x - 1;
-      if (s_last) *gp.ticket = 0;
-    }
-    __syncthreads();
-    if (s_last) {
-      __threadfence();
-      moe_plan_body<int64_t, 256>(out_idx, out_w, 0, gp.P, gp.E, gp.N1, gp.K1, gp.BN, gp.pl, reinterpret_cast<int*>(smem_raw));
-    }
-  }
 }
 
 // --------------------------------------------------------------------------------------------
@@ -748,13 +679,14 @@ __global__ void moe_sum_kernel(const __nv_bfloat16* __restrict__ c3, __nv_bfloat
 //   moe_combine_kernel       out[t] = sum_j c3[pos[t*topk+j]]  (fp32 sum, one rounding)
 // --------------------------------------------------------------------------------------------
 template <typename IdT>
-__global__ void __launch_bounds__(1024) moe_plan_kernel(const IdT* __restrict__ ids, const void* __restrict__ topk_w,
-                                                       int topk_w_f32, int P, int E, int N1, int K1, int BN, MoePlan pl) {
+__global__ void __launch_bounds__(kPlanThreads) moe_plan_kernel(const IdT* __restrict__ ids, const void* __restrict__ topk_w,
+                                                               int topk_w_f32, int P, int E, int N1, int K1, int BN, MoePlan pl) {
   mprobe(0);
   cb::pdl_prologue();
   mprobe(1);
   extern __shared__ int sm[];
-  moe_plan_body<IdT, 1024>(ids, topk_w, topk_w_f32, P, E, N1, K1, BN, pl, sm);
+  if (P <= kPlanThreads) moe_plan_small<IdT>(ids, topk_w, topk_w_f32, P, E, N1, K1, BN, pl, sm);
+  else moe_plan_large<IdT>(ids, topk_w, topk_w_f32, P, E, N1, K1, BN, pl, sm);
   mprobe(7);
 }
 
@@ -788,84 +720,6 @@ __global__ void moe_gather_quant_kernel(const __nv_bfloat16* __restrict__ x, con
   }
   *reinterpret_cast<uint32_t*>(xq + (int64_t)r * K + gk * 128 + lane * 4) = packed;
   if (lane == 0) xs[(int64_t)r * groups + gk] = sc;
-}
-
-// Plan + gather in ONE launch for decode-sized batches (P <= 1024 pairs): CTA p finds the sorted row of pair p by itself —
-// histogram of all pairs in shared memory, then (sum of the counts of lower experts) + (earlier pairs of the same
-// expert), one block reduction — and gathers / quantises its token's row there; CTA 0 then also writes the plan arrays the
-// two grouped GEMMs and the combine read (moe_plan_small).  One dependent stage fewer per MoE layer — and measured slower
-// than the separate plan + gather launches (see the launch site), so it is an opt-in experiment.
-template <typename IdT>
-__global__ void __launch_bounds__(256) moe_plan_gather_kernel(const IdT* __restrict__ ids, const void* __restrict__ topk_w,
-                                                             int topk_w_f32, int P, int E, int N1, int K1, int BN, MoePlan pl,
-                                                             const __nv_bfloat16* __restrict__ x, int topk, int quant,
-                                                             uint8_t* __restrict__ xq, float* __restrict__ xs,
-                                                             __nv_bfloat16* __restrict__ xb) {
-  cb::pdl_prologue();
-  extern __shared__ int sm[];
-  int* cnt = sm;                                   // [E]   (same prefix of the layout as moe_plan_small)
-  int* sid = sm + 3 * E + 1;                       // [P]
-  __shared__ int s_red[2][8];
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int p = blockIdx.x;
-  for (int e = tid; e < E; e += 256) cnt[e] = 0;
-  for (int q = tid; q < P; q += 256) sid[q] = (int)ids[q];
-  __syncthreads();
-  for (int q = tid; q < P; q += 256) {
-    const int e = sid[q];
-    if (e >= 0 && e < E) atomicAdd(&cnt[e], 1);
-  }
-  __syncthreads();
-  const int e = sid[p];
-  if (e >= 0 && e < E) {                           // uniform over the CTA
-    int below = 0, rank = 0;
-    for (int ee = tid; ee < e; ee += 256) below += cnt[ee];
-    for (int q = tid; q < p; q += 256) rank += (sid[q] == e);
-    below = (int)warp_sum((float)below);           // counts <= 1024: exact in fp32
-    rank = (int)warp_sum((float)rank);
-    if (lane == 0) { s_red[0][warp] = below; s_red[1][warp] = rank; }
-    __syncthreads();
-    int r = 0;
-#pragma unroll
-    for (int w = 0; w < 8; ++w) r += s_red[0][w] + s_red[1][w];
-    // gather (+ per_token_group_quant_fp8) of token p / topk into sorted row r: one warp per 128-group, loads first
-    const int groups = K1 / 128;
-    const __nv_bfloat16* src = x + (int64_t)(p / topk) * K1;
-    constexpr int kG = 8;                           // groups in flight per warp
-    for (int g0 = warp; g0 < groups; g0 += 8 * kG) {
-      uint2 raw[kG];
-#pragma unroll
-      for (int u = 0; u < kG; ++u) {
-        const int gk = g0 + u * 8;
-        raw[u] = gk < groups ? *reinterpret_cast<const uint2*>(src + gk * 128 + lane * 4) : make_uint2(0, 0);
-      }
-#pragma unroll
-      for (int u = 0; u < kG; ++u) {
-        const int gk = g0 + u * 8;
-        if (gk >= groups) break;
-        if (!quant) {
-          *reinterpret_cast<uint2*>(xb + (int64_t)r * K1 + gk * 128 + lane * 4) = raw[u];
-          continue;
-        }
-        float v[4] = {bf16lo(raw[u].x), bf16hi(raw[u].x), bf16lo(raw[u].y), bf16hi(raw[u].y)};
-        float amax = fmaxf(fmaxf(fabsf(v[0]), fabsf(v[1])), fmaxf(fabsf(v[2]), fabsf(v[3])));
-        amax = fmaxf(warp_max(amax), 1e-10f);
-        const float sc = __fdiv_rn(amax, 448.0f);
-        uint32_t packed = 0;
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          float qv = fminf(fmaxf(__fdiv_rn(v[i], sc), -448.f), 448.f);
-          packed |= (uint32_t)float_to_fp8(qv) << (8 * i);
-        }
-        *reinterpret_cast<uint32_t*>(xq + (int64_t)r * K1 + gk * 128 + lane * 4) = packed;
-        if (lane == 0) xs[(int64_t)r * groups + gk] = sc;
-      }
-    }
-  }
-  if (blockIdx.x == 0) {
-    __syncthreads();                               // the plan rebuilds cnt / sid in the same buffer
-    moe_plan_small<IdT, 256>(ids, topk_w, topk_w_f32, P, E, N1, K1, BN, pl, sm);
-  }
 }
 
 // a2 = SiluAndMul(c1) in sorted space, then per_token_group_quant_fp8 (or bf16 copy)
@@ -958,31 +812,14 @@ int tc_grouped_gemm(int kind, const void* xs, const float* a_s, const void* w, c
 }  // namespace cb
 
 extern "C" int64_t chitu_b200_moe_gate_workspace_bytes(int T, int E) {
-  return align256(cb::tc_workspace_bytes(T, E)) + align256((int64_t)T * E * 2) + 256;   // + the gate->plan ticket
+  return align256(cb::tc_workspace_bytes(T, E)) + align256((int64_t)T * E * 2);
 }
-
-static int moe_gate_impl(const void* x, const void* w, const void* bias, int bias_dtype, int T,
-                         int dim, int E, int n_groups, int topk_groups, int topk,
-                         int score_sigmoid, float route_scale, void* out_weights,
-                         int64_t* out_indices, int out_stride, void* workspace,
-                         int64_t workspace_bytes, void* stream, GatePlanArgs gp);
 
 extern "C" int chitu_b200_moe_gate(const void* x, const void* w, const void* bias, int bias_dtype, int T,
                                    int dim, int E, int n_groups, int topk_groups, int topk,
                                    int score_sigmoid, float route_scale, void* out_weights,
                                    int64_t* out_indices, int out_stride, void* workspace,
                                    int64_t workspace_bytes, void* stream) {
-  GatePlanArgs gp;
-  memset(&gp, 0, sizeof(gp));
-  return moe_gate_impl(x, w, bias, bias_dtype, T, dim, E, n_groups, topk_groups, topk, score_sigmoid, route_scale, out_weights,
-                       out_indices, out_stride, workspace, workspace_bytes, stream, gp);
-}
-
-static int moe_gate_impl(const void* x, const void* w, const void* bias, int bias_dtype, int T,
-                         int dim, int E, int n_groups, int topk_groups, int topk,
-                         int score_sigmoid, float route_scale, void* out_weights,
-                         int64_t* out_indices, int out_stride, void* workspace,
-                         int64_t workspace_bytes, void* stream, GatePlanArgs gp) {
   CB_ARG(x && w && out_weights && out_indices && out_stride >= topk);
   CB_ARG(T >= 0 && dim > 0 && dim % 8 == 0 && E > 0 && topk > 0 && topk <= E && topk <= 32);
   CB_ARG(n_groups >= 1 && n_groups <= 64 && E % n_groups == 0 && topk_groups >= 1 && topk_groups <= n_groups);
@@ -996,8 +833,7 @@ static int moe_gate_impl(const void* x, const void* w, const void* bias, int bia
     // layout: [GEMM scratch (ticket counters first: they must stay zero between calls) | logits]
     const int64_t lin = cb::tc_workspace_bytes(T, E);
     void* lg = (uint8_t*)workspace + align256(lin);
-    static const int simt_env = getenv("CHITU_B200_GATE_LOGITS_SIMT") ? atoi(getenv("CHITU_B200_GATE_LOGITS_SIMT")) : 1;
-    if (simt_env && T <= 16 && dim <= 256 * kGateVecIters * 8) {
+    if (T <= 16 && dim <= 256 * kGateVecIters * 8) {
       // decode batches: one CTA per pair of experts, no split-K (see gate_logits_kernel)
       const dim3 grid((E + 1) / 2), block(256);
       const __nv_bfloat16* xb = (const __nv_bfloat16*)x;
@@ -1013,12 +849,7 @@ static int moe_gate_impl(const void* x, const void* w, const void* bias, int bia
     }
     logits = (const __nv_bfloat16*)lg;
   }
-  size_t smem = (size_t)dim * 2 + (size_t)(2 * E + n_groups) * 4 + (size_t)topk * 4 + 16;
-  if (gp.enabled) {
-    const size_t psm = (size_t)moe_plan_smem_ints(gp.P, gp.E) * sizeof(int);      // the last CTA reuses the buffer for the plan
-    if (psm > smem) smem = psm;
-    gp.ticket = (int*)((uint8_t*)workspace + chitu_b200_moe_gate_workspace_bytes(T, E) - 256);
-  }
+  const size_t smem = (size_t)dim * 2 + (size_t)(2 * E + n_groups) * 4 + (size_t)topk * 4 + 16;
   static size_t attr_bytes = 48 * 1024;
   if (smem > attr_bytes) {
     CB_CUDA(cudaFuncSetAttribute(moe_gate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -1026,7 +857,7 @@ static int moe_gate_impl(const void* x, const void* w, const void* bias, int bia
   }
   cb::launch_k(moe_gate_kernel, dim3(T), dim3(256), smem, st, (const __nv_bfloat16*)x, (const __nv_bfloat16*)w, bias,
                (int)(bias_dtype == CB_F32), dim, E, n_groups, topk_groups, topk, score_sigmoid, route_scale,
-               (__nv_bfloat16*)out_weights, out_indices, logits, out_stride, gp);
+               (__nv_bfloat16*)out_weights, out_indices, logits, out_stride);
   CB_LAUNCHED(1);
   return 0;
 }
@@ -1192,7 +1023,7 @@ static int fused_experts_impl(const void* x, const void* w1, const void* w2, con
                               const float* w2_s, const void* topk_w, int topk_w_dtype,
                               const void* topk_ids, int ids_dtype, int T, int topk, int E, int N1,
                               int K1, int wmode, void* out, const void* residual, void* workspace,
-                              int64_t workspace_bytes, void* stream, void* comm, int planned);
+                              int64_t workspace_bytes, void* stream, void* comm);
 
 // rows per chunk (= wgmma N of the grouped GEMMs): twice the mean number of routed rows per expert, 16 .. 128
 static int moe_chunk_rows(int64_t P, int E) {
@@ -1214,27 +1045,6 @@ static uint8_t* moe_plan_layout(void* workspace, int64_t P, int E, int N1, int K
   return q;
 }
 
-// GateDeepSeekV3.forward + the expert plan of the following fused_experts call in ONE launch chain (logits GEMM + gate):
-// out_indices / out_weights rows of `out_stride` = the (token, slot) pairs fused_experts will be given (engines append
-// the shared expert as an extra pre-filled column); moe_workspace = the workspace of that fused_experts call, which must
-// then be made with chitu_b200_fused_experts_planned (same T, topk = out_stride, E_total, N1, K1).
-extern "C" int chitu_b200_moe_gate_plan(const void* x, const void* w, const void* bias, int bias_dtype, int T, int dim, int E,
-                                        int n_groups, int topk_groups, int topk, int score_sigmoid, float route_scale,
-                                        void* out_weights, int64_t* out_indices, int out_stride, void* workspace,
-                                        int64_t workspace_bytes, int E_total, int N1, int K1, void* moe_workspace,
-                                        int64_t moe_workspace_bytes, void* stream) {
-  CB_ARG(moe_workspace && E_total >= E && E_total <= 1024 && N1 % 256 == 0 && K1 % 128 == 0 && out_stride >= topk);
-  CB_ARG(workspace && workspace_bytes >= chitu_b200_moe_gate_workspace_bytes(T, E));
-  const int64_t P = (int64_t)T * out_stride;
-  CB_ARG(P <= 8192 && moe_workspace_bytes >= chitu_b200_moe_workspace_bytes(T, out_stride, E_total, N1, K1));
-  GatePlanArgs gp;
-  memset(&gp, 0, sizeof(gp));
-  gp.enabled = 1; gp.P = (int)P; gp.E = E_total; gp.N1 = N1; gp.K1 = K1; gp.BN = moe_chunk_rows(P, E_total);
-  moe_plan_layout(moe_workspace, P, E_total, N1, K1, &gp.pl);
-  return moe_gate_impl(x, w, bias, bias_dtype, T, dim, E, n_groups, topk_groups, topk, score_sigmoid, route_scale, out_weights,
-                       out_indices, out_stride, workspace, workspace_bytes, stream, gp);
-}
-
 extern "C" int chitu_b200_fused_experts(const void* x, const void* w1, const void* w2, const float* w1_s,
                                         const float* w2_s, const void* topk_w, int topk_w_dtype,
                                         const void* topk_ids, int ids_dtype, int T, int topk, int E, int N1,
@@ -1242,18 +1052,7 @@ extern "C" int chitu_b200_fused_experts(const void* x, const void* w1, const voi
                                         int64_t workspace_bytes, void* stream) {
   CB_ARG(out);
   return fused_experts_impl(x, w1, w2, w1_s, w2_s, topk_w, topk_w_dtype, topk_ids, ids_dtype, T, topk, E, N1, K1, wmode, out,
-                            residual, workspace, workspace_bytes, stream, nullptr, 0);
-}
-
-// fused_experts whose plan was already written into `workspace` by chitu_b200_moe_gate_plan for exactly these pairs
-extern "C" int chitu_b200_fused_experts_planned(const void* x, const void* w1, const void* w2, const float* w1_s,
-                                                const float* w2_s, const void* topk_w, int topk_w_dtype,
-                                                const void* topk_ids, int ids_dtype, int T, int topk, int E, int N1,
-                                                int K1, int wmode, void* out, const void* residual, void* workspace,
-                                                int64_t workspace_bytes, void* stream) {
-  CB_ARG(out);
-  return fused_experts_impl(x, w1, w2, w1_s, w2_s, topk_w, topk_w_dtype, topk_ids, ids_dtype, T, topk, E, N1, K1, wmode, out,
-                            residual, workspace, workspace_bytes, stream, nullptr, 1);
+                            residual, workspace, workspace_bytes, stream, nullptr);
 }
 
 // fused_experts whose result (this rank's partial of the MoE block) is pushed into every rank's all-reduce area from the
@@ -1262,17 +1061,17 @@ extern "C" int chitu_b200_fused_experts_ar(const void* x, const void* w1, const 
                                            const float* w2_s, const void* topk_w, int topk_w_dtype,
                                            const void* topk_ids, int ids_dtype, int T, int topk, int E, int N1,
                                            int K1, int wmode, void* comm, void* workspace, int64_t workspace_bytes,
-                                           int planned, void* stream) {
+                                           void* stream) {
   CB_ARG(comm && K1 % 2 == 0 && (int64_t)T * K1 * 2 <= cb::comm_slot_bytes(comm));
   return fused_experts_impl(x, w1, w2, w1_s, w2_s, topk_w, topk_w_dtype, topk_ids, ids_dtype, T, topk, E, N1, K1, wmode, nullptr,
-                            nullptr, workspace, workspace_bytes, stream, comm, planned);
+                            nullptr, workspace, workspace_bytes, stream, comm);
 }
 
 static int fused_experts_impl(const void* x, const void* w1, const void* w2, const float* w1_s,
                               const float* w2_s, const void* topk_w, int topk_w_dtype,
                               const void* topk_ids, int ids_dtype, int T, int topk, int E, int N1,
                               int K1, int wmode, void* out, const void* residual, void* workspace,
-                              int64_t workspace_bytes, void* stream, void* comm, int planned) {
+                              int64_t workspace_bytes, void* stream, void* comm) {
   CB_ARG(x && w1 && w2 && topk_w && topk_ids && (out || comm) && workspace);
   CB_ARG(T >= 0 && topk > 0 && E > 0 && N1 > 0 && N1 % 2 == 0 && K1 > 0);
   CB_ARG(wmode >= 0 && wmode <= 2);
@@ -1289,10 +1088,9 @@ static int fused_experts_impl(const void* x, const void* w1, const void* w2, con
   CB_ARG(P <= 65535);
 
   // ---- grouped wgmma path: sort pairs by expert, stream every distinct expert once ----
-  static const bool force_pair = getenv("CHITU_B200_MOE_PAIR") != nullptr;
   const int BN = moe_chunk_rows(P, E);
   const int64_t chunks = E + P / 16 + 1;
-  if (!force_pair && P <= 8192 && E <= 1024 && N1 % 256 == 0 && K1 % 128 == 0 && (wmode != 2 || (N1 / 2) % 128 == 0) &&
+  if (P <= 8192 && E <= 1024 && N1 % 256 == 0 && K1 % 128 == 0 && (wmode != 2 || (N1 / 2) % 128 == 0) &&
       chunks * (N1 / 128) <= cb::tc_max_tiles() && chunks * (K1 / 128) <= cb::tc_max_tiles() && cb::tma_available()) {
     void* gws = workspace;
     MoePlan pl;
@@ -1305,50 +1103,22 @@ static int fused_experts_impl(const void* x, const void* w1, const void* w2, con
     __nv_bfloat16* c3 = (__nv_bfloat16*)q;
     const int quant = wmode == 1;
     const size_t psm = (size_t)moe_plan_smem_ints(P, E) * sizeof(int);
-    // plan + gather in one launch (every gather CTA places its own pair, CTA 0 writes the plan arrays): parity-green but
-    // SLOWER than the two launches — DeepSeek shard 13.23 -> 13.51 ms at bs = 16, 6.65 -> 6.80 ms at bs = 1, Mixtral shard
-    // 6.00 -> 6.11 ms (r2 call 17): every CTA repeats the staging + histogram and CTA 0 still runs the whole plan.  Off by
-    // default (CHITU_B200_MOE_PLAN_GATHER=1 turns it on).
-    static const int fuse_env = getenv("CHITU_B200_MOE_PLAN_GATHER") ? atoi(getenv("CHITU_B200_MOE_PLAN_GATHER")) : 0;
-    const bool plan_gather = !planned && fuse_env && P <= 1024;
-    if (plan_gather) {
-      static size_t pg_attr = 48 * 1024;
-      if (psm > pg_attr) {
-        CB_CUDA(cudaFuncSetAttribute(moe_plan_gather_kernel<int64_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psm));
-        CB_CUDA(cudaFuncSetAttribute(moe_plan_gather_kernel<int32_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psm));
-        pg_attr = psm;
-      }
-      if (ids_dtype == CB_I64)
-        cb::launch_k(moe_plan_gather_kernel<int64_t>, dim3((unsigned)P), dim3(256), psm, st, (const int64_t*)topk_ids, topk_w,
-                     (int)(topk_w_dtype == CB_F32), (int)P, E, N1, K1, BN, pl, (const __nv_bfloat16*)x, topk, quant, xs, xs_s,
-                     (__nv_bfloat16*)xs);
-      else
-        cb::launch_k(moe_plan_gather_kernel<int32_t>, dim3((unsigned)P), dim3(256), psm, st, (const int32_t*)topk_ids, topk_w,
-                     (int)(topk_w_dtype == CB_F32), (int)P, E, N1, K1, BN, pl, (const __nv_bfloat16*)x, topk, quant, xs, xs_s,
-                     (__nv_bfloat16*)xs);
-      CB_LAUNCHED(1);
-    } else if (planned) {
-      // the plan for exactly these pairs was written by the gate kernel's last CTA (chitu_b200_moe_gate_plan)
-    } else {
-      static size_t plan_attr = 48 * 1024;
-      if (psm > plan_attr) {
-        CB_CUDA(cudaFuncSetAttribute(moe_plan_kernel<int64_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psm));
-        CB_CUDA(cudaFuncSetAttribute(moe_plan_kernel<int32_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psm));
-        plan_attr = psm;
-      }
-      if (ids_dtype == CB_I64)
-        cb::launch_k(moe_plan_kernel<int64_t>, dim3(1), dim3(1024), psm, st, (const int64_t*)topk_ids, topk_w,
-                     (int)(topk_w_dtype == CB_F32), (int)P, E, N1, K1, BN, pl);
-      else
-        cb::launch_k(moe_plan_kernel<int32_t>, dim3(1), dim3(1024), psm, st, (const int32_t*)topk_ids, topk_w,
-                     (int)(topk_w_dtype == CB_F32), (int)P, E, N1, K1, BN, pl);
-      CB_LAUNCHED(1);
+    static size_t plan_attr = 48 * 1024;
+    if (psm > plan_attr) {
+      CB_CUDA(cudaFuncSetAttribute(moe_plan_kernel<int64_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psm));
+      CB_CUDA(cudaFuncSetAttribute(moe_plan_kernel<int32_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psm));
+      plan_attr = psm;
     }
-    if (!plan_gather) {
-      cb::launch_k(moe_gather_quant_kernel, dim3(cdiv(P * (K1 / 128), 8)), dim3(256), 0, st, (const __nv_bfloat16*)x,
-                   (const int*)pl.pair_sorted, (const int*)pl.seg_start, E, topk, K1, quant, xs, xs_s, (__nv_bfloat16*)xs);
-      CB_LAUNCHED(1);
-    }
+    if (ids_dtype == CB_I64)
+      cb::launch_k(moe_plan_kernel<int64_t>, dim3(1), dim3(kPlanThreads), psm, st, (const int64_t*)topk_ids, topk_w,
+                   (int)(topk_w_dtype == CB_F32), (int)P, E, N1, K1, BN, pl);
+    else
+      cb::launch_k(moe_plan_kernel<int32_t>, dim3(1), dim3(kPlanThreads), psm, st, (const int32_t*)topk_ids, topk_w,
+                   (int)(topk_w_dtype == CB_F32), (int)P, E, N1, K1, BN, pl);
+    CB_LAUNCHED(1);
+    cb::launch_k(moe_gather_quant_kernel, dim3(cdiv(P * (K1 / 128), 8)), dim3(256), 0, st, (const __nv_bfloat16*)x,
+                 (const int*)pl.pair_sorted, (const int*)pl.seg_start, E, topk, K1, quant, xs, xs_s, (__nv_bfloat16*)xs);
+    CB_LAUNCHED(1);
     const int gkind = wmode == 1 ? 1 : (wmode == 2 ? 3 : 0);     // KIND_FP8 / KIND_SOFT (fp8 weights -> bf16 in smem) / KIND_16
     int rc = cb::tc_grouped_gemm(gkind, xs, xs_s, w1, w1_s, c1, (int)P, E, N1, K1, BN, pl.num_tiles1, pl.tile1_wrow,
                                  pl.tile1_xrow, pl.tile1_cnt, nullptr, nullptr, gws, cb::tc_workspace_bytes(128, 128), st);

@@ -130,13 +130,12 @@ class LlamaDecodeEngine:
         import os
         # SiluAndMul inside the w13 GEMM epilogue: the merged gate/up weight is stored with its rows interleaved
         # (row 2i = gate_i, row 2i+1 = up_i) — a load-time permutation of the reference's merged tensor
-        self.fuse_silu = os.environ.get("CHITU_B200_FUSE_SILU", "1") != "0" and linear_impl != 1
+        self.fuse_silu = linear_impl != 1
         if self.fuse_silu:
             for lw in self.layers:
                 lw["w13"] = lw["w13"].view(2, self.F, dim).transpose(0, 1).reshape(2 * self.F, dim).contiguous()
-        self.fuse_rope = (D == 128 and (page_size & (page_size - 1)) == 0 and self.Hq // self.Hkv in (1, 2, 4, 8)
-                          and os.environ.get("CHITU_B200_FUSE_ROPE", "1") != "0"
-                          and int(os.environ.get("CHITU_B200_GQA_CFG", "5")) >= 4 and not os.environ.get("CHITU_B200_GQA_SIMT"))
+        # rotary fused into the tensor-core decode kernel (head dim 128, power-of-two pages)
+        self.fuse_rope = D == 128 and (page_size & (page_size - 1)) == 0 and self.Hq // self.Hkv in (1, 2, 4, 8)
         self.graph = None
         self.launches_per_step = 0
         # push mode: the row-parallel GEMM's epilogue starts the all-reduce (A/B: CHITU_B200_AR_PUSH=0 -> pull kernel)

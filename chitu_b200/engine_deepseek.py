@@ -209,14 +209,8 @@ class DeepSeekDecodeEngine:
         self.max_seq_len = max_seq_len
         # the wgmma MLA kernel can leave its split-KV partials for the absorb-o kernel to merge (one launch fewer)
         import os
-        self.defer_merge = (page_size == 64 and os.environ.get("CHITU_B200_MLA_IMPL", "0") == "0"
-                            and os.environ.get("CHITU_B200_MLA_DEFER_MERGE", "1") != "0"
-                            and c.v_head_dim == 128 and self.C == 512)
+        self.defer_merge = page_size == 64 and c.v_head_dim == 128 and self.C == 512
         self.ar_push = os.environ.get("CHITU_B200_AR_PUSH", "1") != "0"
-        # optional: the gate kernel's last CTA writes the expert plan (chitu_b200_moe_gate_plan, one launch fewer); off by
-        # default: the in-kernel hand-off (fence + ticket + a 256-thread plan) is serial work on the critical path where the
-        # separate plan kernel only costs a PDL launch.
-        self.gate_plan = os.environ.get("CHITU_B200_GATE_PLAN", "0") == "1" and B * self.topk1 <= 8192
         self.graph = None
         self.launches_per_step = 0
         self.trace = None          # set to [] to record per-layer intermediates (tests; not under CUDA graphs)
@@ -373,29 +367,18 @@ class DeepSeekDecodeEngine:
                     norm_only(h, next_norm, last, not last)
             else:
                 E1 = c.n_routed_experts + 1
-                planned = 1 if self.gate_plan else 0
-                if planned:
-                    # the gate's last CTA also writes the expert plan of the fused_experts call below (one launch fewer)
-                    check(lib.chitu_b200_moe_gate_plan(ptr(self.xn), ptr(L["gate_w"]), ptr(L["gate_b"]), _lib.CB_F32, B, c.dim,
-                                                       c.n_routed_experts, c.n_expert_groups, c.n_limited_groups,
-                                                       c.n_activated_experts, 1 if c.score_func == "sigmoid" else 0,
-                                                       float(c.route_scale), ptr(self.gate_w_all[li]), ptr(self.gate_i_all[li]),
-                                                       self.topk1, ptr(self.gate_ws), self.gate_ws.numel(), E1, 2 * self.F_moe,
-                                                       c.dim, ptr(self.moe_ws), self.moe_ws.numel(), st), "moe_gate_plan")
-                else:
-                    check(lib.chitu_b200_moe_gate(ptr(self.xn), ptr(L["gate_w"]), ptr(L["gate_b"]), _lib.CB_F32, B, c.dim,
-                                                  c.n_routed_experts, c.n_expert_groups, c.n_limited_groups,
-                                                  c.n_activated_experts, 1 if c.score_func == "sigmoid" else 0,
-                                                  float(c.route_scale), ptr(self.gate_w_all[li]), ptr(self.gate_i_all[li]),
-                                                  self.topk1, ptr(self.gate_ws), self.gate_ws.numel(), st), "moe_gate")
+                check(lib.chitu_b200_moe_gate(ptr(self.xn), ptr(L["gate_w"]), ptr(L["gate_b"]), _lib.CB_F32, B, c.dim,
+                                              c.n_routed_experts, c.n_expert_groups, c.n_limited_groups,
+                                              c.n_activated_experts, 1 if c.score_func == "sigmoid" else 0,
+                                              float(c.route_scale), ptr(self.gate_w_all[li]), ptr(self.gate_i_all[li]),
+                                              self.topk1, ptr(self.gate_ws), self.gate_ws.numel(), st), "moe_gate")
                 if push:
                     self.comm.experts_push(self.xn, L["we1"], L["we2"], L["we1_s"], L["we2_s"], self.gate_w_all[li], _lib.CB_BF16,
                                                self.gate_i_all[li], _lib.CB_I64, B, self.topk1, E1,
-                                               2 * self.F_moe, c.dim, 1, self.moe_ws, planned=planned)
+                                               2 * self.F_moe, c.dim, 1, self.moe_ws)
                     consume(h2, h, next_norm, last, not last)
                 else:
-                    fe = lib.chitu_b200_fused_experts_planned if planned else lib.chitu_b200_fused_experts
-                    check(fe(
+                    check(lib.chitu_b200_fused_experts(
                         ptr(self.xn), ptr(L["we1"]), ptr(L["we2"]), ptr(L["we1_s"]), ptr(L["we2_s"]), ptr(self.gate_w_all[li]),
                         _lib.CB_BF16, ptr(self.gate_i_all[li]), _lib.CB_I64, B, self.topk1, E1,
                         2 * self.F_moe, c.dim, 1, ptr(self.y if tp_on else h), None if tp_on else ptr(h2), ptr(self.moe_ws),

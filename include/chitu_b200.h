@@ -78,17 +78,6 @@ int chitu_b200_moe_gate(const void* x, const void* w, const void* bias, int bias
                         float route_scale, void* out_weights, int64_t* out_indices,
                         int out_stride /* elements per token row of both outputs, >= topk */, void* workspace,
                         int64_t workspace_bytes, void* stream);
-/* The same gate, whose LAST CTA also writes the expert plan (sort by expert, row chunks, tile lists — the work of
- * moe_align_block_size, fused_moe.py:599-610, inside fused_experts_impl fused_moe.py:1130-1307) of the fused_experts call
- * that follows, into that call's workspace: the pairs are the [T, out_stride] rows of out_indices / out_weights (engines pre-fill column `topk` with the shared
- * expert).  Follow with chitu_b200_fused_experts_planned(T, topk = out_stride, E_total, N1, K1, moe_workspace).
- * One dependent launch fewer per MoE layer; the in-kernel hand-off is serial work on the critical path, so the
- * engines keep it off by default. */
-int chitu_b200_moe_gate_plan(const void* x, const void* w, const void* bias, int bias_dtype, int T, int dim, int E,
-                             int n_groups, int topk_groups, int topk, int score_sigmoid, float route_scale,
-                             void* out_weights, int64_t* out_indices, int out_stride, void* workspace,
-                             int64_t workspace_bytes, int E_total, int N1, int K1, void* moe_workspace,
-                             int64_t moe_workspace_bytes, void* stream);
 
 /* ---- rotary --------------------------------------------------------------------------- */
 /* Replaces triton_kernels.py:101-190 (rotary_type="llama", interleaved pairs; cos/sin f32
@@ -212,11 +201,11 @@ int chitu_b200_gqa_paged_decode_rope(const void* q, int64_t q_sb, void* k_cache,
 
 /* *.mla_attn_with_kvcache (attn_backend.py:536-572 / 660-684 / 707-774) = append
  * (ops.py:50-91) + mla_decode (triton_decode_attention.py:259-290) in one call.
- * q_nope:[B,H,C] q_pe:[B,H,R] kv_cache:[num_blocks,page,C+R] new_kv:[B,C+R] (may be NULL)
+ * q_nope:[B,H,C] q_pe:[B,H,R] kv_cache:[num_blocks,64,C+R] new_kv:[B,C+R] (may be NULL)
  * seqlens_excl:[B] (length before this token) ; attention runs over seqlens_excl+1 keys when
  * new_kv != NULL else over seqlens_excl keys.  out:[B,H,C] (latent space). bf16.
- * num_blocks = kv_cache.shape[0] (bounds the TMA tensor map that stages whole 64-key pages).
- * out == NULL (wgmma kernel only: page 64): the split merge is deferred to chitu_b200_mla_absorb_o_merge_quant. */
+ * page_size must be 64; num_blocks = kv_cache.shape[0] (bounds the TMA tensor map that stages whole pages).
+ * out == NULL: the split merge is deferred to chitu_b200_mla_absorb_o_merge_quant. */
 int chitu_b200_mla_decode(const void* q_nope, const void* q_pe, void* kv_cache, const void* new_kv,
                           const int32_t* seqlens_excl, const int32_t* block_table, int bt_stride,
                           int B, int H, int C, int R, int page_size, int num_blocks, int max_seqlen_hint,
@@ -324,13 +313,6 @@ int chitu_b200_fused_experts(const void* x, const void* w1, const void* w2, cons
                              int K1, int wmode, void* out,
                              const void* residual /* [T,K1] bf16 added to the rounded result, or NULL */,
                              void* workspace, int64_t workspace_bytes, void* stream);
-/* fused_experts whose plan chitu_b200_moe_gate_plan already wrote into `workspace` (same T, topk, E, N1, K1). */
-int chitu_b200_fused_experts_planned(const void* x, const void* w1, const void* w2, const float* w1_s,
-                             const float* w2_s, const void* topk_w, int topk_w_dtype,
-                             const void* topk_ids, int ids_dtype, int T, int topk, int E, int N1,
-                             int K1, int wmode, void* out,
-                             const void* residual /* [T,K1] bf16 added to the rounded result, or NULL */,
-                             void* workspace, int64_t workspace_bytes, void* stream);
 
 /* ---- tensor-parallel collective fused with what follows it ------------------------------------------ */
 /* Replaces `all_reduce` of RowParallelLinear.forward (tensor_parallel.py:157-169) / MoEDeepSeekV3
@@ -360,7 +342,7 @@ int chitu_b200_linear_bf16_ar(const void* x, const void* w, int M, int N, int K,
 int chitu_b200_fused_experts_ar(const void* x, const void* w1, const void* w2, const float* w1_s, const float* w2_s,
                                 const void* topk_w, int topk_w_dtype, const void* topk_ids, int ids_dtype, int T, int topk,
                                 int E, int N1, int K1, int wmode, void* comm, void* workspace, int64_t workspace_bytes,
-                                int planned /* 1: plan written by chitu_b200_moe_gate_plan */, void* stream);
+                                void* stream);
 int chitu_b200_allreduce_consume(void* comm, const void* residual, void* h_out, const void* norm_w, void* y,
                                  void* q, float* q_scales, int rows, int dim, float eps, void* stream);
 /* h = bf16(sum_r partial_r) (+ residual);  optional outputs of RMSNorm(h)*norm_w: y (bf16) and / or q (fp8,

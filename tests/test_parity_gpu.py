@@ -509,50 +509,6 @@ def test_fused_experts_inplace_and_flags():
                                 use_int8_w8a16=True)
 
 
-@pytest.mark.parametrize("T", [1, 16, 96])
-def test_gate_plan_fused_equals_separate_plan(T):
-    """chitu_b200_moe_gate_plan (+ fused_experts_planned) == moe_gate + fused_experts, bit for bit, call after call
-    (the ticket that elects the gate's last CTA re-arms itself)."""
-    from chitu_b200 import _lib
-    from chitu_b200._lib import check, current_stream, ptr
-    lib = _lib.load()
-    dev = torch.device("cuda")
-    torch.manual_seed(77)
-    dim, E, topk, F = 1024, 256, 8, 256
-    wg = (torch.randn(E, dim, device=dev) * 0.02).to(BF)
-    bias = torch.randn(E, device=dev) * 0.01
-    w1 = (torch.randn(E + 1, 2 * F, dim, device=dev) * 0.05).to(BF)
-    w2 = (torch.randn(E + 1, dim, F, device=dev) * 0.05).to(BF)
-    gate_ws = torch.zeros(lib.chitu_b200_moe_gate_workspace_bytes(T, E), dtype=torch.uint8, device=dev)
-    moe_ws = torch.zeros(lib.chitu_b200_moe_workspace_bytes(T, topk + 1, E + 1, 2 * F, dim), dtype=torch.uint8, device=dev)
-    st = current_stream()
-
-    def outputs():
-        gw = torch.ones(T, topk + 1, dtype=BF, device=dev)
-        gi = torch.full((T, topk + 1), E, dtype=torch.int64, device=dev)       # column topk = the shared expert
-        return gw, gi, torch.empty(T, dim, dtype=BF, device=dev)
-
-    for it in range(3):
-        x = torch.randn(T, dim, device=dev).to(BF)
-        gw_a, gi_a, out_a = outputs()
-        check(lib.chitu_b200_moe_gate(ptr(x), ptr(wg), ptr(bias), _lib.CB_F32, T, dim, E, 8, 4, topk, 1, 2.5, ptr(gw_a), ptr(gi_a),
-                                      topk + 1, ptr(gate_ws), gate_ws.numel(), st), "moe_gate")
-        check(lib.chitu_b200_fused_experts(ptr(x), ptr(w1), ptr(w2), None, None, ptr(gw_a), _lib.CB_BF16, ptr(gi_a), _lib.CB_I64, T,
-                                           topk + 1, E + 1, 2 * F, dim, 0, ptr(out_a), None, ptr(moe_ws), moe_ws.numel(), st),
-              "fused_experts")
-        gw_b, gi_b, out_b = outputs()
-        check(lib.chitu_b200_moe_gate_plan(ptr(x), ptr(wg), ptr(bias), _lib.CB_F32, T, dim, E, 8, 4, topk, 1, 2.5, ptr(gw_b),
-                                           ptr(gi_b), topk + 1, ptr(gate_ws), gate_ws.numel(), E + 1, 2 * F, dim, ptr(moe_ws),
-                                           moe_ws.numel(), st), "moe_gate_plan")
-        check(lib.chitu_b200_fused_experts_planned(ptr(x), ptr(w1), ptr(w2), None, None, ptr(gw_b), _lib.CB_BF16, ptr(gi_b),
-                                                   _lib.CB_I64, T, topk + 1, E + 1, 2 * F, dim, 0, ptr(out_b), None, ptr(moe_ws),
-                                                   moe_ws.numel(), st), "fused_experts_planned")
-        torch.cuda.synchronize()
-        assert torch.equal(gi_a, gi_b) and torch.equal(gw_a, gw_b)
-        assert torch.equal(out_a, out_b), (it, (out_a.float() - out_b.float()).abs().max().item())
-        assert out_a.float().abs().max() > 0
-
-
 # ------------------------------------------------------------------------- fused decode-engine ops
 def test_fused_rmsnorm_quant_and_silu_quant():
     from chitu_b200 import ops
