@@ -7,18 +7,24 @@ but every operator is a libchitu_b200 kernel and the whole step is one CUDA grap
 It exists so `bench.py` can measure BASELINE.json's metric (decode tokens/s) on synthetic
 weights of the named architecture; it is not a re-implementation of the reference's model zoo
 (checkpoint loading, prefill, PP stay in the reference).
+
+`DecodeEngine` is the part every model shares; the LLaMA, DeepSeek (engine_deepseek.py) and
+Mixtral (engine_mixtral.py) engines add their weights and their layers.
 """
 from __future__ import annotations
 
 import math
+import os
 from dataclasses import dataclass
 from typing import Optional
 
 import torch
 
-from . import _lib, workspace
-from ._lib import check, current_stream, dtype_code, ptr
+from . import _lib
+from ._lib import check, current_stream, ptr
 from .tensor_parallel import global_argmax
+
+BF = torch.bfloat16
 
 
 @dataclass
@@ -52,99 +58,63 @@ LLAMA2_7B = LlamaConfig(dim=4096, n_layers=32, n_heads=32, n_kv_heads=32, vocab_
                         ffn_dim_multiplier=None, norm_eps=1e-5, rope_theta=10000.0)
 
 
-class LlamaDecodeEngine:
-    """Single-GPU (tp=1) or tensor-parallel LLaMA decode.  Weights are random (`do_load=False`,
-    serve_config.yaml:9).  KV cache layout = PagedKVCacheManager (cache_manager.py:71-87):
-    paged_k_cache / paged_v_cache [L, num_blocks, page, n_local_kv_heads, head_dim], page 256
-    (backend.py:237), persistent int32 block_table [max_reqs, max_blocks] and seq_lens buffers."""
+class DecodeEngine:
+    """Greedy decode over persistent buffers, eager or replayed as one CUDA graph: embedding + rotary-position gather,
+    the model's layers, then the vocab-parallel head and argmax.
 
-    def __init__(self, cfg: LlamaConfig, max_reqs: int, max_seq_len: int, device="cuda:0", page_size: int = 256,
-                 seed: int = 0, tp_rank: int = 0, tp_size: int = 1, process_group=None, linear_impl: int = 0,
-                 use_fused_allreduce: bool = True):
+    A subclass builds its weights, its KV caches (listed in `self.caches`) and its rotary tables (`_rope_tables`),
+    and runs its layers in `_decode_layers`: from the embedded tokens in `self.h` to the final norm in `self.xn`.
+    `_norm` is the RMSNorm the row-parallel reduce ends with (bf16 here).
+
+    Tensor parallel when a process group is given and tp_size > 1 (`tp_on`).  With tp_size > 1 and no group the engine
+    runs ONE rank's shard without collectives ("shard mode": the per-rank kernel time of a tensor-parallel
+    configuration measured on one GPU)."""
+
+    linear_impl = 0          # `impl` of the bf16 linear entries: 0 = auto
+
+    def __init__(self, cfg, max_reqs: int, max_seq_len: int, device, page_size: int, seed: int, tp_rank: int,
+                 tp_size: int, process_group, use_fused_allreduce: bool, attn_ws: tuple, lin_n: int):
+        """attn_ws: (heads, head_dim_v, max_splits) the attention workspace is sized for; lin_n: the widest N the
+        linear workspace is sized for."""
         self.cfg, self.B, self.device = cfg, max_reqs, torch.device(device)
         self.tp_rank, self.tp_size, self.pg = tp_rank, tp_size, process_group
-        self.tp_gather = None
-        self.linear_impl = linear_impl
+        self.tp_on = process_group is not None and tp_size > 1
         self.lib = _lib.load()
-        dt = torch.bfloat16
-        D = cfg.head_dim
-        assert cfg.n_heads % tp_size == 0 and cfg.n_kv_heads % tp_size == 0
-        self.Hq, self.Hkv, self.D = cfg.n_heads // tp_size, cfg.n_kv_heads // tp_size, D
-        self.F = cfg.ffn_dim // tp_size
-        self.page = page_size
+        dev, B, dim = self.device, max_reqs, cfg.dim
+        self.g = torch.Generator(device=dev).manual_seed(seed + 1000 * tp_rank)       # this rank's shards
+        self.g_rep = torch.Generator(device=dev).manual_seed(seed + 7)                # replicated across TP ranks
+        # paged KV cache (PagedKVCacheManager, cache_manager.py:71-87): persistent int32 block_table and seq_lens
+        self.page, self.max_seq_len = page_size, max_seq_len
         self.max_blocks = max_seq_len // page_size + 1
-        nblk = self.max_blocks * max_reqs
-        g = torch.Generator(device=self.device).manual_seed(seed + 1000 * tp_rank)
-
-        def rnd(*shape, scale=0.02):
-            return (torch.randn(*shape, generator=g, dtype=torch.float32, device=self.device) * scale).to(dt)
-
-        dim = cfg.dim
-        g_rep = torch.Generator(device=self.device).manual_seed(seed + 7)     # replicated across TP ranks
-        self.embed = (torch.randn(cfg.vocab_size, dim, generator=g_rep, dtype=torch.float32, device=self.device) * 0.02).to(dt)
-        self.layers = []
-        for _ in range(cfg.n_layers):
-            self.layers.append(dict(
-                attn_norm=torch.ones(dim, dtype=dt, device=self.device),
-                ffn_norm=torch.ones(dim, dtype=dt, device=self.device),
-                # column-parallel wq|wk|wv merged along N (shards of each concatenated); row-parallel wo
-                wqkv=rnd((self.Hq + 2 * self.Hkv) * D, dim),
-                wo=rnd(dim, self.Hq * D),
-                w13=rnd(2 * self.F, dim),          # [w1 (gate) ; w3 (up)]  (interleaved below when the epilogue fuses SiLU)
-                w2=rnd(dim, self.F),
-            ))
-        self.norm = torch.ones(dim, dtype=dt, device=self.device)
-        self.head = rnd(cfg.vocab_size // tp_size, dim)
-        self.k_cache = torch.zeros(cfg.n_layers, nblk, page_size, self.Hkv, D, dtype=dt, device=self.device)
-        self.v_cache = torch.zeros_like(self.k_cache)
-        self.block_table = torch.zeros(max_reqs, self.max_blocks, dtype=torch.int32, device=self.device)
-        self.seq_lens = torch.zeros(max_reqs, dtype=torch.int32, device=self.device)
-        # precompute_freqs_cis (models/model.py:81-89) as cos/sin tables
-        freqs = 1.0 / (cfg.rope_theta ** (torch.arange(0, D, 2)[: D // 2].float() / D))
-        t = torch.arange(max_seq_len * 2, dtype=torch.float32)
-        ang = torch.outer(t, freqs)
-        self.cos_table, self.sin_table = ang.cos().to(self.device), ang.sin().to(self.device)
-        # persistent activations (CUDA-graph safe)
-        B = max_reqs
-        self.tokens = torch.zeros(B, dtype=torch.int64, device=self.device)
-        self.cos = torch.zeros(B, D // 2, dtype=torch.float32, device=self.device)
-        self.sin = torch.zeros_like(self.cos)
-        self.h = torch.zeros(B, dim, dtype=dt, device=self.device)
-        self.h2 = torch.zeros_like(self.h)
-        self.xn = torch.zeros_like(self.h)
-        self.qkv = torch.zeros(B, (self.Hq + 2 * self.Hkv) * D, dtype=dt, device=self.device)
-        self.q_rot = torch.zeros(B, self.Hq, D, dtype=dt, device=self.device)
-        self.k_rot = torch.zeros(B, self.Hkv, D, dtype=dt, device=self.device)
-        self.attn_out = torch.zeros(B, self.Hq * D, dtype=dt, device=self.device)
-        self.gate_up = torch.zeros(B, 2 * self.F, dtype=dt, device=self.device)
-        self.act = torch.zeros(B, self.F, dtype=dt, device=self.device)
-        self.logits = torch.zeros(B, cfg.vocab_size // tp_size, dtype=dt, device=self.device)
-        self.next_tokens = torch.zeros(B, dtype=torch.int64, device=self.device)
-        if self.tp_size > 1:
-            self.tp_gather = torch.empty(self.tp_size, B, 2, dtype=torch.float32, device=self.device)
-        n_attn = self.lib.chitu_b200_attn_workspace_bytes(B, self.Hq, D, 64)
-        self.attn_ws = torch.empty(n_attn, dtype=torch.uint8, device=self.device)
-        n_lin = max(self.lib.chitu_b200_linear_workspace_bytes(B, max(2 * self.F, cfg.vocab_size // tp_size)), 256)
-        self.lin_ws = torch.zeros(n_lin, dtype=torch.uint8, device=self.device)   # tickets start at 0
-        self.max_seq_len = max_seq_len
-        import os
-        # SiluAndMul inside the w13 GEMM epilogue: the merged gate/up weight is stored with its rows interleaved
-        # (row 2i = gate_i, row 2i+1 = up_i) — a load-time permutation of the reference's merged tensor
-        self.fuse_silu = linear_impl != 1
-        if self.fuse_silu:
-            for lw in self.layers:
-                lw["w13"] = lw["w13"].view(2, self.F, dim).transpose(0, 1).reshape(2 * self.F, dim).contiguous()
-        # rotary fused into the tensor-core decode kernel (head dim 128, power-of-two pages)
-        self.fuse_rope = D == 128 and (page_size & (page_size - 1)) == 0 and self.Hq // self.Hkv in (1, 2, 4, 8)
+        self.block_table = torch.zeros(max_reqs, self.max_blocks, dtype=torch.int32, device=dev)
+        self.seq_lens = torch.zeros(max_reqs, dtype=torch.int32, device=dev)
+        # persistent step I/O and residual stream (CUDA-graph safe)
+        self.tokens = torch.zeros(B, dtype=torch.int64, device=dev)
+        self.h, self.h2, self.xn = (torch.zeros(B, dim, dtype=BF, device=dev) for _ in range(3))
+        self.logits = torch.zeros(B, cfg.vocab_size // tp_size, dtype=BF, device=dev)
+        self.next_tokens = torch.zeros(B, dtype=torch.int64, device=dev)
+        self.tp_gather = torch.empty(tp_size, B, 2, dtype=torch.float32, device=dev) if self.tp_on else None
+        heads, head_dim_v, max_splits = attn_ws
+        self.attn_ws = torch.zeros(self.lib.chitu_b200_attn_workspace_bytes(B, heads, head_dim_v, max_splits),
+                                   dtype=torch.uint8, device=dev)
+        self.lin_ws = torch.zeros(max(self.lib.chitu_b200_linear_workspace_bytes(B, lin_n), 256), dtype=torch.uint8,
+                                  device=dev)                    # split-K tickets start at 0
+        # push mode: the row-parallel GEMM's epilogue starts the all-reduce; "0" selects the pull kernel
+        self.ar_push = os.environ.get("CHITU_B200_AR_PUSH", "1") != "0"
+        # fused one-shot all-reduce + residual + RMSNorm(+quant) over NVLink peer memory (csrc/comm.cu); NCCL otherwise
+        self.comm = None
+        if self.tp_on and use_fused_allreduce:
+            from .comm import FusedAllReduce
+            self.comm = FusedAllReduce(process_group, max_reqs, dim, dev)
         self.graph = None
         self.launches_per_step = 0
-        # push mode: the row-parallel GEMM's epilogue starts the all-reduce (A/B: CHITU_B200_AR_PUSH=0 -> pull kernel)
-        self.ar_push = os.environ.get("CHITU_B200_AR_PUSH", "1") != "0" and linear_impl != 1
-        # fused one-shot all-reduce + residual + RMSNorm over NVLink peer memory (csrc/comm.cu); NCCL otherwise
-        self.comm = None
-        if tp_size > 1 and process_group is not None and use_fused_allreduce:
-            from .comm import FusedAllReduce
-            self.comm = FusedAllReduce(process_group, max_reqs, dim, self.device)
+
+    def _rope_tables(self, ang: torch.Tensor, dtype=torch.float32):
+        """cos / sin tables from the rotary angles [positions, rot_dim / 2], and the per-step buffers that
+        `_step_body` gathers them into by position."""
+        self.cos_table, self.sin_table = ang.cos().to(dtype).to(self.device), ang.sin().to(dtype).to(self.device)
+        self.cos = torch.zeros(self.B, ang.shape[1], dtype=dtype, device=self.device)
+        self.sin = torch.zeros_like(self.cos)
 
     # ---- cache bookkeeping (host side of PagedKVCacheManager, cache_manager.py:148-209) ----------
     def set_synthetic_context(self, seq_len: int, seed: int = 2):
@@ -152,23 +122,12 @@ class LlamaDecodeEngine:
         (non-identity) block table (SURVEY §8d synthetic inputs)."""
         g = torch.Generator(device="cpu").manual_seed(seed)
         gd = torch.Generator(device=self.device).manual_seed(seed + 11)     # deterministic cache contents
-        nblk = self.k_cache.shape[1]
-        perm = torch.randperm(nblk, generator=g).to(torch.int32)
+        perm = torch.randperm(self.block_table.numel(), generator=g).to(torch.int32)
         self.block_table.copy_(perm.view(self.B, self.max_blocks))
         self.seq_lens.fill_(seq_len)
         for l in range(self.cfg.n_layers):
-            self.k_cache[l].normal_(0, 1, generator=gd)
-            self.v_cache[l].normal_(0, 1, generator=gd)
-
-    def ref_layers(self):
-        """The layer weights in the REFERENCE's layout (w13 = [w1 ; w3] halves) for the oracle side of the tests."""
-        out = []
-        for lw in self.layers:
-            d = dict(lw)
-            if self.fuse_silu:
-                d["w13"] = lw["w13"].view(self.F, 2, self.cfg.dim).transpose(0, 1).reshape(2 * self.F, self.cfg.dim).contiguous()
-            out.append(d)
-        return out
+            for cache in self.caches:
+                cache[l].normal_(0, 1, generator=gd)
 
     # ---- one decode step ---------------------------------------------------------------------------
     def _linear(self, x, w, y, M, residual=None):
@@ -177,87 +136,56 @@ class LlamaDecodeEngine:
                                               ptr(self.lin_ws), self.lin_ws.numel(), self.linear_impl,
                                               current_stream()), "linear_bf16")
 
-    def _rmsnorm(self, x, w, y, M):
-        check(self.lib.chitu_b200_rmsnorm(ptr(x), ptr(w), ptr(y), M, self.cfg.dim, self.cfg.norm_eps, _lib.CB_BF16,
+    def _norm(self, x, w, y, q=None, qs=None):
+        assert q is None and qs is None, "this engine has no fp8 norm output"
+        check(self.lib.chitu_b200_rmsnorm(ptr(x), ptr(w), ptr(y), self.B, self.cfg.dim, self.cfg.norm_eps, _lib.CB_BF16,
                                           current_stream()), "rmsnorm")
 
     def _allreduce(self, t):
-        if self.tp_size > 1:
+        if self.tp_on:
             torch.distributed.all_reduce(t, group=self.pg)
 
+    def _row_parallel(self, gemm, push, residual, h_out, norm_w, y=None, q=None, qs=None, partial=None):
+        """h_out = residual + the sum over ranks of a row-parallel product, then RMSNorm(h_out) * norm_w into the
+        wanted outputs (bf16 `y`, fp8 `q` + scales `qs`).
+
+        `gemm(out, residual)` writes this rank's product into `out`, adding `residual` when it is given; `push()` is the
+        same product with the epilogue that starts the fused all-reduce.  Single GPU (and shard mode) fuses the residual
+        into the GEMM; tensor parallel reduces by push + consume, by the fused pull kernel, or by NCCL + add + norm,
+        with this rank's product in `partial` (default: `h_out`)."""
+        B, dim, eps = self.B, self.cfg.dim, self.cfg.norm_eps
+        if not self.tp_on:
+            gemm(h_out, residual)
+            self._norm(h_out, norm_w, y, q, qs)
+        elif self.comm is not None and self.ar_push:
+            push()
+            self.comm.consume(residual, h_out, norm_w, y, q, qs, B, dim, eps)
+        else:
+            partial = h_out if partial is None else partial
+            gemm(partial, None)
+            if self.comm is not None:
+                self.comm(partial, residual, h_out, norm_w, y, q, qs, B, dim, eps)
+            else:
+                self._allreduce(partial)
+                check(self.lib.chitu_b200_add(ptr(partial), ptr(residual), ptr(h_out), B * dim, _lib.CB_BF16,
+                                              current_stream()), "add")
+                self._norm(h_out, norm_w, y, q, qs)
+
     def _step_body(self):
-        lib, B, D = self.lib, self.B, self.D
+        lib, B, cfg = self.lib, self.B, self.cfg
         st = current_stream()
-        cfg = self.cfg
         # prepare_freqs_cis_decode (models/model.py:429-448): gather cos/sin by position
         torch.index_select(self.cos_table, 0, self.seq_lens, out=self.cos)
         torch.index_select(self.sin_table, 0, self.seq_lens, out=self.sin)
-        vocab_local = cfg.vocab_size // self.tp_size
-        check(lib.chitu_b200_embedding(ptr(self.tokens), ptr(self.embed), ptr(self.h), B, cfg.dim,
-                                       0, cfg.vocab_size, _lib.CB_BF16, st), "embedding")
-        h, h2 = self.h, self.h2
-        qkv_w = (self.Hq + 2 * self.Hkv) * D
-        n_layers = len(self.layers)
-
-        def reduce_add_norm(partial, residual, h_out, norm_w):
-            """h_out = all_reduce(partial) + residual ; self.xn = RMSNorm(h_out) * norm_w"""
-            if self.comm is not None:
-                self.comm(partial, residual, h_out, norm_w, self.xn, None, None, B, cfg.dim, cfg.norm_eps)
-            else:
-                self._allreduce(partial)
-                check(lib.chitu_b200_add(ptr(partial), ptr(residual), ptr(h_out), B * cfg.dim, _lib.CB_BF16, st), "add")
-                self._rmsnorm(h_out, norm_w, self.xn, B)
-
-        self._rmsnorm(h, self.layers[0]["attn_norm"], self.xn, B)
-        for li, lw in enumerate(self.layers):
-            next_norm = self.layers[li + 1]["attn_norm"] if li + 1 < n_layers else self.norm
-            self._linear(self.xn, lw["wqkv"], self.qkv, B)
-            q_view, k_view = self.qkv, self.qkv[:, self.Hq * D:]
-            v_view = self.qkv[:, (self.Hq + self.Hkv) * D:]
-            if self.fuse_rope:
-                # rotary (q and the new k) inside the attention kernel: q / k / v are views of the qkv GEMM output
-                check(lib.chitu_b200_gqa_paged_decode_rope(
-                    ptr(q_view), qkv_w, ptr(self.k_cache[li]), ptr(self.v_cache[li]), ptr(k_view), ptr(v_view), qkv_w, qkv_w,
-                    ptr(self.cos), ptr(self.sin), ptr(self.seq_lens), ptr(self.block_table), self.max_blocks, B, self.Hq,
-                    self.Hkv, D, self.page, self.max_seq_len, 1.0 / math.sqrt(D), ptr(self.attn_out), ptr(self.attn_ws),
-                    self.attn_ws.numel(), _lib.CB_BF16, st), "gqa_paged_decode_rope")
-            else:
-                check(lib.chitu_b200_rotary_interleaved(ptr(q_view), ptr(k_view), ptr(self.q_rot), ptr(self.k_rot),
-                                                        ptr(self.cos), ptr(self.sin), B, self.Hq, self.Hkv, D, qkv_w, D,
-                                                        qkv_w, D, _lib.CB_BF16, st), "rotary")
-                check(lib.chitu_b200_gqa_paged_decode(
-                    ptr(self.q_rot), ptr(self.k_cache[li]), ptr(self.v_cache[li]), ptr(self.k_rot), ptr(v_view),
-                    self.Hkv * D, qkv_w, ptr(self.seq_lens), ptr(self.block_table), self.max_blocks, B, self.Hq,
-                    self.Hkv, D, self.page, self.max_seq_len, 1.0 / math.sqrt(D), ptr(self.attn_out), ptr(self.attn_ws),
-                    self.attn_ws.numel(), _lib.CB_BF16, st), "gqa_paged_decode")
-            if self.tp_size == 1:
-                self._linear(self.attn_out, lw["wo"], h2, B, residual=h)      # h2 = wo(o) + h
-                self._rmsnorm(h2, lw["ffn_norm"], self.xn, B)
-            elif self.comm is not None and self.ar_push:
-                self.comm.linear_push(self.attn_out, lw["wo"], B, self.lin_ws)
-                self.comm.consume(h, h2, lw["ffn_norm"], self.xn, None, None, B, cfg.dim, cfg.norm_eps)
-            else:
-                self._linear(self.attn_out, lw["wo"], h2, B)
-                reduce_add_norm(h2, h, h2, lw["ffn_norm"])
-            if self.fuse_silu:
-                check(lib.chitu_b200_linear_bf16_silu_pairs(ptr(self.xn), ptr(lw["w13"]), ptr(self.act), B, 2 * self.F, cfg.dim,
-                                                            ptr(self.lin_ws), self.lin_ws.numel(), st), "w13 + silu")
-            else:
-                self._linear(self.xn, lw["w13"], self.gate_up, B)
-                check(lib.chitu_b200_silu_and_mul(ptr(self.gate_up), ptr(self.act), B, self.F, _lib.CB_BF16, st), "silu")
-            if self.tp_size == 1:
-                self._linear(self.act, lw["w2"], h, B, residual=h2)           # h = w2(act) + h2
-                self._rmsnorm(h, next_norm, self.xn, B)
-            elif self.comm is not None and self.ar_push:
-                self.comm.linear_push(self.act, lw["w2"], B, self.lin_ws)
-                self.comm.consume(h2, h, next_norm, self.xn, None, None, B, cfg.dim, cfg.norm_eps)
-            else:
-                self._linear(self.act, lw["w2"], h, B)
-                reduce_add_norm(h, h2, h, next_norm)
+        # (embedding table replicated per rank here; the reference shards it by vocab + all_reduce)
+        check(lib.chitu_b200_embedding(ptr(self.tokens), ptr(self.embed), ptr(self.h), B, cfg.dim, 0, cfg.vocab_size,
+                                       _lib.CB_BF16, st), "embedding")
+        self._decode_layers()
         self._linear(self.xn, self.head, self.logits, B)          # self.xn = norm(h) already
+        vocab_local = self.head.shape[0]
         check(lib.chitu_b200_argmax(ptr(self.logits), ptr(self.next_tokens), B, vocab_local, _lib.CB_BF16, st),
               "argmax")
-        if self.tp_size > 1:
+        if self.tp_on:
             # vocab-parallel head: the reference all-gathers the logits shards before sampling
             # (tensor_parallel.py:94-102); the same token from a (max, index) all-gather of B*8 bytes per rank
             self.next_tokens.copy_(global_argmax(self.logits, self.next_tokens, self.tp_rank, vocab_local, self.pg,
@@ -299,3 +227,119 @@ class LlamaDecodeEngine:
         self.tokens.copy_(tokens_host, non_blocking=True)
         self.step()
         return self.next_tokens.cpu()
+
+
+class LlamaDecodeEngine(DecodeEngine):
+    """Single-GPU (tp=1) or tensor-parallel LLaMA decode.  Weights are random (`do_load=False`,
+    serve_config.yaml:9).  KV cache layout = PagedKVCacheManager (cache_manager.py:71-87):
+    paged_k_cache / paged_v_cache [L, num_blocks, page, n_local_kv_heads, head_dim], page 256
+    (backend.py:237)."""
+
+    def __init__(self, cfg: LlamaConfig, max_reqs: int, max_seq_len: int, device="cuda:0", page_size: int = 256,
+                 seed: int = 0, tp_rank: int = 0, tp_size: int = 1, process_group=None, linear_impl: int = 0,
+                 use_fused_allreduce: bool = True):
+        D = cfg.head_dim
+        assert cfg.n_heads % tp_size == 0 and cfg.n_kv_heads % tp_size == 0
+        self.Hq, self.Hkv, self.D = cfg.n_heads // tp_size, cfg.n_kv_heads // tp_size, D
+        self.F = cfg.ffn_dim // tp_size
+        self.linear_impl = linear_impl
+        super().__init__(cfg, max_reqs, max_seq_len, device, page_size, seed, tp_rank, tp_size, process_group,
+                         use_fused_allreduce, attn_ws=(self.Hq, D, 64),
+                         lin_n=max(2 * self.F, cfg.vocab_size // tp_size))
+        dev, g, dim = self.device, self.g, cfg.dim
+
+        def rnd(*shape, scale=0.02):
+            return (torch.randn(*shape, generator=g, dtype=torch.float32, device=dev) * scale).to(BF)
+
+        self.embed = (torch.randn(cfg.vocab_size, dim, generator=self.g_rep, dtype=torch.float32, device=dev) * 0.02).to(BF)
+        self.layers = []
+        for _ in range(cfg.n_layers):
+            self.layers.append(dict(
+                attn_norm=torch.ones(dim, dtype=BF, device=dev),
+                ffn_norm=torch.ones(dim, dtype=BF, device=dev),
+                # column-parallel wq|wk|wv merged along N (shards of each concatenated); row-parallel wo
+                wqkv=rnd((self.Hq + 2 * self.Hkv) * D, dim),
+                wo=rnd(dim, self.Hq * D),
+                w13=rnd(2 * self.F, dim),          # [w1 (gate) ; w3 (up)]  (interleaved below when the epilogue fuses SiLU)
+                w2=rnd(dim, self.F),
+            ))
+        self.norm = torch.ones(dim, dtype=BF, device=dev)
+        self.head = rnd(cfg.vocab_size // tp_size, dim)
+        nblk = self.max_blocks * max_reqs
+        self.k_cache = torch.zeros(cfg.n_layers, nblk, page_size, self.Hkv, D, dtype=BF, device=dev)
+        self.v_cache = torch.zeros_like(self.k_cache)
+        self.caches = (self.k_cache, self.v_cache)
+        # precompute_freqs_cis (models/model.py:81-89) as cos/sin tables
+        freqs = 1.0 / (cfg.rope_theta ** (torch.arange(0, D, 2)[: D // 2].float() / D))
+        self._rope_tables(torch.outer(torch.arange(max_seq_len * 2, dtype=torch.float32), freqs))
+        B = max_reqs
+        self.qkv = torch.zeros(B, (self.Hq + 2 * self.Hkv) * D, dtype=BF, device=dev)
+        self.q_rot = torch.zeros(B, self.Hq, D, dtype=BF, device=dev)
+        self.k_rot = torch.zeros(B, self.Hkv, D, dtype=BF, device=dev)
+        self.attn_out = torch.zeros(B, self.Hq * D, dtype=BF, device=dev)
+        self.gate_up = torch.zeros(B, 2 * self.F, dtype=BF, device=dev)
+        self.act = torch.zeros(B, self.F, dtype=BF, device=dev)
+        # SiluAndMul inside the w13 GEMM epilogue: the merged gate/up weight is stored with its rows interleaved
+        # (row 2i = gate_i, row 2i+1 = up_i) — a load-time permutation of the reference's merged tensor.
+        # It and push mode need the wgmma GEMM, which linear_impl=1 (the SIMT GEMV) turns off.
+        self.fuse_silu = linear_impl != 1
+        self.ar_push = self.ar_push and linear_impl != 1
+        if self.fuse_silu:
+            for lw in self.layers:
+                lw["w13"] = lw["w13"].view(2, self.F, dim).transpose(0, 1).reshape(2 * self.F, dim).contiguous()
+        # rotary fused into the tensor-core decode kernel (head dim 128, power-of-two pages)
+        self.fuse_rope = D == 128 and (page_size & (page_size - 1)) == 0 and self.Hq // self.Hkv in (1, 2, 4, 8)
+
+    def ref_layers(self):
+        """The layer weights in the REFERENCE's layout (w13 = [w1 ; w3] halves) for the oracle side of the tests."""
+        out = []
+        for lw in self.layers:
+            d = dict(lw)
+            if self.fuse_silu:
+                d["w13"] = lw["w13"].view(self.F, 2, self.cfg.dim).transpose(0, 1).reshape(2 * self.F, self.cfg.dim).contiguous()
+            out.append(d)
+        return out
+
+    def _decode_layers(self):
+        lib, B, D = self.lib, self.B, self.D
+        st = current_stream()
+        h, h2 = self.h, self.h2
+        qkv_w = (self.Hq + 2 * self.Hkv) * D
+        n_layers = len(self.layers)
+        self._norm(h, self.layers[0]["attn_norm"], self.xn)
+        for li, lw in enumerate(self.layers):
+            next_norm = self.layers[li + 1]["attn_norm"] if li + 1 < n_layers else self.norm
+            self._linear(self.xn, lw["wqkv"], self.qkv, B)
+            q_view, k_view = self.qkv, self.qkv[:, self.Hq * D:]
+            v_view = self.qkv[:, (self.Hq + self.Hkv) * D:]
+            if self.fuse_rope:
+                # rotary (q and the new k) inside the attention kernel: q / k / v are views of the qkv GEMM output
+                check(lib.chitu_b200_gqa_paged_decode_rope(
+                    ptr(q_view), qkv_w, ptr(self.k_cache[li]), ptr(self.v_cache[li]), ptr(k_view), ptr(v_view), qkv_w, qkv_w,
+                    ptr(self.cos), ptr(self.sin), ptr(self.seq_lens), ptr(self.block_table), self.max_blocks, B, self.Hq,
+                    self.Hkv, D, self.page, self.max_seq_len, 1.0 / math.sqrt(D), ptr(self.attn_out), ptr(self.attn_ws),
+                    self.attn_ws.numel(), _lib.CB_BF16, st), "gqa_paged_decode_rope")
+            else:
+                check(lib.chitu_b200_rotary_interleaved(ptr(q_view), ptr(k_view), ptr(self.q_rot), ptr(self.k_rot),
+                                                        ptr(self.cos), ptr(self.sin), B, self.Hq, self.Hkv, D, qkv_w, D,
+                                                        qkv_w, D, _lib.CB_BF16, st), "rotary")
+                check(lib.chitu_b200_gqa_paged_decode(
+                    ptr(self.q_rot), ptr(self.k_cache[li]), ptr(self.v_cache[li]), ptr(self.k_rot), ptr(v_view),
+                    self.Hkv * D, qkv_w, ptr(self.seq_lens), ptr(self.block_table), self.max_blocks, B, self.Hq,
+                    self.Hkv, D, self.page, self.max_seq_len, 1.0 / math.sqrt(D), ptr(self.attn_out), ptr(self.attn_ws),
+                    self.attn_ws.numel(), _lib.CB_BF16, st), "gqa_paged_decode")
+            # h2 = wo(o) + h
+            self._row_parallel(lambda out, res: self._linear(self.attn_out, lw["wo"], out, B, residual=res),
+                               lambda: self.comm.linear_push(self.attn_out, lw["wo"], B, self.lin_ws),
+                               h, h2, lw["ffn_norm"], y=self.xn)
+            if self.fuse_silu:
+                check(lib.chitu_b200_linear_bf16_silu_pairs(ptr(self.xn), ptr(lw["w13"]), ptr(self.act), B, 2 * self.F,
+                                                            self.cfg.dim, ptr(self.lin_ws), self.lin_ws.numel(), st),
+                      "w13 + silu")
+            else:
+                self._linear(self.xn, lw["w13"], self.gate_up, B)
+                check(lib.chitu_b200_silu_and_mul(ptr(self.gate_up), ptr(self.act), B, self.F, _lib.CB_BF16, st), "silu")
+            # h = w2(act) + h2
+            self._row_parallel(lambda out, res: self._linear(self.act, lw["w2"], out, B, residual=res),
+                               lambda: self.comm.linear_push(self.act, lw["w2"], B, self.lin_ws),
+                               h2, h, next_norm, y=self.xn)

@@ -20,7 +20,7 @@ import torch
 
 from . import _lib
 from ._lib import check, current_stream, ptr
-from .tensor_parallel import global_argmax
+from .engine import DecodeEngine
 
 BF = torch.bfloat16
 F8 = torch.float8_e4m3fn
@@ -95,26 +95,25 @@ def yarn_freqs(cfg: DeepSeekConfig, max_pos: int) -> torch.Tensor:
     return torch.outer(torch.arange(max_pos, dtype=torch.float32), freqs)
 
 
-class DeepSeekDecodeEngine:
+class DeepSeekDecodeEngine(DecodeEngine):
     def __init__(self, cfg: DeepSeekConfig, max_reqs: int, max_seq_len: int, device="cuda:0", seed: int = 0,
                  tp_rank: int = 0, tp_size: int = 8, process_group=None, page_size: int = 64,
-                 cache_dequant_wkv_b: bool = True, use_fused_allreduce: bool = True):
-        self.cfg, self.B, self.device = cfg, max_reqs, torch.device(device)
-        self.tp_rank, self.tp_size, self.pg = tp_rank, tp_size, process_group
-        self.lib = _lib.load()
-        self.page = page_size                          # backend.py:234-237: paged + absorb => 64
+                 use_fused_allreduce: bool = True):
         c = cfg
         T = tp_size
         assert c.n_heads % T == 0
+        # the MLA kernels stage 64-token pages of a 512 + 64 wide latent; absorb-o quantises one 128-wide head per
+        # act_quant group
+        assert page_size == 64 and c.kv_lora_rank == 512 and c.qk_rope_head_dim == 64 and c.v_head_dim == 128, \
+            "the MLA decode kernels are built for page 64, kv_lora_rank 512, qk_rope_head_dim 64, v_head_dim 128"
         self.H = c.n_heads // T
         self.qk_head = c.qk_nope_head_dim + c.qk_rope_head_dim
         self.C, self.R = c.kv_lora_rank, c.qk_rope_head_dim
         self.F_dense = c.inter_dim // T
         self.F_moe = c.moe_inter_dim // T
-        self.cache_dequant = cache_dequant_wkv_b
-        dev = self.device
-        g = torch.Generator(device=dev).manual_seed(seed + 1000 * tp_rank)
-        g_rep = torch.Generator(device=dev).manual_seed(seed + 7)        # replicated weights: same on all ranks
+        super().__init__(cfg, max_reqs, max_seq_len, device, page_size, seed, tp_rank, tp_size, process_group,
+                         use_fused_allreduce, attn_ws=(self.H, self.C, 128), lin_n=max(c.vocab_size // T, c.dim))
+        dev, g, g_rep = self.device, self.g, self.g_rep
 
         def rnd(gen, *shape, scale=0.02):
             return torch.randn(*shape, generator=gen, dtype=torch.float32, device=dev) * scale
@@ -153,25 +152,18 @@ class DeepSeekDecodeEngine:
                 L["we2"], L["we2_s"] = fp8(g, c.n_routed_experts + 1, dim, self.F_moe)
                 L["ws13"], L["ws13_s"] = L["we1"][-1], L["we1_s"][-1]      # views (used by the tests)
                 L["ws2"], L["ws2_s"] = L["we2"][-1], L["we2_s"][-1]
-            if self.cache_dequant:
-                # SURVEY §8f n1: dequantise wkv_b once instead of every step (model_deepseek_v3.py:516-528)
-                L["wkv_b_bf16"] = self._dequant(L["wkv_b"], L["wkv_b_s"])
+            # SURVEY §8f n1: dequantise wkv_b once instead of every step (model_deepseek_v3.py:516-528)
+            L["wkv_b_bf16"] = self._dequant(L["wkv_b"], L["wkv_b_s"])
             self.layers.append(L)
         self.norm = torch.ones(dim, dtype=BF, device=dev)
         self.head = rnd(g, c.vocab_size // T, dim).to(BF)
         # paged MLA cache: [L, num_blocks, 64, 576], replicated on every rank (cache_manager.py:71-76)
-        self.max_blocks = max_seq_len // page_size + 1
         nblk = self.max_blocks * max_reqs
         self.kv_cache = torch.zeros(c.n_layers, nblk, page_size, self.C + self.R, dtype=BF, device=dev)
-        self.block_table = torch.zeros(max_reqs, self.max_blocks, dtype=torch.int32, device=dev)
-        self.seq_lens = torch.zeros(max_reqs, dtype=torch.int32, device=dev)
-        ang = yarn_freqs(c, max_seq_len * 2)
-        self.cos_table, self.sin_table = ang.cos().to(dev), ang.sin().to(dev)
+        self.caches = (self.kv_cache,)
+        self._rope_tables(yarn_freqs(c, max_seq_len * 2))
         B = max_reqs
         z = lambda *s, dt=BF: torch.zeros(*s, dtype=dt, device=dev)
-        self.tokens = torch.zeros(B, dtype=torch.int64, device=dev)
-        self.cos, self.sin = z(B, self.R // 2, dt=torch.float32), z(B, self.R // 2, dt=torch.float32)
-        self.h, self.h2, self.xn = z(B, dim), z(B, dim), z(B, dim)
         kmax = max(dim, self.F_dense, self.H * c.v_head_dim, c.q_lora_rank)
         self.xq = torch.zeros(B, kmax, dtype=F8, device=dev)
         self.xs = z(B, kmax // 128 + 1, dt=torch.float32)
@@ -183,10 +175,9 @@ class DeepSeekDecodeEngine:
         self.new_kv = z(B, self.C + self.R)
         self.o_lat = z(B, self.H, self.C)
         self.o = z(B, self.H * c.v_head_dim)
-        self.wkv_tmp = z(self.H * (c.qk_nope_head_dim + c.v_head_dim), self.C)
         self.ff = z(B, 2 * max(self.F_dense, self.F_moe))
         self.act = z(B, max(self.F_dense, self.F_moe))
-        self.y, self.y1 = z(B, dim), z(B, dim)
+        self.y = z(B, dim)
         # routing results of every layer stay resident (bench.py counts the distinct experts per layer)
         # one extra slot per token = the shared expert (id n_routed_experts, weight 1): it rides through the
         # grouped expert GEMM instead of five separate launches
@@ -195,31 +186,12 @@ class DeepSeekDecodeEngine:
         self.gate_i_all = torch.zeros(c.n_layers, B, self.topk1, dtype=torch.int64, device=dev)
         self.gate_w_all[..., -1] = 1.0
         self.gate_i_all[..., -1] = c.n_routed_experts
-        self.logits = z(B, c.vocab_size // T)
-        self.next_tokens = torch.zeros(B, dtype=torch.int64, device=dev)
-        self.tp_gather = (torch.empty(self.tp_size, B, 2, dtype=torch.float32, device=dev)
-                          if (self.pg is not None and self.tp_size > 1) else None)
         lib = self.lib
-        self.attn_ws = torch.zeros(lib.chitu_b200_attn_workspace_bytes(B, self.H, self.C, 128), dtype=torch.uint8, device=dev)
-        self.lin_ws = torch.zeros(max(lib.chitu_b200_linear_workspace_bytes(B, max(c.vocab_size // T, dim)), 256),
-                                  dtype=torch.uint8, device=dev)
         self.moe_ws = torch.zeros(lib.chitu_b200_moe_workspace_bytes(B, self.topk1, c.n_routed_experts + 1,
                                                                      2 * self.F_moe, dim), dtype=torch.uint8, device=dev)
         self.gate_ws = torch.zeros(lib.chitu_b200_moe_gate_workspace_bytes(B, c.n_routed_experts), dtype=torch.uint8, device=dev)
-        self.max_seq_len = max_seq_len
-        # the wgmma MLA kernel can leave its split-KV partials for the absorb-o kernel to merge (one launch fewer)
-        import os
-        self.defer_merge = page_size == 64 and c.v_head_dim == 128 and self.C == 512
-        self.ar_push = os.environ.get("CHITU_B200_AR_PUSH", "1") != "0"
-        self.graph = None
-        self.launches_per_step = 0
         self.trace = None          # set to [] to record per-layer intermediates (tests; not under CUDA graphs)
         self.capture_h = None      # set to [] to record the residual stream at every layer boundary of the FAST path
-        # fused one-shot all-reduce + residual + RMSNorm(+quant) over NVLink peer memory; NCCL otherwise
-        self.comm = None
-        if tp_size > 1 and process_group is not None and use_fused_allreduce:
-            from .comm import FusedAllReduce
-            self.comm = FusedAllReduce(process_group, max_reqs, dim, self.device)
 
     # ---- helpers -----------------------------------------------------------------------------------
     def _dequant(self, w, s):
@@ -237,75 +209,77 @@ class DeepSeekDecodeEngine:
         check(self.lib.chitu_b200_rmsnorm_quant_fp8(ptr(x), ptr(w), ptr(y), ptr(self.xq), ptr(self.xs), rows, dim,
                                                     xs or dim, dim, self.cfg.norm_eps, current_stream()), "rmsnorm_quant")
 
+    def _norm(self, x, w, y=None, q=None, qs=None):
+        """RMSNorm of the residual stream into bf16 `y` and / or the fp8 activations `q` + scales `qs`."""
+        c = self.cfg
+        check(self.lib.chitu_b200_rmsnorm_quant_fp8(ptr(x), ptr(w), ptr(y), ptr(q), ptr(qs), self.B, c.dim, c.dim, c.dim,
+                                                    c.norm_eps, current_stream()), "rmsnorm_quant")
+
+    def _norm_out(self, bf16: bool):
+        """The norm outputs the next consumer reads: bf16 for the MoE gate / experts and the head, fp8 for a GEMM."""
+        return dict(y=self.xn) if bf16 else dict(q=self.xq, qs=self.xs)
+
     def _fp8_gemm(self, w, w_s, y, M, residual=None):
         """fp8_gemm_deepseek_v3 on the already quantised activations in self.xq / self.xs."""
         N, K = w.shape
         check(self.lib.chitu_b200_fp8_gemm(ptr(self.xq), ptr(self.xs), ptr(w), ptr(w_s), ptr(y), M, N, K, ptr(residual),
                                            ptr(self.lin_ws), self.lin_ws.numel(), 0, current_stream()), "fp8_gemm")
 
-    def _allreduce(self, t):
-        if self.pg is not None and self.tp_size > 1:
-            torch.distributed.all_reduce(t, group=self.pg)
-
     def _add(self, a, b, y):
         check(self.lib.chitu_b200_add(ptr(a), ptr(b), ptr(y), a.numel(), _lib.CB_BF16, current_stream()), "add")
 
-    def set_synthetic_context(self, seq_len: int, seed: int = 2):
-        g = torch.Generator(device="cpu").manual_seed(seed)
-        gd = torch.Generator(device=self.device).manual_seed(seed + 11)     # deterministic cache contents
-        nblk = self.kv_cache.shape[1]
-        self.block_table.copy_(torch.randperm(nblk, generator=g).to(torch.int32).view(self.B, self.max_blocks))
-        self.seq_lens.fill_(seq_len)
-        for l in range(self.cfg.n_layers):
-            self.kv_cache[l].normal_(0, 1, generator=gd)
+    def _moe_gate(self, li):
+        c, L = self.cfg, self.layers[li]
+        check(self.lib.chitu_b200_moe_gate(ptr(self.xn), ptr(L["gate_w"]), ptr(L["gate_b"]), _lib.CB_F32, self.B, c.dim,
+                                           c.n_routed_experts, c.n_expert_groups, c.n_limited_groups,
+                                           c.n_activated_experts, 1 if c.score_func == "sigmoid" else 0,
+                                           float(c.route_scale), ptr(self.gate_w_all[li]), ptr(self.gate_i_all[li]),
+                                           self.topk1, ptr(self.gate_ws), self.gate_ws.numel(), current_stream()),
+              "moe_gate")
+
+    def _fused_experts(self, li, out, residual):
+        """shared expert (model_deepseek_v3.py:936-949) + routed experts (fused_experts, :995-1009) in ONE grouped fp8
+        GEMM pass: the shared expert is slot `topk` of every token with weight 1"""
+        c, L = self.cfg, self.layers[li]
+        check(self.lib.chitu_b200_fused_experts(
+            ptr(self.xn), ptr(L["we1"]), ptr(L["we2"]), ptr(L["we1_s"]), ptr(L["we2_s"]), ptr(self.gate_w_all[li]),
+            _lib.CB_BF16, ptr(self.gate_i_all[li]), _lib.CB_I64, self.B, self.topk1, c.n_routed_experts + 1,
+            2 * self.F_moe, c.dim, 1, ptr(out), ptr(residual), ptr(self.moe_ws), self.moe_ws.numel(), current_stream()),
+            "fused_experts")
+
+    def _mla_prep(self, li):
+        """rotary(q_pe, k_pe) + kv_norm + cat + W_UK absorption in one launch"""
+        c, L = self.cfg, self.layers[li]
+        check(self.lib.chitu_b200_mla_prep(ptr(self.q), ptr(self.qkv_a[:, c.q_lora_rank:]), c.q_lora_rank + self.C + self.R,
+                                           ptr(L["kv_norm"]), ptr(self.cos), ptr(self.sin), ptr(L["wkv_b_bf16"]),
+                                           ptr(self.q_abs), ptr(self.q_pe), ptr(self.new_kv), self.B, self.H,
+                                           c.qk_nope_head_dim, c.v_head_dim, self.C, self.R, c.norm_eps, current_stream()),
+              "mla_prep")
+
+    def _mla_decode(self, li, out):
+        """paged absorbed-MLA decode, appending new_kv; out = None leaves the split-KV partials in the workspace"""
+        check(self.lib.chitu_b200_mla_decode(ptr(self.q_abs), ptr(self.q_pe), ptr(self.kv_cache[li]), ptr(self.new_kv),
+                                             ptr(self.seq_lens), ptr(self.block_table), self.max_blocks, self.B, self.H,
+                                             self.C, self.R, self.page, self.kv_cache.shape[1], self.max_seq_len,
+                                             float(self.cfg.softmax_scale), ptr(out), ptr(self.attn_ws),
+                                             self.attn_ws.numel(), current_stream()), "mla_decode")
 
     # ---- one decode step ---------------------------------------------------------------------------
-    def _step_body(self):
+    def _decode_layers(self):
         if self.trace is None:
-            return self._step_body_fast()
-        return self._step_body_traced()
+            self._layers_fast()
+        else:
+            self._layers_traced()
 
-    def _step_body_fast(self):
+    def _layers_fast(self):
         """Production flow: every RMSNorm is fused either into the collective that precedes it (tensor parallel:
         all-reduce + residual + norm + quant in one kernel) or into a norm+quant kernel; residual adds ride in
-        the GEMM / expert-combine epilogues.  Arithmetic is identical to `_step_body_traced`."""
+        the GEMM / expert-combine epilogues.  Arithmetic is identical to `_layers_traced`."""
         lib, B, c = self.lib, self.B, self.cfg
         st = current_stream()
-        H, C, R, dn, dv = self.H, self.C, self.R, c.qk_nope_head_dim, c.v_head_dim
-        tp_on = self.pg is not None and self.tp_size > 1
-        torch.index_select(self.cos_table, 0, self.seq_lens, out=self.cos)
-        torch.index_select(self.sin_table, 0, self.seq_lens, out=self.sin)
-        check(lib.chitu_b200_embedding(ptr(self.tokens), ptr(self.embed), ptr(self.h), B, c.dim, 0, c.vocab_size,
-                                       _lib.CB_BF16, st), "embedding")
         h, h2 = self.h, self.h2
-        qa_w = c.q_lora_rank + C + R
         n_layers = len(self.layers)
-
-        def reduce_add_norm(partial, residual, h_out, norm_w, want_y, want_q):
-            """h_out = all_reduce(partial) + residual; then RMSNorm(h_out)*norm_w -> self.xn (bf16) and/or xq/xs (fp8)"""
-            y = self.xn if want_y else None
-            if self.comm is not None:
-                self.comm(partial, residual, h_out, norm_w, y, self.xq if want_q else None, self.xs if want_q else None,
-                          B, c.dim, c.norm_eps)
-            else:
-                self._allreduce(partial)
-                self._add(partial, residual, h_out)
-                check(lib.chitu_b200_rmsnorm_quant_fp8(ptr(h_out), ptr(norm_w), ptr(y), ptr(self.xq) if want_q else None,
-                                                       ptr(self.xs) if want_q else None, B, c.dim, c.dim, c.dim,
-                                                       c.norm_eps, st), "rmsnorm_quant")
-
-        def consume(residual, h_out, norm_w, want_y, want_q):
-            """push-mode reduce: h_out = sum over ranks of the pushed partials + residual, then the fused norm (+ quant)"""
-            self.comm.consume(residual, h_out, norm_w, self.xn if want_y else None, self.xq if want_q else None,
-                              self.xs if want_q else None, B, c.dim, c.norm_eps)
-        push = tp_on and self.comm is not None and self.ar_push
-
-        def norm_only(x, norm_w, want_y, want_q):
-            check(lib.chitu_b200_rmsnorm_quant_fp8(ptr(x), ptr(norm_w), ptr(self.xn) if want_y else None,
-                                                   ptr(self.xq) if want_q else None, ptr(self.xs) if want_q else None,
-                                                   B, c.dim, c.dim, c.dim, c.norm_eps, st), "rmsnorm_quant")
-
-        norm_only(h, self.layers[0]["attn_norm"], False, True)
+        self._norm(h, self.layers[0]["attn_norm"], **self._norm_out(False))
         for li, L in enumerate(self.layers):
             if self.capture_h is not None:       # tests: the residual stream entering every layer (never under a graph)
                 self.capture_h.append(h.clone())
@@ -314,229 +288,89 @@ class DeepSeekDecodeEngine:
             is_moe = li >= c.n_dense_layers
             # ---------------- attention ----------------
             self._fp8_gemm(L["wqkv_a"], L["wqkv_a_s"], self.qkv_a, B)
-            self._rms_quant(self.qkv_a, L["q_norm"], c.q_lora_rank, B, xs=qa_w)
+            self._rms_quant(self.qkv_a, L["q_norm"], c.q_lora_rank, B, xs=c.q_lora_rank + self.C + self.R)
             self._fp8_gemm(L["wq_b"], L["wq_b_s"], self.q, B)
-            if self.cache_dequant:
-                wkv = L["wkv_b_bf16"]
-            else:
-                check(lib.chitu_b200_weight_dequant_fp8(ptr(L["wkv_b"]), ptr(L["wkv_b_s"]), ptr(self.wkv_tmp), 1,
-                                                        self.wkv_tmp.shape[0], C, 128, 0, st), "wkv_b dequant")
-                wkv = self.wkv_tmp
-            check(lib.chitu_b200_mla_prep(ptr(self.q), ptr(self.qkv_a[:, c.q_lora_rank:]), qa_w, ptr(L["kv_norm"]),
-                                          ptr(self.cos), ptr(self.sin), ptr(wkv), ptr(self.q_abs), ptr(self.q_pe),
-                                          ptr(self.new_kv), B, H, dn, dv, C, R, c.norm_eps, st), "mla_prep")
-            if self.defer_merge:
-                # split-KV partials stay in the workspace; the LSE merge happens inside the absorb-o kernel
-                check(lib.chitu_b200_mla_decode(ptr(self.q_abs), ptr(self.q_pe), ptr(self.kv_cache[li]), ptr(self.new_kv),
-                                                ptr(self.seq_lens), ptr(self.block_table), self.max_blocks, B, H, C, R,
-                                                self.page, self.kv_cache.shape[1], self.max_seq_len, float(c.softmax_scale),
-                                                None, ptr(self.attn_ws), self.attn_ws.numel(), st), "mla_decode")
-                check(lib.chitu_b200_mla_absorb_o_merge_quant(ptr(self.attn_ws), self.attn_ws.numel(), self.max_seq_len,
-                                                              ptr(wkv), None, None, ptr(self.xq), ptr(self.xs), B, H, dn, dv,
-                                                              C, st), "absorb_o_merge")
-            else:
-                check(lib.chitu_b200_mla_decode(ptr(self.q_abs), ptr(self.q_pe), ptr(self.kv_cache[li]), ptr(self.new_kv),
-                                                ptr(self.seq_lens), ptr(self.block_table), self.max_blocks, B, H, C, R,
-                                                self.page, self.kv_cache.shape[1], self.max_seq_len, float(c.softmax_scale),
-                                                ptr(self.o_lat), ptr(self.attn_ws), self.attn_ws.numel(), st), "mla_decode")
-                check(lib.chitu_b200_mla_absorb_o_quant(ptr(self.o_lat), ptr(wkv), None, ptr(self.xq), ptr(self.xs), B, H, dn,
-                                                        dv, C, st), "absorb_o")
+            self._mla_prep(li)
+            # split-KV partials stay in the workspace; the LSE merge happens inside the absorb-o kernel
+            self._mla_decode(li, None)
+            check(lib.chitu_b200_mla_absorb_o_merge_quant(ptr(self.attn_ws), self.attn_ws.numel(), self.max_seq_len,
+                                                          ptr(L["wkv_b_bf16"]), None, None, ptr(self.xq), ptr(self.xs),
+                                                          B, self.H, c.qk_nope_head_dim, c.v_head_dim, self.C, st),
+                  "absorb_o_merge")
             # the ffn_norm output is needed in bf16 by the gate / expert gather (MoE) and in fp8 by the dense FFN
-            if push:
-                self.comm.fp8_gemm_push(self.xq, self.xs, L["wo"], L["wo_s"], B, self.lin_ws)
-                consume(h, h2, L["ffn_norm"], is_moe, not is_moe)
-            elif tp_on:
-                self._fp8_gemm(L["wo"], L["wo_s"], h2, B)
-                reduce_add_norm(h2, h, h2, L["ffn_norm"], want_y=is_moe, want_q=not is_moe)
-            else:
-                self._fp8_gemm(L["wo"], L["wo_s"], h2, B, residual=h)
-                norm_only(h2, L["ffn_norm"], is_moe, not is_moe)
+            self._row_parallel(lambda out, res: self._fp8_gemm(L["wo"], L["wo_s"], out, B, residual=res),
+                               lambda: self.comm.fp8_gemm_push(self.xq, self.xs, L["wo"], L["wo_s"], B, self.lin_ws),
+                               h, h2, L["ffn_norm"], **self._norm_out(is_moe))
             # ---------------- FFN ----------------
             if not is_moe:
                 self._fp8_gemm(L["w13"], L["w13_s"], self.ff, B)
                 check(lib.chitu_b200_silu_mul_quant_fp8(ptr(self.ff), ptr(self.xq), ptr(self.xs), B, self.F_dense, st),
                       "silu_quant")
-                if push:
-                    self.comm.fp8_gemm_push(self.xq, self.xs, L["w2"], L["w2_s"], B, self.lin_ws)
-                    consume(h2, h, next_norm, last, not last)
-                elif tp_on:
-                    self._fp8_gemm(L["w2"], L["w2_s"], self.y, B)
-                    reduce_add_norm(self.y, h2, h, next_norm, want_y=last, want_q=not last)
-                else:
-                    self._fp8_gemm(L["w2"], L["w2_s"], h, B, residual=h2)
-                    norm_only(h, next_norm, last, not last)
+                self._row_parallel(lambda out, res: self._fp8_gemm(L["w2"], L["w2_s"], out, B, residual=res),
+                                   lambda: self.comm.fp8_gemm_push(self.xq, self.xs, L["w2"], L["w2_s"], B, self.lin_ws),
+                                   h2, h, next_norm, partial=self.y, **self._norm_out(last))
             else:
-                E1 = c.n_routed_experts + 1
-                check(lib.chitu_b200_moe_gate(ptr(self.xn), ptr(L["gate_w"]), ptr(L["gate_b"]), _lib.CB_F32, B, c.dim,
-                                              c.n_routed_experts, c.n_expert_groups, c.n_limited_groups,
-                                              c.n_activated_experts, 1 if c.score_func == "sigmoid" else 0,
-                                              float(c.route_scale), ptr(self.gate_w_all[li]), ptr(self.gate_i_all[li]),
-                                              self.topk1, ptr(self.gate_ws), self.gate_ws.numel(), st), "moe_gate")
-                if push:
-                    self.comm.experts_push(self.xn, L["we1"], L["we2"], L["we1_s"], L["we2_s"], self.gate_w_all[li], _lib.CB_BF16,
-                                               self.gate_i_all[li], _lib.CB_I64, B, self.topk1, E1,
-                                               2 * self.F_moe, c.dim, 1, self.moe_ws)
-                    consume(h2, h, next_norm, last, not last)
-                else:
-                    check(lib.chitu_b200_fused_experts(
-                        ptr(self.xn), ptr(L["we1"]), ptr(L["we2"]), ptr(L["we1_s"]), ptr(L["we2_s"]), ptr(self.gate_w_all[li]),
-                        _lib.CB_BF16, ptr(self.gate_i_all[li]), _lib.CB_I64, B, self.topk1, E1,
-                        2 * self.F_moe, c.dim, 1, ptr(self.y if tp_on else h), None if tp_on else ptr(h2), ptr(self.moe_ws),
-                        self.moe_ws.numel(), st), "fused_experts")
-                    if tp_on:
-                        reduce_add_norm(self.y, h2, h, next_norm, want_y=last, want_q=not last)
-                    else:
-                        norm_only(h, next_norm, last, not last)
+                self._moe_gate(li)
+                self._row_parallel(lambda out, res: self._fused_experts(li, out, res),
+                                   lambda: self.comm.experts_push(self.xn, L["we1"], L["we2"], L["we1_s"], L["we2_s"],
+                                                                  self.gate_w_all[li], _lib.CB_BF16, self.gate_i_all[li],
+                                                                  _lib.CB_I64, B, self.topk1, c.n_routed_experts + 1,
+                                                                  2 * self.F_moe, c.dim, 1, self.moe_ws),
+                                   h2, h, next_norm, partial=self.y, **self._norm_out(last))
         if self.capture_h is not None:
             self.capture_h.append(h.clone())
-        N, K = self.head.shape
-        check(lib.chitu_b200_linear_bf16(ptr(self.xn), ptr(self.head), None, None, ptr(self.logits), B, N, K,
-                                         _lib.CB_BF16, ptr(self.lin_ws), self.lin_ws.numel(), 0, st), "head")
-        check(lib.chitu_b200_argmax(ptr(self.logits), ptr(self.next_tokens), B, N, _lib.CB_BF16, st), "argmax")
-        if self.pg is not None and self.tp_size > 1:
-            # vocab-parallel head: the reference all-gathers the logits shards before sampling
-            # (tensor_parallel.py:94-102); the same token from a (max, index) all-gather of B*8 bytes per rank
-            self.next_tokens.copy_(global_argmax(self.logits, self.next_tokens, self.tp_rank, N, self.pg, self.tp_gather))
-        self.seq_lens.add_(1)
 
-    def _step_body_traced(self):
+    def _layers_traced(self):
+        """The unfused flow, recording the intermediates of every layer into a new dict in self.trace (the
+        stage-by-stage test compares each with the oracle): the attention output lands in o_lat before absorb-o, an
+        extra SiLU launch exposes the dense FFN activation, and the residual adds and all-reduces run outside the GEMMs."""
         lib, B, c = self.lib, self.B, self.cfg
         st = current_stream()
-        H, C, R, dn, dv = self.H, self.C, self.R, c.qk_nope_head_dim, c.v_head_dim
-        torch.index_select(self.cos_table, 0, self.seq_lens, out=self.cos)
-        torch.index_select(self.sin_table, 0, self.seq_lens, out=self.sin)
-        check(lib.chitu_b200_embedding(ptr(self.tokens), ptr(self.embed), ptr(self.h), B, c.dim, 0, c.vocab_size,
-                                       _lib.CB_BF16, st), "embedding")
-        # (embedding table replicated per rank here; the reference shards it by vocab + all_reduce)
         h, h2 = self.h, self.h2
-        qa_w = c.q_lora_rank + C + R
         for li, L in enumerate(self.layers):
-            tr = None
-            if self.trace is not None:
-                tr = {}
-                self.trace.append(tr)
-                tr["h_in"] = h.clone()
+            tr = {"h_in": h.clone()}
+            self.trace.append(tr)
             # ---------------- attention (decode_forward_paged, :672-699) ----------------
-            tp_on = self.pg is not None and self.tp_size > 1
-            self._rms_quant(h, L["attn_norm"], c.dim, B, y=self.xn if tr is not None else None)
-            if tr is not None: tr["xn_attn"] = self.xn.clone()
+            self._rms_quant(h, L["attn_norm"], c.dim, B, y=self.xn)
+            tr["xn_attn"] = self.xn.clone()
             self._fp8_gemm(L["wqkv_a"], L["wqkv_a_s"], self.qkv_a, B)
-            if tr is not None: tr["qkv_a"] = self.qkv_a.clone()
-            self._rms_quant(self.qkv_a, L["q_norm"], c.q_lora_rank, B, xs=qa_w, y=self.qa_n if tr is not None else None)
-            if tr is not None: tr["qa_n"] = self.qa_n.clone()
+            tr["qkv_a"] = self.qkv_a.clone()
+            self._rms_quant(self.qkv_a, L["q_norm"], c.q_lora_rank, B, xs=c.q_lora_rank + self.C + self.R, y=self.qa_n)
+            tr["qa_n"] = self.qa_n.clone()
             self._fp8_gemm(L["wq_b"], L["wq_b_s"], self.q, B)
-            if tr is not None: tr["q"] = self.q.clone()
-            if self.cache_dequant:
-                wkv = L["wkv_b_bf16"]
-            else:
-                check(lib.chitu_b200_weight_dequant_fp8(ptr(L["wkv_b"]), ptr(L["wkv_b_s"]), ptr(self.wkv_tmp), 1,
-                                                        self.wkv_tmp.shape[0], C, 128, 0, st), "wkv_b dequant")
-                wkv = self.wkv_tmp
-            # rotary(q_pe, k_pe) + kv_norm + cat + W_UK absorption in one launch
-            check(lib.chitu_b200_mla_prep(ptr(self.q), ptr(self.qkv_a[:, c.q_lora_rank:]), qa_w, ptr(L["kv_norm"]),
-                                          ptr(self.cos), ptr(self.sin), ptr(wkv), ptr(self.q_abs), ptr(self.q_pe),
-                                          ptr(self.new_kv), B, H, dn, dv, C, R, c.norm_eps, st), "mla_prep")
-            if tr is not None: tr["q_pe"] = self.q_pe.clone()
-            if tr is not None: tr["q_abs"] = self.q_abs.clone()
-            if tr is not None: tr["new_kv"] = self.new_kv.clone()
-            if tr is not None: tr["cache_before"] = self.kv_cache[li].clone(); tr["lens"] = self.seq_lens.clone()
-            check(lib.chitu_b200_mla_decode(ptr(self.q_abs), ptr(self.q_pe), ptr(self.kv_cache[li]), ptr(self.new_kv),
-                                            ptr(self.seq_lens), ptr(self.block_table), self.max_blocks, B, H, C, R,
-                                            self.page, self.kv_cache.shape[1], self.max_seq_len, float(c.softmax_scale), ptr(self.o_lat),
-                                            ptr(self.attn_ws), self.attn_ws.numel(), st), "mla_decode")
+            tr["q"] = self.q.clone()
+            self._mla_prep(li)
+            tr["q_pe"], tr["q_abs"], tr["new_kv"] = self.q_pe.clone(), self.q_abs.clone(), self.new_kv.clone()
+            tr["cache_before"], tr["lens"] = self.kv_cache[li].clone(), self.seq_lens.clone()
+            self._mla_decode(li, self.o_lat)
             # absorb_o fused with the act_quant of the `wo` linear (one head = one 128-wide group)
-            check(lib.chitu_b200_mla_absorb_o_quant(ptr(self.o_lat), ptr(wkv), ptr(self.o) if tr is not None else None,
-                                                    ptr(self.xq), ptr(self.xs), B, H, dn, dv, C, st), "absorb_o")
-            if tr is not None: tr["o_lat"] = self.o_lat.clone()
-            if tr is not None: tr["o"] = self.o.clone()
-            if tp_on or tr is not None:
-                self._fp8_gemm(L["wo"], L["wo_s"], h2, B)
-                if tr is not None: tr["attn_out"] = h2.clone()
-                self._allreduce(h2)
-                self._add(h2, h, h2)                                # x = x + attn(...)
-            else:
-                self._fp8_gemm(L["wo"], L["wo_s"], h2, B, residual=h)      # residual fused in the epilogue
-            if tr is not None: tr["h_mid"] = h2.clone()
+            check(lib.chitu_b200_mla_absorb_o_quant(ptr(self.o_lat), ptr(L["wkv_b_bf16"]), ptr(self.o), ptr(self.xq),
+                                                    ptr(self.xs), B, self.H, c.qk_nope_head_dim, c.v_head_dim, self.C, st),
+                  "absorb_o")
+            tr["o_lat"], tr["o"] = self.o_lat.clone(), self.o.clone()
+            self._fp8_gemm(L["wo"], L["wo_s"], h2, B)
+            tr["attn_out"] = h2.clone()
+            self._allreduce(h2)
+            self._add(h2, h, h2)                                # x = x + attn(...)
+            tr["h_mid"] = h2.clone()
             # ---------------- FFN ----------------
             self._rms_quant(h2, L["ffn_norm"], c.dim, B, y=self.xn)         # bf16 copy feeds the gate / experts
-            if tr is not None: tr["xn_ffn"] = self.xn.clone()
+            tr["xn_ffn"] = self.xn.clone()
             if li < c.n_dense_layers:
-                F = self.F_dense
                 self._fp8_gemm(L["w13"], L["w13_s"], self.ff, B)
-                if tr is not None:
-                    check(lib.chitu_b200_silu_and_mul(ptr(self.ff), ptr(self.act), B, F, _lib.CB_BF16, st), "silu")
-                    tr["ff"] = self.ff.clone(); tr["act"] = self.act.clone()
-                check(lib.chitu_b200_silu_mul_quant_fp8(ptr(self.ff), ptr(self.xq), ptr(self.xs), B, F, st), "silu_quant")
-                if tp_on or tr is not None:
-                    self._fp8_gemm(L["w2"], L["w2_s"], self.y, B)
-                    if tr is not None: tr["y"] = self.y.clone()
-                    self._allreduce(self.y)
-                    self._add(self.y, h2, h)                        # x = x + ffn(...)
-                else:
-                    self._fp8_gemm(L["w2"], L["w2_s"], h, B, residual=h2)
+                check(lib.chitu_b200_silu_and_mul(ptr(self.ff), ptr(self.act), B, self.F_dense, _lib.CB_BF16, st), "silu")
+                tr["ff"], tr["act"] = self.ff.clone(), self.act.clone()
+                check(lib.chitu_b200_silu_mul_quant_fp8(ptr(self.ff), ptr(self.xq), ptr(self.xs), B, self.F_dense, st),
+                      "silu_quant")
+                self._fp8_gemm(L["w2"], L["w2_s"], self.y, B)
             else:
-                F = self.F_moe
-                check(lib.chitu_b200_moe_gate(ptr(self.xn), ptr(L["gate_w"]), ptr(L["gate_b"]), _lib.CB_F32, B, c.dim,
-                                              c.n_routed_experts, c.n_expert_groups, c.n_limited_groups,
-                                              c.n_activated_experts, 1 if c.score_func == "sigmoid" else 0,
-                                              float(c.route_scale), ptr(self.gate_w_all[li]), ptr(self.gate_i_all[li]),
-                                              self.topk1, ptr(self.gate_ws), self.gate_ws.numel(), st),
-                      "moe_gate")
-                # shared expert (model_deepseek_v3.py:936-949) + routed experts (fused_experts, :995-1009) in ONE
-                # grouped fp8 GEMM pass: the shared expert is slot `topk` of every token with weight 1
-                fuse_res = not (tp_on or tr is not None)
-                check(lib.chitu_b200_fused_experts(
-                    ptr(self.xn), ptr(L["we1"]), ptr(L["we2"]), ptr(L["we1_s"]), ptr(L["we2_s"]), ptr(self.gate_w_all[li]),
-                    _lib.CB_BF16, ptr(self.gate_i_all[li]), _lib.CB_I64, B, self.topk1, c.n_routed_experts + 1,
-                    2 * F, c.dim, 1, ptr(h if fuse_res else self.y), ptr(h2) if fuse_res else None, ptr(self.moe_ws),
-                    self.moe_ws.numel(), st), "fused_experts")
-                if not fuse_res:
-                    if tr is not None: tr["y"] = self.y.clone()
-                    self._allreduce(self.y)
-                    self._add(self.y, h2, h)                        # x = x + ffn(...)
-            if tr is not None: tr["h_out"] = h.clone()
+                self._moe_gate(li)
+                self._fused_experts(li, self.y, None)
+            tr["y"] = self.y.clone()
+            self._allreduce(self.y)
+            self._add(self.y, h2, h)                            # x = x + ffn(...)
+            tr["h_out"] = h.clone()
         self._rms(h, self.norm, self.xn, B, c.dim)
-        N, K = self.head.shape
-        check(lib.chitu_b200_linear_bf16(ptr(self.xn), ptr(self.head), None, None, ptr(self.logits), B, N, K,
-                                         _lib.CB_BF16, ptr(self.lin_ws), self.lin_ws.numel(), 0, st), "head")
-        check(lib.chitu_b200_argmax(ptr(self.logits), ptr(self.next_tokens), B, N, _lib.CB_BF16, st), "argmax")
-        if self.pg is not None and self.tp_size > 1:
-            # vocab-parallel head: the reference all-gathers the logits shards before sampling
-            # (tensor_parallel.py:94-102); the same token from a (max, index) all-gather of B*8 bytes per rank
-            self.next_tokens.copy_(global_argmax(self.logits, self.next_tokens, self.tp_rank, N, self.pg, self.tp_gather))
-        self.seq_lens.add_(1)
-
-    def capture(self):
-        torch.cuda.synchronize(self.device)
-        saved = self.seq_lens.clone()
-        s = torch.cuda.Stream(device=self.device)
-        s.wait_stream(torch.cuda.current_stream(self.device))
-        with torch.cuda.stream(s):
-            for _ in range(2):
-                self._step_body()
-        torch.cuda.current_stream(self.device).wait_stream(s)
-        torch.cuda.synchronize(self.device)
-        self.seq_lens.copy_(saved)
-        before = _lib.launch_count()
-        self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph):
-            self._step_body()
-        self.launches_per_step = _lib.launch_count() - before
-        self.seq_lens.copy_(saved)
-        torch.cuda.synchronize(self.device)
-
-    def step(self):
-        if self.graph is not None:
-            self.graph.replay()
-        else:
-            before = _lib.launch_count()
-            self._step_body()
-            self.launches_per_step = _lib.launch_count() - before
-
-    def decode(self, tokens_host: torch.Tensor) -> torch.Tensor:
-        self.tokens.copy_(tokens_host, non_blocking=True)
-        self.step()
-        return self.next_tokens.cpu()
 
     def distinct_experts_per_layer(self) -> float:
         """Mean number of distinct routed experts per MoE layer in the last step."""

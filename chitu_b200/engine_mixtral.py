@@ -16,7 +16,7 @@ import torch
 
 from . import _lib
 from ._lib import check, current_stream, ptr
-from .tensor_parallel import global_argmax
+from .engine import DecodeEngine
 
 BF = torch.bfloat16
 
@@ -43,24 +43,18 @@ class MixtralConfig:
 MIXTRAL_8X7B = MixtralConfig()
 
 
-class MixtralDecodeEngine:
+class MixtralDecodeEngine(DecodeEngine):
     def __init__(self, cfg: MixtralConfig, max_reqs: int, max_seq_len: int, device="cuda:0", page_size: int = 256,
                  seed: int = 0, tp_rank: int = 0, tp_size: int = 4, process_group=None, use_fused_allreduce: bool = True):
-        self.cfg, self.B, self.device = cfg, max_reqs, torch.device(device)
-        self.tp_rank, self.tp_size, self.pg = tp_rank, tp_size, process_group
-        self.lib = _lib.load()
         D = cfg.head_dim
         T = tp_size
         assert cfg.n_heads % T == 0 and cfg.n_kv_heads % T == 0 and cfg.intermediate_dim % (128 * T) == 0
         self.Hq, self.Hkv, self.D = cfg.n_heads // T, cfg.n_kv_heads // T, D
         self.F = cfg.intermediate_dim // T
         self.E, self.topk = cfg.num_local_experts, cfg.num_experts_per_tok
-        self.page = page_size
-        self.max_blocks = max_seq_len // page_size + 1
-        nblk = self.max_blocks * max_reqs
-        dev = self.device
-        g = torch.Generator(device=dev).manual_seed(seed + 1000 * tp_rank)
-        g_rep = torch.Generator(device=dev).manual_seed(seed + 7)
+        super().__init__(cfg, max_reqs, max_seq_len, device, page_size, seed, tp_rank, tp_size, process_group,
+                         use_fused_allreduce, attn_ws=(self.Hq, D, 64), lin_n=max(cfg.vocab_size // T, cfg.dim))
+        dev, g, g_rep = self.device, self.g, self.g_rep
 
         def rnd(gen, *shape, scale=0.02):
             return (torch.randn(*shape, generator=gen, dtype=torch.float32, device=dev) * scale).to(BF)
@@ -77,85 +71,33 @@ class MixtralDecodeEngine:
                 w1=rnd(g, self.E, 2 * self.F, dim), w2=rnd(g, self.E, dim, self.F)))
         self.norm = torch.ones(dim, dtype=BF, device=dev)
         self.head = rnd(g, cfg.vocab_size // T, dim)
+        nblk = self.max_blocks * max_reqs
         self.k_cache = torch.zeros(cfg.n_layers, nblk, page_size, self.Hkv, D, dtype=BF, device=dev)
         self.v_cache = torch.zeros_like(self.k_cache)
-        self.block_table = torch.zeros(max_reqs, self.max_blocks, dtype=torch.int32, device=dev)
-        self.seq_lens = torch.zeros(max_reqs, dtype=torch.int32, device=dev)
+        self.caches = (self.k_cache, self.v_cache)
         # hf rotary: cos/sin [pos, D/2] in the model dtype, half-split layout (ops.py:243-308 "hf-llama")
         freqs = 1.0 / (cfg.rope_theta ** (torch.arange(0, D, 2).float() / D))
-        ang = torch.outer(torch.arange(max_seq_len * 2, dtype=torch.float32), freqs)
-        self.cos_table, self.sin_table = ang.cos().to(BF).to(dev), ang.sin().to(BF).to(dev)
+        self._rope_tables(torch.outer(torch.arange(max_seq_len * 2, dtype=torch.float32), freqs), BF)
         B = max_reqs
         z = lambda *s, dt=BF: torch.zeros(*s, dtype=dt, device=dev)
-        self.tokens = torch.zeros(B, dtype=torch.int64, device=dev)
-        self.cos, self.sin = z(B, D // 2), z(B, D // 2)
-        self.h, self.h2, self.xn, self.y = z(B, dim), z(B, dim), z(B, dim), z(B, dim)
+        self.y = z(B, dim)
         self.qkv = z(B, (self.Hq + 2 * self.Hkv) * D)
         self.q_rot, self.k_rot = z(B, self.Hq, D), z(B, self.Hkv, D)
         self.attn_out = z(B, self.Hq * D)
         self.gate_w_all = z(cfg.n_layers, B, self.topk)
         self.gate_i_all = torch.zeros(cfg.n_layers, B, self.topk, dtype=torch.int64, device=dev)
-        self.logits = z(B, cfg.vocab_size // T)
-        self.next_tokens = torch.zeros(B, dtype=torch.int64, device=dev)
-        self.tp_gather = (torch.empty(T, B, 2, dtype=torch.float32, device=dev) if (process_group is not None and T > 1) else None)
         lib = self.lib
-        self.attn_ws = torch.zeros(lib.chitu_b200_attn_workspace_bytes(B, self.Hq, D, 64), dtype=torch.uint8, device=dev)
-        self.lin_ws = torch.zeros(max(lib.chitu_b200_linear_workspace_bytes(B, max(cfg.vocab_size // T, dim)), 256),
-                                  dtype=torch.uint8, device=dev)
         self.moe_ws = torch.zeros(lib.chitu_b200_moe_workspace_bytes(B, self.topk, self.E, 2 * self.F, dim), dtype=torch.uint8,
                                   device=dev)
         self.gate_ws = torch.zeros(lib.chitu_b200_moe_gate_workspace_bytes(B, self.E), dtype=torch.uint8, device=dev)
-        self.max_seq_len = max_seq_len
-        self.graph = None
-        self.launches_per_step = 0
-        self.comm = None
-        if T > 1 and process_group is not None and use_fused_allreduce:
-            from .comm import FusedAllReduce
-            self.comm = FusedAllReduce(process_group, max_reqs, dim, self.device)
-        import os
-        # all-reduce started from the producing kernel's epilogue (csrc/comm.cu push mode); 0 = the pull kernel
-        self.ar_push = os.environ.get("CHITU_B200_AR_PUSH", "1") != "0"
 
-    def set_synthetic_context(self, seq_len: int, seed: int = 2):
-        g = torch.Generator(device="cpu").manual_seed(seed)
-        gd = torch.Generator(device=self.device).manual_seed(seed + 11)
-        nblk = self.k_cache.shape[1]
-        self.block_table.copy_(torch.randperm(nblk, generator=g).to(torch.int32).view(self.B, self.max_blocks))
-        self.seq_lens.fill_(seq_len)
-        for l in range(self.cfg.n_layers):
-            self.k_cache[l].normal_(0, 1, generator=gd)
-            self.v_cache[l].normal_(0, 1, generator=gd)
-
-    def _linear(self, x, w, y, M, residual=None):
-        N, K = w.shape
-        check(self.lib.chitu_b200_linear_bf16(ptr(x), ptr(w), None, ptr(residual), ptr(y), M, N, K, _lib.CB_BF16,
-                                              ptr(self.lin_ws), self.lin_ws.numel(), 0, current_stream()), "linear_bf16")
-
-    def _rmsnorm(self, x, w, y, M):
-        check(self.lib.chitu_b200_rmsnorm(ptr(x), ptr(w), ptr(y), M, self.cfg.dim, self.cfg.norm_eps, _lib.CB_BF16,
-                                          current_stream()), "rmsnorm")
-
-    def _step_body(self):
+    def _decode_layers(self):
         lib, B, D, cfg = self.lib, self.B, self.D, self.cfg
         st = current_stream()
-        tp_on = self.pg is not None and self.tp_size > 1
-        torch.index_select(self.cos_table, 0, self.seq_lens, out=self.cos)
-        torch.index_select(self.sin_table, 0, self.seq_lens, out=self.sin)
-        check(lib.chitu_b200_embedding(ptr(self.tokens), ptr(self.embed), ptr(self.h), B, cfg.dim, 0, cfg.vocab_size,
-                                       _lib.CB_BF16, st), "embedding")
         h, h2 = self.h, self.h2
         qkv_w = (self.Hq + 2 * self.Hkv) * D
         n_layers = len(self.layers)
-
-        def reduce_add_norm(partial, residual, h_out, norm_w):
-            if self.comm is not None:
-                self.comm(partial, residual, h_out, norm_w, self.xn, None, None, B, cfg.dim, cfg.norm_eps)
-            else:
-                torch.distributed.all_reduce(partial, group=self.pg)
-                check(lib.chitu_b200_add(ptr(partial), ptr(residual), ptr(h_out), B * cfg.dim, _lib.CB_BF16, st), "add")
-                self._rmsnorm(h_out, norm_w, self.xn, B)
-
-        self._rmsnorm(h, self.layers[0]["attn_norm"], self.xn, B)
+        self._norm(h, self.layers[0]["attn_norm"], self.xn)
         for li, lw in enumerate(self.layers):
             next_norm = self.layers[li + 1]["attn_norm"] if li + 1 < n_layers else self.norm
             self._linear(self.xn, lw["wqkv"], self.qkv, B)
@@ -172,72 +114,22 @@ class MixtralDecodeEngine:
                 self.Hkv * D, qkv_w, ptr(self.seq_lens), ptr(self.block_table), self.max_blocks, B, self.Hq, self.Hkv, D,
                 self.page, self.max_seq_len, 1.0 / math.sqrt(D), ptr(self.attn_out), ptr(self.attn_ws),
                 self.attn_ws.numel(), _lib.CB_BF16, st), "gqa_paged_decode")
-            push = tp_on and self.comm is not None and self.ar_push
-            if push:
-                self.comm.linear_push(self.attn_out, lw["wo"], B, self.lin_ws)
-                self.comm.consume(h, h2, lw["ffn_norm"], self.xn, None, None, B, cfg.dim, cfg.norm_eps)
-            elif tp_on:
-                self._linear(self.attn_out, lw["wo"], h2, B)
-                reduce_add_norm(h2, h, h2, lw["ffn_norm"])
-            else:
-                self._linear(self.attn_out, lw["wo"], h2, B, residual=h)
-                self._rmsnorm(h2, lw["ffn_norm"], self.xn, B)
+            self._row_parallel(lambda out, res: self._linear(self.attn_out, lw["wo"], out, B, residual=res),
+                               lambda: self.comm.linear_push(self.attn_out, lw["wo"], B, self.lin_ws),
+                               h, h2, lw["ffn_norm"], y=self.xn)
             # ---- sparse MoE block (model_hf_mixtral.py:51-96) through the fused experts ----
             check(lib.chitu_b200_moe_gate(ptr(self.xn), ptr(lw["gate_w"]), None, 0, B, cfg.dim, self.E, 1, 1, self.topk, 2,
                                           1.0, ptr(self.gate_w_all[li]), ptr(self.gate_i_all[li]), self.topk,
                                           ptr(self.gate_ws), self.gate_ws.numel(), st), "moe_gate")
-            if push:
-                self.comm.experts_push(self.xn, lw["w1"], lw["w2"], None, None, self.gate_w_all[li], _lib.CB_BF16,
-                                       self.gate_i_all[li], _lib.CB_I64, B, self.topk, self.E, 2 * self.F, cfg.dim, 0, self.moe_ws)
-                self.comm.consume(h2, h, next_norm, self.xn, None, None, B, cfg.dim, cfg.norm_eps)
-                continue
-            check(lib.chitu_b200_fused_experts(
-                ptr(self.xn), ptr(lw["w1"]), ptr(lw["w2"]), None, None, ptr(self.gate_w_all[li]), _lib.CB_BF16,
-                ptr(self.gate_i_all[li]), _lib.CB_I64, B, self.topk, self.E, 2 * self.F, cfg.dim, 0,
-                ptr(self.y if tp_on else h), None if tp_on else ptr(h2), ptr(self.moe_ws), self.moe_ws.numel(), st),
-                "fused_experts")
-            if tp_on:
-                reduce_add_norm(self.y, h2, h, next_norm)
-            else:
-                self._rmsnorm(h, next_norm, self.xn, B)
-        self._linear(self.xn, self.head, self.logits, B)
-        vocab_local = cfg.vocab_size // self.tp_size
-        check(lib.chitu_b200_argmax(ptr(self.logits), ptr(self.next_tokens), B, vocab_local, _lib.CB_BF16, st), "argmax")
-        if tp_on:
-            self.next_tokens.copy_(global_argmax(self.logits, self.next_tokens, self.tp_rank, vocab_local, self.pg, self.tp_gather))
-        self.seq_lens.add_(1)
-
-    def capture(self):
-        torch.cuda.synchronize(self.device)
-        saved = self.seq_lens.clone()
-        s = torch.cuda.Stream(device=self.device)
-        s.wait_stream(torch.cuda.current_stream(self.device))
-        with torch.cuda.stream(s):
-            for _ in range(2):
-                self._step_body()
-        torch.cuda.current_stream(self.device).wait_stream(s)
-        torch.cuda.synchronize(self.device)
-        self.seq_lens.copy_(saved)
-        before = _lib.launch_count()
-        self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph):
-            self._step_body()
-        self.launches_per_step = _lib.launch_count() - before
-        self.seq_lens.copy_(saved)
-        torch.cuda.synchronize(self.device)
-
-    def step(self):
-        if self.graph is not None:
-            self.graph.replay()
-        else:
-            before = _lib.launch_count()
-            self._step_body()
-            self.launches_per_step = _lib.launch_count() - before
-
-    def decode(self, tokens_host: torch.Tensor) -> torch.Tensor:
-        self.tokens.copy_(tokens_host, non_blocking=True)
-        self.step()
-        return self.next_tokens.cpu()
+            self._row_parallel(
+                lambda out, res: check(lib.chitu_b200_fused_experts(
+                    ptr(self.xn), ptr(lw["w1"]), ptr(lw["w2"]), None, None, ptr(self.gate_w_all[li]), _lib.CB_BF16,
+                    ptr(self.gate_i_all[li]), _lib.CB_I64, B, self.topk, self.E, 2 * self.F, cfg.dim, 0, ptr(out), ptr(res),
+                    ptr(self.moe_ws), self.moe_ws.numel(), st), "fused_experts"),
+                lambda: self.comm.experts_push(self.xn, lw["w1"], lw["w2"], None, None, self.gate_w_all[li], _lib.CB_BF16,
+                                               self.gate_i_all[li], _lib.CB_I64, B, self.topk, self.E, 2 * self.F, cfg.dim, 0,
+                                               self.moe_ws),
+                h2, h, next_norm, y=self.xn, partial=self.y)
 
     def distinct_experts_per_layer(self) -> float:
         ids = self.gate_i_all.cpu()

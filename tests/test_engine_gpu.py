@@ -28,12 +28,12 @@ def test_llama_engine_cuda_graph_two_steps():
     assert eng.launches_per_step > 0
 
 
-def _deepseek_case(n_layers, n_dense, cache_dq, B=3, S=150):
+def _deepseek_case(n_layers, n_dense, B=3, S=150):
     from chitu_b200.engine_deepseek import DeepSeekConfig, DeepSeekDecodeEngine
     cfg = DeepSeekConfig(vocab_size=1024, dim=512, inter_dim=1024, moe_inter_dim=256, n_layers=n_layers,
                          n_dense_layers=n_dense, n_heads=4, n_routed_experts=16, n_activated_experts=4,
                          n_expert_groups=4, n_limited_groups=2, q_lora_rank=256)
-    eng = DeepSeekDecodeEngine(cfg, max_reqs=B, max_seq_len=512, device="cuda:0", tp_size=1, cache_dequant_wkv_b=cache_dq)
+    eng = DeepSeekDecodeEngine(cfg, max_reqs=B, max_seq_len=512, device="cuda:0", tp_size=1)
     eng.set_synthetic_context(S)
     eng.seq_lens.copy_(torch.tensor([S, 63, 128], dtype=torch.int32))
     tokens = torch.tensor([5, 17, 900], dtype=torch.int64)
@@ -58,8 +58,8 @@ def test_deepseek_engine_step_vs_oracle():
     so a 1-ulp bf16 difference upstream flips a few e4m3 roundings (6-12 % each) and two CORRECT
     implementations differ by ~1 % per GEMM (cos_diff ~1e-3 after a layer) — the tight, teacher-forced
     comparison is test_deepseek_engine_wiring_stage_by_stage; here only gross errors are caught."""
-    for n_layers, n_dense, cache_dq in [(1, 1, True), (2, 1, True), (3, 1, False)]:
-        cd, mr, same_routes = _deepseek_case(n_layers, n_dense, cache_dq)
+    for n_layers, n_dense in [(1, 1), (2, 1), (3, 1)]:
+        cd, mr, same_routes = _deepseek_case(n_layers, n_dense)
         print(f"deepseek engine vs oracle L={n_layers}: cos_diff {cd:.3e} max_rel {mr:.3e} same_routes {same_routes}")
         if same_routes:
             assert cd < 1e-2, (n_layers, cd)
@@ -75,7 +75,7 @@ def test_deepseek_engine_wiring_stage_by_stage():
                          n_heads=4, n_routed_experts=16, n_activated_experts=4, n_expert_groups=4, n_limited_groups=2,
                          q_lora_rank=256)
     B, S = 3, 150
-    eng = DeepSeekDecodeEngine(cfg, max_reqs=B, max_seq_len=512, device="cuda:0", tp_size=1, cache_dequant_wkv_b=False)
+    eng = DeepSeekDecodeEngine(cfg, max_reqs=B, max_seq_len=512, device="cuda:0", tp_size=1)
     eng.set_synthetic_context(S)
     eng.seq_lens.copy_(torch.tensor([S, 63, 128], dtype=torch.int32))
     eng.trace = []
