@@ -54,6 +54,8 @@ SIGNATURES = {
     "chitu_b200_attn_workspace_bytes": (L, [I, I, I, I]),
     "chitu_b200_gqa_paged_decode": (I, [P, P, P, P, P, L, L, P, P, I, I, I, I, I, I, I, F, P, P, L, I, P]),
     "chitu_b200_gqa_paged_decode_rope": (I, [P, L, P, P, P, P, L, L, P, P, P, P, I, I, I, I, I, I, I, F, P, P, L, I, P]),
+    "chitu_b200_gqa_paged_prefill": (I, [P, P, P, P, P, L, L, L, L, P, P, I, I, I, I, I, I, I, I, I, I, F, P, P, L, I,
+                                         P]),
     "chitu_b200_mla_decode": (I, [P, P, P, P, P, P, I, I, I, I, I, I, I, I, F, P, P, L, P]),
     "chitu_b200_mla_prefill": (I, [P, P, L, P, L, P, P, I, I, I, I, I, I, F, P, P]),
     "chitu_b200_debug_timeline": (I, [P]),

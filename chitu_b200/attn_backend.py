@@ -2,8 +2,10 @@
 
 `B200AttnBackend` implements the four methods the models call (SURVEY.md §8b):
 prepare_metadata_for_decode, attn_varlen_func (prefill: the absorbed-MLA form runs the sm_90a
-prefill kernel; GQA prefill stays on flash_attn / torch SDPA), attn_with_kvcache (GQA paged decode
-with in-place append) and mla_attn_with_kvcache (absorbed-MLA paged decode with fused append).
+prefill kernel; GQA prefill stays on flash_attn / torch SDPA), attn_with_kvcache (GQA attention over the paged
+cache with in-place append: the decode kernel for seqlen_q == 1, the sm_90a multi-token kernel for seqlen_q > 1 —
+chunked prefill, prefill on a cached prefix, speculative verification) and mla_attn_with_kvcache (absorbed-MLA
+paged decode with fused append).
 """
 from __future__ import annotations
 
@@ -175,7 +177,8 @@ class B200AttnBackend(AttnBackend):
         assert cache_leftpad is None and window_size == (-1, -1) and softcap == 0.0
         require_cuda(q, k_cache, v_cache, block_table)
         B, sq, Hq, D = q.shape
-        assert sq == 1, "decode only (seqlen_q == 1)"
+        if sq > 1:
+            return self._paged_prefill(q, k_cache, v_cache, k, v, cache_seqlens, block_table, causal, softmax_scale)
         num_blocks, page, Hkv, Dk = k_cache.shape
         assert Dk == D and v_cache.shape == k_cache.shape
         assert q.is_contiguous() and k_cache.is_contiguous() and v_cache.is_contiguous()
@@ -197,6 +200,35 @@ class B200AttnBackend(AttnBackend):
             ptr(q), ptr(k_cache), ptr(v_cache), ptr(k), ptr(v), ksb, vsb, ptr(cache_seqlens), ptr(block_table),
             block_table.stride(0), B, Hq, Hkv, D, page, int(hint), float(scale), ptr(out), ptr(ws), wsn,
             dtype_code(q.dtype), current_stream()), "gqa_paged_decode")
+        return out
+
+    def _paged_prefill(self, q, k_cache, v_cache, k, v, cache_seqlens, block_table, causal, softmax_scale):
+        """seqlen_q > 1 (chunked prefill, prefill on a cached prefix, speculative verification): the sq new k / v rows
+        are appended at cache_seqlens[b] + i, then query i attends to the first cache_seqlens[b] + sq keys (without k / v:
+        cache_seqlens[b]), bottom-right causal when `causal` (chitu_b200_gqa_paged_prefill)."""
+        B, sq, Hq, D = q.shape
+        num_blocks, page, Hkv, Dk = k_cache.shape
+        assert Dk == D and v_cache.shape == k_cache.shape
+        assert k_cache.dtype == v_cache.dtype == q.dtype and (k is None or k.dtype == v.dtype == q.dtype)
+        assert q.is_contiguous() and k_cache.is_contiguous() and v_cache.is_contiguous()
+        assert block_table.dtype == torch.int32 and block_table.stride(-1) == 1
+        if not torch.is_tensor(cache_seqlens):
+            cache_seqlens = torch.full((B,), int(cache_seqlens), dtype=torch.int32, device=q.device)
+        assert cache_seqlens.dtype == torch.int32 and cache_seqlens.is_contiguous()
+        strides = (0, 0, 0, 0)
+        if k is not None:
+            assert v is not None and k.shape == (B, sq, Hkv, D) and v.shape == (B, sq, Hkv, D)
+            # heads must be dense; the batch and token strides are free (views into a fused qkv GEMM output)
+            assert k.stride(-1) == 1 and k.stride(-2) == D and v.stride(-1) == 1 and v.stride(-2) == D
+            strides = (k.stride(0), k.stride(1), v.stride(0), v.stride(1))
+        scale = softmax_scale if softmax_scale is not None else 1.0 / math.sqrt(D)
+        out = torch.empty_like(q)
+        ws, wsn = self._ws(B, Hq, D, q.device)
+        hint = self.max_seq_len if self.max_seq_len else block_table.shape[1] * page
+        check(_lib.load().chitu_b200_gqa_paged_prefill(
+            ptr(q), ptr(k_cache), ptr(v_cache), ptr(k), ptr(v), *strides, ptr(cache_seqlens), ptr(block_table),
+            block_table.stride(0), B, sq, Hq, Hkv, D, page, num_blocks, int(hint), int(bool(causal)), float(scale),
+            ptr(out), ptr(ws), wsn, dtype_code(q.dtype), current_stream()), "gqa_paged_prefill")
         return out
 
     # -- a2: attn_backend.py:707-774 (Triton), :536-572 (FlashMLA), :660-684 (FlashInfer)

@@ -557,6 +557,23 @@ static int splits_that_fit(int splits, int B, int H, int DV, int64_t workspace_b
   return splits;
 }
 
+namespace cb {
+// Split count of chitu_b200_gqa_paged_prefill (gqa_prefill.cu): the wave rule of the decode kernels on its CTA count,
+// shrunk to the workspace it is given (none: 1 split).  H = sq * Hq partial rows per request.
+int gqa_prefill_num_splits(int ctas_without_split, int max_len, int slots, int B, int H, int DV, int64_t workspace_bytes) {
+  if (workspace_bytes <= 0) return 1;
+  return splits_that_fit(pick_splits_waves(ctas_without_split, max_len, slots), B, H, DV, workspace_bytes);
+}
+// merge of `rows` head-dim-128 partial rows in the [rows, S, 128] + LSE layout above (gqa_prefill.cu)
+cudaError_t launch_merge_splits(const float* o_part, const float* lse, void* out, int rows, int splits, int dtype,
+                                cudaStream_t st) {
+  if (dtype == CB_BF16)
+    return cb::launch_k(merge_splits_kernel<__nv_bfloat16, 128>, dim3(rows), dim3(128), 0, st, o_part, lse,
+                        (__nv_bfloat16*)out, splits);
+  return cb::launch_k(merge_splits_kernel<__half, 128>, dim3(rows), dim3(128), 0, st, o_part, lse, (__half*)out, splits);
+}
+}  // namespace cb
+
 extern "C" int chitu_b200_gqa_paged_decode(const void* q, void* k_cache, void* v_cache, const void* k_new,
                                            const void* v_new, int64_t k_new_sb, int64_t v_new_sb,
                                            const int32_t* cache_seqlens,

@@ -49,6 +49,7 @@ int chitu_b200_tl_set_linear(unsigned long long*);
 int chitu_b200_tl_set_attention(unsigned long long*);
 int chitu_b200_tl_set_mla_tc(unsigned long long*);
 int chitu_b200_tl_set_mla_prefill(unsigned long long*);
+int chitu_b200_tl_set_gqa_prefill(unsigned long long*);
 int chitu_b200_tl_set_moe(unsigned long long*);
 int chitu_b200_tl_set_comm(unsigned long long*);
 int chitu_b200_tl_set_sampling(unsigned long long*);
@@ -59,7 +60,8 @@ extern "C" int chitu_b200_debug_timeline(void* buf) {
   unsigned long long* p = (unsigned long long*)buf;
   int rc = chitu_b200_tl_set_core(p) | chitu_b200_tl_set_elementwise(p) | chitu_b200_tl_set_gemv(p) |
            chitu_b200_tl_set_gemm_tc(p) | chitu_b200_tl_set_linear(p) | chitu_b200_tl_set_attention(p) |
-           chitu_b200_tl_set_mla_tc(p) | chitu_b200_tl_set_mla_prefill(p) | chitu_b200_tl_set_moe(p) | chitu_b200_tl_set_comm(p) | chitu_b200_tl_set_sampling(p);
+           chitu_b200_tl_set_mla_tc(p) | chitu_b200_tl_set_mla_prefill(p) | chitu_b200_tl_set_gqa_prefill(p) |
+           chitu_b200_tl_set_moe(p) | chitu_b200_tl_set_comm(p) | chitu_b200_tl_set_sampling(p);
   cb::g_tl_on = p != nullptr;
   cb::g_tl_len = 0;
   cb::g_tl_names[0] = 0;

@@ -197,6 +197,25 @@ int chitu_b200_gqa_paged_decode_rope(const void* q, int64_t q_sb, void* k_cache,
                                      int bt_stride, int B, int Hq, int Hkv, int D, int page_size, int max_seqlen_hint,
                                      float softmax_scale, void* out, void* workspace, int64_t workspace_bytes,
                                      int dtype, void* stream);
+/* AttnBackend.attn_with_kvcache with block_table and seqlen_q = sq >= 1 (attn_backend.py:92-164, FlashAttn impl
+ * :208-243, flash_attn_with_kvcache semantics): chunked prefill, prefill on a cached prefix, speculative verification.
+ * q [B, sq, Hq, D] contiguous; k_cache / v_cache [num_blocks, page_size, Hkv, D] contiguous; k_new / v_new
+ * [B, sq, Hkv, D] with dense heads and batch / token strides *_sb / *_st in elements (views into a fused-qkv GEMM
+ * output), or both NULL.  With k_new: token i of request b is written to position cache_seqlens[b] + i (true page
+ * indexing) before the attention, which then runs over Lk = cache_seqlens[b] + sq keys; without, Lk = cache_seqlens[b].
+ * cache_seqlens is not modified.  causal != 0: query i sees key j iff j <= i + Lk - sq; a row that sees no key is 0.
+ * fp32 scores and softmax, P rounded to the io dtype before P.V.  out [B, sq, Hq, D] contiguous.
+ * Only block_table[b, 0 .. ceil(Lk / page_size) - 1] is read; cache slots past Lk may hold anything (NaN included).
+ * Splits over keys when the GPU would otherwise be idle (count from B, Hkv, sq and max_seqlen_hint, shrunk to the
+ * workspace; NULL workspace: no split) -> no host synchronisation, capturable in a CUDA graph, deterministic.
+ * Built for D == 128, page_size % 64 == 0, Hq / Hkv in {1, 2, 4, 8}, bf16 | fp16; 16-byte aligned bases and strides
+ * that are multiples of 8 elements.  Anything else returns a negative status. */
+int chitu_b200_gqa_paged_prefill(const void* q, void* k_cache, void* v_cache, const void* k_new, const void* v_new,
+                                 int64_t k_new_sb, int64_t k_new_st, int64_t v_new_sb, int64_t v_new_st,
+                                 const int32_t* cache_seqlens, const int32_t* block_table, int bt_stride, int B, int sq,
+                                 int Hq, int Hkv, int D, int page_size, int num_blocks, int max_seqlen_hint, int causal,
+                                 float softmax_scale, void* out, void* workspace, int64_t workspace_bytes, int dtype,
+                                 void* stream);
 
 
 /* *.mla_attn_with_kvcache (attn_backend.py:536-572 / 660-684 / 707-774) = append
