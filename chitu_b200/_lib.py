@@ -18,6 +18,9 @@ CSRC_DIR = os.path.join(_HERE, "csrc")
 
 # dtype codes (include/chitu_b200.h)
 CB_BF16, CB_F16, CB_F32, CB_FP8_E4M3, CB_I8, CB_U8, CB_I16, CB_I32, CB_I64 = range(9)
+# split-KV attention workspace (csrc/splitkv.cuh): the kernels split the keys at most ATTN_MAX_SPLITS ways, and the
+# last ATTN_PLAN_BYTES bytes hold the device-side split plan
+ATTN_MAX_SPLITS, ATTN_PLAN_BYTES = 128, 256
 
 _lock = threading.Lock()
 _lib = None

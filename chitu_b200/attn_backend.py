@@ -19,7 +19,6 @@ from ._lib import check, current_stream, dtype_code, ptr, require_cuda
 
 __all__ = ["AttnBackend", "B200AttnBackend"]
 
-_MAX_SPLITS = 128
 _MLA_QK, _MLA_V = 576, 512          # absorbed MLA: kv_lora_rank + qk_rope_head_dim, kv_lora_rank
 
 
@@ -71,34 +70,25 @@ class B200AttnBackend(AttnBackend):
         # (graphs are captured per batch size in arrival order, models/model.py:537-622; a buffer a captured
         # kernel was given is never freed — see workspace.py — so this only avoids a second allocation).
         Bmax = max(B, self.max_reqs or 0, 1)
-        workspace.reserve("attn", self._ws_bytes(Bmax, self.n_local_heads, max(self.kv_lora_rank, 128)),
+        workspace.reserve("attn", workspace.attn_bytes(Bmax, self.n_local_heads, max(self.kv_lora_rank, 128)),
                           block_table.device)
         # a1 proper: the length-aware split-KV plan of this step, computed ON THE DEVICE from the step's lengths (the
         # reference's FlashInfer variant does O(B) .item() syncs here, attn_backend.py:620-637; FlashMLA runs
-        # get_mla_metadata).  The MLA decode kernel finds it in the last 256 bytes of the attention workspace.
+        # get_mla_metadata).  The MLA decode kernel finds it at the end of the attention workspace.
         if block_size == 64 and B > 0 and torch.is_tensor(cache_seqlens_incl_this_decode):
             H = self.n_local_heads
             buf, n = self._ws(B, H, max(self.kv_lora_rank, 128), block_table.device)
             hint = self.max_seq_len if self.max_seq_len else block_table.shape[1] * block_size
             check(_lib.load().chitu_b200_attn_plan(ptr(cache_seqlens_incl_this_decode), B, H, block_size, int(hint), ptr(buf), n,
                                                    current_stream()), "attn_plan")
-            self._plan_view = buf[n - 256:].view(torch.int32)
+            self._plan_view = buf[n - _lib.ATTN_PLAN_BYTES:].view(torch.int32)
 
     def last_plan(self):
         """int32 view of the device-side split plan written by the last prepare_metadata_for_decode (tests / debugging)."""
         return self._plan_view
 
-    @staticmethod
-    def _ws_bytes(B, H, DV):
-        lib = _lib.load()
-        # largest split count whose partials fit a bounded workspace (<= 256 MiB)
-        splits = _MAX_SPLITS
-        while splits > 1 and lib.chitu_b200_attn_workspace_bytes(B, H, DV, splits) > (256 << 20):
-            splits //= 2
-        return lib.chitu_b200_attn_workspace_bytes(B, H, DV, splits)
-
     def _ws(self, B, H, DV, device):
-        buf = workspace.get("attn", self._ws_bytes(B, H, DV), device)
+        buf = workspace.get("attn", workspace.attn_bytes(B, H, DV), device)
         return buf, buf.numel()
 
     # -- prefill (SURVEY §8f n4).  attn_backend.py:193-206 (FlashAttnBackend), flash_attn_varlen_func semantics.

@@ -5,17 +5,18 @@
 //    block table, online softmax in fp32, LSE-weighted merge of the splits.  Head dim 128 with
 //    power-of-two pages runs on tensor cores (gqa_decode_mmaT_kernel, optional fused rotary);
 //    head dim 64 and other page sizes run on the SIMT kernel (gqa_decode_kernel).
-//  * mla_decode       : *.mla_attn_with_kvcache (attn_backend.py:707-774) = append (ops.py:50-91)
-//    + absorbed-MLA split-KV attention (triton_decode_attention.py:20-130) + merge (:185-232), on
-//    the wgmma kernel of mla_tc.cu (64-token pages).  V is a view of the first C columns of the
-//    same cache row, so each row is read once.
+//  * merge_splits_kernel : the LSE-weighted merge of split-KV partials, for GQA decode, MLA decode
+//    (mla_tc.cu) and GQA paged prefill (gqa_prefill.cu).  The workspace layout, the split counts
+//    and the split plan are defined once in splitkv.cuh.
+//  * MLA weight absorption (absorb-o can also merge the MLA decode partials) and mla_prep.
 //
-// Both kernels never read the cache row of the token being appended: the CTA that owns that
+// The GQA kernels never read the cache row of the token being appended: the CTA that owns that
 // position takes it from `k_new` directly and split 0 writes it to the cache -> no RAW hazard.
 // The reference fixes NUM_KV_SPLITS = 4 (attn_backend.py:735) -> 4 CTAs at B=1; here the split
 // count is sized from the SM count so the 132 SMs of an H100 are busy at B=1.
 
 #include "common.cuh"
+#include "splitkv.cuh"
 #include "tc_ptx.cuh"
 
 using namespace cb;
@@ -24,14 +25,11 @@ namespace {
 
 constexpr float kLog2e = 1.4426950408889634f;
 
-// partial layout in the workspace: o_part[B, H, S, Dv] fp32 (already normalised), lse[B, H, S]
-// (log2 domain: m + log2(l)), S = num_splits.
-
 template <typename T, int DV>
 __global__ void merge_splits_kernel(const float* __restrict__ o_part, const float* __restrict__ lse,
                                     T* __restrict__ out, int num_splits) {
   cb::pdl_prologue();
-  __shared__ float s_w[128];                      // normalised split weights (num_splits <= 128)
+  __shared__ float s_w[kMaxSplits];               // normalised split weights
   const int64_t bh = blockIdx.x;  // b * H + h
   const float* l = lse + bh * num_splits;
   if (threadIdx.x < 32) {
@@ -518,59 +516,25 @@ __global__ void __launch_bounds__(kGqaWarps * 32, kGqaCtas) gqa_decode_mmaT_kern
   }
 }
 
-constexpr int kMlaC = 512, kMlaR = 64;   // absorbed MLA: kv_lora_rank latent dims, qk_rope_head_dim rope dims
-
-// split count for a kernel with `slots` resident CTAs on the GPU: minimise waves x (keys per split + a fixed
-// per-CTA cost worth ~192 keys).  Waves are whole: a CTA streams at its SM's rate however empty the GPU is
-// (measured over split counts: bs=16 128 CTAs x 4096 keys beat every split; bs=1 wants ~one full wave).
-inline int pick_splits_waves(int ctas_without_split, int max_len, int slots) {
-  int by_len = (max_len + 127) / 128;
-  if (by_len > 64) by_len = 64;
-  int best = 1;
-  double best_cost = 1e30;
-  for (int s = 1; s <= by_len; ++s) {
-    const int ctas = ctas_without_split * s;
-    const int waves = (ctas + slots - 1) / slots;
-    const double cost = waves * ((double)max_len / s + 192.0) + (s > 1 ? 64.0 : 0.0);   // + the merge launch
-    if (cost < best_cost - 1e-9) { best_cost = cost; best = s; }
-  }
-  return best;
-}
-
-inline int pick_splits(int ctas_without_split, int max_len, int min_keys_per_split, int max_splits) {
-  int want = (132 * 4 + ctas_without_split - 1) / ctas_without_split;  // ~4 CTAs per SM
-  int by_len = (max_len + min_keys_per_split - 1) / min_keys_per_split;
-  int s = want < by_len ? want : by_len;
-  if (s > max_splits) s = max_splits;
-  if (s < 1) s = 1;
-  return s;
-}
-
 }  // namespace
 
 extern "C" int64_t chitu_b200_attn_workspace_bytes(int batch, int heads, int head_dim_v, int max_splits) {
-  return (int64_t)batch * heads * max_splits * (head_dim_v + 1) * (int64_t)sizeof(float) + 256;
-}
-
-static int splits_that_fit(int splits, int B, int H, int DV, int64_t workspace_bytes) {
-  while (splits > 1 && chitu_b200_attn_workspace_bytes(B, H, DV, splits) > workspace_bytes) --splits;
-  return splits;
+  return split_kv_bytes((int64_t)batch * heads, head_dim_v, max_splits);
 }
 
 namespace cb {
-// Split count of chitu_b200_gqa_paged_prefill (gqa_prefill.cu): the wave rule of the decode kernels on its CTA count,
-// shrunk to the workspace it is given (none: 1 split).  H = sq * Hq partial rows per request.
-int gqa_prefill_num_splits(int ctas_without_split, int max_len, int slots, int B, int H, int DV, int64_t workspace_bytes) {
-  if (workspace_bytes <= 0) return 1;
-  return splits_that_fit(pick_splits_waves(ctas_without_split, max_len, slots), B, H, DV, workspace_bytes);
-}
-// merge of `rows` head-dim-128 partial rows in the [rows, S, 128] + LSE layout above (gqa_prefill.cu)
-cudaError_t launch_merge_splits(const float* o_part, const float* lse, void* out, int rows, int splits, int dtype,
-                                cudaStream_t st) {
-  if (dtype == CB_BF16)
-    return cb::launch_k(merge_splits_kernel<__nv_bfloat16, 128>, dim3(rows), dim3(128), 0, st, o_part, lse,
-                        (__nv_bfloat16*)out, splits);
-  return cb::launch_k(merge_splits_kernel<__half, 128>, dim3(rows), dim3(128), 0, st, o_part, lse, (__half*)out, splits);
+int launch_merge_splits(const float* o_part, const float* lse, void* out, int rows, int splits, int dv, int dtype,
+                        cudaStream_t st) {
+#define MERGE(T, DV, THREADS) \
+  launch_k(merge_splits_kernel<T, DV>, dim3(rows), dim3(THREADS), 0, st, o_part, lse, (T*)out, splits)
+  if (dtype == CB_BF16 && dv == 128) MERGE(__nv_bfloat16, 128, 128);
+  else if (dtype == CB_BF16 && dv == 64) MERGE(__nv_bfloat16, 64, 64);
+  else if (dtype == CB_BF16 && dv == kMlaC) MERGE(__nv_bfloat16, kMlaC, 256);
+  else if (dtype == CB_F16 && dv == 128) MERGE(__half, 128, 128);
+  else if (dtype == CB_F16 && dv == 64) MERGE(__half, 64, 64);
+  else return fail(-1, "merge_splits: no merge kernel for dtype %d, head dim %d", dtype, dv);
+#undef MERGE
+  return 0;
 }
 }  // namespace cb
 
@@ -608,9 +572,8 @@ extern "C" int chitu_b200_gqa_paged_decode_rope(const void* q, int64_t q_sb, voi
     return fail(-2, "gqa_paged_decode_rope: fused rotary / strided q need head_dim 128 and a power-of-two page");
   const int max_len = max_seqlen_hint > 0 ? max_seqlen_hint : bt_stride * page_size;
   int splits = tc ? pick_splits_waves(B * Hkv, max_len, 132 * kGqaCtas) : pick_splits(B * Hkv, max_len, 256, 64);
-  splits = workspace ? splits_that_fit(splits, B, Hq, D, workspace_bytes) : 1;
-  float* o_part = (float*)workspace;
-  float* lse = o_part ? o_part + (int64_t)B * Hq * splits * D : nullptr;
+  splits = workspace ? splits_that_fit(splits, (int64_t)B * Hq, D, workspace_bytes) : 1;
+  const auto [o_part, lse, plan] = split_kv_carve(workspace, workspace_bytes, (int64_t)B * Hq, D, splits);
   cudaStream_t st = (cudaStream_t)stream;
   const dim3 grid(splits, Hkv, B);
 
@@ -663,70 +626,8 @@ extern "C" int chitu_b200_gqa_paged_decode_rope(const void* q, int64_t q_sb, voi
   }
   CB_LAUNCHED(1);
   if (splits > 1) {
-    if (dtype == CB_BF16) {
-      if (D == 128) cb::launch_k(merge_splits_kernel<__nv_bfloat16, 128>, dim3(B * Hq), dim3(128), 0, st, o_part, lse, (__nv_bfloat16*)out, splits);
-      else cb::launch_k(merge_splits_kernel<__nv_bfloat16, 64>, dim3(B * Hq), dim3(64), 0, st, o_part, lse, (__nv_bfloat16*)out, splits);
-    } else {
-      if (D == 128) cb::launch_k(merge_splits_kernel<__half, 128>, dim3(B * Hq), dim3(128), 0, st, o_part, lse, (__half*)out, splits);
-      else cb::launch_k(merge_splits_kernel<__half, 64>, dim3(B * Hq), dim3(64), 0, st, o_part, lse, (__half*)out, splits);
-    }
-    CB_LAUNCHED(1);
-  }
-  return 0;
-}
-
-namespace cb {
-int mla_decode_tc_launch(const void* q_nope, const void* q_pe, void* kv_cache, const void* new_kv,
-                         const int32_t* seqlens_excl, const int32_t* block_table, int bt_stride, int B, int H,
-                         int num_blocks, int num_splits, float scale, void* out, float* o_part, float* lse,
-                         const int32_t* plan, cudaStream_t st);
-// KV splits of the wgmma MLA kernel (1 CTA per SM): one wave of CTAs, whole pages, at least two pages per split, and
-// the partials must fit the workspace.  Deterministic in its arguments: the merging absorb-o kernel recomputes it.
-int mla_tc_num_splits(int B, int H, int max_len, int64_t workspace_bytes) {
-  const int hgroups = cdiv(H, 16);
-  int want = 132 / (B * hgroups);
-  const int pages = cdiv(max_len, 64);
-  int by_len = pages / 2;
-  int splits = want < by_len ? want : by_len;
-  if (splits > 128) splits = 128;
-  if (splits < 1) splits = 1;
-  if (workspace_bytes <= 0) return 1;
-  while (splits > 1 && chitu_b200_attn_workspace_bytes(B, H, 512, splits) > workspace_bytes) --splits;
-  return splits;
-}
-}  // namespace cb
-
-extern "C" int chitu_b200_mla_num_splits(int B, int H, int max_seqlen_hint, int64_t workspace_bytes) {
-  return cb::mla_tc_num_splits(B, H, max_seqlen_hint, workspace_bytes);
-}
-
-extern "C" int chitu_b200_mla_decode(const void* q_nope, const void* q_pe, void* kv_cache,
-                                     const void* new_kv, const int32_t* seqlens_excl,
-                                     const int32_t* block_table, int bt_stride, int B, int H, int C, int R,
-                                     int page_size, int num_blocks, int max_seqlen_hint, float softmax_scale, void* out,
-                                     void* workspace, int64_t workspace_bytes, void* stream) {
-  CB_ARG(q_nope && q_pe && kv_cache && seqlens_excl && block_table);
-  CB_ARG(B >= 0 && H > 0 && bt_stride > 0 && num_blocks > 0);
-  if (C != kMlaC || R != kMlaR)
-    return fail(-1, "mla_decode: only kv_lora_rank=512, qk_rope_head_dim=64 is built (got %d,%d)", C, R);
-  // the kernel stages one 64-token page per tile; the reference builds 64-token pages for absorbed MLA
-  // (backend.py:234-237) and its append indexes pages with a literal 64
-  if (page_size != 64) return fail(-1, "mla_decode: page_size must be 64 (got %d)", page_size);
-  if (B == 0) return 0;
-  if (!cb::tma_available()) return fail(-3, "mla_decode: TMA is not available");
-  const int max_len = max_seqlen_hint > 0 ? max_seqlen_hint : bt_stride * page_size;
-  cudaStream_t st = (cudaStream_t)stream;
-  const int splits = cb::mla_tc_num_splits(B, H, max_len, workspace ? workspace_bytes : 0);
-  float* o_part = (float*)workspace;
-  float* lse = o_part ? o_part + (int64_t)B * H * splits * kMlaC : nullptr;
-  // a split plan written by chitu_b200_attn_plan for this step (last 256 bytes of the workspace) overrides the
-  // hint-derived keys per split: ragged batches get splits of equal size instead of equal count
-  const int32_t* plan = workspace ? (const int32_t*)((const uint8_t*)workspace + workspace_bytes - 256) : nullptr;
-  int rc = cb::mla_decode_tc_launch(q_nope, q_pe, kv_cache, new_kv, seqlens_excl, block_table, bt_stride, B, H, num_blocks,
-                                    splits, softmax_scale, out, o_part, lse, plan, st);
-  if (rc) return rc;
-  if (splits > 1 && out) {        // out == NULL: the caller merges (chitu_b200_mla_absorb_o_merge_quant)
-    cb::launch_k(merge_splits_kernel<__nv_bfloat16, kMlaC>, dim3(B * H), dim3(256), 0, st, o_part, lse, (__nv_bfloat16*)out, splits);
+    int rc = launch_merge_splits(o_part, lse, out, B * Hq, splits, D, dtype, st);
+    if (rc) return rc;
     CB_LAUNCHED(1);
   }
   return 0;
@@ -817,7 +718,7 @@ __global__ void __launch_bounds__(256) mla_absorb_o_kernel(const __nv_bfloat16* 
                                                           __nv_bfloat16* __restrict__ x_out) {
   cb::pdl_launch_dependents();
   __shared__ float s_o[MT][128];
-  __shared__ float s_mw[MT][128];                               // normalised split weights (num_splits <= 128)
+  __shared__ float s_mw[MT][kMaxSplits];                        // normalised split weights
   extern __shared__ __align__(16) uint8_t s_x_raw[];            // [MT][C] bf16 latent outputs of this head
   __nv_bfloat16* s_x = reinterpret_cast<__nv_bfloat16*>(s_x_raw);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -1036,10 +937,9 @@ extern "C" int chitu_b200_mla_absorb_o_merge_quant(const void* workspace, int64_
   CB_ARG(workspace && wkv_b && (out || q_out) && B >= 0 && H > 0 && dn > 0 && dv == 128 && C == kMlaC);
   CB_ARG((q_out == nullptr) == (q_scales == nullptr) && max_seqlen_hint > 0);
   if (B == 0) return 0;
-  const int splits = cb::mla_tc_num_splits(B, H, max_seqlen_hint, workspace_bytes);
-  CB_ARG(splits <= 128);
-  const float* o_part = (const float*)workspace;
-  const float* lse = o_part + (int64_t)B * H * splits * kMlaC;
+  const int splits = mla_num_splits(B, H, max_seqlen_hint, workspace_bytes);
+  CB_ARG(split_kv_bytes((int64_t)B * H, kMlaC, splits) <= workspace_bytes);
+  const auto [o_part, lse, plan] = split_kv_carve((void*)workspace, workspace_bytes, (int64_t)B * H, kMlaC, splits);
   constexpr int MT = 2;
   dim3 grid(H, cdiv(B, MT));
   cb::launch_k(mla_absorb_o_kernel<MT>, grid, dim3(256), (size_t)MT * C * 2, (cudaStream_t)stream,

@@ -18,6 +18,7 @@
 #include <string.h>
 
 #include "common.cuh"
+#include "gemm.cuh"
 
 using namespace cb;
 

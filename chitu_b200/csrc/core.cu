@@ -2,6 +2,7 @@
 #include <string.h>
 
 #include "common.cuh"
+#include "splitkv.cuh"
 
 namespace cb {
 
@@ -247,8 +248,8 @@ extern "C" int chitu_b200_moe_align_block_size(const void* topk_ids, int ids_dty
 //    finalize_cache_single_decode (:211-215, seq_len += 1) of the previous step, so one launch per decode step suffices.
 //  * attn_plan      : AttnBackend.prepare_metadata_for_decode (attn_backend.py:515-534; FlashMLA get_mla_metadata,
 //    third_party/FlashMLA/csrc/flash_fwd_mla_metadata.cu:5-75): a length-aware split-KV plan — the number of keys per
-//    split (whole pages) such that the batch's splits fill one wave of CTAs; written to the last 256 bytes of the
-//    attention workspace, where the decode kernels find it.
+//    split (whole pages) such that the batch's splits fill one wave of CTAs; written to the plan tail of the attention
+//    workspace (splitkv.cuh), where the MLA decode kernel finds it.
 //
 // Neither kernel triggers its dependents early (no griddepcontrol.launch_dependents): everything launched after them
 // sees their writes, even kernels that prefetch before their own griddepcontrol.wait.
@@ -283,9 +284,6 @@ extern "C" int chitu_b200_decode_prepare(int32_t* seq_lens_excl, int32_t* seq_le
   return 0;
 }
 
-// plan words (int32) at workspace + workspace_bytes - 256:
-//   [0] magic 0x504c414e ("PLAN")  [1] keys per split (multiple of the page size)  [2] max splits of a request
-//   [3] total splits of the batch  [4] B  [5] page size  [6] heads the plan was made for
 __global__ void attn_plan_kernel(const int32_t* __restrict__ seqlens_incl, int B, int page_size, int slots,
                                  int max_splits, int min_pages, int heads, int32_t* __restrict__ plan) {
   cb::pdl_wait();
@@ -324,14 +322,14 @@ __global__ void attn_plan_kernel(const int32_t* __restrict__ seqlens_incl, int B
     ++pps;
   }
   if (lane == 0) {
-    plan[1] = pps * page_size;
-    plan[2] = mx;
-    plan[3] = total;
-    plan[4] = B;
-    plan[5] = page_size;
-    plan[6] = heads;
+    plan[cb::kPlanWordKeysPerSplit] = pps * page_size;
+    plan[cb::kPlanWordMaxSplits] = mx;
+    plan[cb::kPlanWordTotalSplits] = total;
+    plan[cb::kPlanWordBatch] = B;
+    plan[cb::kPlanWordPageSize] = page_size;
+    plan[cb::kPlanWordHeads] = heads;
     __threadfence();
-    plan[0] = 0x504c414e;
+    plan[cb::kPlanWordMagic] = cb::kPlanMagic;
   }
 }
 
@@ -343,10 +341,9 @@ extern "C" int chitu_b200_attn_plan(const int32_t* seqlens_incl, int B, int head
   int slots = 132 / hgroups;                                  // one CTA per H100 SM
   if (slots < 1) slots = 1;
   // the grid the decode kernel will be launched with for this (B, heads, hint): upper bound of a request's splits
-  const int max_splits = chitu_b200_mla_num_splits(B, heads, max_seqlen_hint, workspace_bytes);
-  int32_t* plan = (int32_t*)((uint8_t*)workspace + workspace_bytes - 256);
+  const int max_splits = cb::mla_num_splits(B, heads, max_seqlen_hint, workspace_bytes);
   cb::launch_k(attn_plan_kernel, dim3(1), dim3(32), 0, (cudaStream_t)stream, seqlens_incl, B, page_size, slots, max_splits,
-               2, heads, plan);
+               2, heads, cb::split_kv_plan(workspace, workspace_bytes));
   CB_LAUNCHED(1);
   return 0;
 }

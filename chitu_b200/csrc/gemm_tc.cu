@@ -27,14 +27,13 @@
 #include <type_traits>
 
 #include "common.cuh"
+#include "gemm.cuh"
 #include "tc_ptx.cuh"
 #include "wgmma.cuh"
 
 namespace cb {
 
 namespace {
-
-enum { KIND_16 = 0, KIND_FP8 = 1, KIND_I8 = 2, KIND_SOFT = 3 };   // SOFT: fp8 weights -> bf16 in shared memory, bf16 MMA
 
 constexpr int kTileN = 128;        // weight rows per CTA tile (two wgmma M = 64 halves)
 constexpr int kStageRowBytes = 128;  // bytes of K per stage row (one 128B swizzle atom)

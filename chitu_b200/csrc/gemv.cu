@@ -7,6 +7,7 @@
 // wgmma + TMA swap-AB kernel in gemm_tc.cu is the tensor-core implementation of the same
 // entry points (impl = 2) and the default for M > 2.
 #include "common.cuh"
+#include "gemm.cuh"
 
 using namespace cb;
 

@@ -32,14 +32,11 @@
 #include <limits.h>
 
 #include "common.cuh"
+#include "splitkv.cuh"
 #include "tc_ptx.cuh"
 #include "wgmma.cuh"
 
 namespace cb {
-int gqa_prefill_num_splits(int ctas_without_split, int max_len, int slots, int B, int H, int DV, int64_t workspace_bytes);
-cudaError_t launch_merge_splits(const float* o_part, const float* lse, void* out, int rows, int splits, int dtype,
-                                cudaStream_t st);
-
 namespace {
 
 constexpr int kD = 128;
@@ -334,12 +331,13 @@ extern "C" int chitu_b200_gqa_paged_prefill(const void* q, void* k_cache, void* 
 
   const int row_tiles = cdiv((int64_t)sq * G, kRows);
   const int max_len = max_seqlen_hint > 0 ? max_seqlen_hint : bt_stride * page_size;
-  const int splits = gqa_prefill_num_splits(row_tiles * Hkv * B, max_len, 132 * kCtasPerSm, B, sq * Hq, kD,
-                                            workspace ? workspace_bytes : 0);
+  // the decode kernels' wave rule on this kernel's CTAs, shrunk to the workspace (none: 1 split)
+  const int64_t rows = (int64_t)B * sq * Hq;
+  int splits = pick_splits_waves(row_tiles * Hkv * B, max_len, 132 * kCtasPerSm);
+  splits = workspace ? splits_that_fit(splits, rows, kD, workspace_bytes) : 1;
   if ((int64_t)row_tiles * splits > INT_MAX)
     return fail(-1, "gqa_paged_prefill: %d row tiles x %d splits exceed the grid", row_tiles, splits);
-  float* o_part = splits > 1 ? (float*)workspace : nullptr;
-  float* lse = o_part ? o_part + (int64_t)B * sq * Hq * splits * kD : nullptr;
+  const auto [o_part, lse, plan] = split_kv_carve(splits > 1 ? workspace : nullptr, workspace_bytes, rows, kD, splits);
 
   // the caches as (D, Hkv, num_blocks * page): a box (64, 1, 64) is 64 keys x 64 dims of one head inside one page
   CUtensorMap mk, mv;
@@ -390,7 +388,8 @@ extern "C" int chitu_b200_gqa_paged_prefill(const void* q, void* k_cache, void* 
 #undef LAUNCH_PREFILL
   CB_LAUNCHED(1);
   if (splits > 1) {
-    launch_merge_splits(o_part, lse, out, B * sq * Hq, splits, dtype, st);
+    rc = launch_merge_splits(o_part, lse, out, B * sq * Hq, splits, kD, dtype, st);
+    if (rc) return rc;
     CB_LAUNCHED(1);
   }
   return 0;

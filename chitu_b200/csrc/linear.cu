@@ -1,36 +1,9 @@
 // C-ABI entry points of the decode linears; dispatch between the SIMT weight-streaming path
 // (gemv.cu) and the wgmma + TMA swap-AB path (gemm_tc.cu).
 #include "common.cuh"
-
-namespace cb {
-// gemv.cu
-int simt_linear16(const void* x, const void* w, const void* bias, const void* residual, void* y, int M,
-                  int N, int K, int dtype, cudaStream_t st);
-int simt_fp8_gemm(const void* a, const float* a_s, const void* b, const float* b_s, void* c, int M, int N,
-                  int K, cudaStream_t st);
-int simt_soft_fp8_gemm(const void* a, const void* b, const float* b_s, void* c, int M, int N, int K,
-                       int out_dtype, cudaStream_t st);
-int simt_w8a8_gemm(void* out, const int8_t* a, const int8_t* b, const float* a_scales,
-                   const float* b_scales, const void* bias, int M, int N, int K, cudaStream_t st);
-// gemm_tc.cu
-bool tc_supported(int kind, int M, int N, int K);
-int tc_linear16(const void* x, const void* w, const void* bias, const void* residual, void* y, int M, int N,
-                int K, int dtype, void* ws, int64_t ws_bytes, cudaStream_t st, void* comm = nullptr);
-int tc_fp8_gemm(const void* a, const float* a_s, const void* b, const float* b_s, void* c, int M, int N,
-                int K, const void* residual, void* ws, int64_t ws_bytes, cudaStream_t st, void* comm = nullptr);
-int64_t comm_slot_bytes(void* handle);
-int tc_w8a8_gemm(void* out, const int8_t* a, const int8_t* b, const float* a_scales, const float* b_scales,
-                 const void* bias, int M, int N, int K, void* ws, int64_t ws_bytes, cudaStream_t st);
-int tc_soft_fp8_gemm(const void* a, const void* b, const float* b_s, void* c, int M, int N, int K, void* ws,
-                     int64_t ws_bytes, cudaStream_t st);
-int tc_linear16_silu_pairs(const void* x, const void* w, void* y, int M, int N, int K, void* ws, int64_t ws_bytes,
-                           cudaStream_t st);
-int64_t tc_workspace_bytes(int M, int N);
-}  // namespace cb
+#include "gemm.cuh"
 
 using namespace cb;
-
-enum { KIND_16 = 0, KIND_FP8 = 1, KIND_I8 = 2, KIND_SOFT = 3 };
 
 // auto policy: the persistent stream-K wgmma kernel (bs=16 needs tensor cores outright: 16 tokens x 2 flop per weight
 // byte exceeds the FMA pipes); the SIMT path remains for

@@ -22,13 +22,14 @@
 #include <cuda.h>
 
 #include "common.cuh"
+#include "splitkv.cuh"
 #include "tc_ptx.cuh"
 #include "wgmma.cuh"
 
 namespace cb {
 namespace {
 
-constexpr int kC = 512, kR = 64, kRow = kC + kR;
+constexpr int kC = kMlaC, kR = 64, kRow = kC + kR;
 constexpr int kTile = 64;                      // keys per tile == page size
 constexpr int kSlot = kTile * 128;             // 8 KB: one TMA box [64 keys x 128 B]
 constexpr int kNSM = 22;                       // main ring slots
@@ -103,9 +104,10 @@ __global__ void __launch_bounds__(kThreads, 1) mla_decode_tc_kernel(
   // length-aware plan of chitu_b200_attn_plan (written by a kernel that does not trigger dependents early): equal-size
   // splits over a ragged batch; splits past a request's end do nothing (their LSE is -inf)
   // (only a plan made for THIS launch shape — same batch, same head count — is honoured)
-  if (plan && plan[0] == 0x504c414e && plan[5] == kTile && plan[4] == (int)gridDim.z && plan[6] == H && plan[1] >= per &&
-      (L + plan[1] - 1) / plan[1] <= num_splits)
-    per = plan[1];
+  if (plan && plan[kPlanWordMagic] == kPlanMagic && plan[kPlanWordPageSize] == kTile &&
+      plan[kPlanWordBatch] == (int)gridDim.z && plan[kPlanWordHeads] == H && plan[kPlanWordKeysPerSplit] >= per &&
+      (L + plan[kPlanWordKeysPerSplit] - 1) / plan[kPlanWordKeysPerSplit] <= num_splits)
+    per = plan[kPlanWordKeysPerSplit];
   const int begin = split * per;
   const int end = min(begin + per, L);
   const int ntiles = end > begin ? (end - begin + kTile - 1) / kTile : 0;
@@ -364,13 +366,39 @@ __global__ void __launch_bounds__(kThreads, 1) mla_decode_tc_kernel(
 
 }  // namespace
 
+}  // namespace cb
+
+extern "C" int chitu_b200_mla_num_splits(int B, int H, int max_seqlen_hint, int64_t workspace_bytes) {
+  return cb::mla_num_splits(B, H, max_seqlen_hint, workspace_bytes);
+}
+
 // q_nope [B,H,512], q_pe [B,H,64], kv_cache [num_blocks,64,576] bf16; new_kv [B,576] or null; seqlens_excl [B] int32;
-// block_table [B, bt_stride] int32.  num_splits == 1: out [B,H,512] bf16; else o_part [B,H,splits,512] fp32 (normalised)
-// and lse [B,H,splits] (log2 domain) — the layout merge_splits_kernel / the merging absorb-o kernel consume.
-int mla_decode_tc_launch(const void* q_nope, const void* q_pe, void* kv_cache, const void* new_kv,
-                         const int32_t* seqlens_excl, const int32_t* block_table, int bt_stride, int B, int H,
-                         int num_blocks, int num_splits, float scale, void* out, float* o_part, float* lse,
-                         const int32_t* plan, cudaStream_t st) {
+// block_table [B, bt_stride] int32.  One split writes out [B,H,512] bf16 directly; more splits write their partials to
+// the workspace (splitkv.cuh) and merge them into `out`.  out == NULL: the partials stay in the workspace, even for one
+// split, for chitu_b200_mla_absorb_o_merge_quant to merge.
+extern "C" int chitu_b200_mla_decode(const void* q_nope, const void* q_pe, void* kv_cache,
+                                     const void* new_kv, const int32_t* seqlens_excl,
+                                     const int32_t* block_table, int bt_stride, int B, int H, int C, int R,
+                                     int page_size, int num_blocks, int max_seqlen_hint, float softmax_scale, void* out,
+                                     void* workspace, int64_t workspace_bytes, void* stream) {
+  using namespace cb;
+  CB_ARG(q_nope && q_pe && kv_cache && seqlens_excl && block_table);
+  CB_ARG(B >= 0 && H > 0 && bt_stride > 0 && num_blocks > 0);
+  if (C != kC || R != kR)
+    return fail(-1, "mla_decode: only kv_lora_rank=512, qk_rope_head_dim=64 is built (got %d,%d)", C, R);
+  // the kernel stages one 64-token page per tile; the reference builds 64-token pages for absorbed MLA
+  // (backend.py:234-237) and its append indexes pages with a literal 64
+  if (page_size != kTile) return fail(-1, "mla_decode: page_size must be 64 (got %d)", page_size);
+  if (B == 0) return 0;
+  CB_ARG(workspace == nullptr || workspace_bytes >= kPlanBytes);
+  CB_ARG(out || (workspace && workspace_bytes >= split_kv_bytes((int64_t)B * H, kC, 1)));
+  if (!tma_available()) return fail(-3, "mla_decode: TMA is not available");
+  const int max_len = max_seqlen_hint > 0 ? max_seqlen_hint : bt_stride * page_size;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int splits = mla_num_splits(B, H, max_len, workspace ? workspace_bytes : 0);
+  // a split plan written by chitu_b200_attn_plan for this step overrides the hint-derived keys per split: ragged
+  // batches get splits of equal size instead of equal count
+  const auto [o_part, lse, plan] = split_kv_carve(workspace, workspace_bytes, (int64_t)B * H, kC, splits);
   CUtensorMap map;
   // the cache as a 2-D [num_rows, 576] bf16 tensor, box = [64 rows x 64 elements (128 B)]
   int rc = make_tma_map_2d(&map, kv_cache, (int64_t)num_blocks * kTile, kRow, 2, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, kTile);
@@ -381,15 +409,18 @@ int mla_decode_tc_launch(const void* q_nope, const void* q_pe, void* kv_cache, c
     CB_CUDA(cudaFuncSetAttribute(mla_decode_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr = true;
   }
-  dim3 grid(num_splits, cdiv(H, 16), B);
+  dim3 grid(splits, cdiv(H, 16), B);
   launch_k(mla_decode_tc_kernel, grid, dim3(kThreads), smem, st, map, (const __nv_bfloat16*)q_nope,
            (const __nv_bfloat16*)q_pe, (__nv_bfloat16*)kv_cache, (const __nv_bfloat16*)new_kv, seqlens_excl, block_table,
-           bt_stride, H, scale, num_splits, o_part, lse, (__nv_bfloat16*)out, plan);
+           bt_stride, H, softmax_scale, splits, o_part, lse, (__nv_bfloat16*)out, plan);
   CB_LAUNCHED(1);
+  if (splits > 1 && out) {
+    rc = launch_merge_splits(o_part, lse, out, B * H, splits, kC, CB_BF16, st);
+    if (rc) return rc;
+    CB_LAUNCHED(1);
+  }
   return 0;
 }
-
-}  // namespace cb
 
 CB_DEFINE_TL_SETTER(mla_tc)
 #ifdef CB_TIMELINE

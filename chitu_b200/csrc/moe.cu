@@ -11,6 +11,8 @@
 #include <string.h>
 
 #include "common.cuh"
+#include "gemm.cuh"
+#include "tc_ptx.cuh"
 
 using namespace cb;
 
@@ -797,20 +799,6 @@ __global__ void moe_combine_kernel(const __nv_bfloat16* __restrict__ c3, const i
 
 }  // namespace
 
-namespace cb {
-int tc_linear16(const void* x, const void* w, const void* bias, const void* residual, void* y, int M, int N,
-                int K, int dtype, void* ws, int64_t ws_bytes, cudaStream_t st, void* comm = nullptr);
-int64_t comm_slot_bytes(void* handle);
-bool tc_supported(int kind, int M, int N, int K);
-int64_t tc_workspace_bytes(int M, int N);
-bool tma_available();
-int64_t tc_max_tiles();
-int tc_grouped_gemm(int kind, const void* xs, const float* a_s, const void* w, const float* b_s, void* out, int rows,
-                    int E, int Ng, int K, int max_tokens_per_expert, const int* g_num_tiles, const int* g_tile_wrow,
-                    const int* g_tile_xrow, const int* g_tile_cnt, const float* row_scale, const int* out_rows, void* ws,
-                    int64_t ws_bytes, cudaStream_t st);
-}  // namespace cb
-
 extern "C" int64_t chitu_b200_moe_gate_workspace_bytes(int T, int E) {
   return align256(cb::tc_workspace_bytes(T, E)) + align256((int64_t)T * E * 2);
 }
@@ -829,7 +817,7 @@ extern "C" int chitu_b200_moe_gate(const void* x, const void* w, const void* bia
   // gate logits: one weight-streaming wgmma GEMM over all tokens (the old per-token in-kernel GEMV
   // re-read the 3.67 MB gate matrix once per token: 360 us per layer at bs=16)
   const __nv_bfloat16* logits = nullptr;
-  if (workspace && workspace_bytes >= chitu_b200_moe_gate_workspace_bytes(T, E) && cb::tc_supported(0, T, E, dim)) {
+  if (workspace && workspace_bytes >= chitu_b200_moe_gate_workspace_bytes(T, E) && cb::tc_supported(cb::KIND_16, T, E, dim)) {
     // layout: [GEMM scratch (ticket counters first: they must stay zero between calls) | logits]
     const int64_t lin = cb::tc_workspace_bytes(T, E);
     void* lg = (uint8_t*)workspace + align256(lin);
@@ -990,7 +978,7 @@ extern "C" int chitu_b200_moe_grouped_gemm(const void* A, const void* B, void* C
                sorted_token_ids, expert_ids, num_tokens_post_padded, EM, numel, top_k, block_m, E, K, N, quant, xs, xs_s,
                (__nv_bfloat16*)xs, (__nv_bfloat16*)C);
   CB_LAUNCHED(1);
-  const int gkind = wmode == 1 ? 1 : (wmode == 2 ? 3 : 0);
+  const int gkind = wmode == 1 ? cb::KIND_FP8 : (wmode == 2 ? cb::KIND_SOFT : cb::KIND_16);
   return cb::tc_grouped_gemm(gkind, xs, xs_s, B, B_scale, C, EM, E, N, K, block_m, num_tiles, t_w, t_x, t_c,
                              mul_routed_weight ? row_scale : nullptr, out_rows, gws, cb::tc_workspace_bytes(128, 128), st);
 }
@@ -1119,7 +1107,7 @@ static int fused_experts_impl(const void* x, const void* w1, const void* w2, con
     cb::launch_k(moe_gather_quant_kernel, dim3(cdiv(P * (K1 / 128), 8)), dim3(256), 0, st, (const __nv_bfloat16*)x,
                  (const int*)pl.pair_sorted, (const int*)pl.seg_start, E, topk, K1, quant, xs, xs_s, (__nv_bfloat16*)xs);
     CB_LAUNCHED(1);
-    const int gkind = wmode == 1 ? 1 : (wmode == 2 ? 3 : 0);     // KIND_FP8 / KIND_SOFT (fp8 weights -> bf16 in smem) / KIND_16
+    const int gkind = wmode == 1 ? cb::KIND_FP8 : (wmode == 2 ? cb::KIND_SOFT : cb::KIND_16);
     int rc = cb::tc_grouped_gemm(gkind, xs, xs_s, w1, w1_s, c1, (int)P, E, N1, K1, BN, pl.num_tiles1, pl.tile1_wrow,
                                  pl.tile1_xrow, pl.tile1_cnt, nullptr, nullptr, gws, cb::tc_workspace_bytes(128, 128), st);
     if (rc) return rc;

@@ -15,6 +15,8 @@ from __future__ import annotations
 
 import torch
 
+from . import _lib
+
 _ws = {}
 _retired = []
 
@@ -48,19 +50,24 @@ def reserve(tag: str, nbytes: int, device) -> None:
     get(tag, nbytes, device)
 
 
-def reserve_decode(device, max_reqs: int, *, heads: int = 128, head_dim_v: int = 512, max_splits: int = 128,
-                   max_out_features: int = 1 << 18, topk: int = 9, num_experts: int = 257, expert_n1: int = 4096,
-                   expert_k: int = 7168, attn_cap_bytes: int = 256 << 20) -> None:
+def attn_bytes(B: int, heads: int, head_dim_v: int, cap_bytes: int = 256 << 20) -> int:
+    """Size of the split-KV attention workspace for B x heads rows of head_dim_v: the partials of the largest split
+    count, halving from the library's maximum, that fit `cap_bytes`, plus the split plan."""
+    lib = _lib.load()
+    splits = _lib.ATTN_MAX_SPLITS
+    while splits > 1 and lib.chitu_b200_attn_workspace_bytes(B, heads, head_dim_v, splits) > cap_bytes:
+        splits //= 2
+    return lib.chitu_b200_attn_workspace_bytes(B, heads, head_dim_v, splits)
+
+
+def reserve_decode(device, max_reqs: int, *, heads: int = 128, head_dim_v: int = 512, max_out_features: int = 1 << 18,
+                   topk: int = 9, num_experts: int = 257, expert_n1: int = 4096, expert_k: int = 7168,
+                   attn_cap_bytes: int = 256 << 20) -> None:
     """Size every workspace tag the plugin path uses for a decode batch of up to `max_reqs` requests, so that
     graphs captured at any smaller batch size, in any order, share buffers that never move."""
-    from . import _lib
-
     lib = _lib.load()
     B = max(int(max_reqs), 1)
-    splits = max_splits
-    while splits > 1 and lib.chitu_b200_attn_workspace_bytes(B, heads, head_dim_v, splits) > attn_cap_bytes:
-        splits //= 2
-    reserve("attn", lib.chitu_b200_attn_workspace_bytes(B, heads, head_dim_v, splits), device)
+    reserve("attn", attn_bytes(B, heads, head_dim_v, attn_cap_bytes), device)
     reserve("linear", lib.chitu_b200_linear_workspace_bytes(B, max_out_features), device)
     reserve("moe", lib.chitu_b200_moe_workspace_bytes(B, topk, num_experts, expert_n1, expert_k), device)
     reserve("moe_gate", lib.chitu_b200_moe_gate_workspace_bytes(B, max(num_experts, 8)), device)

@@ -224,7 +224,8 @@ int chitu_b200_gqa_paged_prefill(const void* q, void* k_cache, void* v_cache, co
  * seqlens_excl:[B] (length before this token) ; attention runs over seqlens_excl+1 keys when
  * new_kv != NULL else over seqlens_excl keys.  out:[B,H,C] (latent space). bf16.
  * page_size must be 64; num_blocks = kv_cache.shape[0] (bounds the TMA tensor map that stages whole pages).
- * out == NULL: the split merge is deferred to chitu_b200_mla_absorb_o_merge_quant. */
+ * out == NULL: the split merge is deferred to chitu_b200_mla_absorb_o_merge_quant, and the workspace must hold the
+ * partials of one split (chitu_b200_attn_workspace_bytes(B, H, C, 1)).  A workspace holds at least the 256-byte plan. */
 int chitu_b200_mla_decode(const void* q_nope, const void* q_pe, void* kv_cache, const void* new_kv,
                           const int32_t* seqlens_excl, const int32_t* block_table, int bt_stride,
                           int B, int H, int C, int R, int page_size, int num_blocks, int max_seqlen_hint,
@@ -303,7 +304,8 @@ int chitu_b200_mla_absorb_o_quant(const void* x, const void* wkv_b, void* out, v
                                   int B, int H, int dn, int dv, int C, void* stream);
 /* Same, but the latent input is the split-KV partials that chitu_b200_mla_decode(out = NULL) left in `workspace`
  * (the LSE merge of triton_decode_attention.py:185-232 happens while staging: one launch instead of merge +
- * absorb).  B, H, max_seqlen_hint, workspace(_bytes) must be those passed to chitu_b200_mla_decode.
+ * absorb).  B, H, max_seqlen_hint, workspace(_bytes) must be those passed to chitu_b200_mla_decode; a workspace too
+ * small for the partials of the recomputed split count is refused.
  * x_out (may be NULL): the merged latent attention output [B,H,C] bf16. */
 int chitu_b200_mla_absorb_o_merge_quant(const void* workspace, int64_t workspace_bytes, int max_seqlen_hint,
                                         const void* wkv_b, void* x_out, void* out, void* q_out, float* q_scales,

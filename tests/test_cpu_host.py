@@ -43,6 +43,46 @@ def test_bad_arguments_return_status_not_abort():
     rc = lib.chitu_b200_mla_decode(dummy, dummy, dummy, None, dummy, dummy, 1, 1, 16, 512, 64, 32, 4, 0, 1.0, None, None, 0, None)
     assert rc < 0 and b"page" in lib.chitu_b200_last_error()
     assert lib.chitu_b200_attn_workspace_bytes(16, 16, 512, 8) > 16 * 16 * 8 * 512 * 4
+    # out = NULL leaves the partials in the workspace, which must hold one split; any workspace must hold the split plan
+    for out, ws, ws_bytes in ((None, None, 0), (None, dummy, 100), (dummy, dummy, 100)):
+        rc = lib.chitu_b200_mla_decode(dummy, dummy, dummy, None, dummy, dummy, 1, 1, 16, 512, 64, 64, 4, 0, 1.0, out, ws,
+                                       ws_bytes, None)
+        assert rc < 0 and b"workspace" in lib.chitu_b200_last_error()
+    # the merging absorb-o reads the partials of the split count it recomputes: one split here, one byte missing
+    one_split = lib.chitu_b200_attn_workspace_bytes(1, 16, 512, 1)
+    rc = lib.chitu_b200_mla_absorb_o_merge_quant(dummy, one_split - 1, 4096, dummy, None, dummy, None, None, 1, 16, 128,
+                                                 128, 512, None)
+    assert rc < 0 and b"workspace" in lib.chitu_b200_last_error()
+
+
+# chitu_b200_mla_num_splits(B, H, hint, workspace_bytes): {(B, H): one row per hint in _HINTS, one column per size in _WS}
+_HINTS, _WS = (200, 4096, 65536), (0, 100, 1 << 18, 1 << 22, 256 << 20)
+_MLA_SPLITS = {
+    (1, 16): [[1, 1, 2, 2, 2], [1, 1, 7, 32, 32], [1, 1, 7, 127, 128]],
+    (1, 40): [[1, 1, 2, 2, 2], [1, 1, 3, 32, 32], [1, 1, 3, 44, 44]],
+    (1, 128): [[1, 1, 1, 2, 2], [1, 1, 1, 15, 16], [1, 1, 1, 15, 16]],
+    (3, 16): [[1, 1, 2, 2, 2], [1, 1, 2, 32, 32], [1, 1, 2, 42, 44]],
+    (3, 40): [[1, 1, 1, 2, 2], [1, 1, 1, 14, 14], [1, 1, 1, 14, 14]],
+    (3, 128): [[1, 1, 1, 2, 2], [1, 1, 1, 5, 5], [1, 1, 1, 5, 5]],
+    (8, 16): [[1, 1, 1, 2, 2], [1, 1, 1, 15, 16], [1, 1, 1, 15, 16]],
+    (8, 40): [[1, 1, 1, 2, 2], [1, 1, 1, 5, 5], [1, 1, 1, 5, 5]],
+    (8, 128): [[1, 1, 1, 1, 2], [1, 1, 1, 1, 2], [1, 1, 1, 1, 2]],
+}
+
+
+def test_split_counts_and_workspace_sizes_are_pinned():
+    """The host arithmetic of the split-KV workspace: the MLA split count, the workspace size of a split count and the
+    capped size the Python side allocates."""
+    from chitu_b200 import _lib, workspace
+    lib = _lib.load()
+    got = {bh: [[lib.chitu_b200_mla_num_splits(*bh, hint, n) for n in _WS] for hint in _HINTS] for bh in _MLA_SPLITS}
+    assert got == _MLA_SPLITS
+    for args, want in (((1, 1, 64, 1), 516), ((16, 16, 512, 8), 4202752), ((16, 128, 512, 128), 537919744),
+                       ((256, 32, 128, 64), 270532864), ((3, 40, 128, 5), 309856)):
+        assert lib.chitu_b200_attn_workspace_bytes(*args) == want, args
+    for args, want in (((1, 128, 512), 33620224), ((64, 128, 512), 134480128), ((256, 32, 128), 135266560),
+                       ((4096, 128, 512), 1075839232)):
+        assert workspace.attn_bytes(*args) == want, args
 
 
 def test_round2_entries_validate_arguments():
