@@ -61,6 +61,7 @@ SIGNATURES = {
                                          P]),
     "chitu_b200_mla_decode": (I, [P, P, P, P, P, P, I, I, I, I, I, I, I, I, F, P, P, L, P]),
     "chitu_b200_mla_prefill": (I, [P, P, L, P, L, P, P, I, I, I, I, I, I, F, P, P]),
+    "chitu_b200_mla_paged_prefill": (I, [P, P, P, P, P, P, I, I, I, I, I, I, I, I, I, I, F, P, P, L, P]),
     "chitu_b200_debug_timeline": (I, [P]),
     "chitu_b200_debug_timeline_names": (c_char_p, []),
     "chitu_b200_decode_prepare": (I, [P, P, P, I, P, P, P, I, I, I, P]),

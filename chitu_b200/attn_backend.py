@@ -5,7 +5,8 @@ prepare_metadata_for_decode, attn_varlen_func (prefill: the absorbed-MLA form ru
 prefill kernel; GQA prefill stays on flash_attn / torch SDPA), attn_with_kvcache (GQA attention over the paged
 cache with in-place append: the decode kernel for seqlen_q == 1, the sm_90a multi-token kernel for seqlen_q > 1 —
 chunked prefill, prefill on a cached prefix, speculative verification) and mla_attn_with_kvcache (absorbed-MLA
-paged decode with fused append).
+attention over the paged latent cache: the decode kernel with fused append for one query token per request, the
+sm_90a multi-token kernel for seqlen_q > 1 — multi-token-prediction verification, chunked prefill on a cached prefix).
 """
 from __future__ import annotations
 
@@ -227,7 +228,17 @@ class B200AttnBackend(AttnBackend):
                               cache_seqlens_incl_this_decode: Union[int, torch.Tensor],
                               block_table: torch.Tensor, causal=True, window_size=(-1, -1), softcap=0.0,
                               softmax_scale=None):
+        """Absorbed-MLA attention over the paged latent cache.  q_nope [B, H, C] (or [B, 1, H, C]): one decode token
+        per request with the fused append of `kv` (chitu_b200_mla_decode), returned as [B, 1, H, C].
+        q_nope [B, sq, H, C] with sq > 1: multi-token-prediction verification or chunked prefill, see
+        `_mla_paged_prefill`."""
         require_cuda(q_nope, q_pe, kv_cache, block_table)
+        if q_nope.dim() == 4:
+            B, sq, H, C = q_nope.shape
+            if sq > 1:
+                return self._mla_paged_prefill(q_nope, q_pe, kv_cache, kv, cache_seqlens_excl_this_decode, block_table,
+                                               causal, window_size, softcap, softmax_scale)
+            q_nope, q_pe = q_nope.view(B, H, C), q_pe.view(B, H, q_pe.shape[-1])
         assert kv_cache.ndim == 3  # (num_blocks, block_size, dim)
         B, H, C = q_nope.shape
         R = q_pe.shape[-1]
@@ -252,3 +263,32 @@ class B200AttnBackend(AttnBackend):
             block_table.stride(0), B, H, C, R, page, kv_cache.size(0), int(hint), float(softmax_scale), ptr(o), ptr(ws), wsn,
             current_stream()), "mla_decode")
         return o.view(B, 1, H, -1)
+
+    def _mla_paged_prefill(self, q_nope, q_pe, kv_cache, kv, seq_excl, block_table, causal, window_size, softcap,
+                           softmax_scale):
+        """sq > 1 query tokens per request (chitu_b200_mla_paged_prefill): the B * sq rows of `kv` ([B, sq, C + R] in
+        any contiguous shape, or None) are appended at seq_excl[b] + i, then query i attends to the first
+        seq_excl[b] + sq keys (without kv: seq_excl[b]), bottom-right causal when `causal`.  The decode arithmetic and
+        default scale; returns [B, sq, H, C] bf16.  No host synchronisation, capturable in a CUDA graph, deterministic."""
+        if tuple(window_size) != (-1, -1) or softcap != 0.0:
+            raise RuntimeError("mla_paged_prefill: window_size and softcap are not built")
+        B, sq, H, C = q_nope.shape
+        R = q_pe.shape[-1]
+        assert kv_cache.ndim == 3 and kv_cache.size(2) == C + R and q_pe.shape == (B, sq, H, R)
+        assert q_nope.is_contiguous() and q_pe.is_contiguous() and kv_cache.is_contiguous()
+        assert q_nope.dtype == q_pe.dtype == kv_cache.dtype == torch.bfloat16
+        assert block_table.dtype == torch.int32 and block_table.stride(-1) == 1
+        assert seq_excl.dtype == torch.int32 and seq_excl.is_contiguous()
+        if kv is not None:
+            assert kv.dtype == torch.bfloat16 and kv.is_contiguous() and kv.numel() == B * sq * (C + R)
+        if softmax_scale is None:
+            softmax_scale = 1.0 / ((self.qk_rope_head_dim + self.qk_nope_head_dim) ** 0.5)
+        page = kv_cache.size(1)
+        o = torch.empty(B, sq, H, C, dtype=q_nope.dtype, device=q_nope.device)
+        ws, wsn = self._ws(B, H, C, q_nope.device)
+        hint = self.max_seq_len if self.max_seq_len else block_table.shape[1] * page
+        check(_lib.load().chitu_b200_mla_paged_prefill(
+            ptr(q_nope), ptr(q_pe), ptr(kv_cache), ptr(kv), ptr(seq_excl), ptr(block_table), block_table.stride(0), B, sq,
+            H, C, R, page, kv_cache.size(0), int(hint), int(bool(causal)), float(softmax_scale), ptr(o), ptr(ws), wsn,
+            current_stream()), "mla_paged_prefill")
+        return o

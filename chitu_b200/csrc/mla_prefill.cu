@@ -24,10 +24,20 @@
 // Scheduling: a 1-D grid of (row tile, sequence) with the LAST row tiles first: under the causal mask they see the most
 // keys, so the long CTAs start in the first wave and the short ones fill in behind them.
 // Deterministic: every key of a row is reduced by one CTA in a fixed order (no split over keys).
+//
+// Paged variant (mla_paged_prefill_kernel, behind AttnBackend.mla_attn_with_kvcache with seqlen_q = sq > 1:
+// multi-token-prediction verification, chunked prefill on a cached prefix): the same CTA over the paged latent cache
+// [num_blocks * 64, 576].  Request b's sq * H rows are row tiles as above (Lq = sq, Lk = seqlens_excl[b] (+ sq)); key
+// tile t is page block_table[b, t], K and V boxes come from the one cache map.  mla_append_kernel writes the new rows
+// first (PDL orders the two).  In the tile holding Lk the V rows >= Lk (unwritten slots, maybe NaN) are zeroed in shared
+// memory before P.V.  When row tiles x B CTAs cannot fill the GPU the keys are split; each split writes normalised fp32
+// partials + LSE (splitkv.cuh, rows = B * sq * H, staged through the ring) and launch_merge_splits merges them.  The
+// split count depends on host values only, so this variant is deterministic too.
 #include <cuda.h>
 #include <limits.h>
 
 #include "common.cuh"
+#include "splitkv.cuh"
 #include "tc_ptx.cuh"
 #include "wgmma.cuh"
 
@@ -45,6 +55,8 @@ constexpr int kPBytes = kRows * 128;           // P as [64 rows x 64 keys] bf16,
 constexpr int kSmemBytes = kTC * kSlot + kQBytes + kPBytes;
 constexpr int kOutPitch = kC * 2 + 16;         // staged output row in bytes (padded: the 4 rows a store touches differ in bank)
 static_assert(kRows * kOutPitch <= kQBytes, "the output tile is staged in the Q buffer");
+constexpr int kPartPitch = kC + 4;             // staged fp32 split-partial row in floats (a warp's stores differ in bank)
+static_assert(kRows * kPartPitch * 4 <= kTC * kSlot, "the fp32 partial tile is staged in the ring");
 constexpr float kLog2e = 1.4426950408889634f;
 constexpr float kRescaleThreshold = 8.f;       // log2 domain
 constexpr int kThreads = 256;
@@ -59,10 +71,17 @@ __device__ __forceinline__ void load_chunks(const CUtensorMap* mk, const CUtenso
   }
 }
 
-__global__ void __launch_bounds__(kThreads, 1) mla_prefill_kernel(
-    const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
-    const __grid_constant__ CUtensorMap map_v, const int32_t* __restrict__ cu_q, const int32_t* __restrict__ cu_k, int B,
-    int H, int row_tiles, int causal, float scale, __nv_bfloat16* __restrict__ out) {
+// One CTA of either variant.  Contiguous (kPaged = false): sequence b's rows and keys start at cu_q[b] / cu_k[b], map_q
+// holds q as [Tq * H, 576].  Paged: request b has sq query tokens at q row b * sq * H (map_q = q_nope [., 512], map_qpe
+// = q_pe [., 64]), Lk = seqlens_excl[b] (+ sq when appended) keys, key tile t is cache page block_table[b, t], and the
+// CTA takes split `split` of its key tiles.
+template <bool kPaged>
+__device__ __forceinline__ void mla_prefill_cta(
+    const CUtensorMap* map_q, const CUtensorMap* map_qpe, const CUtensorMap* map_k, const CUtensorMap* map_v,
+    const int32_t* __restrict__ cu_q, const int32_t* __restrict__ cu_k, const int32_t* __restrict__ seqlens_excl,
+    const int32_t* __restrict__ block_table, int bt_stride, int sq, int appended, int splits, int B, int H,
+    int row_tiles, int causal, float scale, float* __restrict__ o_part, float* __restrict__ lse,
+    __nv_bfloat16* __restrict__ out) {
   extern __shared__ __align__(1024) uint8_t mla_prefill_smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(mla_prefill_smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* s_ring = smem;                                   // [kTC][64 rows][128 B]  K / V chunks of one tile
@@ -75,13 +94,28 @@ __global__ void __launch_bounds__(kThreads, 1) mla_prefill_kernel(
   __shared__ float s_inv[kRows];                            // 1 / row sum (0 for a row that sees no key)
 
   const int b = blockIdx.x % B;
-  const int tile = row_tiles - 1 - blockIdx.x / B;          // last row tiles (most causal work) first
+  int tile, split = 0;
+  if constexpr (kPaged) {
+    split = blockIdx.x / B % splits;
+    tile = row_tiles - 1 - blockIdx.x / B / splits;
+  } else {
+    tile = row_tiles - 1 - blockIdx.x / B;                  // last row tiles (most causal work) first
+  }
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const bool wg0 = __shfl_sync(0xffffffffu, threadIdx.x / 128, 0) == 0;   // warp-uniform for the compiler (wgmma paths)
 
   cb::pdl_prologue();                                       // q, k, v and the lengths are written by earlier kernels
-  const int q0 = cu_q[b], Lq = cu_q[b + 1] - q0;
-  const int k0 = cu_k[b], Lk = cu_k[b + 1] - k0;
+  int q0, Lq, k0 = 0, Lk;                                   // q0: first query token of the sequence
+  if constexpr (kPaged) {
+    q0 = b * sq;
+    Lq = sq;
+    Lk = seqlens_excl[b] + (appended ? sq : 0);
+  } else {
+    q0 = cu_q[b];
+    Lq = cu_q[b + 1] - q0;
+    k0 = cu_k[b];
+    Lk = cu_k[b + 1] - k0;
+  }
   const int nrows = Lq * H;
   const int r0 = tile * kRows;
   if (r0 >= nrows) return;                                  // uniform over the CTA
@@ -91,6 +125,14 @@ __global__ void __launch_bounds__(kThreads, 1) mla_prefill_kernel(
   const int nkeys = lim(rlast);
   const int all_see = lim(r0);                              // keys below this are visible to every row of the tile
   const int ntiles = (nkeys + kTile - 1) / kTile;
+  int t_begin = 0, t_end = ntiles;                          // this CTA's key tiles
+  if constexpr (kPaged) {
+    const int per_split = (ntiles + splits - 1) / splits;
+    t_begin = min(ntiles, split * per_split);
+    t_end = min(ntiles, t_begin + per_split);
+  }
+  // paged: first cache row of key tile t (read by the thread that issues the tile's loads)
+  auto page_row = [&](int t) { return block_table[(int64_t)b * bt_stride + t] * kTile; };
   const uint64_t pol_kv = l2_policy_evict_last();           // K / V are re-read by every row tile of the sequence
 
   if (threadIdx.x == 0) {
@@ -99,10 +141,15 @@ __global__ void __launch_bounds__(kThreads, 1) mla_prefill_kernel(
     mbar_init(&p_full, 1);
     mbar_init(&p_empty, 4);                                 // one arrival per WG1 warp
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    if (ntiles > 0) {
+    if (t_end > t_begin) {
       mbar_expect_tx(&q_bar, kQBytes);
-      for (int c = 0; c < kKC; ++c) tma_load_2d(s_q + c * kSlot, &map_q, &q_bar, c * 64, q0 * H + r0, l2_policy_evict_first());
-      load_chunks(&map_k, &map_v, s_ring, full_b, 0, kTC, k0, pol_kv);
+      if constexpr (kPaged) {
+        for (int c = 0; c < kVC; ++c) tma_load_2d(s_q + c * kSlot, map_q, &q_bar, c * 64, q0 * H + r0, l2_policy_evict_first());
+        tma_load_2d(s_q + kVC * kSlot, map_qpe, &q_bar, 0, q0 * H + r0, l2_policy_evict_first());
+      } else {
+        for (int c = 0; c < kKC; ++c) tma_load_2d(s_q + c * kSlot, map_q, &q_bar, c * 64, q0 * H + r0, l2_policy_evict_first());
+      }
+      load_chunks(map_k, map_v, s_ring, full_b, 0, kTC, kPaged ? page_row(t_begin) : k0, pol_kv);
     }
   }
   if (threadIdx.x < kRows) s_m[threadIdx.x] = -INFINITY;
@@ -121,12 +168,14 @@ __global__ void __launch_bounds__(kThreads, 1) mla_prefill_kernel(
 #pragma unroll
   for (int x = 0; x < 16; ++x) l_part[x] = 0.f;
 
-  if (wg0 && ntiles > 0) mbar_wait(&q_bar, 0);
+  if (wg0 && t_end > t_begin) mbar_wait(&q_bar, 0);
   const float sc = scale * kLog2e;
-  for (int it = 0; it < ntiles; ++it) {
+  for (int it = 0; it < t_end - t_begin; ++it) {
     const uint32_t ph = it & 1;                             // phase of every chunk slot for tile it
-    const bool more = it + 1 < ntiles;
-    const int next_row = k0 + (it + 1) * kTile;             // rows past the sequence are masked; past the tensor, zero
+    const bool more = t_begin + it + 1 < t_end;
+    const int key0 = (t_begin + it) * kTile;
+    // contiguous: rows past the sequence are masked; past the tensor, zero
+    const int next_row = kPaged ? 0 : k0 + (it + 1) * kTile;
     if (wg0) {
       // ---- S^T = K . Q^T over the 9 chunks of 64 dims ----
       float s[32];
@@ -144,7 +193,6 @@ __global__ void __launch_bounds__(kThreads, 1) mla_prefill_kernel(
       wgmma_wait<0>();
 
       // ---- scale, mask (only tiles that reach past some row's last visible key), per-row tile max ----
-      const int key0 = it * kTile;
       if (key0 + kTile > all_see) {
 #pragma unroll
         for (int x = 0; x < 16; ++x) {
@@ -208,7 +256,8 @@ __global__ void __launch_bounds__(kThreads, 1) mla_prefill_kernel(
     } else {
       // ---- WG1: the K slots are free once P(it) is published; then the rescale WG0 decided for this tile ----
       mbar_wait(&p_full, ph);
-      if (more && threadIdx.x == 128) load_chunks(&map_k, &map_v, s_ring, full_b, 0, kKC, next_row, pol_kv);
+      if (more && threadIdx.x == 128)
+        load_chunks(map_k, map_v, s_ring, full_b, 0, kKC, kPaged ? page_row(t_begin + it + 1) : next_row, pol_kv);
       float al[16];
       bool need = false;
 #pragma unroll
@@ -223,6 +272,21 @@ __global__ void __launch_bounds__(kThreads, 1) mla_prefill_kernel(
 #pragma unroll
           for (int m = 0; m < 4; ++m) { o[m][e] *= al[x]; o[m][e + 2] *= al[x]; }
         }
+      }
+    }
+    if constexpr (kPaged) {
+      // ---- the tile holding Lk: V rows of keys >= Lk are unwritten cache slots (maybe NaN) and 0 * NaN would poison
+      // O, so they are zeroed (whole 128 B rows: the swizzle permutes within a row) in this warpgroup's V chunks ----
+      if (key0 + kTile > Lk) {
+        for (int m = 0; m < 4; ++m) {
+          const int c = kKC + vc0 + m;
+          mbar_wait(&full_b[c], ph);
+          for (int u = (Lk - key0) * 8 + (threadIdx.x & 127); u < kTile * 8; u += 128)
+            *reinterpret_cast<uint4*>(s_ring + c * kSlot + u * 16) = make_uint4(0, 0, 0, 0);
+        }
+        fence_async_smem();
+        if (wg0) asm volatile("bar.sync 1, 128;" ::: "memory");
+        else asm volatile("bar.sync 3, 128;" ::: "memory");
       }
     }
     // ---- O^T += V^T . P^T over this warpgroup's 4 V chunks, each a 64-dim M tile read MN-major ----
@@ -242,7 +306,9 @@ __global__ void __launch_bounds__(kThreads, 1) mla_prefill_kernel(
     if (more) {                                             // this warpgroup's V slots are free: load tile it + 1's
       if (wg0) asm volatile("bar.sync 1, 128;" ::: "memory");
       else asm volatile("bar.sync 3, 128;" ::: "memory");
-      if ((threadIdx.x & 127) == 0) load_chunks(&map_k, &map_v, s_ring, full_b, kKC + vc0, kKC + vc0 + 4, next_row, pol_kv);
+      if ((threadIdx.x & 127) == 0)
+        load_chunks(map_k, map_v, s_ring, full_b, kKC + vc0, kKC + vc0 + 4,
+                    kPaged ? page_row(t_begin + it + 1) : next_row, pol_kv);
     }
   }
 
@@ -258,9 +324,38 @@ __global__ void __launch_bounds__(kThreads, 1) mla_prefill_kernel(
       const int r = threadIdx.x;
       const float l = (red[0][r] + red[1][r]) + (red[2][r] + red[3][r]);
       s_inv[r] = l > 0.f ? 1.f / l : 0.f;
+      if constexpr (kPaged) s_m[r] = l > 0.f ? s_m[r] + log2f(l) : -INFINITY;   // the split's LSE (log2 domain)
     }
   }
   __syncthreads();                                          // s_inv ready; Q no longer read by any wgmma
+  if constexpr (kPaged) {
+    if (splits > 1) {
+      // ---- split partials: O^T / l as fp32 rows staged in the ring (free: no load is in flight after the last tile)
+      // -> 16-byte coalesced stores in the splitkv.cuh layout, row = q0 * H + r0 + r ----
+      float* stage = reinterpret_cast<float*>(s_ring);
+#pragma unroll
+      for (int x = 0; x < 16; ++x) {
+        const int r = 8 * (x >> 1) + qd + (x & 1);
+        const float inv = s_inv[r];
+        const int e = 4 * (x >> 1) + (x & 1);
+#pragma unroll
+        for (int m = 0; m < 4; ++m) {
+          stage[r * kPartPitch + 64 * (vc0 + m) + krow] = o[m][e] * inv;
+          stage[r * kPartPitch + 64 * (vc0 + m) + krow + 8] = o[m][e + 2] * inv;
+        }
+      }
+      __syncthreads();
+      for (int u = threadIdx.x; u < kRows * (kC / 4); u += kThreads) {
+        const int r = u / (kC / 4), c4 = u % (kC / 4);
+        if (r0 + r > rlast) break;                          // rows are consecutive in u
+        const int64_t row = (int64_t)q0 * H + r0 + r;
+        *reinterpret_cast<float4*>(o_part + (row * splits + split) * kC + c4 * 4) =
+            *reinterpret_cast<const float4*>(stage + r * kPartPitch + c4 * 4);
+        if (c4 == 0) lse[row * splits + split] = s_m[r];
+      }
+      return;
+    }
+  }
 #pragma unroll
   for (int x = 0; x < 16; ++x) {
     const int r = 8 * (x >> 1) + qd + (x & 1);
@@ -280,6 +375,42 @@ __global__ void __launch_bounds__(kThreads, 1) mla_prefill_kernel(
     if (r0 + r <= rlast)
       *reinterpret_cast<uint4*>(orow + (int64_t)r * kC + cu * 8) = *reinterpret_cast<const uint4*>(s_q + r * kOutPitch + cu * 16);
   }
+}
+
+__global__ void __launch_bounds__(kThreads, 1) mla_prefill_kernel(
+    const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
+    const __grid_constant__ CUtensorMap map_v, const int32_t* __restrict__ cu_q, const int32_t* __restrict__ cu_k, int B,
+    int H, int row_tiles, int causal, float scale, __nv_bfloat16* __restrict__ out) {
+  mla_prefill_cta<false>(&map_q, nullptr, &map_k, &map_v, cu_q, cu_k, nullptr, nullptr, 0, 0, 0, 1, B, H, row_tiles,
+                         causal, scale, nullptr, nullptr, out);
+}
+
+// K and V are the same cache rows: map_kv serves the 9 K boxes and, again, the first 8 as V (the second read of a page
+// is expected to hit L2)
+__global__ void __launch_bounds__(kThreads, 1) mla_paged_prefill_kernel(
+    const __grid_constant__ CUtensorMap map_qn, const __grid_constant__ CUtensorMap map_qpe,
+    const __grid_constant__ CUtensorMap map_kv, const int32_t* __restrict__ seqlens_excl,
+    const int32_t* __restrict__ block_table, int bt_stride, int B, int sq, int H, int appended, int row_tiles,
+    int splits, int causal, float scale, float* __restrict__ o_part, float* __restrict__ lse,
+    __nv_bfloat16* __restrict__ out) {
+  mla_prefill_cta<true>(&map_qn, &map_qpe, &map_kv, &map_kv, nullptr, nullptr, seqlens_excl, block_table, bt_stride, sq,
+                        appended, splits, B, H, row_tiles, causal, scale, o_part, lse, out);
+}
+
+// the B * sq new latent rows into the cache before the attention reads it: token i of request b goes to position
+// seqlens_excl[b] + i, pages indexed with a literal 64 as the reference's append does; one thread per 16 bytes
+__global__ void __launch_bounds__(256) mla_append_kernel(__nv_bfloat16* __restrict__ kv_cache,
+                                                         const __nv_bfloat16* __restrict__ new_kv,
+                                                         const int32_t* __restrict__ seqlens_excl,
+                                                         const int32_t* __restrict__ block_table, int bt_stride, int sq,
+                                                         int64_t units) {
+  cb::pdl_prologue();
+  const int64_t u = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (u >= units) return;
+  const int64_t row = u / (kRow / 8);                       // b * sq + i
+  const int b = (int)(row / sq), p = seqlens_excl[b] + (int)(row % sq);
+  const int64_t dst = ((int64_t)block_table[(int64_t)b * bt_stride + p / 64] * 64 + p % 64) * kRow;
+  reinterpret_cast<uint4*>(kv_cache + dst)[u % (kRow / 8)] = reinterpret_cast<const uint4*>(new_kv)[u];
 }
 
 }  // namespace
@@ -316,6 +447,66 @@ extern "C" int chitu_b200_mla_prefill(const void* q, const void* k, int64_t k_sb
   launch_k(mla_prefill_kernel, dim3(row_tiles * B), dim3(kThreads), smem, (cudaStream_t)stream, mq, mk, mv, cu_seqlens_q,
            cu_seqlens_k, B, H, row_tiles, causal ? 1 : 0, softmax_scale, (__nv_bfloat16*)out);
   CB_LAUNCHED(1);
+  return 0;
+}
+
+// mla_attn_with_kvcache with more than one query token per request (include/chitu_b200.h).
+extern "C" int chitu_b200_mla_paged_prefill(const void* q_nope, const void* q_pe, void* kv_cache, const void* new_kv,
+                                            const int32_t* seqlens_excl, const int32_t* block_table, int bt_stride,
+                                            int B, int sq, int H, int C, int R, int page_size, int num_blocks,
+                                            int max_seqlen_hint, int causal, float softmax_scale, void* out,
+                                            void* workspace, int64_t workspace_bytes, void* stream) {
+  using namespace cb;
+  CB_ARG(q_nope && q_pe && kv_cache && seqlens_excl && block_table && out);
+  CB_ARG(B >= 0 && sq >= 1 && H >= 1 && bt_stride > 0 && num_blocks > 0);
+  if (C != kC || R != kR)
+    return fail(-1, "mla_paged_prefill: only kv_lora_rank=512, qk_rope_head_dim=64 is built (got %d,%d)", C, R);
+  if (page_size != kTile) return fail(-1, "mla_paged_prefill: page_size must be 64 (got %d)", page_size);
+  CB_ARG(((uintptr_t)q_nope | (uintptr_t)q_pe | (uintptr_t)kv_cache | (uintptr_t)new_kv | (uintptr_t)out |
+          (uintptr_t)workspace) % 16 == 0);                                     // TMA / vector accesses: 16-byte bases
+  CB_ARG((int64_t)B * sq * H <= INT_MAX && (int64_t)num_blocks * kTile <= INT_MAX);   // int32 TMA row coordinates
+  if (B == 0) return 0;
+
+  const int row_tiles = cdiv((int64_t)sq * H, kRows);
+  const int max_len = max_seqlen_hint > 0 ? max_seqlen_hint : bt_stride * kTile;
+  // the decode kernels' wave rule on this kernel's CTAs (1 per SM), shrunk to the workspace (none: 1 split)
+  const int64_t rows = (int64_t)B * sq * H;
+  int splits = pick_splits_waves(row_tiles * B, max_len, 132);
+  splits = workspace ? splits_that_fit(splits, rows, kC, workspace_bytes) : 1;
+  if ((int64_t)row_tiles * splits * B > INT_MAX)
+    return fail(-1, "mla_paged_prefill: %d requests x %d row tiles x %d splits exceed the grid", B, row_tiles, splits);
+  if (!tma_available()) return fail(-3, "mla_paged_prefill: TMA is not available");
+  const auto [o_part, lse, plan] = split_kv_carve(splits > 1 ? workspace : nullptr, workspace_bytes, rows, kC, splits);
+
+  CUtensorMap mqn, mqp, mkv;
+  int rc = make_tma_map_2d(&mqn, q_nope, rows, kC, 2, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, kRows);
+  if (!rc) rc = make_tma_map_2d(&mqp, q_pe, rows, kR, 2, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, kRows);
+  if (!rc) rc = make_tma_map_2d(&mkv, kv_cache, (int64_t)num_blocks * kTile, kRow, 2, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16,
+                                kTile);
+  if (rc) return rc;
+
+  cudaStream_t st = (cudaStream_t)stream;
+  if (new_kv) {
+    const int64_t units = rows / H * (kRow / 8);
+    launch_k(mla_append_kernel, dim3(cdiv(units, 256)), dim3(256), 0, st, (__nv_bfloat16*)kv_cache,
+             (const __nv_bfloat16*)new_kv, seqlens_excl, block_table, bt_stride, sq, units);
+    CB_LAUNCHED(1);
+  }
+  const size_t smem = 1024 + (size_t)kSmemBytes;
+  static bool attr = false;
+  if (!attr) {
+    CB_CUDA(cudaFuncSetAttribute(mla_paged_prefill_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    attr = true;
+  }
+  launch_k(mla_paged_prefill_kernel, dim3(row_tiles * splits * B), dim3(kThreads), smem, st, mqn, mqp, mkv,
+           seqlens_excl, block_table, bt_stride, B, sq, H, new_kv ? 1 : 0, row_tiles, splits, causal ? 1 : 0,
+           softmax_scale, o_part, lse, (__nv_bfloat16*)out);
+  CB_LAUNCHED(1);
+  if (splits > 1) {
+    rc = launch_merge_splits(o_part, lse, out, (int)rows, splits, kC, CB_BF16, st);
+    if (rc) return rc;
+    CB_LAUNCHED(1);
+  }
   return 0;
 }
 

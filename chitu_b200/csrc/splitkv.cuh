@@ -1,5 +1,6 @@
 // The split-KV ("flash decoding") workspace contract of the attention kernels: GQA decode and the absorb-o merge
-// (attention.cu), MLA decode (mla_tc.cu), GQA paged prefill (gqa_prefill.cu) and the device-side split plan (core.cu).
+// (attention.cu), MLA decode (mla_tc.cu), GQA paged prefill (gqa_prefill.cu), MLA paged prefill (mla_prefill.cu) and
+// the device-side split plan (core.cu).
 //
 // A kernel that splits the keys of `rows` partial rows (B * H) into S splits writes, from the start of the workspace,
 //   o_part [rows, S, dv] fp32, each split normalised by its own softmax sum

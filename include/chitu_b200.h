@@ -245,6 +245,26 @@ int chitu_b200_mla_prefill(const void* q, const void* k, int64_t k_sb, const voi
                            int total_q, int total_k, int max_seqlen_q, int causal, float softmax_scale,
                            void* out, void* stream);
 
+/* *.mla_attn_with_kvcache with sq >= 1 query tokens per request (FlashMLA's s_q > 1): multi-token-prediction
+ * verification and chunked prefill on the paged latent cache of absorbed MLA.
+ * q_nope [B, sq, H, C] and q_pe [B, sq, H, R] contiguous; kv_cache [num_blocks, 64, C + R] contiguous; new_kv
+ * [B, sq, C + R] contiguous, or NULL.  With new_kv: token i of request b is written to position seqlens_excl[b] + i
+ * (pages indexed with a literal 64, as the decode append) before the attention, which then runs over
+ * Lk = seqlens_excl[b] + sq keys; without, Lk = seqlens_excl[b].  seqlens_excl is not modified.
+ * causal != 0: query i sees key j iff j <= i + Lk - sq; a row that sees no key is 0.  The decode arithmetic:
+ * scale * (q_nope.k_c + q_pe.k_pe) in fp32, softmax in fp32, P rounded to bf16 before P.V, V = the first C columns of the
+ * same cache rows.  out [B, sq, H, C] bf16 contiguous, never NULL (no deferred merge).
+ * Only block_table[b, 0 .. ceil(Lk / 64) - 1] is read; cache slots past Lk may hold anything (NaN included).
+ * Splits over keys when B x ceil(sq * H / 64) CTAs cannot fill the GPU (count from max_seqlen_hint, shrunk to the
+ * workspace; NULL workspace: no split) -> no host synchronisation, capturable in a CUDA graph, deterministic.
+ * Built for C = 512, R = 64, page_size = 64; bases 16-byte aligned; B * sq * H and num_blocks * 64 must fit int32.
+ * Anything else returns a negative status. */
+int chitu_b200_mla_paged_prefill(const void* q_nope, const void* q_pe, void* kv_cache, const void* new_kv,
+                                 const int32_t* seqlens_excl, const int32_t* block_table, int bt_stride, int B, int sq,
+                                 int H, int C, int R, int page_size, int num_blocks, int max_seqlen_hint, int causal,
+                                 float softmax_scale, void* out, void* workspace, int64_t workspace_bytes,
+                                 void* stream);
+
 /* invoke_fused_moe_kernel (fused_moe.py:796-891; Triton kernel :62-307) as ONE grouped wgmma GEMM:
  * A bf16 [numel/top_k (GEMM1) or numel (top_k = 1), K]; B stacked expert weights [E, N, K] (bf16 for wmode 0, fp8 +
  * B_scale [E, N/128, K/128] for wmode 1 = fp8_w8a8 — A is quantised per_token_group_quant_fp8 inside, as the reference
