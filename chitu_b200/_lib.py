@@ -37,7 +37,6 @@ SIGNATURES = {
     "chitu_b200_moe_gate_workspace_bytes": (L, [I, I]),
     "chitu_b200_moe_gate": (I, [P, P, P, I, I, I, I, I, I, I, I, F, P, P, I, P, L, P]),
     "chitu_b200_rotary_interleaved": (I, [P, P, P, P, P, P, I, I, I, I, L, L, L, L, I, P]),
-    "chitu_b200_rotary_interleaved_strided": (I, [P, P, P, P, P, P, I, I, I, I, L, L, L, L, L, L, I, P]),
     "chitu_b200_rotary_half": (I, [P, P, P, P, I, I, I, I, P]),
     "chitu_b200_rotary_half_strided": (I, [P, L, P, P, P, I, I, I, I, P]),
     "chitu_b200_rmsnorm": (I, [P, P, P, I, I, F, I, P]),
@@ -67,8 +66,6 @@ SIGNATURES = {
     "chitu_b200_decode_prepare": (I, [P, P, P, I, P, P, P, I, I, I, P]),
     "chitu_b200_attn_plan": (I, [P, I, I, I, I, P, L, P]),
     "chitu_b200_mla_num_splits": (I, [I, I, I, L]),
-    "chitu_b200_mla_absorb_q": (I, [P, L, L, P, P, I, I, I, I, I, P]),
-    "chitu_b200_mla_absorb_o": (I, [P, P, P, I, I, I, I, I, P]),
     "chitu_b200_mla_absorb_o_quant": (I, [P, P, P, P, P, I, I, I, I, I, P]),
     "chitu_b200_mla_absorb_o_merge_quant": (I, [P, L, I, P, P, P, P, P, I, I, I, I, I, P]),
     "chitu_b200_mla_prep": (I, [P, P, L, P, P, P, P, P, P, P, I, I, I, I, I, I, F, P]),

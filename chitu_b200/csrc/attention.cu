@@ -6,9 +6,10 @@
 //    power-of-two pages runs on tensor cores (gqa_decode_mmaT_kernel, optional fused rotary);
 //    head dim 64 and other page sizes run on the SIMT kernel (gqa_decode_kernel).
 //  * merge_splits_kernel : the LSE-weighted merge of split-KV partials, for GQA decode, MLA decode
-//    (mla_tc.cu) and GQA paged prefill (gqa_prefill.cu).  The workspace layout, the split counts
-//    and the split plan are defined once in splitkv.cuh.
-//  * MLA weight absorption (absorb-o can also merge the MLA decode partials) and mla_prep.
+//    (mla_tc.cu) and the GQA and MLA paged prefills (gqa_prefill.cu, mla_prefill.cu).  The workspace
+//    layout, the split counts, the split plan and the merge weights are defined once in splitkv.cuh.
+//  * MLA absorb-o (it can also merge the MLA decode partials) and mla_prep (rotary, kv_norm and
+//    absorb-q in one launch).
 //
 // The GQA kernels never read the cache row of the token being appended: the CTA that owns that
 // position takes it from `k_new` directly and split 0 writes it to the cache -> no RAW hazard.
@@ -32,21 +33,7 @@ __global__ void merge_splits_kernel(const float* __restrict__ o_part, const floa
   __shared__ float s_w[kMaxSplits];               // normalised split weights
   const int64_t bh = blockIdx.x;  // b * H + h
   const float* l = lse + bh * num_splits;
-  if (threadIdx.x < 32) {
-    float mx = -INFINITY;
-    for (int s = threadIdx.x; s < num_splits; s += 32) mx = fmaxf(mx, l[s]);
-    mx = warp_max(mx);
-    float den = 0.f;
-    for (int s = threadIdx.x; s < num_splits; s += 32) {
-      const float ls = l[s];
-      const float wv = ls == -INFINITY ? 0.f : exp2f(ls - mx);
-      s_w[s] = wv;
-      den += wv;
-    }
-    den = warp_sum(den);
-    const float inv = den > 0.f ? 1.f / den : 0.f;
-    for (int s = threadIdx.x; s < num_splits; s += 32) s_w[s] *= inv;
-  }
+  if (threadIdx.x < 32) split_weights(l, num_splits, s_w, threadIdx.x);
   __syncthreads();
   const float* base = o_part + bh * num_splits * DV;
   for (int d = threadIdx.x; d < DV; d += blockDim.x) {
@@ -637,77 +624,16 @@ extern "C" int chitu_b200_gqa_paged_decode_rope(const void* q, int64_t q_sb, voi
 // ============================================================================================
 // MLA weight absorption (the two torch.einsum of AttentionDeepSeekV3, model_deepseek_v3.py:529-531
 // and :697; SURVEY K8): wkv_b (bf16, [H, dn + dv, C]) is W_UK = [:, :dn] and W_UV = [:, dn:].
-//   absorb_q : q'[b,h,c] = sum_d q_nope[b,h,d] * W_UK[h,d,c]        ("shd,hdc->shc")
+//   absorb_q : q'[b,h,c] = sum_d q_nope[b,h,d] * W_UK[h,d,c]        ("shd,hdc->shc", a role of mla_prep below)
 //   absorb_o : o[b,h,d]  = sum_c x[b,h,c]     * W_UV[h,d,c]        ("bshc,hdc->bshd")
 // Both stream the 2 MB of per-rank absorbed weights once for all tokens (fp32 accumulate).
 // ============================================================================================
-// CTA = (64-column chunk of C, head): 8 warps split the dn reduction dim (16 d each), a lane owns two
-// adjacent columns; partial sums are combined through shared memory.  W_UK is read once (2 MB per rank).
-template <int MT>
-__global__ void __launch_bounds__(256) mla_absorb_q_kernel(const __nv_bfloat16* __restrict__ q, int64_t q_sb,
-                                                          int64_t q_sh, const __nv_bfloat16* __restrict__ w,
-                                                          __nv_bfloat16* __restrict__ out, int B, int H, int dn,
-                                                          int dv, int C) {
-  cb::pdl_prologue();
-  extern __shared__ float s_abs[];               // [MT][dn] q  |  [8 warps][MT][64] partial sums
-  float* s_q = s_abs;
-  float* s_red = s_abs + MT * dn;
-  const int h = blockIdx.y;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int c = blockIdx.x * 64 + lane * 2;
-  const int b0 = blockIdx.z * MT;
-  for (int i = threadIdx.x; i < MT * dn; i += 256) {
-    const int m = i / dn, d = i - m * dn;
-    s_q[i] = (b0 + m < B) ? __bfloat162float(q[(int64_t)(b0 + m) * q_sb + (int64_t)h * q_sh + d]) : 0.f;
-  }
-  __syncthreads();
-  float acc0[MT], acc1[MT];
-#pragma unroll
-  for (int m = 0; m < MT; ++m) acc0[m] = acc1[m] = 0.f;
-  const int dper = dn / 8;                        // d slice of this warp
-  const __nv_bfloat16* wp = w + ((int64_t)h * (dn + dv) + warp * dper) * C + c;
-  if (c < C) {
-    // all weight loads of a block of 16 rows are issued before the first FMA (one L2 round trip instead of four)
-    for (int d0 = 0; d0 < dper; d0 += 16) {
-      uint32_t uu[16];
-#pragma unroll
-      for (int i = 0; i < 16; ++i)
-        uu[i] = d0 + i < dper ? *reinterpret_cast<const uint32_t*>(wp + (int64_t)(d0 + i) * C) : 0u;
-#pragma unroll
-      for (int i = 0; i < 16; ++i) {
-        if (d0 + i >= dper) break;
-        const float w0 = bf16lo(uu[i]), w1 = bf16hi(uu[i]);
-#pragma unroll
-        for (int m = 0; m < MT; ++m) {
-          const float qv = s_q[m * dn + warp * dper + d0 + i];
-          acc0[m] = fmaf(qv, w0, acc0[m]);
-          acc1[m] = fmaf(qv, w1, acc1[m]);
-        }
-      }
-    }
-  }
-#pragma unroll
-  for (int m = 0; m < MT; ++m) {
-    s_red[(warp * MT + m) * 64 + lane * 2] = acc0[m];
-    s_red[(warp * MT + m) * 64 + lane * 2 + 1] = acc1[m];
-  }
-  __syncthreads();
-  for (int i = threadIdx.x; i < MT * 64; i += 256) {
-    const int m = i / 64, cc = i - m * 64;
-    float v = 0.f;
-#pragma unroll
-    for (int wq = 0; wq < 8; ++wq) v += s_red[(wq * MT + m) * 64 + cc];
-    if (b0 + m < B && blockIdx.x * 64 + cc < C)
-      out[((int64_t)(b0 + m) * H + h) * C + blockIdx.x * 64 + cc] = __float2bfloat16_rn(v);
-  }
-}
-
 // CTA = (head, token chunk): warp w computes output dims [w*dv/8, (w+1)*dv/8) (one W_UV row at a time,
 // lanes stride C); with dv == 128 the head's 128 outputs are exactly one act_quant group, so the fp8
 // payload + scale of the following `wo` linear can be produced here (q_out != null).
 // With `o_part` != null the latent input is the split-KV partials of the attention kernel and the LSE-weighted merge
-// (merge_splits_kernel's arithmetic: same weights, same fmaf order, one bf16 rounding) happens while staging: the merge
-// launch and its [B,H,C] round trip disappear.
+// (merge_splits_kernel's arithmetic: split_weights, the same fmaf order, one bf16 rounding) happens while staging: the
+// merge launch and its [B,H,C] round trip disappear.
 template <int MT>
 __global__ void __launch_bounds__(256) mla_absorb_o_kernel(const __nv_bfloat16* __restrict__ x,
                                                           const __nv_bfloat16* __restrict__ w,
@@ -743,20 +669,7 @@ __global__ void __launch_bounds__(256) mla_absorb_o_kernel(const __nv_bfloat16* 
   if (o_part) {
     for (int m = warp; m < MT; m += 8) {                        // warp m: the split weights of token b0 + m
       const int b = min(b0 + m, B - 1);
-      const float* l = lse + ((int64_t)b * H + h) * num_splits;
-      float mx = -INFINITY;
-      for (int sp = lane; sp < num_splits; sp += 32) mx = fmaxf(mx, l[sp]);
-      mx = warp_max(mx);
-      float den = 0.f;
-      for (int sp = lane; sp < num_splits; sp += 32) {
-        const float ls = l[sp];
-        const float wv = ls == -INFINITY ? 0.f : exp2f(ls - mx);
-        s_mw[m][sp] = wv;
-        den += wv;
-      }
-      den = warp_sum(den);
-      const float inv = den > 0.f ? 1.f / den : 0.f;
-      for (int sp = lane; sp < num_splits; sp += 32) s_mw[m][sp] *= inv;
+      split_weights(lse + ((int64_t)b * H + h) * num_splits, num_splits, s_mw[m], lane);
     }
     __syncthreads();
     for (int i = threadIdx.x; i < MT * (C / 4); i += 256) {
@@ -895,24 +808,6 @@ __global__ void __launch_bounds__(256) mla_absorb_o_kernel(const __nv_bfloat16* 
   }
 }
 
-extern "C" int chitu_b200_mla_absorb_q(const void* q_nope, int64_t q_sb, int64_t q_sh, const void* wkv_b,
-                                       void* out, int B, int H, int dn, int dv, int C, void* stream) {
-  CB_ARG(q_nope && wkv_b && out && B >= 0 && H > 0 && dn > 0 && dv > 0 && C > 0 && C % 2 == 0);
-  if (B == 0) return 0;
-  constexpr int MT = 16;
-  CB_ARG(dn % 8 == 0);
-  dim3 grid(cdiv(C, 64), H, cdiv(B, MT));
-  cb::launch_k(mla_absorb_q_kernel<MT>, grid, dim3(256), (size_t)(MT * dn + 8 * MT * 64) * 4, (cudaStream_t)stream,
-               (const __nv_bfloat16*)q_nope, q_sb, q_sh, (const __nv_bfloat16*)wkv_b, (__nv_bfloat16*)out, B, H, dn, dv, C);
-  CB_LAUNCHED(1);
-  return 0;
-}
-
-extern "C" int chitu_b200_mla_absorb_o(const void* x, const void* wkv_b, void* out, int B, int H, int dn, int dv,
-                                       int C, void* stream) {
-  return chitu_b200_mla_absorb_o_quant(x, wkv_b, out, nullptr, nullptr, B, H, dn, dv, C, stream);
-}
-
 extern "C" int chitu_b200_mla_absorb_o_quant(const void* x, const void* wkv_b, void* out, void* q_out,
                                              float* q_scales, int B, int H, int dn, int dv, int C, void* stream) {
   CB_ARG(x && wkv_b && (out || q_out) && B >= 0 && H > 0 && dn > 0 && dv > 0 && C > 0 && C % 8 == 0);
@@ -968,7 +863,8 @@ __global__ void __launch_bounds__(256) mla_prep_kernel(
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int qk = dn + R;
   if ((int)blockIdx.x < nA) {
-    // ---- absorb_q role: CTA = (64-column chunk, head, token chunk) ----
+    // ---- absorb_q role: CTA = (64-column chunk, head, token chunk); the 8 warps split the dn reduction dim, a lane
+    // owns two adjacent columns, and the partial sums are combined through shared memory ----
     const int ncx = C / 64;
     const int cx = blockIdx.x % ncx, h = (blockIdx.x / ncx) % H, z = blockIdx.x / (ncx * H);
     float* s_q = s_abs;

@@ -116,6 +116,20 @@ struct PushDev {
 };
 int comm_push_desc(void* handle, void* out_desc);
 
+// ---- paged append (core.cu): new rows into one or two paged caches, for the append and paged prefill entries ------
+// Row i of request b (i < sq, b < B) comes from src + b * src_sb + i * src_st (bytes) and goes to position
+// p = seqlens[b] + i: cache row block_table[b, p / index_div] * page_size + p % index_div.  index_div is page_size for
+// true page indexing and 64 for the reference's append (triton_kernels.py:38,42).  c1.cache == NULL: one cache only.
+// One PDL launch; the caller counts it.
+struct PagedAppend {
+  void* cache;
+  const void* src;
+  int64_t src_sb, src_st;
+};
+void launch_paged_append(PagedAppend c0, PagedAppend c1, int64_t row_bytes, const int32_t* seqlens,
+                         const int32_t* block_table, int bt_stride, int B, int sq, int page_size, int index_div,
+                         cudaStream_t st);
+
 #ifdef __CUDACC__
 // byte offset of this rank's area inside every push buffer, for the reduce that is being produced
 __device__ __forceinline__ int64_t push_area(const PushDev& d, uint32_t calls) {

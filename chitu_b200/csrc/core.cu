@@ -71,33 +71,68 @@ extern "C" int chitu_b200_debug_timeline(void* buf) {
 extern "C" const char* chitu_b200_debug_timeline_names(void) { return cb::g_tl_names; }
 
 // ============================================================================================
-// append_to_paged_kv_cache   (reference: chitu/ops.py:50-91, triton_kernels.py:18-48)
-// One CTA per request; the token's row (row_bytes) is copied with 16-byte vectors when aligned.
+// Paged append: row i of request b is written to position p = seqlens[b] + i, i.e. to cache row
+// block_table[b, p / index_div] * page_size + p % index_div, of one or two caches.  One CTA per
+// row; 16-byte copies when every address and stride allows them, byte copies otherwise.
 // ============================================================================================
-__global__ void append_paged_kv_kernel(uint8_t* __restrict__ kv_cache,
-                                       const int32_t* __restrict__ page_table,
-                                       const uint8_t* __restrict__ this_kv,
-                                       const int32_t* __restrict__ old_seq_lens,
-                                       int pages_per_sample, int page_size, int index_div,
-                                       int64_t row_bytes, int vec_ok) {
-  cb::pdl_prologue();
-  const int b = blockIdx.x;
-  const int seqlen = old_seq_lens[b];
-  // Reference quirk kept on purpose: page index and in-page offset use `index_div` (literal 64
-  // in triton_kernels.py:38,42) while the row address uses the real PAGE_SIZE.
-  const int page_id = page_table[(int64_t)b * pages_per_sample + seqlen / index_div];
-  const int64_t row = (int64_t)page_id * page_size + seqlen % index_div;
-  uint8_t* dst = kv_cache + row * row_bytes;
-  const uint8_t* src = this_kv + (int64_t)b * row_bytes;
-  if (vec_ok) {
-    const int64_t n16 = row_bytes >> 4;
-    for (int64_t i = threadIdx.x; i < n16; i += blockDim.x)
-      reinterpret_cast<uint4*>(dst)[i] = reinterpret_cast<const uint4*>(src)[i];
-  } else {
-    for (int64_t i = threadIdx.x; i < row_bytes; i += blockDim.x) dst[i] = src[i];
+// Row i of request b (n units of V) into both caches; bt is the request's block-table row.  A thread issues its source
+// loads for two passes over both caches before the page lookup and the stores, so the copy's memory round trip
+// overlaps the lookup's.  The compiler would not order them so itself: it cannot tell that sources and caches never
+// overlap, and with bt __restrict__ it hoists the lookup above the loads.
+template <typename V>
+__device__ __forceinline__ void copy_row(const cb::PagedAppend& c0, const cb::PagedAppend& c1, int p,
+                                         const int32_t* bt, int page_size, int index_div, int b, int i, int64_t n) {
+  const V* s0 = reinterpret_cast<const V*>((const uint8_t*)c0.src + b * c0.src_sb + i * c0.src_st);
+  const V* s1 = reinterpret_cast<const V*>((const uint8_t*)c1.src + b * c1.src_sb + i * c1.src_st);
+  const bool two = c1.cache != nullptr;
+#pragma unroll 1
+  for (int64_t u = threadIdx.x; u < n; u += 2 * blockDim.x) {
+    const int64_t w = u + blockDim.x;
+    V x0 = s0[u], x1, y0, y1;
+    if (w < n) y0 = s0[w];
+    if (two) x1 = s1[u];
+    if (two && w < n) y1 = s1[w];
+    const int64_t row = (int64_t)bt[p / index_div] * page_size + p % index_div;
+    V* d0 = reinterpret_cast<V*>(c0.cache) + row * n;
+    V* d1 = reinterpret_cast<V*>(c1.cache) + row * n;
+    d0[u] = x0;
+    if (w < n) d0[w] = y0;
+    if (two) d1[u] = x1;
+    if (two && w < n) d1[w] = y1;
   }
 }
 
+__global__ void __launch_bounds__(128) paged_append_kernel(cb::PagedAppend c0, cb::PagedAppend c1, int64_t row_bytes,
+                                                           const int32_t* __restrict__ seqlens,
+                                                           const int32_t* block_table, int bt_stride, int B,
+                                                           int page_size, int index_div, int vec) {
+  cb::pdl_prologue();
+  const int i = blockIdx.x;
+  for (int b = blockIdx.y; b < B; b += gridDim.y) {     // more than 65535 requests: a CTA takes several
+    const int p = seqlens[b] + i;
+    const int32_t* bt = block_table + (int64_t)b * bt_stride;
+    if (vec) copy_row<uint4>(c0, c1, p, bt, page_size, index_div, b, i, row_bytes >> 4);
+    else copy_row<uint8_t>(c0, c1, p, bt, page_size, index_div, b, i, row_bytes);
+  }
+}
+
+namespace cb {
+void launch_paged_append(PagedAppend c0, PagedAppend c1, int64_t row_bytes, const int32_t* seqlens,
+                         const int32_t* block_table, int bt_stride, int B, int sq, int page_size, int index_div,
+                         cudaStream_t st) {
+  uintptr_t bits = (uintptr_t)row_bytes;
+  for (const PagedAppend& c : {c0, c1})
+    if (c.cache) bits |= (uintptr_t)c.cache | (uintptr_t)c.src | (uintptr_t)c.src_sb | (uintptr_t)c.src_st;
+  const int vec = bits % 16 == 0;
+  const int threads = row_bytes / (vec ? 16 : 1) < 128 ? 64 : 128;
+  launch_k(paged_append_kernel, dim3(sq, B < 65535 ? B : 65535), dim3(threads), 0, st, c0, c1, row_bytes, seqlens,
+           block_table, bt_stride, B, page_size, index_div, vec);
+}
+}  // namespace cb
+
+// append_to_paged_kv_cache (reference: chitu/ops.py:50-91, triton_kernels.py:18-48).  Reference quirk kept on purpose:
+// page index and in-page offset use `index_div` (literal 64 in triton_kernels.py:38,42) while the row address uses
+// the real page_size.
 extern "C" int chitu_b200_append_paged_kv(void* kv_cache, const int32_t* page_table,
                                           const void* this_kv, const int32_t* old_seq_lens,
                                           int batch, int pages_per_sample, int page_size,
@@ -105,11 +140,8 @@ extern "C" int chitu_b200_append_paged_kv(void* kv_cache, const int32_t* page_ta
   CB_ARG(kv_cache && page_table && this_kv && old_seq_lens);
   CB_ARG(batch >= 0 && pages_per_sample > 0 && page_size > 0 && index_div > 0 && row_bytes > 0);
   if (batch == 0) return 0;
-  int vec_ok = (row_bytes % 16 == 0) && ((uintptr_t)kv_cache % 16 == 0) && ((uintptr_t)this_kv % 16 == 0);
-  int threads = (int)((row_bytes / (vec_ok ? 16 : 1)) < 128 ? 64 : 128);
-  cb::launch_k(append_paged_kv_kernel, dim3(batch), dim3(threads), 0, (cudaStream_t)stream, 
-      (uint8_t*)kv_cache, page_table, (const uint8_t*)this_kv, old_seq_lens, pages_per_sample,
-      page_size, index_div, row_bytes, vec_ok);
+  cb::launch_paged_append({kv_cache, this_kv, row_bytes, row_bytes}, {}, row_bytes, old_seq_lens, page_table,
+                          pages_per_sample, batch, 1, page_size, index_div, (cudaStream_t)stream);
   CB_LAUNCHED(1);
   return 0;
 }

@@ -89,19 +89,11 @@ extern "C" int chitu_b200_rotary_interleaved(const void* q, const void* k, void*
                                              const float* cos, const float* sin, int bs, int hq,
                                              int hk, int rot_dim, int64_t q_sb, int64_t q_sh,
                                              int64_t k_sb, int64_t k_sh, int dtype, void* stream) {
-  return chitu_b200_rotary_interleaved_strided(q, k, out_q, out_k, cos, sin, bs, hq, hk, rot_dim, q_sb, q_sh, k_sb,
-                                               k_sh, (int64_t)hq * rot_dim, (int64_t)hk * rot_dim, dtype, stream);
-}
-
-extern "C" int chitu_b200_rotary_interleaved_strided(const void* q, const void* k, void* out_q, void* out_k,
-                                                     const float* cos, const float* sin, int bs, int hq, int hk,
-                                                     int rot_dim, int64_t q_sb, int64_t q_sh, int64_t k_sb,
-                                                     int64_t k_sh, int64_t oq_sb, int64_t ok_sb, int dtype,
-                                                     void* stream) {
   CB_ARG(q && k && out_q && out_k && cos && sin);
   CB_ARG(bs >= 0 && hq >= 0 && hk >= 0 && rot_dim > 0 && rot_dim % 2 == 0);
   if (bs == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
+  const int64_t oq_sb = (int64_t)hq * rot_dim, ok_sb = (int64_t)hk * rot_dim;   // dense outputs
   int total = (hq + hk) * rot_dim / 2;
   // 16-byte path: a thread rotates 4 pairs (one uint4 of 2-byte elements); needs 16 B aligned rows
   const bool vec_ok = (dtype == CB_BF16 || dtype == CB_F16) && rot_dim % 8 == 0 &&

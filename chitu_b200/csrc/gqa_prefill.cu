@@ -87,30 +87,6 @@ template <> struct Mma<__half> {
   }
 };
 
-// the sq new k / v rows of every request into the cache: one CTA per (token, request), 16-byte copies
-template <typename T>
-__global__ void __launch_bounds__(128) gqa_append_kernel(T* __restrict__ k_cache, T* __restrict__ v_cache,
-                                                         const T* __restrict__ k_new, const T* __restrict__ v_new,
-                                                         int64_t k_sb, int64_t k_st, int64_t v_sb, int64_t v_st,
-                                                         const int32_t* __restrict__ cache_seqlens,
-                                                         const int32_t* __restrict__ block_table, int bt_stride,
-                                                         int Hkv, int page) {
-  cb::pdl_prologue();
-  const int i = blockIdx.x, b = blockIdx.y;
-  const int p = cache_seqlens[b] + i;
-  const int64_t blk = block_table[(int64_t)b * bt_stride + p / page];
-  const int64_t dst = (blk * page + p % page) * Hkv * kD;
-  const uint4* ks = reinterpret_cast<const uint4*>(k_new + b * k_sb + i * k_st);
-  const uint4* vs = reinterpret_cast<const uint4*>(v_new + b * v_sb + i * v_st);
-  uint4* kd = reinterpret_cast<uint4*>(k_cache + dst);
-  uint4* vd = reinterpret_cast<uint4*>(v_cache + dst);
-  const int n = Hkv * kD * (int)sizeof(T) / 16;
-  for (int u = threadIdx.x; u < n; u += blockDim.x) {
-    kd[u] = ks[u];
-    vd[u] = vs[u];
-  }
-}
-
 template <typename T, int G>
 __global__ void __launch_bounds__(kThreads, kCtasPerSm) gqa_prefill_kernel(
     const __grid_constant__ CUtensorMap map_k, const __grid_constant__ CUtensorMap map_v, const T* __restrict__ q,
@@ -351,15 +327,9 @@ extern "C" int chitu_b200_gqa_paged_prefill(const void* q, void* k_cache, void* 
   if (rc) return rc;
 
   cudaStream_t st = (cudaStream_t)stream;
-  if (k_new) {
-    if (dtype == CB_BF16)
-      launch_k(gqa_append_kernel<__nv_bfloat16>, dim3(sq, B), dim3(128), 0, st, (__nv_bfloat16*)k_cache,
-               (__nv_bfloat16*)v_cache, (const __nv_bfloat16*)k_new, (const __nv_bfloat16*)v_new, k_new_sb, k_new_st,
-               v_new_sb, v_new_st, cache_seqlens, block_table, bt_stride, Hkv, page_size);
-    else
-      launch_k(gqa_append_kernel<__half>, dim3(sq, B), dim3(128), 0, st, (__half*)k_cache, (__half*)v_cache,
-               (const __half*)k_new, (const __half*)v_new, k_new_sb, k_new_st, v_new_sb, v_new_st, cache_seqlens,
-               block_table, bt_stride, Hkv, page_size);
+  if (k_new) {                                              // the sq new k / v rows first, true page indexing
+    launch_paged_append({k_cache, k_new, k_new_sb * 2, k_new_st * 2}, {v_cache, v_new, v_new_sb * 2, v_new_st * 2},
+                        (int64_t)Hkv * kD * 2, cache_seqlens, block_table, bt_stride, B, sq, page_size, page_size, st);
     CB_LAUNCHED(1);
   }
 

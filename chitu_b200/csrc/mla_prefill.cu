@@ -28,9 +28,9 @@
 // Paged variant (mla_paged_prefill_kernel, behind AttnBackend.mla_attn_with_kvcache with seqlen_q = sq > 1:
 // multi-token-prediction verification, chunked prefill on a cached prefix): the same CTA over the paged latent cache
 // [num_blocks * 64, 576].  Request b's sq * H rows are row tiles as above (Lq = sq, Lk = seqlens_excl[b] (+ sq)); key
-// tile t is page block_table[b, t], K and V boxes come from the one cache map.  mla_append_kernel writes the new rows
-// first (PDL orders the two).  In the tile holding Lk the V rows >= Lk (unwritten slots, maybe NaN) are zeroed in shared
-// memory before P.V.  When row tiles x B CTAs cannot fill the GPU the keys are split; each split writes normalised fp32
+// tile t is page block_table[b, t], K and V boxes come from the one cache map.  The paged append (core.cu) writes the
+// new rows first (PDL orders the two).  In the tile holding Lk the V rows >= Lk (unwritten slots, maybe NaN) are zeroed
+// in shared memory before P.V.  When row tiles x B CTAs cannot fill the GPU the keys are split; each split writes normalised fp32
 // partials + LSE (splitkv.cuh, rows = B * sq * H, staged through the ring) and launch_merge_splits merges them.  The
 // split count depends on host values only, so this variant is deterministic too.
 #include <cuda.h>
@@ -397,22 +397,6 @@ __global__ void __launch_bounds__(kThreads, 1) mla_paged_prefill_kernel(
                         appended, splits, B, H, row_tiles, causal, scale, o_part, lse, out);
 }
 
-// the B * sq new latent rows into the cache before the attention reads it: token i of request b goes to position
-// seqlens_excl[b] + i, pages indexed with a literal 64 as the reference's append does; one thread per 16 bytes
-__global__ void __launch_bounds__(256) mla_append_kernel(__nv_bfloat16* __restrict__ kv_cache,
-                                                         const __nv_bfloat16* __restrict__ new_kv,
-                                                         const int32_t* __restrict__ seqlens_excl,
-                                                         const int32_t* __restrict__ block_table, int bt_stride, int sq,
-                                                         int64_t units) {
-  cb::pdl_prologue();
-  const int64_t u = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (u >= units) return;
-  const int64_t row = u / (kRow / 8);                       // b * sq + i
-  const int b = (int)(row / sq), p = seqlens_excl[b] + (int)(row % sq);
-  const int64_t dst = ((int64_t)block_table[(int64_t)b * bt_stride + p / 64] * 64 + p % 64) * kRow;
-  reinterpret_cast<uint4*>(kv_cache + dst)[u % (kRow / 8)] = reinterpret_cast<const uint4*>(new_kv)[u];
-}
-
 }  // namespace
 }  // namespace cb
 
@@ -486,10 +470,10 @@ extern "C" int chitu_b200_mla_paged_prefill(const void* q_nope, const void* q_pe
   if (rc) return rc;
 
   cudaStream_t st = (cudaStream_t)stream;
-  if (new_kv) {
-    const int64_t units = rows / H * (kRow / 8);
-    launch_k(mla_append_kernel, dim3(cdiv(units, 256)), dim3(256), 0, st, (__nv_bfloat16*)kv_cache,
-             (const __nv_bfloat16*)new_kv, seqlens_excl, block_table, bt_stride, sq, units);
+  if (new_kv) {       // the B * sq new latent rows first, pages indexed with a literal 64 as the reference's append does
+    const int64_t row_bytes = kRow * 2;
+    launch_paged_append({kv_cache, new_kv, sq * row_bytes, row_bytes}, {}, row_bytes, seqlens_excl, block_table,
+                        bt_stride, B, sq, kTile, 64, st);
     CB_LAUNCHED(1);
   }
   const size_t smem = 1024 + (size_t)kSmemBytes;

@@ -5,8 +5,8 @@
 // A kernel that splits the keys of `rows` partial rows (B * H) into S splits writes, from the start of the workspace,
 //   o_part [rows, S, dv] fp32, each split normalised by its own softmax sum
 //   lse    [rows, S]     fp32, log2 domain (m + log2(l)), -inf for a split that saw no key
-// and a merge weights the S partials of a row by exp2(lse - max).  The last kPlanBytes of the workspace hold the split
-// plan that chitu_b200_attn_plan writes for the MLA decode kernel.
+// and a merge weights the S partials of a row by split_weights below.  The last kPlanBytes of the workspace hold the
+// split plan that chitu_b200_attn_plan writes for the MLA decode kernel.
 #pragma once
 #include "common.cuh"
 
@@ -82,6 +82,25 @@ inline int mla_num_splits(int B, int H, int max_len, int64_t workspace_bytes) {
   if (splits > kMaxSplits) splits = kMaxSplits;
   if (splits < 1) splits = 1;
   return splits_that_fit(splits, (int64_t)B * H, kMlaC, workspace_bytes);
+}
+
+// One warp turns the `n` split LSEs of a row into its merge weights w[s] = exp2(lse[s] - max) / sum: 0 for a split
+// that saw no key, all 0 when no split did.  merge_splits_kernel and the fused merge of mla_absorb_o_kernel both call
+// it and then add the splits in ascending order, so the two merges give bit-identical results.
+__device__ __forceinline__ void split_weights(const float* lse, int n, float* w, int lane) {
+  float mx = -INFINITY;
+  for (int s = lane; s < n; s += 32) mx = fmaxf(mx, lse[s]);
+  mx = warp_max(mx);
+  float den = 0.f;
+  for (int s = lane; s < n; s += 32) {
+    const float ls = lse[s];
+    const float wv = ls == -INFINITY ? 0.f : exp2f(ls - mx);
+    w[s] = wv;
+    den += wv;
+  }
+  den = warp_sum(den);
+  const float inv = den > 0.f ? 1.f / den : 0.f;
+  for (int s = lane; s < n; s += 32) w[s] *= inv;
 }
 
 // LSE-weighted merge of the partials of `rows` rows into out [rows, dv] (attention.cu).  Built for bf16 and fp16 with

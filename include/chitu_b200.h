@@ -86,14 +86,6 @@ int chitu_b200_rotary_interleaved(const void* q, const void* k, void* out_q, voi
                                   const float* cos, const float* sin, int bs, int hq, int hk,
                                   int rot_dim, int64_t q_sb, int64_t q_sh, int64_t k_sb, int64_t k_sh,
                                   int dtype, void* stream);
-/* Same, with explicit output batch strides (elements) so the rotated k_pe can be written
- * straight into the [kv_norm(kv) | k_pe] row that is appended to the MLA cache
- * (model_deepseek_v3.py:684-686 builds it with torch.cat). */
-int chitu_b200_rotary_interleaved_strided(const void* q, const void* k, void* out_q, void* out_k,
-                                          const float* cos, const float* sin, int bs, int hq, int hk,
-                                          int rot_dim, int64_t q_sb, int64_t q_sh, int64_t k_sb,
-                                          int64_t k_sh, int64_t oq_sb, int64_t ok_sb, int dtype,
-                                          void* stream);
 /* Replaces triton_kernels.py:51-98 (rotary_type="hf-llama", half-split); cos/sin in the
  * tensor dtype [bs, head_dim/2] (ops.py:124-176).  x:[bs,h,head_dim] contiguous. */
 int chitu_b200_rotary_half(const void* x, void* out, const void* cos, const void* sin, int bs,
@@ -310,16 +302,11 @@ int chitu_b200_attn_plan(const int32_t* seqlens_incl, int B, int heads, int page
 /* grid.x (upper bound of KV splits per request) the wgmma MLA kernel uses for these arguments */
 int chitu_b200_mla_num_splits(int B, int H, int max_seqlen_hint, int64_t workspace_bytes);
 
-/* MLA weight absorption = the two torch.einsum around the attention call
- * (AttentionDeepSeekV3._run_linear model_deepseek_v3.py:529-531 "shd,hdc->shc" and
- * decode_forward_paged :697 "bshc,hdc->bshd").  wkv_b: bf16 [H, dn+dv, C] (dequantised,
- * ops.py:356-392); q_nope: [B,H,dn] with element strides q_sb / q_sh (a view of q[B,H,dn+R]). */
-int chitu_b200_mla_absorb_q(const void* q_nope, int64_t q_sb, int64_t q_sh, const void* wkv_b, void* out,
-                            int B, int H, int dn, int dv, int C, void* stream);
-int chitu_b200_mla_absorb_o(const void* x, const void* wkv_b, void* out, int B, int H, int dn, int dv, int C,
-                            void* stream);
-/* absorb_o + act_quant_deepseek_v3 of the result (the input of the `wo` linear): out (bf16, may be NULL),
- * q_out fp8 [B, H*dv], q_scales [B, H*dv/128]. dv must be 128 (one quantisation group per head). */
+/* MLA output absorption = the torch.einsum after the attention call (AttentionDeepSeekV3.decode_forward_paged
+ * model_deepseek_v3.py:697 "bshc,hdc->bshd"; the q side, :529-531, is part of chitu_b200_mla_prep).  wkv_b: bf16
+ * [H, dn+dv, C] (dequantised, ops.py:356-392); x: [B,H,C] bf16.  absorb_o + act_quant_deepseek_v3 of the result (the
+ * input of the `wo` linear): out (bf16, may be NULL), q_out fp8 [B, H*dv], q_scales [B, H*dv/128]. dv must be 128
+ * (one quantisation group per head). */
 int chitu_b200_mla_absorb_o_quant(const void* x, const void* wkv_b, void* out, void* q_out, float* q_scales,
                                   int B, int H, int dn, int dv, int C, void* stream);
 /* Same, but the latent input is the split-KV partials that chitu_b200_mla_decode(out = NULL) left in `workspace`
