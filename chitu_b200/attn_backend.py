@@ -2,9 +2,10 @@
 
 `B200AttnBackend` implements the four methods the models call (SURVEY.md §8b):
 prepare_metadata_for_decode, attn_varlen_func (prefill: the absorbed-MLA form runs the sm_90a
-prefill kernel; GQA prefill stays on flash_attn / torch SDPA), attn_with_kvcache (GQA attention over the paged
-cache with in-place append: the decode kernel for seqlen_q == 1, the sm_90a multi-token kernel for seqlen_q > 1 —
-chunked prefill, prefill on a cached prefix, speculative verification) and mla_attn_with_kvcache (absorbed-MLA
+prefill kernel; GQA prefill stays on flash_attn / torch SDPA), attn_with_kvcache (GQA attention over the KV cache
+with in-place append: the decode kernel for seqlen_q == 1, the sm_90a multi-token kernel for seqlen_q > 1 — chunked
+prefill, prefill on a cached prefix, speculative verification; over the paged cache with a block_table, and over the
+non-paged [B, S, Hkv, D] cache of KVCacheManager without one) and mla_attn_with_kvcache (absorbed-MLA
 attention over the paged latent cache: the decode kernel with fused append for one query token per request, the
 sm_90a multi-token kernel for seqlen_q > 1 — multi-token-prediction verification, chunked prefill on a cached prefix).
 """
@@ -164,7 +165,8 @@ class B200AttnBackend(AttnBackend):
                           block_table: Optional[torch.Tensor] = None, causal=False, window_size=(-1, -1),
                           softcap=0.0, softmax_scale=None):
         if block_table is None:
-            raise NotImplementedError("B200AttnBackend implements the paged (block_table) decode path")
+            return self._contiguous(q, k_cache, v_cache, k, v, cache_seqlens, cache_leftpad, causal, window_size,
+                                    softcap, softmax_scale)
         assert cache_leftpad is None and window_size == (-1, -1) and softcap == 0.0
         require_cuda(q, k_cache, v_cache, block_table)
         B, sq, Hq, D = q.shape
@@ -220,6 +222,41 @@ class B200AttnBackend(AttnBackend):
             ptr(q), ptr(k_cache), ptr(v_cache), ptr(k), ptr(v), *strides, ptr(cache_seqlens), ptr(block_table),
             block_table.stride(0), B, sq, Hq, Hkv, D, page, num_blocks, int(hint), int(bool(causal)), float(scale),
             ptr(out), ptr(ws), wsn, dtype_code(q.dtype), current_stream()), "gqa_paged_prefill")
+        return out
+
+    def _contiguous(self, q, k_cache, v_cache, k, v, cache_seqlens, cache_leftpad, causal, window_size, softcap,
+                    softmax_scale):
+        """No block table (chitu_b200_gqa_contiguous_attn): k_cache / v_cache [Bc, S, Hkv, D] with Bc >= B, request b
+        on cache row b; the sq new k / v rows are appended at cache_seqlens[b] + i, then query i attends to the first
+        cache_seqlens[b] + sq keys (without k / v: cache_seqlens[b]), bottom-right causal when `causal`.  A new row at a
+        position >= S is not written and no key >= S is read.  sq == 1 and sq > 1 alike; no host synchronisation,
+        capturable in a CUDA graph, deterministic."""
+        if cache_leftpad is not None or tuple(window_size) != (-1, -1) or softcap != 0.0:
+            raise RuntimeError("gqa_contiguous_attn: cache_leftpad, window_size and softcap are not built")
+        if not torch.is_tensor(cache_seqlens):
+            cache_seqlens = torch.full((q.shape[0],), int(cache_seqlens), dtype=torch.int32, device=q.device)
+        require_cuda(q, k_cache, v_cache, k, v, cache_seqlens)
+        B, sq, Hq, D = q.shape
+        Bc, S, Hkv, Dk = k_cache.shape
+        cst = k_cache.stride()
+        assert v_cache.shape == k_cache.shape and v_cache.stride() == cst and cst[1:] == (Hkv * D, D, 1)
+        assert Dk == D and Bc >= B and k_cache.dtype == v_cache.dtype == q.dtype and q.is_contiguous()
+        assert cache_seqlens.dtype == torch.int32 and cache_seqlens.is_contiguous()
+        strides = (0, 0, 0, 0)
+        if k is not None:
+            assert v is not None and k.shape == (B, sq, Hkv, D) and v.shape == (B, sq, Hkv, D)
+            assert k.dtype == v.dtype == q.dtype
+            # heads must be dense; the batch and token strides are free (views into a fused qkv GEMM output)
+            assert k.stride(-1) == 1 and k.stride(-2) == D and v.stride(-1) == 1 and v.stride(-2) == D
+            strides = (k.stride(0), k.stride(1), v.stride(0), v.stride(1))
+        scale = softmax_scale if softmax_scale is not None else 1.0 / math.sqrt(D)
+        out = torch.empty_like(q)
+        ws, wsn = self._ws(B, Hq, D, q.device)
+        hint = self.max_seq_len if self.max_seq_len else S
+        check(_lib.load().chitu_b200_gqa_contiguous_attn(
+            ptr(q), ptr(k_cache), ptr(v_cache), cst[0], S, ptr(k), ptr(v), *strides, ptr(cache_seqlens), B, sq,
+            Hq, Hkv, D, int(hint), int(bool(causal)), float(scale), ptr(out), ptr(ws), wsn, dtype_code(q.dtype),
+            current_stream()), "gqa_contiguous_attn")
         return out
 
     # -- a2: attn_backend.py:707-774 (Triton), :536-572 (FlashMLA), :660-684 (FlashInfer)

@@ -5,6 +5,9 @@
 //    block table, online softmax in fp32, LSE-weighted merge of the splits.  Head dim 128 with
 //    power-of-two pages runs on tensor cores (gqa_decode_mmaT_kernel, optional fused rotary);
 //    head dim 64 and other page sizes run on the SIMT kernel (gqa_decode_kernel).
+//  * gqa_contiguous_attn : the same without a block table, over a [Bc, S, Hkv, D] cache (any S): the contiguous
+//    variants of both decode kernels for seqlen_q == 1 (head dim 128 always on tensor cores), gqa_prefill.cu's for
+//    seqlen_q > 1.
 //  * merge_splits_kernel : the LSE-weighted merge of split-KV partials, for GQA decode, MLA decode
 //    (mla_tc.cu) and the GQA and MLA paged prefills (gqa_prefill.cu, mla_prefill.cu).  The workspace
 //    layout, the split counts, the split plan and the merge weights are defined once in splitkv.cuh.
@@ -55,28 +58,37 @@ __global__ void merge_splits_kernel(const float* __restrict__ o_part, const floa
 // GQA: one CTA per (split, kv head, request); 4 warps interleave over keys, a lane owns D/32
 // consecutive dims, G = Hq/Hkv query heads share every K/V row that is loaded.
 // --------------------------------------------------------------------------------------------
-template <typename T, int D, int G>
-__global__ void __launch_bounds__(128) gqa_decode_kernel(
+// CONTIG: the cache is [Bc, cache_rows, Hkv, D] and request b owns the rows from b * rows_sb (rows of Hkv * D) instead
+// of the pages of its block-table row.  Its length is clamped to cache_rows, so no key at or past cache_rows is read, and
+// a new row at cache_rows or past it is not written.
+template <typename T, int D, int G, bool CONTIG>
+__device__ __forceinline__ void gqa_decode_cta(
     const T* __restrict__ q, T* __restrict__ k_cache, T* __restrict__ v_cache,
     const T* __restrict__ k_new, const T* __restrict__ v_new, int64_t k_new_sb, int64_t v_new_sb,
     const int32_t* __restrict__ seqlens,
-    const int32_t* __restrict__ block_table, int bt_stride, int Hq, int Hkv, int page_size, float scale,
-    int num_splits, float* __restrict__ o_part, float* __restrict__ lse, T* __restrict__ out) {
+    const int32_t* __restrict__ block_table, int bt_stride, int64_t rows_sb, int cache_rows, int Hq, int Hkv,
+    int page_size, float scale, int num_splits, float* __restrict__ o_part, float* __restrict__ lse,
+    T* __restrict__ out) {
   cb::pdl_prologue();
   constexpr int VEC = D / 32;
   const int split = blockIdx.x, kvh = blockIdx.y, b = blockIdx.z;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int L_cache = seqlens[b];
+  const int L_cache = CONTIG ? min(seqlens[b], cache_rows) : seqlens[b];
   const int L = L_cache + (k_new ? 1 : 0);
   const int chunk = (L + num_splits - 1) / num_splits;
   const int begin = split * chunk;
   const int end = min(begin + chunk, L);
   const int32_t* bt = block_table + (int64_t)b * bt_stride;
 
+  auto cache_row = [&](int key) -> int64_t {           // row of (key, kvh) in units of D
+    if constexpr (CONTIG) return ((int64_t)b * rows_sb + key) * Hkv + kvh;
+    const int page = bt[key / page_size];
+    return ((int64_t)page * page_size + key % page_size) * Hkv + kvh;
+  };
+
   // in-place append of the new token (true page_size indexing, as flash_attn_with_kvcache does)
-  if (k_new && split == 0 && warp == 0) {
-    const int page = bt[L_cache / page_size];
-    const int64_t row = ((int64_t)page * page_size + L_cache % page_size) * Hkv + kvh;
+  if (k_new && split == 0 && warp == 0 && (!CONTIG || L_cache < cache_rows)) {
+    const int64_t row = cache_row(L_cache);
     const T* ks = k_new + (int64_t)b * k_new_sb + kvh * D;
     const T* vs = v_new + (int64_t)b * v_new_sb + kvh * D;
 #pragma unroll
@@ -108,8 +120,7 @@ __global__ void __launch_bounds__(128) gqa_decode_kernel(
       valid[j] = key < end;
       const T *kp, *vp;
       if (valid[j] && key < L_cache) {
-        const int page = bt[key / page_size];
-        const int64_t row = ((int64_t)page * page_size + key % page_size) * Hkv + kvh;
+        const int64_t row = cache_row(key);
         kp = k_cache + row * D + lane * VEC;
         vp = v_cache + row * D + lane * VEC;
       } else {  // the token being appended (or a masked slot: loads are harmless, result unused)
@@ -185,6 +196,27 @@ __global__ void __launch_bounds__(128) gqa_decode_kernel(
   }
 }
 
+template <typename T, int D, int G>
+__global__ void __launch_bounds__(128) gqa_decode_kernel(
+    const T* __restrict__ q, T* __restrict__ k_cache, T* __restrict__ v_cache,
+    const T* __restrict__ k_new, const T* __restrict__ v_new, int64_t k_new_sb, int64_t v_new_sb,
+    const int32_t* __restrict__ seqlens,
+    const int32_t* __restrict__ block_table, int bt_stride, int Hq, int Hkv, int page_size, float scale,
+    int num_splits, float* __restrict__ o_part, float* __restrict__ lse, T* __restrict__ out) {
+  gqa_decode_cta<T, D, G, false>(q, k_cache, v_cache, k_new, v_new, k_new_sb, v_new_sb, seqlens, block_table, bt_stride,
+                                 0, 0, Hq, Hkv, page_size, scale, num_splits, o_part, lse, out);
+}
+
+template <typename T, int D, int G>
+__global__ void __launch_bounds__(128) gqa_decode_contig_kernel(
+    const T* __restrict__ q, T* __restrict__ k_cache, T* __restrict__ v_cache,
+    const T* __restrict__ k_new, const T* __restrict__ v_new, int64_t k_new_sb, int64_t v_new_sb,
+    const int32_t* __restrict__ seqlens, int64_t rows_sb, int cache_rows, int Hq, int Hkv, float scale,
+    int num_splits, float* __restrict__ o_part, float* __restrict__ lse, T* __restrict__ out) {
+  gqa_decode_cta<T, D, G, true>(q, k_cache, v_cache, k_new, v_new, k_new_sb, v_new_sb, seqlens, nullptr, 0, rows_sb,
+                                cache_rows, Hq, Hkv, 1, scale, num_splits, o_part, lse, out);
+}
+
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;"); }
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N)); }
@@ -244,13 +276,15 @@ __device__ __forceinline__ uint32_t movmatrix_trans(uint32_t a) {
   return d;
 }
 
-template <typename T, int G>
-__global__ void __launch_bounds__(kGqaWarps * 32, kGqaCtas) gqa_decode_mmaT_kernel(
+// CONTIG: the contiguous cache of gqa_decode_cta, with no page shift, so any cache_rows runs on tensor cores.
+template <typename T, int G, bool CONTIG>
+__device__ __forceinline__ void gqa_decode_mmaT_cta(
     const T* __restrict__ q, T* __restrict__ k_cache, T* __restrict__ v_cache, const T* __restrict__ k_new,
     const T* __restrict__ v_new, int64_t k_new_sb, int64_t v_new_sb,
     const int32_t* __restrict__ seqlens, const int32_t* __restrict__ block_table, int bt_stride, int Hq, int Hkv,
     int page_shift, float scale, int num_splits, float* __restrict__ o_part, float* __restrict__ lse,
-    T* __restrict__ out, int64_t q_sb, const float* __restrict__ cosp, const float* __restrict__ sinp) {
+    T* __restrict__ out, int64_t q_sb, const float* __restrict__ cosp, const float* __restrict__ sinp, int64_t rows_sb,
+    int cache_rows) {
   static_assert(G <= 8, "heads of one kv group are the n = 8 side of the MMA");
   // The K/V pages are only written by earlier decode steps and by this kernel; sequence lengths and the block table by
   // kernels that do not trigger dependents early: the first tiles of every warp are put in flight BEFORE
@@ -265,7 +299,7 @@ __global__ void __launch_bounds__(kGqaWarps * 32, kGqaCtas) gqa_decode_mmaT_kern
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int g = lane >> 2, t = lane & 3;
   const int page_size = 1 << page_shift;
-  const int L_cache = seqlens[b];
+  const int L_cache = CONTIG ? min(seqlens[b], cache_rows) : seqlens[b];
   const int L = L_cache + (k_new ? 1 : 0);
   const int chunk = (((L + num_splits - 1) / num_splits) + kGqaTile - 1) / kGqaTile * kGqaTile;
   const int begin = split * chunk;
@@ -288,8 +322,13 @@ __global__ void __launch_bounds__(kGqaWarps * 32, kGqaCtas) gqa_decode_mmaT_kern
       const T *ksrc = k_cache, *vsrc = v_cache;
       int nbytes = 16;
       if (key < L_cache && key < end) {
-        const int page = bt[key >> page_shift];
-        const int64_t row = ((int64_t)page * page_size + (key & (page_size - 1))) * Hkv + kvh;
+        int64_t row;                         // row of (key, kvh) in units of D
+        if constexpr (CONTIG) {
+          row = ((int64_t)b * rows_sb + key) * Hkv + kvh;
+        } else {
+          const int page = bt[key >> page_shift];
+          row = ((int64_t)page * page_size + (key & (page_size - 1))) * Hkv + kvh;
+        }
         ksrc = k_cache + row * D;
         vsrc = v_cache + row * D;
       } else if (key < end) {                // the token being appended (key == L_cache)
@@ -332,9 +371,14 @@ __global__ void __launch_bounds__(kGqaWarps * 32, kGqaCtas) gqa_decode_mmaT_kern
     k_rot = reinterpret_cast<const uint2*>(k_new + (int64_t)b * k_new_sb + kvh * D)[lane];
     if (cosp) { k_rot.x = rot_pair(k_rot.x, 2 * lane); k_rot.y = rot_pair(k_rot.y, 2 * lane + 1); }
   }
-  if (k_new && split == 0 && warp == 0) {   // in-place append (true page_size indexing)
-    const int page = bt[L_cache >> page_shift];
-    const int64_t row = ((int64_t)page * page_size + (L_cache & (page_size - 1))) * Hkv + kvh;
+  if (k_new && split == 0 && warp == 0 && (!CONTIG || L_cache < cache_rows)) {   // in-place append (true page_size indexing)
+    int64_t row;
+    if constexpr (CONTIG) {
+      row = ((int64_t)b * rows_sb + L_cache) * Hkv + kvh;
+    } else {
+      const int page = bt[L_cache >> page_shift];
+      row = ((int64_t)page * page_size + (L_cache & (page_size - 1))) * Hkv + kvh;
+    }
     const uint2* vs = reinterpret_cast<const uint2*>(v_new + (int64_t)b * v_new_sb + kvh * D);
     reinterpret_cast<uint2*>(k_cache + row * D)[lane] = k_rot;
     reinterpret_cast<uint2*>(v_cache + row * D)[lane] = vs[lane];
@@ -358,7 +402,7 @@ __global__ void __launch_bounds__(kGqaWarps * 32, kGqaCtas) gqa_decode_mmaT_kern
   float o[8][4];
 #pragma unroll
   for (int j = 0; j < 8; ++j) o[j][0] = o[j][1] = o[j][2] = o[j][3] = 0.f;
-  float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;     // heads 2t and 2t+1 (log2 domain max)
+  float m1 = -INFINITY, m0 = -INFINITY, l0 = 0.f, l1 = 0.f;     // heads 2t and 2t+1 (log2 domain max)
   const float sc = scale * kLog2e;
 
   for (int s = 0; s < kGqaStages - 1; ++s) {
@@ -503,6 +547,29 @@ __global__ void __launch_bounds__(kGqaWarps * 32, kGqaCtas) gqa_decode_mmaT_kern
   }
 }
 
+template <typename T, int G>
+__global__ void __launch_bounds__(kGqaWarps * 32, kGqaCtas) gqa_decode_mmaT_kernel(
+    const T* __restrict__ q, T* __restrict__ k_cache, T* __restrict__ v_cache, const T* __restrict__ k_new,
+    const T* __restrict__ v_new, int64_t k_new_sb, int64_t v_new_sb,
+    const int32_t* __restrict__ seqlens, const int32_t* __restrict__ block_table, int bt_stride, int Hq, int Hkv,
+    int page_shift, float scale, int num_splits, float* __restrict__ o_part, float* __restrict__ lse,
+    T* __restrict__ out, int64_t q_sb, const float* __restrict__ cosp, const float* __restrict__ sinp) {
+  gqa_decode_mmaT_cta<T, G, false>(q, k_cache, v_cache, k_new, v_new, k_new_sb, v_new_sb, seqlens, block_table,
+                                   bt_stride, Hq, Hkv, page_shift, scale, num_splits, o_part, lse, out, q_sb, cosp, sinp,
+                                   0, 0);
+}
+
+template <typename T, int G>
+__global__ void __launch_bounds__(kGqaWarps * 32, kGqaCtas) gqa_decode_mmaT_contig_kernel(
+    const T* __restrict__ q, T* __restrict__ k_cache, T* __restrict__ v_cache, const T* __restrict__ k_new,
+    const T* __restrict__ v_new, int64_t k_new_sb, int64_t v_new_sb, const int32_t* __restrict__ seqlens,
+    int64_t rows_sb, int cache_rows, int Hq, int Hkv, float scale, int num_splits, float* __restrict__ o_part,
+    float* __restrict__ lse, T* __restrict__ out) {
+  gqa_decode_mmaT_cta<T, G, true>(q, k_cache, v_cache, k_new, v_new, k_new_sb, v_new_sb, seqlens, nullptr, 0, Hq, Hkv,
+                                  0, scale, num_splits, o_part, lse, out, (int64_t)Hq * kGqaD, nullptr, nullptr, rows_sb,
+                                  cache_rows);
+}
+
 }  // namespace
 
 extern "C" int64_t chitu_b200_attn_workspace_bytes(int batch, int heads, int head_dim_v, int max_splits) {
@@ -620,6 +687,78 @@ extern "C" int chitu_b200_gqa_paged_decode_rope(const void* q, int64_t q_sb, voi
   return 0;
 }
 
+// flash_attn_with_kvcache without a block table (include/chitu_b200.h): sq == 1 runs the decode kernels' contiguous
+// variants here, sq > 1 the multi-token kernel's (gqa_prefill.cu).
+extern "C" int chitu_b200_gqa_contiguous_attn(const void* q, void* k_cache, void* v_cache, int64_t cache_sb,
+                                              int cache_rows, const void* k_new, const void* v_new, int64_t k_new_sb,
+                                              int64_t k_new_st, int64_t v_new_sb, int64_t v_new_st,
+                                              const int32_t* cache_seqlens, int B, int sq, int Hq, int Hkv, int D,
+                                              int max_seqlen_hint, int causal, float softmax_scale, void* out,
+                                              void* workspace, int64_t workspace_bytes, int dtype, void* stream) {
+  CB_ARG(q && k_cache && v_cache && cache_seqlens && out);
+  CB_ARG((k_new == nullptr) == (v_new == nullptr));
+  CB_ARG(B >= 0 && B <= 65535 && sq >= 1 && Hq > 0 && Hkv > 0 && Hkv <= 65535 && Hq % Hkv == 0);
+  const int G = Hq / Hkv;
+  CB_ARG(G == 1 || G == 2 || G == 4 || G == 8);
+  CB_ARG(D == 128 || (D == 64 && sq == 1));
+  CB_ARG(dtype == CB_BF16 || dtype == CB_F16);
+  const int64_t row = (int64_t)Hkv * D;                     // elements of one cache position
+  CB_ARG(cache_rows >= 1 && cache_sb >= cache_rows * row && cache_sb % row == 0 && cache_sb % 8 == 0);
+  CB_ARG(((uintptr_t)q | (uintptr_t)k_cache | (uintptr_t)v_cache | (uintptr_t)out | (uintptr_t)k_new |
+          (uintptr_t)v_new) % 16 == 0);
+  const int sa = sq == 1 ? 4 : 8;                           // k / v stride multiple: the decode kernels load 8 bytes
+  CB_ARG(k_new == nullptr || (k_new_sb % sa == 0 && k_new_st % sa == 0 && v_new_sb % sa == 0 && v_new_st % sa == 0));
+  CB_ARG(workspace == nullptr || (uintptr_t)workspace % 16 == 0);
+  if (B == 0) return 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int max_len = max_seqlen_hint > 0 ? max_seqlen_hint : cache_rows;
+  const int64_t rows_sb = cache_sb / row;
+  if (sq > 1)
+    return gqa_contiguous_prefill(q, k_cache, v_cache, rows_sb, cache_rows, k_new, v_new, k_new_sb, k_new_st,
+                                  v_new_sb, v_new_st, cache_seqlens, B, sq, Hq, Hkv, max_len, causal, softmax_scale, out,
+                                  workspace, workspace_bytes, dtype, st);
+
+  const bool tc = D == kGqaD;
+  int splits = tc ? pick_splits_waves(B * Hkv, max_len, 132 * kGqaCtas) : pick_splits(B * Hkv, max_len, 256, 64);
+  splits = workspace ? splits_that_fit(splits, (int64_t)B * Hq, D, workspace_bytes) : 1;
+  const auto [o_part, lse, plan] = split_kv_carve(workspace, workspace_bytes, (int64_t)B * Hq, D, splits);
+  const dim3 grid(splits, Hkv, B);
+#define LAUNCH_CONTIG(T, GG)                                                                                      \
+  do {                                                                                                            \
+    if (tc) {                                                                                                     \
+      static bool attr = false;                                                                                   \
+      if (!attr) {                                                                                                \
+        CB_CUDA(cudaFuncSetAttribute(gqa_decode_mmaT_contig_kernel<T, GG>,                                        \
+                                     cudaFuncAttributeMaxDynamicSharedMemorySize, kGqaSmemBytes));                \
+        attr = true;                                                                                              \
+      }                                                                                                           \
+      cb::launch_k(gqa_decode_mmaT_contig_kernel<T, GG>, grid, dim3(kGqaWarps * 32), (size_t)kGqaSmemBytes, st,   \
+                   (const T*)q, (T*)k_cache, (T*)v_cache, (const T*)k_new, (const T*)v_new, k_new_sb, v_new_sb,   \
+                   cache_seqlens, rows_sb, cache_rows, Hq, Hkv, softmax_scale, splits, o_part, lse, (T*)out);     \
+    } else {                                                                                                      \
+      cb::launch_k(gqa_decode_contig_kernel<T, 64, GG>, grid, dim3(128), 0, st, (const T*)q, (T*)k_cache,         \
+                   (T*)v_cache, (const T*)k_new, (const T*)v_new, k_new_sb, v_new_sb, cache_seqlens, rows_sb,     \
+                   cache_rows, Hq, Hkv, softmax_scale, splits, o_part, lse, (T*)out);                             \
+    }                                                                                                             \
+  } while (0)
+#define DISPATCH_CONTIG(T)                 \
+  switch (G) {                             \
+    case 1: LAUNCH_CONTIG(T, 1); break;    \
+    case 2: LAUNCH_CONTIG(T, 2); break;    \
+    case 4: LAUNCH_CONTIG(T, 4); break;    \
+    default: LAUNCH_CONTIG(T, 8); break;   \
+  }
+  if (dtype == CB_BF16) { DISPATCH_CONTIG(__nv_bfloat16); } else { DISPATCH_CONTIG(__half); }
+#undef DISPATCH_CONTIG
+#undef LAUNCH_CONTIG
+  CB_LAUNCHED(1);
+  if (splits > 1) {
+    int rc = launch_merge_splits(o_part, lse, out, B * Hq, splits, D, dtype, st);
+    if (rc) return rc;
+    CB_LAUNCHED(1);
+  }
+  return 0;
+}
 
 // ============================================================================================
 // MLA weight absorption (the two torch.einsum of AttentionDeepSeekV3, model_deepseek_v3.py:529-531

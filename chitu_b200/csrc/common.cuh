@@ -129,6 +129,19 @@ struct PagedAppend {
 void launch_paged_append(PagedAppend c0, PagedAppend c1, int64_t row_bytes, const int32_t* seqlens,
                          const int32_t* block_table, int bt_stride, int B, int sq, int page_size, int index_div,
                          cudaStream_t st);
+// The same copy into contiguous caches: position p of request b is cache row b * rows_sb + p, and rows with
+// p >= cache_rows are skipped.
+void launch_contiguous_append(PagedAppend c0, PagedAppend c1, int64_t row_bytes, const int32_t* seqlens,
+                              int64_t rows_sb, int cache_rows, int B, int sq, cudaStream_t st);
+
+// ---- GQA attention over a contiguous cache with sq > 1 (gqa_prefill.cu), the multi-token path of
+// chitu_b200_gqa_contiguous_attn, which checks the arguments.  rows_sb: the caches' batch stride in rows of Hkv * D.
+// Launches the append (with k_new), the attention and, with a split, the merge, and counts them.
+int gqa_contiguous_prefill(const void* q, void* k_cache, void* v_cache, int64_t rows_sb, int cache_rows,
+                           const void* k_new, const void* v_new, int64_t k_new_sb, int64_t k_new_st, int64_t v_new_sb,
+                           int64_t v_new_st, const int32_t* cache_seqlens, int B, int sq, int Hq, int Hkv, int max_len,
+                           int causal, float softmax_scale, void* out, void* workspace, int64_t workspace_bytes,
+                           int dtype, cudaStream_t st);
 
 #ifdef __CUDACC__
 // byte offset of this rank's area inside every push buffer, for the reduce that is being produced

@@ -72,16 +72,19 @@ extern "C" const char* chitu_b200_debug_timeline_names(void) { return cb::g_tl_n
 
 // ============================================================================================
 // Paged append: row i of request b is written to position p = seqlens[b] + i, i.e. to cache row
-// block_table[b, p / index_div] * page_size + p % index_div, of one or two caches.  One CTA per
-// row; 16-byte copies when every address and stride allows them, byte copies otherwise.
+// block_table[b, p / index_div] * page_size + p % index_div, of one or two caches (contiguous
+// caches: row b * rows_sb + p, p < cache_rows).  One CTA per row; 16-byte copies when every
+// address and stride allows them, byte copies otherwise.
 // ============================================================================================
 // Row i of request b (n units of V) into both caches; bt is the request's block-table row.  A thread issues its source
 // loads for two passes over both caches before the page lookup and the stores, so the copy's memory round trip
 // overlaps the lookup's.  The compiler would not order them so itself: it cannot tell that sources and caches never
 // overlap, and with bt __restrict__ it hoists the lookup above the loads.
-template <typename V>
+// CONTIG: the destination is row b * rows_sb + p of contiguous caches; bt, page_size and index_div are unused.
+template <typename V, bool CONTIG>
 __device__ __forceinline__ void copy_row(const cb::PagedAppend& c0, const cb::PagedAppend& c1, int p,
-                                         const int32_t* bt, int page_size, int index_div, int b, int i, int64_t n) {
+                                         const int32_t* bt, int page_size, int index_div, int64_t rows_sb, int b, int i,
+                                         int64_t n) {
   const V* s0 = reinterpret_cast<const V*>((const uint8_t*)c0.src + b * c0.src_sb + i * c0.src_st);
   const V* s1 = reinterpret_cast<const V*>((const uint8_t*)c1.src + b * c1.src_sb + i * c1.src_st);
   const bool two = c1.cache != nullptr;
@@ -92,7 +95,7 @@ __device__ __forceinline__ void copy_row(const cb::PagedAppend& c0, const cb::Pa
     if (w < n) y0 = s0[w];
     if (two) x1 = s1[u];
     if (two && w < n) y1 = s1[w];
-    const int64_t row = (int64_t)bt[p / index_div] * page_size + p % index_div;
+    const int64_t row = CONTIG ? (int64_t)b * rows_sb + p : (int64_t)bt[p / index_div] * page_size + p % index_div;
     V* d0 = reinterpret_cast<V*>(c0.cache) + row * n;
     V* d1 = reinterpret_cast<V*>(c1.cache) + row * n;
     d0[u] = x0;
@@ -102,31 +105,58 @@ __device__ __forceinline__ void copy_row(const cb::PagedAppend& c0, const cb::Pa
   }
 }
 
-__global__ void __launch_bounds__(128) paged_append_kernel(cb::PagedAppend c0, cb::PagedAppend c1, int64_t row_bytes,
-                                                           const int32_t* __restrict__ seqlens,
-                                                           const int32_t* block_table, int bt_stride, int B,
-                                                           int page_size, int index_div, int vec) {
+template <bool CONTIG>
+__device__ __forceinline__ void append_rows(const cb::PagedAppend& c0, const cb::PagedAppend& c1, int64_t row_bytes,
+                                            const int32_t* __restrict__ seqlens, const int32_t* block_table,
+                                            int bt_stride, int B, int page_size, int index_div, int64_t rows_sb,
+                                            int cache_rows, int vec) {
   cb::pdl_prologue();
   const int i = blockIdx.x;
   for (int b = blockIdx.y; b < B; b += gridDim.y) {     // more than 65535 requests: a CTA takes several
     const int p = seqlens[b] + i;
+    if (CONTIG && p >= cache_rows) continue;           // past the contiguous cache's capacity: not written
     const int32_t* bt = block_table + (int64_t)b * bt_stride;
-    if (vec) copy_row<uint4>(c0, c1, p, bt, page_size, index_div, b, i, row_bytes >> 4);
-    else copy_row<uint8_t>(c0, c1, p, bt, page_size, index_div, b, i, row_bytes);
+    if (vec) copy_row<uint4, CONTIG>(c0, c1, p, bt, page_size, index_div, rows_sb, b, i, row_bytes >> 4);
+    else copy_row<uint8_t, CONTIG>(c0, c1, p, bt, page_size, index_div, rows_sb, b, i, row_bytes);
   }
 }
 
+__global__ void __launch_bounds__(128) paged_append_kernel(cb::PagedAppend c0, cb::PagedAppend c1, int64_t row_bytes,
+                                                           const int32_t* __restrict__ seqlens,
+                                                           const int32_t* block_table, int bt_stride, int B,
+                                                           int page_size, int index_div, int vec) {
+  append_rows<false>(c0, c1, row_bytes, seqlens, block_table, bt_stride, B, page_size, index_div, 0, 0, vec);
+}
+
+__global__ void __launch_bounds__(128) contiguous_append_kernel(cb::PagedAppend c0, cb::PagedAppend c1,
+                                                                int64_t row_bytes, const int32_t* __restrict__ seqlens,
+                                                                int64_t rows_sb, int cache_rows, int B, int vec) {
+  append_rows<true>(c0, c1, row_bytes, seqlens, nullptr, 0, B, 1, 1, rows_sb, cache_rows, vec);
+}
+
 namespace cb {
-void launch_paged_append(PagedAppend c0, PagedAppend c1, int64_t row_bytes, const int32_t* seqlens,
-                         const int32_t* block_table, int bt_stride, int B, int sq, int page_size, int index_div,
-                         cudaStream_t st) {
+// 16-byte copies when every address and stride allows them; 64 threads for rows of fewer than 128 copy units
+static int append_vec(const PagedAppend& c0, const PagedAppend& c1, int64_t row_bytes) {
   uintptr_t bits = (uintptr_t)row_bytes;
   for (const PagedAppend& c : {c0, c1})
     if (c.cache) bits |= (uintptr_t)c.cache | (uintptr_t)c.src | (uintptr_t)c.src_sb | (uintptr_t)c.src_st;
-  const int vec = bits % 16 == 0;
-  const int threads = row_bytes / (vec ? 16 : 1) < 128 ? 64 : 128;
-  launch_k(paged_append_kernel, dim3(sq, B < 65535 ? B : 65535), dim3(threads), 0, st, c0, c1, row_bytes, seqlens,
-           block_table, bt_stride, B, page_size, index_div, vec);
+  return bits % 16 == 0;
+}
+static int append_threads(int64_t row_bytes, int vec) { return row_bytes / (vec ? 16 : 1) < 128 ? 64 : 128; }
+
+void launch_paged_append(PagedAppend c0, PagedAppend c1, int64_t row_bytes, const int32_t* seqlens,
+                         const int32_t* block_table, int bt_stride, int B, int sq, int page_size, int index_div,
+                         cudaStream_t st) {
+  const int vec = append_vec(c0, c1, row_bytes);
+  launch_k(paged_append_kernel, dim3(sq, B < 65535 ? B : 65535), dim3(append_threads(row_bytes, vec)), 0, st, c0, c1,
+           row_bytes, seqlens, block_table, bt_stride, B, page_size, index_div, vec);
+}
+
+void launch_contiguous_append(PagedAppend c0, PagedAppend c1, int64_t row_bytes, const int32_t* seqlens,
+                              int64_t rows_sb, int cache_rows, int B, int sq, cudaStream_t st) {
+  const int vec = append_vec(c0, c1, row_bytes);
+  launch_k(contiguous_append_kernel, dim3(sq, B < 65535 ? B : 65535), dim3(append_threads(row_bytes, vec)), 0, st, c0,
+           c1, row_bytes, seqlens, rows_sb, cache_rows, B, vec);
 }
 }  // namespace cb
 

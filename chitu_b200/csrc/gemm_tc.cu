@@ -590,17 +590,19 @@ int make_tma_map_2d(CUtensorMap* map, const void* base, int64_t rows, int64_t co
   return 0;
 }
 
-int make_tma_map_3d(CUtensorMap* map, const void* base, const cuuint64_t dims[3], const cuuint64_t strides[2],
+int make_tma_map_nd(CUtensorMap* map, const void* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides,
                     int elem_bytes, CUtensorMapDataType dt, int box_outer) {
   PFN_encodeTiled enc = get_encode();
   if (!enc) return fail(-3, "cuTensorMapEncodeTiled is not available from the driver");
-  cuuint32_t box[3] = {(cuuint32_t)(128 / elem_bytes), 1, (cuuint32_t)box_outer};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = enc(map, dt, 3, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+  if (rank != 3 && rank != 4) return fail(-1, "make_tma_map_nd: rank %d is not 3 or 4", rank);
+  cuuint32_t box[4] = {(cuuint32_t)(128 / elem_bytes), 1, (cuuint32_t)box_outer, 1};
+  cuuint32_t estr[4] = {1, 1, 1, 1};
+  CUresult r = enc(map, dt, rank, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                    CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS)
-    return fail(-3, "cuTensorMapEncodeTiled failed (CUresult %d) dims=%llu,%llu,%llu", (int)r, (unsigned long long)dims[0],
-                (unsigned long long)dims[1], (unsigned long long)dims[2]);
+    return fail(-3, "cuTensorMapEncodeTiled failed (CUresult %d) rank %d dims=%llu,%llu,%llu,%llu", (int)r, rank,
+                (unsigned long long)dims[0], (unsigned long long)dims[1], (unsigned long long)dims[2],
+                (unsigned long long)(rank > 3 ? dims[3] : 1));
   return 0;
 }
 

@@ -24,6 +24,8 @@
 // Paging safety: only block_table[b, 0 .. ceil(Lk / page) - 1] is read; V rows of keys >= Lk in the last tile are zeroed
 // in shared memory before P.V (unused slots may hold NaN, and 0 * NaN would poison O); their scores are replaced by -inf.
 // Shared memory: Q 16 KB + 2 x 32 KB ring = 80 KB + 1 KB alignment.
+// Non-paged cache (chitu_b200_gqa_contiguous_attn, no block table): the same CTA compiled with a 4-D map over
+// [B, S, Hkv, 128] caches (gqa_prefill_contig_kernel); TMA zero-fills keys >= S, so any S works.
 // Split over keys when (row tiles x Hkv x B) CTAs cannot fill the GPU: split s of a CTA takes an equal share of the
 // CTA's key tiles and writes normalised fp32 partials + LSE to the workspace as [B, sq * Hq, S, 128] (the decode
 // layout with H = sq * Hq), merged by attention.cu's merge_splits_kernel.  Deterministic: the split count depends on
@@ -87,9 +89,21 @@ template <> struct Mma<__half> {
   }
 };
 
-template <typename T, int G>
-__global__ void __launch_bounds__(kThreads, kCtasPerSm) gqa_prefill_kernel(
-    const __grid_constant__ CUtensorMap map_k, const __grid_constant__ CUtensorMap map_v, const T* __restrict__ q,
+__device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2,
+                                            int c3, uint64_t policy) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
+      " [%0], [%1, {%3, %4, %5, %6}], [%2], %7;"
+      ::"r"(smem_u32(smem_dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "l"(policy)
+      : "memory");
+}
+
+// CONTIG: the maps are 4-D over a contiguous cache, (128, Hkv, cache_rows, B) with the cache's batch stride, and key
+// tile t of request b is the box at (c, kvh, 64 t, b).  Rows at or past cache_rows are zero-filled by TMA, so no box
+// reads another request's rows; block_table, bt_stride and page are unused.
+template <typename T, int G, bool CONTIG>
+__device__ __forceinline__ void gqa_prefill_cta(
+    const CUtensorMap& map_k, const CUtensorMap& map_v, const T* __restrict__ q,
     const int32_t* __restrict__ cache_seqlens, const int32_t* __restrict__ block_table, int bt_stride, int sq, int Hq,
     int Hkv, int page, int appended, int causal, float scale, int row_tiles, int splits, float* __restrict__ o_part,
     float* __restrict__ lse, T* __restrict__ out) {
@@ -121,6 +135,16 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) gqa_prefill_kernel(
   auto load_tile = [&](int t) {                             // key tile t into its ring slot (one thread)
     const int slot = (t - t_begin) % kStages;
     const int key0 = t * kTile;
+    if constexpr (CONTIG) {
+      uint8_t* dst = s_ring + slot * kStageBytes;
+      mbar_expect_tx(&kfull[slot], 2 * kSlot);
+      tma_load_4d(dst, &map_k, &kfull[slot], 0, kvh, key0, b, pol_kv);
+      tma_load_4d(dst + kSlot, &map_k, &kfull[slot], 64, kvh, key0, b, pol_kv);
+      mbar_expect_tx(&vfull[slot], 2 * kSlot);
+      tma_load_4d(dst + 2 * kSlot, &map_v, &vfull[slot], 0, kvh, key0, b, pol_kv);
+      tma_load_4d(dst + 3 * kSlot, &map_v, &vfull[slot], 64, kvh, key0, b, pol_kv);
+      return;
+    }
     const int prow = block_table[(int64_t)b * bt_stride + key0 / page] * page + key0 % page;
     uint8_t* dst = s_ring + slot * kStageBytes;
     mbar_expect_tx(&kfull[slot], 2 * kSlot);
@@ -276,7 +300,99 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) gqa_prefill_kernel(
   }
 }
 
+template <typename T, int G>
+__global__ void __launch_bounds__(kThreads, kCtasPerSm) gqa_prefill_kernel(
+    const __grid_constant__ CUtensorMap map_k, const __grid_constant__ CUtensorMap map_v, const T* __restrict__ q,
+    const int32_t* __restrict__ cache_seqlens, const int32_t* __restrict__ block_table, int bt_stride, int sq, int Hq,
+    int Hkv, int page, int appended, int causal, float scale, int row_tiles, int splits, float* __restrict__ o_part,
+    float* __restrict__ lse, T* __restrict__ out) {
+  gqa_prefill_cta<T, G, false>(map_k, map_v, q, cache_seqlens, block_table, bt_stride, sq, Hq, Hkv, page, appended,
+                               causal, scale, row_tiles, splits, o_part, lse, out);
+}
+
+template <typename T, int G>
+__global__ void __launch_bounds__(kThreads, kCtasPerSm) gqa_prefill_contig_kernel(
+    const __grid_constant__ CUtensorMap map_k, const __grid_constant__ CUtensorMap map_v, const T* __restrict__ q,
+    const int32_t* __restrict__ cache_seqlens, int sq, int Hq, int Hkv, int appended, int causal, float scale,
+    int row_tiles, int splits, float* __restrict__ o_part, float* __restrict__ lse, T* __restrict__ out) {
+  gqa_prefill_cta<T, G, true>(map_k, map_v, q, cache_seqlens, nullptr, 0, sq, Hq, Hkv, kTile, appended, causal, scale,
+                              row_tiles, splits, o_part, lse, out);
+}
+
+// splits of the multi-token kernel: the decode kernels' wave rule on its CTAs, shrunk to the workspace (none: 1 split)
+int prefill_splits(int row_tiles, int Hkv, int B, int64_t rows, int max_len, const void* workspace,
+                   int64_t workspace_bytes) {
+  const int splits = pick_splits_waves(row_tiles * Hkv * B, max_len, 132 * kCtasPerSm);
+  return workspace ? splits_that_fit(splits, rows, kD, workspace_bytes) : 1;
+}
+
+CUtensorMapDataType tma_dtype(int dtype) {
+  return dtype == CB_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+}
+
 }  // namespace
+
+// The multi-token path of chitu_b200_gqa_contiguous_attn (attention.cu), which has checked the arguments.
+int gqa_contiguous_prefill(const void* q, void* k_cache, void* v_cache, int64_t rows_sb, int cache_rows,
+                           const void* k_new, const void* v_new, int64_t k_new_sb, int64_t k_new_st, int64_t v_new_sb,
+                           int64_t v_new_st, const int32_t* cache_seqlens, int B, int sq, int Hq, int Hkv, int max_len,
+                           int causal, float softmax_scale, void* out, void* workspace, int64_t workspace_bytes,
+                           int dtype, cudaStream_t st) {
+  if (!tma_available()) return fail(-3, "gqa_contiguous_attn: TMA is not available");
+  const int G = Hq / Hkv;
+  const int row_tiles = cdiv((int64_t)sq * G, kRows);
+  const int64_t rows = (int64_t)B * sq * Hq;
+  const int splits = prefill_splits(row_tiles, Hkv, B, rows, max_len, workspace, workspace_bytes);
+  if ((int64_t)row_tiles * splits > INT_MAX)
+    return fail(-1, "gqa_contiguous_attn: %d row tiles x %d splits exceed the grid", row_tiles, splits);
+  const auto [o_part, lse, plan] = split_kv_carve(splits > 1 ? workspace : nullptr, workspace_bytes, rows, kD, splits);
+
+  // the caches as (D, Hkv, cache_rows, B): a box (64, 1, 64, 1) is 64 keys x 64 dims of one head of one request
+  CUtensorMap mk, mv;
+  const cuuint64_t dims[4] = {(cuuint64_t)kD, (cuuint64_t)Hkv, (cuuint64_t)cache_rows, (cuuint64_t)B};
+  const cuuint64_t strides[3] = {(cuuint64_t)kD * 2, (cuuint64_t)Hkv * kD * 2, (cuuint64_t)rows_sb * Hkv * kD * 2};
+  int rc = make_tma_map_nd(&mk, k_cache, 4, dims, strides, 2, tma_dtype(dtype), kTile);
+  if (!rc) rc = make_tma_map_nd(&mv, v_cache, 4, dims, strides, 2, tma_dtype(dtype), kTile);
+  if (rc) return rc;
+
+  if (k_new) {                                              // the sq new k / v rows first
+    launch_contiguous_append({k_cache, k_new, k_new_sb * 2, k_new_st * 2}, {v_cache, v_new, v_new_sb * 2, v_new_st * 2},
+                             (int64_t)Hkv * kD * 2, cache_seqlens, rows_sb, cache_rows, B, sq, st);
+    CB_LAUNCHED(1);
+  }
+
+  const size_t smem = 1024 + (size_t)kSmemBytes;
+  const dim3 grid(row_tiles * splits, Hkv, B);
+#define LAUNCH_PREFILL(T, GG)                                                                                     \
+  do {                                                                                                            \
+    static bool attr = false;                                                                                     \
+    if (!attr) {                                                                                                  \
+      CB_CUDA(cudaFuncSetAttribute(gqa_prefill_contig_kernel<T, GG>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
+                                   (int)smem));                                                                   \
+      attr = true;                                                                                                \
+    }                                                                                                             \
+    launch_k(gqa_prefill_contig_kernel<T, GG>, grid, dim3(kThreads), smem, st, mk, mv, (const T*)q, cache_seqlens, \
+             sq, Hq, Hkv, k_new ? 1 : 0, causal ? 1 : 0, softmax_scale, row_tiles, splits, o_part, lse, (T*)out);  \
+  } while (0)
+#define DISPATCH_PREFILL(T)                \
+  switch (G) {                             \
+    case 1: LAUNCH_PREFILL(T, 1); break;   \
+    case 2: LAUNCH_PREFILL(T, 2); break;   \
+    case 4: LAUNCH_PREFILL(T, 4); break;   \
+    default: LAUNCH_PREFILL(T, 8); break;  \
+  }
+  if (dtype == CB_BF16) { DISPATCH_PREFILL(__nv_bfloat16); } else { DISPATCH_PREFILL(__half); }
+#undef DISPATCH_PREFILL
+#undef LAUNCH_PREFILL
+  CB_LAUNCHED(1);
+  if (splits > 1) {
+    rc = launch_merge_splits(o_part, lse, out, B * sq * Hq, splits, kD, dtype, st);
+    if (rc) return rc;
+    CB_LAUNCHED(1);
+  }
+  return 0;
+}
+
 }  // namespace cb
 
 // flash_attn_with_kvcache (paged) with seqlen_q >= 1 (include/chitu_b200.h).
@@ -307,10 +423,8 @@ extern "C" int chitu_b200_gqa_paged_prefill(const void* q, void* k_cache, void* 
 
   const int row_tiles = cdiv((int64_t)sq * G, kRows);
   const int max_len = max_seqlen_hint > 0 ? max_seqlen_hint : bt_stride * page_size;
-  // the decode kernels' wave rule on this kernel's CTAs, shrunk to the workspace (none: 1 split)
   const int64_t rows = (int64_t)B * sq * Hq;
-  int splits = pick_splits_waves(row_tiles * Hkv * B, max_len, 132 * kCtasPerSm);
-  splits = workspace ? splits_that_fit(splits, rows, kD, workspace_bytes) : 1;
+  const int splits = prefill_splits(row_tiles, Hkv, B, rows, max_len, workspace, workspace_bytes);
   if ((int64_t)row_tiles * splits > INT_MAX)
     return fail(-1, "gqa_paged_prefill: %d row tiles x %d splits exceed the grid", row_tiles, splits);
   const auto [o_part, lse, plan] = split_kv_carve(splits > 1 ? workspace : nullptr, workspace_bytes, rows, kD, splits);
@@ -319,11 +433,8 @@ extern "C" int chitu_b200_gqa_paged_prefill(const void* q, void* k_cache, void* 
   CUtensorMap mk, mv;
   const cuuint64_t dims[3] = {(cuuint64_t)kD, (cuuint64_t)Hkv, (cuuint64_t)num_blocks * page_size};
   const cuuint64_t strides[2] = {(cuuint64_t)kD * 2, (cuuint64_t)Hkv * kD * 2};
-  int rc = make_tma_map_3d(&mk, k_cache, dims, strides, 2,
-                           dtype == CB_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, kTile);
-  if (!rc) rc = make_tma_map_3d(&mv, v_cache, dims, strides, 2,
-                                dtype == CB_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16,
-                                kTile);
+  int rc = make_tma_map_nd(&mk, k_cache, 3, dims, strides, 2, tma_dtype(dtype), kTile);
+  if (!rc) rc = make_tma_map_nd(&mv, v_cache, 3, dims, strides, 2, tma_dtype(dtype), kTile);
   if (rc) return rc;
 
   cudaStream_t st = (cudaStream_t)stream;

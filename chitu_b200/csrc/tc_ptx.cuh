@@ -96,8 +96,9 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
 // between rows (0 = dense, cols); a multiple of 16 bytes.
 int make_tma_map_2d(CUtensorMap* map, const void* base, int64_t rows, int64_t cols, int elem_bytes,
                     CUtensorMapDataType dt, int box_rows, int64_t row_stride = 0);
-// 3-D tensor, dims innermost first, byte strides of dims 1 and 2; box = [128 bytes, 1, box_outer], 128B swizzle.
-int make_tma_map_3d(CUtensorMap* map, const void* base, const cuuint64_t dims[3], const cuuint64_t strides[2],
+// 3-D or 4-D tensor (rank), dims innermost first, byte strides of dims 1 .. rank - 1; box = [128 bytes, 1, box_outer]
+// (and 1 along dim 3), 128B swizzle, zero fill outside the tensor.
+int make_tma_map_nd(CUtensorMap* map, const void* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides,
                     int elem_bytes, CUtensorMapDataType dt, int box_outer);
 bool tma_available();
 

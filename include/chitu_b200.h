@@ -208,6 +208,29 @@ int chitu_b200_gqa_paged_prefill(const void* q, void* k_cache, void* v_cache, co
                                  int Hq, int Hkv, int D, int page_size, int num_blocks, int max_seqlen_hint, int causal,
                                  float softmax_scale, void* out, void* workspace, int64_t workspace_bytes, int dtype,
                                  void* stream);
+/* AttnBackend.attn_with_kvcache WITHOUT block_table (attn_backend.py:92-164; FlashAttn impl :208-243 passes no block
+ * table, RefAttnBackend :458-501 implements only this form), seqlen_q = sq >= 1: GQA attention over the non-paged
+ * per-request cache of KVCacheManager (cache_manager.py:228-370).  k_cache / v_cache [Bc, cache_rows, Hkv, D] with
+ * Bc >= B, the same shape and strides, dense last two dims and a batch stride cache_sb in elements (a multiple of
+ * Hkv * D and of 8, at least cache_rows * Hkv * D: a [:B, :S] view of a larger buffer is accepted); request b uses
+ * cache row b.  q [B, sq, Hq, D] contiguous; k_new / v_new [B, sq, Hkv, D] with dense heads and batch / token strides
+ * *_sb / *_st in elements, or both NULL.  With k_new: token i of request b is written to position cache_seqlens[b] + i
+ * before the attention, which then runs over Lk = cache_seqlens[b] + sq keys; without, Lk = cache_seqlens[b].
+ * cache_seqlens is not modified.  causal != 0: query i sees key j iff j <= i + Lk - sq; a row that sees no key is 0.
+ * fp32 scores and softmax, P rounded to the io dtype before P.V.  out [B, sq, Hq, D] contiguous.
+ * Capacity: a new row at a position >= cache_rows is not written and no key >= cache_rows is read (the output of such
+ * a request is unspecified); nothing outside the request's rows of the caches is touched.
+ * sq == 1 runs the decode kernels (tensor cores for D == 128), sq > 1 the multi-token kernel; splits over keys as in
+ * the paged entries, from B, Hkv, sq and max_seqlen_hint (<= 0: cache_rows), shrunk to the workspace (NULL: no split)
+ * -> no host synchronisation, capturable in a CUDA graph, deterministic.
+ * Built for Hq / Hkv in {1, 2, 4, 8}, bf16 | fp16, D in {64, 128} for sq == 1 and D == 128 for sq > 1, any
+ * cache_rows >= 1; 16-byte aligned bases; k / v strides multiples of 4 elements (sq == 1) or 8 (sq > 1).  Anything
+ * else returns a negative status.  B == 0 launches nothing. */
+int chitu_b200_gqa_contiguous_attn(const void* q, void* k_cache, void* v_cache, int64_t cache_sb, int cache_rows,
+                                   const void* k_new, const void* v_new, int64_t k_new_sb, int64_t k_new_st,
+                                   int64_t v_new_sb, int64_t v_new_st, const int32_t* cache_seqlens, int B, int sq,
+                                   int Hq, int Hkv, int D, int max_seqlen_hint, int causal, float softmax_scale,
+                                   void* out, void* workspace, int64_t workspace_bytes, int dtype, void* stream);
 
 
 /* *.mla_attn_with_kvcache (attn_backend.py:536-572 / 660-684 / 707-774) = append
