@@ -59,6 +59,8 @@ SIGNATURES = {
     "chitu_b200_gqa_paged_prefill": (I, [P, P, P, P, P, L, L, L, L, P, P, I, I, I, I, I, I, I, I, I, I, F, P, P, L, I,
                                          P]),
     "chitu_b200_gqa_contiguous_attn": (I, [P, P, P, L, I, P, P, L, L, L, L, P, I, I, I, I, I, I, I, F, P, P, L, I, P]),
+    "chitu_b200_gqa_paged_attn_fp8kv": (I, [P, L, P, P, P, P, L, L, L, L, P, P, P, P, I, I, I, I, I, I, I, I, I, I, F, P,
+                                            P, L, I, P]),
     "chitu_b200_mla_decode": (I, [P, P, P, P, P, P, I, I, I, I, I, I, I, I, F, P, P, L, P]),
     "chitu_b200_mla_prefill": (I, [P, P, L, P, L, P, P, I, I, I, I, I, I, F, P, P]),
     "chitu_b200_mla_paged_prefill": (I, [P, P, P, P, P, P, I, I, I, I, I, I, I, I, I, I, F, P, P, L, P]),

@@ -4,10 +4,11 @@
 prepare_metadata_for_decode, attn_varlen_func (prefill: the absorbed-MLA form runs the sm_90a
 prefill kernel; GQA prefill stays on flash_attn / torch SDPA), attn_with_kvcache (GQA attention over the KV cache
 with in-place append: the decode kernel for seqlen_q == 1, the sm_90a multi-token kernel for seqlen_q > 1 — chunked
-prefill, prefill on a cached prefix, speculative verification; over the paged cache with a block_table, and over the
-non-paged [B, S, Hkv, D] cache of KVCacheManager without one) and mla_attn_with_kvcache (absorbed-MLA
-attention over the paged latent cache: the decode kernel with fused append for one query token per request, the
-sm_90a multi-token kernel for seqlen_q > 1 — multi-token-prediction verification, chunked prefill on a cached prefix).
+prefill, prefill on a cached prefix, speculative verification; over the paged cache with a block_table, in the io dtype
+or in fp8 e4m3 (half the KV bytes), and over the non-paged [B, S, Hkv, D] cache of KVCacheManager without one) and
+mla_attn_with_kvcache (absorbed-MLA attention over the paged latent cache: the decode kernel with fused append for one
+query token per request, the sm_90a multi-token kernel for seqlen_q > 1 — multi-token-prediction verification, chunked
+prefill on a cached prefix).
 """
 from __future__ import annotations
 
@@ -164,16 +165,27 @@ class B200AttnBackend(AttnBackend):
                           cache_leftpad: Optional[torch.Tensor] = None,
                           block_table: Optional[torch.Tensor] = None, causal=False, window_size=(-1, -1),
                           softcap=0.0, softmax_scale=None):
+        """GQA attention over the KV cache with the in-place append of k / v (flash_attn_with_kvcache semantics).
+        q [B, sq, Hq, D]; with block_table the caches are paged [num_blocks, page, Hkv, D], without it [Bc, S, Hkv, D].
+        A paged cache in torch.float8_e4m3fn (both caches) runs `_paged_fp8`; otherwise the caches are in q's dtype."""
+        fp8 = (k_cache.dtype == torch.float8_e4m3fn, v_cache.dtype == torch.float8_e4m3fn)
+        if fp8[0] != fp8[1]:
+            raise RuntimeError("attn_with_kvcache: k_cache and v_cache must have the same dtype")
         if block_table is None:
+            if fp8[0]:
+                raise RuntimeError("attn_with_kvcache: the fp8 KV cache is built for the paged cache only")
             return self._contiguous(q, k_cache, v_cache, k, v, cache_seqlens, cache_leftpad, causal, window_size,
                                     softcap, softmax_scale)
         assert cache_leftpad is None and window_size == (-1, -1) and softcap == 0.0
         require_cuda(q, k_cache, v_cache, block_table)
         B, sq, Hq, D = q.shape
+        if fp8[0]:
+            return self._paged_fp8(q, k_cache, v_cache, k, v, cache_seqlens, block_table, causal, softmax_scale)
         if sq > 1:
             return self._paged_prefill(q, k_cache, v_cache, k, v, cache_seqlens, block_table, causal, softmax_scale)
         num_blocks, page, Hkv, Dk = k_cache.shape
         assert Dk == D and v_cache.shape == k_cache.shape
+        assert k_cache.dtype == v_cache.dtype == q.dtype and (k is None or k.dtype == v.dtype == q.dtype)
         assert q.is_contiguous() and k_cache.is_contiguous() and v_cache.is_contiguous()
         assert block_table.dtype == torch.int32 and block_table.stride(-1) == 1
         if not torch.is_tensor(cache_seqlens):
@@ -222,6 +234,37 @@ class B200AttnBackend(AttnBackend):
             ptr(q), ptr(k_cache), ptr(v_cache), ptr(k), ptr(v), *strides, ptr(cache_seqlens), ptr(block_table),
             block_table.stride(0), B, sq, Hq, Hkv, D, page, num_blocks, int(hint), int(bool(causal)), float(scale),
             ptr(out), ptr(ws), wsn, dtype_code(q.dtype), current_stream()), "gqa_paged_prefill")
+        return out
+
+    def _paged_fp8(self, q, k_cache, v_cache, k, v, cache_seqlens, block_table, causal, softmax_scale):
+        """Paged e4m3 caches, sq >= 1 (chitu_b200_gqa_paged_attn_fp8kv): the semantics of the io-dtype paged cache, with
+        each new k / v element stored as x.float().clamp(-448, 448).to(float8_e4m3fn) and each cache element decoded
+        exactly to q's dtype (bf16 | fp16) before the unchanged arithmetic.  The appended rows are attended in their
+        stored form.  No scale.  Built for D == 128, Hq / Hkv in {1, 2, 4, 8} and a power-of-two page that is a multiple
+        of 64; no host synchronisation, capturable in a CUDA graph, deterministic."""
+        B, sq, Hq, D = q.shape
+        num_blocks, page, Hkv, Dk = k_cache.shape
+        assert Dk == D and v_cache.shape == k_cache.shape
+        assert q.dtype in (torch.bfloat16, torch.float16) and (k is None or k.dtype == v.dtype == q.dtype)
+        assert q.is_contiguous() and k_cache.is_contiguous() and v_cache.is_contiguous()
+        assert block_table.dtype == torch.int32 and block_table.stride(-1) == 1
+        if not torch.is_tensor(cache_seqlens):
+            cache_seqlens = torch.full((B,), int(cache_seqlens), dtype=torch.int32, device=q.device)
+        assert cache_seqlens.dtype == torch.int32 and cache_seqlens.is_contiguous()
+        strides = (0, 0, 0, 0)
+        if k is not None:
+            assert v is not None and k.shape == (B, sq, Hkv, D) and v.shape == (B, sq, Hkv, D)
+            # heads must be dense; the batch and token strides are free (views into a fused qkv GEMM output)
+            assert k.stride(-1) == 1 and k.stride(-2) == D and v.stride(-1) == 1 and v.stride(-2) == D
+            strides = (k.stride(0), k.stride(1), v.stride(0), v.stride(1))
+        scale = softmax_scale if softmax_scale is not None else 1.0 / math.sqrt(D)
+        out = torch.empty_like(q)
+        ws, wsn = self._ws(B, Hq, D, q.device)
+        hint = self.max_seq_len if self.max_seq_len else block_table.shape[1] * page
+        check(_lib.load().chitu_b200_gqa_paged_attn_fp8kv(
+            ptr(q), sq * Hq * D, ptr(k_cache), ptr(v_cache), ptr(k), ptr(v), *strides, None, None, ptr(cache_seqlens),
+            ptr(block_table), block_table.stride(0), B, sq, Hq, Hkv, D, page, num_blocks, int(hint), int(bool(causal)),
+            float(scale), ptr(out), ptr(ws), wsn, dtype_code(q.dtype), current_stream()), "gqa_paged_attn_fp8kv")
         return out
 
     def _contiguous(self, q, k_cache, v_cache, k, v, cache_seqlens, cache_leftpad, causal, window_size, softcap,

@@ -8,6 +8,8 @@
 //  * gqa_contiguous_attn : the same without a block table, over a [Bc, S, Hkv, D] cache (any S): the contiguous
 //    variants of both decode kernels for seqlen_q == 1 (head dim 128 always on tensor cores), gqa_prefill.cu's for
 //    seqlen_q > 1.
+//  * gqa_paged_attn_fp8kv : the paged cache in fp8 e4m3 (half the KV bytes): the e4m3 instance of the tensor-core
+//    decode kernel for seqlen_q == 1 (gqa_decode_mmaT_e4m3_kernel), gqa_prefill.cu's e4m3 instance for seqlen_q > 1.
 //  * merge_splits_kernel : the LSE-weighted merge of split-KV partials, for GQA decode, MLA decode
 //    (mla_tc.cu) and the GQA and MLA paged prefills (gqa_prefill.cu, mla_prefill.cu).  The workspace
 //    layout, the split counts, the split plan and the merge weights are defined once in splitkv.cuh.
@@ -276,16 +278,25 @@ __device__ __forceinline__ uint32_t movmatrix_trans(uint32_t a) {
   return d;
 }
 
+// Smem of the e4m3-cache instances: per warp the ring of e4m3 tiles and one K | V tile pair in the io dtype.
+constexpr int kGqaE4m3SmemBytes = kGqaWarps * (kGqaStages * 2 * (kGqaTile * kGqaD) + 2 * (kGqaTile * kGqaD * 2));
+
 // CONTIG: the contiguous cache of gqa_decode_cta, with no page shift, so any cache_rows runs on tensor cores.
-template <typename T, int G, bool CONTIG>
+// C: the cache element, T or uint8_t (e4m3).  With e4m3 the ring stages e4m3 tiles (half the bytes per key) and each
+// warp converts its tile into the io-dtype swizzled tile the MMA path reads; the new row is rounded to e4m3 once, and
+// that value is both stored and staged.  Same tiles and splits as the io-dtype cache, so on e4m3-representable data
+// the result is bit-identical.
+template <typename T, typename C, int G, bool CONTIG>
 __device__ __forceinline__ void gqa_decode_mmaT_cta(
-    const T* __restrict__ q, T* __restrict__ k_cache, T* __restrict__ v_cache, const T* __restrict__ k_new,
+    const T* __restrict__ q, C* __restrict__ k_cache, C* __restrict__ v_cache, const T* __restrict__ k_new,
     const T* __restrict__ v_new, int64_t k_new_sb, int64_t v_new_sb,
     const int32_t* __restrict__ seqlens, const int32_t* __restrict__ block_table, int bt_stride, int Hq, int Hkv,
     int page_shift, float scale, int num_splits, float* __restrict__ o_part, float* __restrict__ lse,
     T* __restrict__ out, int64_t q_sb, const float* __restrict__ cosp, const float* __restrict__ sinp, int64_t rows_sb,
     int cache_rows) {
   static_assert(G <= 8, "heads of one kv group are the n = 8 side of the MMA");
+  constexpr bool kE4m3 = sizeof(C) == 1;
+  static_assert(!(kE4m3 && CONTIG), "the e4m3 cache is paged");
   // The K/V pages are only written by earlier decode steps and by this kernel; sequence lengths and the block table by
   // kernels that do not trigger dependents early: the first tiles of every warp are put in flight BEFORE
   // griddepcontrol.wait (they overlap the tail of the qkv GEMM); q / k_new / v_new (the previous kernel's output) are
@@ -293,8 +304,9 @@ __device__ __forceinline__ void gqa_decode_mmaT_cta(
   cb::pdl_launch_dependents();
   constexpr int D = kGqaD;
   constexpr int kTileBytes = kGqaTile * D * 2;              // K tile bytes (V the same)
+  constexpr int kRingTile = kGqaTile * D * sizeof(C);       // bytes of a staged K tile
   constexpr int MT = kGqaTile / 16;                         // key m-tiles per tile
-  extern __shared__ __align__(128) uint8_t gqa_smem[];      // [warp][stage][K tile | V tile]
+  extern __shared__ __align__(128) uint8_t gqa_smem[];      // [warp][stage][K tile | V tile] (e4m3: + [K | V] io)
   const int split = blockIdx.x, kvh = blockIdx.y, b = blockIdx.z;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int g = lane >> 2, t = lane & 3;
@@ -306,42 +318,65 @@ __device__ __forceinline__ void gqa_decode_mmaT_cta(
   const int end = min(begin + chunk, L);
   const int32_t* bt = block_table + (int64_t)b * bt_stride;
 
-  const uint32_t smem_warp = (uint32_t)__cvta_generic_to_shared(gqa_smem) + warp * (kGqaStages * 2 * kTileBytes);
+  const uint32_t smem_warp = (uint32_t)__cvta_generic_to_shared(gqa_smem) +
+                             warp * (kGqaStages * 2 * kRingTile + (kE4m3 ? 2 * kTileBytes : 0));
   const int ntiles_total = end > begin ? (end - begin + kGqaTile - 1) / kGqaTile : 0;
   // tiles warp, warp + kGqaWarps, ...
   const int my_tiles = ntiles_total > warp ? (ntiles_total - warp + kGqaWarps - 1) / kGqaWarps : 0;
 
   auto issue = [&](int ti, int stage) {
     const int key0 = begin + (warp + kGqaWarps * ti) * kGqaTile;
-    const uint32_t sk = smem_warp + stage * (2 * kTileBytes), sv = sk + kTileBytes;
+    if constexpr (kE4m3) {                   // rows of 128 bytes, unswizzled; the appended and masked rows are zero
+      const uint32_t sk = smem_warp + stage * (2 * kRingTile), sv = sk + kRingTile;
 #pragma unroll
-    for (int i = 0; i < kGqaTile / 2; ++i) {
-      const int c = i * 32 + lane;           // 16-byte chunk id within the tile: row = c/16, col = c%16
-      const int r = c >> 4, cc = c & 15;
-      const int key = key0 + r;
-      const T *ksrc = k_cache, *vsrc = v_cache;
-      int nbytes = 16;
-      if (key < L_cache && key < end) {
-        int64_t row;                         // row of (key, kvh) in units of D
-        if constexpr (CONTIG) {
-          row = ((int64_t)b * rows_sb + key) * Hkv + kvh;
-        } else {
+      for (int i = 0; i < kGqaTile / 4; ++i) {
+        const int c = i * 32 + lane;         // 16-byte chunk id within the tile: row = c/8, col = c%8
+        const int r = c >> 3, cc = c & 7;
+        const int key = key0 + r;
+        const C *ksrc = k_cache, *vsrc = v_cache;
+        int nbytes = 0;
+        if (key < L_cache && key < end) {
           const int page = bt[key >> page_shift];
-          row = ((int64_t)page * page_size + (key & (page_size - 1))) * Hkv + kvh;
+          const int64_t row = ((int64_t)page * page_size + (key & (page_size - 1))) * Hkv + kvh;
+          ksrc = k_cache + row * D;
+          vsrc = v_cache + row * D;
+          nbytes = 16;
         }
-        ksrc = k_cache + row * D;
-        vsrc = v_cache + row * D;
-      } else if (key < end) {                // the token being appended (key == L_cache)
-        ksrc = k_new + (int64_t)b * k_new_sb + kvh * D;
-        vsrc = v_new + (int64_t)b * v_new_sb + kvh * D;
-      } else {
-        nbytes = 0;                          // masked row: zero fill
+        cp_async16_g(sk + c * 16, ksrc + cc * 16, nbytes);
+        cp_async16_g(sv + c * 16, vsrc + cc * 16, nbytes);
       }
-      const uint32_t off = r * 256 + ((cc ^ (r & 7)) << 4);
-      cp_async16_g(sk + off, ksrc + cc * 8, nbytes);
-      cp_async16_g(sv + off, vsrc + cc * 8, nbytes);
+      cp_async_commit();
+    } else {
+      const uint32_t sk = smem_warp + stage * (2 * kTileBytes), sv = sk + kTileBytes;
+#pragma unroll
+      for (int i = 0; i < kGqaTile / 2; ++i) {
+        const int c = i * 32 + lane;         // 16-byte chunk id within the tile: row = c/16, col = c%16
+        const int r = c >> 4, cc = c & 15;
+        const int key = key0 + r;
+        const T *ksrc = k_cache, *vsrc = v_cache;
+        int nbytes = 16;
+        if (key < L_cache && key < end) {
+          int64_t row;                       // row of (key, kvh) in units of D
+          if constexpr (CONTIG) {
+            row = ((int64_t)b * rows_sb + key) * Hkv + kvh;
+          } else {
+            const int page = bt[key >> page_shift];
+            row = ((int64_t)page * page_size + (key & (page_size - 1))) * Hkv + kvh;
+          }
+          ksrc = k_cache + row * D;
+          vsrc = v_cache + row * D;
+        } else if (key < end) {              // the token being appended (key == L_cache)
+          ksrc = k_new + (int64_t)b * k_new_sb + kvh * D;
+          vsrc = v_new + (int64_t)b * v_new_sb + kvh * D;
+        } else {
+          nbytes = 0;                        // masked row: zero fill
+        }
+        const uint32_t off = r * 256 + ((cc ^ (r & 7)) << 4);
+        cp_async16_g(sk + off, ksrc + cc * 8, nbytes);
+        cp_async16_g(sv + off, vsrc + cc * 8, nbytes);
+      }
+      cp_async_commit();
     }
-    cp_async_commit();
   };
 
   // tiles that lie completely inside the cached part of the sequence can be fetched before the previous kernel is done
@@ -371,6 +406,16 @@ __device__ __forceinline__ void gqa_decode_mmaT_cta(
     k_rot = reinterpret_cast<const uint2*>(k_new + (int64_t)b * k_new_sb + kvh * D)[lane];
     if (cosp) { k_rot.x = rot_pair(k_rot.x, 2 * lane); k_rot.y = rot_pair(k_rot.y, 2 * lane + 1); }
   }
+  // e4m3: the new row rounded once; k8 / v8 are stored, their decoded values kd / vd replace the zero-filled staged row
+  uint32_t k8 = 0u, v8 = 0u;
+  uint2 kd = make_uint2(0u, 0u), vd = make_uint2(0u, 0u);
+  if (kE4m3 && k_new) {
+    const uint2 vr = reinterpret_cast<const uint2*>(v_new + (int64_t)b * v_new_sb + kvh * D)[lane];
+    k8 = io2_to_e4m3x2<T>(k_rot.x) | io2_to_e4m3x2<T>(k_rot.y) << 16;
+    v8 = io2_to_e4m3x2<T>(vr.x) | io2_to_e4m3x2<T>(vr.y) << 16;
+    E4m3<T>::to_io(k8, kd.x, kd.y);
+    E4m3<T>::to_io(v8, vd.x, vd.y);
+  }
   if (k_new && split == 0 && warp == 0 && (!CONTIG || L_cache < cache_rows)) {   // in-place append (true page_size indexing)
     int64_t row;
     if constexpr (CONTIG) {
@@ -379,9 +424,14 @@ __device__ __forceinline__ void gqa_decode_mmaT_cta(
       const int page = bt[L_cache >> page_shift];
       row = ((int64_t)page * page_size + (L_cache & (page_size - 1))) * Hkv + kvh;
     }
-    const uint2* vs = reinterpret_cast<const uint2*>(v_new + (int64_t)b * v_new_sb + kvh * D);
-    reinterpret_cast<uint2*>(k_cache + row * D)[lane] = k_rot;
-    reinterpret_cast<uint2*>(v_cache + row * D)[lane] = vs[lane];
+    if constexpr (kE4m3) {
+      reinterpret_cast<uint32_t*>(k_cache + row * D)[lane] = k8;
+      reinterpret_cast<uint32_t*>(v_cache + row * D)[lane] = v8;
+    } else {
+      const uint2* vs = reinterpret_cast<const uint2*>(v_new + (int64_t)b * v_new_sb + kvh * D);
+      reinterpret_cast<uint2*>(k_cache + row * D)[lane] = k_rot;
+      reinterpret_cast<uint2*>(v_cache + row * D)[lane] = vs[lane];
+    }
   }
 
   // Q^T fragments (B operand, k = 16 dims x n = 8 heads): head g of the group, zero for g >= G
@@ -415,9 +465,36 @@ __device__ __forceinline__ void gqa_decode_mmaT_cta(
     else cp_async_commit();
     cp_async_wait<kGqaStages - 1>();
     __syncwarp();
-    const uint32_t sk = smem_warp + stage * (2 * kTileBytes), sv = sk + kTileBytes;
+    const uint32_t sk = smem_warp + (kE4m3 ? kGqaStages : stage) * (2 * kRingTile), sv = sk + kTileBytes;
     const int key0 = begin + (warp + kGqaWarps * ti) * kGqaTile;
-    if (cosp && k_new && L_cache >= key0 && L_cache < key0 + kGqaTile && L_cache < end) {
+    if constexpr (kE4m3) {
+      // the staged e4m3 tiles -> io tiles: lane converts 16-byte chunks (16 dims of one key) into two swizzled chunks
+      const uint32_t rk = smem_warp + stage * (2 * kRingTile);
+#pragma unroll
+      for (int kv = 0; kv < 2; ++kv) {
+#pragma unroll
+        for (int i = 0; i < kGqaTile / 4; ++i) {
+          const int c = i * 32 + lane, r = c >> 3, cc = c & 7;
+          uint32_t w[4], h[8];
+          asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];"
+                       : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3]) : "r"(rk + kv * kRingTile + c * 16));
+#pragma unroll
+          for (int j = 0; j < 4; ++j) E4m3<T>::to_io(w[j], h[2 * j], h[2 * j + 1]);
+          const uint32_t dst = sk + kv * kTileBytes + r * 256;
+          asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};"
+                       ::"r"(dst + (((2 * cc) ^ (r & 7)) << 4)), "r"(h[0]), "r"(h[1]), "r"(h[2]), "r"(h[3]) : "memory");
+          asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};"
+                       ::"r"(dst + (((2 * cc + 1) ^ (r & 7)) << 4)), "r"(h[4]), "r"(h[5]), "r"(h[6]), "r"(h[7]) : "memory");
+        }
+      }
+      if (k_new && L_cache >= key0 && L_cache < key0 + kGqaTile && L_cache < end) {
+        const int r = L_cache - key0;
+        const uint32_t a = sk + r * 256 + (((lane >> 1) ^ (r & 7)) << 4) + (lane & 1) * 8;
+        asm volatile("st.shared.v2.u32 [%0], {%1, %2};" ::"r"(a), "r"(kd.x), "r"(kd.y) : "memory");
+        asm volatile("st.shared.v2.u32 [%0], {%1, %2};" ::"r"(a + kTileBytes), "r"(vd.x), "r"(vd.y) : "memory");
+      }
+      __syncwarp();
+    } else if (cosp && k_new && L_cache >= key0 && L_cache < key0 + kGqaTile && L_cache < end) {
       // the appended row was staged un-rotated from k_new: overwrite it with the rotated row
       const int r = L_cache - key0;
       const uint32_t a = sk + r * 256 + (((lane >> 1) ^ (r & 7)) << 4) + (lane & 1) * 8;
@@ -554,9 +631,21 @@ __global__ void __launch_bounds__(kGqaWarps * 32, kGqaCtas) gqa_decode_mmaT_kern
     const int32_t* __restrict__ seqlens, const int32_t* __restrict__ block_table, int bt_stride, int Hq, int Hkv,
     int page_shift, float scale, int num_splits, float* __restrict__ o_part, float* __restrict__ lse,
     T* __restrict__ out, int64_t q_sb, const float* __restrict__ cosp, const float* __restrict__ sinp) {
-  gqa_decode_mmaT_cta<T, G, false>(q, k_cache, v_cache, k_new, v_new, k_new_sb, v_new_sb, seqlens, block_table,
-                                   bt_stride, Hq, Hkv, page_shift, scale, num_splits, o_part, lse, out, q_sb, cosp, sinp,
-                                   0, 0);
+  gqa_decode_mmaT_cta<T, T, G, false>(q, k_cache, v_cache, k_new, v_new, k_new_sb, v_new_sb, seqlens, block_table,
+                                      bt_stride, Hq, Hkv, page_shift, scale, num_splits, o_part, lse, out, q_sb, cosp,
+                                      sinp, 0, 0);
+}
+
+template <typename T, int G>
+__global__ void __launch_bounds__(kGqaWarps * 32, kGqaCtas) gqa_decode_mmaT_e4m3_kernel(
+    const T* __restrict__ q, uint8_t* __restrict__ k_cache, uint8_t* __restrict__ v_cache, const T* __restrict__ k_new,
+    const T* __restrict__ v_new, int64_t k_new_sb, int64_t v_new_sb,
+    const int32_t* __restrict__ seqlens, const int32_t* __restrict__ block_table, int bt_stride, int Hq, int Hkv,
+    int page_shift, float scale, int num_splits, float* __restrict__ o_part, float* __restrict__ lse,
+    T* __restrict__ out, int64_t q_sb, const float* __restrict__ cosp, const float* __restrict__ sinp) {
+  gqa_decode_mmaT_cta<T, uint8_t, G, false>(q, k_cache, v_cache, k_new, v_new, k_new_sb, v_new_sb, seqlens,
+                                            block_table, bt_stride, Hq, Hkv, page_shift, scale, num_splits, o_part, lse,
+                                            out, q_sb, cosp, sinp, 0, 0);
 }
 
 template <typename T, int G>
@@ -565,9 +654,9 @@ __global__ void __launch_bounds__(kGqaWarps * 32, kGqaCtas) gqa_decode_mmaT_cont
     const T* __restrict__ v_new, int64_t k_new_sb, int64_t v_new_sb, const int32_t* __restrict__ seqlens,
     int64_t rows_sb, int cache_rows, int Hq, int Hkv, float scale, int num_splits, float* __restrict__ o_part,
     float* __restrict__ lse, T* __restrict__ out) {
-  gqa_decode_mmaT_cta<T, G, true>(q, k_cache, v_cache, k_new, v_new, k_new_sb, v_new_sb, seqlens, nullptr, 0, Hq, Hkv,
-                                  0, scale, num_splits, o_part, lse, out, (int64_t)Hq * kGqaD, nullptr, nullptr, rows_sb,
-                                  cache_rows);
+  gqa_decode_mmaT_cta<T, T, G, true>(q, k_cache, v_cache, k_new, v_new, k_new_sb, v_new_sb, seqlens, nullptr, 0, Hq,
+                                     Hkv, 0, scale, num_splits, o_part, lse, out, (int64_t)Hq * kGqaD, nullptr, nullptr,
+                                     rows_sb, cache_rows);
 }
 
 }  // namespace
@@ -751,6 +840,79 @@ extern "C" int chitu_b200_gqa_contiguous_attn(const void* q, void* k_cache, void
   if (dtype == CB_BF16) { DISPATCH_CONTIG(__nv_bfloat16); } else { DISPATCH_CONTIG(__half); }
 #undef DISPATCH_CONTIG
 #undef LAUNCH_CONTIG
+  CB_LAUNCHED(1);
+  if (splits > 1) {
+    int rc = launch_merge_splits(o_part, lse, out, B * Hq, splits, D, dtype, st);
+    if (rc) return rc;
+    CB_LAUNCHED(1);
+  }
+  return 0;
+}
+
+// flash_attn_with_kvcache (paged) over an e4m3 cache (include/chitu_b200.h): sq == 1 runs the e4m3 instance of the
+// tensor-core decode kernel here, sq > 1 the multi-token kernel's (gqa_prefill.cu).
+extern "C" int chitu_b200_gqa_paged_attn_fp8kv(const void* q, int64_t q_sb, void* k_cache, void* v_cache,
+                                               const void* k_new, const void* v_new, int64_t k_new_sb, int64_t k_new_st,
+                                               int64_t v_new_sb, int64_t v_new_st, const float* rope_cos,
+                                               const float* rope_sin, const int32_t* cache_seqlens,
+                                               const int32_t* block_table, int bt_stride, int B, int sq, int Hq,
+                                               int Hkv, int D, int page_size, int num_blocks, int max_seqlen_hint,
+                                               int causal, float softmax_scale, void* out, void* workspace,
+                                               int64_t workspace_bytes, int dtype, void* stream) {
+  CB_ARG(q && k_cache && v_cache && cache_seqlens && block_table && out);
+  CB_ARG((k_new == nullptr) == (v_new == nullptr) && (rope_cos == nullptr) == (rope_sin == nullptr));
+  CB_ARG(B >= 0 && B <= 65535 && sq >= 1 && Hq > 0 && Hkv > 0 && Hkv <= 65535 && Hq % Hkv == 0);
+  const int G = Hq / Hkv;
+  CB_ARG(G == 1 || G == 2 || G == 4 || G == 8);
+  CB_ARG(D == kGqaD);
+  CB_ARG(dtype == CB_BF16 || dtype == CB_F16);
+  CB_ARG(bt_stride > 0 && num_blocks > 0 && page_size >= 64 && page_size % 64 == 0 &&
+         (page_size & (page_size - 1)) == 0 && (int64_t)num_blocks * page_size <= 0x7fffffff);
+  CB_ARG(rope_cos == nullptr || sq == 1);
+  CB_ARG((int64_t)sq * Hq <= 0x7fffffff / D && q_sb % 8 == 0 &&
+         (sq == 1 ? q_sb >= (int64_t)Hq * D : q_sb == (int64_t)sq * Hq * D));
+  CB_ARG(((uintptr_t)q | (uintptr_t)k_cache | (uintptr_t)v_cache | (uintptr_t)out | (uintptr_t)k_new |
+          (uintptr_t)v_new) % 16 == 0);
+  CB_ARG(k_new == nullptr || (k_new_sb % 8 == 0 && v_new_sb % 8 == 0 && (sq == 1 || (k_new_st % 8 == 0 &&
+                                                                                      v_new_st % 8 == 0))));
+  CB_ARG(workspace == nullptr || (uintptr_t)workspace % 16 == 0);
+  if (B == 0) return 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int max_len = max_seqlen_hint > 0 ? max_seqlen_hint : bt_stride * page_size;
+  if (sq > 1)
+    return gqa_paged_prefill_e4m3(q, k_cache, v_cache, k_new, v_new, k_new_sb, k_new_st, v_new_sb, v_new_st,
+                                  cache_seqlens, block_table, bt_stride, B, sq, Hq, Hkv, page_size, num_blocks, max_len,
+                                  causal, softmax_scale, out, workspace, workspace_bytes, dtype, st);
+
+  int page_shift = 0;
+  while ((1 << page_shift) < page_size) ++page_shift;
+  int splits = pick_splits_waves(B * Hkv, max_len, 132 * kGqaCtas);      // the io-dtype decode's splits
+  splits = workspace ? splits_that_fit(splits, (int64_t)B * Hq, D, workspace_bytes) : 1;
+  const auto [o_part, lse, plan] = split_kv_carve(workspace, workspace_bytes, (int64_t)B * Hq, D, splits);
+  const dim3 grid(splits, Hkv, B);
+#define LAUNCH_E4M3(T, GG)                                                                                         \
+  do {                                                                                                             \
+    static bool attr = false;                                                                                      \
+    if (!attr) {                                                                                                   \
+      CB_CUDA(cudaFuncSetAttribute(gqa_decode_mmaT_e4m3_kernel<T, GG>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
+                                   kGqaE4m3SmemBytes));                                                            \
+      attr = true;                                                                                                 \
+    }                                                                                                              \
+    cb::launch_k(gqa_decode_mmaT_e4m3_kernel<T, GG>, grid, dim3(kGqaWarps * 32), (size_t)kGqaE4m3SmemBytes, st,    \
+                 (const T*)q, (uint8_t*)k_cache, (uint8_t*)v_cache, (const T*)k_new, (const T*)v_new, k_new_sb,      \
+                 v_new_sb, cache_seqlens, block_table, bt_stride, Hq, Hkv, page_shift, softmax_scale, splits, o_part, \
+                 lse, (T*)out, q_sb, rope_cos, rope_sin);                                                          \
+  } while (0)
+#define DISPATCH_E4M3(T)                 \
+  switch (G) {                           \
+    case 1: LAUNCH_E4M3(T, 1); break;    \
+    case 2: LAUNCH_E4M3(T, 2); break;    \
+    case 4: LAUNCH_E4M3(T, 4); break;    \
+    default: LAUNCH_E4M3(T, 8); break;   \
+  }
+  if (dtype == CB_BF16) { DISPATCH_E4M3(__nv_bfloat16); } else { DISPATCH_E4M3(__half); }
+#undef DISPATCH_E4M3
+#undef LAUNCH_E4M3
   CB_LAUNCHED(1);
   if (splits > 1) {
     int rc = launch_merge_splits(o_part, lse, out, B * Hq, splits, D, dtype, st);

@@ -133,6 +133,19 @@ void launch_paged_append(PagedAppend c0, PagedAppend c1, int64_t row_bytes, cons
 // p >= cache_rows are skipped.
 void launch_contiguous_append(PagedAppend c0, PagedAppend c1, int64_t row_bytes, const int32_t* seqlens,
                               int64_t rows_sb, int cache_rows, int B, int sq, cudaStream_t st);
+// The paged append (true page indexing) into two e4m3 caches: rows of n io elements (dtype CB_BF16 | CB_F16,
+// n % 8 == 0, 16-byte aligned sources and strides) stored as e4m3 with io2_to_e4m3x2's rounding.
+void launch_paged_append_e4m3(PagedAppend c0, PagedAppend c1, int n, int dtype, const int32_t* seqlens,
+                              const int32_t* block_table, int bt_stride, int B, int sq, int page_size, cudaStream_t st);
+
+// ---- GQA attention over an e4m3 paged cache with sq > 1 (gqa_prefill.cu), the multi-token path of
+// chitu_b200_gqa_paged_attn_fp8kv, which checks the arguments.  Launches the append (with k_new), the attention and,
+// with a split, the merge, and counts them.
+int gqa_paged_prefill_e4m3(const void* q, void* k_cache, void* v_cache, const void* k_new, const void* v_new,
+                           int64_t k_new_sb, int64_t k_new_st, int64_t v_new_sb, int64_t v_new_st,
+                           const int32_t* cache_seqlens, const int32_t* block_table, int bt_stride, int B, int sq,
+                           int Hq, int Hkv, int page_size, int num_blocks, int max_len, int causal, float softmax_scale,
+                           void* out, void* workspace, int64_t workspace_bytes, int dtype, cudaStream_t st);
 
 // ---- GQA attention over a contiguous cache with sq > 1 (gqa_prefill.cu), the multi-token path of
 // chitu_b200_gqa_contiguous_attn, which checks the arguments.  rows_sb: the caches' batch stride in rows of Hkv * D.
@@ -202,6 +215,39 @@ __device__ __forceinline__ float fp8_to_float(uint8_t v) {
 __device__ __forceinline__ uint8_t float_to_fp8(float v) {
   return (uint8_t)__nv_cvt_float_to_fp8(v, __NV_SATFINITE, __NV_E4M3);
 }
+
+// ---- e4m3 KV cache (chitu_b200_gqa_paged_attn_fp8kv) -------------------------------------------------------------
+// Store: an io pair (element 0 in the low half) -> two e4m3 bytes (element 0 in the low byte), cvt.rn.satfinite:
+// nearest even, clamped to +-448, NaN stays NaN (torch: x.float().clamp(-448, 448).to(float8_e4m3fn)).
+template <typename T>
+__device__ __forceinline__ uint32_t io2_to_e4m3x2(uint32_t u) {
+  return (uint32_t)__nv_cvt_float2_to_fp8x2(unpack2(u, (const T*)nullptr), __NV_SATFINITE, __NV_E4M3);
+}
+// Read: four e4m3 bytes (element k in byte k) -> io pairs lo = (0, 1), hi = (2, 3), exact (every e4m3 value is a
+// bf16 and an fp16 value).  fp16: the hardware conversion.  bf16: the byte's exponent and mantissa placed in a bf16
+// whose exponent is 127 lower than e4m3's bias wants, times 2^120 (exact, subnormals included), then e4m3's NaN
+// (S.1111.111, which the scaling maps to 480) restored.
+template <typename T> struct E4m3;
+template <> struct E4m3<__half> {
+  static __device__ __forceinline__ void to_io(uint32_t w, uint32_t& lo, uint32_t& hi) {
+    const __half2_raw a = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(w & 0xffffu), __NV_E4M3);
+    const __half2_raw b = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(w >> 16), __NV_E4M3);
+    lo = *reinterpret_cast<const uint32_t*>(&a);
+    hi = *reinterpret_cast<const uint32_t*>(&b);
+  }
+};
+template <> struct E4m3<__nv_bfloat16> {
+  static __device__ __forceinline__ uint32_t pair(uint32_t x) {     // x: the two bytes in bits 8-15 and 24-31
+    const uint32_t em = x & 0x7f007f00u;
+    uint32_t r;
+    asm("mul.rn.bf16x2 %0, %1, %2;" : "=r"(r) : "r"((em >> 4) | (x & 0x80008000u)), "r"(0x7b807b80u));
+    return r | (__vcmpeq2(em, 0x7f007f00u) & 0x7fc07fc0u);
+  }
+  static __device__ __forceinline__ void to_io(uint32_t w, uint32_t& lo, uint32_t& hi) {
+    lo = pair(__byte_perm(w, 0u, 0x1404));
+    hi = pair(__byte_perm(w, 0u, 0x3424));
+  }
+};
 
 // 128-bit streaming load that does not pollute L1 (weights / KV are read exactly once).
 __device__ __forceinline__ uint4 ld_stream(const void* p) {

@@ -134,7 +134,41 @@ __global__ void __launch_bounds__(128) contiguous_append_kernel(cb::PagedAppend 
   append_rows<true>(c0, c1, row_bytes, seqlens, nullptr, 0, B, 1, 1, rows_sb, cache_rows, vec);
 }
 
+// Rows of n io elements into two e4m3 caches, 8 elements (16 bytes in, 8 out) per thread and step.
+template <typename T>
+__global__ void __launch_bounds__(128) paged_append_e4m3_kernel(cb::PagedAppend c0, cb::PagedAppend c1, int n,
+                                                                const int32_t* __restrict__ seqlens,
+                                                                const int32_t* __restrict__ block_table, int bt_stride,
+                                                                int B, int page_size) {
+  cb::pdl_prologue();
+  const int i = blockIdx.x;
+  for (int b = blockIdx.y; b < B; b += gridDim.y) {
+    const int p = seqlens[b] + i;
+    const int64_t row = (int64_t)block_table[(int64_t)b * bt_stride + p / page_size] * page_size + p % page_size;
+    for (int u = threadIdx.x; u < 2 * (n / 8); u += blockDim.x) {
+      const cb::PagedAppend& c = u < n / 8 ? c0 : c1;
+      const int e = (u < n / 8 ? u : u - n / 8) * 8;
+      const uint4 x = *reinterpret_cast<const uint4*>((const uint8_t*)c.src + b * c.src_sb + i * c.src_st + e * 2);
+      const uint2 y = make_uint2(cb::io2_to_e4m3x2<T>(x.x) | cb::io2_to_e4m3x2<T>(x.y) << 16,
+                                 cb::io2_to_e4m3x2<T>(x.z) | cb::io2_to_e4m3x2<T>(x.w) << 16);
+      *reinterpret_cast<uint2*>((uint8_t*)c.cache + row * n + e) = y;
+    }
+  }
+}
+
 namespace cb {
+void launch_paged_append_e4m3(PagedAppend c0, PagedAppend c1, int n, int dtype, const int32_t* seqlens,
+                              const int32_t* block_table, int bt_stride, int B, int sq, int page_size, cudaStream_t st) {
+  const dim3 grid(sq, B < 65535 ? B : 65535);
+  const int threads = n / 4 < 128 ? 64 : 128;
+  if (dtype == CB_BF16)
+    launch_k(paged_append_e4m3_kernel<__nv_bfloat16>, grid, dim3(threads), 0, st, c0, c1, n, seqlens, block_table,
+             bt_stride, B, page_size);
+  else
+    launch_k(paged_append_e4m3_kernel<__half>, grid, dim3(threads), 0, st, c0, c1, n, seqlens, block_table, bt_stride,
+             B, page_size);
+}
+
 // 16-byte copies when every address and stride allows them; 64 threads for rows of fewer than 128 copy units
 static int append_vec(const PagedAppend& c0, const PagedAppend& c1, int64_t row_bytes) {
   uintptr_t bits = (uintptr_t)row_bytes;

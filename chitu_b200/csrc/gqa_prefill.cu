@@ -26,6 +26,8 @@
 // Shared memory: Q 16 KB + 2 x 32 KB ring = 80 KB + 1 KB alignment.
 // Non-paged cache (chitu_b200_gqa_contiguous_attn, no block table): the same CTA compiled with a 4-D map over
 // [B, S, Hkv, 128] caches (gqa_prefill_contig_kernel); TMA zero-fills keys >= S, so any S works.
+// e4m3 cache (chitu_b200_gqa_paged_attn_fp8kv, gqa_prefill_e4m3_kernel): UINT8 maps, one [64 keys x 128 B] box per K and
+// per V tile in a 2-stage ring, converted by the warpgroup into one io-dtype stage; the same 80 KB of shared memory.
 // Split over keys when (row tiles x Hkv x B) CTAs cannot fill the GPU: split s of a CTA takes an equal share of the
 // CTA's key tiles and writes normalised fp32 partials + LSE to the workspace as [B, sq * Hq, S, 128] (the decode
 // layout with H = sq * Hq), merged by attention.cu's merge_splits_kernel.  Deterministic: the split count depends on
@@ -101,7 +103,11 @@ __device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* m
 // CONTIG: the maps are 4-D over a contiguous cache, (128, Hkv, cache_rows, B) with the cache's batch stride, and key
 // tile t of request b is the box at (c, kvh, 64 t, b).  Rows at or past cache_rows are zero-filled by TMA, so no box
 // reads another request's rows; block_table, bt_stride and page are unused.
-template <typename T, int G, bool CONTIG>
+// C: the cache element, T or uint8_t (e4m3, paged only).  With e4m3 the maps are UINT8 (128 B = 128 dims, 1, keys) and
+// a tile is one [64 keys x 128 B] K box and one V box in a 2-stage e4m3 ring behind a single io-dtype stage: the
+// warpgroup converts each box into the two 64-dim io chunks the wgmmas read (V rows of keys >= Lk become 0 there), so
+// shared memory stays at kSmemBytes.
+template <typename T, typename C, int G, bool CONTIG>
 __device__ __forceinline__ void gqa_prefill_cta(
     const CUtensorMap& map_k, const CUtensorMap& map_v, const T* __restrict__ q,
     const int32_t* __restrict__ cache_seqlens, const int32_t* __restrict__ block_table, int bt_stride, int sq, int Hq,
@@ -111,6 +117,10 @@ __device__ __forceinline__ void gqa_prefill_cta(
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(gqa_prefill_smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* s_q = smem;                                      // [2][64 rows][128 B]
   uint8_t* s_ring = s_q + kQBytes;                          // [kStages][K0 K1 V0 V1][64 keys][128 B]; output staging
+  constexpr bool kE4m3 = sizeof(C) == 1;
+  static_assert(!(kE4m3 && CONTIG), "the e4m3 cache is paged");
+  static_assert(kStageBytes + kStages * 2 * kSlot == kStages * kStageBytes, "e4m3: one io stage + the e4m3 ring");
+  uint8_t* s_e4m3 = s_ring + kStageBytes;                   // e4m3: [kStages][K V][64 keys][128 B]
   __shared__ __align__(8) uint64_t kfull[kStages], vfull[kStages];
   __shared__ float s_lse[kRows];                            // row LSE (log2 domain) for the split partials
 
@@ -146,6 +156,14 @@ __device__ __forceinline__ void gqa_prefill_cta(
       return;
     }
     const int prow = block_table[(int64_t)b * bt_stride + key0 / page] * page + key0 % page;
+    if constexpr (kE4m3) {
+      uint8_t* dst = s_e4m3 + slot * 2 * kSlot;
+      mbar_expect_tx(&kfull[slot], kSlot);
+      tma_load_3d(dst, &map_k, &kfull[slot], 0, kvh, prow, pol_kv);
+      mbar_expect_tx(&vfull[slot], kSlot);
+      tma_load_3d(dst + kSlot, &map_v, &vfull[slot], 0, kvh, prow, pol_kv);
+      return;
+    }
     uint8_t* dst = s_ring + slot * kStageBytes;
     mbar_expect_tx(&kfull[slot], 2 * kSlot);
     tma_load_3d(dst, &map_k, &kfull[slot], 0, kvh, prow, pol_kv);
@@ -187,14 +205,36 @@ __device__ __forceinline__ void gqa_prefill_cta(
   float m_run[2] = {-INFINITY, -INFINITY};                  // running row max (log2 domain), the same in a lane quad
   float l_run[2] = {0.f, 0.f};                              // this thread's share of the row sums
 
+  // e4m3: one [64 keys x 128 B] box (16-byte unit c = dims 16c .. 16c+15) -> units 2c, 2c+1 of io chunk c / 4; rows at
+  // or past `valid` are written as 0
+  auto e4m3_to_io = [&](const uint8_t* src, uint8_t* dst, int valid) {
+    for (int u = threadIdx.x; u < kTile * 8; u += kThreads) {
+      const int r = u >> 3, c = u & 7;
+      uint4 lo = make_uint4(0, 0, 0, 0), hi = make_uint4(0, 0, 0, 0);
+      if (r < valid) {
+        const uint4 w = *reinterpret_cast<const uint4*>(src + sw128(r, c));
+        E4m3<T>::to_io(w.x, lo.x, lo.y);
+        E4m3<T>::to_io(w.y, lo.z, lo.w);
+        E4m3<T>::to_io(w.z, hi.x, hi.y);
+        E4m3<T>::to_io(w.w, hi.z, hi.w);
+      }
+      uint8_t* d = dst + (c >> 2) * kSlot;
+      *reinterpret_cast<uint4*>(d + sw128(r, (2 * c) & 7)) = lo;
+      *reinterpret_cast<uint4*>(d + sw128(r, (2 * c + 1) & 7)) = hi;
+    }
+    fence_async_smem();
+    __syncthreads();
+  };
+
   const float sc = scale * kLog2e;
   for (int t = t_begin; t < t_end; ++t) {
     const int slot = (t - t_begin) % kStages;
     const uint32_t ph = ((t - t_begin) / kStages) & 1;
-    const uint32_t st_a = ring_a + slot * kStageBytes;
+    const uint32_t st_a = ring_a + (kE4m3 ? 0 : slot) * kStageBytes;
     // ---- S = Q . K^T over the 2 chunks of 64 dims ----
     float s[32];
     mbar_wait(&kfull[slot], ph);
+    if constexpr (kE4m3) e4m3_to_io(s_e4m3 + slot * 2 * kSlot, s_ring, kTile);
     wgmma_fence();
 #pragma unroll
     for (int c = 0; c < 2; ++c)
@@ -243,25 +283,31 @@ __device__ __forceinline__ void gqa_prefill_cta(
       }
     }
     // ---- V rows of keys past the sequence (unwritten slots, possibly NaN) -> 0 before P.V reads them ----
-    if (key0 + kTile > Lk) {
+    if constexpr (kE4m3) {
       mbar_wait(&vfull[slot], ph);
-      uint4* v0 = reinterpret_cast<uint4*>(s_ring + slot * kStageBytes + 2 * kSlot);
-      for (int u = threadIdx.x; u < 2 * kTile * 8; u += kThreads) {
-        const int c = u / (kTile * 8), key = (u / 8) % kTile;
-        if (key0 + key >= Lk) v0[c * (kSlot / 16) + key * 8 + (u & 7)] = make_uint4(0, 0, 0, 0);
+      e4m3_to_io(s_e4m3 + slot * 2 * kSlot + kSlot, s_ring + 2 * kSlot, Lk - key0);
+      if (threadIdx.x == 0 && t + kStages < t_end) load_tile(t + kStages);     // both boxes of the slot are converted
+    } else {
+      if (key0 + kTile > Lk) {
+        mbar_wait(&vfull[slot], ph);
+        uint4* v0 = reinterpret_cast<uint4*>(s_ring + slot * kStageBytes + 2 * kSlot);
+        for (int u = threadIdx.x; u < 2 * kTile * 8; u += kThreads) {
+          const int c = u / (kTile * 8), key = (u / 8) % kTile;
+          if (key0 + key >= Lk) v0[c * (kSlot / 16) + key * 8 + (u & 7)] = make_uint4(0, 0, 0, 0);
+        }
+        fence_async_smem();
+        __syncthreads();
       }
-      fence_async_smem();
-      __syncthreads();
+      mbar_wait(&vfull[slot], ph);
     }
     // ---- O += P . V: 4 steps of 16 keys, N = 128 dims over the two V chunks (64-dim blocks kSlot apart) ----
-    mbar_wait(&vfull[slot], ph);
     wgmma_fence();
 #pragma unroll
     for (int ks = 0; ks < 4; ++ks) Mma<T>::pv(o, pa[ks], make_sw128_desc(st_a + 2 * kSlot + ks * 2048, kSlot, 1024));
     wgmma_commit();
     wgmma_wait<0>();
     __syncthreads();                                        // the slot is free
-    if (threadIdx.x == 0 && t + kStages < t_end) load_tile(t + kStages);
+    if (!kE4m3 && threadIdx.x == 0 && t + kStages < t_end) load_tile(t + kStages);
   }
 
   // ---- epilogue: row sums over the lane quad, O / l staged as fp32 rows in the ring -> coalesced stores ----
@@ -306,8 +352,18 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) gqa_prefill_kernel(
     const int32_t* __restrict__ cache_seqlens, const int32_t* __restrict__ block_table, int bt_stride, int sq, int Hq,
     int Hkv, int page, int appended, int causal, float scale, int row_tiles, int splits, float* __restrict__ o_part,
     float* __restrict__ lse, T* __restrict__ out) {
-  gqa_prefill_cta<T, G, false>(map_k, map_v, q, cache_seqlens, block_table, bt_stride, sq, Hq, Hkv, page, appended,
-                               causal, scale, row_tiles, splits, o_part, lse, out);
+  gqa_prefill_cta<T, T, G, false>(map_k, map_v, q, cache_seqlens, block_table, bt_stride, sq, Hq, Hkv, page, appended,
+                                  causal, scale, row_tiles, splits, o_part, lse, out);
+}
+
+template <typename T, int G>
+__global__ void __launch_bounds__(kThreads, kCtasPerSm) gqa_prefill_e4m3_kernel(
+    const __grid_constant__ CUtensorMap map_k, const __grid_constant__ CUtensorMap map_v, const T* __restrict__ q,
+    const int32_t* __restrict__ cache_seqlens, const int32_t* __restrict__ block_table, int bt_stride, int sq, int Hq,
+    int Hkv, int page, int appended, int causal, float scale, int row_tiles, int splits, float* __restrict__ o_part,
+    float* __restrict__ lse, T* __restrict__ out) {
+  gqa_prefill_cta<T, uint8_t, G, false>(map_k, map_v, q, cache_seqlens, block_table, bt_stride, sq, Hq, Hkv, page,
+                                        appended, causal, scale, row_tiles, splits, o_part, lse, out);
 }
 
 template <typename T, int G>
@@ -315,8 +371,8 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) gqa_prefill_contig_kerne
     const __grid_constant__ CUtensorMap map_k, const __grid_constant__ CUtensorMap map_v, const T* __restrict__ q,
     const int32_t* __restrict__ cache_seqlens, int sq, int Hq, int Hkv, int appended, int causal, float scale,
     int row_tiles, int splits, float* __restrict__ o_part, float* __restrict__ lse, T* __restrict__ out) {
-  gqa_prefill_cta<T, G, true>(map_k, map_v, q, cache_seqlens, nullptr, 0, sq, Hq, Hkv, kTile, appended, causal, scale,
-                              row_tiles, splits, o_part, lse, out);
+  gqa_prefill_cta<T, T, G, true>(map_k, map_v, q, cache_seqlens, nullptr, 0, sq, Hq, Hkv, kTile, appended, causal,
+                                 scale, row_tiles, splits, o_part, lse, out);
 }
 
 // splits of the multi-token kernel: the decode kernels' wave rule on its CTAs, shrunk to the workspace (none: 1 split)
@@ -373,6 +429,68 @@ int gqa_contiguous_prefill(const void* q, void* k_cache, void* v_cache, int64_t 
     }                                                                                                             \
     launch_k(gqa_prefill_contig_kernel<T, GG>, grid, dim3(kThreads), smem, st, mk, mv, (const T*)q, cache_seqlens, \
              sq, Hq, Hkv, k_new ? 1 : 0, causal ? 1 : 0, softmax_scale, row_tiles, splits, o_part, lse, (T*)out);  \
+  } while (0)
+#define DISPATCH_PREFILL(T)                \
+  switch (G) {                             \
+    case 1: LAUNCH_PREFILL(T, 1); break;   \
+    case 2: LAUNCH_PREFILL(T, 2); break;   \
+    case 4: LAUNCH_PREFILL(T, 4); break;   \
+    default: LAUNCH_PREFILL(T, 8); break;  \
+  }
+  if (dtype == CB_BF16) { DISPATCH_PREFILL(__nv_bfloat16); } else { DISPATCH_PREFILL(__half); }
+#undef DISPATCH_PREFILL
+#undef LAUNCH_PREFILL
+  CB_LAUNCHED(1);
+  if (splits > 1) {
+    rc = launch_merge_splits(o_part, lse, out, B * sq * Hq, splits, kD, dtype, st);
+    if (rc) return rc;
+    CB_LAUNCHED(1);
+  }
+  return 0;
+}
+
+// The multi-token path of chitu_b200_gqa_paged_attn_fp8kv (attention.cu), which has checked the arguments.
+int gqa_paged_prefill_e4m3(const void* q, void* k_cache, void* v_cache, const void* k_new, const void* v_new,
+                           int64_t k_new_sb, int64_t k_new_st, int64_t v_new_sb, int64_t v_new_st,
+                           const int32_t* cache_seqlens, const int32_t* block_table, int bt_stride, int B, int sq,
+                           int Hq, int Hkv, int page_size, int num_blocks, int max_len, int causal, float softmax_scale,
+                           void* out, void* workspace, int64_t workspace_bytes, int dtype, cudaStream_t st) {
+  if (!tma_available()) return fail(-3, "gqa_paged_attn_fp8kv: TMA is not available");
+  const int G = Hq / Hkv;
+  const int row_tiles = cdiv((int64_t)sq * G, kRows);
+  const int64_t rows = (int64_t)B * sq * Hq;
+  const int splits = prefill_splits(row_tiles, Hkv, B, rows, max_len, workspace, workspace_bytes);
+  if ((int64_t)row_tiles * splits > INT_MAX)
+    return fail(-1, "gqa_paged_attn_fp8kv: %d row tiles x %d splits exceed the grid", row_tiles, splits);
+  const auto [o_part, lse, plan] = split_kv_carve(splits > 1 ? workspace : nullptr, workspace_bytes, rows, kD, splits);
+
+  // the caches as bytes (128, Hkv, num_blocks * page): a box (128, 1, 64) is 64 keys x 128 dims of one head in one page
+  CUtensorMap mk, mv;
+  const cuuint64_t dims[3] = {(cuuint64_t)kD, (cuuint64_t)Hkv, (cuuint64_t)num_blocks * page_size};
+  const cuuint64_t strides[2] = {(cuuint64_t)kD, (cuuint64_t)Hkv * kD};
+  int rc = make_tma_map_nd(&mk, k_cache, 3, dims, strides, 1, CU_TENSOR_MAP_DATA_TYPE_UINT8, kTile);
+  if (!rc) rc = make_tma_map_nd(&mv, v_cache, 3, dims, strides, 1, CU_TENSOR_MAP_DATA_TYPE_UINT8, kTile);
+  if (rc) return rc;
+
+  if (k_new) {                                              // the sq new k / v rows first, rounded to e4m3
+    launch_paged_append_e4m3({k_cache, k_new, k_new_sb * 2, k_new_st * 2}, {v_cache, v_new, v_new_sb * 2, v_new_st * 2},
+                             Hkv * kD, dtype, cache_seqlens, block_table, bt_stride, B, sq, page_size, st);
+    CB_LAUNCHED(1);
+  }
+
+  const size_t smem = 1024 + (size_t)kSmemBytes;
+  const dim3 grid(row_tiles * splits, Hkv, B);
+#define LAUNCH_PREFILL(T, GG)                                                                                     \
+  do {                                                                                                            \
+    static bool attr = false;                                                                                     \
+    if (!attr) {                                                                                                  \
+      CB_CUDA(cudaFuncSetAttribute(gqa_prefill_e4m3_kernel<T, GG>, cudaFuncAttributeMaxDynamicSharedMemorySize,   \
+                                   (int)smem));                                                                   \
+      attr = true;                                                                                                \
+    }                                                                                                             \
+    launch_k(gqa_prefill_e4m3_kernel<T, GG>, grid, dim3(kThreads), smem, st, mk, mv, (const T*)q, cache_seqlens,  \
+             block_table, bt_stride, sq, Hq, Hkv, page_size, k_new ? 1 : 0, causal ? 1 : 0, softmax_scale,        \
+             row_tiles, splits, o_part, lse, (T*)out);                                                            \
   } while (0)
 #define DISPATCH_PREFILL(T)                \
   switch (G) {                             \

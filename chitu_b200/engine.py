@@ -127,7 +127,11 @@ class DecodeEngine:
         self.seq_lens.fill_(seq_len)
         for l in range(self.cfg.n_layers):
             for cache in self.caches:
-                cache[l].normal_(0, 1, generator=gd)
+                if cache.dtype == torch.float8_e4m3fn:        # normal_ is not defined for fp8: draw, clamp, cast
+                    x = torch.empty(cache[l].shape, dtype=torch.float32, device=self.device).normal_(0, 1, generator=gd)
+                    cache[l].copy_(x.clamp_(-448.0, 448.0))
+                else:
+                    cache[l].normal_(0, 1, generator=gd)
 
     # ---- one decode step ---------------------------------------------------------------------------
     def _linear(self, x, w, y, M, residual=None):
@@ -233,11 +237,12 @@ class LlamaDecodeEngine(DecodeEngine):
     """Single-GPU (tp=1) or tensor-parallel LLaMA decode.  Weights are random (`do_load=False`,
     serve_config.yaml:9).  KV cache layout = PagedKVCacheManager (cache_manager.py:71-87):
     paged_k_cache / paged_v_cache [L, num_blocks, page, n_local_kv_heads, head_dim], page 256
-    (backend.py:237)."""
+    (backend.py:237).  kv_dtype=torch.float8_e4m3fn keeps the caches in e4m3 (half the KV bytes; new rows rounded
+    to nearest even after a clamp to +-448, no scale) and decodes through chitu_b200_gqa_paged_attn_fp8kv."""
 
     def __init__(self, cfg: LlamaConfig, max_reqs: int, max_seq_len: int, device="cuda:0", page_size: int = 256,
                  seed: int = 0, tp_rank: int = 0, tp_size: int = 1, process_group=None, linear_impl: int = 0,
-                 use_fused_allreduce: bool = True):
+                 use_fused_allreduce: bool = True, kv_dtype: torch.dtype = BF):
         D = cfg.head_dim
         assert cfg.n_heads % tp_size == 0 and cfg.n_kv_heads % tp_size == 0
         self.Hq, self.Hkv, self.D = cfg.n_heads // tp_size, cfg.n_kv_heads // tp_size, D
@@ -266,7 +271,10 @@ class LlamaDecodeEngine(DecodeEngine):
         self.norm = torch.ones(dim, dtype=BF, device=dev)
         self.head = rnd(cfg.vocab_size // tp_size, dim)
         nblk = self.max_blocks * max_reqs
-        self.k_cache = torch.zeros(cfg.n_layers, nblk, page_size, self.Hkv, D, dtype=BF, device=dev)
+        if kv_dtype not in (BF, torch.float8_e4m3fn):
+            raise ValueError(f"kv_dtype must be torch.bfloat16 or torch.float8_e4m3fn, not {kv_dtype}")
+        self.kv_fp8 = kv_dtype == torch.float8_e4m3fn
+        self.k_cache = torch.zeros(cfg.n_layers, nblk, page_size, self.Hkv, D, dtype=kv_dtype, device=dev)
         self.v_cache = torch.zeros_like(self.k_cache)
         self.caches = (self.k_cache, self.v_cache)
         # precompute_freqs_cis (models/model.py:81-89) as cos/sin tables
@@ -289,6 +297,9 @@ class LlamaDecodeEngine(DecodeEngine):
                 lw["w13"] = lw["w13"].view(2, self.F, dim).transpose(0, 1).reshape(2 * self.F, dim).contiguous()
         # rotary fused into the tensor-core decode kernel (head dim 128, power-of-two pages)
         self.fuse_rope = D == 128 and (page_size & (page_size - 1)) == 0 and self.Hq // self.Hkv in (1, 2, 4, 8)
+        if self.kv_fp8 and not (self.fuse_rope and page_size % 64 == 0):
+            raise ValueError("the fp8 KV cache needs head dim 128, Hq / Hkv in {1, 2, 4, 8} and a power-of-two page "
+                             "that is a multiple of 64")
 
     def ref_layers(self):
         """The layer weights in the REFERENCE's layout (w13 = [w1 ; w3] halves) for the oracle side of the tests."""
@@ -312,7 +323,14 @@ class LlamaDecodeEngine(DecodeEngine):
             self._linear(self.xn, lw["wqkv"], self.qkv, B)
             q_view, k_view = self.qkv, self.qkv[:, self.Hq * D:]
             v_view = self.qkv[:, (self.Hq + self.Hkv) * D:]
-            if self.fuse_rope:
+            if self.kv_fp8:
+                # the same fused rotary over the e4m3 caches; the new k / v rows are rounded to e4m3 as they are stored
+                check(lib.chitu_b200_gqa_paged_attn_fp8kv(
+                    ptr(q_view), qkv_w, ptr(self.k_cache[li]), ptr(self.v_cache[li]), ptr(k_view), ptr(v_view), qkv_w, 0,
+                    qkv_w, 0, ptr(self.cos), ptr(self.sin), ptr(self.seq_lens), ptr(self.block_table), self.max_blocks, B,
+                    1, self.Hq, self.Hkv, D, self.page, self.k_cache.shape[1], self.max_seq_len, 1, 1.0 / math.sqrt(D),
+                    ptr(self.attn_out), ptr(self.attn_ws), self.attn_ws.numel(), _lib.CB_BF16, st), "gqa_paged_attn_fp8kv")
+            elif self.fuse_rope:
                 # rotary (q and the new k) inside the attention kernel: q / k / v are views of the qkv GEMM output
                 check(lib.chitu_b200_gqa_paged_decode_rope(
                     ptr(q_view), qkv_w, ptr(self.k_cache[li]), ptr(self.v_cache[li]), ptr(k_view), ptr(v_view), qkv_w, qkv_w,

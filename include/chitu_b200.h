@@ -232,6 +232,31 @@ int chitu_b200_gqa_contiguous_attn(const void* q, void* k_cache, void* v_cache, 
                                    int Hq, int Hkv, int D, int max_seqlen_hint, int causal, float softmax_scale,
                                    void* out, void* workspace, int64_t workspace_bytes, int dtype, void* stream);
 
+/* AttnBackend.attn_with_kvcache with block_table over an fp8 (e4m3fn) paged cache, seqlen_q = sq >= 1: the
+ * arguments and semantics of chitu_b200_gqa_paged_prefill with k_cache / v_cache [num_blocks, page_size, Hkv, D] of
+ * e4m3 bytes and q / k_new / v_new / out in the io dtype (bf16 | fp16), with these differences:
+ *  - Store: a new k / v element x is written as e4m3(clamp(x, -448, 448)), rounded to nearest even; NaN stays NaN
+ *    (torch: x.float().clamp(-448, 448).to(float8_e4m3fn)).  No scale (a per-tensor scale of 1).
+ *  - Read: a cache element is decoded to the io dtype exactly; the arithmetic is then the io-dtype cache's (fp32 scores
+ *    and softmax, P rounded to the io dtype before P.V, bottom-right causal mask, 0 for a row that sees no key).  The
+ *    rows appended by the call are attended in their stored form, so sq = n agrees with n successive decodes.
+ *  - q [B, sq, Hq, D] with batch stride q_sb elements: any multiple of 8 >= Hq * D for sq == 1 (a view of a fused qkv
+ *    GEMM output), sq * Hq * D for sq > 1.
+ *  - rope_cos / rope_sin (fp32 [B, D / 2], both or neither, sq == 1 only): the rotary of
+ *    chitu_b200_gqa_paged_decode_rope on q and the new k, which is rotated and rounded to the io dtype before it is
+ *    stored as above.
+ *  - k / v strides: multiples of 8 elements (the token strides are unused for sq == 1).
+ * sq == 1 runs the tensor-core decode kernel, sq > 1 the multi-token kernel after an append; the splits and the
+ * workspace are those of the io-dtype entries -> no host synchronisation, capturable in a CUDA graph, deterministic.
+ * Built for D == 128, Hq / Hkv in {1, 2, 4, 8}, page_size a power of two and a multiple of 64, bf16 | fp16 io,
+ * 16-byte aligned bases.  Anything else returns a negative status before any launch.  B == 0 launches nothing. */
+int chitu_b200_gqa_paged_attn_fp8kv(const void* q, int64_t q_sb, void* k_cache, void* v_cache, const void* k_new,
+                                    const void* v_new, int64_t k_new_sb, int64_t k_new_st, int64_t v_new_sb,
+                                    int64_t v_new_st, const float* rope_cos, const float* rope_sin,
+                                    const int32_t* cache_seqlens, const int32_t* block_table, int bt_stride, int B,
+                                    int sq, int Hq, int Hkv, int D, int page_size, int num_blocks, int max_seqlen_hint,
+                                    int causal, float softmax_scale, void* out, void* workspace,
+                                    int64_t workspace_bytes, int dtype, void* stream);
 
 /* *.mla_attn_with_kvcache (attn_backend.py:536-572 / 660-684 / 707-774) = append
  * (ops.py:50-91) + mla_decode (triton_decode_attention.py:259-290) in one call.
