@@ -505,11 +505,16 @@ extern "C" int chitu_b200_quant_act_int8(const void* x, int8_t* q, float* scales
 
 // ============================================================================================
 // fp8 weight dequant (ops.py:356-449, triton_kernels.py:217-287) -> bf16
+//
+// Its output is a GEMM weight, and the decode GEMM streams its first weight stages before its own
+// griddepcontrol.wait.  So this kernel does not trigger its dependents early (no griddepcontrol.launch_dependents):
+// whatever is launched after it starts once every block has written its rows.
 // ============================================================================================
 __global__ void weight_dequant_fp8_kernel(const uint8_t* __restrict__ x, const float* __restrict__ s,
                                           __nv_bfloat16* __restrict__ y, int M, int N, int block,
                                           int soft) {
-  cb::pdl_prologue();
+  cb::pdl_wait();
+  cb::tl_stamp();
   const int b = blockIdx.z;
   const int m = blockIdx.y;
   const int sn = (N + block - 1) / block, sm = (M + block - 1) / block;

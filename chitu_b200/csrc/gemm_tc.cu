@@ -209,10 +209,10 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
   }
   pdl_launch_dependents();
   __syncthreads();
-  // everything above (barrier init, tensormap prefetch) overlapped the previous kernel's tail.  The WEIGHTS are never
-  // written by a preceding kernel, so the producer also starts streaming them now — up to the whole ring (10 x 16 KB per
-  // SM) is in flight or landed before the activations exist; everything else waits here for the previous kernel to
-  // complete and flush.
+  // everything above (barrier init, tensormap prefetch) overlapped the previous kernel's tail.  The WEIGHTS are written
+  // only by kernels that do not trigger dependents early (torch copies, chitu_b200_weight_dequant_fp8), so the producer
+  // also starts streaming them now — up to the whole ring (10 x 16 KB per SM) is in flight or landed before the
+  // activations exist; everything else waits here for the previous kernel to complete and flush.
   if (warp == C::kProducerWarp) {
     // ================= TMA producer =================
     if (elect_one()) {

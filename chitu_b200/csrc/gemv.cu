@@ -1,11 +1,12 @@
-// SIMT weight-streaming skinny GEMM ("GEMV" path): y[M,N] = x[M,K] · W[N,K]^T for M <= 16.
+// SIMT weight-streaming skinny GEMM ("GEMV" path): y[M,N] = x[M,K] · W[N,K]^T, M in chunks of <= 16.
 //
 // Decode linears are HBM-bound weight streams (SURVEY §7.3-1): each warp owns two weight rows,
 // the 32 lanes stride K with 128-bit `ld.global.nc.L1::no_allocate` loads (each weight byte is
 // read exactly once from HBM), activations are re-read through L1 (they are tiny), fp32
-// accumulation, butterfly reduce.  This path is the small-M / any-shape implementation; the
-// wgmma + TMA swap-AB kernel in gemm_tc.cu is the tensor-core implementation of the same
-// entry points (impl = 2) and the default for M > 2.
+// accumulation, butterfly reduce.  This path is impl = 1 and the fall-back for shapes TMA cannot
+// address; the wgmma + TMA swap-AB kernel in gemm_tc.cu is the tensor-core implementation of the
+// same entry points (impl = 2) and the default whenever it supports the shape and the workspace
+// is large enough (linear.cu use_tc()).
 #include "common.cuh"
 #include "gemm.cuh"
 

@@ -124,7 +124,8 @@ int chitu_b200_quant_act_int8(const void* x, int8_t* q, float* scales, int64_t r
                               int dtype, void* stream);
 /* weight_dequant_deepseek_v3 / weight_dequant_soft_fp8_deepseek_v3 (ops.py:356-449):
  * y[b,m,n] = fp8(x[b,m,n]) * s[b, m/128, n/128]  -> bf16.  soft != 0 reproduces the
- * bit-trick path ((x&0x80)<<24 | (x&0x7f)<<20) * (s * 2^120). */
+ * bit-trick path ((x&0x80)<<24 | (x&0x7f)<<20) * (s * 2^120).  The kernel does not let the next kernel of the stream
+ * start before it has finished, so a linear launched right after it may read y as its weight. */
 int chitu_b200_weight_dequant_fp8(const void* x, const float* s, void* y, int B, int M, int N,
                                   int block, int soft, void* stream);
 
@@ -132,7 +133,11 @@ int chitu_b200_weight_dequant_fp8(const void* x, const float* s, void* y, int B,
 /* Workspace for split-K partials + ticket counters: chitu_b200_linear_workspace_bytes(M_max, N_max).
  * It must be zero-filled ONCE before its first use; every call leaves the counters at zero again. */
 int64_t chitu_b200_linear_workspace_bytes(int M, int N);
-/* impl: 0 = auto, 1 = SIMT weight-streaming GEMV, 2 = wgmma/TMA swap-AB GEMM. */
+/* impl: 0 = auto, 1 = SIMT weight-streaming GEMV, 2 = wgmma/TMA swap-AB GEMM.
+ * Weight contract: the wgmma GEMM starts streaming its weights while the previous kernel of the stream is still running
+ * (before griddepcontrol.wait).  A weight must therefore be written by host copies, torch kernels or
+ * chitu_b200_weight_dequant_fp8, never by a kernel that triggers its dependents early (griddepcontrol.launch_dependents)
+ * directly before the linear. */
 /* F.linear for bf16/fp16 weights (linear_deepseek_v3 element_size()>1 branch,
  * model_deepseek_v3.py:84-85; tensor_parallel.py linear_op default). y = x W^T (+bias) (+residual). */
 int chitu_b200_linear_bf16(const void* x, const void* w, const void* bias, const void* residual,
