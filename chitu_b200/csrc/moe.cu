@@ -268,7 +268,8 @@ __device__ __forceinline__ void moe_plan_small(const IdT* ids, const void* topk_
 // gate: one CTA (256 threads) per token.
 // dtype pipeline reproduced from the reference (x, W bf16):
 //   logits = bf16(F.linear)                       -> sigmoid -> bf16  (original_scores)
-//   scores = original + bias  (bf16 if bias is bf16, fp32 if bias is fp32: torch promotion)
+//   scores = original + bias  (bf16 if bias is bf16, fp32 if bias is fp32: torch promotion; softmax scores are fp32, so
+//                              any bias is an fp32 add there)
 //   group score = sum of top-2 (in that dtype), keep top `topk_groups` groups, others * 0
 //   indices = top-k of masked scores (ties -> lowest index), weights = original.gather,
 //   /= sum (bf16), *= route_scale (bf16).
@@ -427,17 +428,19 @@ __global__ void __launch_bounds__(256) moe_gate_kernel(
     for (int e = tid; e < E; e += 256) s_orig[e] = s_orig[e] / sum;
   }
   __syncthreads();
+  const bool low_prec = score_sigmoid == 1 && !(bias && bias_is_f32);   // score dtype is bf16
   for (int e = tid; e < E; e += 256) {
     float v = s_orig[e];
     if (bias) {
-      if (bias_is_f32) v = v + reinterpret_cast<const float*>(bias)[e];
-      else v = round_bf16(v + __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(bias)[e]));
+      // bf16 scores + bf16 bias is a bf16 add; softmax scores are fp32, so a bf16 bias promotes to an fp32 add
+      const float b = bias_is_f32 ? reinterpret_cast<const float*>(bias)[e]
+                                  : __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(bias)[e]);
+      v = low_prec ? round_bf16(v + b) : v + b;
     }
     s_score[e] = v;
   }
   __syncthreads();
 
-  const bool low_prec = score_sigmoid == 1 && !(bias && bias_is_f32);   // score dtype is bf16
   if (n_groups > 1) {
     const int gs = E / n_groups;
     for (int g = warp; g < n_groups; g += 8) {
@@ -949,7 +952,8 @@ extern "C" int chitu_b200_moe_grouped_gemm(const void* A, const void* B, void* C
   CB_ARG(A && B && C && sorted_token_ids && expert_ids && num_tokens_post_padded && workspace);
   CB_ARG(EM >= 0 && numel >= 0 && top_k >= 1 && E > 0 && N > 0 && K > 0 && wmode >= 0 && wmode <= 2);
   CB_ARG(block_m == 16 || block_m == 32 || block_m == 64 || block_m == 128);
-  CB_ARG(N % 128 == 0 && K % 16 == 0 && (wmode == 0 || (K % 128 == 0 && B_scale)));
+  // moe_rows_gather_kernel copies / quantises whole 128-column groups of A
+  CB_ARG(N % 128 == 0 && K % 128 == 0 && (wmode == 0 || B_scale));
   EM -= EM % block_m;     // num_tokens_post_padded is a multiple of block_m, so whole blocks cover every valid entry
   CB_ARG(!mul_routed_weight || topk_weights);
   CB_ARG(topk_w_dtype == CB_BF16 || topk_w_dtype == CB_F32);

@@ -97,7 +97,9 @@ def invoke_fused_moe_kernel(A: torch.Tensor, B: torch.Tensor, C: torch.Tensor, A
                             soft_fp8: bool = False) -> None:
     """fused_moe.py:796-891 — same signature, writes C in place.  One grouped wgmma GEMM over the blocks that
     `moe_align_block_size(topk_ids, config["BLOCK_SIZE_M"], E)` produced (BLOCK_SIZE_M in {16, 32, 64, 128}; the Triton
-    tiling keys BLOCK_SIZE_N / K / GROUP_SIZE_M have no meaning here and are ignored)."""
+    tiling keys BLOCK_SIZE_N / K / GROUP_SIZE_M have no meaning here and are ignored).  Unlike the Triton kernel, it needs
+    N and K to be multiples of 128, as they are in every reference model: the A rows are gathered and quantised in
+    128-column groups.  Other shapes raise RuntimeError."""
     if use_int8_w8a16 or use_int4_w4a16 or B_zp is not None:
         raise NotImplementedError("int8_w8a16 / int4_w4a16 expert weights are outside the hot path of this library")
     assert topk_weights.stride(1) == 1

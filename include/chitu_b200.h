@@ -315,7 +315,8 @@ int chitu_b200_mla_paged_prefill(const void* q_nope, const void* q_pe, void* kv_
  * B_scale [E, N/128, K/128] for wmode 1 = fp8_w8a8 — A is quantised per_token_group_quant_fp8 inside, as the reference
  * does at :826 — and wmode 2 = soft_fp8); C bf16 = C.view(-1, N) with `numel` rows; sorted_token_ids int32 [EM],
  * expert_ids int32 [EM / block_m], num_tokens_post_padded int32 [1] = the outputs of moe_align_block_size with
- * block_size = block_m (16 / 32 / 64 / 128); topk_weights flat [numel] (bf16 or fp32), applied when mul_routed_weight. */
+ * block_size = block_m (16 / 32 / 64 / 128); topk_weights flat [numel] (bf16 or fp32), applied when mul_routed_weight.
+ * N and K are multiples of 128 for every wmode. */
 int64_t chitu_b200_moe_grouped_gemm_workspace_bytes(int EM, int N, int K);
 int chitu_b200_moe_grouped_gemm(const void* A, const void* B, void* C, const float* B_scale, const void* topk_weights,
                                 int topk_w_dtype, const int32_t* sorted_token_ids, const int32_t* expert_ids,
