@@ -705,7 +705,11 @@ extern "C" int chitu_b200_gqa_paged_decode_rope(const void* q, int64_t q_sb, voi
   CB_ARG((k_new == nullptr) == (v_new == nullptr));
   CB_ARG(B >= 0 && Hq > 0 && Hkv > 0 && Hq % Hkv == 0 && page_size > 0 && bt_stride > 0);
   CB_ARG(D == 64 || D == 128);
-  CB_ARG(k_new == nullptr || (k_new_sb % 4 == 0 && v_new_sb % 4 == 0));
+  // the tensor-core kernel stages the appended row with 16-byte cp.async from k_new + b * k_new_sb: 8-element strides
+  // and 16-byte aligned operands, as the fp8 entry requires
+  CB_ARG(k_new == nullptr || (k_new_sb % 8 == 0 && v_new_sb % 8 == 0));
+  CB_ARG(((uintptr_t)q | (uintptr_t)k_cache | (uintptr_t)v_cache | (uintptr_t)out | (uintptr_t)k_new |
+          (uintptr_t)v_new) % 16 == 0);
   CB_ARG(dtype == CB_BF16 || dtype == CB_F16);
   if (B == 0) return 0;
   const int G = Hq / Hkv;
@@ -795,8 +799,10 @@ extern "C" int chitu_b200_gqa_contiguous_attn(const void* q, void* k_cache, void
   CB_ARG(cache_rows >= 1 && cache_sb >= cache_rows * row && cache_sb % row == 0 && cache_sb % 8 == 0);
   CB_ARG(((uintptr_t)q | (uintptr_t)k_cache | (uintptr_t)v_cache | (uintptr_t)out | (uintptr_t)k_new |
           (uintptr_t)v_new) % 16 == 0);
-  const int sa = sq == 1 ? 4 : 8;                           // k / v stride multiple: the decode kernels load 8 bytes
-  CB_ARG(k_new == nullptr || (k_new_sb % sa == 0 && k_new_st % sa == 0 && v_new_sb % sa == 0 && v_new_st % sa == 0));
+  // k / v strides in multiples of 8 elements: the tensor-core decode kernel (D = 128) and the multi-token kernel stage
+  // the new rows with 16-byte cp.async (sq == 1 reads only the batch strides)
+  CB_ARG(k_new == nullptr || (k_new_sb % 8 == 0 && v_new_sb % 8 == 0 && (sq == 1 || (k_new_st % 8 == 0 &&
+                                                                                      v_new_st % 8 == 0))));
   CB_ARG(workspace == nullptr || (uintptr_t)workspace % 16 == 0);
   if (B == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;

@@ -384,6 +384,8 @@ extern "C" int chitu_b200_mla_decode(const void* q_nope, const void* q_pe, void*
   using namespace cb;
   CB_ARG(q_nope && q_pe && kv_cache && seqlens_excl && block_table);
   CB_ARG(B >= 0 && H > 0 && bt_stride > 0 && num_blocks > 0);
+  // q and the new row are read with 16-byte loads, the cache through TMA and 16-byte stores
+  CB_ARG(((uintptr_t)q_nope | (uintptr_t)q_pe | (uintptr_t)kv_cache | (uintptr_t)new_kv) % 16 == 0);
   if (C != kC || R != kR)
     return fail(-1, "mla_decode: only kv_lora_rank=512, qk_rope_head_dim=64 is built (got %d,%d)", C, R);
   // the kernel stages one 64-token page per tile; the reference builds 64-token pages for absorbed MLA
