@@ -379,17 +379,19 @@ LSE_TOL = 2e-3             # log2 domain
 
 def ref_splits(q, K, V, L, S, chunk, scale):
     """fp64 attention of q [Hkv, G, Dk] over keys [0, L) of K [N, Hkv, Dk] / V [N, Hkv, Dv] in S ranges of `chunk`
-    keys.  Returns the per-range output o [Hkv, G, S, Dv], its log2-sum-exp lse [Hkv, G, S] (-inf when empty) and the
-    three bound terms rss, l1, st [Hkv, G, S, Dv]."""
+    keys; L is one key count or a tensor [G] of per-row counts (row g sees keys [0, L[g]), as under a causal mask).
+    Returns the per-range output o [Hkv, G, S, Dv], its log2-sum-exp lse [Hkv, G, S] (-inf when empty) and the three
+    bound terms rss, l1, st [Hkv, G, S, Dv]."""
     Hkv, G, Dk = q.shape
     Dv = V.shape[-1]
     Lp = S * chunk
+    n = int(L.max()) if torch.is_tensor(L) else L
     Kp = torch.zeros(Lp, Hkv, Dk, dtype=torch.float64, device=q.device)
     Vp = torch.zeros(Lp, Hkv, Dv, dtype=torch.float64, device=q.device)
-    Kp[:L], Vp[:L] = K[:L], V[:L]
+    Kp[:n], Vp[:n] = K[:n], V[:n]
     s = torch.einsum("kgd,lkd->kgl", q, Kp) * scale
     a = torch.einsum("kgd,lkd->kgl", q.abs(), Kp.abs()) * scale
-    valid = torch.arange(Lp, device=q.device) < L
+    valid = torch.arange(Lp, device=q.device) < (L[:, None] if torch.is_tensor(L) else L)
     a = torch.where(valid, a, 0.0)
     a = a + a.amax(dim=-1, keepdim=True) if Lp else a
     s = torch.where(valid, s, -math.inf).view(Hkv, G, S, chunk)
