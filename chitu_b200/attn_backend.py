@@ -167,7 +167,7 @@ class B200AttnBackend(AttnBackend):
                           softcap=0.0, softmax_scale=None):
         """GQA attention over the KV cache with the in-place append of k / v (flash_attn_with_kvcache semantics).
         q [B, sq, Hq, D]; with block_table the caches are paged [num_blocks, page, Hkv, D], without it [Bc, S, Hkv, D].
-        A paged cache in torch.float8_e4m3fn (both caches) runs `_paged_fp8`; otherwise the caches are in q's dtype."""
+        A paged cache in torch.float8_e4m3fn (both caches) runs the e4m3 kernels; otherwise the caches are in q's dtype."""
         fp8 = (k_cache.dtype == torch.float8_e4m3fn, v_cache.dtype == torch.float8_e4m3fn)
         if fp8[0] != fp8[1]:
             raise RuntimeError("attn_with_kvcache: k_cache and v_cache must have the same dtype")
@@ -178,93 +178,72 @@ class B200AttnBackend(AttnBackend):
                                     softcap, softmax_scale)
         assert cache_leftpad is None and window_size == (-1, -1) and softcap == 0.0
         require_cuda(q, k_cache, v_cache, block_table)
-        B, sq, Hq, D = q.shape
-        if fp8[0]:
-            return self._paged_fp8(q, k_cache, v_cache, k, v, cache_seqlens, block_table, causal, softmax_scale)
-        if sq > 1:
-            return self._paged_prefill(q, k_cache, v_cache, k, v, cache_seqlens, block_table, causal, softmax_scale)
-        num_blocks, page, Hkv, Dk = k_cache.shape
-        assert Dk == D and v_cache.shape == k_cache.shape
-        assert k_cache.dtype == v_cache.dtype == q.dtype and (k is None or k.dtype == v.dtype == q.dtype)
-        assert q.is_contiguous() and k_cache.is_contiguous() and v_cache.is_contiguous()
-        assert block_table.dtype == torch.int32 and block_table.stride(-1) == 1
-        if not torch.is_tensor(cache_seqlens):
-            cache_seqlens = torch.full((B,), int(cache_seqlens), dtype=torch.int32, device=q.device)
-        assert cache_seqlens.dtype == torch.int32 and cache_seqlens.is_contiguous()
-        ksb = vsb = 0
-        if k is not None:
-            assert v is not None and k.shape == (B, 1, Hkv, D) and v.shape == (B, 1, Hkv, D)
-            # heads must be dense; the batch stride is free (views into a fused qkv GEMM output)
-            assert k.stride(-1) == 1 and k.stride(-2) == D and v.stride(-1) == 1 and v.stride(-2) == D
-            ksb, vsb = k.stride(0), v.stride(0)
-        scale = softmax_scale if softmax_scale is not None else 1.0 / math.sqrt(D)
-        out = torch.empty_like(q)
-        ws, wsn = self._ws(B, Hq, D, q.device)
-        hint = self.max_seq_len if self.max_seq_len else block_table.shape[1] * page
-        check(_lib.load().chitu_b200_gqa_paged_decode(
-            ptr(q), ptr(k_cache), ptr(v_cache), ptr(k), ptr(v), ksb, vsb, ptr(cache_seqlens), ptr(block_table),
-            block_table.stride(0), B, Hq, Hkv, D, page, int(hint), float(scale), ptr(out), ptr(ws), wsn,
-            dtype_code(q.dtype), current_stream()), "gqa_paged_decode")
-        return out
+        return self._paged(q, k_cache, v_cache, k, v, cache_seqlens, block_table, causal, softmax_scale, fp8[0])
 
-    def _paged_prefill(self, q, k_cache, v_cache, k, v, cache_seqlens, block_table, causal, softmax_scale):
-        """seqlen_q > 1 (chunked prefill, prefill on a cached prefix, speculative verification): the sq new k / v rows
-        are appended at cache_seqlens[b] + i, then query i attends to the first cache_seqlens[b] + sq keys (without k / v:
-        cache_seqlens[b]), bottom-right causal when `causal` (chitu_b200_gqa_paged_prefill)."""
-        B, sq, Hq, D = q.shape
-        num_blocks, page, Hkv, Dk = k_cache.shape
-        assert Dk == D and v_cache.shape == k_cache.shape
-        assert k_cache.dtype == v_cache.dtype == q.dtype and (k is None or k.dtype == v.dtype == q.dtype)
-        assert q.is_contiguous() and k_cache.is_contiguous() and v_cache.is_contiguous()
-        assert block_table.dtype == torch.int32 and block_table.stride(-1) == 1
+    @staticmethod
+    def _seqlens(q, cache_seqlens):
+        """cache_seqlens as a tensor on q's device: an int stands for every request."""
         if not torch.is_tensor(cache_seqlens):
-            cache_seqlens = torch.full((B,), int(cache_seqlens), dtype=torch.int32, device=q.device)
+            cache_seqlens = torch.full((q.shape[0],), int(cache_seqlens), dtype=torch.int32, device=q.device)
+        return cache_seqlens
+
+    def _kv_args(self, q, k, v, Hkv, cache_seqlens, softmax_scale, cache_keys):
+        """What both cache layouts check and pass: cache_seqlens (a tensor, see _seqlens) int32 and contiguous, the
+        new k / v rows [B, sq, Hkv, D] in q's dtype as their strides (k_sb, k_st, v_sb, v_st) (zeros without them),
+        the softmax scale (default 1/sqrt(D)) and the length hint (max_seq_len, else the keys the cache holds)."""
+        B, sq, _, D = q.shape
         assert cache_seqlens.dtype == torch.int32 and cache_seqlens.is_contiguous()
         strides = (0, 0, 0, 0)
         if k is not None:
             assert v is not None and k.shape == (B, sq, Hkv, D) and v.shape == (B, sq, Hkv, D)
+            assert k.dtype == v.dtype == q.dtype
             # heads must be dense; the batch and token strides are free (views into a fused qkv GEMM output)
             assert k.stride(-1) == 1 and k.stride(-2) == D and v.stride(-1) == 1 and v.stride(-2) == D
             strides = (k.stride(0), k.stride(1), v.stride(0), v.stride(1))
         scale = softmax_scale if softmax_scale is not None else 1.0 / math.sqrt(D)
-        out = torch.empty_like(q)
-        ws, wsn = self._ws(B, Hq, D, q.device)
-        hint = self.max_seq_len if self.max_seq_len else block_table.shape[1] * page
-        check(_lib.load().chitu_b200_gqa_paged_prefill(
-            ptr(q), ptr(k_cache), ptr(v_cache), ptr(k), ptr(v), *strides, ptr(cache_seqlens), ptr(block_table),
-            block_table.stride(0), B, sq, Hq, Hkv, D, page, num_blocks, int(hint), int(bool(causal)), float(scale),
-            ptr(out), ptr(ws), wsn, dtype_code(q.dtype), current_stream()), "gqa_paged_prefill")
-        return out
+        hint = self.max_seq_len if self.max_seq_len else cache_keys
+        return strides, float(scale), int(hint)
 
-    def _paged_fp8(self, q, k_cache, v_cache, k, v, cache_seqlens, block_table, causal, softmax_scale):
-        """Paged e4m3 caches, sq >= 1 (chitu_b200_gqa_paged_attn_fp8kv): the semantics of the io-dtype paged cache, with
-        each new k / v element stored as x.float().clamp(-448, 448).to(float8_e4m3fn) and each cache element decoded
-        exactly to q's dtype (bf16 | fp16) before the unchanged arithmetic.  The appended rows are attended in their
-        stored form.  No scale.  Built for D == 128, Hq / Hkv in {1, 2, 4, 8} and a power-of-two page that is a multiple
-        of 64; no host synchronisation, capturable in a CUDA graph, deterministic."""
+    def _paged(self, q, k_cache, v_cache, k, v, cache_seqlens, block_table, causal, softmax_scale, fp8):
+        """Paged caches [num_blocks, page, Hkv, D]: the sq new k / v rows are appended at cache_seqlens[b] + i (true
+        page indexing), then query i attends to the first cache_seqlens[b] + sq keys (without k / v:
+        cache_seqlens[b]), bottom-right causal when `causal`.  sq == 1 runs the decode kernel
+        (chitu_b200_gqa_paged_decode), sq > 1 the multi-token kernel (chitu_b200_gqa_paged_prefill: chunked prefill,
+        prefill on a cached prefix, speculative verification).
+        `fp8`: e4m3 caches, sq >= 1 (chitu_b200_gqa_paged_attn_fp8kv): the same semantics, with each new k / v element
+        stored as x.float().clamp(-448, 448).to(float8_e4m3fn) and each cache element decoded exactly to q's dtype
+        (bf16 | fp16) before the unchanged arithmetic.  The appended rows are attended in their stored form.  No scale.
+        Built for D == 128, Hq / Hkv in {1, 2, 4, 8} and a power-of-two page that is a multiple of 64; no host
+        synchronisation, capturable in a CUDA graph, deterministic."""
         B, sq, Hq, D = q.shape
         num_blocks, page, Hkv, Dk = k_cache.shape
         assert Dk == D and v_cache.shape == k_cache.shape
-        assert q.dtype in (torch.bfloat16, torch.float16) and (k is None or k.dtype == v.dtype == q.dtype)
+        if fp8:
+            assert q.dtype in (torch.bfloat16, torch.float16)
+        else:
+            assert k_cache.dtype == v_cache.dtype == q.dtype
         assert q.is_contiguous() and k_cache.is_contiguous() and v_cache.is_contiguous()
         assert block_table.dtype == torch.int32 and block_table.stride(-1) == 1
-        if not torch.is_tensor(cache_seqlens):
-            cache_seqlens = torch.full((B,), int(cache_seqlens), dtype=torch.int32, device=q.device)
-        assert cache_seqlens.dtype == torch.int32 and cache_seqlens.is_contiguous()
-        strides = (0, 0, 0, 0)
-        if k is not None:
-            assert v is not None and k.shape == (B, sq, Hkv, D) and v.shape == (B, sq, Hkv, D)
-            # heads must be dense; the batch and token strides are free (views into a fused qkv GEMM output)
-            assert k.stride(-1) == 1 and k.stride(-2) == D and v.stride(-1) == 1 and v.stride(-2) == D
-            strides = (k.stride(0), k.stride(1), v.stride(0), v.stride(1))
-        scale = softmax_scale if softmax_scale is not None else 1.0 / math.sqrt(D)
+        cache_seqlens = self._seqlens(q, cache_seqlens)
+        strides, scale, hint = self._kv_args(q, k, v, Hkv, cache_seqlens, softmax_scale, block_table.shape[1] * page)
         out = torch.empty_like(q)
         ws, wsn = self._ws(B, Hq, D, q.device)
-        hint = self.max_seq_len if self.max_seq_len else block_table.shape[1] * page
-        check(_lib.load().chitu_b200_gqa_paged_attn_fp8kv(
-            ptr(q), sq * Hq * D, ptr(k_cache), ptr(v_cache), ptr(k), ptr(v), *strides, None, None, ptr(cache_seqlens),
-            ptr(block_table), block_table.stride(0), B, sq, Hq, Hkv, D, page, num_blocks, int(hint), int(bool(causal)),
-            float(scale), ptr(out), ptr(ws), wsn, dtype_code(q.dtype), current_stream()), "gqa_paged_attn_fp8kv")
+        lib, bt = _lib.load(), (ptr(block_table), block_table.stride(0))
+        if fp8:
+            check(lib.chitu_b200_gqa_paged_attn_fp8kv(
+                ptr(q), sq * Hq * D, ptr(k_cache), ptr(v_cache), ptr(k), ptr(v), *strides, None, None,
+                ptr(cache_seqlens), *bt, B, sq, Hq, Hkv, D, page, num_blocks, hint, int(bool(causal)), scale, ptr(out),
+                ptr(ws), wsn, dtype_code(q.dtype), current_stream()), "gqa_paged_attn_fp8kv")
+        elif sq == 1:
+            check(lib.chitu_b200_gqa_paged_decode(
+                ptr(q), ptr(k_cache), ptr(v_cache), ptr(k), ptr(v), strides[0], strides[2], ptr(cache_seqlens), *bt, B,
+                Hq, Hkv, D, page, hint, scale, ptr(out), ptr(ws), wsn, dtype_code(q.dtype), current_stream()),
+                "gqa_paged_decode")
+        else:
+            check(lib.chitu_b200_gqa_paged_prefill(
+                ptr(q), ptr(k_cache), ptr(v_cache), ptr(k), ptr(v), *strides, ptr(cache_seqlens), *bt, B, sq, Hq, Hkv,
+                D, page, num_blocks, hint, int(bool(causal)), scale, ptr(out), ptr(ws), wsn, dtype_code(q.dtype),
+                current_stream()), "gqa_paged_prefill")
         return out
 
     def _contiguous(self, q, k_cache, v_cache, k, v, cache_seqlens, cache_leftpad, causal, window_size, softcap,
@@ -276,29 +255,19 @@ class B200AttnBackend(AttnBackend):
         capturable in a CUDA graph, deterministic."""
         if cache_leftpad is not None or tuple(window_size) != (-1, -1) or softcap != 0.0:
             raise RuntimeError("gqa_contiguous_attn: cache_leftpad, window_size and softcap are not built")
-        if not torch.is_tensor(cache_seqlens):
-            cache_seqlens = torch.full((q.shape[0],), int(cache_seqlens), dtype=torch.int32, device=q.device)
+        cache_seqlens = self._seqlens(q, cache_seqlens)
         require_cuda(q, k_cache, v_cache, k, v, cache_seqlens)
         B, sq, Hq, D = q.shape
         Bc, S, Hkv, Dk = k_cache.shape
         cst = k_cache.stride()
         assert v_cache.shape == k_cache.shape and v_cache.stride() == cst and cst[1:] == (Hkv * D, D, 1)
         assert Dk == D and Bc >= B and k_cache.dtype == v_cache.dtype == q.dtype and q.is_contiguous()
-        assert cache_seqlens.dtype == torch.int32 and cache_seqlens.is_contiguous()
-        strides = (0, 0, 0, 0)
-        if k is not None:
-            assert v is not None and k.shape == (B, sq, Hkv, D) and v.shape == (B, sq, Hkv, D)
-            assert k.dtype == v.dtype == q.dtype
-            # heads must be dense; the batch and token strides are free (views into a fused qkv GEMM output)
-            assert k.stride(-1) == 1 and k.stride(-2) == D and v.stride(-1) == 1 and v.stride(-2) == D
-            strides = (k.stride(0), k.stride(1), v.stride(0), v.stride(1))
-        scale = softmax_scale if softmax_scale is not None else 1.0 / math.sqrt(D)
+        strides, scale, hint = self._kv_args(q, k, v, Hkv, cache_seqlens, softmax_scale, S)
         out = torch.empty_like(q)
         ws, wsn = self._ws(B, Hq, D, q.device)
-        hint = self.max_seq_len if self.max_seq_len else S
         check(_lib.load().chitu_b200_gqa_contiguous_attn(
             ptr(q), ptr(k_cache), ptr(v_cache), cst[0], S, ptr(k), ptr(v), *strides, ptr(cache_seqlens), B, sq,
-            Hq, Hkv, D, int(hint), int(bool(causal)), float(scale), ptr(out), ptr(ws), wsn, dtype_code(q.dtype),
+            Hq, Hkv, D, hint, int(bool(causal)), scale, ptr(out), ptr(ws), wsn, dtype_code(q.dtype),
             current_stream()), "gqa_contiguous_attn")
         return out
 

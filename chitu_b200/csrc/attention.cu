@@ -10,6 +10,8 @@
 //    seqlen_q > 1.
 //  * gqa_paged_attn_fp8kv : the paged cache in fp8 e4m3 (half the KV bytes): the e4m3 instance of the tensor-core
 //    decode kernel for seqlen_q == 1 (gqa_decode_mmaT_e4m3_kernel), gqa_prefill.cu's e4m3 instance for seqlen_q > 1.
+//    The three entries check their arguments; gqa_decode() launches seqlen_q == 1 for all of them, gqa_prefill()
+//    (gqa_prefill.cu) seqlen_q > 1.
 //  * merge_splits_kernel : the LSE-weighted merge of split-KV partials, for GQA decode, MLA decode
 //    (mla_tc.cu) and the GQA and MLA paged prefills (gqa_prefill.cu, mla_prefill.cu).  The workspace
 //    layout, the split counts, the split plan and the merge weights are defined once in splitkv.cuh.
@@ -659,6 +661,60 @@ __global__ void __launch_bounds__(kGqaWarps * 32, kGqaCtas) gqa_decode_mmaT_cont
                                      rows_sb, cache_rows);
 }
 
+// The seqlen_q == 1 path of the three GQA entries, for arguments the entry has checked (B > 0): the split count
+// (tensor cores: whole waves of kGqaCtas CTAs per SM; SIMT: ~4 CTAs per SM), shrunk to the workspace (none: 1 split),
+// the attention and, with a split, the merge, logged as `entry`.  The paged layouts read block_table, bt_stride and
+// page_size, the contiguous one rows_sb and cache_rows; q_sb and the rotary tables reach the paged tensor-core kernels.
+int gqa_decode(const char* entry, KvLayout layout, bool tc, const void* q, int64_t q_sb, void* k_cache, void* v_cache,
+               const void* k_new, const void* v_new, int64_t k_new_sb, int64_t v_new_sb, const float* rope_cos,
+               const float* rope_sin, const int32_t* cache_seqlens, const int32_t* block_table, int bt_stride,
+               int page_size, int64_t rows_sb, int cache_rows, int B, int Hq, int Hkv, int D, int max_len,
+               float softmax_scale, void* out, void* workspace, int64_t workspace_bytes, int dtype, cudaStream_t st) {
+  int splits = tc ? pick_splits_waves(B * Hkv, max_len, 132 * kGqaCtas) : pick_splits(B * Hkv, max_len, 256, 64);
+  splits = workspace ? splits_that_fit(splits, (int64_t)B * Hq, D, workspace_bytes) : 1;
+  const SplitKv part = split_kv_carve(workspace, workspace_bytes, (int64_t)B * Hq, D, splits);
+  int page_shift = 0;                                       // the paged tensor-core kernels' power-of-two page
+  if (tc && layout != KvLayout::kContiguous)
+    while ((1 << page_shift) < page_size) ++page_shift;
+  const dim3 grid(splits, Hkv, B), tc_block(kGqaWarps * 32), simt_block(128);
+  int rc = dispatch_io_g(dtype, Hq / Hkv, [&](auto t, auto g) {
+    using T = decltype(t);
+    constexpr int G = decltype(g)::value;
+    const T *qt = (const T*)q, *kn = (const T*)k_new, *vn = (const T*)v_new;
+    T *kc = (T*)k_cache, *vc = (T*)v_cache, *o = (T*)out;
+    float *op = part.o_part, *lse = part.lse;
+    if (layout == KvLayout::kPagedE4m3)
+      return launch_smem<gqa_decode_mmaT_e4m3_kernel<T, G>>(
+          entry, grid, tc_block, kGqaE4m3SmemBytes, st, qt, (uint8_t*)k_cache, (uint8_t*)v_cache, kn, vn, k_new_sb,
+          v_new_sb, cache_seqlens, block_table, bt_stride, Hq, Hkv, page_shift, softmax_scale, splits, op, lse, o, q_sb,
+          rope_cos, rope_sin);
+    if (layout == KvLayout::kContiguous && tc)
+      return launch_smem<gqa_decode_mmaT_contig_kernel<T, G>>(
+          entry, grid, tc_block, kGqaSmemBytes, st, qt, kc, vc, kn, vn, k_new_sb, v_new_sb, cache_seqlens, rows_sb,
+          cache_rows, Hq, Hkv, softmax_scale, splits, op, lse, o);
+    if (layout == KvLayout::kContiguous)
+      launch_k(gqa_decode_contig_kernel<T, 64, G>, grid, simt_block, 0, st, qt, kc, vc, kn, vn, k_new_sb, v_new_sb,
+               cache_seqlens, rows_sb, cache_rows, Hq, Hkv, softmax_scale, splits, op, lse, o);
+    else if (tc)
+      return launch_smem<gqa_decode_mmaT_kernel<T, G>>(
+          entry, grid, tc_block, kGqaSmemBytes, st, qt, kc, vc, kn, vn, k_new_sb, v_new_sb, cache_seqlens, block_table,
+          bt_stride, Hq, Hkv, page_shift, softmax_scale, splits, op, lse, o, q_sb, rope_cos, rope_sin);
+    else
+      launch_k(D == 128 ? gqa_decode_kernel<T, 128, G> : gqa_decode_kernel<T, 64, G>, grid, simt_block, 0, st, qt, kc,
+               vc, kn, vn, k_new_sb, v_new_sb, cache_seqlens, block_table, bt_stride, Hq, Hkv, page_size,
+               softmax_scale, splits, op, lse, o);
+    return 0;
+  });
+  if (rc) return rc;
+  CB_LAUNCHED_AS(entry, 1);
+  if (splits > 1) {
+    rc = launch_merge_splits(part.o_part, part.lse, out, B * Hq, splits, D, dtype, st);
+    if (rc) return rc;
+    CB_LAUNCHED_AS(entry, 1);
+  }
+  return 0;
+}
+
 }  // namespace
 
 extern "C" int64_t chitu_b200_attn_workspace_bytes(int batch, int heads, int head_dim_v, int max_splits) {
@@ -700,17 +756,13 @@ extern "C" int chitu_b200_gqa_paged_decode_rope(const void* q, int64_t q_sb, voi
                                                 int bt_stride, int B, int Hq, int Hkv, int D, int page_size,
                                                 int max_seqlen_hint, float softmax_scale, void* out, void* workspace,
                                                 int64_t workspace_bytes, int dtype, void* stream) {
-  CB_ARG(q && k_cache && v_cache && cache_seqlens && block_table && out);
+  if (int rc = check_gqa_operands(__func__, q, k_cache, v_cache, cache_seqlens, out, k_new, v_new, k_new_sb, 0,
+                                  v_new_sb, 0, false, dtype))
+    return rc;
+  CB_ARG(block_table);
   CB_ARG((rope_cos == nullptr) == (rope_sin == nullptr) && q_sb >= (int64_t)Hq * D && q_sb % 2 == 0);
-  CB_ARG((k_new == nullptr) == (v_new == nullptr));
   CB_ARG(B >= 0 && Hq > 0 && Hkv > 0 && Hq % Hkv == 0 && page_size > 0 && bt_stride > 0);
   CB_ARG(D == 64 || D == 128);
-  // the tensor-core kernel stages the appended row with 16-byte cp.async from k_new + b * k_new_sb: 8-element strides
-  // and 16-byte aligned operands, as the fp8 entry requires
-  CB_ARG(k_new == nullptr || (k_new_sb % 8 == 0 && v_new_sb % 8 == 0));
-  CB_ARG(((uintptr_t)q | (uintptr_t)k_cache | (uintptr_t)v_cache | (uintptr_t)out | (uintptr_t)k_new |
-          (uintptr_t)v_new) % 16 == 0);
-  CB_ARG(dtype == CB_BF16 || dtype == CB_F16);
   if (B == 0) return 0;
   const int G = Hq / Hkv;
   CB_ARG(G == 1 || G == 2 || G == 4 || G == 8);
@@ -718,66 +770,9 @@ extern "C" int chitu_b200_gqa_paged_decode_rope(const void* q, int64_t q_sb, voi
   if (!tc && (rope_cos || q_sb != (int64_t)Hq * D))
     return fail(-2, "gqa_paged_decode_rope: fused rotary / strided q need head_dim 128 and a power-of-two page");
   const int max_len = max_seqlen_hint > 0 ? max_seqlen_hint : bt_stride * page_size;
-  int splits = tc ? pick_splits_waves(B * Hkv, max_len, 132 * kGqaCtas) : pick_splits(B * Hkv, max_len, 256, 64);
-  splits = workspace ? splits_that_fit(splits, (int64_t)B * Hq, D, workspace_bytes) : 1;
-  const auto [o_part, lse, plan] = split_kv_carve(workspace, workspace_bytes, (int64_t)B * Hq, D, splits);
-  cudaStream_t st = (cudaStream_t)stream;
-  const dim3 grid(splits, Hkv, B);
-
-  if (tc) {
-    int page_shift = 0;
-    while ((1 << page_shift) < page_size) ++page_shift;
-#define LAUNCH_MMAT(T, GG)                                                                                   \
-  do {                                                                                                       \
-    static bool attr = false;                                                                                \
-    if (!attr) {                                                                                             \
-      CB_CUDA(cudaFuncSetAttribute(gqa_decode_mmaT_kernel<T, GG>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
-                                   kGqaSmemBytes));                                                          \
-      attr = true;                                                                                           \
-    }                                                                                                        \
-    cb::launch_k(gqa_decode_mmaT_kernel<T, GG>, grid, dim3(kGqaWarps * 32), (size_t)kGqaSmemBytes, st,       \
-        (const T*)q, (T*)k_cache, (T*)v_cache, (const T*)k_new, (const T*)v_new, k_new_sb, v_new_sb,         \
-        cache_seqlens, block_table, bt_stride, Hq, Hkv, page_shift, softmax_scale, splits, o_part, lse,      \
-        (T*)out, q_sb, rope_cos, rope_sin);                                                                  \
-  } while (0)
-#define DISPATCH_MMAT(T)                 \
-  switch (G) {                           \
-    case 1: LAUNCH_MMAT(T, 1); break;    \
-    case 2: LAUNCH_MMAT(T, 2); break;    \
-    case 4: LAUNCH_MMAT(T, 4); break;    \
-    default: LAUNCH_MMAT(T, 8); break;   \
-  }
-    if (dtype == CB_BF16) { DISPATCH_MMAT(__nv_bfloat16); } else { DISPATCH_MMAT(__half); }
-#undef DISPATCH_MMAT
-#undef LAUNCH_MMAT
-  } else {
-#define LAUNCH_GQA(T, DD, GG)                                                                       \
-  cb::launch_k(gqa_decode_kernel<T, DD, GG>, grid, dim3(128), 0, st,                                \
-      (const T*)q, (T*)k_cache, (T*)v_cache, (const T*)k_new, (const T*)v_new, k_new_sb, v_new_sb,  \
-      cache_seqlens,                                                                                \
-      block_table, bt_stride, Hq, Hkv, page_size, softmax_scale, splits, o_part, lse, (T*)out)
-#define DISPATCH_G(T, DD)                         \
-  switch (G) {                                    \
-    case 1: LAUNCH_GQA(T, DD, 1); break;          \
-    case 2: LAUNCH_GQA(T, DD, 2); break;          \
-    case 4: LAUNCH_GQA(T, DD, 4); break;          \
-    default: LAUNCH_GQA(T, DD, 8); break;         \
-  }
-    if (dtype == CB_BF16) {
-      if (D == 128) { DISPATCH_G(__nv_bfloat16, 128) } else { DISPATCH_G(__nv_bfloat16, 64) }
-    } else {
-      if (D == 128) { DISPATCH_G(__half, 128) } else { DISPATCH_G(__half, 64) }
-    }
-#undef DISPATCH_G
-#undef LAUNCH_GQA
-  }
-  CB_LAUNCHED(1);
-  if (splits > 1) {
-    int rc = launch_merge_splits(o_part, lse, out, B * Hq, splits, D, dtype, st);
-    if (rc) return rc;
-    CB_LAUNCHED(1);
-  }
-  return 0;
+  return gqa_decode(__func__, KvLayout::kPaged, tc, q, q_sb, k_cache, v_cache, k_new, v_new, k_new_sb, v_new_sb,
+                    rope_cos, rope_sin, cache_seqlens, block_table, bt_stride, page_size, 0, 0, B, Hq, Hkv, D, max_len,
+                    softmax_scale, out, workspace, workspace_bytes, dtype, (cudaStream_t)stream);
 }
 
 // flash_attn_with_kvcache without a block table (include/chitu_b200.h): sq == 1 runs the decode kernels' contiguous
@@ -788,71 +783,27 @@ extern "C" int chitu_b200_gqa_contiguous_attn(const void* q, void* k_cache, void
                                               const int32_t* cache_seqlens, int B, int sq, int Hq, int Hkv, int D,
                                               int max_seqlen_hint, int causal, float softmax_scale, void* out,
                                               void* workspace, int64_t workspace_bytes, int dtype, void* stream) {
-  CB_ARG(q && k_cache && v_cache && cache_seqlens && out);
-  CB_ARG((k_new == nullptr) == (v_new == nullptr));
+  if (int rc = check_gqa_operands(__func__, q, k_cache, v_cache, cache_seqlens, out, k_new, v_new, k_new_sb, k_new_st,
+                                  v_new_sb, v_new_st, sq > 1, dtype))
+    return rc;
   CB_ARG(B >= 0 && B <= 65535 && sq >= 1 && Hq > 0 && Hkv > 0 && Hkv <= 65535 && Hq % Hkv == 0);
   const int G = Hq / Hkv;
   CB_ARG(G == 1 || G == 2 || G == 4 || G == 8);
   CB_ARG(D == 128 || (D == 64 && sq == 1));
-  CB_ARG(dtype == CB_BF16 || dtype == CB_F16);
   const int64_t row = (int64_t)Hkv * D;                     // elements of one cache position
   CB_ARG(cache_rows >= 1 && cache_sb >= cache_rows * row && cache_sb % row == 0 && cache_sb % 8 == 0);
-  CB_ARG(((uintptr_t)q | (uintptr_t)k_cache | (uintptr_t)v_cache | (uintptr_t)out | (uintptr_t)k_new |
-          (uintptr_t)v_new) % 16 == 0);
-  // k / v strides in multiples of 8 elements: the tensor-core decode kernel (D = 128) and the multi-token kernel stage
-  // the new rows with 16-byte cp.async (sq == 1 reads only the batch strides)
-  CB_ARG(k_new == nullptr || (k_new_sb % 8 == 0 && v_new_sb % 8 == 0 && (sq == 1 || (k_new_st % 8 == 0 &&
-                                                                                      v_new_st % 8 == 0))));
   CB_ARG(workspace == nullptr || (uintptr_t)workspace % 16 == 0);
   if (B == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
   const int max_len = max_seqlen_hint > 0 ? max_seqlen_hint : cache_rows;
   const int64_t rows_sb = cache_sb / row;
   if (sq > 1)
-    return gqa_contiguous_prefill(q, k_cache, v_cache, rows_sb, cache_rows, k_new, v_new, k_new_sb, k_new_st,
-                                  v_new_sb, v_new_st, cache_seqlens, B, sq, Hq, Hkv, max_len, causal, softmax_scale, out,
-                                  workspace, workspace_bytes, dtype, st);
-
-  const bool tc = D == kGqaD;
-  int splits = tc ? pick_splits_waves(B * Hkv, max_len, 132 * kGqaCtas) : pick_splits(B * Hkv, max_len, 256, 64);
-  splits = workspace ? splits_that_fit(splits, (int64_t)B * Hq, D, workspace_bytes) : 1;
-  const auto [o_part, lse, plan] = split_kv_carve(workspace, workspace_bytes, (int64_t)B * Hq, D, splits);
-  const dim3 grid(splits, Hkv, B);
-#define LAUNCH_CONTIG(T, GG)                                                                                      \
-  do {                                                                                                            \
-    if (tc) {                                                                                                     \
-      static bool attr = false;                                                                                   \
-      if (!attr) {                                                                                                \
-        CB_CUDA(cudaFuncSetAttribute(gqa_decode_mmaT_contig_kernel<T, GG>,                                        \
-                                     cudaFuncAttributeMaxDynamicSharedMemorySize, kGqaSmemBytes));                \
-        attr = true;                                                                                              \
-      }                                                                                                           \
-      cb::launch_k(gqa_decode_mmaT_contig_kernel<T, GG>, grid, dim3(kGqaWarps * 32), (size_t)kGqaSmemBytes, st,   \
-                   (const T*)q, (T*)k_cache, (T*)v_cache, (const T*)k_new, (const T*)v_new, k_new_sb, v_new_sb,   \
-                   cache_seqlens, rows_sb, cache_rows, Hq, Hkv, softmax_scale, splits, o_part, lse, (T*)out);     \
-    } else {                                                                                                      \
-      cb::launch_k(gqa_decode_contig_kernel<T, 64, GG>, grid, dim3(128), 0, st, (const T*)q, (T*)k_cache,         \
-                   (T*)v_cache, (const T*)k_new, (const T*)v_new, k_new_sb, v_new_sb, cache_seqlens, rows_sb,     \
-                   cache_rows, Hq, Hkv, softmax_scale, splits, o_part, lse, (T*)out);                             \
-    }                                                                                                             \
-  } while (0)
-#define DISPATCH_CONTIG(T)                 \
-  switch (G) {                             \
-    case 1: LAUNCH_CONTIG(T, 1); break;    \
-    case 2: LAUNCH_CONTIG(T, 2); break;    \
-    case 4: LAUNCH_CONTIG(T, 4); break;    \
-    default: LAUNCH_CONTIG(T, 8); break;   \
-  }
-  if (dtype == CB_BF16) { DISPATCH_CONTIG(__nv_bfloat16); } else { DISPATCH_CONTIG(__half); }
-#undef DISPATCH_CONTIG
-#undef LAUNCH_CONTIG
-  CB_LAUNCHED(1);
-  if (splits > 1) {
-    int rc = launch_merge_splits(o_part, lse, out, B * Hq, splits, D, dtype, st);
-    if (rc) return rc;
-    CB_LAUNCHED(1);
-  }
-  return 0;
+    return gqa_prefill(__func__, "gqa_contiguous_prefill", KvLayout::kContiguous, q, k_cache, v_cache, k_new, v_new,
+                       k_new_sb, k_new_st, v_new_sb, v_new_st, cache_seqlens, nullptr, 0, 0, 0, rows_sb, cache_rows, B,
+                       sq, Hq, Hkv, max_len, causal, softmax_scale, out, workspace, workspace_bytes, dtype, st);
+  return gqa_decode(__func__, KvLayout::kContiguous, D == kGqaD, q, (int64_t)Hq * D, k_cache, v_cache, k_new, v_new,
+                    k_new_sb, v_new_sb, nullptr, nullptr, cache_seqlens, nullptr, 0, 0, rows_sb, cache_rows, B, Hq, Hkv,
+                    D, max_len, softmax_scale, out, workspace, workspace_bytes, dtype, st);
 }
 
 // flash_attn_with_kvcache (paged) over an e4m3 cache (include/chitu_b200.h): sq == 1 runs the e4m3 instance of the
@@ -865,67 +816,31 @@ extern "C" int chitu_b200_gqa_paged_attn_fp8kv(const void* q, int64_t q_sb, void
                                                int Hkv, int D, int page_size, int num_blocks, int max_seqlen_hint,
                                                int causal, float softmax_scale, void* out, void* workspace,
                                                int64_t workspace_bytes, int dtype, void* stream) {
-  CB_ARG(q && k_cache && v_cache && cache_seqlens && block_table && out);
-  CB_ARG((k_new == nullptr) == (v_new == nullptr) && (rope_cos == nullptr) == (rope_sin == nullptr));
+  if (int rc = check_gqa_operands(__func__, q, k_cache, v_cache, cache_seqlens, out, k_new, v_new, k_new_sb, k_new_st,
+                                  v_new_sb, v_new_st, sq > 1, dtype))
+    return rc;
+  CB_ARG(block_table && (rope_cos == nullptr) == (rope_sin == nullptr));
   CB_ARG(B >= 0 && B <= 65535 && sq >= 1 && Hq > 0 && Hkv > 0 && Hkv <= 65535 && Hq % Hkv == 0);
   const int G = Hq / Hkv;
   CB_ARG(G == 1 || G == 2 || G == 4 || G == 8);
   CB_ARG(D == kGqaD);
-  CB_ARG(dtype == CB_BF16 || dtype == CB_F16);
   CB_ARG(bt_stride > 0 && num_blocks > 0 && page_size >= 64 && page_size % 64 == 0 &&
          (page_size & (page_size - 1)) == 0 && (int64_t)num_blocks * page_size <= 0x7fffffff);
   CB_ARG(rope_cos == nullptr || sq == 1);
   CB_ARG((int64_t)sq * Hq <= 0x7fffffff / D && q_sb % 8 == 0 &&
          (sq == 1 ? q_sb >= (int64_t)Hq * D : q_sb == (int64_t)sq * Hq * D));
-  CB_ARG(((uintptr_t)q | (uintptr_t)k_cache | (uintptr_t)v_cache | (uintptr_t)out | (uintptr_t)k_new |
-          (uintptr_t)v_new) % 16 == 0);
-  CB_ARG(k_new == nullptr || (k_new_sb % 8 == 0 && v_new_sb % 8 == 0 && (sq == 1 || (k_new_st % 8 == 0 &&
-                                                                                      v_new_st % 8 == 0))));
   CB_ARG(workspace == nullptr || (uintptr_t)workspace % 16 == 0);
   if (B == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
   const int max_len = max_seqlen_hint > 0 ? max_seqlen_hint : bt_stride * page_size;
   if (sq > 1)
-    return gqa_paged_prefill_e4m3(q, k_cache, v_cache, k_new, v_new, k_new_sb, k_new_st, v_new_sb, v_new_st,
-                                  cache_seqlens, block_table, bt_stride, B, sq, Hq, Hkv, page_size, num_blocks, max_len,
-                                  causal, softmax_scale, out, workspace, workspace_bytes, dtype, st);
-
-  int page_shift = 0;
-  while ((1 << page_shift) < page_size) ++page_shift;
-  int splits = pick_splits_waves(B * Hkv, max_len, 132 * kGqaCtas);      // the io-dtype decode's splits
-  splits = workspace ? splits_that_fit(splits, (int64_t)B * Hq, D, workspace_bytes) : 1;
-  const auto [o_part, lse, plan] = split_kv_carve(workspace, workspace_bytes, (int64_t)B * Hq, D, splits);
-  const dim3 grid(splits, Hkv, B);
-#define LAUNCH_E4M3(T, GG)                                                                                         \
-  do {                                                                                                             \
-    static bool attr = false;                                                                                      \
-    if (!attr) {                                                                                                   \
-      CB_CUDA(cudaFuncSetAttribute(gqa_decode_mmaT_e4m3_kernel<T, GG>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
-                                   kGqaE4m3SmemBytes));                                                            \
-      attr = true;                                                                                                 \
-    }                                                                                                              \
-    cb::launch_k(gqa_decode_mmaT_e4m3_kernel<T, GG>, grid, dim3(kGqaWarps * 32), (size_t)kGqaE4m3SmemBytes, st,    \
-                 (const T*)q, (uint8_t*)k_cache, (uint8_t*)v_cache, (const T*)k_new, (const T*)v_new, k_new_sb,      \
-                 v_new_sb, cache_seqlens, block_table, bt_stride, Hq, Hkv, page_shift, softmax_scale, splits, o_part, \
-                 lse, (T*)out, q_sb, rope_cos, rope_sin);                                                          \
-  } while (0)
-#define DISPATCH_E4M3(T)                 \
-  switch (G) {                           \
-    case 1: LAUNCH_E4M3(T, 1); break;    \
-    case 2: LAUNCH_E4M3(T, 2); break;    \
-    case 4: LAUNCH_E4M3(T, 4); break;    \
-    default: LAUNCH_E4M3(T, 8); break;   \
-  }
-  if (dtype == CB_BF16) { DISPATCH_E4M3(__nv_bfloat16); } else { DISPATCH_E4M3(__half); }
-#undef DISPATCH_E4M3
-#undef LAUNCH_E4M3
-  CB_LAUNCHED(1);
-  if (splits > 1) {
-    int rc = launch_merge_splits(o_part, lse, out, B * Hq, splits, D, dtype, st);
-    if (rc) return rc;
-    CB_LAUNCHED(1);
-  }
-  return 0;
+    return gqa_prefill(__func__, "gqa_paged_prefill_e4m3", KvLayout::kPagedE4m3, q, k_cache, v_cache, k_new, v_new,
+                       k_new_sb, k_new_st, v_new_sb, v_new_st, cache_seqlens, block_table, bt_stride, page_size,
+                       num_blocks, 0, 0, B, sq, Hq, Hkv, max_len, causal, softmax_scale, out, workspace,
+                       workspace_bytes, dtype, st);
+  return gqa_decode(__func__, KvLayout::kPagedE4m3, true, q, q_sb, k_cache, v_cache, k_new, v_new, k_new_sb, v_new_sb,
+                    rope_cos, rope_sin, cache_seqlens, block_table, bt_stride, page_size, 0, 0, B, Hq, Hkv, D, max_len,
+                    softmax_scale, out, workspace, workspace_bytes, dtype, st);
 }
 
 // ============================================================================================

@@ -8,6 +8,7 @@
 #include <stdio.h>
 #include <stdarg.h>
 #include <atomic>
+#include <type_traits>
 #include <utility>
 
 #include "../../include/chitu_b200.h"
@@ -17,19 +18,22 @@ namespace cb {
 int fail(int code, const char* fmt, ...);
 void count_launch(int n = 1);
 
-#define CB_ARG(cond)                                                                  \
-  do {                                                                                \
-    if (!(cond)) return cb::fail(-1, "%s: argument check failed: %s", __func__, #cond); \
+// The _AS forms report under `name` (a helper shared by several C entries passes the name of the entry it serves).
+#define CB_ARG_AS(name, cond)                                                                \
+  do {                                                                                       \
+    if (!(cond)) return cb::fail(-1, "%s: argument check failed: %s", (name), #cond);        \
   } while (0)
+#define CB_ARG(cond) CB_ARG_AS(__func__, cond)
 
-#define CB_LAUNCHED(n)                                                                        \
+#define CB_LAUNCHED_AS(name, n)                                                               \
   do {                                                                                        \
     cudaError_t e__ = cudaGetLastError();                                                     \
     if (e__ != cudaSuccess)                                                                   \
-      return cb::fail((int)e__, "%s: launch failed: %s", __func__, cudaGetErrorString(e__)); \
+      return cb::fail((int)e__, "%s: launch failed: %s", (name), cudaGetErrorString(e__));   \
     cb::count_launch(n);                                                                      \
-    if (cb::tl_enabled()) cb::tl_log_launch(__func__, n);                                     \
+    if (cb::tl_enabled()) cb::tl_log_launch((name), n);                                       \
   } while (0)
+#define CB_LAUNCHED(n) CB_LAUNCHED_AS(__func__, n)
 
 #define CB_CUDA(call)                                                                       \
   do {                                                                                      \
@@ -100,6 +104,35 @@ inline cudaError_t launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, siz
   cfg.numAttrs = 1;
   return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
 }
+
+// launch_k of kernel K with `smem` bytes of dynamic shared memory, after raising K's limit to `smem` on its first
+// launch.  The flag is keyed on K itself (two instances with one signature get one each), set by a thread-safe static
+// initializer, and keeps the outcome: a failed limit is reported under `name` by every call.  Launch errors are left
+// to CB_LAUNCHED.
+template <auto K, typename... Args>
+inline int launch_smem(const char* name, dim3 grid, dim3 block, int smem, cudaStream_t st, Args&&... args) {
+  static const cudaError_t limit = cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  if (limit != cudaSuccess)
+    return fail((int)limit, "%s: cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed: %s", name,
+                cudaGetErrorString(limit));
+  launch_k(K, grid, block, (size_t)smem, st, std::forward<Args>(args)...);
+  return 0;
+}
+
+// f(T{}, std::integral_constant<int, G>{}) for the io type of `dtype` (CB_BF16, else fp16) and G = 1, 2, 4, else 8;
+// returns f's status.
+template <typename F>
+inline int dispatch_io_g(int dtype, int G, F&& f) {
+  auto by_g = [&](auto t) {
+    switch (G) {
+      case 1: return f(t, std::integral_constant<int, 1>{});
+      case 2: return f(t, std::integral_constant<int, 2>{});
+      case 4: return f(t, std::integral_constant<int, 4>{});
+      default: return f(t, std::integral_constant<int, 8>{});
+    }
+  };
+  return dtype == CB_BF16 ? by_g(__nv_bfloat16{}) : by_g(__half{});
+}
 #endif
 
 // ---- push-mode all-reduce: descriptor handed to the producing kernels (comm.cu fills it) -------------------------
@@ -138,23 +171,38 @@ void launch_contiguous_append(PagedAppend c0, PagedAppend c1, int64_t row_bytes,
 void launch_paged_append_e4m3(PagedAppend c0, PagedAppend c1, int n, int dtype, const int32_t* seqlens,
                               const int32_t* block_table, int bt_stride, int B, int sq, int page_size, cudaStream_t st);
 
-// ---- GQA attention over an e4m3 paged cache with sq > 1 (gqa_prefill.cu), the multi-token path of
-// chitu_b200_gqa_paged_attn_fp8kv, which checks the arguments.  Launches the append (with k_new), the attention and,
-// with a split, the merge, and counts them.
-int gqa_paged_prefill_e4m3(const void* q, void* k_cache, void* v_cache, const void* k_new, const void* v_new,
-                           int64_t k_new_sb, int64_t k_new_st, int64_t v_new_sb, int64_t v_new_st,
-                           const int32_t* cache_seqlens, const int32_t* block_table, int bt_stride, int B, int sq,
-                           int Hq, int Hkv, int page_size, int num_blocks, int max_len, int causal, float softmax_scale,
-                           void* out, void* workspace, int64_t workspace_bytes, int dtype, cudaStream_t st);
+// ---- GQA attention over the KV cache (attention.cu, gqa_prefill.cu) -------------------------------------------------
+// The cache layouts of the GQA entries: paged in the io dtype, contiguous [Bc, cache_rows, Hkv, D] (request b from row
+// b * rows_sb, in rows of Hkv * D), paged in e4m3.
+enum class KvLayout { kPaged, kContiguous, kPagedE4m3 };
 
-// ---- GQA attention over a contiguous cache with sq > 1 (gqa_prefill.cu), the multi-token path of
-// chitu_b200_gqa_contiguous_attn, which checks the arguments.  rows_sb: the caches' batch stride in rows of Hkv * D.
-// Launches the append (with k_new), the attention and, with a split, the merge, and counts them.
-int gqa_contiguous_prefill(const void* q, void* k_cache, void* v_cache, int64_t rows_sb, int cache_rows,
-                           const void* k_new, const void* v_new, int64_t k_new_sb, int64_t k_new_st, int64_t v_new_sb,
-                           int64_t v_new_st, const int32_t* cache_seqlens, int B, int sq, int Hq, int Hkv, int max_len,
-                           int causal, float softmax_scale, void* out, void* workspace, int64_t workspace_bytes,
-                           int dtype, cudaStream_t st);
+// The argument checks every GQA entry shares, reported under `entry`: the operands, k_new and v_new given together,
+// bf16 / fp16, 16-byte aligned bases and 8-element k / v batch strides (token strides too with `token_strides`), as
+// the kernels stage q and the new rows 16 bytes at a time.
+inline int check_gqa_operands(const char* entry, const void* q, const void* k_cache, const void* v_cache,
+                              const int32_t* cache_seqlens, const void* out, const void* k_new, const void* v_new,
+                              int64_t k_new_sb, int64_t k_new_st, int64_t v_new_sb, int64_t v_new_st,
+                              bool token_strides, int dtype) {
+  CB_ARG_AS(entry, q && k_cache && v_cache && cache_seqlens && out);
+  CB_ARG_AS(entry, (k_new == nullptr) == (v_new == nullptr));
+  CB_ARG_AS(entry, dtype == CB_BF16 || dtype == CB_F16);
+  CB_ARG_AS(entry, ((uintptr_t)q | (uintptr_t)k_cache | (uintptr_t)v_cache | (uintptr_t)out | (uintptr_t)k_new |
+                    (uintptr_t)v_new) % 16 == 0);
+  CB_ARG_AS(entry, k_new == nullptr || (k_new_sb % 8 == 0 && v_new_sb % 8 == 0 &&
+                                        (!token_strides || (k_new_st % 8 == 0 && v_new_st % 8 == 0))));
+  return 0;
+}
+
+// The multi-token kernel of gqa_prefill.cu over any layout, for arguments the calling entry has checked (B > 0):
+// launches the append (with k_new), the attention and, with a split, the merge, and logs them as `name`; refusals
+// name `entry`.  block_table, bt_stride, page_size and num_blocks describe a paged cache, rows_sb and cache_rows a
+// contiguous one.
+int gqa_prefill(const char* entry, const char* name, KvLayout layout, const void* q, void* k_cache, void* v_cache,
+                const void* k_new, const void* v_new, int64_t k_new_sb, int64_t k_new_st, int64_t v_new_sb,
+                int64_t v_new_st, const int32_t* cache_seqlens, const int32_t* block_table, int bt_stride,
+                int page_size, int num_blocks, int64_t rows_sb, int cache_rows, int B, int sq, int Hq, int Hkv,
+                int max_len, int causal, float softmax_scale, void* out, void* workspace, int64_t workspace_bytes,
+                int dtype, cudaStream_t st);
 
 #ifdef __CUDACC__
 // byte offset of this rank's area inside every push buffer, for the reduce that is being produced

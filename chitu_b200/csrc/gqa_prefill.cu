@@ -32,6 +32,8 @@
 // CTA's key tiles and writes normalised fp32 partials + LSE to the workspace as [B, sq * Hq, S, 128] (the decode
 // layout with H = sq * Hq), merged by attention.cu's merge_splits_kernel.  Deterministic: the split count depends on
 // host values only and every partial is reduced in a fixed order.
+// gqa_prefill() launches all three layouts: for chitu_b200_gqa_paged_prefill here and for the multi-token paths of
+// chitu_b200_gqa_contiguous_attn and chitu_b200_gqa_paged_attn_fp8kv (attention.cu), which check their arguments.
 #include <cuda.h>
 #include <limits.h>
 
@@ -375,138 +377,80 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) gqa_prefill_contig_kerne
                                  scale, row_tiles, splits, o_part, lse, out);
 }
 
-// splits of the multi-token kernel: the decode kernels' wave rule on its CTAs, shrunk to the workspace (none: 1 split)
-int prefill_splits(int row_tiles, int Hkv, int B, int64_t rows, int max_len, const void* workspace,
-                   int64_t workspace_bytes) {
-  const int splits = pick_splits_waves(row_tiles * Hkv * B, max_len, 132 * kCtasPerSm);
-  return workspace ? splits_that_fit(splits, rows, kD, workspace_bytes) : 1;
-}
-
-CUtensorMapDataType tma_dtype(int dtype) {
-  return dtype == CB_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-}
-
 }  // namespace
 
-// The multi-token path of chitu_b200_gqa_contiguous_attn (attention.cu), which has checked the arguments.
-int gqa_contiguous_prefill(const void* q, void* k_cache, void* v_cache, int64_t rows_sb, int cache_rows,
-                           const void* k_new, const void* v_new, int64_t k_new_sb, int64_t k_new_st, int64_t v_new_sb,
-                           int64_t v_new_st, const int32_t* cache_seqlens, int B, int sq, int Hq, int Hkv, int max_len,
-                           int causal, float softmax_scale, void* out, void* workspace, int64_t workspace_bytes,
-                           int dtype, cudaStream_t st) {
-  if (!tma_available()) return fail(-3, "gqa_contiguous_attn: TMA is not available");
+int gqa_prefill(const char* entry, const char* name, KvLayout layout, const void* q, void* k_cache, void* v_cache,
+                const void* k_new, const void* v_new, int64_t k_new_sb, int64_t k_new_st, int64_t v_new_sb,
+                int64_t v_new_st, const int32_t* cache_seqlens, const int32_t* block_table, int bt_stride,
+                int page_size, int num_blocks, int64_t rows_sb, int cache_rows, int B, int sq, int Hq, int Hkv,
+                int max_len, int causal, float softmax_scale, void* out, void* workspace, int64_t workspace_bytes,
+                int dtype, cudaStream_t st) {
+  if (!tma_available()) return fail(-3, "%s: TMA is not available", entry);
   const int G = Hq / Hkv;
   const int row_tiles = cdiv((int64_t)sq * G, kRows);
   const int64_t rows = (int64_t)B * sq * Hq;
-  const int splits = prefill_splits(row_tiles, Hkv, B, rows, max_len, workspace, workspace_bytes);
+  // the decode kernels' wave rule on this kernel's CTAs, shrunk to the workspace (none: 1 split)
+  int splits = pick_splits_waves(row_tiles * Hkv * B, max_len, 132 * kCtasPerSm);
+  splits = workspace ? splits_that_fit(splits, rows, kD, workspace_bytes) : 1;
   if ((int64_t)row_tiles * splits > INT_MAX)
-    return fail(-1, "gqa_contiguous_attn: %d row tiles x %d splits exceed the grid", row_tiles, splits);
-  const auto [o_part, lse, plan] = split_kv_carve(splits > 1 ? workspace : nullptr, workspace_bytes, rows, kD, splits);
+    return fail(-1, "%s: %d row tiles x %d splits exceed the grid", entry, row_tiles, splits);
+  const SplitKv part = split_kv_carve(splits > 1 ? workspace : nullptr, workspace_bytes, rows, kD, splits);
 
-  // the caches as (D, Hkv, cache_rows, B): a box (64, 1, 64, 1) is 64 keys x 64 dims of one head of one request
+  // the caches as (128 dims, Hkv, keys[, B]) with a box of 128 B of dims x 1 head x 64 keys: paged (keys = num_blocks *
+  // page, a box lies inside one page), contiguous (keys = cache_rows, 4-D with the batch stride), e4m3 paged (UINT8)
+  const bool contig = layout == KvLayout::kContiguous, e4m3 = layout == KvLayout::kPagedE4m3;
+  const int esize = e4m3 ? 1 : 2;
+  const cuuint64_t dims[4] = {(cuuint64_t)kD, (cuuint64_t)Hkv,
+                              contig ? (cuuint64_t)cache_rows : (cuuint64_t)num_blocks * page_size, (cuuint64_t)B};
+  const cuuint64_t strides[3] = {(cuuint64_t)kD * esize, (cuuint64_t)Hkv * kD * esize,
+                                 (cuuint64_t)rows_sb * Hkv * kD * esize};
+  const CUtensorMapDataType tdt = e4m3              ? CU_TENSOR_MAP_DATA_TYPE_UINT8
+                                  : dtype == CB_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                                                     : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
   CUtensorMap mk, mv;
-  const cuuint64_t dims[4] = {(cuuint64_t)kD, (cuuint64_t)Hkv, (cuuint64_t)cache_rows, (cuuint64_t)B};
-  const cuuint64_t strides[3] = {(cuuint64_t)kD * 2, (cuuint64_t)Hkv * kD * 2, (cuuint64_t)rows_sb * Hkv * kD * 2};
-  int rc = make_tma_map_nd(&mk, k_cache, 4, dims, strides, 2, tma_dtype(dtype), kTile);
-  if (!rc) rc = make_tma_map_nd(&mv, v_cache, 4, dims, strides, 2, tma_dtype(dtype), kTile);
+  int rc = make_tma_map_nd(&mk, k_cache, contig ? 4 : 3, dims, strides, esize, tdt, kTile);
+  if (!rc) rc = make_tma_map_nd(&mv, v_cache, contig ? 4 : 3, dims, strides, esize, tdt, kTile);
   if (rc) return rc;
 
   if (k_new) {                                              // the sq new k / v rows first
-    launch_contiguous_append({k_cache, k_new, k_new_sb * 2, k_new_st * 2}, {v_cache, v_new, v_new_sb * 2, v_new_st * 2},
-                             (int64_t)Hkv * kD * 2, cache_seqlens, rows_sb, cache_rows, B, sq, st);
-    CB_LAUNCHED(1);
+    const PagedAppend kc{k_cache, k_new, k_new_sb * 2, k_new_st * 2}, vc{v_cache, v_new, v_new_sb * 2, v_new_st * 2};
+    if (contig)
+      launch_contiguous_append(kc, vc, (int64_t)Hkv * kD * 2, cache_seqlens, rows_sb, cache_rows, B, sq, st);
+    else if (e4m3)
+      launch_paged_append_e4m3(kc, vc, Hkv * kD, dtype, cache_seqlens, block_table, bt_stride, B, sq, page_size, st);
+    else                                                    // true page indexing
+      launch_paged_append(kc, vc, (int64_t)Hkv * kD * 2, cache_seqlens, block_table, bt_stride, B, sq, page_size,
+                          page_size, st);
+    CB_LAUNCHED_AS(name, 1);
   }
 
-  const size_t smem = 1024 + (size_t)kSmemBytes;
-  const dim3 grid(row_tiles * splits, Hkv, B);
-#define LAUNCH_PREFILL(T, GG)                                                                                     \
-  do {                                                                                                            \
-    static bool attr = false;                                                                                     \
-    if (!attr) {                                                                                                  \
-      CB_CUDA(cudaFuncSetAttribute(gqa_prefill_contig_kernel<T, GG>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
-                                   (int)smem));                                                                   \
-      attr = true;                                                                                                \
-    }                                                                                                             \
-    launch_k(gqa_prefill_contig_kernel<T, GG>, grid, dim3(kThreads), smem, st, mk, mv, (const T*)q, cache_seqlens, \
-             sq, Hq, Hkv, k_new ? 1 : 0, causal ? 1 : 0, softmax_scale, row_tiles, splits, o_part, lse, (T*)out);  \
-  } while (0)
-#define DISPATCH_PREFILL(T)                \
-  switch (G) {                             \
-    case 1: LAUNCH_PREFILL(T, 1); break;   \
-    case 2: LAUNCH_PREFILL(T, 2); break;   \
-    case 4: LAUNCH_PREFILL(T, 4); break;   \
-    default: LAUNCH_PREFILL(T, 8); break;  \
-  }
-  if (dtype == CB_BF16) { DISPATCH_PREFILL(__nv_bfloat16); } else { DISPATCH_PREFILL(__half); }
-#undef DISPATCH_PREFILL
-#undef LAUNCH_PREFILL
-  CB_LAUNCHED(1);
-  if (splits > 1) {
-    rc = launch_merge_splits(o_part, lse, out, B * sq * Hq, splits, kD, dtype, st);
-    if (rc) return rc;
-    CB_LAUNCHED(1);
-  }
-  return 0;
-}
-
-// The multi-token path of chitu_b200_gqa_paged_attn_fp8kv (attention.cu), which has checked the arguments.
-int gqa_paged_prefill_e4m3(const void* q, void* k_cache, void* v_cache, const void* k_new, const void* v_new,
-                           int64_t k_new_sb, int64_t k_new_st, int64_t v_new_sb, int64_t v_new_st,
-                           const int32_t* cache_seqlens, const int32_t* block_table, int bt_stride, int B, int sq,
-                           int Hq, int Hkv, int page_size, int num_blocks, int max_len, int causal, float softmax_scale,
-                           void* out, void* workspace, int64_t workspace_bytes, int dtype, cudaStream_t st) {
-  if (!tma_available()) return fail(-3, "gqa_paged_attn_fp8kv: TMA is not available");
-  const int G = Hq / Hkv;
-  const int row_tiles = cdiv((int64_t)sq * G, kRows);
-  const int64_t rows = (int64_t)B * sq * Hq;
-  const int splits = prefill_splits(row_tiles, Hkv, B, rows, max_len, workspace, workspace_bytes);
-  if ((int64_t)row_tiles * splits > INT_MAX)
-    return fail(-1, "gqa_paged_attn_fp8kv: %d row tiles x %d splits exceed the grid", row_tiles, splits);
-  const auto [o_part, lse, plan] = split_kv_carve(splits > 1 ? workspace : nullptr, workspace_bytes, rows, kD, splits);
-
-  // the caches as bytes (128, Hkv, num_blocks * page): a box (128, 1, 64) is 64 keys x 128 dims of one head in one page
-  CUtensorMap mk, mv;
-  const cuuint64_t dims[3] = {(cuuint64_t)kD, (cuuint64_t)Hkv, (cuuint64_t)num_blocks * page_size};
-  const cuuint64_t strides[2] = {(cuuint64_t)kD, (cuuint64_t)Hkv * kD};
-  int rc = make_tma_map_nd(&mk, k_cache, 3, dims, strides, 1, CU_TENSOR_MAP_DATA_TYPE_UINT8, kTile);
-  if (!rc) rc = make_tma_map_nd(&mv, v_cache, 3, dims, strides, 1, CU_TENSOR_MAP_DATA_TYPE_UINT8, kTile);
+  const int smem = 1024 + kSmemBytes;
+  const dim3 grid(row_tiles * splits, Hkv, B), block(kThreads);
+  const int appended = k_new ? 1 : 0;
+  causal = causal ? 1 : 0;
+  rc = dispatch_io_g(dtype, G, [&](auto t, auto g) {
+    using T = decltype(t);
+    constexpr int GG = decltype(g)::value;
+    const T* qt = (const T*)q;
+    float *op = part.o_part, *lse = part.lse;
+    if (contig)
+      return launch_smem<gqa_prefill_contig_kernel<T, GG>>(entry, grid, block, smem, st, mk, mv, qt, cache_seqlens, sq,
+                                                           Hq, Hkv, appended, causal, softmax_scale, row_tiles, splits,
+                                                           op, lse, (T*)out);
+    if (e4m3)
+      return launch_smem<gqa_prefill_e4m3_kernel<T, GG>>(entry, grid, block, smem, st, mk, mv, qt, cache_seqlens,
+                                                         block_table, bt_stride, sq, Hq, Hkv, page_size, appended,
+                                                         causal, softmax_scale, row_tiles, splits, op, lse, (T*)out);
+    return launch_smem<gqa_prefill_kernel<T, GG>>(entry, grid, block, smem, st, mk, mv, qt, cache_seqlens, block_table,
+                                                  bt_stride, sq, Hq, Hkv, page_size, appended, causal, softmax_scale,
+                                                  row_tiles, splits, op, lse, (T*)out);
+  });
   if (rc) return rc;
-
-  if (k_new) {                                              // the sq new k / v rows first, rounded to e4m3
-    launch_paged_append_e4m3({k_cache, k_new, k_new_sb * 2, k_new_st * 2}, {v_cache, v_new, v_new_sb * 2, v_new_st * 2},
-                             Hkv * kD, dtype, cache_seqlens, block_table, bt_stride, B, sq, page_size, st);
-    CB_LAUNCHED(1);
-  }
-
-  const size_t smem = 1024 + (size_t)kSmemBytes;
-  const dim3 grid(row_tiles * splits, Hkv, B);
-#define LAUNCH_PREFILL(T, GG)                                                                                     \
-  do {                                                                                                            \
-    static bool attr = false;                                                                                     \
-    if (!attr) {                                                                                                  \
-      CB_CUDA(cudaFuncSetAttribute(gqa_prefill_e4m3_kernel<T, GG>, cudaFuncAttributeMaxDynamicSharedMemorySize,   \
-                                   (int)smem));                                                                   \
-      attr = true;                                                                                                \
-    }                                                                                                             \
-    launch_k(gqa_prefill_e4m3_kernel<T, GG>, grid, dim3(kThreads), smem, st, mk, mv, (const T*)q, cache_seqlens,  \
-             block_table, bt_stride, sq, Hq, Hkv, page_size, k_new ? 1 : 0, causal ? 1 : 0, softmax_scale,        \
-             row_tiles, splits, o_part, lse, (T*)out);                                                            \
-  } while (0)
-#define DISPATCH_PREFILL(T)                \
-  switch (G) {                             \
-    case 1: LAUNCH_PREFILL(T, 1); break;   \
-    case 2: LAUNCH_PREFILL(T, 2); break;   \
-    case 4: LAUNCH_PREFILL(T, 4); break;   \
-    default: LAUNCH_PREFILL(T, 8); break;  \
-  }
-  if (dtype == CB_BF16) { DISPATCH_PREFILL(__nv_bfloat16); } else { DISPATCH_PREFILL(__half); }
-#undef DISPATCH_PREFILL
-#undef LAUNCH_PREFILL
-  CB_LAUNCHED(1);
+  CB_LAUNCHED_AS(name, 1);
   if (splits > 1) {
-    rc = launch_merge_splits(o_part, lse, out, B * sq * Hq, splits, kD, dtype, st);
+    rc = launch_merge_splits(part.o_part, part.lse, out, B * sq * Hq, splits, kD, dtype, st);
     if (rc) return rc;
-    CB_LAUNCHED(1);
+    CB_LAUNCHED_AS(name, 1);
   }
   return 0;
 }
@@ -522,76 +466,23 @@ extern "C" int chitu_b200_gqa_paged_prefill(const void* q, void* k_cache, void* 
                                             void* out, void* workspace, int64_t workspace_bytes, int dtype,
                                             void* stream) {
   using namespace cb;
-  CB_ARG(q && k_cache && v_cache && cache_seqlens && block_table && out);
-  CB_ARG((k_new == nullptr) == (v_new == nullptr));
+  if (int rc = check_gqa_operands(__func__, q, k_cache, v_cache, cache_seqlens, out, k_new, v_new, k_new_sb, k_new_st,
+                                  v_new_sb, v_new_st, true, dtype))
+    return rc;
+  CB_ARG(block_table);
   CB_ARG(B >= 0 && B <= 65535 && sq >= 1 && Hq > 0 && Hkv > 0 && Hkv <= 65535 && Hq % Hkv == 0);
   CB_ARG(bt_stride > 0 && num_blocks > 0);
   CB_ARG(D == kD);
   CB_ARG(page_size > 0 && page_size % kTile == 0 && (int64_t)num_blocks * page_size <= INT_MAX);
-  CB_ARG(dtype == CB_BF16 || dtype == CB_F16);
   const int G = Hq / Hkv;
   CB_ARG(G == 1 || G == 2 || G == 4 || G == 8);
   CB_ARG((int64_t)sq * Hq <= INT_MAX / kD);
-  CB_ARG(((uintptr_t)q | (uintptr_t)k_cache | (uintptr_t)v_cache | (uintptr_t)out | (uintptr_t)k_new |
-          (uintptr_t)v_new) % 16 == 0);
-  CB_ARG(k_new == nullptr || (k_new_sb % 8 == 0 && k_new_st % 8 == 0 && v_new_sb % 8 == 0 && v_new_st % 8 == 0));
   CB_ARG(workspace == nullptr || (uintptr_t)workspace % 16 == 0);
   if (B == 0) return 0;
-  if (!tma_available()) return fail(-3, "gqa_paged_prefill: TMA is not available");
-
-  const int row_tiles = cdiv((int64_t)sq * G, kRows);
   const int max_len = max_seqlen_hint > 0 ? max_seqlen_hint : bt_stride * page_size;
-  const int64_t rows = (int64_t)B * sq * Hq;
-  const int splits = prefill_splits(row_tiles, Hkv, B, rows, max_len, workspace, workspace_bytes);
-  if ((int64_t)row_tiles * splits > INT_MAX)
-    return fail(-1, "gqa_paged_prefill: %d row tiles x %d splits exceed the grid", row_tiles, splits);
-  const auto [o_part, lse, plan] = split_kv_carve(splits > 1 ? workspace : nullptr, workspace_bytes, rows, kD, splits);
-
-  // the caches as (D, Hkv, num_blocks * page): a box (64, 1, 64) is 64 keys x 64 dims of one head inside one page
-  CUtensorMap mk, mv;
-  const cuuint64_t dims[3] = {(cuuint64_t)kD, (cuuint64_t)Hkv, (cuuint64_t)num_blocks * page_size};
-  const cuuint64_t strides[2] = {(cuuint64_t)kD * 2, (cuuint64_t)Hkv * kD * 2};
-  int rc = make_tma_map_nd(&mk, k_cache, 3, dims, strides, 2, tma_dtype(dtype), kTile);
-  if (!rc) rc = make_tma_map_nd(&mv, v_cache, 3, dims, strides, 2, tma_dtype(dtype), kTile);
-  if (rc) return rc;
-
-  cudaStream_t st = (cudaStream_t)stream;
-  if (k_new) {                                              // the sq new k / v rows first, true page indexing
-    launch_paged_append({k_cache, k_new, k_new_sb * 2, k_new_st * 2}, {v_cache, v_new, v_new_sb * 2, v_new_st * 2},
-                        (int64_t)Hkv * kD * 2, cache_seqlens, block_table, bt_stride, B, sq, page_size, page_size, st);
-    CB_LAUNCHED(1);
-  }
-
-  const size_t smem = 1024 + (size_t)kSmemBytes;
-  const dim3 grid(row_tiles * splits, Hkv, B);
-#define LAUNCH_PREFILL(T, GG)                                                                                     \
-  do {                                                                                                            \
-    static bool attr = false;                                                                                     \
-    if (!attr) {                                                                                                  \
-      CB_CUDA(cudaFuncSetAttribute(gqa_prefill_kernel<T, GG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-      attr = true;                                                                                                \
-    }                                                                                                             \
-    launch_k(gqa_prefill_kernel<T, GG>, grid, dim3(kThreads), smem, st, mk, mv, (const T*)q, cache_seqlens,       \
-             block_table, bt_stride, sq, Hq, Hkv, page_size, k_new ? 1 : 0, causal ? 1 : 0, softmax_scale,        \
-             row_tiles, splits, o_part, lse, (T*)out);                                                            \
-  } while (0)
-#define DISPATCH_PREFILL(T)                \
-  switch (G) {                             \
-    case 1: LAUNCH_PREFILL(T, 1); break;   \
-    case 2: LAUNCH_PREFILL(T, 2); break;   \
-    case 4: LAUNCH_PREFILL(T, 4); break;   \
-    default: LAUNCH_PREFILL(T, 8); break;  \
-  }
-  if (dtype == CB_BF16) { DISPATCH_PREFILL(__nv_bfloat16); } else { DISPATCH_PREFILL(__half); }
-#undef DISPATCH_PREFILL
-#undef LAUNCH_PREFILL
-  CB_LAUNCHED(1);
-  if (splits > 1) {
-    rc = launch_merge_splits(o_part, lse, out, B * sq * Hq, splits, kD, dtype, st);
-    if (rc) return rc;
-    CB_LAUNCHED(1);
-  }
-  return 0;
+  return gqa_prefill(__func__, __func__, KvLayout::kPaged, q, k_cache, v_cache, k_new, v_new, k_new_sb, k_new_st,
+                     v_new_sb, v_new_st, cache_seqlens, block_table, bt_stride, page_size, num_blocks, 0, 0, B, sq, Hq,
+                     Hkv, max_len, causal, softmax_scale, out, workspace, workspace_bytes, dtype, (cudaStream_t)stream);
 }
 
 CB_DEFINE_TL_SETTER(gqa_prefill)

@@ -422,14 +422,10 @@ extern "C" int chitu_b200_mla_prefill(const void* q, const void* k, int64_t k_sb
   if (!rc) rc = make_tma_map_2d(&mk, k, krows, kRow, 2, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, kTile, k_sb);
   if (!rc) rc = make_tma_map_2d(&mv, v, krows, kC, 2, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, kTile, v_sb);
   if (rc) return rc;
-  const size_t smem = 1024 + (size_t)kSmemBytes;
-  static bool attr = false;
-  if (!attr) {
-    CB_CUDA(cudaFuncSetAttribute(mla_prefill_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr = true;
-  }
-  launch_k(mla_prefill_kernel, dim3(row_tiles * B), dim3(kThreads), smem, (cudaStream_t)stream, mq, mk, mv, cu_seqlens_q,
-           cu_seqlens_k, B, H, row_tiles, causal ? 1 : 0, softmax_scale, (__nv_bfloat16*)out);
+  rc = launch_smem<mla_prefill_kernel>(__func__, dim3(row_tiles * B), dim3(kThreads), 1024 + kSmemBytes,
+                                       (cudaStream_t)stream, mq, mk, mv, cu_seqlens_q, cu_seqlens_k, B, H, row_tiles,
+                                       causal ? 1 : 0, softmax_scale, (__nv_bfloat16*)out);
+  if (rc) return rc;
   CB_LAUNCHED(1);
   return 0;
 }
@@ -476,15 +472,11 @@ extern "C" int chitu_b200_mla_paged_prefill(const void* q_nope, const void* q_pe
                         bt_stride, B, sq, kTile, 64, st);
     CB_LAUNCHED(1);
   }
-  const size_t smem = 1024 + (size_t)kSmemBytes;
-  static bool attr = false;
-  if (!attr) {
-    CB_CUDA(cudaFuncSetAttribute(mla_paged_prefill_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr = true;
-  }
-  launch_k(mla_paged_prefill_kernel, dim3(row_tiles * splits * B), dim3(kThreads), smem, st, mqn, mqp, mkv,
-           seqlens_excl, block_table, bt_stride, B, sq, H, new_kv ? 1 : 0, row_tiles, splits, causal ? 1 : 0,
-           softmax_scale, o_part, lse, (__nv_bfloat16*)out);
+  rc = launch_smem<mla_paged_prefill_kernel>(__func__, dim3(row_tiles * splits * B), dim3(kThreads),
+                                             1024 + kSmemBytes, st, mqn, mqp, mkv, seqlens_excl, block_table, bt_stride,
+                                             B, sq, H, new_kv ? 1 : 0, row_tiles, splits, causal ? 1 : 0,
+                                             softmax_scale, o_part, lse, (__nv_bfloat16*)out);
+  if (rc) return rc;
   CB_LAUNCHED(1);
   if (splits > 1) {
     rc = launch_merge_splits(o_part, lse, out, (int)rows, splits, kC, CB_BF16, st);

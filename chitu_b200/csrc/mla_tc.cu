@@ -405,16 +405,13 @@ extern "C" int chitu_b200_mla_decode(const void* q_nope, const void* q_pe, void*
   // the cache as a 2-D [num_rows, 576] bf16 tensor, box = [64 rows x 64 elements (128 B)]
   int rc = make_tma_map_2d(&map, kv_cache, (int64_t)num_blocks * kTile, kRow, 2, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, kTile);
   if (rc) return rc;
-  const size_t smem = 1024 + (size_t)kSmemBytes;
-  static bool attr = false;
-  if (!attr) {
-    CB_CUDA(cudaFuncSetAttribute(mla_decode_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr = true;
-  }
   dim3 grid(splits, cdiv(H, 16), B);
-  launch_k(mla_decode_tc_kernel, grid, dim3(kThreads), smem, st, map, (const __nv_bfloat16*)q_nope,
-           (const __nv_bfloat16*)q_pe, (__nv_bfloat16*)kv_cache, (const __nv_bfloat16*)new_kv, seqlens_excl, block_table,
-           bt_stride, H, softmax_scale, splits, o_part, lse, (__nv_bfloat16*)out, plan);
+  rc = launch_smem<mla_decode_tc_kernel>(__func__, grid, dim3(kThreads), 1024 + kSmemBytes, st, map,
+                                         (const __nv_bfloat16*)q_nope, (const __nv_bfloat16*)q_pe,
+                                         (__nv_bfloat16*)kv_cache, (const __nv_bfloat16*)new_kv, seqlens_excl,
+                                         block_table, bt_stride, H, softmax_scale, splits, o_part, lse,
+                                         (__nv_bfloat16*)out, plan);
+  if (rc) return rc;
   CB_LAUNCHED(1);
   if (splits > 1 && out) {
     rc = launch_merge_splits(o_part, lse, out, B * H, splits, kC, CB_BF16, st);
