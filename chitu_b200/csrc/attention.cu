@@ -1017,14 +1017,9 @@ __global__ void __launch_bounds__(256) mla_absorb_o_kernel(const __nv_bfloat16* 
         *reinterpret_cast<uint2*>(out + o) = make_uint2(pack2(v[0], v[1], tag), pack2(v[2], v[3], tag));
       }
       if (q_out) {
-        float amax = fmaxf(fmaxf(fabsf(v[0]), fabsf(v[1])), fmaxf(fabsf(v[2]), fabsf(v[3])));
-        amax = warp_max(amax);
-        const float sc = __fdiv_rn(amax, 448.0f);
-        uint32_t packed = 0;
-#pragma unroll
-        for (int i = 0; i < 4; ++i) packed |= (uint32_t)float_to_fp8(__fdiv_rn(v[i], sc)) << (8 * i);
-        *reinterpret_cast<uint32_t*>(q_out + o) = packed;
-        if (lane == 0) q_scales[((int64_t)(b0 + m) * H + h) * (dv / 128) + d0 / 128] = sc;
+        const E4m3Word g = e4m3_group_quant<E4m3Group::kActQuant>(v);
+        *reinterpret_cast<uint32_t*>(q_out + o) = g.bits;
+        if (lane == 0) q_scales[((int64_t)(b0 + m) * H + h) * (dv / 128) + d0 / 128] = g.scale;
       }
     }
   }

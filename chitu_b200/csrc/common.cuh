@@ -105,17 +105,24 @@ inline cudaError_t launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, siz
   return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
 }
 
-// launch_k of kernel K with `smem` bytes of dynamic shared memory, after raising K's limit to `smem` on its first
-// launch.  The flag is keyed on K itself (two instances with one signature get one each), set by a thread-safe static
-// initializer, and keeps the outcome: a failed limit is reported under `name` by every call.  Launch errors are left
-// to CB_LAUNCHED.
-template <auto K, typename... Args>
-inline int launch_smem(const char* name, dim3 grid, dim3 block, int smem, cudaStream_t st, Args&&... args) {
-  static const cudaError_t limit = cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-  if (limit != cudaSuccess)
-    return fail((int)limit, "%s: cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed: %s", name,
-                cudaGetErrorString(limit));
-  launch_k(K, grid, block, (size_t)smem, st, std::forward<Args>(args)...);
+// launch_k of kernel K with `smem` bytes of dynamic shared memory, after raising K's limit once: with Bound = 0 to
+// `smem` on K's first launch (every launch of K asks the same), else to Bound, an upper bound of every launch of K, on
+// the first launch above the 48 KB default (raising it up front measured slower on the DeepSeek-R1 MoE step).
+// The flag is keyed on K itself (two instances with one signature get one each), set by a thread-safe static
+// initializer, and keeps the outcome: a failed limit, and a launch above Bound, are reported under `name` by every call.
+// Launch errors are left to CB_LAUNCHED.
+template <auto K, int Bound = 0, typename... Args>
+inline int launch_smem(const char* name, dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
+  if (Bound == 0 || smem > 48 * 1024) {
+    static const cudaError_t limit =
+        cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, Bound ? Bound : (int)smem);
+    if (limit != cudaSuccess)
+      return fail((int)limit, "%s: cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed: %s", name,
+                  cudaGetErrorString(limit));
+    if (Bound && smem > (size_t)Bound)
+      return fail((int)cudaErrorInvalidValue, "%s: %zu bytes of dynamic shared memory exceed %d", name, smem, Bound);
+  }
+  launch_k(K, grid, block, smem, st, std::forward<Args>(args)...);
   return 0;
 }
 
@@ -320,6 +327,27 @@ __device__ __forceinline__ float warp_max(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
   return v;
+}
+
+// ---- e4m3 group quantisation: one warp per 128-element group, 4 consecutive elements per lane ---------------------
+// scale = amax / 448 and q = v / scale, both divided as torch divides (__fdiv_rn), bit-exact with one of two references:
+// kActQuant (act_quant_deepseek_v3) takes amax as is and leaves q unclamped; kPerTokenGroup (per_token_group_quant_fp8)
+// floors amax at 1e-10 and clamps q to +-448, which also turns a NaN q (kept as NaN by float_to_fp8) into -448.
+enum class E4m3Group { kActQuant, kPerTokenGroup };
+struct E4m3Word { uint32_t bits; float scale; };    // the lane's element i in byte i; the group's scale, on every lane
+template <E4m3Group kRule>
+__device__ __forceinline__ E4m3Word e4m3_group_quant(const float (&v)[4]) {
+  float amax = warp_max(fmaxf(fmaxf(fabsf(v[0]), fabsf(v[1])), fmaxf(fabsf(v[2]), fabsf(v[3]))));
+  if constexpr (kRule == E4m3Group::kPerTokenGroup) amax = fmaxf(amax, 1e-10f);
+  const float sc = __fdiv_rn(amax, 448.0f);
+  uint32_t bits = 0;
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    float q = __fdiv_rn(v[i], sc);
+    if constexpr (kRule == E4m3Group::kPerTokenGroup) q = fminf(fmaxf(q, -448.f), 448.f);
+    bits |= (uint32_t)float_to_fp8(q) << (8 * i);
+  }
+  return {bits, sc};
 }
 
 }  // namespace cb

@@ -295,14 +295,9 @@ __global__ void __launch_bounds__(256) rmsnorm_quant_kernel(const __nv_bfloat16*
         *reinterpret_cast<uint2*>(y + row * y_stride + e) = make_uint2(pack2(o[0], o[1], tag), pack2(o[2], o[3], tag));
       }
       if (q) {                                      // a warp covers exactly one 128-element group
-        float amax = fmaxf(fmaxf(fabsf(o[0]), fabsf(o[1])), fmaxf(fabsf(o[2]), fabsf(o[3])));
-        amax = warp_max(amax);
-        const float sc = __fdiv_rn(amax, 448.0f);
-        uint32_t packed = 0;
-#pragma unroll
-        for (int i = 0; i < 4; ++i) packed |= (uint32_t)float_to_fp8(__fdiv_rn(o[i], sc)) << (8 * i);
-        *reinterpret_cast<uint32_t*>(q + row * dim + e) = packed;
-        if (lane == 0) qs[row * (dim / 128) + (e >> 7)] = sc;
+        const E4m3Word g = e4m3_group_quant<E4m3Group::kActQuant>(o);
+        *reinterpret_cast<uint32_t*>(q + row * dim + e) = g.bits;
+        if (lane == 0) qs[row * (dim / 128) + (e >> 7)] = g.scale;
       }
     }
   }
@@ -345,14 +340,9 @@ __global__ void silu_mul_quant_kernel(const __nv_bfloat16* __restrict__ x, uint8
     const float sl = __bfloat162float(__float2bfloat16_rn(gv[i] / (1.f + expf(-gv[i]))));
     v[i] = __bfloat162float(__float2bfloat16_rn(sl * uv[i]));
   }
-  float amax = fmaxf(fmaxf(fabsf(v[0]), fabsf(v[1])), fmaxf(fabsf(v[2]), fabsf(v[3])));
-  amax = warp_max(amax);
-  const float sc = __fdiv_rn(amax, 448.0f);
-  uint32_t packed = 0;
-#pragma unroll
-  for (int i = 0; i < 4; ++i) packed |= (uint32_t)float_to_fp8(__fdiv_rn(v[i], sc)) << (8 * i);
-  *reinterpret_cast<uint32_t*>(q + r * F + gk * 128 + lane * 4) = packed;
-  if (lane == 0) qs[r * groups + gk] = sc;
+  const E4m3Word g = e4m3_group_quant<E4m3Group::kActQuant>(v);
+  *reinterpret_cast<uint32_t*>(q + r * F + gk * 128 + lane * 4) = g.bits;
+  if (lane == 0) qs[r * groups + gk] = g.scale;
 }
 
 extern "C" int chitu_b200_silu_mul_quant_fp8(const void* x, void* q, float* q_scales, int64_t rows, int F,

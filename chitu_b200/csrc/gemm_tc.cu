@@ -637,12 +637,8 @@ int launch_epi(const CUtensorMap& mw, const CUtensorMap& mx, Params& p, int grid
   using C = Cfg<KIND, BN>;
   size_t smem = 1024 + (size_t)C::kStages * C::kStageBytes + (size_t)C::kCvtStages * C::kCvtBytes;
   // opt-in dynamic shared memory: static (barriers, tile geometry) + dynamic must stay within 227 KB
-  static size_t attr_bytes = 0;
-  if (smem > attr_bytes) {
-    CB_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<KIND, BN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_bytes = smem;
-  }
-  cb::launch_k(tc_gemm_kernel<KIND, BN, EPI>, dim3(grid), dim3(C::kThreads), smem, st, mw, mx, p);
+  const int rc = launch_smem<tc_gemm_kernel<KIND, BN, EPI>>(__func__, dim3(grid), dim3(C::kThreads), smem, st, mw, mx, p);
+  if (rc) return rc;
   CB_LAUNCHED(1);
   return 0;
 }

@@ -55,7 +55,7 @@ __device__ __forceinline__ void mprobe(int) {}
 // The plan itself, run by one CTA of kPlanThreads threads.  `sm` needs moe_plan_smem_ints(P, E) ints.  E <= kPlanThreads:
 // a thread owns one expert in the block-wide scans.
 constexpr int kPlanThreads = 1024;
-__host__ __device__ inline int64_t moe_plan_smem_ints(int64_t P, int E) { return 3 * (int64_t)E + 2 + 2 * P + 2 * (E + P / 16 + 2); }
+__host__ __device__ constexpr int64_t moe_plan_smem_ints(int64_t P, int E) { return 3 * (int64_t)E + 2 + 2 * P + 2 * (E + P / 16 + 2); }
 
 template <typename IdT>
 __device__ __forceinline__ void moe_plan_large(const IdT* ids, const void* topk_w, int topk_w_f32,
@@ -713,18 +713,10 @@ __global__ void moe_gather_quant_kernel(const __nv_bfloat16* __restrict__ x, con
     *reinterpret_cast<uint2*>(xb + (int64_t)r * K + gk * 128 + lane * 4) = raw;
     return;
   }
-  float v[4] = {bf16lo(raw.x), bf16hi(raw.x), bf16lo(raw.y), bf16hi(raw.y)};
-  float amax = fmaxf(fmaxf(fabsf(v[0]), fabsf(v[1])), fmaxf(fabsf(v[2]), fabsf(v[3])));
-  amax = fmaxf(warp_max(amax), 1e-10f);
-  const float sc = __fdiv_rn(amax, 448.0f);
-  uint32_t packed = 0;
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    float q = fminf(fmaxf(__fdiv_rn(v[i], sc), -448.f), 448.f);
-    packed |= (uint32_t)float_to_fp8(q) << (8 * i);
-  }
-  *reinterpret_cast<uint32_t*>(xq + (int64_t)r * K + gk * 128 + lane * 4) = packed;
-  if (lane == 0) xs[(int64_t)r * groups + gk] = sc;
+  const float v[4] = {bf16lo(raw.x), bf16hi(raw.x), bf16lo(raw.y), bf16hi(raw.y)};
+  const E4m3Word g = e4m3_group_quant<E4m3Group::kPerTokenGroup>(v);
+  *reinterpret_cast<uint32_t*>(xq + (int64_t)r * K + gk * 128 + lane * 4) = g.bits;
+  if (lane == 0) xs[(int64_t)r * groups + gk] = g.scale;
 }
 
 // a2 = SiluAndMul(c1) in sorted space, then per_token_group_quant_fp8 (or bf16 copy)
@@ -752,17 +744,9 @@ __global__ void moe_silu_quant_kernel(const __nv_bfloat16* __restrict__ c1, cons
     *reinterpret_cast<uint2*>(ab + (int64_t)r * F + gk * 128 + lane * 4) = o;
     return;
   }
-  float amax = fmaxf(fmaxf(fabsf(v[0]), fabsf(v[1])), fmaxf(fabsf(v[2]), fabsf(v[3])));
-  amax = fmaxf(warp_max(amax), 1e-10f);
-  const float sc = __fdiv_rn(amax, 448.0f);
-  uint32_t packed = 0;
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    float q = fminf(fmaxf(__fdiv_rn(v[i], sc), -448.f), 448.f);
-    packed |= (uint32_t)float_to_fp8(q) << (8 * i);
-  }
-  *reinterpret_cast<uint32_t*>(aq + (int64_t)r * F + gk * 128 + lane * 4) = packed;
-  if (lane == 0) as[(int64_t)r * groups + gk] = sc;
+  const E4m3Word g = e4m3_group_quant<E4m3Group::kPerTokenGroup>(v);
+  *reinterpret_cast<uint32_t*>(aq + (int64_t)r * F + gk * 128 + lane * 4) = g.bits;
+  if (lane == 0) as[(int64_t)r * groups + gk] = g.scale;
 }
 
 // out[t,:] = sum_j c3[pos[t*topk+j], :]   (torch.sum(dim=1) on bf16: fp32 accumulate, one rounding)
@@ -800,11 +784,107 @@ __global__ void moe_combine_kernel(const __nv_bfloat16* __restrict__ c3, const i
   }
 }
 
+// moe_gate_kernel's dynamic shared memory grows with dim and E, so its bound is the device's: the 227 KB a block may
+// opt into on sm_90, less the kernel's 32 bytes of static shared memory (`red`).
+constexpr int kGateSmemBound = 227 * 1024 - 32;
+// The grouped path's plan: E <= kPlanThreads and P <= kPlanMaxPairs keep its shared memory within kPlanSmemBound.
+constexpr int kPlanMaxPairs = 8192;
+constexpr int kPlanSmemBound = (int)(moe_plan_smem_ints(kPlanMaxPairs, kPlanThreads) * sizeof(int));
+
+// ---- workspace layouts --------------------------------------------------------------------------------------------
+// Each layout carves its workspace from `base` in order, or with base == nullptr only measures it; `end` is the size
+// the *_workspace_bytes entries are built from.  Every array starts on a 256-byte boundary.
+struct Carve {
+  uintptr_t base;
+  int64_t end = 0;
+  template <typename T>
+  T* take(int64_t bytes) {
+    T* p = reinterpret_cast<T*>(base + end);
+    end += align256(bytes);
+    return p;
+  }
+};
+
+// moe_gate: the logits GEMM's scratch (ticket counters first: they must stay zero between calls), then the logits.
+struct GateWs : Carve {
+  __nv_bfloat16* logits;
+  GateWs(void* base, int T, int E) : Carve{(uintptr_t)base} {
+    take<void>(cb::tc_workspace_bytes(T, E));
+    logits = take<__nv_bfloat16>((int64_t)T * E * 2);
+  }
+};
+
+// moe_grouped_gemm: the grouped GEMM's scratch, out_rows, row_scale, the tile count, three tile lists of `tiles`
+// entries, then the gathered rows (fp8 or bf16) and their scales.
+struct BlocksWs : Carve {
+  int64_t tiles;
+  int *out_rows, *num_tiles, *t_w, *t_x, *t_c;
+  float *row_scale, *xs_s;
+  uint8_t* xs;
+  BlocksWs(void* base, int EM, int N, int K) : Carve{(uintptr_t)base}, tiles(((int64_t)EM / 16 + 1) * (N / 128 + 1)) {
+    take<void>(cb::tc_workspace_bytes(128, 128));
+    out_rows = take<int>((int64_t)EM * 4);
+    row_scale = take<float>((int64_t)EM * 4);
+    num_tiles = take<int>(4);
+    t_w = take<int>(tiles * 4);
+    t_x = take<int>(tiles * 4);
+    t_c = take<int>(tiles * 4);
+    xs = take<uint8_t>((int64_t)EM * K * 2);
+    xs_s = take<float>((int64_t)EM * (K / 128 + 1) * 4);
+  }
+};
+
+// fused_experts, grouped path: the grouped GEMMs' scratch (tickets + partials, zeroed once), the plan, then in sorted
+// row order xs (fp8 or bf16) and its scales, c1, a2 (fp8 or bf16) and its scales, c3.
+struct GroupedWs : Carve {
+  MoePlan pl;
+  uint8_t *xs, *a2;
+  float *xs_s, *a2_s;
+  __nv_bfloat16 *c1, *c3;
+  GroupedWs(void* base, int64_t P, int E, int N1, int K1) : Carve{(uintptr_t)base} {
+    const int64_t chunks = E + P / 16 + 1;                  // row chunks of >= 16 sorted rows
+    take<void>(cb::tc_workspace_bytes(128, 128));
+    int* ip = take<int>((P + P + (E + 1) + 2 + P) * 4);     // pair_sorted, pos, seg_start, counts, w_sorted
+    pl.pair_sorted = ip; pl.pos = ip + P; pl.seg_start = ip + 2 * P; pl.num_tiles1 = ip + 2 * P + E + 1;
+    pl.num_tiles2 = pl.num_tiles1 + 1; pl.w_sorted = (float*)(ip + 2 * P + E + 3);
+    int* t1 = take<int>(chunks * (N1 / 128 + 1) * 3 * 4);
+    pl.tile1_wrow = t1; pl.tile1_xrow = t1 + chunks * (N1 / 128); pl.tile1_cnt = t1 + 2 * chunks * (N1 / 128);
+    int* t2 = take<int>(chunks * (K1 / 128 + 1) * 3 * 4);
+    pl.tile2_wrow = t2; pl.tile2_xrow = t2 + chunks * (K1 / 128); pl.tile2_cnt = t2 + 2 * chunks * (K1 / 128);
+    xs = take<uint8_t>(P * K1 * 2);
+    xs_s = take<float>(P * (K1 / 128 + 1) * 4);
+    c1 = take<__nv_bfloat16>(P * N1 * 2);
+    a2 = take<uint8_t>(P * (N1 / 2) * 2);
+    a2_s = take<float>(P * (N1 / 2 / 128 + 1) * 4);
+    c3 = take<__nv_bfloat16>(P * K1 * 2);
+  }
+};
+
+// fused_experts, pair-GEMV path: after the grouped GEMMs' scratch (its ticket counters must stay zero), x quantised
+// and its scales (mode 1), c1, a2, a2 quantised and its scales (mode 1), c3.
+struct PairWs : Carve {
+  uint8_t *a1_q, *a2_q;
+  float *a1_s, *a2_s;
+  __nv_bfloat16 *c1, *a2, *c3;
+  PairWs(void* base, int T, int64_t P, int N1, int K1) : Carve{(uintptr_t)base} {
+    take<void>(cb::tc_workspace_bytes(128, 128));
+    a1_q = take<uint8_t>((int64_t)T * K1);
+    a1_s = take<float>((int64_t)T * (K1 / 128 + 1) * 4);
+    c1 = take<__nv_bfloat16>(P * N1 * 2);
+    a2 = take<__nv_bfloat16>(P * (N1 / 2) * 2);
+    a2_q = take<uint8_t>(P * (N1 / 2));
+    a2_s = take<float>(P * (N1 / 2 / 128 + 1) * 4);
+    c3 = take<__nv_bfloat16>(P * K1 * 2);
+  }
+};
+
+// The grouped GEMM kind of a weight mode (0 bf16, 1 fp8 w8a8, 2 fp8 weights x bf16 activations); the pair-GEMV
+// kernel's MODE is the weight mode itself.
+int moe_gemm_kind(int wmode) { return wmode == 1 ? cb::KIND_FP8 : (wmode == 2 ? cb::KIND_SOFT : cb::KIND_16); }
+
 }  // namespace
 
-extern "C" int64_t chitu_b200_moe_gate_workspace_bytes(int T, int E) {
-  return align256(cb::tc_workspace_bytes(T, E)) + align256((int64_t)T * E * 2);
-}
+extern "C" int64_t chitu_b200_moe_gate_workspace_bytes(int T, int E) { return GateWs(nullptr, T, E).end; }
 
 extern "C" int chitu_b200_moe_gate(const void* x, const void* w, const void* bias, int bias_dtype, int T,
                                    int dim, int E, int n_groups, int topk_groups, int topk,
@@ -821,34 +901,29 @@ extern "C" int chitu_b200_moe_gate(const void* x, const void* w, const void* bia
   // re-read the 3.67 MB gate matrix once per token: 360 us per layer at bs=16)
   const __nv_bfloat16* logits = nullptr;
   if (workspace && workspace_bytes >= chitu_b200_moe_gate_workspace_bytes(T, E) && cb::tc_supported(cb::KIND_16, T, E, dim)) {
-    // layout: [GEMM scratch (ticket counters first: they must stay zero between calls) | logits]
-    const int64_t lin = cb::tc_workspace_bytes(T, E);
-    void* lg = (uint8_t*)workspace + align256(lin);
+    __nv_bfloat16* lg = GateWs(workspace, T, E).logits;
     if (T <= 16 && dim <= 256 * kGateVecIters * 8) {
       // decode batches: one CTA per pair of experts, no split-K (see gate_logits_kernel)
       const dim3 grid((E + 1) / 2), block(256);
       const __nv_bfloat16* xb = (const __nv_bfloat16*)x;
       const __nv_bfloat16* wb = (const __nv_bfloat16*)w;
-      if (T <= 1) cb::launch_k(gate_logits_kernel<1>, grid, block, 0, st, xb, wb, (__nv_bfloat16*)lg, T, dim, E);
-      else if (T <= 4) cb::launch_k(gate_logits_kernel<4>, grid, block, 0, st, xb, wb, (__nv_bfloat16*)lg, T, dim, E);
-      else if (T <= 8) cb::launch_k(gate_logits_kernel<8>, grid, block, 0, st, xb, wb, (__nv_bfloat16*)lg, T, dim, E);
-      else cb::launch_k(gate_logits_kernel<16>, grid, block, 0, st, xb, wb, (__nv_bfloat16*)lg, T, dim, E);
+      if (T <= 1) cb::launch_k(gate_logits_kernel<1>, grid, block, 0, st, xb, wb, lg, T, dim, E);
+      else if (T <= 4) cb::launch_k(gate_logits_kernel<4>, grid, block, 0, st, xb, wb, lg, T, dim, E);
+      else if (T <= 8) cb::launch_k(gate_logits_kernel<8>, grid, block, 0, st, xb, wb, lg, T, dim, E);
+      else cb::launch_k(gate_logits_kernel<16>, grid, block, 0, st, xb, wb, lg, T, dim, E);
       CB_LAUNCHED(1);
     } else {
-      int rc = cb::tc_linear16(x, w, nullptr, nullptr, lg, T, E, dim, CB_BF16, workspace, lin, st);
+      int rc = cb::tc_linear16(x, w, nullptr, nullptr, lg, T, E, dim, CB_BF16, workspace, cb::tc_workspace_bytes(T, E), st);
       if (rc) return rc;
     }
-    logits = (const __nv_bfloat16*)lg;
+    logits = lg;
   }
   const size_t smem = (size_t)dim * 2 + (size_t)(2 * E + n_groups) * 4 + (size_t)topk * 4 + 16;
-  static size_t attr_bytes = 48 * 1024;
-  if (smem > attr_bytes) {
-    CB_CUDA(cudaFuncSetAttribute(moe_gate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_bytes = smem;
-  }
-  cb::launch_k(moe_gate_kernel, dim3(T), dim3(256), smem, st, (const __nv_bfloat16*)x, (const __nv_bfloat16*)w, bias,
-               (int)(bias_dtype == CB_F32), dim, E, n_groups, topk_groups, topk, score_sigmoid, route_scale,
-               (__nv_bfloat16*)out_weights, out_indices, logits, out_stride);
+  const int rc = launch_smem<moe_gate_kernel, kGateSmemBound>(
+      __func__, dim3(T), dim3(256), smem, st, (const __nv_bfloat16*)x, (const __nv_bfloat16*)w, bias,
+      (int)(bias_dtype == CB_F32), dim, E, n_groups, topk_groups, topk, score_sigmoid, route_scale,
+      (__nv_bfloat16*)out_weights, out_indices, logits, out_stride);
+  if (rc) return rc;
   CB_LAUNCHED(1);
   return 0;
 }
@@ -921,27 +996,14 @@ __global__ void moe_rows_gather_kernel(const __nv_bfloat16* __restrict__ A, cons
     *reinterpret_cast<uint2*>(xb + (int64_t)r * K + gk * 128 + lane * 4) = raw;
     return;
   }
-  float v[4] = {bf16lo(raw.x), bf16hi(raw.x), bf16lo(raw.y), bf16hi(raw.y)};
-  float amax = fmaxf(fmaxf(fabsf(v[0]), fabsf(v[1])), fmaxf(fabsf(v[2]), fabsf(v[3])));
-  amax = fmaxf(warp_max(amax), 1e-10f);
-  const float sc = __fdiv_rn(amax, 448.0f);
-  uint32_t packed = 0;
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    float q = fminf(fmaxf(__fdiv_rn(v[i], sc), -448.f), 448.f);
-    packed |= (uint32_t)float_to_fp8(q) << (8 * i);
-  }
-  *reinterpret_cast<uint32_t*>(xq + (int64_t)r * K + gk * 128 + lane * 4) = packed;
-  if (lane == 0) xs[(int64_t)r * groups + gk] = sc;
+  const float v[4] = {bf16lo(raw.x), bf16hi(raw.x), bf16lo(raw.y), bf16hi(raw.y)};
+  const E4m3Word g = e4m3_group_quant<E4m3Group::kPerTokenGroup>(v);
+  *reinterpret_cast<uint32_t*>(xq + (int64_t)r * K + gk * 128 + lane * 4) = g.bits;
+  if (lane == 0) xs[(int64_t)r * groups + gk] = g.scale;
 }
 
 extern "C" int64_t chitu_b200_moe_grouped_gemm_workspace_bytes(int EM, int N, int K) {
-  int64_t b = align256(cb::tc_workspace_bytes(128, 128));
-  b += align256((int64_t)EM * 4) * 2;                                       // out_rows, row_scale
-  const int64_t tiles = ((int64_t)EM / 16 + 1) * (N / 128 + 1);
-  b += align256(tiles * 4) * 3 + 256;                                       // tile lists + count
-  b += align256((int64_t)EM * K * 2) + align256((int64_t)EM * (K / 128 + 1) * 4);   // gathered rows (+ scales)
-  return b + 256;
+  return BlocksWs(nullptr, EM, N, K).end + 256;
 }
 
 extern "C" int chitu_b200_moe_grouped_gemm(const void* A, const void* B, void* C, const float* B_scale, const void* topk_weights,
@@ -961,61 +1023,27 @@ extern "C" int chitu_b200_moe_grouped_gemm(const void* A, const void* B, void* C
   CB_ARG(workspace_bytes >= chitu_b200_moe_grouped_gemm_workspace_bytes(EM, N, K));
   if (!cb::tma_available()) return cb::fail(-3, "moe_grouped_gemm: TMA is not available");
   cudaStream_t st = (cudaStream_t)stream;
-  uint8_t* q = (uint8_t*)workspace;
-  void* gws = q;                       q += align256(cb::tc_workspace_bytes(128, 128));
-  int* out_rows = (int*)q;             q += align256((int64_t)EM * 4);
-  float* row_scale = (float*)q;        q += align256((int64_t)EM * 4);
-  const int64_t tiles = ((int64_t)EM / 16 + 1) * (N / 128 + 1);
-  CB_ARG(tiles <= cb::tc_max_tiles());
-  int* num_tiles = (int*)q;            q += 256;
-  int* t_w = (int*)q;                  q += align256(tiles * 4);
-  int* t_x = (int*)q;                  q += align256(tiles * 4);
-  int* t_c = (int*)q;                  q += align256(tiles * 4);
-  uint8_t* xs = q;                     q += align256((int64_t)EM * K * 2);
-  float* xs_s = (float*)q;
+  const BlocksWs ws(workspace, EM, N, K);
+  CB_ARG(ws.tiles <= cb::tc_max_tiles());
   const int quant = wmode == 1;
   cb::launch_k(moe_blocks_prepare_kernel, dim3(cdiv(EM, 256)), dim3(256), 0, st, sorted_token_ids, expert_ids,
                num_tokens_post_padded, EM, numel, block_m, E, N, topk_weights, (int)(topk_w_dtype == CB_F32),
-               mul_routed_weight, out_rows, row_scale, num_tiles, t_w, t_x, t_c);
+               mul_routed_weight, ws.out_rows, ws.row_scale, ws.num_tiles, ws.t_w, ws.t_x, ws.t_c);
   CB_LAUNCHED(1);
   cb::launch_k(moe_rows_gather_kernel, dim3(cdiv((int64_t)EM * (K / 128), 8)), dim3(256), 0, st, (const __nv_bfloat16*)A,
-               sorted_token_ids, expert_ids, num_tokens_post_padded, EM, numel, top_k, block_m, E, K, N, quant, xs, xs_s,
-               (__nv_bfloat16*)xs, (__nv_bfloat16*)C);
+               sorted_token_ids, expert_ids, num_tokens_post_padded, EM, numel, top_k, block_m, E, K, N, quant, ws.xs,
+               ws.xs_s, (__nv_bfloat16*)ws.xs, (__nv_bfloat16*)C);
   CB_LAUNCHED(1);
-  const int gkind = wmode == 1 ? cb::KIND_FP8 : (wmode == 2 ? cb::KIND_SOFT : cb::KIND_16);
-  return cb::tc_grouped_gemm(gkind, xs, xs_s, B, B_scale, C, EM, E, N, K, block_m, num_tiles, t_w, t_x, t_c,
-                             mul_routed_weight ? row_scale : nullptr, out_rows, gws, cb::tc_workspace_bytes(128, 128), st);
+  return cb::tc_grouped_gemm(moe_gemm_kind(wmode), ws.xs, ws.xs_s, B, B_scale, C, EM, E, N, K, block_m, ws.num_tiles,
+                             ws.t_w, ws.t_x, ws.t_c, mul_routed_weight ? ws.row_scale : nullptr, ws.out_rows, workspace,
+                             cb::tc_workspace_bytes(128, 128), st);
 }
 
 extern "C" int64_t chitu_b200_moe_workspace_bytes(int T, int topk, int E, int N1, int K1) {
   const int64_t P = (int64_t)T * topk;
-  int64_t b = 0;
-  // pair-GEMV path
-  b += align256((int64_t)T * K1);                    // a1_q
-  b += align256((int64_t)T * (K1 / 128 + 1) * 4);    // a1_s
-  b += align256(P * N1 * 2);                         // c1
-  b += align256(P * (N1 / 2) * 2);                   // a2
-  b += align256(P * (N1 / 2));                       // a2_q
-  b += align256(P * (N1 / 2 / 128 + 1) * 4);         // a2_s
-  b += align256(P * K1 * 2);                         // c3
-  // grouped wgmma path (laid out separately; see fused_experts)
-  int64_t g = align256(cb::tc_workspace_bytes(128, 128));                 // GEMM tickets + partials (zeroed once)
-  g += align256((P + P + (E + 1) + 2 + P) * 4);                           // pair_sorted, pos, seg_start, counts, w_sorted
-  const int64_t chunks = E + P / 16 + 1;                                  // row chunks of >= 16 sorted rows
-  g += align256(chunks * (N1 / 128 + 1) * 3 * 4) + align256(chunks * (K1 / 128 + 1) * 3 * 4);   // tile lists
-  g += align256(P * K1 * 2) + align256(P * (K1 / 128 + 1) * 4);           // xs (fp8 or bf16) + scales
-  g += align256(P * N1 * 2);                                              // c1 sorted
-  g += align256(P * (N1 / 2) * 2) + align256(P * (N1 / 2 / 128 + 1) * 4); // a2 (fp8 or bf16) + scales
-  g += align256(P * K1 * 2);                                              // c3 sorted
-  b += align256(cb::tc_workspace_bytes(128, 128));
-  return (b > g ? b : g) + 256;
+  const int64_t pair = PairWs(nullptr, T, P, N1, K1).end, grouped = GroupedWs(nullptr, P, E, N1, K1).end;
+  return (pair > grouped ? pair : grouped) + 256;
 }
-
-static int fused_experts_impl(const void* x, const void* w1, const void* w2, const float* w1_s,
-                              const float* w2_s, const void* topk_w, int topk_w_dtype,
-                              const void* topk_ids, int ids_dtype, int T, int topk, int E, int N1,
-                              int K1, int wmode, void* out, const void* residual, void* workspace,
-                              int64_t workspace_bytes, void* stream, void* comm);
 
 // rows per chunk (= wgmma N of the grouped GEMMs): twice the mean number of routed rows per expert, 16 .. 128
 static int moe_chunk_rows(int64_t P, int E) {
@@ -1023,18 +1051,103 @@ static int moe_chunk_rows(int64_t P, int E) {
   while (BN < 128 && BN < 2 * (int)((P + E - 1) / E)) BN *= 2;
   return BN;
 }
-// the plan's arrays inside the fused-experts workspace (after the grouped GEMM's scratch); returns the first free byte
-static uint8_t* moe_plan_layout(void* workspace, int64_t P, int E, int N1, int K1, MoePlan* pl) {
-  uint8_t* q = (uint8_t*)workspace + align256(cb::tc_workspace_bytes(128, 128));
-  int* ip = (int*)q;                          q += align256((P + P + (E + 1) + 2 + P) * 4);
-  pl->pair_sorted = ip; pl->pos = ip + P; pl->seg_start = ip + 2 * P; pl->num_tiles1 = ip + 2 * P + E + 1;
-  pl->num_tiles2 = pl->num_tiles1 + 1; pl->w_sorted = (float*)(ip + 2 * P + E + 3);
+
+static int fused_experts_impl(const void* x, const void* w1, const void* w2, const float* w1_s,
+                              const float* w2_s, const void* topk_w, int topk_w_dtype,
+                              const void* topk_ids, int ids_dtype, int T, int topk, int E, int N1,
+                              int K1, int wmode, void* out, const void* residual, void* workspace,
+                              int64_t workspace_bytes, void* stream, void* comm) {
+  CB_ARG(x && w1 && w2 && topk_w && topk_ids && (out || comm) && workspace);
+  CB_ARG(T >= 0 && topk > 0 && E > 0 && N1 > 0 && N1 % 2 == 0 && K1 > 0);
+  CB_ARG(wmode >= 0 && wmode <= 2);
+  CB_ARG(wmode == 0 || (w1_s && w2_s));
+  CB_ARG(topk_w_dtype == CB_BF16 || topk_w_dtype == CB_F32);
+  CB_ARG(ids_dtype == CB_I32 || ids_dtype == CB_I64);
+  CB_ARG(K1 % 16 == 0 && (N1 / 2) % 16 == 0);
+  if (wmode == 1) CB_ARG(K1 % 128 == 0 && (N1 / 2) % 128 == 0);
+  CB_ARG(workspace_bytes >= chitu_b200_moe_workspace_bytes(T, topk, E, N1, K1));
+  if (T == 0) return 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int64_t P = (int64_t)T * topk;
+  const int N2 = N1 / 2;
+  CB_ARG(P <= 65535);
+  const int w_f32 = topk_w_dtype == CB_F32, ids_i64 = ids_dtype == CB_I64;
+
+  // ---- grouped wgmma path: sort pairs by expert, stream every distinct expert once ----
+  const int BN = moe_chunk_rows(P, E);
   const int64_t chunks = E + P / 16 + 1;
-  int* t1 = (int*)q;                          q += align256(chunks * (N1 / 128 + 1) * 3 * 4);
-  pl->tile1_wrow = t1; pl->tile1_xrow = t1 + chunks * (N1 / 128); pl->tile1_cnt = t1 + 2 * chunks * (N1 / 128);
-  int* t2 = (int*)q;                          q += align256(chunks * (K1 / 128 + 1) * 3 * 4);
-  pl->tile2_wrow = t2; pl->tile2_xrow = t2 + chunks * (K1 / 128); pl->tile2_cnt = t2 + 2 * chunks * (K1 / 128);
-  return q;
+  if (P <= kPlanMaxPairs && E <= kPlanThreads && N1 % 256 == 0 && K1 % 128 == 0 && (wmode != 2 || (N1 / 2) % 128 == 0) &&
+      chunks * (N1 / 128) <= cb::tc_max_tiles() && chunks * (K1 / 128) <= cb::tc_max_tiles() && cb::tma_available()) {
+    const GroupedWs ws(workspace, P, E, N1, K1);
+    const MoePlan& pl = ws.pl;
+    const int quant = wmode == 1, gkind = moe_gemm_kind(wmode);
+    const size_t psm = (size_t)moe_plan_smem_ints(P, E) * sizeof(int);
+    int rc = ids_i64
+        ? launch_smem<moe_plan_kernel<int64_t>, kPlanSmemBound>(__func__, dim3(1), dim3(kPlanThreads), psm, st,
+                                                                (const int64_t*)topk_ids, topk_w, w_f32, (int)P, E, N1, K1, BN, pl)
+        : launch_smem<moe_plan_kernel<int32_t>, kPlanSmemBound>(__func__, dim3(1), dim3(kPlanThreads), psm, st,
+                                                                (const int32_t*)topk_ids, topk_w, w_f32, (int)P, E, N1, K1, BN, pl);
+    if (rc) return rc;
+    CB_LAUNCHED(1);
+    cb::launch_k(moe_gather_quant_kernel, dim3(cdiv(P * (K1 / 128), 8)), dim3(256), 0, st, (const __nv_bfloat16*)x,
+                 (const int*)pl.pair_sorted, (const int*)pl.seg_start, E, topk, K1, quant, ws.xs, ws.xs_s,
+                 (__nv_bfloat16*)ws.xs);
+    CB_LAUNCHED(1);
+    rc = cb::tc_grouped_gemm(gkind, ws.xs, ws.xs_s, w1, w1_s, ws.c1, (int)P, E, N1, K1, BN, pl.num_tiles1, pl.tile1_wrow,
+                             pl.tile1_xrow, pl.tile1_cnt, nullptr, nullptr, workspace, cb::tc_workspace_bytes(128, 128), st);
+    if (rc) return rc;
+    cb::launch_k(moe_silu_quant_kernel, dim3(cdiv(P * (N2 / 128), 8)), dim3(256), 0, st, (const __nv_bfloat16*)ws.c1,
+                 (const int*)pl.seg_start, E, N2, quant, ws.a2, ws.a2_s, (__nv_bfloat16*)ws.a2);
+    CB_LAUNCHED(1);
+    rc = cb::tc_grouped_gemm(gkind, ws.a2, ws.a2_s, w2, w2_s, ws.c3, (int)P, E, K1, N2, BN, pl.num_tiles2, pl.tile2_wrow,
+                             pl.tile2_xrow, pl.tile2_cnt, pl.w_sorted, nullptr, workspace, cb::tc_workspace_bytes(128, 128),
+                             st);
+    if (rc) return rc;
+    int cblocks = cdiv((int64_t)T * K1 / 2, 256);
+    if (cblocks > 132 * 8) cblocks = 132 * 8;
+    PushDev push;
+    memset(&push, 0, sizeof(push));
+    if (comm) {
+      rc = cb::comm_push_desc(comm, &push);
+      if (rc) return rc;
+    }
+    cb::launch_k(moe_combine_kernel, dim3(cblocks), dim3(256), 0, st, (const __nv_bfloat16*)ws.c3, (const int*)pl.pos,
+                 (__nv_bfloat16*)out, T, topk, K1, (const __nv_bfloat16*)residual, comm ? 1 : 0, push);
+    CB_LAUNCHED(1);
+    return 0;
+  }
+  if (comm) return cb::fail(-2, "fused_experts_ar: only the grouped wgmma path pushes (T=%d topk=%d E=%d N1=%d K1=%d)", T, topk, E, N1, K1);
+
+  // ---- pair-GEMV path: both GEMMs run the kernel of the weight mode, mode 1 on activations quantised per 128-group ----
+  const PairWs ws(workspace, T, P, N1, K1);
+  const auto gemv = wmode == 1 ? moe_pair_gemv_kernel<1> : (wmode == 2 ? moe_pair_gemv_kernel<2> : moe_pair_gemv_kernel<0>);
+  int rc;
+  // GEMM1
+  if (wmode == 1) {
+    rc = chitu_b200_act_quant_fp8(x, ws.a1_q, ws.a1_s, T, K1, 128, 1, 1e-10f, CB_BF16, stream);
+    if (rc) return rc;
+  }
+  cb::launch_k(gemv, dim3(cdiv(N1, 16), (unsigned)P), dim3(256), 0, st, wmode == 1 ? (const void*)ws.a1_q : x,
+               wmode == 1 ? ws.a1_s : nullptr, (const uint8_t*)w1, wmode ? w1_s : nullptr, topk_ids, ids_i64, topk_w,
+               w_f32, 0, topk, E, N1, K1, ws.c1);
+  CB_LAUNCHED(1);
+  rc = chitu_b200_silu_and_mul(ws.c1, ws.a2, P, N2, CB_BF16, stream);
+  if (rc) return rc;
+  // GEMM2 (x routed weight)
+  if (wmode == 1) {
+    rc = chitu_b200_act_quant_fp8(ws.a2, ws.a2_q, ws.a2_s, P, N2, 128, 1, 1e-10f, CB_BF16, stream);
+    if (rc) return rc;
+  }
+  cb::launch_k(gemv, dim3(cdiv(K1, 16), (unsigned)P), dim3(256), 0, st, wmode == 1 ? (const void*)ws.a2_q : ws.a2,
+               wmode == 1 ? ws.a2_s : nullptr, (const uint8_t*)w2, wmode ? w2_s : nullptr, topk_ids, ids_i64, topk_w,
+               w_f32, 1, 1, E, K1, N2, ws.c3);
+  CB_LAUNCHED(1);
+  int blocks = cdiv((int64_t)T * K1, 256);
+  if (blocks > 132 * 8) blocks = 132 * 8;
+  cb::launch_k(moe_sum_kernel, dim3(blocks), dim3(256), 0, st, ws.c3, (__nv_bfloat16*)out, T, topk, K1);
+  CB_LAUNCHED(1);
+  if (residual) return chitu_b200_add(out, residual, out, (int64_t)T * K1, CB_BF16, stream);
+  return 0;
 }
 
 extern "C" int chitu_b200_fused_experts(const void* x, const void* w1, const void* w2, const float* w1_s,
@@ -1057,129 +1170,6 @@ extern "C" int chitu_b200_fused_experts_ar(const void* x, const void* w1, const 
   CB_ARG(comm && K1 % 2 == 0 && (int64_t)T * K1 * 2 <= cb::comm_slot_bytes(comm));
   return fused_experts_impl(x, w1, w2, w1_s, w2_s, topk_w, topk_w_dtype, topk_ids, ids_dtype, T, topk, E, N1, K1, wmode, nullptr,
                             nullptr, workspace, workspace_bytes, stream, comm);
-}
-
-static int fused_experts_impl(const void* x, const void* w1, const void* w2, const float* w1_s,
-                              const float* w2_s, const void* topk_w, int topk_w_dtype,
-                              const void* topk_ids, int ids_dtype, int T, int topk, int E, int N1,
-                              int K1, int wmode, void* out, const void* residual, void* workspace,
-                              int64_t workspace_bytes, void* stream, void* comm) {
-  CB_ARG(x && w1 && w2 && topk_w && topk_ids && (out || comm) && workspace);
-  CB_ARG(T >= 0 && topk > 0 && E > 0 && N1 > 0 && N1 % 2 == 0 && K1 > 0);
-  CB_ARG(wmode >= 0 && wmode <= 2);
-  CB_ARG(wmode == 0 || (w1_s && w2_s));
-  CB_ARG(topk_w_dtype == CB_BF16 || topk_w_dtype == CB_F32);
-  CB_ARG(ids_dtype == CB_I32 || ids_dtype == CB_I64);
-  CB_ARG(K1 % 16 == 0 && (N1 / 2) % 16 == 0);
-  if (wmode == 1) CB_ARG(K1 % 128 == 0 && (N1 / 2) % 128 == 0);
-  CB_ARG(workspace_bytes >= chitu_b200_moe_workspace_bytes(T, topk, E, N1, K1));
-  if (T == 0) return 0;
-  cudaStream_t st = (cudaStream_t)stream;
-  const int64_t P = (int64_t)T * topk;
-  const int N2 = N1 / 2;
-  CB_ARG(P <= 65535);
-
-  // ---- grouped wgmma path: sort pairs by expert, stream every distinct expert once ----
-  const int BN = moe_chunk_rows(P, E);
-  const int64_t chunks = E + P / 16 + 1;
-  if (P <= 8192 && E <= 1024 && N1 % 256 == 0 && K1 % 128 == 0 && (wmode != 2 || (N1 / 2) % 128 == 0) &&
-      chunks * (N1 / 128) <= cb::tc_max_tiles() && chunks * (K1 / 128) <= cb::tc_max_tiles() && cb::tma_available()) {
-    void* gws = workspace;
-    MoePlan pl;
-    uint8_t* q = moe_plan_layout(workspace, P, E, N1, K1, &pl);
-    uint8_t* xs = q;                            q += align256(P * K1 * 2);
-    float* xs_s = (float*)q;                    q += align256(P * (K1 / 128 + 1) * 4);
-    __nv_bfloat16* c1 = (__nv_bfloat16*)q;      q += align256(P * N1 * 2);
-    uint8_t* a2 = q;                            q += align256(P * N2 * 2);
-    float* a2_s = (float*)q;                    q += align256(P * (N2 / 128 + 1) * 4);
-    __nv_bfloat16* c3 = (__nv_bfloat16*)q;
-    const int quant = wmode == 1;
-    const size_t psm = (size_t)moe_plan_smem_ints(P, E) * sizeof(int);
-    static size_t plan_attr = 48 * 1024;
-    if (psm > plan_attr) {
-      CB_CUDA(cudaFuncSetAttribute(moe_plan_kernel<int64_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psm));
-      CB_CUDA(cudaFuncSetAttribute(moe_plan_kernel<int32_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psm));
-      plan_attr = psm;
-    }
-    if (ids_dtype == CB_I64)
-      cb::launch_k(moe_plan_kernel<int64_t>, dim3(1), dim3(kPlanThreads), psm, st, (const int64_t*)topk_ids, topk_w,
-                   (int)(topk_w_dtype == CB_F32), (int)P, E, N1, K1, BN, pl);
-    else
-      cb::launch_k(moe_plan_kernel<int32_t>, dim3(1), dim3(kPlanThreads), psm, st, (const int32_t*)topk_ids, topk_w,
-                   (int)(topk_w_dtype == CB_F32), (int)P, E, N1, K1, BN, pl);
-    CB_LAUNCHED(1);
-    cb::launch_k(moe_gather_quant_kernel, dim3(cdiv(P * (K1 / 128), 8)), dim3(256), 0, st, (const __nv_bfloat16*)x,
-                 (const int*)pl.pair_sorted, (const int*)pl.seg_start, E, topk, K1, quant, xs, xs_s, (__nv_bfloat16*)xs);
-    CB_LAUNCHED(1);
-    const int gkind = wmode == 1 ? cb::KIND_FP8 : (wmode == 2 ? cb::KIND_SOFT : cb::KIND_16);
-    int rc = cb::tc_grouped_gemm(gkind, xs, xs_s, w1, w1_s, c1, (int)P, E, N1, K1, BN, pl.num_tiles1, pl.tile1_wrow,
-                                 pl.tile1_xrow, pl.tile1_cnt, nullptr, nullptr, gws, cb::tc_workspace_bytes(128, 128), st);
-    if (rc) return rc;
-    cb::launch_k(moe_silu_quant_kernel, dim3(cdiv(P * (N2 / 128), 8)), dim3(256), 0, st, (const __nv_bfloat16*)c1,
-                 (const int*)pl.seg_start, E, N2, quant, a2, a2_s, (__nv_bfloat16*)a2);
-    CB_LAUNCHED(1);
-    rc = cb::tc_grouped_gemm(gkind, a2, a2_s, w2, w2_s, c3, (int)P, E, K1, N2, BN, pl.num_tiles2, pl.tile2_wrow,
-                             pl.tile2_xrow, pl.tile2_cnt, pl.w_sorted, nullptr, gws, cb::tc_workspace_bytes(128, 128), st);
-    if (rc) return rc;
-    int cblocks = cdiv((int64_t)T * K1 / 2, 256);
-    if (cblocks > 132 * 8) cblocks = 132 * 8;
-    PushDev push;
-    memset(&push, 0, sizeof(push));
-    if (comm) {
-      rc = cb::comm_push_desc(comm, &push);
-      if (rc) return rc;
-    }
-    cb::launch_k(moe_combine_kernel, dim3(cblocks), dim3(256), 0, st, (const __nv_bfloat16*)c3, (const int*)pl.pos,
-                 (__nv_bfloat16*)out, T, topk, K1, (const __nv_bfloat16*)residual, comm ? 1 : 0, push);
-    CB_LAUNCHED(1);
-    return 0;
-  }
-  if (comm) return cb::fail(-2, "fused_experts_ar: only the grouped wgmma path pushes (T=%d topk=%d E=%d N1=%d K1=%d)", T, topk, E, N1, K1);
-
-  // (the first bytes of the workspace hold the grouped path's ticket counters and must stay zero)
-  uint8_t* p = (uint8_t*)workspace + align256(cb::tc_workspace_bytes(128, 128));
-  uint8_t* a1_q = p;            p += align256((int64_t)T * K1);
-  float* a1_s = (float*)p;      p += align256((int64_t)T * (K1 / 128 + 1) * 4);
-  __nv_bfloat16* c1 = (__nv_bfloat16*)p;   p += align256(P * N1 * 2);
-  __nv_bfloat16* a2 = (__nv_bfloat16*)p;   p += align256(P * N2 * 2);
-  uint8_t* a2_q = p;            p += align256(P * N2);
-  float* a2_s = (float*)p;      p += align256(P * (N2 / 128 + 1) * 4);
-  __nv_bfloat16* c3 = (__nv_bfloat16*)p;
-
-  const int ids_i64 = ids_dtype == CB_I64, w_f32 = topk_w_dtype == CB_F32;
-  int rc;
-  // GEMM1
-  dim3 g1(cdiv(N1, 16), (unsigned)P);
-  if (wmode == 1) {
-    rc = chitu_b200_act_quant_fp8(x, a1_q, a1_s, T, K1, 128, 1, 1e-10f, CB_BF16, stream);
-    if (rc) return rc;
-    cb::launch_k(moe_pair_gemv_kernel<1>, dim3(g1), dim3(256), 0, st, a1_q, a1_s, (const uint8_t*)w1, w1_s, topk_ids, ids_i64, topk_w, w_f32, 0, topk, E, N1, K1, c1);
-  } else if (wmode == 2) {
-    cb::launch_k(moe_pair_gemv_kernel<2>, dim3(g1), dim3(256), 0, st, x, nullptr, (const uint8_t*)w1, w1_s, topk_ids, ids_i64, topk_w, w_f32, 0, topk, E, N1, K1, c1);
-  } else {
-    cb::launch_k(moe_pair_gemv_kernel<0>, dim3(g1), dim3(256), 0, st, x, nullptr, (const uint8_t*)w1, nullptr, topk_ids, ids_i64, topk_w, w_f32, 0, topk, E, N1, K1, c1);
-  }
-  CB_LAUNCHED(1);
-  rc = chitu_b200_silu_and_mul(c1, a2, P, N2, CB_BF16, stream);
-  if (rc) return rc;
-  // GEMM2 (x routed weight)
-  dim3 g2(cdiv(K1, 16), (unsigned)P);
-  if (wmode == 1) {
-    rc = chitu_b200_act_quant_fp8(a2, a2_q, a2_s, P, N2, 128, 1, 1e-10f, CB_BF16, stream);
-    if (rc) return rc;
-    cb::launch_k(moe_pair_gemv_kernel<1>, dim3(g2), dim3(256), 0, st, a2_q, a2_s, (const uint8_t*)w2, w2_s, topk_ids, ids_i64, topk_w, w_f32, 1, 1, E, K1, N2, c3);
-  } else if (wmode == 2) {
-    cb::launch_k(moe_pair_gemv_kernel<2>, dim3(g2), dim3(256), 0, st, a2, nullptr, (const uint8_t*)w2, w2_s, topk_ids, ids_i64, topk_w, w_f32, 1, 1, E, K1, N2, c3);
-  } else {
-    cb::launch_k(moe_pair_gemv_kernel<0>, dim3(g2), dim3(256), 0, st, a2, nullptr, (const uint8_t*)w2, nullptr, topk_ids, ids_i64, topk_w, w_f32, 1, 1, E, K1, N2, c3);
-  }
-  CB_LAUNCHED(1);
-  int blocks = cdiv((int64_t)T * K1, 256);
-  if (blocks > 132 * 8) blocks = 132 * 8;
-  cb::launch_k(moe_sum_kernel, dim3(blocks), dim3(256), 0, st, c3, (__nv_bfloat16*)out, T, topk, K1);
-  CB_LAUNCHED(1);
-  if (residual) return chitu_b200_add(out, residual, out, (int64_t)T * K1, CB_BF16, stream);
-  return 0;
 }
 
 CB_DEFINE_TL_SETTER(moe)
