@@ -126,19 +126,22 @@ inline int launch_smem(const char* name, dim3 grid, dim3 block, size_t smem, cud
   return 0;
 }
 
-// f(T{}, std::integral_constant<int, G>{}) for the io type of `dtype` (CB_BF16, else fp16) and G = 1, 2, 4, else 8;
-// returns f's status.
+// f(T{}) for the io type T of `dtype` (CB_BF16, else fp16); returns f's result.
+template <typename F>
+inline auto dispatch_io(int dtype, F&& f) {
+  return dtype == CB_BF16 ? f(__nv_bfloat16{}) : f(__half{});
+}
+// f(T{}, std::integral_constant<int, G>{}) for the io type of `dtype` and G = 1, 2, 4, else 8; returns f's status.
 template <typename F>
 inline int dispatch_io_g(int dtype, int G, F&& f) {
-  auto by_g = [&](auto t) {
+  return dispatch_io(dtype, [&](auto t) {
     switch (G) {
       case 1: return f(t, std::integral_constant<int, 1>{});
       case 2: return f(t, std::integral_constant<int, 2>{});
       case 4: return f(t, std::integral_constant<int, 4>{});
       default: return f(t, std::integral_constant<int, 8>{});
     }
-  };
-  return dtype == CB_BF16 ? by_g(__nv_bfloat16{}) : by_g(__half{});
+  });
 }
 #endif
 

@@ -608,8 +608,15 @@ int make_tma_map_nd(CUtensorMap* map, const void* base, int rank, const cuuint64
 
 namespace {
 
-int make_map(CUtensorMap* map, const void* base, int rows, int K, int elem_bytes, CUtensorMapDataType dt, int box_rows) {
-  return make_tma_map_2d(map, base, rows, K, elem_bytes, dt, box_rows);
+// The operands of a kind: bytes and TMA type of a weight and of an activation element.  KIND_16's follow the io dtype
+// (CB_BF16, else fp16); soft fp8 multiplies bf16 activations.
+struct Operands { int w_elem; CUtensorMapDataType w_dt; int x_elem; CUtensorMapDataType x_dt; };
+Operands operands(int kind, int dtype) {
+  const CUtensorMapDataType u8 = CU_TENSOR_MAP_DATA_TYPE_UINT8, bf16 = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+  const CUtensorMapDataType io = dtype == CB_BF16 ? bf16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  if (kind == KIND_16) return {2, io, 2, io};
+  if (kind == KIND_SOFT) return {1, u8, 2, bf16};
+  return {1, u8, 1, u8};                              // fp8, int8
 }
 
 int pick_bn(int M) { return M <= 16 ? 16 : M <= 32 ? 32 : M <= 64 ? 64 : 128; }
@@ -670,12 +677,32 @@ int dispatch_bn(int BN, const CUtensorMap& mw, const CUtensorMap& mx, Params& p,
   }
 }
 
-int run(int kind, const void* x, const void* w, Params& p, int elem, CUtensorMapDataType dt, void* ws, int64_t ws_bytes,
-        cudaStream_t st, int x_elem = 0, CUtensorMapDataType x_dt = CU_TENSOR_MAP_DATA_TYPE_UINT8) {
+// The kernel of `kind` for p over the weights w [w_rows, p.K] and the activations x [x_rows, p.K], after their TMA maps.
+int launch_kind(int kind, const void* x, int64_t x_rows, const void* w, int64_t w_rows, Params& p, int BN, int grid,
+                cudaStream_t st) {
+  const Operands op = operands(kind, p.out_dtype);
+  CUtensorMap mw, mx;
+  int rc = make_tma_map_2d(&mw, w, w_rows, p.K, op.w_elem, op.w_dt, kTileN);
+  if (rc) return rc;
+  rc = make_tma_map_2d(&mx, x, x_rows, p.K, op.x_elem, op.x_dt, BN);
+  if (rc) return rc;
+  if (kind == KIND_16) return dispatch_bn<KIND_16>(BN, mw, mx, p, grid, st);
+  if (kind == KIND_FP8) return dispatch_bn<KIND_FP8>(BN, mw, mx, p, grid, st);
+  if (kind == KIND_SOFT) return dispatch_bn<KIND_SOFT>(BN, mw, mx, p, grid, st);
+  return dispatch_bn<KIND_I8>(BN, mw, mx, p, grid, st);
+}
+
+int run(int kind, const void* x, const void* w, Params& p, void* ws, int64_t ws_bytes, cudaStream_t st,
+        void* comm = nullptr) {
+  if (comm) {
+    const int rc = comm_push_desc(comm, &p.push);
+    if (rc) return rc;
+    p.has_push = 1;
+  }
   const int BN = pick_bn(p.M);
   p.n_tiles = cdiv(p.N, kTileN);
   p.m_chunks = cdiv(p.M, BN);
-  p.S = cdiv((int64_t)p.K * elem, kStageRowBytes);
+  p.S = cdiv((int64_t)p.K * operands(kind, p.out_dtype).w_elem, kStageRowBytes);
   p.kblocks = cdiv(p.K, 128);
   const int tiles = p.n_tiles * p.m_chunks;
   if (tiles > kMaxTickets) return fail(-2, "tc_gemm: too many tiles (%d)", tiles);
@@ -700,15 +727,7 @@ int run(int kind, const void* x, const void* w, Params& p, int elem, CUtensorMap
   }
   p.tickets = (int*)ws;
   p.partial = ws ? (float*)((uint8_t*)ws + kTicketBytes) : nullptr;
-  CUtensorMap mw, mx;
-  int rc = make_map(&mw, w, p.N, p.K, elem, dt, kTileN);
-  if (rc) return rc;
-  rc = x_elem ? make_map(&mx, x, p.M, p.K, x_elem, x_dt, BN) : make_map(&mx, x, p.M, p.K, elem, dt, BN);
-  if (rc) return rc;
-  if (kind == KIND_16) return dispatch_bn<KIND_16>(BN, mw, mx, p, grid, st);
-  if (kind == KIND_FP8) return dispatch_bn<KIND_FP8>(BN, mw, mx, p, grid, st);
-  if (kind == KIND_SOFT) return dispatch_bn<KIND_SOFT>(BN, mw, mx, p, grid, st);
-  return dispatch_bn<KIND_I8>(BN, mw, mx, p, grid, st);
+  return launch_kind(kind, x, p.M, w, p.N, p, BN, grid, st);
 }
 
 }  // namespace
@@ -717,8 +736,7 @@ int64_t tc_max_tiles() { return kMaxTickets; }
 
 bool tc_supported(int kind, int M, int N, int K) {
   if (M < 1 || N < 1 || K < 1) return false;
-  const int elem = kind == KIND_16 ? 2 : 1;
-  if (((int64_t)K * elem) % 16 != 0) return false;          // TMA row pitch
+  if (((int64_t)K * operands(kind, CB_BF16).w_elem) % 16 != 0) return false;   // TMA row pitch
   if ((kind == KIND_FP8 || kind == KIND_SOFT) && K % 128 != 0) return false;   // one scale block per pipeline stage
   return tma_available();
 }
@@ -736,9 +754,8 @@ int tc_grouped_gemm(int kind, const void* xs, const float* a_s, const void* w, c
                     const int* g_tile_xrow, const int* g_tile_cnt, const float* row_scale, const int* out_rows, void* ws,
                     int64_t ws_bytes, cudaStream_t st) {
   Params p{};
-  const int elem = kind == KIND_16 ? 2 : 1;             // weight bytes per element
   p.M = rows; p.N = Ng; p.K = K;
-  p.S = cdiv((int64_t)K * elem, kStageRowBytes);
+  p.S = cdiv((int64_t)K * operands(kind, CB_BF16).w_elem, kStageRowBytes);
   p.kblocks = cdiv(K, 128);
   p.out_dtype = CB_BF16; p.a_s = a_s; p.b_s = b_s; p.out = out;
   p.g_num_tiles = g_num_tiles; p.g_tile_wrow = g_tile_wrow; p.g_tile_xrow = g_tile_xrow; p.g_tile_cnt = g_tile_cnt;
@@ -751,16 +768,7 @@ int tc_grouped_gemm(int kind, const void* xs, const float* a_s, const void* w, c
   if (!ws || ws_bytes < ws_bytes_for(grid, BN)) return fail(-2, "tc_grouped_gemm: workspace too small");
   p.tickets = (int*)ws;
   p.partial = (float*)((uint8_t*)ws + kTicketBytes);
-  CUtensorMap mw, mx;
-  const CUtensorMapDataType wdt = kind == KIND_16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_UINT8;
-  const bool x16 = kind != KIND_FP8;                  // bf16 activations (bf16 and soft-fp8 kinds)
-  int rc = make_tma_map_2d(&mw, w, (int64_t)E * Ng, K, elem, wdt, kTileN);
-  if (rc) return rc;
-  rc = make_tma_map_2d(&mx, xs, rows, K, x16 ? 2 : 1, x16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_UINT8, BN);
-  if (rc) return rc;
-  if (kind == KIND_16) return dispatch_bn<KIND_16>(BN, mw, mx, p, grid, st);
-  if (kind == KIND_SOFT) return dispatch_bn<KIND_SOFT>(BN, mw, mx, p, grid, st);
-  return dispatch_bn<KIND_FP8>(BN, mw, mx, p, grid, st);
+  return launch_kind(kind, xs, rows, w, (int64_t)E * Ng, p, BN, grid, st);
 }
 
 int tc_linear16(const void* x, const void* w, const void* bias, const void* residual, void* y, int M, int N, int K,
@@ -768,13 +776,7 @@ int tc_linear16(const void* x, const void* w, const void* bias, const void* resi
   Params p{};
   p.M = M; p.N = N; p.K = K;
   p.out_dtype = dtype; p.bias = bias; p.residual = residual; p.out = y;
-  if (comm) {
-    int rc = comm_push_desc(comm, &p.push);
-    if (rc) return rc;
-    p.has_push = 1;
-  }
-  return run(KIND_16, x, w, p, 2, dtype == CB_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16,
-             ws, ws_bytes, st);
+  return run(KIND_16, x, w, p, ws, ws_bytes, st, comm);
 }
 
 // y[M, N/2] = SiluAndMul(x . W^T) with W's rows interleaved (gate_0, up_0, gate_1, up_1, ...); bf16 only
@@ -783,7 +785,7 @@ int tc_linear16_silu_pairs(const void* x, const void* w, void* y, int M, int N, 
   Params p{};
   p.M = M; p.N = N; p.K = K;
   p.out_dtype = CB_BF16; p.out = y; p.act_pairs = 1;
-  return run(KIND_16, x, w, p, 2, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, ws, ws_bytes, st);
+  return run(KIND_16, x, w, p, ws, ws_bytes, st);
 }
 
 int tc_fp8_gemm(const void* a, const float* a_s, const void* b, const float* b_s, void* c, int M, int N, int K,
@@ -791,12 +793,7 @@ int tc_fp8_gemm(const void* a, const float* a_s, const void* b, const float* b_s
   Params p{};
   p.M = M; p.N = N; p.K = K;
   p.out_dtype = CB_BF16; p.a_s = a_s; p.b_s = b_s; p.out = c; p.residual = residual;
-  if (comm) {
-    int rc = comm_push_desc(comm, &p.push);
-    if (rc) return rc;
-    p.has_push = 1;
-  }
-  return run(KIND_FP8, a, b, p, 1, CU_TENSOR_MAP_DATA_TYPE_UINT8, ws, ws_bytes, st);
+  return run(KIND_FP8, a, b, p, ws, ws_bytes, st, comm);
 }
 
 // soft_fp8_gemm_deepseek_v3 (ops.py:486-511): a bf16 [M,K], b fp8 [N,K] + block scales -> c bf16 [M,N]
@@ -805,7 +802,7 @@ int tc_soft_fp8_gemm(const void* a, const void* b, const float* b_s, void* c, in
   Params p{};
   p.M = M; p.N = N; p.K = K;
   p.out_dtype = CB_BF16; p.b_s = b_s; p.out = c;
-  return run(KIND_SOFT, a, b, p, 1, CU_TENSOR_MAP_DATA_TYPE_UINT8, ws, ws_bytes, st, 2, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
+  return run(KIND_SOFT, a, b, p, ws, ws_bytes, st);
 }
 
 int tc_w8a8_gemm(void* out, const int8_t* a, const int8_t* b, const float* a_scales, const float* b_scales,
@@ -813,7 +810,7 @@ int tc_w8a8_gemm(void* out, const int8_t* a, const int8_t* b, const float* a_sca
   Params p{};
   p.M = M; p.N = N; p.K = K;
   p.out_dtype = CB_F16; p.a_s = a_scales; p.b_s = b_scales; p.bias = bias; p.out = out;
-  return run(KIND_I8, a, b, p, 1, CU_TENSOR_MAP_DATA_TYPE_UINT8, ws, ws_bytes, st);
+  return run(KIND_I8, a, b, p, ws, ws_bytes, st);
 }
 
 }  // namespace cb

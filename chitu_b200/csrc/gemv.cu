@@ -1,12 +1,14 @@
-// SIMT weight-streaming skinny GEMM ("GEMV" path): y[M,N] = x[M,K] · W[N,K]^T, M in chunks of <= 16.
+// SIMT weight-streaming skinny GEMM ("GEMV" path): y[M,N] = x[M,K] · W[N,K]^T, M in chunks of <= 16 tokens (soft fp8:
+// <= 8), one launch each.
 //
 // Decode linears are HBM-bound weight streams (SURVEY §7.3-1): each warp owns two weight rows,
 // the 32 lanes stride K with 128-bit `ld.global.nc.L1::no_allocate` loads (each weight byte is
 // read exactly once from HBM), activations are re-read through L1 (they are tiny), fp32
-// accumulation, butterfly reduce.  This path is impl = 1 and the fall-back for shapes TMA cannot
-// address; the wgmma + TMA swap-AB kernel in gemm_tc.cu is the tensor-core implementation of the
-// same entry points (impl = 2) and the default whenever it supports the shape and the workspace
-// is large enough (linear.cu use_tc()).
+// accumulation, butterfly reduce.  The linear entries (linear.cu) run this path for impl = 1 and,
+// under auto, for the calls the wgmma + TMA kernel of gemm_tc.cu cannot take (a shape TMA cannot
+// address, soft fp8 with fp16 activations, a missing or short workspace).
+#include <algorithm>
+
 #include "common.cuh"
 #include "gemm.cuh"
 
@@ -305,45 +307,41 @@ __global__ void __launch_bounds__(kWarps * 32) gemv_i8_kernel(__half* __restrict
 
 inline int grid_for(int N) { return cdiv(N, kWarps * kRowsPerWarp); }
 
-}  // namespace
+// The SIMT launcher: walks M in chunks of at most max(kMT) tokens and calls f(std::integral_constant<int, MT>{}, m0, Mc)
+// for each chunk [m0, m0 + Mc), MT the first of kMT (ascending) that holds it; f makes one launch.  Returns the number
+// of launches.
+template <int... kMT, typename F>
+int simt_chunks(int M, F&& f) {
+  constexpr int kMax = std::max({kMT...});
+  int launches = 0;
+  for (int m0 = 0; m0 < M; m0 += kMax, ++launches) {
+    const int Mc = M - m0 < kMax ? M - m0 : kMax;
+    auto run = [&](auto mt) {
+      if (Mc > mt) return false;
+      f(mt, m0, Mc);
+      return true;
+    };
+    (run(std::integral_constant<int, kMT>{}) || ...);
+  }
+  return launches;
+}
 
-// The SIMT entry points process M in chunks of <= 16 tokens.
-#define DISPATCH_MT(Mc, CALL)          \
-  if (Mc <= 1) { CALL(1); }            \
-  else if (Mc <= 2) { CALL(2); }       \
-  else if (Mc <= 4) { CALL(4); }       \
-  else if (Mc <= 8) { CALL(8); }       \
-  else { CALL(16); }
+}  // namespace
 
 namespace cb {
 
 int simt_linear16(const void* x, const void* w, const void* bias, const void* residual, void* y, int M,
                   int N, int K, int dtype, cudaStream_t st) {
   CB_ARG(K % 8 == 0);
-  int launches = 0;
-  for (int m0 = 0; m0 < M; m0 += 16) {
-    int Mc = M - m0 < 16 ? M - m0 : 16;
-    if (dtype == CB_BF16) {
-      using T = __nv_bfloat16;
-#define CALL(MT)                                                                                   \
-  cb::launch_k(gemv16_kernel<T, MT>, dim3(grid_for(N)), dim3(kWarps * 32), 0, st,                                        \
-      (const T*)x + (int64_t)m0 * K, (const T*)w, (const T*)bias,                                  \
-      residual ? (const T*)residual + (int64_t)m0 * N : nullptr, (T*)y + (int64_t)m0 * N, Mc, N, K)
-      DISPATCH_MT(Mc, CALL)
-#undef CALL
-    } else if (dtype == CB_F16) {
-      using T = __half;
-#define CALL(MT)                                                                                   \
-  cb::launch_k(gemv16_kernel<T, MT>, dim3(grid_for(N)), dim3(kWarps * 32), 0, st,                                        \
-      (const T*)x + (int64_t)m0 * K, (const T*)w, (const T*)bias,                                  \
-      residual ? (const T*)residual + (int64_t)m0 * N : nullptr, (T*)y + (int64_t)m0 * N, Mc, N, K)
-      DISPATCH_MT(Mc, CALL)
-#undef CALL
-    } else {
-      return fail(-1, "linear_bf16: unsupported dtype %d", dtype);
-    }
-    ++launches;
-  }
+  if (dtype != CB_BF16 && dtype != CB_F16) return fail(-1, "linear_bf16: unsupported dtype %d", dtype);
+  const int launches = dispatch_io(dtype, [&](auto t) {
+    using T = decltype(t);
+    return simt_chunks<1, 2, 4, 8, 16>(M, [&](auto mt, int m0, int Mc) {
+      launch_k(gemv16_kernel<T, decltype(mt)::value>, dim3(grid_for(N)), dim3(kWarps * 32), 0, st,
+               (const T*)x + (int64_t)m0 * K, (const T*)w, (const T*)bias,
+               residual ? (const T*)residual + (int64_t)m0 * N : nullptr, (T*)y + (int64_t)m0 * N, Mc, N, K);
+    });
+  });
   CB_LAUNCHED(launches);
   return 0;
 }
@@ -352,17 +350,11 @@ int simt_fp8_gemm(const void* a, const float* a_s, const void* b, const float* b
                   int K, cudaStream_t st) {
   CB_ARG(K % 16 == 0);
   const int kblocks = (K + 127) / 128;
-  int launches = 0;
-  for (int m0 = 0; m0 < M; m0 += 16) {
-    int Mc = M - m0 < 16 ? M - m0 : 16;
-#define CALL(MT)                                                                                      \
-  cb::launch_k(gemv_fp8_kernel<MT>, dim3(grid_for(N)), dim3(kWarps * 32), 0, st,                                            \
-      (const uint8_t*)a + (int64_t)m0 * K, a_s + (int64_t)m0 * kblocks, (const uint8_t*)b, b_s,       \
-      (__nv_bfloat16*)c + (int64_t)m0 * N, Mc, N, K)
-    DISPATCH_MT(Mc, CALL)
-#undef CALL
-    ++launches;
-  }
+  const int launches = simt_chunks<1, 2, 4, 8, 16>(M, [&](auto mt, int m0, int Mc) {
+    launch_k(gemv_fp8_kernel<decltype(mt)::value>, dim3(grid_for(N)), dim3(kWarps * 32), 0, st,
+             (const uint8_t*)a + (int64_t)m0 * K, a_s + (int64_t)m0 * kblocks, (const uint8_t*)b, b_s,
+             (__nv_bfloat16*)c + (int64_t)m0 * N, Mc, N, K);
+  });
   CB_LAUNCHED(launches);
   return 0;
 }
@@ -370,28 +362,14 @@ int simt_fp8_gemm(const void* a, const float* a_s, const void* b, const float* b
 int simt_soft_fp8_gemm(const void* a, const void* b, const float* b_s, void* c, int M, int N, int K,
                        int out_dtype, cudaStream_t st) {
   CB_ARG(K % 16 == 0);
-  int launches = 0;
-  for (int m0 = 0; m0 < M; m0 += 8) {
-    int Mc = M - m0 < 8 ? M - m0 : 8;
-    if (out_dtype == CB_BF16) {
-      using T = __nv_bfloat16;
-#define CALL(MT)                                                                              \
-  cb::launch_k(gemv_softfp8_kernel<T, MT>, dim3(grid_for(N)), dim3(kWarps * 32), 0, st,                             \
-      (const T*)a + (int64_t)m0 * K, (const uint8_t*)b, b_s, (T*)c + (int64_t)m0 * N, Mc, N, K)
-      if (Mc <= 1) { CALL(1); } else if (Mc <= 2) { CALL(2); } else if (Mc <= 4) { CALL(4); } else { CALL(8); }
-#undef CALL
-    } else if (out_dtype == CB_F16) {
-      using T = __half;
-#define CALL(MT)                                                                              \
-  cb::launch_k(gemv_softfp8_kernel<T, MT>, dim3(grid_for(N)), dim3(kWarps * 32), 0, st,                             \
-      (const T*)a + (int64_t)m0 * K, (const uint8_t*)b, b_s, (T*)c + (int64_t)m0 * N, Mc, N, K)
-      if (Mc <= 1) { CALL(1); } else if (Mc <= 2) { CALL(2); } else if (Mc <= 4) { CALL(4); } else { CALL(8); }
-#undef CALL
-    } else {
-      return fail(-1, "soft_fp8_gemm: unsupported dtype %d", out_dtype);
-    }
-    ++launches;
-  }
+  if (out_dtype != CB_BF16 && out_dtype != CB_F16) return fail(-1, "soft_fp8_gemm: unsupported dtype %d", out_dtype);
+  const int launches = dispatch_io(out_dtype, [&](auto t) {
+    using T = decltype(t);
+    return simt_chunks<1, 2, 4, 8>(M, [&](auto mt, int m0, int Mc) {
+      launch_k(gemv_softfp8_kernel<T, decltype(mt)::value>, dim3(grid_for(N)), dim3(kWarps * 32), 0, st,
+               (const T*)a + (int64_t)m0 * K, (const uint8_t*)b, b_s, (T*)c + (int64_t)m0 * N, Mc, N, K);
+    });
+  });
   CB_LAUNCHED(launches);
   return 0;
 }
@@ -399,17 +377,11 @@ int simt_soft_fp8_gemm(const void* a, const void* b, const float* b_s, void* c, 
 int simt_w8a8_gemm(void* out, const int8_t* a, const int8_t* b, const float* a_scales,
                    const float* b_scales, const void* bias, int M, int N, int K, cudaStream_t st) {
   CB_ARG(K % 16 == 0);
-  int launches = 0;
-  for (int m0 = 0; m0 < M; m0 += 16) {
-    int Mc = M - m0 < 16 ? M - m0 : 16;
-#define CALL(MT)                                                                                   \
-  cb::launch_k(gemv_i8_kernel<MT>, dim3(grid_for(N)), dim3(kWarps * 32), 0, st, (__half*)out + (int64_t)m0 * N,          \
-                                                          a + (int64_t)m0 * K, b, a_scales + m0,   \
-                                                          b_scales, (const __half*)bias, Mc, N, K)
-    DISPATCH_MT(Mc, CALL)
-#undef CALL
-    ++launches;
-  }
+  const int launches = simt_chunks<1, 2, 4, 8, 16>(M, [&](auto mt, int m0, int Mc) {
+    launch_k(gemv_i8_kernel<decltype(mt)::value>, dim3(grid_for(N)), dim3(kWarps * 32), 0, st,
+             (__half*)out + (int64_t)m0 * N, a + (int64_t)m0 * K, b, a_scales + m0, b_scales, (const __half*)bias, Mc,
+             N, K);
+  });
   CB_LAUNCHED(launches);
   return 0;
 }

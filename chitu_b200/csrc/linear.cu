@@ -1,18 +1,20 @@
-// C-ABI entry points of the decode linears; dispatch between the SIMT weight-streaming path
-// (gemv.cu) and the wgmma + TMA swap-AB path (gemm_tc.cu).
+// C-ABI entry points of the decode linears: each runs the persistent stream-K wgmma + TMA kernel (gemm_tc.cu) wherever
+// it can (bs=16 needs tensor cores outright: 16 tokens x 2 flop per weight byte exceed the FMA pipes) or the SIMT
+// weight-streaming kernels (gemv.cu), as linear_path() picks.
 #include "common.cuh"
 #include "gemm.cuh"
 
 using namespace cb;
 
-// auto policy: the persistent stream-K wgmma kernel (bs=16 needs tensor cores outright: 16 tokens x 2 flop per weight
-// byte exceeds the FMA pipes); the SIMT path remains for
-// shapes TMA cannot address (row pitch not a multiple of 16 B, fp8 K % 128 != 0) and as impl=1.
-static bool use_tc(int impl, int kind, int M, int N, int K, void* ws, int64_t ws_bytes) {
-  if (impl == 1) return false;
-  bool ok = tc_supported(kind, M, N, K) && ws && ws_bytes >= tc_workspace_bytes(M, N);
-  if (impl == 2) return ok;
-  return ok;
+// The path of a linear entry: impl = 1 SIMT, impl = 2 wgmma or the -2 refusal, any other impl wgmma where it can run (a
+// shape TMA can address, bf16 activations for soft fp8, a workspace of tc_workspace_bytes) and SIMT elsewhere.
+enum { kSimt = 0, kWgmma = 1 };
+static int linear_path(const char* entry, int kind, int impl, int dtype, int M, int N, int K, void* ws, int64_t ws_bytes) {
+  if (impl == 1) return kSimt;
+  if ((kind != KIND_SOFT || dtype == CB_BF16) && tc_supported(kind, M, N, K) && ws && ws_bytes >= tc_workspace_bytes(M, N))
+    return kWgmma;
+  if (impl != 2) return kSimt;
+  return fail(-2, "%s: wgmma path unavailable for M=%d N=%d K=%d (shape, dtype or workspace)", entry, M, N, K);
 }
 
 extern "C" int64_t chitu_b200_linear_workspace_bytes(int M, int N) { return tc_workspace_bytes(M, N); }
@@ -24,10 +26,9 @@ extern "C" int chitu_b200_linear_bf16(const void* x, const void* w, const void* 
   CB_ARG(dtype == CB_BF16 || dtype == CB_F16);
   if (M == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
-  if (use_tc(impl, KIND_16, M, N, K, workspace, workspace_bytes))
-    return tc_linear16(x, w, bias, residual, y, M, N, K, dtype, workspace, workspace_bytes, st);
-  if (impl == 2) return fail(-2, "linear_bf16: wgmma path unavailable for M=%d N=%d K=%d (or workspace too small)", M, N, K);
-  return simt_linear16(x, w, bias, residual, y, M, N, K, dtype, st);
+  const int path = linear_path(__func__, KIND_16, impl, dtype, M, N, K, workspace, workspace_bytes);
+  if (path == kWgmma) return tc_linear16(x, w, bias, residual, y, M, N, K, dtype, workspace, workspace_bytes, st);
+  return path == kSimt ? simt_linear16(x, w, bias, residual, y, M, N, K, dtype, st) : path;
 }
 
 // FeedForward's gate_up linear + SiluAndMul (models/model_llama.py:139-149, fused_moe.py:24-39) in one launch:
@@ -37,8 +38,8 @@ extern "C" int chitu_b200_linear_bf16_silu_pairs(const void* x, const void* w_pa
                                                  void* workspace, int64_t workspace_bytes, void* stream) {
   CB_ARG(x && w_pairs && y && M >= 0 && N > 0 && N % 2 == 0 && K > 0);
   if (M == 0) return 0;
-  if (!use_tc(2, KIND_16, M, N, K, workspace, workspace_bytes))
-    return fail(-2, "linear_bf16_silu_pairs: wgmma path unavailable for M=%d N=%d K=%d (or workspace too small)", M, N, K);
+  const int path = linear_path(__func__, KIND_16, 2, CB_BF16, M, N, K, workspace, workspace_bytes);
+  if (path != kWgmma) return path;
   return tc_linear16_silu_pairs(x, w_pairs, y, M, N, K, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
@@ -48,9 +49,9 @@ extern "C" int chitu_b200_fp8_gemm(const void* a, const float* a_s, const void* 
   CB_ARG(a && a_s && b && b_s && c && M >= 0 && N > 0 && K > 0);
   if (M == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
-  if (use_tc(impl, KIND_FP8, M, N, K, workspace, workspace_bytes))
-    return tc_fp8_gemm(a, a_s, b, b_s, c, M, N, K, residual, workspace, workspace_bytes, st);
-  if (impl == 2) return fail(-2, "fp8_gemm: wgmma path unavailable for M=%d N=%d K=%d (or workspace too small)", M, N, K);
+  const int path = linear_path(__func__, KIND_FP8, impl, CB_BF16, M, N, K, workspace, workspace_bytes);
+  if (path == kWgmma) return tc_fp8_gemm(a, a_s, b, b_s, c, M, N, K, residual, workspace, workspace_bytes, st);
+  if (path != kSimt) return path;
   int rc = simt_fp8_gemm(a, a_s, b, b_s, c, M, N, K, st);
   if (rc || !residual) return rc;
   return chitu_b200_add(c, residual, c, (int64_t)M * N, CB_BF16, stream);
@@ -64,8 +65,8 @@ extern "C" int chitu_b200_fp8_gemm_ar(const void* a, const float* a_s, const voi
                                       void* comm, void* workspace, int64_t workspace_bytes, void* stream) {
   CB_ARG(a && a_s && b && b_s && comm && M > 0 && N > 0 && N % 2 == 0 && K > 0);
   CB_ARG((int64_t)M * N * 2 <= comm_slot_bytes(comm));
-  if (!use_tc(2, KIND_FP8, M, N, K, workspace, workspace_bytes))
-    return fail(-2, "fp8_gemm_ar: wgmma path unavailable for M=%d N=%d K=%d (or workspace too small)", M, N, K);
+  const int path = linear_path(__func__, KIND_FP8, 2, CB_BF16, M, N, K, workspace, workspace_bytes);
+  if (path != kWgmma) return path;
   return tc_fp8_gemm(a, a_s, b, b_s, nullptr, M, N, K, nullptr, workspace, workspace_bytes, (cudaStream_t)stream, comm);
 }
 
@@ -73,21 +74,20 @@ extern "C" int chitu_b200_linear_bf16_ar(const void* x, const void* w, int M, in
                                          int64_t workspace_bytes, void* stream) {
   CB_ARG(x && w && comm && M > 0 && N > 0 && N % 2 == 0 && K > 0);
   CB_ARG((int64_t)M * N * 2 <= comm_slot_bytes(comm));
-  if (!use_tc(2, KIND_16, M, N, K, workspace, workspace_bytes))
-    return fail(-2, "linear_bf16_ar: wgmma path unavailable for M=%d N=%d K=%d (or workspace too small)", M, N, K);
+  const int path = linear_path(__func__, KIND_16, 2, CB_BF16, M, N, K, workspace, workspace_bytes);
+  if (path != kWgmma) return path;
   return tc_linear16(x, w, nullptr, nullptr, nullptr, M, N, K, CB_BF16, workspace, workspace_bytes, (cudaStream_t)stream, comm);
 }
 
+// wgmma path: the fp8 weight tile is converted to bf16 in shared memory between the TMA landing and the bf16 MMA
 extern "C" int chitu_b200_soft_fp8_gemm(const void* a, const void* b, const float* b_s, void* c, int M,
                                         int N, int K, int out_dtype, void* workspace,
                                         int64_t workspace_bytes, int impl, void* stream) {
   CB_ARG(a && b && b_s && c && M >= 0 && N > 0 && K > 0);
   if (M == 0) return 0;
-  // wgmma path: the fp8 weight tile is converted to bf16 in shared memory between the TMA landing and the bf16 MMA
-  if (out_dtype == CB_BF16 && use_tc(impl, KIND_SOFT, M, N, K, workspace, workspace_bytes))
-    return tc_soft_fp8_gemm(a, b, b_s, c, M, N, K, workspace, workspace_bytes, (cudaStream_t)stream);
-  if (impl == 2) return fail(-2, "soft_fp8_gemm: wgmma path unavailable for M=%d N=%d K=%d (bf16 only, K %% 128 == 0)", M, N, K);
-  return simt_soft_fp8_gemm(a, b, b_s, c, M, N, K, out_dtype, (cudaStream_t)stream);
+  const int path = linear_path(__func__, KIND_SOFT, impl, out_dtype, M, N, K, workspace, workspace_bytes);
+  if (path == kWgmma) return tc_soft_fp8_gemm(a, b, b_s, c, M, N, K, workspace, workspace_bytes, (cudaStream_t)stream);
+  return path == kSimt ? simt_soft_fp8_gemm(a, b, b_s, c, M, N, K, out_dtype, (cudaStream_t)stream) : path;
 }
 
 extern "C" int chitu_b200_w8a8_gemm(void* out, const int8_t* a, const int8_t* b, const float* a_scales,
@@ -96,10 +96,9 @@ extern "C" int chitu_b200_w8a8_gemm(void* out, const int8_t* a, const int8_t* b,
   CB_ARG(out && a && b && a_scales && b_scales && M >= 0 && N > 0 && K > 0);
   if (M == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
-  if (use_tc(impl, KIND_I8, M, N, K, workspace, workspace_bytes))
-    return tc_w8a8_gemm(out, a, b, a_scales, b_scales, bias, M, N, K, workspace, workspace_bytes, st);
-  if (impl == 2) return fail(-2, "w8a8_gemm: wgmma path unavailable for M=%d N=%d K=%d (or workspace too small)", M, N, K);
-  return simt_w8a8_gemm(out, a, b, a_scales, b_scales, bias, M, N, K, st);
+  const int path = linear_path(__func__, KIND_I8, impl, CB_F16, M, N, K, workspace, workspace_bytes);
+  if (path == kWgmma) return tc_w8a8_gemm(out, a, b, a_scales, b_scales, bias, M, N, K, workspace, workspace_bytes, st);
+  return path == kSimt ? simt_w8a8_gemm(out, a, b, a_scales, b_scales, bias, M, N, K, st) : path;
 }
 
 CB_DEFINE_TL_SETTER(linear)
