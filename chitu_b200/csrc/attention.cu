@@ -1029,6 +1029,7 @@ extern "C" int chitu_b200_mla_absorb_o_quant(const void* x, const void* wkv_b, v
                                              float* q_scales, int B, int H, int dn, int dv, int C, void* stream) {
   CB_ARG(x && wkv_b && (out || q_out) && B >= 0 && H > 0 && dn > 0 && dv > 0 && C > 0 && C % 8 == 0);
   CB_ARG(dv == 128 && (q_out == nullptr) == (q_scales == nullptr));
+  CB_ARG(((uintptr_t)x | (uintptr_t)wkv_b) % 16 == 0 && (uintptr_t)out % 8 == 0 && (uintptr_t)q_out % 4 == 0);
   if (B == 0) return 0;
   constexpr int MT = 2;          // tokens per CTA: 128 CTAs at bs = 16, one merge item per thread
   CB_ARG(dv % 32 == 0);
@@ -1048,6 +1049,8 @@ extern "C" int chitu_b200_mla_absorb_o_merge_quant(const void* workspace, int64_
                                                    int B, int H, int dn, int dv, int C, void* stream) {
   CB_ARG(workspace && wkv_b && (out || q_out) && B >= 0 && H > 0 && dn > 0 && dv == 128 && C == kMlaC);
   CB_ARG((q_out == nullptr) == (q_scales == nullptr) && max_seqlen_hint > 0);
+  CB_ARG(((uintptr_t)workspace | (uintptr_t)wkv_b) % 16 == 0 && ((uintptr_t)x_out | (uintptr_t)out) % 8 == 0 &&
+         (uintptr_t)q_out % 4 == 0);                                   // float4 partials, uint4 weights, uint2 rows
   if (B == 0) return 0;
   const int splits = mla_num_splits(B, H, max_seqlen_hint, workspace_bytes);
   CB_ARG(split_kv_bytes((int64_t)B * H, kMlaC, splits) <= workspace_bytes);
@@ -1170,6 +1173,7 @@ extern "C" int chitu_b200_mla_prep(const void* q, const void* kv_in, int64_t kv_
                                    void* stream) {
   CB_ARG(q && kv_in && kv_norm_w && cos && sin && wkv_b && q_abs && q_pe && new_kv);
   CB_ARG(B >= 0 && H > 0 && dn % 8 == 0 && C % 64 == 0 && R % 2 == 0);
+  CB_ARG((uintptr_t)wkv_b % 4 == 0);                                   // W_UK column pairs are read as uint32
   if (B == 0) return 0;
   constexpr int MT = 16;
   const int nA = (C / 64) * H * cdiv(B, MT);

@@ -33,14 +33,15 @@ __global__ void rotary_interleaved_kernel(const T* __restrict__ q, const T* __re
     }
     float c = cosp[(int64_t)b * half + i], s = sinp[(int64_t)b * half + i];
     float x0 = io<T>::to_f(src[2 * i]), x1 = io<T>::to_f(src[2 * i + 1]);
-    dst[2 * i] = io<T>::from_f(x0 * c - x1 * s);
-    dst[2 * i + 1] = io<T>::from_f(x1 * c + x0 * s);
+    // the contraction of the 16-byte kernel below, spelled out (left to nvcc, o1 became fma(x0, s, x1*c))
+    dst[2 * i] = io<T>::from_f(__fmaf_rn(x0, c, -__fmul_rn(x1, s)));
+    dst[2 * i + 1] = io<T>::from_f(__fmaf_rn(x1, c, __fmul_rn(x0, s)));
   }
 }
 
 // 16-byte variant for 2-byte dtypes: one thread rotates 4 adjacent pairs of one head (the scalar kernel above
 // spent 8.7 us on [16, 40, 128] — ten serial 2-byte round trips per thread and an integer division each).
-// Same arithmetic, same contraction: o0 = fma(x0, c, -(x1*s)), o1 = fma(x1, c, x0*s).
+// Same arithmetic, same contraction as the scalar kernel: o0 = fma(x0, c, -(x1*s)), o1 = fma(x1, c, x0*s).
 template <typename T>
 __global__ void __launch_bounds__(128) rotary_interleaved_vec_kernel(
     const T* __restrict__ q, const T* __restrict__ k, T* __restrict__ oq, T* __restrict__ ok,
@@ -151,9 +152,10 @@ __global__ void rotary_half_kernel(const T* __restrict__ x, T* __restrict__ out,
     T* dst = out + ((int64_t)b * heads + h) * head_dim;
     float c = io<T>::to_f(cosp[(int64_t)b * half + i]), s = io<T>::to_f(sinp[(int64_t)b * half + i]);
     float x0 = io<T>::to_f(src[i]), x1 = io<T>::to_f(src[i + half]);
-    // emulate the reference's dtype-level rounding of each product before the add
-    float p0 = io<T>::to_f(io<T>::from_f(x0 * c)), p1 = io<T>::to_f(io<T>::from_f(x1 * s));
-    float p2 = io<T>::to_f(io<T>::from_f(x1 * c)), p3 = io<T>::to_f(io<T>::from_f(x0 * s));
+    // emulate the reference's dtype-level rounding of each product before the add (__fmul_rn: for fp32 the round trip
+    // is a no-op, and nvcc would otherwise contract the product and the add into one fma)
+    float p0 = io<T>::to_f(io<T>::from_f(__fmul_rn(x0, c))), p1 = io<T>::to_f(io<T>::from_f(__fmul_rn(x1, s)));
+    float p2 = io<T>::to_f(io<T>::from_f(__fmul_rn(x1, c))), p3 = io<T>::to_f(io<T>::from_f(__fmul_rn(x0, s)));
     dst[i] = io<T>::from_f(p0 - p1);
     dst[i + half] = io<T>::from_f(p2 + p3);
   }
@@ -309,6 +311,7 @@ extern "C" int chitu_b200_rmsnorm_quant_fp8(const void* x, const void* w, void* 
   CB_ARG(x && w && (y || q) && rows >= 0 && dim > 0 && dim % 128 == 0 && dim <= 8192);
   CB_ARG((q == nullptr) == (q_scales == nullptr));
   CB_ARG(x_stride >= dim && x_stride % 4 == 0 && (y == nullptr || (y_stride >= dim && y_stride % 4 == 0)));
+  CB_ARG(((uintptr_t)x | (uintptr_t)w | (uintptr_t)y) % 8 == 0 && (uintptr_t)q % 4 == 0);   // uint2 rows, uint32 payload
   if (rows == 0) return 0;
   cb::launch_k(rmsnorm_quant_kernel, dim3(rows), dim3(256), 0, (cudaStream_t)stream, (const __nv_bfloat16*)x,
                (const __nv_bfloat16*)w, (__nv_bfloat16*)y, (uint8_t*)q, q_scales, dim, eps, x_stride, y_stride);
@@ -348,6 +351,7 @@ __global__ void silu_mul_quant_kernel(const __nv_bfloat16* __restrict__ x, uint8
 extern "C" int chitu_b200_silu_mul_quant_fp8(const void* x, void* q, float* q_scales, int64_t rows, int F,
                                              void* stream) {
   CB_ARG(x && q && q_scales && rows >= 0 && F > 0 && F % 128 == 0);
+  CB_ARG((uintptr_t)x % 8 == 0 && (uintptr_t)q % 4 == 0);                                  // uint2 rows, uint32 payload
   if (rows == 0) return 0;
   const int64_t ng = rows * (F / 128);
   cb::launch_k(silu_mul_quant_kernel, dim3((unsigned)((ng + 7) / 8)), dim3(256), 0, (cudaStream_t)stream,
@@ -556,6 +560,7 @@ extern "C" int chitu_b200_embedding(const int64_t* ids, const void* table, void*
   CB_ARG(ids && table && out && T >= 0 && dim > 0 && rows > 0);
   CB_ARG(dtype == CB_BF16 || dtype == CB_F16);
   CB_ARG((dim * 2) % 16 == 0);
+  CB_ARG(((uintptr_t)table | (uintptr_t)out) % 16 == 0);                                  // uint4 rows
   if (T == 0) return 0;
   cb::launch_k(embedding_kernel<uint16_t>, dim3(T), dim3(128), 0, (cudaStream_t)stream, ids, (const uint16_t*)table, (uint16_t*)out, dim, vocab_start, rows);
   CB_LAUNCHED(1);

@@ -53,6 +53,7 @@ __global__ void __launch_bounds__(kThreads) sample_kernel(const T* __restrict__ 
   __shared__ int s_above_cnt;
   __shared__ float s_scan[kThreads];
   __shared__ int s_pick;
+  __shared__ bool s_tail;
   const int b = blockIdx.x, tid = threadIdx.x;
   const T* row = logits + (int64_t)b * row_stride;
   const float inv_t = 1.f / temperatures[b];
@@ -111,6 +112,8 @@ __global__ void __launch_bounds__(kThreads) sample_kernel(const T* __restrict__ 
     __syncthreads();
   }
   const uint32_t thr = s_prefix;               // entries with key >= thr are kept
+  // ... except p == 0: the walk ends on the bin of p = 0 when the fp32 mass of the positive entries is <= top_p
+  auto kept_p = [&](float p) { return p > 0.f && okey(p) >= thr; };
 
   // ---- kept mass / count, then the inverse-CDF draw in vocabulary order ----
   const int per = (V + kThreads - 1) / kThreads;
@@ -119,7 +122,7 @@ __global__ void __launch_bounds__(kThreads) sample_kernel(const T* __restrict__ 
   int kept = 0;
   for (int i = i0; i < i1; ++i) {
     const float p = prob(i);
-    if (okey(p) >= thr) { part += p; ++kept; }
+    if (kept_p(p)) { part += p; ++kept; }
   }
   s_scan[tid] = part;
   const float z = block_reduce(part, false, red);
@@ -128,13 +131,17 @@ __global__ void __launch_bounds__(kThreads) sample_kernel(const T* __restrict__ 
   if (tid == 0) {
     const float target = uniforms[b] * z;
     float run = 0.f;
-    int pick = kThreads - 1;
+    int pick = -1;
     for (int t = 0; t < kThreads; ++t) {
       if (run + s_scan[t] > target) { pick = t; break; }
       run += s_scan[t];
     }
-    // the last thread with any kept entry if rounding pushed the target past the end
-    while (pick > 0 && s_scan[pick] == 0.f) --pick;
+    // rounding pushed the target past the end of the scan: the draw is the last kept entry (of the last thread with any)
+    s_tail = pick < 0;
+    if (pick < 0) {
+      pick = kThreads - 1;
+      while (pick > 0 && s_scan[pick] == 0.f) --pick;
+    }
     s_pick = pick;
     s_above_mass = run;
     if (out_kept) out_kept[b] = nkept;
@@ -147,10 +154,10 @@ __global__ void __launch_bounds__(kThreads) sample_kernel(const T* __restrict__ 
     int tok = -1, last = -1;
     for (int i = i0; i < i1; ++i) {
       const float p = prob(i);
-      if (okey(p) >= thr) {
+      if (kept_p(p)) {
         last = i;
         run += p;
-        if (run > target) { tok = i; break; }
+        if (!s_tail && run > target) { tok = i; break; }
       }
     }
     out_tokens[b] = tok >= 0 ? tok : last;

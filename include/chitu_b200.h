@@ -106,10 +106,12 @@ int chitu_b200_rmsnorm_strided(const void* x, const void* w, void* y, int rows, 
                                int64_t y_stride, float eps, int dtype, void* stream);
 /* Fused RMSNorm + act_quant_deepseek_v3 (the `norm -> linear_deepseek_v3` pairs of the DeepSeek layer,
  * model_deepseek_v3.py:488,1108,1113 + :53-106): reads the row once; writes y (bf16, may be NULL) and / or
- * the fp8 payload q [rows, dim] + scales [rows, dim/128] (both NULL to skip).  bf16, dim % 128 == 0. */
+ * the fp8 payload q [rows, dim] + scales [rows, dim/128] (both NULL to skip).  bf16, dim % 128 == 0; x / w / y 8-byte
+ * aligned, q 4-byte aligned. */
 int chitu_b200_rmsnorm_quant_fp8(const void* x, const void* w, void* y, void* q, float* q_scales, int rows,
                                  int dim, int64_t x_stride, int64_t y_stride, float eps, void* stream);
-/* Fused SiluAndMul + act_quant_deepseek_v3: x [rows, 2F] bf16 -> q fp8 [rows, F], scales [rows, F/128]. */
+/* Fused SiluAndMul + act_quant_deepseek_v3: x [rows, 2F] bf16 -> q fp8 [rows, F], scales [rows, F/128].  x 8-byte
+ * aligned, q 4-byte aligned. */
 int chitu_b200_silu_mul_quant_fp8(const void* x, void* q, float* q_scales, int64_t rows, int F, void* stream);
 /* SiluAndMul (fused_moe.py:24-39): out[r, :d] = silu(x[r, :d]) * x[r, d:2d]. */
 int chitu_b200_silu_and_mul(const void* x, void* out, int64_t rows, int d, int dtype, void* stream);
@@ -326,7 +328,7 @@ int chitu_b200_moe_grouped_gemm(const void* A, const void* B, void* C, const flo
 
 /* Sampling of the decode step (executor.py:104-110 + utils.py:62-81): softmax(logits / temperature), keep the entries
  * whose exclusive cumulative mass (descending order) is <= top_p and whose rank is < top_k, draw from the renormalised
- * kept set.  No sort: the kept set's probability threshold is found by a radix histogram; the draw is the inverse CDF
+ * kept set (an entry of probability 0 is never kept).  No sort: the kept set's probability threshold is found by a radix histogram; the draw is the inverse CDF
  * in vocabulary order at the caller's uniform u in [0,1) (same distribution as torch.multinomial; its RNG stream cannot
  * be reproduced).  logits [B, V] bf16 / fp16 / fp32 with row stride; top_ks int32 (<= 0 = off); out_kept / out_mass may
  * be NULL (size and mass of the kept set, diagnostics). */
@@ -360,7 +362,7 @@ int chitu_b200_mla_num_splits(int B, int H, int max_seqlen_hint, int64_t workspa
  * model_deepseek_v3.py:697 "bshc,hdc->bshd"; the q side, :529-531, is part of chitu_b200_mla_prep).  wkv_b: bf16
  * [H, dn+dv, C] (dequantised, ops.py:356-392); x: [B,H,C] bf16.  absorb_o + act_quant_deepseek_v3 of the result (the
  * input of the `wo` linear): out (bf16, may be NULL), q_out fp8 [B, H*dv], q_scales [B, H*dv/128]. dv must be 128
- * (one quantisation group per head). */
+ * (one quantisation group per head).  x / wkv_b 16-byte aligned, out 8-byte, q_out 4-byte. */
 int chitu_b200_mla_absorb_o_quant(const void* x, const void* wkv_b, void* out, void* q_out, float* q_scales,
                                   int B, int H, int dn, int dv, int C, void* stream);
 /* Same, but the latent input is the split-KV partials that chitu_b200_mla_decode(out = NULL) left in `workspace`
@@ -435,7 +437,7 @@ int chitu_b200_allreduce_residual_rmsnorm(void* handle, const void* partial, con
 
 /* ---- small decode-engine helpers (adjacent rows §8f; used by bench/engine) -------------------- */
 /* out[t,:] = table[ids[t],:]  (VocabParallelEmbedding local lookup, tensor_parallel.py:199-208;
- * rows outside [vocab_start, vocab_start+rows) produce zeros). */
+ * rows outside [vocab_start, vocab_start+rows) produce zeros).  table / out 16-byte aligned. */
 int chitu_b200_embedding(const int64_t* ids, const void* table, void* out, int T, int dim,
                          int64_t vocab_start, int64_t rows, int dtype, void* stream);
 /* y = a + b (residual add), bf16/fp16. */
