@@ -33,6 +33,7 @@ SIGNATURES = {
     "chitu_b200_version": (I, []),
     "chitu_b200_launch_count": (L, []),
     "chitu_b200_append_paged_kv": (I, [P, P, P, P, I, I, I, I, L, P]),
+    "chitu_b200_append_paged_kv_e4m3": (I, [P, P, P, P, I, I, I, I, P]),
     "chitu_b200_moe_align_block_size": (I, [P, I, L, I, I, P, P, P, P, P]),
     "chitu_b200_moe_gate_workspace_bytes": (L, [I, I]),
     "chitu_b200_moe_gate": (I, [P, P, P, I, I, I, I, I, I, I, I, F, P, P, I, P, L, P]),
@@ -64,6 +65,7 @@ SIGNATURES = {
     "chitu_b200_mla_decode": (I, [P, P, P, P, P, P, I, I, I, I, I, I, I, I, F, P, P, L, P]),
     "chitu_b200_mla_prefill": (I, [P, P, L, P, L, P, P, I, I, I, I, I, I, F, P, P]),
     "chitu_b200_mla_paged_prefill": (I, [P, P, P, P, P, P, I, I, I, I, I, I, I, I, I, I, F, P, P, L, P]),
+    "chitu_b200_mla_attn_fp8kv": (I, [P, P, P, P, P, P, I, I, I, I, I, I, I, I, I, I, F, P, P, L, P]),
     "chitu_b200_debug_timeline": (I, [P]),
     "chitu_b200_debug_timeline_names": (c_char_p, []),
     "chitu_b200_decode_prepare": (I, [P, P, P, I, P, P, P, I, I, I, P]),

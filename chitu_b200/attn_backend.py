@@ -6,9 +6,9 @@ prefill kernel; GQA prefill stays on flash_attn / torch SDPA), attn_with_kvcache
 with in-place append: the decode kernel for seqlen_q == 1, the sm_90a multi-token kernel for seqlen_q > 1 — chunked
 prefill, prefill on a cached prefix, speculative verification; over the paged cache with a block_table, in the io dtype
 or in fp8 e4m3 (half the KV bytes), and over the non-paged [B, S, Hkv, D] cache of KVCacheManager without one) and
-mla_attn_with_kvcache (absorbed-MLA attention over the paged latent cache: the decode kernel with fused append for one
-query token per request, the sm_90a multi-token kernel for seqlen_q > 1 — multi-token-prediction verification, chunked
-prefill on a cached prefix).
+mla_attn_with_kvcache (absorbed-MLA attention over the paged latent cache, in bf16 or fp8 e4m3: the decode kernel with
+fused append for one query token per request, the sm_90a multi-token kernel for seqlen_q > 1 — multi-token-prediction
+verification, chunked prefill on a cached prefix).
 """
 from __future__ import annotations
 
@@ -280,8 +280,11 @@ class B200AttnBackend(AttnBackend):
         """Absorbed-MLA attention over the paged latent cache.  q_nope [B, H, C] (or [B, 1, H, C]): one decode token
         per request with the fused append of `kv` (chitu_b200_mla_decode), returned as [B, 1, H, C].
         q_nope [B, sq, H, C] with sq > 1: multi-token-prediction verification or chunked prefill, see
-        `_mla_paged_prefill`."""
+        `_mla_paged_prefill`.  A kv_cache in torch.float8_e4m3fn takes both call shapes through `_mla_fp8kv`."""
         require_cuda(q_nope, q_pe, kv_cache, block_table)
+        if kv_cache.dtype == torch.float8_e4m3fn:
+            return self._mla_fp8kv(q_nope, q_pe, kv_cache, kv, cache_seqlens_excl_this_decode, block_table, causal,
+                                   window_size, softcap, softmax_scale)
         if q_nope.dim() == 4:
             B, sq, H, C = q_nope.shape
             if sq > 1:
@@ -340,4 +343,39 @@ class B200AttnBackend(AttnBackend):
             ptr(q_nope), ptr(q_pe), ptr(kv_cache), ptr(kv), ptr(seq_excl), ptr(block_table), block_table.stride(0), B, sq,
             H, C, R, page, kv_cache.size(0), int(hint), int(bool(causal)), float(softmax_scale), ptr(o), ptr(ws), wsn,
             current_stream()), "mla_paged_prefill")
+        return o
+
+    def _mla_fp8kv(self, q_nope, q_pe, kv_cache, kv, seq_excl, block_table, causal, window_size, softcap,
+                   softmax_scale):
+        """The e4m3 latent cache [num_blocks, 64, C + R] (chitu_b200_mla_attn_fp8kv), both call shapes: q_nope
+        [B, H, C] or [B, sq, H, C], bf16 q / kv / output.  The semantics of the bf16 cache, with each new kv element
+        stored as x.float().clamp(-448, 448).to(float8_e4m3fn) and each cache element decoded exactly to bf16 before
+        the unchanged arithmetic; the appended rows are attended in their stored form.  sq == 1 is the decode with the
+        fused append and the device split plan of prepare_metadata_for_decode; returns [B, sq, H, C].  No host
+        synchronisation, capturable in a CUDA graph, deterministic."""
+        if tuple(window_size) != (-1, -1) or softcap != 0.0:
+            raise RuntimeError("mla_attn_fp8kv: window_size and softcap are not built")
+        if q_nope.dtype != torch.bfloat16 or q_pe.dtype != torch.bfloat16 or (kv is not None and kv.dtype != torch.bfloat16):
+            raise RuntimeError("mla_attn_fp8kv: q_nope, q_pe and kv must be bfloat16 (only the cache is fp8)")
+        require_cuda(seq_excl, kv)
+        if q_nope.dim() == 3:
+            q_nope, q_pe = q_nope.unsqueeze(1), q_pe.unsqueeze(1)
+        B, sq, H, C = q_nope.shape
+        R = q_pe.shape[-1]
+        assert kv_cache.ndim == 3 and kv_cache.size(2) == C + R and q_pe.shape == (B, sq, H, R)
+        assert q_nope.is_contiguous() and q_pe.is_contiguous() and kv_cache.is_contiguous()
+        assert block_table.dtype == torch.int32 and block_table.stride(-1) == 1
+        assert seq_excl.dtype == torch.int32 and seq_excl.is_contiguous()
+        if kv is not None:
+            assert kv.is_contiguous() and kv.numel() == B * sq * (C + R)
+        if softmax_scale is None:
+            softmax_scale = 1.0 / ((self.qk_rope_head_dim + self.qk_nope_head_dim) ** 0.5)
+        page = kv_cache.size(1)
+        o = torch.empty(B, sq, H, C, dtype=q_nope.dtype, device=q_nope.device)
+        ws, wsn = self._ws(B, H, C, q_nope.device)
+        hint = self.max_seq_len if self.max_seq_len else block_table.shape[1] * page
+        check(_lib.load().chitu_b200_mla_attn_fp8kv(
+            ptr(q_nope), ptr(q_pe), ptr(kv_cache), ptr(kv), ptr(seq_excl), ptr(block_table), block_table.stride(0), B, sq,
+            H, C, R, page, kv_cache.size(0), int(hint), int(bool(causal)), float(softmax_scale), ptr(o), ptr(ws), wsn,
+            current_stream()), "mla_attn_fp8kv")
         return o

@@ -176,10 +176,25 @@ void launch_paged_append(PagedAppend c0, PagedAppend c1, int64_t row_bytes, cons
 // p >= cache_rows are skipped.
 void launch_contiguous_append(PagedAppend c0, PagedAppend c1, int64_t row_bytes, const int32_t* seqlens,
                               int64_t rows_sb, int cache_rows, int B, int sq, cudaStream_t st);
-// The paged append (true page indexing) into two e4m3 caches: rows of n io elements (dtype CB_BF16 | CB_F16,
-// n % 8 == 0, 16-byte aligned sources and strides) stored as e4m3 with io2_to_e4m3x2's rounding.
+// The paged append (true page indexing) into one or two e4m3 caches (c1.cache == NULL: one): rows of n io elements
+// (dtype CB_BF16 | CB_F16, n % 8 == 0, 16-byte aligned sources and strides) stored as e4m3 with io2_to_e4m3x2's
+// rounding.
 void launch_paged_append_e4m3(PagedAppend c0, PagedAppend c1, int n, int dtype, const int32_t* seqlens,
                               const int32_t* block_table, int bt_stride, int B, int sq, int page_size, cudaStream_t st);
+
+// ---- absorbed MLA over the paged latent cache (mla_tc.cu, mla_prefill.cu) ---------------------------------------------
+// The arguments of chitu_b200_mla_decode / chitu_b200_mla_paged_prefill over a bf16 cache, or (e4m3) over a cache of
+// e4m3 bytes with the store and read rules of chitu_b200_mla_attn_fp8kv.  Argument checks and launches report under
+// `entry`, the other refusals under `tag`.
+int mla_decode(const char* entry, const char* tag, bool e4m3, const void* q_nope, const void* q_pe, void* kv_cache,
+               const void* new_kv, const int32_t* seqlens_excl, const int32_t* block_table, int bt_stride, int B, int H,
+               int C, int R, int page_size, int num_blocks, int max_seqlen_hint, float softmax_scale, void* out,
+               void* workspace, int64_t workspace_bytes, cudaStream_t st);
+int mla_paged_prefill(const char* entry, const char* tag, bool e4m3, const void* q_nope, const void* q_pe,
+                      void* kv_cache, const void* new_kv, const int32_t* seqlens_excl, const int32_t* block_table,
+                      int bt_stride, int B, int sq, int H, int C, int R, int page_size, int num_blocks,
+                      int max_seqlen_hint, int causal, float softmax_scale, void* out, void* workspace,
+                      int64_t workspace_bytes, cudaStream_t st);
 
 // ---- GQA attention over the KV cache (attention.cu, gqa_prefill.cu) -------------------------------------------------
 // The cache layouts of the GQA entries: paged in the io dtype, contiguous [Bc, cache_rows, Hkv, D] (request b from row

@@ -134,7 +134,7 @@ __global__ void __launch_bounds__(128) contiguous_append_kernel(cb::PagedAppend 
   append_rows<true>(c0, c1, row_bytes, seqlens, nullptr, 0, B, 1, 1, rows_sb, cache_rows, vec);
 }
 
-// Rows of n io elements into two e4m3 caches, 8 elements (16 bytes in, 8 out) per thread and step.
+// Rows of n io elements into one or two e4m3 caches, 8 elements (16 bytes in, 8 out) per thread and step.
 template <typename T>
 __global__ void __launch_bounds__(128) paged_append_e4m3_kernel(cb::PagedAppend c0, cb::PagedAppend c1, int n,
                                                                 const int32_t* __restrict__ seqlens,
@@ -145,7 +145,7 @@ __global__ void __launch_bounds__(128) paged_append_e4m3_kernel(cb::PagedAppend 
   for (int b = blockIdx.y; b < B; b += gridDim.y) {
     const int p = seqlens[b] + i;
     const int64_t row = (int64_t)block_table[(int64_t)b * bt_stride + p / page_size] * page_size + p % page_size;
-    for (int u = threadIdx.x; u < 2 * (n / 8); u += blockDim.x) {
+    for (int u = threadIdx.x; u < (c1.cache ? 2 : 1) * (n / 8); u += blockDim.x) {
       const cb::PagedAppend& c = u < n / 8 ? c0 : c1;
       const int e = (u < n / 8 ? u : u - n / 8) * 8;
       const uint4 x = *reinterpret_cast<const uint4*>((const uint8_t*)c.src + b * c.src_sb + i * c.src_st + e * 2);
@@ -206,6 +206,20 @@ extern "C" int chitu_b200_append_paged_kv(void* kv_cache, const int32_t* page_ta
   if (batch == 0) return 0;
   cb::launch_paged_append({kv_cache, this_kv, row_bytes, row_bytes}, {}, row_bytes, old_seq_lens, page_table,
                           pages_per_sample, batch, 1, page_size, index_div, (cudaStream_t)stream);
+  CB_LAUNCHED(1);
+  return 0;
+}
+
+extern "C" int chitu_b200_append_paged_kv_e4m3(void* kv_cache, const int32_t* page_table, const void* this_kv,
+                                               const int32_t* old_seq_lens, int batch, int pages_per_sample, int n,
+                                               int dtype, void* stream) {
+  CB_ARG(kv_cache && page_table && this_kv && old_seq_lens);
+  CB_ARG(batch >= 0 && pages_per_sample > 0 && n > 0 && n % 8 == 0 && (dtype == CB_BF16 || dtype == CB_F16));
+  CB_ARG((uintptr_t)this_kv % 16 == 0);
+  if (batch == 0) return 0;
+  const int64_t row_bytes = (int64_t)n * 2;
+  cb::launch_paged_append_e4m3({kv_cache, this_kv, row_bytes, row_bytes}, {}, n, dtype, old_seq_lens, page_table,
+                               pages_per_sample, batch, 1, 64, (cudaStream_t)stream);
   CB_LAUNCHED(1);
   return 0;
 }

@@ -576,15 +576,16 @@ static PFN_encodeTiled get_encode() {
 bool tma_available() { return get_encode() != nullptr; }
 
 int make_tma_map_2d(CUtensorMap* map, const void* base, int64_t rows, int64_t cols, int elem_bytes,
-                    CUtensorMapDataType dt, int box_rows, int64_t row_stride) {
+                    CUtensorMapDataType dt, int box_rows, int64_t row_stride, int box_bytes) {
   PFN_encodeTiled enc = get_encode();
   if (!enc) return fail(-3, "cuTensorMapEncodeTiled is not available from the driver");
   cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
   cuuint64_t strides[1] = {(cuuint64_t)(row_stride > 0 ? row_stride : cols) * elem_bytes};
-  cuuint32_t box[2] = {(cuuint32_t)(128 / elem_bytes), (cuuint32_t)box_rows};
+  cuuint32_t box[2] = {(cuuint32_t)(box_bytes / elem_bytes), (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(map, dt, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  const CUtensorMapSwizzle sw = box_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE;
+  CUresult r = enc(map, dt, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
+                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS)
     return fail(-3, "cuTensorMapEncodeTiled failed (CUresult %d) rows=%lld cols=%lld", (int)r, (long long)rows, (long long)cols);
   return 0;

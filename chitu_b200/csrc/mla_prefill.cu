@@ -61,27 +61,58 @@ constexpr float kLog2e = 1.4426950408889634f;
 constexpr float kRescaleThreshold = 8.f;       // log2 domain
 constexpr int kThreads = 256;
 
-// one 64-key tile's chunks [c_begin, c_end) into their slots (issued by one thread)
+// one 64-key tile's chunks [c_begin, c_end) into their slots (issued by one thread).  e4m3: each chunk is a 4 KB box
+// [64 rows x 64 B] that lands in the upper half of its slot, where expand_e4m3 finds it.
+template <bool kFp8 = false>
 __device__ __forceinline__ void load_chunks(const CUtensorMap* mk, const CUtensorMap* mv, uint8_t* s_ring, uint64_t* full,
                                             int c_begin, int c_end, int row, uint64_t pol) {
+  constexpr int kLand = kFp8 ? kSlot / 2 : 0;
   for (int c = c_begin; c < c_end; ++c) {
-    mbar_expect_tx(&full[c], kSlot);
-    if (c < kKC) tma_load_2d(s_ring + c * kSlot, mk, &full[c], c * 64, row, pol);
-    else tma_load_2d(s_ring + c * kSlot, mv, &full[c], (c - kKC) * 64, row, pol);
+    mbar_expect_tx(&full[c], kSlot - kLand);
+    if (c < kKC) tma_load_2d(s_ring + c * kSlot + kLand, mk, &full[c], c * 64, row, pol);
+    else tma_load_2d(s_ring + c * kSlot + kLand, mv, &full[c], (c - kKC) * 64, row, pol);
+  }
+}
+
+// e4m3: the box in the upper half of `slot` expanded in place into the swizzled bf16 chunk [64 rows x 128 B] by one
+// warpgroup (t: thread in it, named barrier kBar), exact; rows >= zero_from are written as 0.  Thread t expands 16
+// bytes (row r, elements 16 u .. 16 u + 15) into bf16 units 2u, 2u + 1 of row r.  Every thread reads its 32 bytes
+// before the barrier and writes after it: the chunk's upper half is the box.  The caller fences and syncs before the
+// wgmma reads the chunk.
+template <int kBar>
+__device__ __forceinline__ void expand_e4m3(uint8_t* slot, int t, int zero_from) {
+  uint4 x[2];
+#pragma unroll
+  for (int j = 0; j < 2; ++j) x[j] = *reinterpret_cast<const uint4*>(slot + kSlot / 2 + (j * 128 + t) * 16);
+  asm volatile("bar.sync %0, 128;" ::"n"(kBar) : "memory");
+#pragma unroll
+  for (int j = 0; j < 2; ++j) {
+    const int task = j * 128 + t, r = task >> 2, u = task & 3;
+    if (r >= zero_from) x[j] = make_uint4(0, 0, 0, 0);
+    uint4 y0, y1;
+    E4m3<__nv_bfloat16>::to_io(x[j].x, y0.x, y0.y);
+    E4m3<__nv_bfloat16>::to_io(x[j].y, y0.z, y0.w);
+    E4m3<__nv_bfloat16>::to_io(x[j].z, y1.x, y1.y);
+    E4m3<__nv_bfloat16>::to_io(x[j].w, y1.z, y1.w);
+    *reinterpret_cast<uint4*>(slot + sw128(r, 2 * u)) = y0;
+    *reinterpret_cast<uint4*>(slot + sw128(r, 2 * u + 1)) = y1;
   }
 }
 
 // One CTA of either variant.  Contiguous (kPaged = false): sequence b's rows and keys start at cu_q[b] / cu_k[b], map_q
 // holds q as [Tq * H, 576].  Paged: request b has sq query tokens at q row b * sq * H (map_q = q_nope [., 512], map_qpe
 // = q_pe [., 64]), Lk = seqlens_excl[b] (+ sq when appended) keys, key tile t is cache page block_table[b, t], and the
-// CTA takes split `split` of its key tiles.
-template <bool kPaged>
+// CTA takes split `split` of its key tiles.  KV: the paged cache's element type, bf16 or e4m3 (the chunks are expanded
+// to bf16 in place, so the MMA code is the same).
+template <bool kPaged, typename KV = __nv_bfloat16>
 __device__ __forceinline__ void mla_prefill_cta(
     const CUtensorMap* map_q, const CUtensorMap* map_qpe, const CUtensorMap* map_k, const CUtensorMap* map_v,
     const int32_t* __restrict__ cu_q, const int32_t* __restrict__ cu_k, const int32_t* __restrict__ seqlens_excl,
     const int32_t* __restrict__ block_table, int bt_stride, int sq, int appended, int splits, int B, int H,
     int row_tiles, int causal, float scale, float* __restrict__ o_part, float* __restrict__ lse,
     __nv_bfloat16* __restrict__ out) {
+  constexpr bool kFp8 = std::is_same_v<KV, __nv_fp8_e4m3>;
+  static_assert(kPaged || !kFp8, "the e4m3 cache is paged");
   extern __shared__ __align__(1024) uint8_t mla_prefill_smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(mla_prefill_smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* s_ring = smem;                                   // [kTC][64 rows][128 B]  K / V chunks of one tile
@@ -149,7 +180,7 @@ __device__ __forceinline__ void mla_prefill_cta(
       } else {
         for (int c = 0; c < kKC; ++c) tma_load_2d(s_q + c * kSlot, map_q, &q_bar, c * 64, q0 * H + r0, l2_policy_evict_first());
       }
-      load_chunks(map_k, map_v, s_ring, full_b, 0, kTC, kPaged ? page_row(t_begin) : k0, pol_kv);
+      load_chunks<kFp8>(map_k, map_v, s_ring, full_b, 0, kTC, kPaged ? page_row(t_begin) : k0, pol_kv);
     }
   }
   if (threadIdx.x < kRows) s_m[threadIdx.x] = -INFINITY;
@@ -178,6 +209,14 @@ __device__ __forceinline__ void mla_prefill_cta(
     const int next_row = kPaged ? 0 : k0 + (it + 1) * kTile;
     if (wg0) {
       // ---- S^T = K . Q^T over the 9 chunks of 64 dims ----
+      if constexpr (kFp8) {                                 // K rows past Lk keep their bytes: masked below
+        for (int c = 0; c < kKC; ++c) {
+          mbar_wait(&full_b[c], ph);
+          expand_e4m3<1>(s_ring + c * kSlot, threadIdx.x, kTile);
+        }
+        fence_async_smem();
+        asm volatile("bar.sync 1, 128;" ::: "memory");
+      }
       float s[32];
 #pragma unroll
       for (int e = 0; e < 32; ++e) s[e] = 0.f;
@@ -257,7 +296,7 @@ __device__ __forceinline__ void mla_prefill_cta(
       // ---- WG1: the K slots are free once P(it) is published; then the rescale WG0 decided for this tile ----
       mbar_wait(&p_full, ph);
       if (more && threadIdx.x == 128)
-        load_chunks(map_k, map_v, s_ring, full_b, 0, kKC, kPaged ? page_row(t_begin + it + 1) : next_row, pol_kv);
+        load_chunks<kFp8>(map_k, map_v, s_ring, full_b, 0, kKC, kPaged ? page_row(t_begin + it + 1) : next_row, pol_kv);
       float al[16];
       bool need = false;
 #pragma unroll
@@ -274,7 +313,18 @@ __device__ __forceinline__ void mla_prefill_cta(
         }
       }
     }
-    if constexpr (kPaged) {
+    if constexpr (kFp8) {
+      // ---- e4m3: this warpgroup's V chunks expanded, with the rows of keys >= Lk zeroed as below ----
+      for (int m = 0; m < 4; ++m) {
+        const int c = kKC + vc0 + m;
+        mbar_wait(&full_b[c], ph);
+        if (wg0) expand_e4m3<1>(s_ring + c * kSlot, threadIdx.x, Lk - key0);
+        else expand_e4m3<3>(s_ring + c * kSlot, threadIdx.x - 128, Lk - key0);
+      }
+      fence_async_smem();
+      if (wg0) asm volatile("bar.sync 1, 128;" ::: "memory");
+      else asm volatile("bar.sync 3, 128;" ::: "memory");
+    } else if constexpr (kPaged) {
       // ---- the tile holding Lk: V rows of keys >= Lk are unwritten cache slots (maybe NaN) and 0 * NaN would poison
       // O, so they are zeroed (whole 128 B rows: the swizzle permutes within a row) in this warpgroup's V chunks ----
       if (key0 + kTile > Lk) {
@@ -307,8 +357,8 @@ __device__ __forceinline__ void mla_prefill_cta(
       if (wg0) asm volatile("bar.sync 1, 128;" ::: "memory");
       else asm volatile("bar.sync 3, 128;" ::: "memory");
       if ((threadIdx.x & 127) == 0)
-        load_chunks(map_k, map_v, s_ring, full_b, kKC + vc0, kKC + vc0 + 4,
-                    kPaged ? page_row(t_begin + it + 1) : next_row, pol_kv);
+        load_chunks<kFp8>(map_k, map_v, s_ring, full_b, kKC + vc0, kKC + vc0 + 4,
+                          kPaged ? page_row(t_begin + it + 1) : next_row, pol_kv);
     }
   }
 
@@ -397,6 +447,18 @@ __global__ void __launch_bounds__(kThreads, 1) mla_paged_prefill_kernel(
                         appended, splits, B, H, row_tiles, causal, scale, o_part, lse, out);
 }
 
+// The same over an e4m3 cache: map_kv holds the cache as bytes, box = [64 rows x 64 B], no swizzle
+__global__ void __launch_bounds__(kThreads, 1) mla_paged_prefill_e4m3_kernel(
+    const __grid_constant__ CUtensorMap map_qn, const __grid_constant__ CUtensorMap map_qpe,
+    const __grid_constant__ CUtensorMap map_kv, const int32_t* __restrict__ seqlens_excl,
+    const int32_t* __restrict__ block_table, int bt_stride, int B, int sq, int H, int appended, int row_tiles,
+    int splits, int causal, float scale, float* __restrict__ o_part, float* __restrict__ lse,
+    __nv_bfloat16* __restrict__ out) {
+  mla_prefill_cta<true, __nv_fp8_e4m3>(&map_qn, &map_qpe, &map_kv, &map_kv, nullptr, nullptr, seqlens_excl, block_table,
+                                       bt_stride, sq, appended, splits, B, H, row_tiles, causal, scale, o_part, lse,
+                                       out);
+}
+
 }  // namespace
 }  // namespace cb
 
@@ -430,21 +492,23 @@ extern "C" int chitu_b200_mla_prefill(const void* q, const void* k, int64_t k_sb
   return 0;
 }
 
-// mla_attn_with_kvcache with more than one query token per request (include/chitu_b200.h).
-extern "C" int chitu_b200_mla_paged_prefill(const void* q_nope, const void* q_pe, void* kv_cache, const void* new_kv,
-                                            const int32_t* seqlens_excl, const int32_t* block_table, int bt_stride,
-                                            int B, int sq, int H, int C, int R, int page_size, int num_blocks,
-                                            int max_seqlen_hint, int causal, float softmax_scale, void* out,
-                                            void* workspace, int64_t workspace_bytes, void* stream) {
-  using namespace cb;
-  CB_ARG(q_nope && q_pe && kv_cache && seqlens_excl && block_table && out);
-  CB_ARG(B >= 0 && sq >= 1 && H >= 1 && bt_stride > 0 && num_blocks > 0);
+namespace cb {
+// chitu_b200_mla_paged_prefill (e4m3 = false) and the sq > 1 form of chitu_b200_mla_attn_fp8kv (e4m3: kv_cache holds
+// e4m3 bytes, the new rows are stored by the e4m3 append).  Argument checks and launches report under `entry`, the
+// other refusals under `tag`.
+int mla_paged_prefill(const char* entry, const char* tag, bool e4m3, const void* q_nope, const void* q_pe,
+                      void* kv_cache, const void* new_kv, const int32_t* seqlens_excl, const int32_t* block_table,
+                      int bt_stride, int B, int sq, int H, int C, int R, int page_size, int num_blocks,
+                      int max_seqlen_hint, int causal, float softmax_scale, void* out, void* workspace,
+                      int64_t workspace_bytes, cudaStream_t st) {
+  CB_ARG_AS(entry, q_nope && q_pe && kv_cache && seqlens_excl && block_table && out);
+  CB_ARG_AS(entry, B >= 0 && sq >= 1 && H >= 1 && bt_stride > 0 && num_blocks > 0);
   if (C != kC || R != kR)
-    return fail(-1, "mla_paged_prefill: only kv_lora_rank=512, qk_rope_head_dim=64 is built (got %d,%d)", C, R);
-  if (page_size != kTile) return fail(-1, "mla_paged_prefill: page_size must be 64 (got %d)", page_size);
-  CB_ARG(((uintptr_t)q_nope | (uintptr_t)q_pe | (uintptr_t)kv_cache | (uintptr_t)new_kv | (uintptr_t)out |
-          (uintptr_t)workspace) % 16 == 0);                                     // TMA / vector accesses: 16-byte bases
-  CB_ARG((int64_t)B * sq * H <= INT_MAX && (int64_t)num_blocks * kTile <= INT_MAX);   // int32 TMA row coordinates
+    return fail(-1, "%s: only kv_lora_rank=512, qk_rope_head_dim=64 is built (got %d,%d)", tag, C, R);
+  if (page_size != kTile) return fail(-1, "%s: page_size must be 64 (got %d)", tag, page_size);
+  CB_ARG_AS(entry, ((uintptr_t)q_nope | (uintptr_t)q_pe | (uintptr_t)kv_cache | (uintptr_t)new_kv | (uintptr_t)out |
+                    (uintptr_t)workspace) % 16 == 0);                           // TMA / vector accesses: 16-byte bases
+  CB_ARG_AS(entry, (int64_t)B * sq * H <= INT_MAX && (int64_t)num_blocks * kTile <= INT_MAX);   // int32 TMA rows
   if (B == 0) return 0;
 
   const int row_tiles = cdiv((int64_t)sq * H, kRows);
@@ -454,36 +518,80 @@ extern "C" int chitu_b200_mla_paged_prefill(const void* q_nope, const void* q_pe
   int splits = pick_splits_waves(row_tiles * B, max_len, 132);
   splits = workspace ? splits_that_fit(splits, rows, kC, workspace_bytes) : 1;
   if ((int64_t)row_tiles * splits * B > INT_MAX)
-    return fail(-1, "mla_paged_prefill: %d requests x %d row tiles x %d splits exceed the grid", B, row_tiles, splits);
-  if (!tma_available()) return fail(-3, "mla_paged_prefill: TMA is not available");
+    return fail(-1, "%s: %d requests x %d row tiles x %d splits exceed the grid", tag, B, row_tiles, splits);
+  if (!tma_available()) return fail(-3, "%s: TMA is not available", tag);
   const auto [o_part, lse, plan] = split_kv_carve(splits > 1 ? workspace : nullptr, workspace_bytes, rows, kC, splits);
 
   CUtensorMap mqn, mqp, mkv;
   int rc = make_tma_map_2d(&mqn, q_nope, rows, kC, 2, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, kRows);
   if (!rc) rc = make_tma_map_2d(&mqp, q_pe, rows, kR, 2, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, kRows);
-  if (!rc) rc = make_tma_map_2d(&mkv, kv_cache, (int64_t)num_blocks * kTile, kRow, 2, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16,
-                                kTile);
+  if (!rc && e4m3)    // one box per 64-element chunk, landed in half of its slot
+    rc = make_tma_map_2d(&mkv, kv_cache, (int64_t)num_blocks * kTile, kRow, 1, CU_TENSOR_MAP_DATA_TYPE_UINT8, kTile, 0,
+                         64);
+  else if (!rc)
+    rc = make_tma_map_2d(&mkv, kv_cache, (int64_t)num_blocks * kTile, kRow, 2, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16,
+                         kTile);
   if (rc) return rc;
 
-  cudaStream_t st = (cudaStream_t)stream;
   if (new_kv) {       // the B * sq new latent rows first, pages indexed with a literal 64 as the reference's append does
     const int64_t row_bytes = kRow * 2;
-    launch_paged_append({kv_cache, new_kv, sq * row_bytes, row_bytes}, {}, row_bytes, seqlens_excl, block_table,
-                        bt_stride, B, sq, kTile, 64, st);
-    CB_LAUNCHED(1);
+    if (e4m3)
+      launch_paged_append_e4m3({kv_cache, new_kv, sq * row_bytes, row_bytes}, {}, kRow, CB_BF16, seqlens_excl,
+                               block_table, bt_stride, B, sq, kTile, st);
+    else
+      launch_paged_append({kv_cache, new_kv, sq * row_bytes, row_bytes}, {}, row_bytes, seqlens_excl, block_table,
+                          bt_stride, B, sq, kTile, 64, st);
+    CB_LAUNCHED_AS(entry, 1);
   }
-  rc = launch_smem<mla_paged_prefill_kernel>(__func__, dim3(row_tiles * splits * B), dim3(kThreads),
-                                             1024 + kSmemBytes, st, mqn, mqp, mkv, seqlens_excl, block_table, bt_stride,
-                                             B, sq, H, new_kv ? 1 : 0, row_tiles, splits, causal ? 1 : 0,
-                                             softmax_scale, o_part, lse, (__nv_bfloat16*)out);
+  const dim3 grid(row_tiles * splits * B), block(kThreads);
+  const int appended = new_kv ? 1 : 0;
+  causal = causal ? 1 : 0;
+  if (e4m3)
+    rc = launch_smem<mla_paged_prefill_e4m3_kernel>(entry, grid, block, 1024 + kSmemBytes, st, mqn, mqp, mkv,
+                                                    seqlens_excl, block_table, bt_stride, B, sq, H, appended,
+                                                    row_tiles, splits, causal, softmax_scale, o_part, lse,
+                                                    (__nv_bfloat16*)out);
+  else
+    rc = launch_smem<mla_paged_prefill_kernel>(entry, grid, block, 1024 + kSmemBytes, st, mqn, mqp, mkv, seqlens_excl,
+                                               block_table, bt_stride, B, sq, H, appended, row_tiles, splits, causal,
+                                               softmax_scale, o_part, lse, (__nv_bfloat16*)out);
   if (rc) return rc;
-  CB_LAUNCHED(1);
+  CB_LAUNCHED_AS(entry, 1);
   if (splits > 1) {
     rc = launch_merge_splits(o_part, lse, out, (int)rows, splits, kC, CB_BF16, st);
     if (rc) return rc;
-    CB_LAUNCHED(1);
+    CB_LAUNCHED_AS(entry, 1);
   }
   return 0;
+}
+}  // namespace cb
+
+// mla_attn_with_kvcache with more than one query token per request (include/chitu_b200.h).
+extern "C" int chitu_b200_mla_paged_prefill(const void* q_nope, const void* q_pe, void* kv_cache, const void* new_kv,
+                                            const int32_t* seqlens_excl, const int32_t* block_table, int bt_stride,
+                                            int B, int sq, int H, int C, int R, int page_size, int num_blocks,
+                                            int max_seqlen_hint, int causal, float softmax_scale, void* out,
+                                            void* workspace, int64_t workspace_bytes, void* stream) {
+  return cb::mla_paged_prefill(__func__, "mla_paged_prefill", false, q_nope, q_pe, kv_cache, new_kv, seqlens_excl,
+                               block_table, bt_stride, B, sq, H, C, R, page_size, num_blocks, max_seqlen_hint, causal,
+                               softmax_scale, out, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+// mla_attn_with_kvcache over an e4m3 paged latent cache (include/chitu_b200.h): sq == 1 the decode kernel, sq > 1 the
+// multi-token kernel, both with the cache type as a compile-time parameter of the bf16 kernels' CTA.
+extern "C" int chitu_b200_mla_attn_fp8kv(const void* q_nope, const void* q_pe, void* kv_cache, const void* new_kv,
+                                         const int32_t* seqlens_excl, const int32_t* block_table, int bt_stride, int B,
+                                         int sq, int H, int C, int R, int page_size, int num_blocks,
+                                         int max_seqlen_hint, int causal, float softmax_scale, void* out,
+                                         void* workspace, int64_t workspace_bytes, void* stream) {
+  CB_ARG(sq >= 1);
+  if (sq == 1)      // one token: causal changes nothing (its only row sees every key)
+    return cb::mla_decode(__func__, __func__, true, q_nope, q_pe, kv_cache, new_kv, seqlens_excl, block_table,
+                          bt_stride, B, H, C, R, page_size, num_blocks, max_seqlen_hint, softmax_scale, out, workspace,
+                          workspace_bytes, (cudaStream_t)stream);
+  return cb::mla_paged_prefill(__func__, __func__, true, q_nope, q_pe, kv_cache, new_kv, seqlens_excl, block_table,
+                               bt_stride, B, sq, H, C, R, page_size, num_blocks, max_seqlen_hint, causal, softmax_scale,
+                               out, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 CB_DEFINE_TL_SETTER(mla_prefill)

@@ -32,14 +32,31 @@ namespace {
 constexpr int kC = kMlaC, kR = 64, kRow = kC + kR;
 constexpr int kTile = 64;                      // keys per tile == page size
 constexpr int kSlot = kTile * 128;             // 8 KB: one TMA box [64 keys x 128 B]
-constexpr int kNSM = 22;                       // main ring slots
-constexpr int kNSR = 3;                        // rope ring slots
+constexpr int kESlot = kTile * 64;             // 4 KB: one e4m3 box [64 keys x 64 B] (one chunk of 64 elements)
 constexpr int kQBytes = 9 * 16 * 128;          // Q as 9 K-major chunks of [16 heads x 128 B]
 constexpr int kPBytes = 16 * 128;              // P as [16 heads x 64 keys] bf16, K-major
-constexpr int kSmemBytes = kNSM * kSlot + kNSR * kSlot + kQBytes + 2 * kPBytes;
 constexpr float kLog2e = 1.4426950408889634f;
 constexpr float kRescaleThreshold = 8.f;       // log2 domain
-constexpr int kThreads = 160;                  // warpgroup (warps 0-3) + producer warp
+
+// The CTA's shape for a cache element type KV.  bf16: warpgroup (warps 0-3) + producer warp, a ring of 22 latent and
+// 3 rope slots.  e4m3: the producer streams each page as 9 boxes of 4 KB into a ring of 14 e4m3 slots, and four
+// converter warps (5-8) expand them into the bf16 rings (16 latent = two pages, 2 rope), so the MMA warps read the same
+// swizzled bf16 chunks and never convert.
+template <typename KV> struct DecodeShape {
+  static constexpr bool kFp8 = false;
+  static constexpr int kNSM = 22, kNSR = 3, kNE = 0, kThreads = 160;
+};
+template <> struct DecodeShape<__nv_fp8_e4m3> {
+  static constexpr bool kFp8 = true;
+  static constexpr int kNSM = 16, kNSR = 2, kNE = 14, kThreads = 288;
+};
+template <typename KV>
+constexpr int decode_smem_bytes() {
+  using S = DecodeShape<KV>;                   // e4m3: the ring's full / empty barriers follow P
+  return (S::kNSM + S::kNSR) * kSlot + kQBytes + 2 * kPBytes + S::kNE * (kESlot + 16);
+}
+static_assert(1024 + decode_smem_bytes<__nv_bfloat16>() <= 227 * 1024, "bf16 decode CTA exceeds shared memory");
+static_assert(1024 + decode_smem_bytes<__nv_fp8_e4m3>() <= 227 * 1024, "e4m3 decode CTA exceeds shared memory");
 
 // dev tool (profiling build only, -DCB_TIMELINE): %globaltimer at fixed points of every CTA, 32 slots per CTA, read by
 // scripts/mla_probe.py.  The product library compiles these to nothing.
@@ -65,13 +82,18 @@ __device__ __forceinline__ float pick16(const float (&v)[16], int h) {
   return r;
 }
 
-__global__ void __launch_bounds__(kThreads, 1) mla_decode_tc_kernel(
-    const __grid_constant__ CUtensorMap map_kv, const __nv_bfloat16* __restrict__ q_nope,
-    const __nv_bfloat16* __restrict__ q_pe, __nv_bfloat16* __restrict__ kv_cache,
+// One CTA for cache elements KV (bf16 | e4m3).  The MMA warps are the same code for both.
+template <typename KV>
+__device__ __forceinline__ void mla_decode_cta(
+    const CUtensorMap& map_kv, const __nv_bfloat16* __restrict__ q_nope,
+    const __nv_bfloat16* __restrict__ q_pe, KV* __restrict__ kv_cache,
     const __nv_bfloat16* __restrict__ new_kv, const int32_t* __restrict__ seqlens_excl,
     const int32_t* __restrict__ block_table, int bt_stride, int H, float scale, int num_splits,
     float* __restrict__ o_part, float* __restrict__ lse, __nv_bfloat16* __restrict__ out,
     const int32_t* __restrict__ plan) {
+  using S = DecodeShape<KV>;
+  constexpr bool kFp8 = S::kFp8;
+  constexpr int kNSM = S::kNSM, kNSR = S::kNSR, kNE = S::kNE;
   extern __shared__ __align__(1024) uint8_t mla_tc_smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(mla_tc_smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* s_ring = smem;                                   // [kNSM][64 keys][128 B]   latent chunks
@@ -80,6 +102,9 @@ __global__ void __launch_bounds__(kThreads, 1) mla_decode_tc_kernel(
   uint8_t* s_p = s_q + kQBytes;                             // [2][16 heads][128 B]
   __shared__ __align__(8) uint64_t full_m[kNSM], empty_m[kNSM], full_r[kNSR], empty_r[kNSR], raw_bar;
   __shared__ float red_max[4][16], red_sum[4][16];
+  uint8_t* s_e = s_p + 2 * kPBytes;                         // e4m3: [kNE][64 keys][64 B]
+  uint64_t* full_e = reinterpret_cast<uint64_t*>(s_e + kNE * kESlot);
+  uint64_t* empty_e = full_e + kNE;
 
   const int split = blockIdx.x, hg = blockIdx.y, b = blockIdx.z;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -87,8 +112,10 @@ __global__ void __launch_bounds__(kThreads, 1) mla_decode_tc_kernel(
 
   if (threadIdx.x == 0) {
     probe(0);
-    for (int i = 0; i < kNSM; ++i) { mbar_init(&full_m[i], 1); mbar_init(&empty_m[i], 1); }
-    for (int i = 0; i < kNSR; ++i) { mbar_init(&full_r[i], 1); mbar_init(&empty_r[i], 1); }
+    // e4m3: a bf16 slot is published by the four converter warps, an e4m3 slot released by them
+    for (int i = 0; i < kNSM; ++i) { mbar_init(&full_m[i], kFp8 ? 4 : 1); mbar_init(&empty_m[i], 1); }
+    for (int i = 0; i < kNSR; ++i) { mbar_init(&full_r[i], kFp8 ? 4 : 1); mbar_init(&empty_r[i], 1); }
+    for (int i = 0; i < kNE; ++i) { mbar_init(&full_e[i], 1); mbar_init(&empty_e[i], 4); }
     mbar_init(&raw_bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_kv) : "memory");
@@ -113,7 +140,81 @@ __global__ void __launch_bounds__(kThreads, 1) mla_decode_tc_kernel(
   const int ntiles = end > begin ? (end - begin + kTile - 1) / kTile : 0;
   const int32_t* bt = block_table + (int64_t)b * bt_stride;
 
-  if (warp == 4) {
+  if (kFp8 && warp == 4) {
+    // ================= e4m3 TMA producer: the 9 boxes of each page, in order, through the e4m3 ring =================
+    constexpr int kNEr = kFp8 ? kNE : 1;                    // (the bf16 instance compiles this branch away)
+    const uint64_t pol = l2_policy_evict_first();
+    for (int it = 0; it < ntiles; ++it) {
+      const int row0 = bt[(begin + it * kTile) / kTile] * kTile;
+      for (int c = 0; c < 9; ++c) {
+        const int g = it * 9 + c, s = g % kNEr;
+        mbar_wait(&empty_e[s], ((g / kNEr) & 1) ^ 1);
+        if (lane == 0) {
+          mbar_expect_tx(&full_e[s], kESlot);
+          tma_load_2d(s_e + s * kESlot, &map_kv, &full_e[s], c * 64, row0, pol);
+        }
+      }
+    }
+  } else if (kFp8 && warp > 4) {
+    // ================= e4m3 converter warps: e4m3 box -> swizzled bf16 chunk, exact =================
+    // A thread expands 16 bytes (row r, elements 16 u .. 16 u + 15 of the chunk) into bf16 units 2u, 2u + 1 of row r:
+    // the loads are contiguous and each store instruction touches every 16-byte bank group four times.  In the page
+    // that holds the end of the sequence the appended token's row is the stored form of `new_kv` (its cache write may
+    // not have landed) and rows past the end are zero (0 * garbage must not poison P.V).
+    constexpr int kNEr = kFp8 ? kNE : 1;
+    const int ct = threadIdx.x - 160;                       // 0..127
+    bool waited = false;
+    for (int it = 0; it < ntiles; ++it) {
+      const int key0 = begin + it * kTile;
+      const int valid_rows = min(kTile, L - key0);
+      const int rnew = (new_kv && L - 1 >= key0 && L - 1 < key0 + kTile) ? L - 1 - key0 : -1;
+      if (rnew >= 0 && !waited) { cb::pdl_wait(); waited = true; }     // new_kv is written by the previous kernel
+      for (int c = 0; c < 9; ++c) {
+        const int ge = it * 9 + c, se = ge % kNEr;
+        uint8_t* dst;
+        uint64_t* full;
+        if (c < 8) {
+          const int g = it * 8 + c, s = g % kNSM;
+          mbar_wait(&empty_m[s], ((g / kNSM) & 1) ^ 1);
+          dst = s_ring + s * kSlot;
+          full = &full_m[s];
+        } else {
+          const int rs = it % kNSR;
+          mbar_wait(&empty_r[rs], ((it / kNSR) & 1) ^ 1);
+          dst = s_rope + rs * kSlot;
+          full = &full_r[rs];
+        }
+        mbar_wait(&full_e[se], (ge / kNEr) & 1);
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+          const int task = j * 128 + ct, r = task >> 2, u = task & 3;
+          uint4 x = *reinterpret_cast<const uint4*>(s_e + se * kESlot + task * 16);
+          if (r == rnew) {
+            const uint4* src = reinterpret_cast<const uint4*>(new_kv + (int64_t)b * kRow + c * 64 + u * 16);
+            const uint4 n0 = src[0], n1 = src[1];
+            x = make_uint4(io2_to_e4m3x2<__nv_bfloat16>(n0.x) | io2_to_e4m3x2<__nv_bfloat16>(n0.y) << 16,
+                           io2_to_e4m3x2<__nv_bfloat16>(n0.z) | io2_to_e4m3x2<__nv_bfloat16>(n0.w) << 16,
+                           io2_to_e4m3x2<__nv_bfloat16>(n1.x) | io2_to_e4m3x2<__nv_bfloat16>(n1.y) << 16,
+                           io2_to_e4m3x2<__nv_bfloat16>(n1.z) | io2_to_e4m3x2<__nv_bfloat16>(n1.w) << 16);
+          }
+          if (r >= valid_rows) x = make_uint4(0, 0, 0, 0);
+          uint4 y0, y1;
+          E4m3<__nv_bfloat16>::to_io(x.x, y0.x, y0.y);
+          E4m3<__nv_bfloat16>::to_io(x.y, y0.z, y0.w);
+          E4m3<__nv_bfloat16>::to_io(x.z, y1.x, y1.y);
+          E4m3<__nv_bfloat16>::to_io(x.w, y1.z, y1.w);
+          *reinterpret_cast<uint4*>(dst + sw128(r, 2 * u)) = y0;
+          *reinterpret_cast<uint4*>(dst + sw128(r, 2 * u + 1)) = y1;
+        }
+        fence_async_smem();
+        __syncwarp();
+        if (lane == 0) {
+          mbar_arrive(&empty_e[se]);
+          mbar_arrive(full);
+        }
+      }
+    }
+  } else if (!kFp8 && warp == 4) {
     // ================= TMA producer (whole warp: lane 0 issues, all lanes patch the tail page) =================
     const uint64_t pol = l2_policy_evict_first();
     uint32_t raw_phase = 0;
@@ -210,9 +311,18 @@ __global__ void __launch_bounds__(kThreads, 1) mla_decode_tc_kernel(
     if (t == 0) probe(2);
     if (new_kv && split == 0 && hg == 0) {                   // append for the following steps (ops.py:50-91)
       const int page = bt[L_cache / kTile];
-      __nv_bfloat16* dst = kv_cache + ((int64_t)page * kTile + L_cache % kTile) * kRow;
+      KV* dst = kv_cache + ((int64_t)page * kTile + L_cache % kTile) * kRow;
       const __nv_bfloat16* src = new_kv + (int64_t)b * kRow;
-      for (int i = t; i < kRow / 8; i += 128) reinterpret_cast<uint4*>(dst)[i] = reinterpret_cast<const uint4*>(src)[i];
+      if constexpr (kFp8) {                                  // 8 elements -> 8 e4m3 bytes, the store rule of the cache
+        for (int i = t; i < kRow / 8; i += 128) {
+          const uint4 x = reinterpret_cast<const uint4*>(src)[i];
+          reinterpret_cast<uint2*>(dst)[i] = make_uint2(
+              io2_to_e4m3x2<__nv_bfloat16>(x.x) | io2_to_e4m3x2<__nv_bfloat16>(x.y) << 16,
+              io2_to_e4m3x2<__nv_bfloat16>(x.z) | io2_to_e4m3x2<__nv_bfloat16>(x.w) << 16);
+        }
+      } else {
+        for (int i = t; i < kRow / 8; i += 128) reinterpret_cast<uint4*>(dst)[i] = reinterpret_cast<const uint4*>(src)[i];
+      }
     }
 
     const uint32_t ring_a = smem_u32(s_ring), rope_a = smem_u32(s_rope), q_a = smem_u32(s_q), p_a = smem_u32(s_p);
@@ -364,8 +474,86 @@ __global__ void __launch_bounds__(kThreads, 1) mla_decode_tc_kernel(
   }
 }
 
+__global__ void __launch_bounds__(DecodeShape<__nv_bfloat16>::kThreads, 1) mla_decode_tc_kernel(
+    const __grid_constant__ CUtensorMap map_kv, const __nv_bfloat16* __restrict__ q_nope,
+    const __nv_bfloat16* __restrict__ q_pe, __nv_bfloat16* __restrict__ kv_cache,
+    const __nv_bfloat16* __restrict__ new_kv, const int32_t* __restrict__ seqlens_excl,
+    const int32_t* __restrict__ block_table, int bt_stride, int H, float scale, int num_splits,
+    float* __restrict__ o_part, float* __restrict__ lse, __nv_bfloat16* __restrict__ out,
+    const int32_t* __restrict__ plan) {
+  mla_decode_cta(map_kv, q_nope, q_pe, kv_cache, new_kv, seqlens_excl, block_table, bt_stride, H, scale, num_splits,
+                 o_part, lse, out, plan);
+}
+
+// map_kv: the cache as e4m3 bytes, box = [64 rows x 64 B], no swizzle
+__global__ void __launch_bounds__(DecodeShape<__nv_fp8_e4m3>::kThreads, 1) mla_decode_e4m3_kernel(
+    const __grid_constant__ CUtensorMap map_kv, const __nv_bfloat16* __restrict__ q_nope,
+    const __nv_bfloat16* __restrict__ q_pe, __nv_fp8_e4m3* __restrict__ kv_cache,
+    const __nv_bfloat16* __restrict__ new_kv, const int32_t* __restrict__ seqlens_excl,
+    const int32_t* __restrict__ block_table, int bt_stride, int H, float scale, int num_splits,
+    float* __restrict__ o_part, float* __restrict__ lse, __nv_bfloat16* __restrict__ out,
+    const int32_t* __restrict__ plan) {
+  mla_decode_cta(map_kv, q_nope, q_pe, kv_cache, new_kv, seqlens_excl, block_table, bt_stride, H, scale, num_splits,
+                 o_part, lse, out, plan);
+}
+
 }  // namespace
 
+// chitu_b200_mla_decode (e4m3 = false) and the sq == 1 form of chitu_b200_mla_attn_fp8kv (e4m3: kv_cache holds e4m3
+// bytes).  Argument checks and launches report under `entry`, the other refusals under `tag`.
+int mla_decode(const char* entry, const char* tag, bool e4m3, const void* q_nope, const void* q_pe, void* kv_cache,
+               const void* new_kv, const int32_t* seqlens_excl, const int32_t* block_table, int bt_stride, int B, int H,
+               int C, int R, int page_size, int num_blocks, int max_seqlen_hint, float softmax_scale, void* out,
+               void* workspace, int64_t workspace_bytes, cudaStream_t st) {
+  CB_ARG_AS(entry, q_nope && q_pe && kv_cache && seqlens_excl && block_table);
+  CB_ARG_AS(entry, B >= 0 && H > 0 && bt_stride > 0 && num_blocks > 0);
+  // q and the new row are read with 16-byte loads, the cache through TMA and 16-byte stores
+  CB_ARG_AS(entry, ((uintptr_t)q_nope | (uintptr_t)q_pe | (uintptr_t)kv_cache | (uintptr_t)new_kv) % 16 == 0);
+  if (C != kC || R != kR)
+    return fail(-1, "%s: only kv_lora_rank=512, qk_rope_head_dim=64 is built (got %d,%d)", tag, C, R);
+  // the kernel stages one 64-token page per tile; the reference builds 64-token pages for absorbed MLA
+  // (backend.py:234-237) and its append indexes pages with a literal 64
+  if (page_size != kTile) return fail(-1, "%s: page_size must be 64 (got %d)", tag, page_size);
+  if (B == 0) return 0;
+  CB_ARG_AS(entry, workspace == nullptr || workspace_bytes >= kPlanBytes);
+  CB_ARG_AS(entry, out || (workspace && workspace_bytes >= split_kv_bytes((int64_t)B * H, kC, 1)));
+  if (!tma_available()) return fail(-3, "%s: TMA is not available", tag);
+  const int max_len = max_seqlen_hint > 0 ? max_seqlen_hint : bt_stride * page_size;
+  const int splits = mla_num_splits(B, H, max_len, workspace ? workspace_bytes : 0);
+  // a split plan written by chitu_b200_attn_plan for this step overrides the hint-derived keys per split: ragged
+  // batches get splits of equal size instead of equal count
+  const auto [o_part, lse, plan] = split_kv_carve(workspace, workspace_bytes, (int64_t)B * H, kC, splits);
+  CUtensorMap map;
+  dim3 grid(splits, cdiv(H, 16), B);
+  const auto qn = (const __nv_bfloat16*)q_nope, qp = (const __nv_bfloat16*)q_pe, nk = (const __nv_bfloat16*)new_kv;
+  int rc;
+  if (e4m3) {
+    // the cache as a 2-D [num_rows, 576] byte tensor, box = [64 rows x 64 B]: one chunk of 64 elements
+    rc = make_tma_map_2d(&map, kv_cache, (int64_t)num_blocks * kTile, kRow, 1, CU_TENSOR_MAP_DATA_TYPE_UINT8, kTile, 0,
+                         64);
+    if (rc) return rc;
+    using S = DecodeShape<__nv_fp8_e4m3>;
+    rc = launch_smem<mla_decode_e4m3_kernel>(entry, grid, dim3(S::kThreads), 1024 + decode_smem_bytes<__nv_fp8_e4m3>(),
+                                             st, map, qn, qp, (__nv_fp8_e4m3*)kv_cache, nk, seqlens_excl, block_table,
+                                             bt_stride, H, softmax_scale, splits, o_part, lse, (__nv_bfloat16*)out, plan);
+  } else {
+    // the cache as a 2-D [num_rows, 576] bf16 tensor, box = [64 rows x 64 elements (128 B)]
+    rc = make_tma_map_2d(&map, kv_cache, (int64_t)num_blocks * kTile, kRow, 2, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, kTile);
+    if (rc) return rc;
+    using S = DecodeShape<__nv_bfloat16>;
+    rc = launch_smem<mla_decode_tc_kernel>(entry, grid, dim3(S::kThreads), 1024 + decode_smem_bytes<__nv_bfloat16>(),
+                                           st, map, qn, qp, (__nv_bfloat16*)kv_cache, nk, seqlens_excl, block_table,
+                                           bt_stride, H, softmax_scale, splits, o_part, lse, (__nv_bfloat16*)out, plan);
+  }
+  if (rc) return rc;
+  CB_LAUNCHED_AS(entry, 1);
+  if (splits > 1 && out) {
+    rc = launch_merge_splits(o_part, lse, out, B * H, splits, kC, CB_BF16, st);
+    if (rc) return rc;
+    CB_LAUNCHED_AS(entry, 1);
+  }
+  return 0;
+}
 }  // namespace cb
 
 extern "C" int chitu_b200_mla_num_splits(int B, int H, int max_seqlen_hint, int64_t workspace_bytes) {
@@ -381,44 +569,9 @@ extern "C" int chitu_b200_mla_decode(const void* q_nope, const void* q_pe, void*
                                      const int32_t* block_table, int bt_stride, int B, int H, int C, int R,
                                      int page_size, int num_blocks, int max_seqlen_hint, float softmax_scale, void* out,
                                      void* workspace, int64_t workspace_bytes, void* stream) {
-  using namespace cb;
-  CB_ARG(q_nope && q_pe && kv_cache && seqlens_excl && block_table);
-  CB_ARG(B >= 0 && H > 0 && bt_stride > 0 && num_blocks > 0);
-  // q and the new row are read with 16-byte loads, the cache through TMA and 16-byte stores
-  CB_ARG(((uintptr_t)q_nope | (uintptr_t)q_pe | (uintptr_t)kv_cache | (uintptr_t)new_kv) % 16 == 0);
-  if (C != kC || R != kR)
-    return fail(-1, "mla_decode: only kv_lora_rank=512, qk_rope_head_dim=64 is built (got %d,%d)", C, R);
-  // the kernel stages one 64-token page per tile; the reference builds 64-token pages for absorbed MLA
-  // (backend.py:234-237) and its append indexes pages with a literal 64
-  if (page_size != kTile) return fail(-1, "mla_decode: page_size must be 64 (got %d)", page_size);
-  if (B == 0) return 0;
-  CB_ARG(workspace == nullptr || workspace_bytes >= kPlanBytes);
-  CB_ARG(out || (workspace && workspace_bytes >= split_kv_bytes((int64_t)B * H, kC, 1)));
-  if (!tma_available()) return fail(-3, "mla_decode: TMA is not available");
-  const int max_len = max_seqlen_hint > 0 ? max_seqlen_hint : bt_stride * page_size;
-  cudaStream_t st = (cudaStream_t)stream;
-  const int splits = mla_num_splits(B, H, max_len, workspace ? workspace_bytes : 0);
-  // a split plan written by chitu_b200_attn_plan for this step overrides the hint-derived keys per split: ragged
-  // batches get splits of equal size instead of equal count
-  const auto [o_part, lse, plan] = split_kv_carve(workspace, workspace_bytes, (int64_t)B * H, kC, splits);
-  CUtensorMap map;
-  // the cache as a 2-D [num_rows, 576] bf16 tensor, box = [64 rows x 64 elements (128 B)]
-  int rc = make_tma_map_2d(&map, kv_cache, (int64_t)num_blocks * kTile, kRow, 2, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, kTile);
-  if (rc) return rc;
-  dim3 grid(splits, cdiv(H, 16), B);
-  rc = launch_smem<mla_decode_tc_kernel>(__func__, grid, dim3(kThreads), 1024 + kSmemBytes, st, map,
-                                         (const __nv_bfloat16*)q_nope, (const __nv_bfloat16*)q_pe,
-                                         (__nv_bfloat16*)kv_cache, (const __nv_bfloat16*)new_kv, seqlens_excl,
-                                         block_table, bt_stride, H, softmax_scale, splits, o_part, lse,
-                                         (__nv_bfloat16*)out, plan);
-  if (rc) return rc;
-  CB_LAUNCHED(1);
-  if (splits > 1 && out) {
-    rc = launch_merge_splits(o_part, lse, out, B * H, splits, kC, CB_BF16, st);
-    if (rc) return rc;
-    CB_LAUNCHED(1);
-  }
-  return 0;
+  return cb::mla_decode(__func__, "mla_decode", false, q_nope, q_pe, kv_cache, new_kv, seqlens_excl, block_table,
+                        bt_stride, B, H, C, R, page_size, num_blocks, max_seqlen_hint, softmax_scale, out, workspace,
+                        workspace_bytes, (cudaStream_t)stream);
 }
 
 CB_DEFINE_TL_SETTER(mla_tc)

@@ -93,9 +93,9 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
 
 // 2-D row-major [rows, cols] tensor of `elem_bytes` elements, box = [box_rows, 128 bytes], 128B swizzle,
 // zero fill outside the tensor (host side; the driver entry point is resolved at run time).  row_stride: elements
-// between rows (0 = dense, cols); a multiple of 16 bytes.
+// between rows (0 = dense, cols); a multiple of 16 bytes.  box_bytes = 64: box = [box_rows, 64 bytes], no swizzle.
 int make_tma_map_2d(CUtensorMap* map, const void* base, int64_t rows, int64_t cols, int elem_bytes,
-                    CUtensorMapDataType dt, int box_rows, int64_t row_stride = 0);
+                    CUtensorMapDataType dt, int box_rows, int64_t row_stride = 0, int box_bytes = 128);
 // 3-D or 4-D tensor (rank), dims innermost first, byte strides of dims 1 .. rank - 1; box = [128 bytes, 1, box_outer]
 // (and 1 along dim 3), 128B swizzle, zero fill outside the tensor.
 int make_tma_map_nd(CUtensorMap* map, const void* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides,

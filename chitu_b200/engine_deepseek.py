@@ -98,8 +98,13 @@ def yarn_freqs(cfg: DeepSeekConfig, max_pos: int) -> torch.Tensor:
 class DeepSeekDecodeEngine(DecodeEngine):
     def __init__(self, cfg: DeepSeekConfig, max_reqs: int, max_seq_len: int, device="cuda:0", seed: int = 0,
                  tp_rank: int = 0, tp_size: int = 8, process_group=None, page_size: int = 64,
-                 use_fused_allreduce: bool = True):
+                 use_fused_allreduce: bool = True, kv_dtype: torch.dtype = BF):
+        """kv_dtype=torch.float8_e4m3fn keeps the latent cache in e4m3 (half the cache bytes, twice the tokens per
+        pool; new rows rounded to nearest even after a clamp to +-448, no scale) and attends through
+        chitu_b200_mla_attn_fp8kv."""
         c = cfg
+        if kv_dtype not in (BF, F8):
+            raise ValueError(f"kv_dtype must be torch.bfloat16 or torch.float8_e4m3fn, not {kv_dtype}")
         T = tp_size
         assert c.n_heads % T == 0
         # the MLA kernels stage 64-token pages of a 512 + 64 wide latent; absorb-o quantises one 128-wide head per
@@ -159,7 +164,7 @@ class DeepSeekDecodeEngine(DecodeEngine):
         self.head = rnd(g, c.vocab_size // T, dim).to(BF)
         # paged MLA cache: [L, num_blocks, 64, 576], replicated on every rank (cache_manager.py:71-76)
         nblk = self.max_blocks * max_reqs
-        self.kv_cache = torch.zeros(c.n_layers, nblk, page_size, self.C + self.R, dtype=BF, device=dev)
+        self.kv_cache = torch.zeros(c.n_layers, nblk, page_size, self.C + self.R, dtype=kv_dtype, device=dev)
         self.caches = (self.kv_cache,)
         self._rope_tables(yarn_freqs(c, max_seq_len * 2))
         B = max_reqs
@@ -258,6 +263,13 @@ class DeepSeekDecodeEngine(DecodeEngine):
 
     def _mla_decode(self, li, out):
         """paged absorbed-MLA decode, appending new_kv; out = None leaves the split-KV partials in the workspace"""
+        if self.kv_cache.dtype == F8:
+            check(self.lib.chitu_b200_mla_attn_fp8kv(
+                ptr(self.q_abs), ptr(self.q_pe), ptr(self.kv_cache[li]), ptr(self.new_kv), ptr(self.seq_lens),
+                ptr(self.block_table), self.max_blocks, self.B, 1, self.H, self.C, self.R, self.page,
+                self.kv_cache.shape[1], self.max_seq_len, 1, float(self.cfg.softmax_scale), ptr(out), ptr(self.attn_ws),
+                self.attn_ws.numel(), current_stream()), "mla_attn_fp8kv")
+            return
         check(self.lib.chitu_b200_mla_decode(ptr(self.q_abs), ptr(self.q_pe), ptr(self.kv_cache[li]), ptr(self.new_kv),
                                              ptr(self.seq_lens), ptr(self.block_table), self.max_blocks, self.B, self.H,
                                              self.C, self.R, self.page, self.kv_cache.shape[1], self.max_seq_len,
@@ -394,7 +406,7 @@ class DeepSeekDecodeEngine(DecodeEngine):
         if distinct_experts_per_layer is None:
             distinct_experts_per_layer = c.n_routed_experts * (1 - (1 - c.n_activated_experts / c.n_routed_experts) ** self.B)
         moe = c.n_routed_experts * c.dim * 2 + (c.n_shared_experts + distinct_experts_per_layer) * expert
-        kv = self.B * (seq_len + 1) * (self.C + self.R) * 2
+        kv = self.B * (seq_len + 1) * (self.C + self.R) * self.kv_cache.element_size()
         n_moe = max(c.n_layers - c.n_dense_layers, 0)
         n_dense = min(c.n_layers, c.n_dense_layers)
         head = self.head.numel() * 2

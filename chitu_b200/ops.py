@@ -41,7 +41,10 @@ def _linear_ws(M: int, N: int, device):
 
 def append_to_paged_kv_cache(kv_cache, page_table, this_kv, old_seq_lens):
     """chitu/ops.py:50-91.  kv_cache[page_table[i][len_i // 64]][len_i % 64] = this_kv[i]
-    (the literal 64 is the reference's, triton_kernels.py:38,42)."""
+    (the literal 64 is the reference's, triton_kernels.py:38,42).
+    A float8_e4m3fn cache of 64-token pages takes bf16 / fp16 rows and stores each element as
+    x.float().clamp(-448, 448).to(float8_e4m3fn) (plain .to() would turn values beyond +-448 into NaN), the rule of
+    the e4m3 attention paths' own appends."""
     assert kv_cache.is_contiguous()
     assert page_table.is_contiguous()
     assert this_kv.is_contiguous()
@@ -54,6 +57,12 @@ def append_to_paged_kv_cache(kv_cache, page_table, this_kv, old_seq_lens):
     tot = this_kv.numel() // batch_size
     assert kv_cache.numel() // (kv_cache.shape[0] * kv_cache.shape[1]) == tot
     assert page_table.dtype == torch.int32 and old_seq_lens.dtype == torch.int32
+    if kv_cache.dtype == torch.float8_e4m3fn and this_kv.dtype != kv_cache.dtype:
+        assert this_kv.dtype in (torch.bfloat16, torch.float16) and page_size == 64
+        check(_lib.load().chitu_b200_append_paged_kv_e4m3(
+            ptr(kv_cache), ptr(page_table), ptr(this_kv), ptr(old_seq_lens), batch_size, num_pages_per_sample, tot,
+            dtype_code(this_kv.dtype), current_stream()), "append_paged_kv_e4m3")
+        return
     assert this_kv.dtype == kv_cache.dtype
     check(
         _lib.load().chitu_b200_append_paged_kv(

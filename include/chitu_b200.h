@@ -54,6 +54,12 @@ int64_t chitu_b200_launch_count(void);
 int chitu_b200_append_paged_kv(void* kv_cache, const int32_t* page_table, const void* this_kv,
                                const int32_t* old_seq_lens, int batch, int pages_per_sample,
                                int page_size, int index_div, int64_t row_bytes, void* stream);
+/* The same append into an fp8 (e4m3fn) paged cache of 64-token pages: this_kv [batch, n] in the io dtype (bf16 | fp16),
+ * each element stored as e4m3(clamp(x, -448, 448)), nearest even, NaN kept (the store rule of
+ * chitu_b200_gqa_paged_attn_fp8kv and chitu_b200_mla_attn_fp8kv).  n % 8 == 0, this_kv 16-byte aligned. */
+int chitu_b200_append_paged_kv_e4m3(void* kv_cache, const int32_t* page_table, const void* this_kv,
+                                    const int32_t* old_seq_lens, int batch, int pages_per_sample, int n, int dtype,
+                                    void* stream);
 
 /* ---- MoE routing / permutation -------------------------------------------------------- */
 /* Replaces csrc/moe_align_kernel.cu:27-122 (pybind csrc/binding.cpp:11,
@@ -311,6 +317,28 @@ int chitu_b200_mla_paged_prefill(const void* q_nope, const void* q_pe, void* kv_
                                  int H, int C, int R, int page_size, int num_blocks, int max_seqlen_hint, int causal,
                                  float softmax_scale, void* out, void* workspace, int64_t workspace_bytes,
                                  void* stream);
+
+/* *.mla_attn_with_kvcache over an fp8 (e4m3fn) paged latent cache, seqlen_q = sq >= 1: the arguments and semantics
+ * of chitu_b200_mla_paged_prefill with kv_cache [num_blocks, 64, C + R] of e4m3 bytes (q_nope, q_pe, new_kv and out
+ * stay bf16), with these differences:
+ *  - Store: every element x of a new row (latent and rope) is written as e4m3(clamp(x, -448, 448)), rounded to
+ *    nearest even; NaN stays NaN (torch: x.float().clamp(-448, 448).to(float8_e4m3fn)).  No scale (a per-tensor scale
+ *    of 1).
+ *  - Read: a cache element is decoded to bf16 exactly; the arithmetic is then the bf16 cache's (scale * (q_nope.k_c +
+ *    q_pe.k_pe) in fp32, softmax in fp32, P rounded to bf16 before P.V with V = the first C columns of the same rows,
+ *    bottom-right causal mask, 0 for a row that sees no key).  The rows appended by the call are attended in their
+ *    stored form, so sq = n agrees with n successive decodes.
+ *  - sq == 1 is the decode of chitu_b200_mla_decode: q_nope [B, 1, H, C] = [B, H, C], new_kv [B, C + R] appended in
+ *    the same launch, the device split plan of chitu_b200_attn_plan honoured, `causal` ignored (the one query row sees
+ *    every key), and out == NULL defers the merge to chitu_b200_mla_absorb_o_merge_quant (the workspace must then hold
+ *    the partials of one split).  sq > 1 appends the new rows first, then runs the multi-token kernel; out != NULL.
+ * Splits and workspace as in the bf16 entries -> no host synchronisation, capturable in a CUDA graph, deterministic.
+ * Built for C = 512, R = 64, page_size = 64; bases 16-byte aligned.  Anything else returns a negative status before any
+ * launch.  B == 0 launches nothing. */
+int chitu_b200_mla_attn_fp8kv(const void* q_nope, const void* q_pe, void* kv_cache, const void* new_kv,
+                              const int32_t* seqlens_excl, const int32_t* block_table, int bt_stride, int B, int sq,
+                              int H, int C, int R, int page_size, int num_blocks, int max_seqlen_hint, int causal,
+                              float softmax_scale, void* out, void* workspace, int64_t workspace_bytes, void* stream);
 
 /* invoke_fused_moe_kernel (fused_moe.py:796-891; Triton kernel :62-307) as ONE grouped wgmma GEMM:
  * A bf16 [numel/top_k (GEMM1) or numel (top_k = 1), K]; B stacked expert weights [E, N, K] (bf16 for wmode 0, fp8 +
