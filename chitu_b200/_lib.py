@@ -34,6 +34,7 @@ SIGNATURES = {
     "chitu_b200_launch_count": (L, []),
     "chitu_b200_append_paged_kv": (I, [P, P, P, P, I, I, I, I, L, P]),
     "chitu_b200_append_paged_kv_e4m3": (I, [P, P, P, P, I, I, I, I, P]),
+    "chitu_b200_scatter_kv": (I, [P, P, P, L, P, L, P, P, P, I, I, L, I, I, I, I, I, I, P]),
     "chitu_b200_moe_align_block_size": (I, [P, I, L, I, I, P, P, P, P, P]),
     "chitu_b200_moe_gate_workspace_bytes": (L, [I, I]),
     "chitu_b200_moe_gate": (I, [P, P, P, I, I, I, I, I, I, I, I, F, P, P, I, P, L, P]),

@@ -159,10 +159,12 @@ struct PushDev {
 };
 int comm_push_desc(void* handle, void* out_desc);
 
-// ---- paged append (core.cu): new rows into one or two paged caches, for the append and paged prefill entries ------
-// Row i of request b (i < sq, b < B) comes from src + b * src_sb + i * src_st (bytes) and goes to position
-// p = seqlens[b] + i: cache row block_table[b, p / index_div] * page_size + p % index_div.  index_div is page_size for
-// true page indexing and 64 for the reference's append (triton_kernels.py:38,42).  c1.cache == NULL: one cache only.
+// ---- paged append (core.cu): new rows into one or two paged caches, for the append, scatter and paged prefill entries
+// Fixed length (cu_seqlens == NULL, rows = sq): row i of request b (i < sq, b < B) comes from src + b * src_sb +
+// i * src_st (bytes).  Ragged (rows = total_rows): row i of request b (i < cu_seqlens[b + 1] - cu_seqlens[b]) comes
+// from src + (cu_seqlens[b] + i) * src_st; src_sb is unused.  Either goes to position p = seqlens[b] + i (seqlens ==
+// NULL: p = i): cache row block_table[b, p / index_div] * page_size + p % index_div.  index_div is page_size for true
+// page indexing and 64 for the reference's append (triton_kernels.py:38,42).  c1.cache == NULL: one cache only.
 // One PDL launch; the caller counts it.
 struct PagedAppend {
   void* cache;
@@ -170,17 +172,19 @@ struct PagedAppend {
   int64_t src_sb, src_st;
 };
 void launch_paged_append(PagedAppend c0, PagedAppend c1, int64_t row_bytes, const int32_t* seqlens,
-                         const int32_t* block_table, int bt_stride, int B, int sq, int page_size, int index_div,
-                         cudaStream_t st);
+                         const int32_t* cu_seqlens, const int32_t* block_table, int bt_stride, int B, int rows,
+                         int page_size, int index_div, cudaStream_t st);
 // The same copy into contiguous caches: position p of request b is cache row b * rows_sb + p, and rows with
 // p >= cache_rows are skipped.
 void launch_contiguous_append(PagedAppend c0, PagedAppend c1, int64_t row_bytes, const int32_t* seqlens,
-                              int64_t rows_sb, int cache_rows, int B, int sq, cudaStream_t st);
+                              const int32_t* cu_seqlens, int64_t rows_sb, int cache_rows, int B, int rows,
+                              cudaStream_t st);
 // The paged append (true page indexing) into one or two e4m3 caches (c1.cache == NULL: one): rows of n io elements
 // (dtype CB_BF16 | CB_F16, n % 8 == 0, 16-byte aligned sources and strides) stored as e4m3 with io2_to_e4m3x2's
 // rounding.
 void launch_paged_append_e4m3(PagedAppend c0, PagedAppend c1, int n, int dtype, const int32_t* seqlens,
-                              const int32_t* block_table, int bt_stride, int B, int sq, int page_size, cudaStream_t st);
+                              const int32_t* cu_seqlens, const int32_t* block_table, int bt_stride, int B, int rows,
+                              int page_size, cudaStream_t st);
 
 // ---- absorbed MLA over the paged latent cache (mla_tc.cu, mla_prefill.cu) ---------------------------------------------
 // The arguments of chitu_b200_mla_decode / chitu_b200_mla_paged_prefill over a bf16 cache, or (e4m3) over a cache of

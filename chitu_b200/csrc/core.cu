@@ -76,6 +76,27 @@ extern "C" const char* chitu_b200_debug_timeline_names(void) { return cb::g_tl_n
 // caches: row b * rows_sb + p, p < cache_rows).  One CTA per row; 16-byte copies when every
 // address and stride allows them, byte copies otherwise.
 // ============================================================================================
+// The rows of one append launch, as f(b, i, sb, si): row i of request b, read from src + sb * src_sb + si * src_st.
+// Fixed length (cu_seqlens == NULL), grid (sq, min(B, 65535)): row blockIdx.x of requests blockIdx.y, blockIdx.y +
+// gridDim.y, ...; sb = b, si = i.  Ragged, grid (total_rows): source row r = blockIdx.x belongs to the request b with
+// cu_seqlens[b] <= r < cu_seqlens[b + 1] (binary search; rows outside [cu[0], cu[B]) belong to none); sb = 0, si = r.
+template <typename F>
+__device__ __forceinline__ void for_each_append_row(const int32_t* __restrict__ cu_seqlens, int B, F&& f) {
+  const int r = blockIdx.x;
+  if (cu_seqlens == nullptr) {
+    for (int b = blockIdx.y; b < B; b += gridDim.y) f(b, r, b, r);     // more than 65535 requests: a CTA takes several
+    return;
+  }
+  if (r < cu_seqlens[0] || r >= cu_seqlens[B]) return;
+  int lo = 0, hi = B;                                 // cu_seqlens[lo] <= r < cu_seqlens[hi]
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (cu_seqlens[mid] <= r) lo = mid;
+    else hi = mid;
+  }
+  f(lo, r - cu_seqlens[lo], 0, r);
+}
+
 // Row i of request b (n units of V) into both caches; bt is the request's block-table row.  A thread issues its source
 // loads for two passes over both caches before the page lookup and the stores, so the copy's memory round trip
 // overlaps the lookup's.  The compiler would not order them so itself: it cannot tell that sources and caches never
@@ -83,10 +104,10 @@ extern "C" const char* chitu_b200_debug_timeline_names(void) { return cb::g_tl_n
 // CONTIG: the destination is row b * rows_sb + p of contiguous caches; bt, page_size and index_div are unused.
 template <typename V, bool CONTIG>
 __device__ __forceinline__ void copy_row(const cb::PagedAppend& c0, const cb::PagedAppend& c1, int p,
-                                         const int32_t* bt, int page_size, int index_div, int64_t rows_sb, int b, int i,
-                                         int64_t n) {
-  const V* s0 = reinterpret_cast<const V*>((const uint8_t*)c0.src + b * c0.src_sb + i * c0.src_st);
-  const V* s1 = reinterpret_cast<const V*>((const uint8_t*)c1.src + b * c1.src_sb + i * c1.src_st);
+                                         const int32_t* bt, int page_size, int index_div, int64_t rows_sb, int b,
+                                         int sb, int si, int64_t n) {
+  const V* s0 = reinterpret_cast<const V*>((const uint8_t*)c0.src + sb * c0.src_sb + si * c0.src_st);
+  const V* s1 = reinterpret_cast<const V*>((const uint8_t*)c1.src + sb * c1.src_sb + si * c1.src_st);
   const bool two = c1.cache != nullptr;
 #pragma unroll 1
   for (int64_t u = threadIdx.x; u < n; u += 2 * blockDim.x) {
@@ -105,68 +126,77 @@ __device__ __forceinline__ void copy_row(const cb::PagedAppend& c0, const cb::Pa
   }
 }
 
+// seqlens == NULL: every request starts at position 0
 template <bool CONTIG>
 __device__ __forceinline__ void append_rows(const cb::PagedAppend& c0, const cb::PagedAppend& c1, int64_t row_bytes,
-                                            const int32_t* __restrict__ seqlens, const int32_t* block_table,
-                                            int bt_stride, int B, int page_size, int index_div, int64_t rows_sb,
-                                            int cache_rows, int vec) {
+                                            const int32_t* __restrict__ seqlens, const int32_t* cu_seqlens,
+                                            const int32_t* block_table, int bt_stride, int B, int page_size,
+                                            int index_div, int64_t rows_sb, int cache_rows, int vec) {
   cb::pdl_prologue();
-  const int i = blockIdx.x;
-  for (int b = blockIdx.y; b < B; b += gridDim.y) {     // more than 65535 requests: a CTA takes several
-    const int p = seqlens[b] + i;
-    if (CONTIG && p >= cache_rows) continue;           // past the contiguous cache's capacity: not written
+  for_each_append_row(cu_seqlens, B, [&](int b, int i, int sb, int si) {
+    const int p = (seqlens ? seqlens[b] : 0) + i;
+    if (CONTIG && p >= cache_rows) return;             // past the contiguous cache's capacity: not written
     const int32_t* bt = block_table + (int64_t)b * bt_stride;
-    if (vec) copy_row<uint4, CONTIG>(c0, c1, p, bt, page_size, index_div, rows_sb, b, i, row_bytes >> 4);
-    else copy_row<uint8_t, CONTIG>(c0, c1, p, bt, page_size, index_div, rows_sb, b, i, row_bytes);
-  }
+    if (vec) copy_row<uint4, CONTIG>(c0, c1, p, bt, page_size, index_div, rows_sb, b, sb, si, row_bytes >> 4);
+    else copy_row<uint8_t, CONTIG>(c0, c1, p, bt, page_size, index_div, rows_sb, b, sb, si, row_bytes);
+  });
 }
 
 __global__ void __launch_bounds__(128) paged_append_kernel(cb::PagedAppend c0, cb::PagedAppend c1, int64_t row_bytes,
                                                            const int32_t* __restrict__ seqlens,
-                                                           const int32_t* block_table, int bt_stride, int B,
-                                                           int page_size, int index_div, int vec) {
-  append_rows<false>(c0, c1, row_bytes, seqlens, block_table, bt_stride, B, page_size, index_div, 0, 0, vec);
+                                                           const int32_t* cu_seqlens, const int32_t* block_table,
+                                                           int bt_stride, int B, int page_size, int index_div,
+                                                           int vec) {
+  append_rows<false>(c0, c1, row_bytes, seqlens, cu_seqlens, block_table, bt_stride, B, page_size, index_div, 0, 0,
+                     vec);
 }
 
 __global__ void __launch_bounds__(128) contiguous_append_kernel(cb::PagedAppend c0, cb::PagedAppend c1,
                                                                 int64_t row_bytes, const int32_t* __restrict__ seqlens,
-                                                                int64_t rows_sb, int cache_rows, int B, int vec) {
-  append_rows<true>(c0, c1, row_bytes, seqlens, nullptr, 0, B, 1, 1, rows_sb, cache_rows, vec);
+                                                                const int32_t* cu_seqlens, int64_t rows_sb,
+                                                                int cache_rows, int B, int vec) {
+  append_rows<true>(c0, c1, row_bytes, seqlens, cu_seqlens, nullptr, 0, B, 1, 1, rows_sb, cache_rows, vec);
 }
 
 // Rows of n io elements into one or two e4m3 caches, 8 elements (16 bytes in, 8 out) per thread and step.
 template <typename T>
 __global__ void __launch_bounds__(128) paged_append_e4m3_kernel(cb::PagedAppend c0, cb::PagedAppend c1, int n,
                                                                 const int32_t* __restrict__ seqlens,
+                                                                const int32_t* __restrict__ cu_seqlens,
                                                                 const int32_t* __restrict__ block_table, int bt_stride,
                                                                 int B, int page_size) {
   cb::pdl_prologue();
-  const int i = blockIdx.x;
-  for (int b = blockIdx.y; b < B; b += gridDim.y) {
-    const int p = seqlens[b] + i;
+  for_each_append_row(cu_seqlens, B, [&](int b, int i, int sb, int si) {
+    const int p = (seqlens ? seqlens[b] : 0) + i;
     const int64_t row = (int64_t)block_table[(int64_t)b * bt_stride + p / page_size] * page_size + p % page_size;
     for (int u = threadIdx.x; u < (c1.cache ? 2 : 1) * (n / 8); u += blockDim.x) {
       const cb::PagedAppend& c = u < n / 8 ? c0 : c1;
       const int e = (u < n / 8 ? u : u - n / 8) * 8;
-      const uint4 x = *reinterpret_cast<const uint4*>((const uint8_t*)c.src + b * c.src_sb + i * c.src_st + e * 2);
+      const uint4 x = *reinterpret_cast<const uint4*>((const uint8_t*)c.src + sb * c.src_sb + si * c.src_st + e * 2);
       const uint2 y = make_uint2(cb::io2_to_e4m3x2<T>(x.x) | cb::io2_to_e4m3x2<T>(x.y) << 16,
                                  cb::io2_to_e4m3x2<T>(x.z) | cb::io2_to_e4m3x2<T>(x.w) << 16);
       *reinterpret_cast<uint2*>((uint8_t*)c.cache + row * n + e) = y;
     }
-  }
+  });
 }
 
 namespace cb {
+// for_each_append_row's grids: `rows` is sq (fixed length) or total_rows (with cu_seqlens)
+static dim3 append_grid(const int32_t* cu_seqlens, int B, int rows) {
+  return cu_seqlens ? dim3(rows) : dim3(rows, B < 65535 ? B : 65535);
+}
+
 void launch_paged_append_e4m3(PagedAppend c0, PagedAppend c1, int n, int dtype, const int32_t* seqlens,
-                              const int32_t* block_table, int bt_stride, int B, int sq, int page_size, cudaStream_t st) {
-  const dim3 grid(sq, B < 65535 ? B : 65535);
+                              const int32_t* cu_seqlens, const int32_t* block_table, int bt_stride, int B, int rows,
+                              int page_size, cudaStream_t st) {
+  const dim3 grid = append_grid(cu_seqlens, B, rows);
   const int threads = n / 4 < 128 ? 64 : 128;
   if (dtype == CB_BF16)
-    launch_k(paged_append_e4m3_kernel<__nv_bfloat16>, grid, dim3(threads), 0, st, c0, c1, n, seqlens, block_table,
-             bt_stride, B, page_size);
+    launch_k(paged_append_e4m3_kernel<__nv_bfloat16>, grid, dim3(threads), 0, st, c0, c1, n, seqlens, cu_seqlens,
+             block_table, bt_stride, B, page_size);
   else
-    launch_k(paged_append_e4m3_kernel<__half>, grid, dim3(threads), 0, st, c0, c1, n, seqlens, block_table, bt_stride,
-             B, page_size);
+    launch_k(paged_append_e4m3_kernel<__half>, grid, dim3(threads), 0, st, c0, c1, n, seqlens, cu_seqlens,
+             block_table, bt_stride, B, page_size);
 }
 
 // 16-byte copies when every address and stride allows them; 64 threads for rows of fewer than 128 copy units
@@ -179,18 +209,19 @@ static int append_vec(const PagedAppend& c0, const PagedAppend& c1, int64_t row_
 static int append_threads(int64_t row_bytes, int vec) { return row_bytes / (vec ? 16 : 1) < 128 ? 64 : 128; }
 
 void launch_paged_append(PagedAppend c0, PagedAppend c1, int64_t row_bytes, const int32_t* seqlens,
-                         const int32_t* block_table, int bt_stride, int B, int sq, int page_size, int index_div,
-                         cudaStream_t st) {
+                         const int32_t* cu_seqlens, const int32_t* block_table, int bt_stride, int B, int rows,
+                         int page_size, int index_div, cudaStream_t st) {
   const int vec = append_vec(c0, c1, row_bytes);
-  launch_k(paged_append_kernel, dim3(sq, B < 65535 ? B : 65535), dim3(append_threads(row_bytes, vec)), 0, st, c0, c1,
-           row_bytes, seqlens, block_table, bt_stride, B, page_size, index_div, vec);
+  launch_k(paged_append_kernel, append_grid(cu_seqlens, B, rows), dim3(append_threads(row_bytes, vec)), 0, st, c0, c1,
+           row_bytes, seqlens, cu_seqlens, block_table, bt_stride, B, page_size, index_div, vec);
 }
 
 void launch_contiguous_append(PagedAppend c0, PagedAppend c1, int64_t row_bytes, const int32_t* seqlens,
-                              int64_t rows_sb, int cache_rows, int B, int sq, cudaStream_t st) {
+                              const int32_t* cu_seqlens, int64_t rows_sb, int cache_rows, int B, int rows,
+                              cudaStream_t st) {
   const int vec = append_vec(c0, c1, row_bytes);
-  launch_k(contiguous_append_kernel, dim3(sq, B < 65535 ? B : 65535), dim3(append_threads(row_bytes, vec)), 0, st, c0,
-           c1, row_bytes, seqlens, rows_sb, cache_rows, B, vec);
+  launch_k(contiguous_append_kernel, append_grid(cu_seqlens, B, rows), dim3(append_threads(row_bytes, vec)), 0, st, c0,
+           c1, row_bytes, seqlens, cu_seqlens, rows_sb, cache_rows, B, vec);
 }
 }  // namespace cb
 
@@ -204,7 +235,7 @@ extern "C" int chitu_b200_append_paged_kv(void* kv_cache, const int32_t* page_ta
   CB_ARG(kv_cache && page_table && this_kv && old_seq_lens);
   CB_ARG(batch >= 0 && pages_per_sample > 0 && page_size > 0 && index_div > 0 && row_bytes > 0);
   if (batch == 0) return 0;
-  cb::launch_paged_append({kv_cache, this_kv, row_bytes, row_bytes}, {}, row_bytes, old_seq_lens, page_table,
+  cb::launch_paged_append({kv_cache, this_kv, row_bytes, row_bytes}, {}, row_bytes, old_seq_lens, nullptr, page_table,
                           pages_per_sample, batch, 1, page_size, index_div, (cudaStream_t)stream);
   CB_LAUNCHED(1);
   return 0;
@@ -218,8 +249,41 @@ extern "C" int chitu_b200_append_paged_kv_e4m3(void* kv_cache, const int32_t* pa
   CB_ARG((uintptr_t)this_kv % 16 == 0);
   if (batch == 0) return 0;
   const int64_t row_bytes = (int64_t)n * 2;
-  cb::launch_paged_append_e4m3({kv_cache, this_kv, row_bytes, row_bytes}, {}, n, dtype, old_seq_lens, page_table,
-                               pages_per_sample, batch, 1, 64, (cudaStream_t)stream);
+  cb::launch_paged_append_e4m3({kv_cache, this_kv, row_bytes, row_bytes}, {}, n, dtype, old_seq_lens, nullptr,
+                               page_table, pages_per_sample, batch, 1, 64, (cudaStream_t)stream);
+  CB_LAUNCHED(1);
+  return 0;
+}
+
+// The prompt's k / v (or latent) rows into the cache after the prefill attention (include/chitu_b200.h): the appends
+// above with ragged lengths, one CTA per source row.
+extern "C" int chitu_b200_scatter_kv(void* cache0, void* cache1, const void* src0, int64_t src0_st, const void* src1,
+                                     int64_t src1_st, const int32_t* cu_seqlens, const int32_t* cache_seqlens,
+                                     const int32_t* block_table, int bt_stride, int page_size, int64_t cache_sb,
+                                     int cache_rows, int B, int total_rows, int n, int src_dtype, int cache_dtype,
+                                     void* stream) {
+  CB_ARG(cache0 && src0 && cu_seqlens && (cache1 == nullptr) == (src1 == nullptr));
+  CB_ARG(B >= 0 && total_rows >= 0 && n > 0);
+  CB_ARG(src_dtype == CB_BF16 || src_dtype == CB_F16);
+  const bool e4m3 = cache_dtype == CB_FP8_E4M3;
+  CB_ARG(cache_dtype == src_dtype || (e4m3 && block_table));          // e4m3: paged caches only
+  if (block_table) CB_ARG(bt_stride > 0 && page_size > 0);
+  else CB_ARG(cache_rows >= 0 && cache_sb % n == 0 && cache_sb >= (int64_t)cache_rows * n);
+  if (e4m3)     // 16-byte loads of 8 elements, 8-byte stores
+    CB_ARG(n % 8 == 0 && ((uintptr_t)src0 | (uintptr_t)src1) % 16 == 0 && src0_st % 8 == 0 &&
+           (!src1 || src1_st % 8 == 0) && ((uintptr_t)cache0 | (uintptr_t)cache1) % 8 == 0);
+  if (B == 0 || total_rows == 0) return 0;
+  const cb::PagedAppend c0{cache0, src0, 0, src0_st * 2}, c1{cache1, src1, 0, src1_st * 2};
+  const cudaStream_t st = (cudaStream_t)stream;
+  if (e4m3)
+    cb::launch_paged_append_e4m3(c0, c1, n, src_dtype, cache_seqlens, cu_seqlens, block_table, bt_stride, B,
+                                 total_rows, page_size, st);
+  else if (block_table)
+    cb::launch_paged_append(c0, c1, (int64_t)n * 2, cache_seqlens, cu_seqlens, block_table, bt_stride, B, total_rows,
+                            page_size, page_size, st);
+  else
+    cb::launch_contiguous_append(c0, c1, (int64_t)n * 2, cache_seqlens, cu_seqlens, cache_sb / n, cache_rows, B,
+                                 total_rows, st);
   CB_LAUNCHED(1);
   return 0;
 }

@@ -415,12 +415,13 @@ int gqa_prefill(const char* entry, const char* name, KvLayout layout, const void
   if (k_new) {                                              // the sq new k / v rows first
     const PagedAppend kc{k_cache, k_new, k_new_sb * 2, k_new_st * 2}, vc{v_cache, v_new, v_new_sb * 2, v_new_st * 2};
     if (contig)
-      launch_contiguous_append(kc, vc, (int64_t)Hkv * kD * 2, cache_seqlens, rows_sb, cache_rows, B, sq, st);
+      launch_contiguous_append(kc, vc, (int64_t)Hkv * kD * 2, cache_seqlens, nullptr, rows_sb, cache_rows, B, sq, st);
     else if (e4m3)
-      launch_paged_append_e4m3(kc, vc, Hkv * kD, dtype, cache_seqlens, block_table, bt_stride, B, sq, page_size, st);
+      launch_paged_append_e4m3(kc, vc, Hkv * kD, dtype, cache_seqlens, nullptr, block_table, bt_stride, B, sq,
+                               page_size, st);
     else                                                    // true page indexing
-      launch_paged_append(kc, vc, (int64_t)Hkv * kD * 2, cache_seqlens, block_table, bt_stride, B, sq, page_size,
-                          page_size, st);
+      launch_paged_append(kc, vc, (int64_t)Hkv * kD * 2, cache_seqlens, nullptr, block_table, bt_stride, B, sq,
+                          page_size, page_size, st);
     CB_LAUNCHED_AS(name, 1);
   }
 

@@ -536,11 +536,11 @@ int mla_paged_prefill(const char* entry, const char* tag, bool e4m3, const void*
   if (new_kv) {       // the B * sq new latent rows first, pages indexed with a literal 64 as the reference's append does
     const int64_t row_bytes = kRow * 2;
     if (e4m3)
-      launch_paged_append_e4m3({kv_cache, new_kv, sq * row_bytes, row_bytes}, {}, kRow, CB_BF16, seqlens_excl,
+      launch_paged_append_e4m3({kv_cache, new_kv, sq * row_bytes, row_bytes}, {}, kRow, CB_BF16, seqlens_excl, nullptr,
                                block_table, bt_stride, B, sq, kTile, st);
     else
-      launch_paged_append({kv_cache, new_kv, sq * row_bytes, row_bytes}, {}, row_bytes, seqlens_excl, block_table,
-                          bt_stride, B, sq, kTile, 64, st);
+      launch_paged_append({kv_cache, new_kv, sq * row_bytes, row_bytes}, {}, row_bytes, seqlens_excl, nullptr,
+                          block_table, bt_stride, B, sq, kTile, 64, st);
     CB_LAUNCHED_AS(entry, 1);
   }
   const dim3 grid(row_tiles * splits * B), block(kThreads);

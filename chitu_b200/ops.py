@@ -5,6 +5,7 @@ Reference: thu-pacman/chitu, chitu/ops.py (file:line cited per function).
 """
 from __future__ import annotations
 
+import math
 from typing import Optional, Tuple
 
 import torch
@@ -14,6 +15,7 @@ from ._lib import check, current_stream, dtype_code, ptr, require_cuda
 
 __all__ = [
     "append_to_paged_kv_cache",
+    "scatter_kv_to_cache",
     "apply_rotary_pos_emb",
     "apply_rotary_pos_emb_triton",
     "act_quant_deepseek_v3",
@@ -43,8 +45,9 @@ def append_to_paged_kv_cache(kv_cache, page_table, this_kv, old_seq_lens):
     """chitu/ops.py:50-91.  kv_cache[page_table[i][len_i // 64]][len_i % 64] = this_kv[i]
     (the literal 64 is the reference's, triton_kernels.py:38,42).
     A float8_e4m3fn cache of 64-token pages takes bf16 / fp16 rows and stores each element as
-    x.float().clamp(-448, 448).to(float8_e4m3fn) (plain .to() would turn values beyond +-448 into NaN), the rule of
-    the e4m3 attention paths' own appends."""
+    x.float().clamp(-448, 448).to(float8_e4m3fn) (plain .to() would turn values beyond +-464 into NaN), the rule of
+    the e4m3 attention paths' own appends.  One row per request per call: to write a prompt's k / v or latent rows into
+    a cache of any page size (e4m3 included), call `scatter_kv_to_cache`."""
     assert kv_cache.is_contiguous()
     assert page_table.is_contiguous()
     assert this_kv.is_contiguous()
@@ -71,6 +74,76 @@ def append_to_paged_kv_cache(kv_cache, page_table, this_kv, old_seq_lens):
         ),
         "append_paged_kv",
     )
+
+
+def scatter_kv_to_cache(k_cache, v_cache, k, v, cu_seqlens, block_table=None, cache_seqlens=None):
+    """Writes the prompts' k / v rows into the KV cache after the prefill attention, every request of the batch in one
+    launch (the page scatter of PagedKVCacheManager.finalize_cache_bylayer_prefill, cache_manager.py:93-142, without
+    its per-request loop).  Row t of request b, k[cu_seqlens[b] + t] for t < cu_seqlens[b + 1] - cu_seqlens[b], goes
+    to position p = cache_seqlens[b] + t (p = t without cache_seqlens).
+
+    GQA: k / v [total, Hkv, D] with dense heads and any row stride (views of a fused qkv output); caches
+    [num_blocks, page, Hkv, D] with a block table (page block_table[b, p // page], slot p % page, any page size), or
+    [Bc, S, Hkv, D] without one (row p of cache entry b; rows with p >= S are not written).  MLA: kv_cache
+    [num_blocks, 64, 576] and kv [total, 576] as k_cache / k, with v_cache = v = None.  cu_seqlens int32 [B + 1] and
+    cache_seqlens int32 [B] on the device.  A float8_e4m3fn paged cache takes bf16 / fp16 rows and stores each element
+    as x.float().clamp(-448, 448).to(float8_e4m3fn); otherwise the caches have the rows' dtype and get their bits.
+    In place, no host synchronisation (capturable in a CUDA graph), returns None."""
+    def refuse(why):
+        raise RuntimeError(f"scatter_kv_to_cache: {why}")
+
+    tensors = [t for t in (k_cache, v_cache, k, v, cu_seqlens, block_table, cache_seqlens) if t is not None]
+    require_cuda(*tensors)
+    if any(t.device != k_cache.device for t in tensors):
+        refuse("every tensor must be on the cache's device")
+    if (v_cache is None) != (v is None):
+        refuse("v_cache and v are given together (GQA) or both None (MLA)")
+    if k.dtype not in (torch.bfloat16, torch.float16) or k_cache.dtype not in (k.dtype, torch.float8_e4m3fn):
+        refuse(f"{k.dtype} rows into a {k_cache.dtype} cache are not built")
+    if block_table is None and k_cache.dtype == torch.float8_e4m3fn:
+        refuse("the fp8 KV cache is built for the paged cache only")
+    row_shape = tuple(k_cache.shape[2:])
+    if k_cache.dim() < 3 or tuple(k.shape[1:]) != row_shape:
+        refuse(f"rows {tuple(k.shape)} do not match the cache {tuple(k_cache.shape)}")
+    if not (_dense_rows(k, 1) and _dense_rows(k_cache, 2)):
+        refuse("the elements of a row must be dense in k and in the cache")
+    if v is not None and (v_cache.shape != k_cache.shape or v_cache.dtype != k_cache.dtype or v.dtype != k.dtype
+                          or v.shape != k.shape or not _dense_rows(v, 1) or v_cache.stride() != k_cache.stride()):
+        refuse("v / v_cache must match k / k_cache in shape, dtype and layout")
+    if k.shape[0] >= 2 ** 31:
+        refuse("more than 2^31 - 1 rows")
+    if cu_seqlens.dtype != torch.int32 or cu_seqlens.dim() != 1 or cu_seqlens.numel() < 1 \
+            or not cu_seqlens.is_contiguous():
+        refuse("cu_seqlens must be a contiguous int32 [B + 1] tensor")
+    B = cu_seqlens.numel() - 1
+    if cache_seqlens is not None and (cache_seqlens.dtype != torch.int32 or tuple(cache_seqlens.shape) != (B,)
+                                      or not cache_seqlens.is_contiguous()):
+        refuse("cache_seqlens must be a contiguous int32 [B] tensor")
+    if block_table is not None:
+        if block_table.dtype != torch.int32 or block_table.dim() != 2 or block_table.stride(-1) != 1 \
+                or block_table.shape[0] < B or not k_cache.is_contiguous():
+            refuse("block_table must be int32 [>= B, pages] with unit column stride, over contiguous caches")
+        paged, cache_sb, cache_rows = (ptr(block_table), block_table.stride(0), k_cache.shape[1]), 0, 0
+    else:
+        if k_cache.shape[0] < B:
+            refuse(f"a non-paged cache holds {k_cache.shape[0]} requests, fewer than {B}")
+        if not _dense_rows(k_cache, 1):
+            refuse("a non-paged cache [Bc, S, ...] must be dense from its second dim on")
+        paged, cache_sb, cache_rows = (None, 0, 0), k_cache.stride(0), k_cache.shape[1]
+    check(_lib.load().chitu_b200_scatter_kv(
+        ptr(k_cache), ptr(v_cache), ptr(k), k.stride(0), ptr(v), 0 if v is None else v.stride(0), ptr(cu_seqlens),
+        ptr(cache_seqlens), *paged, cache_sb, cache_rows, B, k.shape[0], math.prod(row_shape), dtype_code(k.dtype),
+        dtype_code(k_cache.dtype), current_stream()), "scatter_kv")
+
+
+def _dense_rows(t, lead):
+    """The dims of `t` from `lead` on are laid out as a contiguous block (dims of size 1 may have any stride)."""
+    want = 1
+    for size, stride in reversed(list(zip(t.shape[lead:], t.stride()[lead:]))):
+        if size != 1 and stride != want:
+            return False
+        want *= size
+    return True
 
 
 def apply_rotary_pos_emb_triton(q, k, cos, sin, rotary_type="hf-llama", block_size=128):

@@ -60,6 +60,28 @@ int chitu_b200_append_paged_kv(void* kv_cache, const int32_t* page_table, const 
 int chitu_b200_append_paged_kv_e4m3(void* kv_cache, const int32_t* page_table, const void* this_kv,
                                     const int32_t* old_seq_lens, int batch, int pages_per_sample, int n, int dtype,
                                     void* stream);
+/* The prompt's k / v (GQA: cache0 = k, cache1 = v) or latent rows (MLA: cache1 = src1 = NULL) into the KV cache after
+ * the prefill attention: the page scatter of PagedKVCacheManager.finalize_cache_bylayer_prefill
+ * (cache_manager.py:93-142) and the prompt write of KVCacheManager, for every request of a batch in one launch.
+ * src0 / src1: [total_rows, n] in src_dtype (bf16 | fp16), row strides src0_st / src1_st in elements.
+ * cu_seqlens: int32 [B + 1] on the device, nondecreasing; cache_seqlens: int32 [B] (tokens already cached) or NULL (0).
+ * Row t < cu_seqlens[b + 1] - cu_seqlens[b] of request b, source row cu_seqlens[b] + t, goes to position
+ * p = cache_seqlens[b] + t of request b:
+ *  - paged (block_table != NULL, int32 [B, bt_stride]): page block_table[b, p / page_size], slot p % page_size (true page
+ *    indexing, any page_size >= 1); only block_table[b, 0 .. ceil((cache_seqlens[b] + len_b) / page_size) - 1] is read;
+ *  - contiguous (block_table == NULL): element b * cache_sb + p * n, with cache_sb a multiple of n and at least
+ *    cache_rows * n; rows with p >= cache_rows are not written (the capacity rule of chitu_b200_gqa_contiguous_attn).
+ * Source rows outside [cu_seqlens[0], cu_seqlens[B]) and from total_rows on are not read; nothing outside the written
+ * slots is touched.  Store: cache_dtype == src_dtype copies the bits (16-byte copies when every address and stride
+ * allows them); cache_dtype CB_FP8_E4M3 (paged only) stores e4m3(clamp(x, -448, 448)), nearest even, NaN kept, the
+ * rule of the e4m3 attention entries, and needs n % 8 == 0, 16-byte aligned sources, strides that are multiples of 8
+ * and 8-byte aligned caches.  One launch whose grid depends on total_rows alone (no host synchronisation, capturable in
+ * a CUDA graph that replays new lengths and positions), deterministic.  Anything else returns a negative status before
+ * any launch; B == 0 or total_rows == 0 launches nothing. */
+int chitu_b200_scatter_kv(void* cache0, void* cache1, const void* src0, int64_t src0_st, const void* src1,
+                          int64_t src1_st, const int32_t* cu_seqlens, const int32_t* cache_seqlens,
+                          const int32_t* block_table, int bt_stride, int page_size, int64_t cache_sb, int cache_rows,
+                          int B, int total_rows, int n, int src_dtype, int cache_dtype, void* stream);
 
 /* ---- MoE routing / permutation -------------------------------------------------------- */
 /* Replaces csrc/moe_align_kernel.cu:27-122 (pybind csrc/binding.cpp:11,
