@@ -126,10 +126,25 @@ inline int launch_smem(const char* name, dim3 grid, dim3 block, size_t smem, cud
   return 0;
 }
 
+// The element type of each dtype code a kernel is built for.
+template <int Code> struct dtype_of;
+template <> struct dtype_of<CB_BF16> { using type = __nv_bfloat16; };
+template <> struct dtype_of<CB_F16> { using type = __half; };
+template <> struct dtype_of<CB_F32> { using type = float; };
+
+// f(T{}) for the element type T of `dtype` when it is one of Codes, returning f's status; any other code is refused
+// under `entry` before f runs.
+template <int... Codes, typename F>
+inline int dispatch_dtype(const char* entry, int dtype, F&& f) {
+  int rc = 0;
+  if (((dtype == Codes && (rc = f(typename dtype_of<Codes>::type{}), true)) || ...)) return rc;
+  return fail(-1, "%s: unsupported dtype %d", entry, dtype);
+}
+
 // f(T{}) for the io type T of `dtype` (CB_BF16, else fp16); returns f's result.
 template <typename F>
 inline auto dispatch_io(int dtype, F&& f) {
-  return dtype == CB_BF16 ? f(__nv_bfloat16{}) : f(__half{});
+  return dtype == CB_BF16 ? f(dtype_of<CB_BF16>::type{}) : f(dtype_of<CB_F16>::type{});
 }
 // f(T{}, std::integral_constant<int, G>{}) for the io type of `dtype` and G = 1, 2, 4, else 8; returns f's status.
 template <typename F>

@@ -191,12 +191,10 @@ void launch_paged_append_e4m3(PagedAppend c0, PagedAppend c1, int n, int dtype, 
                               int page_size, cudaStream_t st) {
   const dim3 grid = append_grid(cu_seqlens, B, rows);
   const int threads = n / 4 < 128 ? 64 : 128;
-  if (dtype == CB_BF16)
-    launch_k(paged_append_e4m3_kernel<__nv_bfloat16>, grid, dim3(threads), 0, st, c0, c1, n, seqlens, cu_seqlens,
+  dispatch_io(dtype, [&](auto t) {
+    launch_k(paged_append_e4m3_kernel<decltype(t)>, grid, dim3(threads), 0, st, c0, c1, n, seqlens, cu_seqlens,
              block_table, bt_stride, B, page_size);
-  else
-    launch_k(paged_append_e4m3_kernel<__half>, grid, dim3(threads), 0, st, c0, c1, n, seqlens, cu_seqlens,
-             block_table, bt_stride, B, page_size);
+  });
 }
 
 // 16-byte copies when every address and stride allows them; 64 threads for rows of fewer than 128 copy units

@@ -96,40 +96,27 @@ extern "C" int chitu_b200_rotary_interleaved(const void* q, const void* k, void*
   cudaStream_t st = (cudaStream_t)stream;
   const int64_t oq_sb = (int64_t)hq * rot_dim, ok_sb = (int64_t)hk * rot_dim;   // dense outputs
   int total = (hq + hk) * rot_dim / 2;
-  // 16-byte path: a thread rotates 4 pairs (one uint4 of 2-byte elements); needs 16 B aligned rows
-  const bool vec_ok = (dtype == CB_BF16 || dtype == CB_F16) && rot_dim % 8 == 0 &&
-                      q_sb % 8 == 0 && q_sh % 8 == 0 && k_sb % 8 == 0 && k_sh % 8 == 0 && oq_sb % 8 == 0 &&
-                      ok_sb % 8 == 0 && aligned16(q) && aligned16(k) && aligned16(out_q) && aligned16(out_k) &&
-                      aligned16(cos) && aligned16(sin);
-  if (vec_ok) {
-    const int64_t nthreads = (int64_t)bs * (hq + hk) * (rot_dim / 8);
-    const int blocks = (int)((nthreads + 127) / 128);
-    if (dtype == CB_BF16)
-      cb::launch_k(rotary_interleaved_vec_kernel<__nv_bfloat16>, dim3(blocks), dim3(128), 0, st,
-                   (const __nv_bfloat16*)q, (const __nv_bfloat16*)k, (__nv_bfloat16*)out_q, (__nv_bfloat16*)out_k, cos, sin,
-                   bs, hq, hk, rot_dim, q_sb, q_sh, k_sb, k_sh, oq_sb, ok_sb);
-    else
-      cb::launch_k(rotary_interleaved_vec_kernel<__half>, dim3(blocks), dim3(128), 0, st, (const __half*)q,
-                   (const __half*)k, (__half*)out_q, (__half*)out_k, cos, sin, bs, hq, hk, rot_dim, q_sb, q_sh, k_sb,
-                   k_sh, oq_sb, ok_sb);
-    CB_LAUNCHED(1);
+  // 16-byte path for 2-byte dtypes: a thread rotates 4 pairs (one uint4); needs 16 B aligned rows
+  const bool vec_ok = rot_dim % 8 == 0 && q_sb % 8 == 0 && q_sh % 8 == 0 && k_sb % 8 == 0 && k_sh % 8 == 0 &&
+                      oq_sb % 8 == 0 && ok_sb % 8 == 0 && aligned16(q) && aligned16(k) && aligned16(out_q) &&
+                      aligned16(out_k) && aligned16(cos) && aligned16(sin);
+  const int rc = dispatch_dtype<CB_BF16, CB_F16, CB_F32>(__func__, dtype, [&](auto t) {
+    using T = decltype(t);
+    if constexpr (sizeof(T) == 2) {
+      if (vec_ok) {
+        const int64_t nthreads = (int64_t)bs * (hq + hk) * (rot_dim / 8);
+        cb::launch_k(rotary_interleaved_vec_kernel<T>, dim3((int)((nthreads + 127) / 128)), dim3(128), 0, st,
+                     (const T*)q, (const T*)k, (T*)out_q, (T*)out_k, cos, sin, bs, hq, hk, rot_dim, q_sb, q_sh, k_sb,
+                     k_sh, oq_sb, ok_sb);
+        return 0;
+      }
+    }
+    const int threads = total >= 256 ? 256 : (total >= 128 ? 128 : 64);
+    cb::launch_k(rotary_interleaved_kernel<T>, dim3(bs), dim3(threads), 0, st, (const T*)q, (const T*)k, (T*)out_q,
+                 (T*)out_k, cos, sin, hq, hk, rot_dim, q_sb, q_sh, k_sb, k_sh, oq_sb, ok_sb);
     return 0;
-  }
-  int threads = total >= 256 ? 256 : (total >= 128 ? 128 : 64);
-  if (dtype == CB_BF16)
-    cb::launch_k(rotary_interleaved_kernel<__nv_bfloat16>, dim3(bs), dim3(threads), 0, st, 
-        (const __nv_bfloat16*)q, (const __nv_bfloat16*)k, (__nv_bfloat16*)out_q, (__nv_bfloat16*)out_k,
-        cos, sin, hq, hk, rot_dim, q_sb, q_sh, k_sb, k_sh, oq_sb, ok_sb);
-  else if (dtype == CB_F16)
-    cb::launch_k(rotary_interleaved_kernel<__half>, dim3(bs), dim3(threads), 0, st, (const __half*)q, (const __half*)k,
-                                                              (__half*)out_q, (__half*)out_k, cos, sin,
-                                                              hq, hk, rot_dim, q_sb, q_sh, k_sb, k_sh, oq_sb, ok_sb);
-  else if (dtype == CB_F32)
-    cb::launch_k(rotary_interleaved_kernel<float>, dim3(bs), dim3(threads), 0, st, (const float*)q, (const float*)k,
-                                                             (float*)out_q, (float*)out_k, cos, sin, hq,
-                                                             hk, rot_dim, q_sb, q_sh, k_sb, k_sh, oq_sb, ok_sb);
-  else
-    return fail(-1, "rotary_interleaved: unsupported dtype %d", dtype);
+  });
+  if (rc) return rc;
   CB_LAUNCHED(1);
   return 0;
 }
@@ -172,19 +159,13 @@ extern "C" int chitu_b200_rotary_half_strided(const void* x, int64_t x_sb, void*
   CB_ARG(x && out && cos && sin);
   CB_ARG(bs >= 0 && heads > 0 && head_dim > 0 && head_dim % 2 == 0 && x_sb >= (int64_t)heads * head_dim);
   if (bs == 0) return 0;
-  cudaStream_t st = (cudaStream_t)stream;
-  int threads = 256;
-  if (dtype == CB_BF16)
-    cb::launch_k(rotary_half_kernel<__nv_bfloat16>, dim3(bs), dim3(threads), 0, st, (const __nv_bfloat16*)x, (__nv_bfloat16*)out,
-                 (const __nv_bfloat16*)cos, (const __nv_bfloat16*)sin, heads, head_dim, x_sb);
-  else if (dtype == CB_F16)
-    cb::launch_k(rotary_half_kernel<__half>, dim3(bs), dim3(threads), 0, st, (const __half*)x, (__half*)out, (const __half*)cos,
-                 (const __half*)sin, heads, head_dim, x_sb);
-  else if (dtype == CB_F32)
-    cb::launch_k(rotary_half_kernel<float>, dim3(bs), dim3(threads), 0, st, (const float*)x, (float*)out, (const float*)cos,
-                 (const float*)sin, heads, head_dim, x_sb);
-  else
-    return fail(-1, "rotary_half: unsupported dtype %d", dtype);
+  const int rc = dispatch_dtype<CB_BF16, CB_F16, CB_F32>(__func__, dtype, [&](auto t) {
+    using T = decltype(t);
+    cb::launch_k(rotary_half_kernel<T>, dim3(bs), dim3(256), 0, (cudaStream_t)stream, (const T*)x, (T*)out,
+                 (const T*)cos, (const T*)sin, heads, head_dim, x_sb);
+    return 0;
+  });
+  if (rc) return rc;
   CB_LAUNCHED(1);
   return 0;
 }
@@ -227,16 +208,13 @@ extern "C" int chitu_b200_rmsnorm_strided(const void* x, const void* w, void* y,
                                           void* stream) {
   CB_ARG(x && w && y && rows >= 0 && dim > 0 && x_stride >= dim && y_stride >= dim);
   if (rows == 0) return 0;
-  cudaStream_t st = (cudaStream_t)stream;
-  if (dtype == CB_BF16)
-    cb::launch_k(rmsnorm_kernel<__nv_bfloat16>, dim3(rows), dim3(256), 0, st, (const __nv_bfloat16*)x, (const __nv_bfloat16*)w,
-                                                        (__nv_bfloat16*)y, dim, eps, x_stride, y_stride);
-  else if (dtype == CB_F16)
-    cb::launch_k(rmsnorm_kernel<__half>, dim3(rows), dim3(256), 0, st, (const __half*)x, (const __half*)w, (__half*)y, dim, eps, x_stride, y_stride);
-  else if (dtype == CB_F32)
-    cb::launch_k(rmsnorm_kernel<float>, dim3(rows), dim3(256), 0, st, (const float*)x, (const float*)w, (float*)y, dim, eps, x_stride, y_stride);
-  else
-    return fail(-1, "rmsnorm: unsupported dtype %d", dtype);
+  const int rc = dispatch_dtype<CB_BF16, CB_F16, CB_F32>(__func__, dtype, [&](auto t) {
+    using T = decltype(t);
+    cb::launch_k(rmsnorm_kernel<T>, dim3(rows), dim3(256), 0, (cudaStream_t)stream, (const T*)x, (const T*)w, (T*)y,
+                 dim, eps, x_stride, y_stride);
+    return 0;
+  });
+  if (rc) return rc;
   CB_LAUNCHED(1);
   return 0;
 }
@@ -383,18 +361,16 @@ extern "C" int chitu_b200_silu_and_mul(const void* x, void* out, int64_t rows, i
                                        void* stream) {
   CB_ARG(x && out && rows >= 0 && d > 0);
   if (rows == 0) return 0;
-  cudaStream_t st = (cudaStream_t)stream;
   int64_t n = rows * d;
   int blocks = (int)((n + 255) / 256);
   if (blocks > 132 * 8) blocks = 132 * 8;
-  if (dtype == CB_BF16)
-    cb::launch_k(silu_and_mul_kernel<__nv_bfloat16>, dim3(blocks), dim3(256), 0, st, (const __nv_bfloat16*)x, (__nv_bfloat16*)out, rows, d);
-  else if (dtype == CB_F16)
-    cb::launch_k(silu_and_mul_kernel<__half>, dim3(blocks), dim3(256), 0, st, (const __half*)x, (__half*)out, rows, d);
-  else if (dtype == CB_F32)
-    cb::launch_k(silu_and_mul_kernel<float>, dim3(blocks), dim3(256), 0, st, (const float*)x, (float*)out, rows, d);
-  else
-    return fail(-1, "silu_and_mul: unsupported dtype %d", dtype);
+  const int rc = dispatch_dtype<CB_BF16, CB_F16, CB_F32>(__func__, dtype, [&](auto t) {
+    using T = decltype(t);
+    cb::launch_k(silu_and_mul_kernel<T>, dim3(blocks), dim3(256), 0, (cudaStream_t)stream, (const T*)x, (T*)out, rows,
+                 d);
+    return 0;
+  });
+  if (rc) return rc;
   CB_LAUNCHED(1);
   return 0;
 }
@@ -436,17 +412,15 @@ extern "C" int chitu_b200_act_quant_fp8(const void* x, void* y, float* s, int64_
   CB_ARG(x && y && s && rows >= 0 && K > 0 && group > 0 && K % group == 0);
   CB_ARG(mode == 0 || mode == 1);
   if (rows == 0) return 0;
-  cudaStream_t st = (cudaStream_t)stream;
   int64_t n_groups = rows * (K / group);
   int blocks = (int)((n_groups + 7) / 8);
-  if (dtype == CB_BF16)
-    cb::launch_k(act_quant_fp8_kernel<__nv_bfloat16>, dim3(blocks), dim3(256), 0, st, (const __nv_bfloat16*)x, (uint8_t*)y, s, n_groups, group, mode, eps);
-  else if (dtype == CB_F16)
-    cb::launch_k(act_quant_fp8_kernel<__half>, dim3(blocks), dim3(256), 0, st, (const __half*)x, (uint8_t*)y, s, n_groups, group, mode, eps);
-  else if (dtype == CB_F32)
-    cb::launch_k(act_quant_fp8_kernel<float>, dim3(blocks), dim3(256), 0, st, (const float*)x, (uint8_t*)y, s, n_groups, group, mode, eps);
-  else
-    return fail(-1, "act_quant_fp8: unsupported dtype %d", dtype);
+  const int rc = dispatch_dtype<CB_BF16, CB_F16, CB_F32>(__func__, dtype, [&](auto t) {
+    using T = decltype(t);
+    cb::launch_k(act_quant_fp8_kernel<T>, dim3(blocks), dim3(256), 0, (cudaStream_t)stream, (const T*)x, (uint8_t*)y,
+                 s, n_groups, group, mode, eps);
+    return 0;
+  });
+  if (rc) return rc;
   CB_LAUNCHED(1);
   return 0;
 }
@@ -484,15 +458,13 @@ extern "C" int chitu_b200_quant_act_int8(const void* x, int8_t* q, float* scales
                                          int dtype, void* stream) {
   CB_ARG(x && q && scales && rows >= 0 && K > 0);
   if (rows == 0) return 0;
-  cudaStream_t st = (cudaStream_t)stream;
-  if (dtype == CB_F16)
-    cb::launch_k(quant_act_int8_kernel<__half>, dim3((unsigned)rows), dim3(256), 0, st, (const __half*)x, q, scales, K);
-  else if (dtype == CB_BF16)
-    cb::launch_k(quant_act_int8_kernel<__nv_bfloat16>, dim3((unsigned)rows), dim3(256), 0, st, (const __nv_bfloat16*)x, q, scales, K);
-  else if (dtype == CB_F32)
-    cb::launch_k(quant_act_int8_kernel<float>, dim3((unsigned)rows), dim3(256), 0, st, (const float*)x, q, scales, K);
-  else
-    return fail(-1, "quant_act_int8: unsupported dtype %d", dtype);
+  const int rc = dispatch_dtype<CB_BF16, CB_F16, CB_F32>(__func__, dtype, [&](auto t) {
+    using T = decltype(t);
+    cb::launch_k(quant_act_int8_kernel<T>, dim3((unsigned)rows), dim3(256), 0, (cudaStream_t)stream, (const T*)x, q,
+                 scales, K);
+    return 0;
+  });
+  if (rc) return rc;
   CB_LAUNCHED(1);
   return 0;
 }
@@ -558,7 +530,8 @@ __global__ void embedding_kernel(const int64_t* __restrict__ ids, const T* __res
 extern "C" int chitu_b200_embedding(const int64_t* ids, const void* table, void* out, int T, int dim,
                                     int64_t vocab_start, int64_t rows, int dtype, void* stream) {
   CB_ARG(ids && table && out && T >= 0 && dim > 0 && rows > 0);
-  CB_ARG(dtype == CB_BF16 || dtype == CB_F16);
+  // the kernel moves rows as 16-byte words, so one uint16_t instance serves both 2-byte dtypes
+  if (int rc = dispatch_dtype<CB_BF16, CB_F16>(__func__, dtype, [](auto) { return 0; })) return rc;
   CB_ARG((dim * 2) % 16 == 0);
   CB_ARG(((uintptr_t)table | (uintptr_t)out) % 16 == 0);                                  // uint4 rows
   if (T == 0) return 0;
@@ -579,13 +552,12 @@ extern "C" int chitu_b200_add(const void* a, const void* b, void* y, int64_t n, 
   if (n == 0) return 0;
   int blocks = (int)((n + 255) / 256);
   if (blocks > 132 * 8) blocks = 132 * 8;
-  cudaStream_t st = (cudaStream_t)stream;
-  if (dtype == CB_BF16)
-    cb::launch_k(add_kernel<__nv_bfloat16>, dim3(blocks), dim3(256), 0, st, (const __nv_bfloat16*)a, (const __nv_bfloat16*)b, (__nv_bfloat16*)y, n);
-  else if (dtype == CB_F16)
-    cb::launch_k(add_kernel<__half>, dim3(blocks), dim3(256), 0, st, (const __half*)a, (const __half*)b, (__half*)y, n);
-  else
-    return fail(-1, "add: unsupported dtype %d", dtype);
+  const int rc = dispatch_dtype<CB_BF16, CB_F16>(__func__, dtype, [&](auto t) {
+    using T = decltype(t);
+    cb::launch_k(add_kernel<T>, dim3(blocks), dim3(256), 0, (cudaStream_t)stream, (const T*)a, (const T*)b, (T*)y, n);
+    return 0;
+  });
+  if (rc) return rc;
   CB_LAUNCHED(1);
   return 0;
 }
@@ -622,13 +594,12 @@ __global__ void __launch_bounds__(1024) argmax_kernel(const T* __restrict__ logi
 extern "C" int chitu_b200_argmax(const void* logits, int64_t* out, int T, int64_t V, int dtype, void* stream) {
   CB_ARG(logits && out && T >= 0 && V > 0);
   if (T == 0) return 0;
-  cudaStream_t st = (cudaStream_t)stream;
-  if (dtype == CB_F32)
-    cb::launch_k(argmax_kernel<float>, dim3(T), dim3(1024), 0, st, (const float*)logits, out, V);
-  else if (dtype == CB_BF16)
-    cb::launch_k(argmax_kernel<__nv_bfloat16>, dim3(T), dim3(1024), 0, st, (const __nv_bfloat16*)logits, out, V);
-  else
-    return fail(-1, "argmax: unsupported dtype %d", dtype);
+  const int rc = dispatch_dtype<CB_F32, CB_BF16>(__func__, dtype, [&](auto t) {
+    using E = decltype(t);
+    cb::launch_k(argmax_kernel<E>, dim3(T), dim3(1024), 0, (cudaStream_t)stream, (const E*)logits, out, V);
+    return 0;
+  });
+  if (rc) return rc;
   CB_LAUNCHED(1);
   return 0;
 }

@@ -174,18 +174,13 @@ extern "C" int chitu_b200_sample_top_k_top_p(const void* logits, int64_t row_str
                                              float* out_mass, void* stream) {
   CB_ARG(logits && temperatures && top_ks && top_ps && uniforms && out_tokens && B >= 0 && V > 0 && row_stride >= V);
   if (B == 0) return 0;
-  cudaStream_t st = (cudaStream_t)stream;
-  if (dtype == CB_BF16)
-    cb::launch_k(sample_kernel<__nv_bfloat16>, dim3(B), dim3(kThreads), 0, st, (const __nv_bfloat16*)logits, row_stride, V,
+  const int rc = cb::dispatch_dtype<CB_BF16, CB_F16, CB_F32>(__func__, dtype, [&](auto t) {
+    using T = decltype(t);
+    cb::launch_k(sample_kernel<T>, dim3(B), dim3(kThreads), 0, (cudaStream_t)stream, (const T*)logits, row_stride, V,
                  temperatures, top_ks, top_ps, uniforms, out_tokens, out_kept, out_mass);
-  else if (dtype == CB_F16)
-    cb::launch_k(sample_kernel<__half>, dim3(B), dim3(kThreads), 0, st, (const __half*)logits, row_stride, V, temperatures,
-                 top_ks, top_ps, uniforms, out_tokens, out_kept, out_mass);
-  else if (dtype == CB_F32)
-    cb::launch_k(sample_kernel<float>, dim3(B), dim3(kThreads), 0, st, (const float*)logits, row_stride, V, temperatures,
-                 top_ks, top_ps, uniforms, out_tokens, out_kept, out_mass);
-  else
-    return cb::fail(-1, "sample_top_k_top_p: unsupported logits dtype %d", dtype);
+    return 0;
+  });
+  if (rc) return rc;
   CB_LAUNCHED(1);
   return 0;
 }
