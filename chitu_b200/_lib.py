@@ -69,6 +69,7 @@ SIGNATURES = {
     "chitu_b200_mla_attn_fp8kv": (I, [P, P, P, P, P, P, I, I, I, I, I, I, I, I, I, I, F, P, P, L, P]),
     "chitu_b200_debug_timeline": (I, [P]),
     "chitu_b200_debug_timeline_names": (c_char_p, []),
+    "chitu_b200_debug_comm_push_area": (I, [P, P, P, P]),
     "chitu_b200_decode_prepare": (I, [P, P, P, I, P, P, P, I, I, I, P]),
     "chitu_b200_attn_plan": (I, [P, I, I, I, I, P, L, P]),
     "chitu_b200_mla_num_splits": (I, [I, I, I, L]),

@@ -503,6 +503,16 @@ extern "C" int chitu_b200_comm_status(void* handle) {
   return (int)v;
 }
 
+// The local push area and the call counter, for tests that write or inspect the words directly (see the header).
+extern "C" int chitu_b200_debug_comm_push_area(void* handle, void** area, int64_t* source_bytes, uint32_t** calls) {
+  CB_ARG(handle && area && source_bytes && calls);
+  Comm* c = (Comm*)handle;
+  *area = c->pbuf[c->rank];
+  *source_bytes = 2 * c->slot_bytes;
+  *calls = c->pflags[c->rank] + 17;
+  return 0;
+}
+
 extern "C" int chitu_b200_comm_destroy(void* handle) {
   if (!handle) return 0;
   Comm* c = (Comm*)handle;

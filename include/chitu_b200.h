@@ -390,6 +390,13 @@ int chitu_b200_sample_top_k_top_p(const void* logits, int64_t row_stride, int B,
 /* ---- dev tool: in-graph kernel timeline (see csrc/common.cuh) ------------------------------------------------ */
 int chitu_b200_debug_timeline(void* buf /* uint64 [2 + capacity] on the device, or NULL to disarm */);
 const char* chitu_b200_debug_timeline_names(void);
+/* Read-only view of a communicator's push-mode state, for tests that write or inspect the words themselves.
+ * *area: this rank's push area on the device, [2 slots][world sources][*source_bytes], *source_bytes = 2 * slot_bytes.
+ * Word k of a source's [rows, dim] bf16 partial sits at byte k * 8 and holds
+ *   { uint32 (bf16 x[2k] | bf16 x[2k+1] << 16), uint32 epoch }.
+ * *calls: the device uint32 counting the reduces this rank has consumed; the next reduce reads slot *calls & 1 and
+ * waits for epoch *calls + 1. */
+int chitu_b200_debug_comm_push_area(void* handle, void** area, int64_t* source_bytes, uint32_t** calls);
 
 /* ---- device-side decode-step preparation (SURVEY §8f n2 / §8a a1) ------------------------------------------
  * chitu_b200_decode_prepare = PagedKVCacheManager.prepare_cache_decode + prepare_block_table_for_decode

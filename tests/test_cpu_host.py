@@ -2,6 +2,7 @@
 declares, argument validation returns status codes (never exits), the host shims refuse CPU
 tensors (no fallback), the roofline byte model matches BASELINE.md, and the tensor-parallel
 host logic (world_size 2, gloo) equals the unsharded result."""
+import ctypes
 import os
 import re
 import sys
@@ -94,6 +95,9 @@ def test_round2_entries_validate_arguments():
     assert lib.chitu_b200_linear_bf16_ar(None, None, 1, 4096, 4096, None, None, 0, None) < 0
     assert lib.chitu_b200_fp8_gemm_ar(None, None, None, None, 1, 4096, 4096, None, None, 0, None) < 0
     assert lib.chitu_b200_comm_status(None) < 0
+    area, nbytes, calls = ctypes.c_void_p(), ctypes.c_int64(), ctypes.c_void_p()
+    assert lib.chitu_b200_debug_comm_push_area(None, ctypes.byref(area), ctypes.byref(nbytes), ctypes.byref(calls)) < 0
+    assert b"debug_comm_push_area" in lib.chitu_b200_last_error()
     # device-side step preparation / plan / sampling
     assert lib.chitu_b200_decode_prepare(None, None, None, 1, None, None, None, 1, 64, 1, None) < 0
     assert lib.chitu_b200_sample_top_k_top_p(None, 128, 1, 128, _lib.CB_BF16, None, None, None, None, None, None, None, None) < 0
