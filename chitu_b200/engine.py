@@ -108,6 +108,9 @@ class DecodeEngine:
             self.comm = FusedAllReduce(process_group, max_reqs, dim, dev)
         self.graph = None
         self.launches_per_step = 0
+        # set to [] to record the residual stream entering every layer, and the last layer's output (tests; eager steps
+        # only, never under a graph)
+        self.capture_h = None
 
     def _rope_tables(self, ang: torch.Tensor, dtype=torch.float32):
         """cos / sin tables from the rotary angles [positions, rot_dim / 2], and the per-step buffers that
@@ -319,6 +322,8 @@ class LlamaDecodeEngine(DecodeEngine):
         n_layers = len(self.layers)
         self._norm(h, self.layers[0]["attn_norm"], self.xn)
         for li, lw in enumerate(self.layers):
+            if self.capture_h is not None:
+                self.capture_h.append(h.clone())
             next_norm = self.layers[li + 1]["attn_norm"] if li + 1 < n_layers else self.norm
             self._linear(self.xn, lw["wqkv"], self.qkv, B)
             q_view, k_view = self.qkv, self.qkv[:, self.Hq * D:]
@@ -361,3 +366,5 @@ class LlamaDecodeEngine(DecodeEngine):
             self._row_parallel(lambda out, res: self._linear(self.act, lw["w2"], out, B, residual=res),
                                lambda: self.comm.linear_push(self.act, lw["w2"], B, self.lin_ws),
                                h2, h, next_norm, y=self.xn)
+        if self.capture_h is not None:
+            self.capture_h.append(h.clone())

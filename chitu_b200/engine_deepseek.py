@@ -196,7 +196,6 @@ class DeepSeekDecodeEngine(DecodeEngine):
                                                                      2 * self.F_moe, dim), dtype=torch.uint8, device=dev)
         self.gate_ws = torch.zeros(lib.chitu_b200_moe_gate_workspace_bytes(B, c.n_routed_experts), dtype=torch.uint8, device=dev)
         self.trace = None          # set to [] to record per-layer intermediates (tests; not under CUDA graphs)
-        self.capture_h = None      # set to [] to record the residual stream at every layer boundary of the FAST path
 
     # ---- helpers -----------------------------------------------------------------------------------
     def _dequant(self, w, s):
@@ -293,7 +292,7 @@ class DeepSeekDecodeEngine(DecodeEngine):
         n_layers = len(self.layers)
         self._norm(h, self.layers[0]["attn_norm"], **self._norm_out(False))
         for li, L in enumerate(self.layers):
-            if self.capture_h is not None:       # tests: the residual stream entering every layer (never under a graph)
+            if self.capture_h is not None:
                 self.capture_h.append(h.clone())
             last = li + 1 == n_layers
             next_norm = self.norm if last else self.layers[li + 1]["attn_norm"]

@@ -99,6 +99,8 @@ class MixtralDecodeEngine(DecodeEngine):
         n_layers = len(self.layers)
         self._norm(h, self.layers[0]["attn_norm"], self.xn)
         for li, lw in enumerate(self.layers):
+            if self.capture_h is not None:
+                self.capture_h.append(h.clone())
             next_norm = self.layers[li + 1]["attn_norm"] if li + 1 < n_layers else self.norm
             self._linear(self.xn, lw["wqkv"], self.qkv, B)
             q = self.qkv[:, : self.Hq * D]
@@ -130,6 +132,8 @@ class MixtralDecodeEngine(DecodeEngine):
                                                self.gate_i_all[li], _lib.CB_I64, B, self.topk, self.E, 2 * self.F, cfg.dim, 0,
                                                self.moe_ws),
                 h2, h, next_norm, y=self.xn, partial=self.y)
+        if self.capture_h is not None:
+            self.capture_h.append(h.clone())
 
     def distinct_experts_per_layer(self) -> float:
         ids = self.gate_i_all.cpu()
