@@ -299,10 +299,11 @@ __device__ __forceinline__ void gqa_decode_mmaT_cta(
   static_assert(G <= 8, "heads of one kv group are the n = 8 side of the MMA");
   constexpr bool kE4m3 = sizeof(C) == 1;
   static_assert(!(kE4m3 && CONTIG), "the e4m3 cache is paged");
-  // The K/V pages are only written by earlier decode steps and by this kernel; sequence lengths and the block table by
-  // kernels that do not trigger dependents early: the first tiles of every warp are put in flight BEFORE
-  // griddepcontrol.wait (they overlap the tail of the qkv GEMM); q / k_new / v_new (the previous kernel's output) are
-  // only touched after it.
+  // Sequence lengths and the block table are written only by kernels that do not trigger dependents early (torch copies,
+  // decode_prepare), so they are read before griddepcontrol.wait.  The K/V rows are not: the appends, the scatter and the
+  // decode kernels (this one included) trigger early and write the cache after their own wait, so a cache row may still
+  // be in flight until this kernel's wait returns.  No tile is loaded before it; the first tiles are only prefetched
+  // into L2, which binds no value (the loads after the wait read through L2, where the writer's stores land).
   cb::pdl_launch_dependents();
   constexpr int D = kGqaD;
   constexpr int kTileBytes = kGqaTile * D * 2;              // K tile bytes (V the same)
@@ -326,6 +327,10 @@ __device__ __forceinline__ void gqa_decode_mmaT_cta(
   // tiles warp, warp + kGqaWarps, ...
   const int my_tiles = ntiles_total > warp ? (ntiles_total - warp + kGqaWarps - 1) / kGqaWarps : 0;
 
+  auto cache_row = [&](int key) -> int64_t {    // row of (key, kvh) in units of D
+    if constexpr (CONTIG) return ((int64_t)b * rows_sb + key) * Hkv + kvh;
+    return ((int64_t)bt[key >> page_shift] * page_size + (key & (page_size - 1))) * Hkv + kvh;
+  };
   auto issue = [&](int ti, int stage) {
     const int key0 = begin + (warp + kGqaWarps * ti) * kGqaTile;
     if constexpr (kE4m3) {                   // rows of 128 bytes, unswizzled; the appended and masked rows are zero
@@ -338,8 +343,7 @@ __device__ __forceinline__ void gqa_decode_mmaT_cta(
         const C *ksrc = k_cache, *vsrc = v_cache;
         int nbytes = 0;
         if (key < L_cache && key < end) {
-          const int page = bt[key >> page_shift];
-          const int64_t row = ((int64_t)page * page_size + (key & (page_size - 1))) * Hkv + kvh;
+          const int64_t row = cache_row(key);
           ksrc = k_cache + row * D;
           vsrc = v_cache + row * D;
           nbytes = 16;
@@ -358,13 +362,7 @@ __device__ __forceinline__ void gqa_decode_mmaT_cta(
         const T *ksrc = k_cache, *vsrc = v_cache;
         int nbytes = 16;
         if (key < L_cache && key < end) {
-          int64_t row;                       // row of (key, kvh) in units of D
-          if constexpr (CONTIG) {
-            row = ((int64_t)b * rows_sb + key) * Hkv + kvh;
-          } else {
-            const int page = bt[key >> page_shift];
-            row = ((int64_t)page * page_size + (key & (page_size - 1))) * Hkv + kvh;
-          }
+          const int64_t row = cache_row(key);
           ksrc = k_cache + row * D;
           vsrc = v_cache + row * D;
         } else if (key < end) {              // the token being appended (key == L_cache)
@@ -381,12 +379,19 @@ __device__ __forceinline__ void gqa_decode_mmaT_cta(
     }
   };
 
-  // tiles that lie completely inside the cached part of the sequence can be fetched before the previous kernel is done
-  bool early[kGqaStages - 1];
+  // the K and V rows of the tiles the prologue below stages, as 128-byte lines into L2
+  constexpr int kRowLines = D * (int)sizeof(C) / 128;
 #pragma unroll
   for (int s = 0; s < kGqaStages - 1; ++s) {
-    early[s] = s < my_tiles && begin + (warp + kGqaWarps * s + 1) * kGqaTile <= min(L_cache, end);
-    if (early[s]) issue(s, s);
+    const int key0 = begin + (warp + kGqaWarps * s) * kGqaTile;
+#pragma unroll
+    for (int i = lane; i < 2 * kGqaTile * kRowLines; i += 32) {
+      const int key = key0 + i % kGqaTile, line = i / kGqaTile;
+      if (s < my_tiles && key < L_cache && key < end) {
+        const C* src = (line & 1 ? v_cache : k_cache) + cache_row(key) * D;
+        asm volatile("prefetch.global.L2 [%0];" ::"l"(reinterpret_cast<const uint8_t*>(src) + (line >> 1) * 128));
+      }
+    }
   }
   cb::pdl_wait();
   cb::tl_stamp();
@@ -458,8 +463,8 @@ __device__ __forceinline__ void gqa_decode_mmaT_cta(
   const float sc = scale * kLog2e;
 
   for (int s = 0; s < kGqaStages - 1; ++s) {
-    if (s < my_tiles && !early[s]) issue(s, s);
-    else if (!early[s]) cp_async_commit();
+    if (s < my_tiles) issue(s, s);
+    else cp_async_commit();
   }
   for (int ti = 0; ti < my_tiles; ++ti) {
     const int stage = ti % kGqaStages;

@@ -13,8 +13,10 @@
 //   so a cache row is read from HBM exactly once and the tensor pipe does 36 + 32 tiny MMAs per 64-key page.
 //   warp 4   TMA producer: one page = 9 boxes [64 keys x 128 B] (128B swizzle); the 8 latent chunks go through a ring of
 //            22 x 8 KB slots (2.75 pages in flight), the rope chunk through its own 3-slot ring (it is released right
-//            after Q.K^T).  KV streaming starts BEFORE griddepcontrol.wait: cache rows are only written by earlier decode
-//            steps and by this kernel, so the stream overlaps the tail of the previous kernel (PDL).
+//            after Q.K^T).  KV streaming starts after griddepcontrol.wait: the appends, the scatter and the decode
+//            kernels (this one included) trigger their dependents early and write cache rows after their own wait, so a
+//            row may be in flight until the wait returns.  Barrier init, the tensormap prefetch and an L2 prefetch of
+//            the first pages (it binds no value) overlap the tail of the previous kernel (PDL).
 //   warps 0-3 one warpgroup: Q.K^T (S^T in registers: 2 keys x 4 heads per thread), softmax, P -> shared memory, P.V
 //            (O^T in registers: 8 tiles x 2 dims x 4 heads per thread).  Per-head running max across the 64 keys by
 //            shuffles + one shared-memory exchange between the 4 warps; O^T is only rescaled when a head's max moved
@@ -37,6 +39,7 @@ constexpr int kQBytes = 9 * 16 * 128;          // Q as 9 K-major chunks of [16 h
 constexpr int kPBytes = 16 * 128;              // P as [16 heads x 64 keys] bf16, K-major
 constexpr float kLog2e = 1.4426950408889634f;
 constexpr float kRescaleThreshold = 8.f;       // log2 domain
+constexpr int kL2Pages = 3;                    // pages prefetched into L2 before griddepcontrol.wait (~ the bf16 ring)
 
 // The CTA's shape for a cache element type KV.  bf16: warpgroup (warps 0-3) + producer warp, a ring of 22 latent and
 // 3 rope slots.  e4m3: the producer streams each page as 9 boxes of 4 KB into a ring of 14 e4m3 slots, and four
@@ -140,10 +143,17 @@ __device__ __forceinline__ void mla_decode_cta(
   const int ntiles = end > begin ? (end - begin + kTile - 1) / kTile : 0;
   const int32_t* bt = block_table + (int64_t)b * bt_stride;
 
+  // The producer's first pages go into L2 before its griddepcontrol.wait; the TMA loads issued after the wait read through
+  // L2, where the stores of a cache writer still in flight land.
+  if (warp == 4 && lane == 0)
+    for (int it = 0; it < min(ntiles, kL2Pages); ++it)
+      for (int c = 0; c < 9; ++c) tma_prefetch_l2_2d(&map_kv, c * 64, bt[(begin + it * kTile) / kTile] * kTile);
+
   if (kFp8 && warp == 4) {
     // ================= e4m3 TMA producer: the 9 boxes of each page, in order, through the e4m3 ring =================
     constexpr int kNEr = kFp8 ? kNE : 1;                    // (the bf16 instance compiles this branch away)
     const uint64_t pol = l2_policy_evict_first();
+    cb::pdl_wait();                                         // cache rows may still be in flight until here
     for (int it = 0; it < ntiles; ++it) {
       const int row0 = bt[(begin + it * kTile) / kTile] * kTile;
       for (int c = 0; c < 9; ++c) {
@@ -218,7 +228,7 @@ __device__ __forceinline__ void mla_decode_cta(
     // ================= TMA producer (whole warp: lane 0 issues, all lanes patch the tail page) =================
     const uint64_t pol = l2_policy_evict_first();
     uint32_t raw_phase = 0;
-    bool waited = false;
+    cb::pdl_wait();                                         // cache rows and new_kv may still be in flight until here
     for (int it = 0; it < ntiles; ++it) {
       const int key0 = begin + it * kTile;
       const int row0 = bt[key0 / kTile] * kTile;
@@ -256,7 +266,6 @@ __device__ __forceinline__ void mla_decode_cta(
             tma_load_2d(s_ring + ((it * 8 + c) % kNSM) * kSlot, &map_kv, &raw_bar, c * 64, row0, pol);
           tma_load_2d(s_rope + rs * kSlot, &map_kv, &raw_bar, 8 * 64, row0, pol);
         }
-        if (!waited) { cb::pdl_wait(); waited = true; }                     // new_kv is written by the previous kernel
         mbar_wait(&raw_bar, raw_phase);
         raw_phase ^= 1;
         for (int c = 0; c < 9; ++c) {

@@ -81,6 +81,10 @@ __device__ __forceinline__ uint64_t l2_policy_evict_last() {
   return p;
 }
 
+// One box into L2 only.  A prefetch binds no value: a load issued later still sees every write made visible to it.
+__device__ __forceinline__ void tma_prefetch_l2_2d(const CUtensorMap* map, int c0, int c1) {
+  asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];" ::"l"(map), "r"(c0), "r"(c1) : "memory");
+}
 __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1,
                                             uint64_t policy) {
   asm volatile(

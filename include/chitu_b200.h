@@ -167,7 +167,13 @@ int64_t chitu_b200_linear_workspace_bytes(int M, int N);
  * Weight contract: the wgmma GEMM starts streaming its weights while the previous kernel of the stream is still running
  * (before griddepcontrol.wait).  A weight must therefore be written by host copies, torch kernels or
  * chitu_b200_weight_dequant_fp8, never by a kernel that triggers its dependents early (griddepcontrol.launch_dependents)
- * directly before the linear. */
+ * directly before the linear.
+ * KV contract: the cache writers (chitu_b200_scatter_kv, chitu_b200_append_paged_kv[_e4m3], the seqlen_q > 1 attention
+ * entries and the in-place append of the decode entries) trigger their dependents early and write after their own
+ * wait, so the attention kernels load no KV cache row before griddepcontrol.wait; any writer may directly precede any
+ * reader of the same cache.  The decode kernels do read cache_seqlens / seqlens_excl, the block table and the MLA split
+ * plan before that wait: those must come from host copies, torch kernels, chitu_b200_decode_prepare or
+ * chitu_b200_attn_plan, none of which triggers its dependents early. */
 /* F.linear for bf16/fp16 weights (linear_deepseek_v3 element_size()>1 branch,
  * model_deepseek_v3.py:84-85; tensor_parallel.py linear_op default). y = x W^T (+bias) (+residual). */
 int chitu_b200_linear_bf16(const void* x, const void* w, const void* bias, const void* residual,
