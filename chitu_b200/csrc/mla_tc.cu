@@ -61,22 +61,6 @@ constexpr int decode_smem_bytes() {
 static_assert(1024 + decode_smem_bytes<__nv_bfloat16>() <= 227 * 1024, "bf16 decode CTA exceeds shared memory");
 static_assert(1024 + decode_smem_bytes<__nv_fp8_e4m3>() <= 227 * 1024, "e4m3 decode CTA exceeds shared memory");
 
-// dev tool (profiling build only, -DCB_TIMELINE): %globaltimer at fixed points of every CTA, 32 slots per CTA, read by
-// scripts/mla_probe.py.  The product library compiles these to nothing.
-#ifdef CB_TIMELINE
-static __device__ unsigned long long* d_mla_probe = nullptr;
-__device__ __forceinline__ void probe(int idx) {
-  unsigned long long* b = d_mla_probe;
-  if (b != nullptr) {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    b[(((int64_t)blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) * 32 + idx] = t;
-  }
-}
-#else
-__device__ __forceinline__ void probe(int) {}
-#endif
-
 // value h of a 16-entry register array without dynamic register indexing
 __device__ __forceinline__ float pick16(const float (&v)[16], int h) {
   float r = v[0];
@@ -114,7 +98,6 @@ __device__ __forceinline__ void mla_decode_cta(
   const int h0 = hg * 16;
 
   if (threadIdx.x == 0) {
-    probe(0);
     // e4m3: a bf16 slot is published by the four converter warps, an e4m3 slot released by them
     for (int i = 0; i < kNSM; ++i) { mbar_init(&full_m[i], kFp8 ? 4 : 1); mbar_init(&empty_m[i], 1); }
     for (int i = 0; i < kNSR; ++i) { mbar_init(&full_r[i], kFp8 ? 4 : 1); mbar_init(&empty_r[i], 1); }
@@ -241,7 +224,6 @@ __device__ __forceinline__ void mla_decode_cta(
           const int g = it * 8 + c, s = g % kNSM;
           mbar_wait(&empty_m[s], ((g / kNSM) & 1) ^ 1);
           if (lane == 0) {
-            if (it == 0 && c == 0) probe(30);
             mbar_expect_tx(&full_m[s], kSlot);
             tma_load_2d(s_ring + s * kSlot, &map_kv, &full_m[s], c * 64, row0, pol);
           }
@@ -292,7 +274,6 @@ __device__ __forceinline__ void mla_decode_cta(
     // ---- Q -> shared memory (K-major, swizzled); rows >= H are zero ----
     cb::pdl_wait();
     cb::tl_stamp();
-    if (t == 0) probe(1);
     {
       // 16 heads x 72 units of 16 B = 9 units per thread: all nine global loads are issued before the first shared-memory
       // store
@@ -317,7 +298,6 @@ __device__ __forceinline__ void mla_decode_cta(
     }
     fence_async_smem();
     asm volatile("bar.sync 1, 128;" ::: "memory");
-    if (t == 0) probe(2);
     if (new_kv && split == 0 && hg == 0) {                   // append for the following steps (ops.py:50-91)
       const int page = bt[L_cache / kTile];
       KV* dst = kv_cache + ((int64_t)page * kTile + L_cache % kTile) * kRow;
@@ -370,10 +350,7 @@ __device__ __forceinline__ void mla_decode_cta(
                             make_sw128_desc(q_a + 8 * 2048 + 32 * k, 16, 1024), 1);
       wgmma_commit();
       wgmma_wait<0>();
-      if (t == 0) {
-        mbar_arrive(&empty_r[rs]);                           // the rope chunk is not needed by P.V
-        if (it < 12) probe(3 + 2 * it);
-      }
+      if (t == 0) mbar_arrive(&empty_r[rs]);                 // the rope chunk is not needed by P.V
 
       // ---- per-head tile maximum over the 64 keys (finite: every tile has a valid key) ----
 #pragma unroll
@@ -428,7 +405,6 @@ __device__ __forceinline__ void mla_decode_cta(
       }
       fence_async_smem();
       asm volatile("bar.sync 1, 128;" ::: "memory");          // P complete; red_max free for the next tile
-      if (t == 0 && it < 12) probe(4 + 2 * it);
 
       // ---- O^T += V^T . P^T: the 8 latent chunks of the page, each a 64-dim M tile read MN-major ----
       wgmma_fence();
@@ -452,7 +428,6 @@ __device__ __forceinline__ void mla_decode_cta(
       const float ls = rows_sum(l_part[x]);
       if (lane < 4) red_sum[warp][hc + 8 * (x >> 1) + (x & 1)] = ls;
     }
-    if (t == 0) probe(28);
     asm volatile("bar.sync 1, 128;" ::: "memory");
     const bool direct = num_splits == 1 && out != nullptr;   // out == NULL: partials even for one split (deferred merge)
     float inv[4];
@@ -479,7 +454,6 @@ __device__ __forceinline__ void mla_decode_cta(
       const float l = (red_sum[0][t] + red_sum[1][t]) + (red_sum[2][t] + red_sum[3][t]);
       lse[((int64_t)b * H + h0 + t) * num_splits + split] = (ntiles > 0 && l > 0.f) ? pick16(m_run, t) + log2f(l) : -INFINITY;
     }
-    if (t == 0) probe(29);
   }
 }
 
@@ -584,8 +558,3 @@ extern "C" int chitu_b200_mla_decode(const void* q_nope, const void* q_pe, void*
 }
 
 CB_DEFINE_TL_SETTER(mla_tc)
-#ifdef CB_TIMELINE
-extern "C" int chitu_b200_debug_mla_probe(unsigned long long* p) {      // p: uint64 [CTAs * 32], zero-filled; NULL disarms
-  return (int)cudaMemcpyToSymbol(cb::d_mla_probe, &p, sizeof(p));
-}
-#endif

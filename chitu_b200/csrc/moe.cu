@@ -37,21 +37,6 @@ struct MoePlan {
   float* w_sorted;    // [P] routed weight of sorted row r
 };
 
-// dev tool (profiling build only, -DCB_TIMELINE): %globaltimer of thread 0 at fixed points of the plan (scripts/moe_probe.py)
-#ifdef CB_TIMELINE
-static __device__ unsigned long long* d_moe_probe = nullptr;
-__device__ __forceinline__ void mprobe(int idx) {
-  unsigned long long* b = d_moe_probe;
-  if (b != nullptr && threadIdx.x == 0) {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    b[idx] = t;
-  }
-}
-#else
-__device__ __forceinline__ void mprobe(int) {}
-#endif
-
 // The plan itself, run by one CTA of kPlanThreads threads.  `sm` needs moe_plan_smem_ints(P, E) ints.  E <= kPlanThreads:
 // a thread owns one expert in the block-wide scans.
 constexpr int kPlanThreads = 1024;
@@ -76,14 +61,12 @@ __device__ __forceinline__ void moe_plan_large(const IdT* ids, const void* topk_
                         : __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(topk_w)[p]);
   }
   __syncthreads();
-  mprobe(2);
   for (int p = tid; p < P; p += NT) {
     const int e = sid[p];
     if (e >= 0 && e < E) atomicAdd(&cnt[e], 1);
     else pl.pos[p] = -1;      // expert not on this rank (expert_map == -1)
   }
   __syncthreads();
-  mprobe(3);
   // block-wide exclusive scan of cnt[] and of the row-chunk counts (E <= 1024).  An expert with more than BN routed rows
   // (bs > 128, or the shared expert that every token visits) is cut into chunks of BN rows: each chunk is a tile column
   // of the grouped GEMM (its weight tile is re-read per chunk, mostly from L2).
@@ -114,7 +97,6 @@ __device__ __forceinline__ void moe_plan_large(const IdT* ids, const void* topk_
     *pl.num_tiles2 = na * (K1 / 128);
   }
   __syncthreads();
-  mprobe(4);
   // stable scatter: one warp per active expert, ballot-compaction over the pairs in order
   for (int e = warp; e < E; e += NW) {
     const int n = cnt[e];
@@ -149,11 +131,6 @@ __device__ __forceinline__ void moe_plan_large(const IdT* ids, const void* topk_
       }
     }
   }
-#ifdef CB_TIMELINE
-  mprobe(5);
-  __syncthreads();
-  mprobe(6);
-#endif
 }
 
 // Decode-sized plans (P <= 1024 pairs): every phase is parallel over PAIRS or over TILE-LIST ENTRIES instead of one warp
@@ -180,7 +157,6 @@ __device__ __forceinline__ void moe_plan_small(const IdT* ids, const void* topk_
                         : __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(topk_w)[p]);
   }
   __syncthreads();
-  mprobe(2);
   // histogram + the pair's rank among the earlier pairs of the same expert (stable order), one pass over shared memory;
   // thread p owns pair p
   int my_rank = -1;
@@ -196,7 +172,6 @@ __device__ __forceinline__ void moe_plan_small(const IdT* ids, const void* topk_
     }
   }
   __syncthreads();
-  mprobe(3);
   // block-wide exclusive scan of the counts and of the row-chunk counts (E <= 1024)
   const int c = tid < E ? cnt[tid] : 0, ch = (c + BN - 1) / BN;
   int ci = c, ai = ch;
@@ -231,7 +206,6 @@ __device__ __forceinline__ void moe_plan_small(const IdT* ids, const void* topk_
     *pl.num_tiles2 = na * (K1 / 128);
   }
   __syncthreads();
-  mprobe(4);
   // one thread per pair: its sorted row
   if (my_rank >= 0) {
     const int rr = start[sid[tid]] + my_rank;
@@ -239,7 +213,6 @@ __device__ __forceinline__ void moe_plan_small(const IdT* ids, const void* topk_
     pl.pos[tid] = rr;
     pl.w_sorted[rr] = swt[tid];
   }
-  mprobe(5);
   // one thread per tile-list entry of either GEMM
   const int t1 = N1 / 128, t2 = K1 / 128, per = t1 + t2;
   for (int wk = tid; wk < na * per; wk += NT) {
@@ -258,10 +231,6 @@ __device__ __forceinline__ void moe_plan_small(const IdT* ids, const void* topk_
       pl.tile2_cnt[ti] = rows;
     }
   }
-#ifdef CB_TIMELINE
-  __syncthreads();
-  mprobe(6);
-#endif
 }
 
 // --------------------------------------------------------------------------------------------
@@ -686,13 +655,10 @@ __global__ void moe_sum_kernel(const __nv_bfloat16* __restrict__ c3, __nv_bfloat
 template <typename IdT>
 __global__ void __launch_bounds__(kPlanThreads) moe_plan_kernel(const IdT* __restrict__ ids, const void* __restrict__ topk_w,
                                                                int topk_w_f32, int P, int E, int N1, int K1, int BN, MoePlan pl) {
-  mprobe(0);
   cb::pdl_prologue();
-  mprobe(1);
   extern __shared__ int sm[];
   if (P <= kPlanThreads) moe_plan_small<IdT>(ids, topk_w, topk_w_f32, P, E, N1, K1, BN, pl, sm);
   else moe_plan_large<IdT>(ids, topk_w, topk_w_f32, P, E, N1, K1, BN, pl, sm);
-  mprobe(7);
 }
 
 // one warp per (sorted row, 128-group): gather the token's row, quantise (mode 1) or copy (bf16 mode)
@@ -1173,8 +1139,3 @@ extern "C" int chitu_b200_fused_experts_ar(const void* x, const void* w1, const 
 }
 
 CB_DEFINE_TL_SETTER(moe)
-#ifdef CB_TIMELINE
-extern "C" int chitu_b200_debug_moe_probe(unsigned long long* p) {      // p: uint64 [16], zero-filled; NULL disarms
-  return (int)cudaMemcpyToSymbol(d_moe_probe, &p, sizeof(p));
-}
-#endif

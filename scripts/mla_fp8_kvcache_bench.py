@@ -33,6 +33,7 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "scripts"))
 
 from chitu_b200.attn_backend import B200AttnBackend  # noqa: E402
+from fp8_kvcache_bench import alternate, quant  # noqa: E402
 from paged_prefill_bench import gpu_info, max_rel, spread, time_ms  # noqa: E402
 
 C, R, PAGE = 512, 64, 64
@@ -42,10 +43,6 @@ SCALE = 1.0 / math.sqrt(192)
 CASES = ([("decode", H, B, S - 1, 1) for H in (8, 16, 128) for B in (1, 16, 64) for S in (4096, 16384)]
          + [("verify", H, 16, 4096, sq) for H in (16, 128) for sq in (2, 4)]
          + [("chunk", 16, 1, 4096, sq) for sq in (512, 2048)])
-
-
-def quant(x):
-    return x.float().clamp(-448.0, 448.0).to(E4M3)
 
 
 def make_inputs(H, B, prefix, sq, seed):
@@ -76,16 +73,6 @@ def reference(qn, qp, kc, kv, prefix, bt):
         p = torch.softmax(s.masked_fill(~mask, float("-inf")), dim=-1)
         out[b] = torch.einsum("hij,jd->ihd", p, rows[:, :C])
     return out
-
-
-def alternate(fns, reps, windows):
-    for fn in fns:
-        time_ms(fn, 3, 1, 1)
-    ts = [[] for _ in fns]
-    for _ in range(windows):
-        for i, fn in enumerate(fns):
-            ts[i] += time_ms(fn, 0, reps, 1)
-    return [spread(t) for t in ts]
 
 
 def attention_cases(args):

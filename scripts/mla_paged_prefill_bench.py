@@ -23,15 +23,16 @@ import argparse
 import json
 import math
 import os
-import subprocess
 import sys
 
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "scripts"))
 
 from chitu_b200.attn_backend import B200AttnBackend  # noqa: E402
+from paged_prefill_bench import gpu_info, max_rel, spread, time_ms  # noqa: E402
 
 C, R, PAGE = 512, 64, 64
 ROW = C + R
@@ -40,44 +41,6 @@ DATASHEET_TB_S = 3.35
 CASES = ([("mtp", H, B, prefix, sq) for H in (8, 16, 128) for sq in (2, 4) for B in (1, 16, 64)
           for prefix in (1024, 4096, 16384)]
          + [("chunk", H, 1, 4096, sq) for H in (8, 16, 128) for sq in (512, 2048)])
-
-
-def time_ms(fn, warmup, reps, windows):
-    """Mean ms per call in each of `windows` CUDA-event windows of `reps` calls, after `warmup` calls."""
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    res = []
-    for _ in range(windows):
-        start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        start.record()
-        for _ in range(reps):
-            fn()
-        end.record()
-        torch.cuda.synchronize()
-        res.append(start.elapsed_time(end) / reps)
-    return res
-
-
-def spread(ts):
-    ts = sorted(ts)
-    return {"median": ts[len(ts) // 2], "min": ts[0], "max": ts[-1]}
-
-
-def gpu_info():
-    info = {"device": torch.cuda.get_device_name()}
-    try:
-        r = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv"],
-                           capture_output=True, text=True, timeout=30)
-        info["nvidia_smi"] = r.stdout.strip()
-    except (OSError, subprocess.SubprocessError) as e:
-        info["nvidia_smi"] = f"unavailable: {e!r}"
-    return info
-
-
-def max_rel(a, b):
-    a, b = a.double(), b.double()
-    return ((a - b).abs().max() / b.abs().max().clamp(min=1e-30)).item()
 
 
 def make_inputs(H, B, prefix, sq, seed):

@@ -15,15 +15,16 @@ import argparse
 import json
 import math
 import os
-import subprocess
 import sys
 
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "scripts"))
 
 from chitu_b200.attn_backend import B200AttnBackend  # noqa: E402
+from paged_prefill_bench import gpu_info  # noqa: E402
 
 QK, DV = 576, 512
 DATASHEET_BF16_TFLOPS = 989.0
@@ -56,17 +57,6 @@ def time_ms(fn, warmup, reps):
     end.record()
     torch.cuda.synchronize()
     return start.elapsed_time(end) / reps
-
-
-def gpu_info():
-    info = {"device": torch.cuda.get_device_name()}
-    try:
-        r = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv"],
-                           capture_output=True, text=True, timeout=30)
-        info["nvidia_smi"] = r.stdout.strip()
-    except (OSError, subprocess.SubprocessError) as e:
-        info["nvidia_smi"] = f"unavailable: {e!r}"
-    return info
 
 
 def main():
