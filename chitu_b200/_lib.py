@@ -55,6 +55,8 @@ SIGNATURES = {
     "chitu_b200_fp8_gemm": (I, [P, P, P, P, P, I, I, I, P, P, L, I, P]),
     "chitu_b200_soft_fp8_gemm": (I, [P, P, P, P, I, I, I, I, P, L, I, P]),
     "chitu_b200_w8a8_gemm": (I, [P, P, P, P, P, P, I, I, I, P, L, I, P]),
+    "chitu_b200_w4a16_gemm": (I, [P, P, P, P, P, P, I, I, I, I, P, L, P]),
+    "chitu_b200_w4a16_gemm_silu_pairs": (I, [P, P, P, P, P, I, I, I, I, P, L, P]),
     "chitu_b200_attn_workspace_bytes": (L, [I, I, I, I]),
     "chitu_b200_gqa_paged_decode": (I, [P, P, P, P, P, L, L, P, P, I, I, I, I, I, I, I, F, P, P, L, I, P]),
     "chitu_b200_gqa_paged_decode_rope": (I, [P, L, P, P, P, P, L, L, P, P, P, P, I, I, I, I, I, I, I, F, P, P, L, I, P]),

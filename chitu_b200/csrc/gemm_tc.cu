@@ -13,7 +13,9 @@
 //   warp 8   : TMA producer — cp.async.bulk.tensor.2d, 128B-swizzled boxes W[128 rows x 128 B] and X[BN rows x 128 B]
 //              into an S-stage shared-memory ring (mbarrier full/empty), weights with an L2 evict-first policy (read
 //              exactly once), activations evict-last.
-//   soft fp8 : 8 more warps convert each fp8 weight stage to bf16 for the bf16 MMA.
+//   soft fp8 : 3 more warps convert each fp8 weight stage to bf16 for the bf16 MMA.
+//   W4       : the same 3 converter warps turn each stage of 4-bit weights (one group of 128 K-elements) into bf16 /
+//              fp16 for the 16-bit MMA.
 // Split-K fills the SMs when N/128 tiles are too few: fp32 (int32) partials go to a workspace, the last CTA of a tile
 // half (atomic ticket) reduces them in split order -> deterministic.
 //
@@ -21,6 +23,7 @@
 //   kind 0: F.linear bf16/fp16 (+bias fp32-joined, +residual as a separate rounding)
 //   kind 1: fp8_gemm_deepseek_v3 (ops.py:452-483, triton_kernels.py:303-365)
 //   kind 2: w8a8gemm.mm / w8a8gemv.mv (quantize/w8a8.py:105,120,125)
+//   kind 4: W4A16, group 128 (GPTQ / AWQ weights after quantize/w4a16.py's repack): w = io((q - z) * s)
 #include <cuda.h>
 
 #include <mutex>
@@ -39,6 +42,7 @@ constexpr int kTileN = 128;        // weight rows per CTA tile (two wgmma M = 64
 constexpr int kStageRowBytes = 128;  // bytes of K per stage row (one 128B swizzle atom)
 constexpr int kMmaThreads = 256;   // two consumer warpgroups; the producer warp and the converter warps follow
 constexpr int kGeomCache = 256;   // grouped mode: tiles whose geometry a CTA stages in shared memory
+constexpr int kW4RowBytes = 64;    // W4: bytes of one weight row per stage (one group of 128 4-bit elements)
 
 __device__ __forceinline__ uint64_t make_kmajor_sw128_desc(uint32_t smem_addr) { return make_sw128_desc(smem_addr, 16, 1024); }
 
@@ -78,23 +82,29 @@ struct Params {
   const float* g_row_scale; // [rows] routed weight per sorted row (GEMM2, fused_moe.py:290-292) or null
   const int* g_out_rows;    // [rows] output row of sorted row r (the reference writes C.view(-1,N)[sorted_ids[r]],
                             // fused_moe.py:296-306), negative = padding row: nothing is written; null = r itself
+  // ---- W4 (KIND_W4): one scale and one zero per weight row and group of 128 K-elements (kblocks groups per row) ----
+  const uint16_t* w4_s;     // [N, kblocks] io dtype bits
+  const uint8_t* w4_z;      // [N, kblocks] 0..15
 };
 
 template <int KIND, int BN>
 struct Cfg {
   static constexpr bool kSoft = KIND == KIND_SOFT;
-  static constexpr int kStageW = kTileN * kStageRowBytes;                     // 16 KB
-  // soft fp8: a stage is 128 K-elements = 128 B of fp8 weights per row but 256 B of bf16 activations (two swizzle atoms)
-  static constexpr int kStageX = BN * kStageRowBytes * (kSoft ? 2 : 1);
+  static constexpr bool kW4 = KIND == KIND_W4;
+  static constexpr bool kCvt = kSoft || kW4;      // weights converted in shared memory before a 16-bit MMA
+  // 16 KB; W4: 8 KB, one group of 128 K-elements ([128 rows x 64 B], unswizzled)
+  static constexpr int kStageW = kTileN * (kW4 ? kW4RowBytes : kStageRowBytes);
+  // soft fp8 / W4: a stage is 128 K-elements but 256 B of 16-bit activations per token (two swizzle atoms)
+  static constexpr int kStageX = BN * kStageRowBytes * (kCvt ? 2 : 1);
   static constexpr int kStageBytes = kStageW + kStageX;
-  // soft fp8: ring of converted (bf16) weight tiles, [2 atoms][128 rows][128 B] each, between the converter warps and
-  // the MMA warpgroups
-  static constexpr int kCvtStages = kSoft ? 3 : 0;
+  // soft fp8 / W4: ring of converted (16-bit) weight tiles, [2 atoms][128 rows][128 B] each, between the converter warps
+  // and the MMA warpgroups
+  static constexpr int kCvtStages = kCvt ? 3 : 0;
   static constexpr int kCvtBytes = 2 * kTileN * kStageRowBytes;               // 32 KB
   // 3 converter warps: with the producer warp they fill a third warpgroup, so the block stays at 384 threads (registers
   // are budgeted per 128 threads; more converter threads would cut every consumer thread to 128 registers)
-  static constexpr int kCvtThreads = kSoft ? 96 : 0;
-  static constexpr int kCvtRing = kSoft ? kCvtStages : 1;                     // modulus of the converter ring
+  static constexpr int kCvtThreads = kCvt ? 96 : 0;
+  static constexpr int kCvtRing = kCvt ? kCvtStages : 1;                      // modulus of the converter ring
   // one CTA per SM with the deepest ring that fits
   static constexpr int kBudget = 200 * 1024 - kCvtStages * kCvtBytes;
   static constexpr int kStages = (kBudget / kStageBytes) > 10 ? 10 : (kBudget / kStageBytes);
@@ -134,7 +144,7 @@ struct ItemIter {
 enum { EPI_PLAIN = 0, EPI_PAIRS = 1, EPI_PUSH = 2, EPI_ROWS = 3 };   // ROWS: Params::g_out_rows (grouped mode only)
 
 // one 128 B K slice of a stage: D[64 weight rows x BN tokens] (+)= W[64 x K] . X[BN x K]^T
-// (KIND_16 multiplies fp16 operands when `f16`, bf16 otherwise)
+// (KIND_16 and KIND_W4 multiply fp16 operands when `f16`, bf16 otherwise)
 template <int KIND, int BN, typename Acc>
 __device__ __forceinline__ void mma_k(Acc (&d)[BN / 2], uint64_t a, uint64_t b, int accumulate, bool f16) {
   if constexpr (KIND == KIND_FP8) WgmmaN<BN>::e4m3(d, a, b, accumulate);
@@ -159,7 +169,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
   uint8_t* smem_x = smem + C::kStages * C::kStageW;
   uint8_t* smem_c = smem_x + C::kStages * C::kStageX;          // soft fp8: converted weight tiles
   __shared__ __align__(8) uint64_t full_bar[C::kStages], empty_bar[C::kStages];
-  __shared__ __align__(8) uint64_t cvt_full[C::kSoft ? C::kCvtStages : 1], cvt_empty[C::kSoft ? C::kCvtStages : 1];
+  __shared__ __align__(8) uint64_t cvt_full[C::kCvt ? C::kCvtStages : 1], cvt_empty[C::kCvt ? C::kCvtStages : 1];
   __shared__ int s_is_last[2];
   __shared__ int4 s_geom[kGeomCache];             // grouped mode: {wrow, xrow, cnt, out col} of this CTA's first tiles
 
@@ -181,6 +191,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
   const int g_begin = min((int)blockIdx.x * per, total);
   const int g_end = min(g_begin + per, total);
   constexpr int kElemsPerStage = KIND == KIND_16 ? 64 : 128;   // K elements per pipeline stage
+  constexpr int kWColsPerStage = C::kW4 ? kW4RowBytes : kElemsPerStage;   // weight TMA columns per stage (W4: bytes)
   // grouped mode: the tile geometry lives in device memory; reading it per tile puts an L2 round trip in front of every
   // tile of the producer and of the epilogue (the K = 256 down projection's tiles are only two stages long).  Stage this
   // CTA's share once.
@@ -199,7 +210,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < C::kStages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 2); }
-    if (C::kSoft)
+    if (C::kCvt)
       for (int i = 0; i < C::kCvtStages; ++i) { mbar_init(&cvt_full[i], 1); mbar_init(&cvt_empty[i], 2); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
@@ -225,7 +236,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
           const int n0 = (w.tile % p.n_tiles) * kTileN;
           for (int st = w.s_lo; st < w.s_hi && it < C::kStages; ++st, ++it) {
             mbar_expect_tx_only(&full_bar[it], C::kStageW);        // first ring pass: every slot is free
-            tma_load_2d(smem_w + it * C::kStageW, &map_w, &full_bar[it], st * kElemsPerStage, n0, pol_w);
+            tma_load_2d(smem_w + it * C::kStageW, &map_w, &full_bar[it], st * kWColsPerStage, n0, pol_w);
           }
         }
         pre = it;
@@ -246,11 +257,92 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
           } else {
             mbar_wait(&empty_bar[s], ph ^ 1);
             mbar_expect_tx(&full_bar[s], C::kStageBytes);
-            tma_load_2d(smem_w + s * C::kStageW, &map_w, &full_bar[s], kc, n0, pol_w);
+            tma_load_2d(smem_w + s * C::kStageW, &map_w, &full_bar[s], st * kWColsPerStage, n0, pol_w);
           }
           tma_load_2d(smem_x + s * C::kStageX, &map_x, &full_bar[s], kc, m0, pol_x);
-          if (C::kSoft)   // second 64-element atom of the bf16 activations
+          if (C::kCvt)    // second 64-element atom of the 16-bit activations
             tma_load_2d(smem_x + s * C::kStageX + BN * kStageRowBytes, &map_x, &full_bar[s], kc + 64, m0, pol_x);
+        }
+      }
+    }
+  } else if (C::kW4 && warp >= C::kCvtWarp0) {
+    // ================= W4: weight converter (3 warps) =================
+    if constexpr (C::kW4) {   // (the branch is compiled for every kind)
+      // w = io((q - z) * s) with one rounding: the nibble q ORed into the mantissa of an io value of magnitude 2^7 (bf16)
+      // or 2^10 (fp16) is that magnitude plus q exactly, subtracting the magnitude plus z leaves q - z exactly, and one
+      // packed multiply by s rounds once.  The stage's [128 rows x 64 B] packed tile (unswizzled; element k of a row in
+      // byte k / 2, low nibble for even k) is 512 units of 16 B = 32 elements of one row, each written as four 16 B chunks
+      // of the row's 128B-swizzled atom (unit u of a row: atom u / 2, chunks 4 (u % 2) .. + 3).  The scale and zero of
+      // the thread's rows are weights too: fetched one stage ahead, each read once per tile (L2 serves the re-reads).
+      const int ct = threadIdx.x - C::kCvtWarp0 * 32;            // 0..95
+      constexpr int kUnits = kTileN * kW4RowBytes / 16;             // 512
+      constexpr int kPer = (kUnits + C::kCvtThreads - 1) / C::kCvtThreads;
+      const bool f16 = p.out_dtype == CB_F16;
+      const uint32_t magic = f16 ? 0x6400u : 0x4300u;              // 1024 (fp16), 128 (bf16): one unit per mantissa step
+      // per unit of the thread: the pairs (s, s) and (magic + z, magic + z) of this stage and of the next
+      uint32_t s2[kPer], mz2[kPer], s2n[kPer], mz2n[kPer];
+      auto fetch = [&](int w_row0, int st) {
+#pragma unroll
+        for (int i = 0; i < kPer; ++i) {
+          const int unit = ct + i * C::kCvtThreads;
+          if (unit >= kUnits) break;
+          const int64_t o = (int64_t)min(w_row0 + (unit >> 2), p.N - 1) * p.kblocks + st;   // rows past N: any finite
+          const uint32_t sv = p.w4_s[o], zv = magic + p.w4_z[o];
+          s2n[i] = sv | (sv << 16);
+          mz2n[i] = zv | (zv << 16);
+        }
+      };
+      auto convert = [&](const uint8_t* src, uint8_t* dst, auto io_tag) {
+        constexpr bool kF16 = std::is_same<decltype(io_tag), __half>::value;
+#pragma unroll
+        for (int i = 0; i < kPer; ++i) {
+          const int unit = ct + i * C::kCvtThreads;
+          if (unit >= kUnits) break;
+          const int r = unit >> 2, u = unit & 3;
+          const uint4 v = *reinterpret_cast<const uint4*>(src + unit * 16);
+          const uint32_t vw[4] = {v.x, v.y, v.z, v.w};
+          uint8_t* drow = dst + (u >> 1) * (kTileN * kStageRowBytes) + r * 128;
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {               // 8 elements: bytes b of vw[q] hold elements 2b (low) and 2b + 1
+            const uint32_t hi4 = vw[q] >> 4;
+            uint32_t o[4];
+#pragma unroll
+            for (int b = 0; b < 4; ++b) {
+              // (magic + q) for elements 2b (low half) and 2b + 1 (high half)
+              const uint32_t t = (__byte_perm(vw[q], hi4, b | ((4 + b) << 8)) & 0x000f000fu) | (magic * 0x10001u);
+              uint32_t d;
+              if constexpr (kF16) {
+                asm("sub.rn.f16x2 %0, %1, %2;" : "=r"(d) : "r"(t), "r"(mz2[i]));
+                asm("mul.rn.f16x2 %0, %1, %2;" : "=r"(o[b]) : "r"(d), "r"(s2[i]));
+              } else {
+                asm("sub.rn.bf16x2 %0, %1, %2;" : "=r"(d) : "r"(t), "r"(mz2[i]));
+                asm("mul.rn.bf16x2 %0, %1, %2;" : "=r"(o[b]) : "r"(d), "r"(s2[i]));
+              }
+            }
+            const int c = 4 * (u & 1) + q;
+            *reinterpret_cast<uint4*>(drow + ((c ^ (r & 7)) << 4)) = make_uint4(o[0], o[1], o[2], o[3]);
+          }
+        }
+      };
+      int it = 0;
+      for (ItemIter ii(g_begin, g_end, S); ii.valid(); ii.next()) {
+        const WorkItem w = ii.item();
+        const int w_row0 = (w.tile % p.n_tiles) * kTileN;
+        fetch(w_row0, w.s_lo);
+        for (int st = w.s_lo; st < w.s_hi; ++st, ++it) {
+          const int s = it % C::kStages, c = it % C::kCvtRing;
+#pragma unroll
+          for (int i = 0; i < kPer; ++i) { s2[i] = s2n[i]; mz2[i] = mz2n[i]; }
+          if (st + 1 < w.s_hi) fetch(w_row0, st + 1);
+          mbar_wait(&full_bar[s], (it / C::kStages) & 1);
+          mbar_wait(&cvt_empty[c], ((it / C::kCvtRing) & 1) ^ 1);
+          const uint8_t* src = smem_w + s * C::kStageW;
+          uint8_t* dst = smem_c + c * C::kCvtBytes;
+          if (f16) convert(src, dst, __half{});
+          else convert(src, dst, __nv_bfloat16{});
+          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+          asm volatile("bar.sync 5, %0;" ::"n"(C::kCvtThreads) : "memory");
+          if (ct == 0) mbar_arrive(&cvt_full[c]);
         }
       }
     }
@@ -305,7 +397,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
     const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);     // tile rows r0 and r0 + 8 (wgmma fragment rows)
     const int cl = 2 * (lane & 3);                               // token columns 8 nb + cl + {0, 1}
     const bool signal = (threadIdx.x & 127) == 0;                // arrives on the ring barriers for its warpgroup
-    const bool f16 = KIND == KIND_16 && p.out_dtype == CB_F16;
+    const bool f16 = (KIND == KIND_16 || KIND == KIND_W4) && p.out_dtype == CB_F16;
     auto row_of = [&](int e) { return r0 + 8 * ((e >> 1) & 1); };
     auto col_of = [&](int e) { return 8 * (e >> 2) + cl + (e & 1); };
 
@@ -406,8 +498,8 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
         mbar_wait(&full_bar[s], (it / C::kStages) & 1);
         const int first = KIND == KIND_FP8 || st == w.s_lo;     // fp8: a fresh accumulator per K block
         wgmma_fence();
-        if constexpr (C::kSoft) {
-          // A = the bf16 tile the converter warps produced from this stage's fp8 weights (two 64-element atoms)
+        if constexpr (C::kCvt) {
+          // A = the 16-bit tile the converter warps produced from this stage's fp8 / 4-bit weights (two 64-element atoms)
           const int c = it % C::kCvtRing;
           mbar_wait(&cvt_full[c], (it / C::kCvtRing) & 1);
           const uint32_t a0 = smem_u32(smem_c + c * C::kCvtBytes) + wg * 64 * kStageRowBytes;
@@ -460,7 +552,13 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
         for (int e = 0; e < NR; ++e) {
           const float other = __shfl_xor_sync(0xffffffffu, v[e], 4);
           const int n = ge.ocol0 + row_of(e), j = col_of(e);
-          if (n_ok(e) && ((lane >> 2) & 1) == 0 && j < cnt) {
+          if (KIND == KIND_W4 && p.out_dtype == CB_F16) {          // the same roundings in fp16
+            if (n_ok(e) && ((lane >> 2) & 1) == 0 && j < cnt) {
+              const float g = __half2float(__float2half_rn(v[e])), u = __half2float(__float2half_rn(other));
+              const float sl = __half2float(__float2half_rn(g / (1.f + expf(-g))));
+              reinterpret_cast<__half*>(p.out)[(int64_t)(m0 + j) * (ld >> 1) + (n >> 1)] = __float2half_rn(sl * u);
+            }
+          } else if (n_ok(e) && ((lane >> 2) & 1) == 0 && j < cnt) {
             const float g = __bfloat162float(__float2bfloat16_rn(v[e])), u = __bfloat162float(__float2bfloat16_rn(other));
             const float sl = __bfloat162float(__float2bfloat16_rn(g / (1.f + expf(-g))));
             reinterpret_cast<__nv_bfloat16*>(p.out)[(int64_t)(m0 + j) * (ld >> 1) + (n >> 1)] = __float2bfloat16_rn(sl * u);
@@ -610,13 +708,16 @@ int make_tma_map_nd(CUtensorMap* map, const void* base, int rank, const cuuint64
 namespace {
 
 // The operands of a kind: bytes and TMA type of a weight and of an activation element.  KIND_16's follow the io dtype
-// (CB_BF16, else fp16); soft fp8 multiplies bf16 activations.
+// (CB_BF16, else fp16); soft fp8 multiplies bf16 activations; W4 weights are bytes of two 4-bit elements (w_elem counts
+// the one byte of the TMA map per K-element pair as a whole element: S = K / 128 either way) and its activations
+// follow the io dtype.
 struct Operands { int w_elem; CUtensorMapDataType w_dt; int x_elem; CUtensorMapDataType x_dt; };
 Operands operands(int kind, int dtype) {
   const CUtensorMapDataType u8 = CU_TENSOR_MAP_DATA_TYPE_UINT8, bf16 = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
   const CUtensorMapDataType io = dtype == CB_BF16 ? bf16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
   if (kind == KIND_16) return {2, io, 2, io};
   if (kind == KIND_SOFT) return {1, u8, 2, bf16};
+  if (kind == KIND_W4) return {1, u8, 2, io};
   return {1, u8, 1, u8};                              // fp8, int8
 }
 
@@ -654,16 +755,16 @@ int launch_epi(const CUtensorMap& mw, const CUtensorMap& mx, Params& p, int grid
 template <int KIND, int BN>
 int launch(const CUtensorMap& mw, const CUtensorMap& mx, Params& p, int grid, cudaStream_t st) {
   if (p.act_pairs) {
-    if constexpr (KIND == KIND_16) return launch_epi<KIND, BN, EPI_PAIRS>(mw, mx, p, grid, st);
-    else return fail(-2, "tc gemm: the SiluAndMul epilogue is built for bf16 weights only");
+    if constexpr (KIND == KIND_16 || KIND == KIND_W4) return launch_epi<KIND, BN, EPI_PAIRS>(mw, mx, p, grid, st);
+    else return fail(-2, "tc gemm: the SiluAndMul epilogue is built for bf16 and 4-bit weights only");
   }
   if (p.has_push) {
     if constexpr (KIND == KIND_16 || KIND == KIND_FP8) return launch_epi<KIND, BN, EPI_PUSH>(mw, mx, p, grid, st);
     else return fail(-2, "tc gemm: the push epilogue is built for bf16 and fp8 weights only");
   }
   if (p.g_out_rows) {
-    if constexpr (KIND != KIND_I8) return launch_epi<KIND, BN, EPI_ROWS>(mw, mx, p, grid, st);
-    else return fail(-2, "tc gemm: output-row indirection is not built for int8");
+    if constexpr (KIND != KIND_I8 && KIND != KIND_W4) return launch_epi<KIND, BN, EPI_ROWS>(mw, mx, p, grid, st);
+    else return fail(-2, "tc gemm: output-row indirection is not built for int8 or 4-bit weights");
   }
   return launch_epi<KIND, BN, EPI_PLAIN>(mw, mx, p, grid, st);
 }
@@ -683,13 +784,16 @@ int launch_kind(int kind, const void* x, int64_t x_rows, const void* w, int64_t 
                 cudaStream_t st) {
   const Operands op = operands(kind, p.out_dtype);
   CUtensorMap mw, mx;
-  int rc = make_tma_map_2d(&mw, w, w_rows, p.K, op.w_elem, op.w_dt, kTileN);
+  // W4: [w_rows, K / 2] bytes, one group (64 B) per box row, unswizzled
+  int rc = kind == KIND_W4 ? make_tma_map_2d(&mw, w, w_rows, p.K / 2, 1, op.w_dt, kTileN, 0, kW4RowBytes)
+                           : make_tma_map_2d(&mw, w, w_rows, p.K, op.w_elem, op.w_dt, kTileN);
   if (rc) return rc;
   rc = make_tma_map_2d(&mx, x, x_rows, p.K, op.x_elem, op.x_dt, BN);
   if (rc) return rc;
   if (kind == KIND_16) return dispatch_bn<KIND_16>(BN, mw, mx, p, grid, st);
   if (kind == KIND_FP8) return dispatch_bn<KIND_FP8>(BN, mw, mx, p, grid, st);
   if (kind == KIND_SOFT) return dispatch_bn<KIND_SOFT>(BN, mw, mx, p, grid, st);
+  if (kind == KIND_W4) return dispatch_bn<KIND_W4>(BN, mw, mx, p, grid, st);
   return dispatch_bn<KIND_I8>(BN, mw, mx, p, grid, st);
 }
 
@@ -738,7 +842,8 @@ int64_t tc_max_tiles() { return kMaxTickets; }
 bool tc_supported(int kind, int M, int N, int K) {
   if (M < 1 || N < 1 || K < 1) return false;
   if (((int64_t)K * operands(kind, CB_BF16).w_elem) % 16 != 0) return false;   // TMA row pitch
-  if ((kind == KIND_FP8 || kind == KIND_SOFT) && K % 128 != 0) return false;   // one scale block per pipeline stage
+  // one scale block (W4: one group of scales and zeros) per pipeline stage
+  if ((kind == KIND_FP8 || kind == KIND_SOFT || kind == KIND_W4) && K % 128 != 0) return false;
   return tma_available();
 }
 
@@ -804,6 +909,17 @@ int tc_soft_fp8_gemm(const void* a, const void* b, const float* b_s, void* c, in
   p.M = M; p.N = N; p.K = K;
   p.out_dtype = CB_BF16; p.b_s = b_s; p.out = c;
   return run(KIND_SOFT, a, b, p, ws, ws_bytes, st);
+}
+
+// W4A16, group 128: y[M, N] = x . W^T (+residual) with W[n, k] = io((q[n, k] - zeros[n, k/128]) * scales[n, k/128]),
+// q = nibble k % 2 of qweight[n, k / 2]; pairs: y[M, N/2] = SiluAndMul of the interleaved gate / up rows
+int tc_w4a16(const void* x, const void* qweight, const void* scales, const uint8_t* zeros, const void* residual, void* y,
+             int M, int N, int K, int dtype, bool pairs, void* ws, int64_t ws_bytes, cudaStream_t st) {
+  Params p{};
+  p.M = M; p.N = N; p.K = K;
+  p.out_dtype = dtype; p.residual = residual; p.out = y; p.act_pairs = pairs ? 1 : 0;
+  p.w4_s = (const uint16_t*)scales; p.w4_z = zeros;
+  return run(KIND_W4, x, qweight, p, ws, ws_bytes, st);
 }
 
 int tc_w8a8_gemm(void* out, const int8_t* a, const int8_t* b, const float* a_scales, const float* b_scales,

@@ -101,4 +101,36 @@ extern "C" int chitu_b200_w8a8_gemm(void* out, const int8_t* a, const int8_t* b,
   return path == kSimt ? simt_w8a8_gemm(out, a, b, a_scales, b_scales, bias, M, N, K, st) : path;
 }
 
+// W4A16, group 128 (GPTQ / AWQ after quantize/w4a16.py's repack): the 4-bit weight tile is turned into bf16 / fp16 in
+// shared memory between the TMA landing and the 16-bit MMA.  wgmma only; refusals name the entry and launch nothing.
+static int w4a16(const char* entry, const void* x, const void* qweight, const void* scales, const uint8_t* zeros,
+                 const void* residual, void* y, int M, int N, int K, int dtype, bool pairs, void* workspace,
+                 int64_t workspace_bytes, void* stream) {
+  CB_ARG_AS(entry, x && qweight && scales && zeros && y && M >= 0 && N > 0 && K > 0);
+  CB_ARG_AS(entry, ((uintptr_t)x | (uintptr_t)qweight | (uintptr_t)scales | (uintptr_t)zeros | (uintptr_t)residual |
+                    (uintptr_t)y) % 16 == 0);
+  CB_ARG_AS(entry, K % 128 == 0);
+  CB_ARG_AS(entry, dtype == CB_BF16 || dtype == CB_F16);
+  CB_ARG_AS(entry, !pairs || N % 2 == 0);
+  if (M == 0) return 0;
+  const int path = linear_path(entry, KIND_W4, 2, dtype, M, N, K, workspace, workspace_bytes);
+  if (path != kWgmma) return path;
+  return tc_w4a16(x, qweight, scales, zeros, residual, y, M, N, K, dtype, pairs, workspace, workspace_bytes,
+                  (cudaStream_t)stream);
+}
+
+extern "C" int chitu_b200_w4a16_gemm(const void* x, const void* qweight, const void* scales, const uint8_t* zeros,
+                                     const void* residual, void* y, int M, int N, int K, int dtype, void* workspace,
+                                     int64_t workspace_bytes, void* stream) {
+  return w4a16(__func__, x, qweight, scales, zeros, residual, y, M, N, K, dtype, false, workspace, workspace_bytes,
+               stream);
+}
+
+extern "C" int chitu_b200_w4a16_gemm_silu_pairs(const void* x, const void* qweight, const void* scales,
+                                                const uint8_t* zeros, void* y, int M, int N, int K, int dtype,
+                                                void* workspace, int64_t workspace_bytes, void* stream) {
+  return w4a16(__func__, x, qweight, scales, zeros, nullptr, y, M, N, K, dtype, true, workspace, workspace_bytes,
+               stream);
+}
+
 CB_DEFINE_TL_SETTER(linear)

@@ -241,12 +241,26 @@ class LlamaDecodeEngine(DecodeEngine):
     serve_config.yaml:9).  KV cache layout = PagedKVCacheManager (cache_manager.py:71-87):
     paged_k_cache / paged_v_cache [L, num_blocks, page, n_local_kv_heads, head_dim], page 256
     (backend.py:237).  kv_dtype=torch.float8_e4m3fn keeps the caches in e4m3 (half the KV bytes; new rows rounded
-    to nearest even after a clamp to +-448, no scale) and decodes through chitu_b200_gqa_paged_attn_fp8kv."""
+    to nearest even after a clamp to +-448, no scale) and decodes through chitu_b200_gqa_paged_attn_fp8kv.
+
+    weight_format="w4a16" holds qkv, o, w13 and w2 as 4-bit groups of 128 (quantize/w4a16.py's round-to-nearest rule
+    applied to the same synthetic weights) and runs them through chitu_b200_w4a16_gemm[_silu_pairs]; embedding, head,
+    norms, rotary and attention stay bf16.  The W4 GEMM has no push epilogue, so it runs on one GPU or in shard mode."""
+
+    W4_LINEARS = ("wqkv", "wo", "w13", "w2")
 
     def __init__(self, cfg: LlamaConfig, max_reqs: int, max_seq_len: int, device="cuda:0", page_size: int = 256,
                  seed: int = 0, tp_rank: int = 0, tp_size: int = 1, process_group=None, linear_impl: int = 0,
-                 use_fused_allreduce: bool = True, kv_dtype: torch.dtype = BF):
+                 use_fused_allreduce: bool = True, kv_dtype: torch.dtype = BF, weight_format: str = "bf16"):
         D = cfg.head_dim
+        if weight_format not in ("bf16", "w4a16"):
+            raise ValueError(f"weight_format must be 'bf16' or 'w4a16', not {weight_format!r}")
+        if weight_format == "w4a16" and process_group is not None and tp_size > 1:
+            raise ValueError("weight_format='w4a16' runs on one GPU or one shard: the 4-bit GEMM has no push epilogue "
+                             "for the tensor-parallel all-reduce")
+        if weight_format == "w4a16" and linear_impl == 1:
+            raise ValueError("weight_format='w4a16' runs on the wgmma GEMM only (linear_impl=1 selects the SIMT GEMV)")
+        self.weight_format = weight_format
         assert cfg.n_heads % tp_size == 0 and cfg.n_kv_heads % tp_size == 0
         self.Hq, self.Hkv, self.D = cfg.n_heads // tp_size, cfg.n_kv_heads // tp_size, D
         self.F = cfg.ffn_dim // tp_size
@@ -298,6 +312,12 @@ class LlamaDecodeEngine(DecodeEngine):
         if self.fuse_silu:
             for lw in self.layers:
                 lw["w13"] = lw["w13"].view(2, self.F, dim).transpose(0, 1).reshape(2 * self.F, dim).contiguous()
+        if weight_format == "w4a16":
+            # per-row quantisation: w13's interleaved rows carry their own scales and zeros
+            from .quantize.w4a16 import quantize_rtn
+            for lw in self.layers:
+                for name in self.W4_LINEARS:
+                    lw[name] = quantize_rtn(lw[name], BF)
         # rotary fused into the tensor-core decode kernel (head dim 128, power-of-two pages)
         self.fuse_rope = D == 128 and (page_size & (page_size - 1)) == 0 and self.Hq // self.Hkv in (1, 2, 4, 8)
         if self.kv_fp8 and not (self.fuse_rope and page_size % 64 == 0):
@@ -306,13 +326,25 @@ class LlamaDecodeEngine(DecodeEngine):
 
     def ref_layers(self):
         """The layer weights in the REFERENCE's layout (w13 = [w1 ; w3] halves) for the oracle side of the tests."""
+        from .quantize.w4a16 import dequantize
         out = []
         for lw in self.layers:
             d = dict(lw)
+            if self.weight_format == "w4a16":
+                d.update({name: dequantize(*lw[name]) for name in self.W4_LINEARS})
             if self.fuse_silu:
-                d["w13"] = lw["w13"].view(self.F, 2, self.cfg.dim).transpose(0, 1).reshape(2 * self.F, self.cfg.dim).contiguous()
+                d["w13"] = d["w13"].view(self.F, 2, self.cfg.dim).transpose(0, 1).reshape(2 * self.F, self.cfg.dim).contiguous()
             out.append(d)
         return out
+
+    def _layer_linear(self, x, lw, name, y, M, residual=None):
+        """y = x . lw[name]^T (+ residual) in the engine's weight format."""
+        if self.weight_format == "bf16":
+            return self._linear(x, lw[name], y, M, residual=residual)
+        q, s, z = lw[name]
+        check(self.lib.chitu_b200_w4a16_gemm(ptr(x), ptr(q), ptr(s), ptr(z), ptr(residual), ptr(y), M, q.shape[0],
+                                             2 * q.shape[1], _lib.CB_BF16, ptr(self.lin_ws), self.lin_ws.numel(),
+                                             current_stream()), f"w4a16 {name}")
 
     def _decode_layers(self):
         lib, B, D = self.lib, self.B, self.D
@@ -325,7 +357,7 @@ class LlamaDecodeEngine(DecodeEngine):
             if self.capture_h is not None:
                 self.capture_h.append(h.clone())
             next_norm = self.layers[li + 1]["attn_norm"] if li + 1 < n_layers else self.norm
-            self._linear(self.xn, lw["wqkv"], self.qkv, B)
+            self._layer_linear(self.xn, lw, "wqkv", self.qkv, B)
             q_view, k_view = self.qkv, self.qkv[:, self.Hq * D:]
             v_view = self.qkv[:, (self.Hq + self.Hkv) * D:]
             if self.kv_fp8:
@@ -352,10 +384,15 @@ class LlamaDecodeEngine(DecodeEngine):
                     self.Hkv, D, self.page, self.max_seq_len, 1.0 / math.sqrt(D), ptr(self.attn_out), ptr(self.attn_ws),
                     self.attn_ws.numel(), _lib.CB_BF16, st), "gqa_paged_decode")
             # h2 = wo(o) + h
-            self._row_parallel(lambda out, res: self._linear(self.attn_out, lw["wo"], out, B, residual=res),
+            self._row_parallel(lambda out, res: self._layer_linear(self.attn_out, lw, "wo", out, B, residual=res),
                                lambda: self.comm.linear_push(self.attn_out, lw["wo"], B, self.lin_ws),
                                h, h2, lw["ffn_norm"], y=self.xn)
-            if self.fuse_silu:
+            if self.weight_format == "w4a16":
+                q, s, z = lw["w13"]
+                check(lib.chitu_b200_w4a16_gemm_silu_pairs(ptr(self.xn), ptr(q), ptr(s), ptr(z), ptr(self.act), B,
+                                                           2 * self.F, self.cfg.dim, _lib.CB_BF16, ptr(self.lin_ws),
+                                                           self.lin_ws.numel(), st), "w4a16 w13 + silu")
+            elif self.fuse_silu:
                 check(lib.chitu_b200_linear_bf16_silu_pairs(ptr(self.xn), ptr(lw["w13"]), ptr(self.act), B, 2 * self.F,
                                                             self.cfg.dim, ptr(self.lin_ws), self.lin_ws.numel(), st),
                       "w13 + silu")
@@ -363,7 +400,7 @@ class LlamaDecodeEngine(DecodeEngine):
                 self._linear(self.xn, lw["w13"], self.gate_up, B)
                 check(lib.chitu_b200_silu_and_mul(ptr(self.gate_up), ptr(self.act), B, self.F, _lib.CB_BF16, st), "silu")
             # h = w2(act) + h2
-            self._row_parallel(lambda out, res: self._linear(self.act, lw["w2"], out, B, residual=res),
+            self._row_parallel(lambda out, res: self._layer_linear(self.act, lw, "w2", out, B, residual=res),
                                lambda: self.comm.linear_push(self.act, lw["w2"], B, self.lin_ws),
                                h2, h, next_norm, y=self.xn)
         if self.capture_h is not None:

@@ -201,6 +201,26 @@ int chitu_b200_w8a8_gemm(void* out, const int8_t* a, const int8_t* b, const floa
                          const float* b_scales, const void* bias, int M, int N, int K,
                          void* workspace, int64_t workspace_bytes, int impl, void* stream);
 
+/* W4A16 with groups of 128 along K (GPTQ / AWQ checkpoints after chitu_b200.quantize.W4A16Linear's repack), for the
+ * weight W[N, K], K % 128 == 0:
+ *   qweight uint8 [N, K/2] row-major: element k of row n in byte k/2, low nibble for even k, high nibble for odd k;
+ *   scales  [N, K/128] in the io dtype;  zeros uint8 [N, K/128], 0..15 (a symmetric checkpoint has zeros = 8).
+ * w[n,k] = io((q[n,k] - zeros[n,k/128]) * scales[n,k/128]) with one rounding (q - z is exact), and y = x w^T with fp32
+ * accumulation, io out; residual [M,N] (or NULL) is added after that rounding, as chitu_b200_linear_bf16 does.
+ * dtype CB_BF16 | CB_F16 for x, scales, residual and y.  wgmma path only: where it cannot run (shape or workspace) the
+ * entries return -2 and launch nothing.  Refused before any launch, under the entry's name: a NULL operand, a base
+ * (residual included) that is not 16-byte aligned, K % 128 != 0, another dtype, an odd N for the pairs entry.  M == 0
+ * launches nothing.  qweight, scales and zeros are weights under the weight contract above. */
+int chitu_b200_w4a16_gemm(const void* x, const void* qweight, const void* scales, const uint8_t* zeros,
+                          const void* residual, void* y, int M, int N, int K, int dtype, void* workspace,
+                          int64_t workspace_bytes, void* stream);
+/* The gate_up linear + SiluAndMul of chitu_b200_linear_bf16_silu_pairs on W4A16 weights: rows 2i / 2i+1 of the [N, K]
+ * weight (with their scales and zeros) are gate_i / up_i; y [M, N/2] in the io dtype with the roundings of the two
+ * separate ops (g, u -> io, silu(g) -> io, product -> io). */
+int chitu_b200_w4a16_gemm_silu_pairs(const void* x, const void* qweight, const void* scales, const uint8_t* zeros,
+                                     void* y, int M, int N, int K, int dtype, void* workspace, int64_t workspace_bytes,
+                                     void* stream);
+
 /* ---- decode attention -------------------------------------------------------------------- */
 /* Workspace sizing for split-KV partials. */
 int64_t chitu_b200_attn_workspace_bytes(int batch, int heads, int head_dim_v, int max_splits);
