@@ -80,6 +80,7 @@ SIGNATURES = {
     "chitu_b200_mla_prep": (I, [P, P, L, P, P, P, P, P, P, P, I, I, I, I, I, I, F, P]),
     "chitu_b200_moe_workspace_bytes": (L, [I, I, I, I, I]),
     "chitu_b200_fused_experts": (I, [P, P, P, P, P, P, I, P, I, I, I, I, I, I, I, P, P, P, L, P]),
+    "chitu_b200_fused_experts_w4a16": (I, [P, P, P, P, P, P, P, P, I, P, I, I, I, I, I, I, P, P, P, L, P]),
     "chitu_b200_moe_grouped_gemm_workspace_bytes": (L, [I, I, I]),
     "chitu_b200_moe_grouped_gemm": (I, [P, P, P, P, P, I, P, P, P, I, I, I, I, I, I, I, I, I, P, L, P]),
     "chitu_b200_comm_create": (I, [I, I, L, P, P]),

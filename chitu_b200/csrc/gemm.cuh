@@ -26,10 +26,10 @@ int tc_w4a16(const void* x, const void* qweight, const void* scales, const uint8
              int M, int N, int K, int dtype, bool pairs, void* ws, int64_t ws_bytes, cudaStream_t st);
 int tc_w8a8_gemm(void* out, const int8_t* a, const int8_t* b, const float* a_scales, const float* b_scales,
                  const void* bias, int M, int N, int K, void* ws, int64_t ws_bytes, cudaStream_t st);
-int tc_grouped_gemm(int kind, const void* xs, const float* a_s, const void* w, const float* b_s, void* out, int rows,
-                    int E, int Ng, int K, int max_tokens_per_expert, const int* g_num_tiles, const int* g_tile_wrow,
-                    const int* g_tile_xrow, const int* g_tile_cnt, const float* row_scale, const int* out_rows, void* ws,
-                    int64_t ws_bytes, cudaStream_t st);
+int tc_grouped_gemm(int kind, const void* xs, const float* a_s, const void* w, const float* b_s, const void* w4_s,
+                    const uint8_t* w4_z, void* out, int rows, int E, int Ng, int K, int max_tokens_per_expert,
+                    const int* g_num_tiles, const int* g_tile_wrow, const int* g_tile_xrow, const int* g_tile_cnt,
+                    const float* row_scale, const int* out_rows, void* ws, int64_t ws_bytes, cudaStream_t st);
 
 // ---- gemv.cu ----
 int simt_linear16(const void* x, const void* w, const void* bias, const void* residual, void* y, int M, int N, int K,

@@ -274,6 +274,9 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
       // byte k / 2, low nibble for even k) is 512 units of 16 B = 32 elements of one row, each written as four 16 B chunks
       // of the row's 128B-swizzled atom (unit u of a row: atom u / 2, chunks 4 (u % 2) .. + 3).  The scale and zero of
       // the thread's rows are weights too: fetched one stage ahead, each read once per tile (L2 serves the re-reads).
+      // A null w4_z means every zero is 8 (symmetric int4).  Rows index the whole weight matrix: dense mode clamps the
+      // rows of a partial last tile to N - 1; in grouped mode p.N is one expert's width Ng and the rows index the stacked
+      // [E*Ng] matrix, which whole tiles (Ng % 128 == 0) never run past.
       const int ct = threadIdx.x - C::kCvtWarp0 * 32;            // 0..95
       constexpr int kUnits = kTileN * kW4RowBytes / 16;             // 512
       constexpr int kPer = (kUnits + C::kCvtThreads - 1) / C::kCvtThreads;
@@ -286,8 +289,9 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
         for (int i = 0; i < kPer; ++i) {
           const int unit = ct + i * C::kCvtThreads;
           if (unit >= kUnits) break;
-          const int64_t o = (int64_t)min(w_row0 + (unit >> 2), p.N - 1) * p.kblocks + st;   // rows past N: any finite
-          const uint32_t sv = p.w4_s[o], zv = magic + p.w4_z[o];
+          const int row = w_row0 + (unit >> 2);
+          const int64_t o = (int64_t)(grouped ? row : min(row, p.N - 1)) * p.kblocks + st;   // rows past N: any finite
+          const uint32_t sv = p.w4_s[o], zv = magic + (p.w4_z ? p.w4_z[o] : 8u);
           s2n[i] = sv | (sv << 16);
           mz2n[i] = zv | (zv << 16);
         }
@@ -327,7 +331,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
       int it = 0;
       for (ItemIter ii(g_begin, g_end, S); ii.valid(); ii.next()) {
         const WorkItem w = ii.item();
-        const int w_row0 = (w.tile % p.n_tiles) * kTileN;
+        const int w_row0 = grouped ? geom(w.tile).x : (w.tile % p.n_tiles) * kTileN;
         fetch(w_row0, w.s_lo);
         for (int st = w.s_lo; st < w.s_hi; ++st, ++it) {
           const int s = it % C::kStages, c = it % C::kCvtRing;
@@ -853,23 +857,27 @@ int64_t tc_workspace_bytes(int M, int N) {
 }
 
 // Grouped (MoE experts) GEMM: sorted activations xs [rows, K], stacked weights w [E*Ng, K]; tile list in
-// device memory (see Params).  kind: KIND_16 (bf16 x bf16) or KIND_FP8 (block-scaled, a_s [rows, K/128],
-// b_s [E*Ng/128, K/128]).  max_tokens_per_expert bounds wgmma N.  Output: sorted rows [rows, Ng] bf16.
-int tc_grouped_gemm(int kind, const void* xs, const float* a_s, const void* w, const float* b_s, void* out, int rows,
-                    int E, int Ng, int K, int max_tokens_per_expert, const int* g_num_tiles, const int* g_tile_wrow,
-                    const int* g_tile_xrow, const int* g_tile_cnt, const float* row_scale, const int* out_rows, void* ws,
-                    int64_t ws_bytes, cudaStream_t st) {
+// device memory (see Params).  kind: KIND_16 (bf16 x bf16), KIND_FP8 (block-scaled, a_s [rows, K/128],
+// b_s [E*Ng/128, K/128]), KIND_SOFT (fp8 weights, b_s as fp8, bf16 activations) or KIND_W4 (w uint8 [E*Ng, K/2],
+// w4_s bf16 [E*Ng, K/128], w4_z uint8 [E*Ng, K/128] or null = 8; bf16 activations).  max_tokens_per_expert bounds
+// wgmma N.  Output: sorted rows [rows, Ng] bf16.
+int tc_grouped_gemm(int kind, const void* xs, const float* a_s, const void* w, const float* b_s, const void* w4_s,
+                    const uint8_t* w4_z, void* out, int rows, int E, int Ng, int K, int max_tokens_per_expert,
+                    const int* g_num_tiles, const int* g_tile_wrow, const int* g_tile_xrow, const int* g_tile_cnt,
+                    const float* row_scale, const int* out_rows, void* ws, int64_t ws_bytes, cudaStream_t st) {
   Params p{};
   p.M = rows; p.N = Ng; p.K = K;
   p.S = cdiv((int64_t)K * operands(kind, CB_BF16).w_elem, kStageRowBytes);
   p.kblocks = cdiv(K, 128);
   p.out_dtype = CB_BF16; p.a_s = a_s; p.b_s = b_s; p.out = out;
+  p.w4_s = (const uint16_t*)w4_s; p.w4_z = w4_z;
   p.g_num_tiles = g_num_tiles; p.g_tile_wrow = g_tile_wrow; p.g_tile_xrow = g_tile_xrow; p.g_tile_cnt = g_tile_cnt;
   p.g_ncols = Ng; p.g_row_scale = row_scale; p.g_out_rows = out_rows;
   const int BN = pick_bn(max_tokens_per_expert);      // rows per chunk: the plan cuts larger experts into chunks
   if (max_tokens_per_expert > 128) return fail(-2, "tc_grouped_gemm: more than 128 rows per chunk");
   if (Ng % kTileN != 0) return fail(-2, "tc_grouped_gemm: expert width %d is not a multiple of 128", Ng);
-  if (kind != KIND_16 && K % 128 != 0) return fail(-2, "tc_grouped_gemm: fp8 weights need K %% 128 == 0 (K = %d)", K);
+  if (kind != KIND_16 && K % 128 != 0) return fail(-2, "tc_grouped_gemm: fp8 and 4-bit weights need K %% 128 == 0 (K = %d)", K);
+  if (kind == KIND_W4 && !w4_s) return fail(-2, "tc_grouped_gemm: 4-bit weights need their scales");
   const int grid = num_sms();
   if (!ws || ws_bytes < ws_bytes_for(grid, BN)) return fail(-2, "tc_grouped_gemm: workspace too small");
   p.tickets = (int*)ws;

@@ -844,9 +844,12 @@ struct PairWs : Carve {
   }
 };
 
-// The grouped GEMM kind of a weight mode (0 bf16, 1 fp8 w8a8, 2 fp8 weights x bf16 activations); the pair-GEMV
-// kernel's MODE is the weight mode itself.
-int moe_gemm_kind(int wmode) { return wmode == 1 ? cb::KIND_FP8 : (wmode == 2 ? cb::KIND_SOFT : cb::KIND_16); }
+// The grouped GEMM kind of a weight mode (0 bf16, 1 fp8 w8a8, 2 fp8 weights x bf16 activations, 3 4-bit weights x bf16
+// activations); the pair-GEMV kernel's MODE is the weight mode itself (0..2: 4-bit weights run on the grouped path only).
+constexpr int kWmodeW4 = 3;
+int moe_gemm_kind(int wmode) {
+  return wmode == 1 ? cb::KIND_FP8 : (wmode == 2 ? cb::KIND_SOFT : (wmode == kWmodeW4 ? cb::KIND_W4 : cb::KIND_16));
+}
 
 }  // namespace
 
@@ -1000,7 +1003,7 @@ extern "C" int chitu_b200_moe_grouped_gemm(const void* A, const void* B, void* C
                sorted_token_ids, expert_ids, num_tokens_post_padded, EM, numel, top_k, block_m, E, K, N, quant, ws.xs,
                ws.xs_s, (__nv_bfloat16*)ws.xs, (__nv_bfloat16*)C);
   CB_LAUNCHED(1);
-  return cb::tc_grouped_gemm(moe_gemm_kind(wmode), ws.xs, ws.xs_s, B, B_scale, C, EM, E, N, K, block_m, ws.num_tiles,
+  return cb::tc_grouped_gemm(moe_gemm_kind(wmode), ws.xs, ws.xs_s, B, B_scale, nullptr, nullptr, C, EM, E, N, K, block_m, ws.num_tiles,
                              ws.t_w, ws.t_x, ws.t_c, mul_routed_weight ? ws.row_scale : nullptr, ws.out_rows, workspace,
                              cb::tc_workspace_bytes(128, 128), st);
 }
@@ -1018,20 +1021,32 @@ static int moe_chunk_rows(int64_t P, int E) {
   return BN;
 }
 
+// The 4-bit operands of weight mode 3: bf16 scales and uint8 zeros (null: every zero is 8), [E, N, K / 128] each.
+struct W4Operands {
+  const void *w1_s, *w2_s;
+  const uint8_t *w1_z, *w2_z;
+};
+
+// w1_s / w2_s: the fp8 block scales of weight modes 1 and 2; w4: the scales and zeros of weight mode 3.
 static int fused_experts_impl(const void* x, const void* w1, const void* w2, const float* w1_s,
-                              const float* w2_s, const void* topk_w, int topk_w_dtype,
+                              const float* w2_s, const W4Operands& w4, const void* topk_w, int topk_w_dtype,
                               const void* topk_ids, int ids_dtype, int T, int topk, int E, int N1,
                               int K1, int wmode, void* out, const void* residual, void* workspace,
                               int64_t workspace_bytes, void* stream, void* comm) {
   CB_ARG(x && w1 && w2 && topk_w && topk_ids && (out || comm) && workspace);
   CB_ARG(T >= 0 && topk > 0 && E > 0 && N1 > 0 && N1 % 2 == 0 && K1 > 0);
-  CB_ARG(wmode >= 0 && wmode <= 2);
-  CB_ARG(wmode == 0 || (w1_s && w2_s));
+  CB_ARG(wmode >= 0 && wmode <= kWmodeW4);
+  CB_ARG(wmode == 0 || wmode == kWmodeW4 || (w1_s && w2_s));
+  CB_ARG(wmode != kWmodeW4 || (w4.w1_s && w4.w2_s));
   CB_ARG(topk_w_dtype == CB_BF16 || topk_w_dtype == CB_F32);
   CB_ARG(ids_dtype == CB_I32 || ids_dtype == CB_I64);
   CB_ARG(K1 % 16 == 0 && (N1 / 2) % 16 == 0);
   if (wmode == 1) CB_ARG(K1 % 128 == 0 && (N1 / 2) % 128 == 0);
   CB_ARG(workspace_bytes >= chitu_b200_moe_workspace_bytes(T, topk, E, N1, K1));
+  // 4-bit weights run on the grouped wgmma path only (one group of 128 per pipeline stage of both GEMMs)
+  if (wmode == kWmodeW4 && !(N1 % 256 == 0 && K1 % 128 == 0 && (N1 / 2) % 128 == 0))
+    return cb::fail(-2, "fused_experts_w4a16: needs N1 %% 256 == 0, K1 %% 128 == 0 and (N1 / 2) %% 128 == 0 "
+                        "(N1 = %d, K1 = %d)", N1, K1);
   if (T == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
   const int64_t P = (int64_t)T * topk;
@@ -1042,8 +1057,14 @@ static int fused_experts_impl(const void* x, const void* w1, const void* w2, con
   // ---- grouped wgmma path: sort pairs by expert, stream every distinct expert once ----
   const int BN = moe_chunk_rows(P, E);
   const int64_t chunks = E + P / 16 + 1;
-  if (P <= kPlanMaxPairs && E <= kPlanThreads && N1 % 256 == 0 && K1 % 128 == 0 && (wmode != 2 || (N1 / 2) % 128 == 0) &&
-      chunks * (N1 / 128) <= cb::tc_max_tiles() && chunks * (K1 / 128) <= cb::tc_max_tiles() && cb::tma_available()) {
+  const bool grouped = P <= kPlanMaxPairs && E <= kPlanThreads && N1 % 256 == 0 && K1 % 128 == 0 &&
+                       (wmode != 2 || (N1 / 2) % 128 == 0) && chunks * (N1 / 128) <= cb::tc_max_tiles() &&
+                       chunks * (K1 / 128) <= cb::tc_max_tiles() && cb::tma_available();
+  if (!grouped && wmode == kWmodeW4)
+    return cb::fail(-2, "fused_experts_w4a16: the grouped wgmma path cannot run (T=%d topk=%d E=%d N1=%d K1=%d; it needs "
+                        "T * topk <= %d, E <= %d and TMA), and 4-bit weights have no other path", T, topk, E, N1, K1,
+                    kPlanMaxPairs, kPlanThreads);
+  if (grouped) {
     const GroupedWs ws(workspace, P, E, N1, K1);
     const MoePlan& pl = ws.pl;
     const int quant = wmode == 1, gkind = moe_gemm_kind(wmode);
@@ -1059,13 +1080,13 @@ static int fused_experts_impl(const void* x, const void* w1, const void* w2, con
                  (const int*)pl.pair_sorted, (const int*)pl.seg_start, E, topk, K1, quant, ws.xs, ws.xs_s,
                  (__nv_bfloat16*)ws.xs);
     CB_LAUNCHED(1);
-    rc = cb::tc_grouped_gemm(gkind, ws.xs, ws.xs_s, w1, w1_s, ws.c1, (int)P, E, N1, K1, BN, pl.num_tiles1, pl.tile1_wrow,
+    rc = cb::tc_grouped_gemm(gkind, ws.xs, ws.xs_s, w1, w1_s, w4.w1_s, w4.w1_z, ws.c1, (int)P, E, N1, K1, BN, pl.num_tiles1, pl.tile1_wrow,
                              pl.tile1_xrow, pl.tile1_cnt, nullptr, nullptr, workspace, cb::tc_workspace_bytes(128, 128), st);
     if (rc) return rc;
     cb::launch_k(moe_silu_quant_kernel, dim3(cdiv(P * (N2 / 128), 8)), dim3(256), 0, st, (const __nv_bfloat16*)ws.c1,
                  (const int*)pl.seg_start, E, N2, quant, ws.a2, ws.a2_s, (__nv_bfloat16*)ws.a2);
     CB_LAUNCHED(1);
-    rc = cb::tc_grouped_gemm(gkind, ws.a2, ws.a2_s, w2, w2_s, ws.c3, (int)P, E, K1, N2, BN, pl.num_tiles2, pl.tile2_wrow,
+    rc = cb::tc_grouped_gemm(gkind, ws.a2, ws.a2_s, w2, w2_s, w4.w2_s, w4.w2_z, ws.c3, (int)P, E, K1, N2, BN, pl.num_tiles2, pl.tile2_wrow,
                              pl.tile2_xrow, pl.tile2_cnt, pl.w_sorted, nullptr, workspace, cb::tc_workspace_bytes(128, 128),
                              st);
     if (rc) return rc;
@@ -1121,9 +1142,22 @@ extern "C" int chitu_b200_fused_experts(const void* x, const void* w1, const voi
                                         const void* topk_ids, int ids_dtype, int T, int topk, int E, int N1,
                                         int K1, int wmode, void* out, const void* residual, void* workspace,
                                         int64_t workspace_bytes, void* stream) {
+  CB_ARG(out && wmode >= 0 && wmode <= 2);
+  return fused_experts_impl(x, w1, w2, w1_s, w2_s, W4Operands{}, topk_w, topk_w_dtype, topk_ids, ids_dtype, T, topk, E, N1,
+                            K1, wmode, out, residual, workspace, workspace_bytes, stream, nullptr);
+}
+
+// fused_experts over 4-bit weights (W4A16, groups of 128): the grouped path of chitu_b200_fused_experts with the W4 kind of
+// the grouped GEMM; the plan, gather, SiLU and combine kernels are the bf16 mode's.
+extern "C" int chitu_b200_fused_experts_w4a16(const void* x, const void* w1, const void* w1_scales, const uint8_t* w1_zeros,
+                                              const void* w2, const void* w2_scales, const uint8_t* w2_zeros,
+                                              const void* topk_w, int topk_w_dtype, const void* topk_ids, int ids_dtype,
+                                              int T, int topk, int E, int N1, int K1, void* out, const void* residual,
+                                              void* workspace, int64_t workspace_bytes, void* stream) {
   CB_ARG(out);
-  return fused_experts_impl(x, w1, w2, w1_s, w2_s, topk_w, topk_w_dtype, topk_ids, ids_dtype, T, topk, E, N1, K1, wmode, out,
-                            residual, workspace, workspace_bytes, stream, nullptr);
+  return fused_experts_impl(x, w1, w2, nullptr, nullptr, W4Operands{w1_scales, w2_scales, w1_zeros, w2_zeros}, topk_w,
+                            topk_w_dtype, topk_ids, ids_dtype, T, topk, E, N1, K1, kWmodeW4, out, residual, workspace,
+                            workspace_bytes, stream, nullptr);
 }
 
 // fused_experts whose result (this rank's partial of the MoE block) is pushed into every rank's all-reduce area from the
@@ -1133,9 +1167,9 @@ extern "C" int chitu_b200_fused_experts_ar(const void* x, const void* w1, const 
                                            const void* topk_ids, int ids_dtype, int T, int topk, int E, int N1,
                                            int K1, int wmode, void* comm, void* workspace, int64_t workspace_bytes,
                                            void* stream) {
-  CB_ARG(comm && K1 % 2 == 0 && (int64_t)T * K1 * 2 <= cb::comm_slot_bytes(comm));
-  return fused_experts_impl(x, w1, w2, w1_s, w2_s, topk_w, topk_w_dtype, topk_ids, ids_dtype, T, topk, E, N1, K1, wmode, nullptr,
-                            nullptr, workspace, workspace_bytes, stream, comm);
+  CB_ARG(comm && K1 % 2 == 0 && (int64_t)T * K1 * 2 <= cb::comm_slot_bytes(comm) && wmode >= 0 && wmode <= 2);
+  return fused_experts_impl(x, w1, w2, w1_s, w2_s, W4Operands{}, topk_w, topk_w_dtype, topk_ids, ids_dtype, T, topk, E, N1,
+                            K1, wmode, nullptr, nullptr, workspace, workspace_bytes, stream, comm);
 }
 
 CB_DEFINE_TL_SETTER(moe)

@@ -71,6 +71,10 @@ class DecodeEngine:
     configuration measured on one GPU)."""
 
     linear_impl = 0          # `impl` of the bf16 linear entries: 0 = auto
+    # "w4a16": the subclass's W4_LINEARS hold (qweight, scales, zeros) in quantize/w4a16.py's layout (stacked per expert
+    # for the MoE weights) and run on the 4-bit GEMMs
+    weight_format = "bf16"
+    W4_LINEARS = ()
 
     def __init__(self, cfg, max_reqs: int, max_seq_len: int, device, page_size: int, seed: int, tp_rank: int,
                  tp_size: int, process_group, use_fused_allreduce: bool, attn_ws: tuple, lin_n: int):
@@ -112,6 +116,23 @@ class DecodeEngine:
         # only, never under a graph)
         self.capture_h = None
 
+    def _set_weight_format(self, weight_format: str, tp_size: int, process_group):
+        if weight_format not in ("bf16", "w4a16"):
+            raise ValueError(f"weight_format must be 'bf16' or 'w4a16', not {weight_format!r}")
+        if weight_format == "w4a16" and process_group is not None and tp_size > 1:
+            raise ValueError("weight_format='w4a16' runs on one GPU or one shard: the 4-bit GEMM has no push epilogue "
+                             "for the tensor-parallel all-reduce")
+        self.weight_format = weight_format
+
+    def _dequantized(self, lw: dict) -> dict:
+        """A copy of the layer's weights with the 4-bit ones as the bf16 values the kernels multiply (the oracle side of
+        the tests)."""
+        from .quantize.w4a16 import dequantize
+        d = dict(lw)
+        if self.weight_format == "w4a16":
+            d.update({name: dequantize(*lw[name]) for name in self.W4_LINEARS})
+        return d
+
     def _rope_tables(self, ang: torch.Tensor, dtype=torch.float32):
         """cos / sin tables from the rotary angles [positions, rot_dim / 2], and the per-step buffers that
         `_step_body` gathers them into by position."""
@@ -142,6 +163,15 @@ class DecodeEngine:
         check(self.lib.chitu_b200_linear_bf16(ptr(x), ptr(w), None, ptr(residual), ptr(y), M, N, K, _lib.CB_BF16,
                                               ptr(self.lin_ws), self.lin_ws.numel(), self.linear_impl,
                                               current_stream()), "linear_bf16")
+
+    def _layer_linear(self, x, lw, name, y, M, residual=None):
+        """y = x . lw[name]^T (+ residual) in the engine's weight format."""
+        if self.weight_format == "bf16":
+            return self._linear(x, lw[name], y, M, residual=residual)
+        q, s, z = lw[name]
+        check(self.lib.chitu_b200_w4a16_gemm(ptr(x), ptr(q), ptr(s), ptr(z), ptr(residual), ptr(y), M, q.shape[0],
+                                             2 * q.shape[1], _lib.CB_BF16, ptr(self.lin_ws), self.lin_ws.numel(),
+                                             current_stream()), f"w4a16 {name}")
 
     def _norm(self, x, w, y, q=None, qs=None):
         assert q is None and qs is None, "this engine has no fp8 norm output"
@@ -253,14 +283,9 @@ class LlamaDecodeEngine(DecodeEngine):
                  seed: int = 0, tp_rank: int = 0, tp_size: int = 1, process_group=None, linear_impl: int = 0,
                  use_fused_allreduce: bool = True, kv_dtype: torch.dtype = BF, weight_format: str = "bf16"):
         D = cfg.head_dim
-        if weight_format not in ("bf16", "w4a16"):
-            raise ValueError(f"weight_format must be 'bf16' or 'w4a16', not {weight_format!r}")
-        if weight_format == "w4a16" and process_group is not None and tp_size > 1:
-            raise ValueError("weight_format='w4a16' runs on one GPU or one shard: the 4-bit GEMM has no push epilogue "
-                             "for the tensor-parallel all-reduce")
+        self._set_weight_format(weight_format, tp_size, process_group)
         if weight_format == "w4a16" and linear_impl == 1:
             raise ValueError("weight_format='w4a16' runs on the wgmma GEMM only (linear_impl=1 selects the SIMT GEMV)")
-        self.weight_format = weight_format
         assert cfg.n_heads % tp_size == 0 and cfg.n_kv_heads % tp_size == 0
         self.Hq, self.Hkv, self.D = cfg.n_heads // tp_size, cfg.n_kv_heads // tp_size, D
         self.F = cfg.ffn_dim // tp_size
@@ -326,25 +351,13 @@ class LlamaDecodeEngine(DecodeEngine):
 
     def ref_layers(self):
         """The layer weights in the REFERENCE's layout (w13 = [w1 ; w3] halves) for the oracle side of the tests."""
-        from .quantize.w4a16 import dequantize
         out = []
         for lw in self.layers:
-            d = dict(lw)
-            if self.weight_format == "w4a16":
-                d.update({name: dequantize(*lw[name]) for name in self.W4_LINEARS})
+            d = self._dequantized(lw)
             if self.fuse_silu:
                 d["w13"] = d["w13"].view(self.F, 2, self.cfg.dim).transpose(0, 1).reshape(2 * self.F, self.cfg.dim).contiguous()
             out.append(d)
         return out
-
-    def _layer_linear(self, x, lw, name, y, M, residual=None):
-        """y = x . lw[name]^T (+ residual) in the engine's weight format."""
-        if self.weight_format == "bf16":
-            return self._linear(x, lw[name], y, M, residual=residual)
-        q, s, z = lw[name]
-        check(self.lib.chitu_b200_w4a16_gemm(ptr(x), ptr(q), ptr(s), ptr(z), ptr(residual), ptr(y), M, q.shape[0],
-                                             2 * q.shape[1], _lib.CB_BF16, ptr(self.lin_ws), self.lin_ws.numel(),
-                                             current_stream()), f"w4a16 {name}")
 
     def _decode_layers(self):
         lib, B, D = self.lib, self.B, self.D

@@ -6,6 +6,12 @@ where the reference all-reduces once per expert (FeedForward.down, 8 per layer).
 Tensor parallel where the reference shards (SURVEY §8e): heads (8 q / 2 kv heads per rank at tp=4), every expert's
 intermediate dim (gate/up chunked separately then concatenated, models/model.py:344-350); the router is computed
 replicated (the reference splits its K dim over the ranks and all-reduces 8 logits: same sum, different order).
+
+weight_format="w4a16" holds qkv, o and the experts as 4-bit groups of 128 (quantize/w4a16.py's round-to-nearest rule
+applied to the same synthetic weights, one layer at a time as it is generated, so the bf16 model never exists whole: at
+tp_size=1 the full Mixtral-8x7B fits on one 80 GB GPU) and runs them through chitu_b200_w4a16_gemm and
+chitu_b200_fused_experts_w4a16; router, embedding, head, norms, rotary and attention stay bf16.  The 4-bit GEMM has no
+push epilogue, so it runs on one GPU or in shard mode.
 """
 from __future__ import annotations
 
@@ -43,11 +49,23 @@ class MixtralConfig:
 MIXTRAL_8X7B = MixtralConfig()
 
 
+def _quantize_experts(w):
+    """Stacked expert weights [E, N, K] -> (qweight [E, N, K/2], scales [E, N, K/128], zeros [E, N, K/128]) by
+    quantize_rtn, one expert at a time."""
+    from .quantize.w4a16 import quantize_rtn
+    parts = [quantize_rtn(w[e], BF) for e in range(w.shape[0])]
+    return tuple(torch.stack(t) for t in zip(*parts))
+
+
 class MixtralDecodeEngine(DecodeEngine):
+    W4_LINEARS = ("wqkv", "wo", "w1", "w2")
+
     def __init__(self, cfg: MixtralConfig, max_reqs: int, max_seq_len: int, device="cuda:0", page_size: int = 256,
-                 seed: int = 0, tp_rank: int = 0, tp_size: int = 4, process_group=None, use_fused_allreduce: bool = True):
+                 seed: int = 0, tp_rank: int = 0, tp_size: int = 4, process_group=None, use_fused_allreduce: bool = True,
+                 weight_format: str = "bf16"):
         D = cfg.head_dim
         T = tp_size
+        self._set_weight_format(weight_format, tp_size, process_group)
         assert cfg.n_heads % T == 0 and cfg.n_kv_heads % T == 0 and cfg.intermediate_dim % (128 * T) == 0
         self.Hq, self.Hkv, self.D = cfg.n_heads // T, cfg.n_kv_heads // T, D
         self.F = cfg.intermediate_dim // T
@@ -63,12 +81,17 @@ class MixtralDecodeEngine(DecodeEngine):
         self.embed = rnd(g_rep, cfg.vocab_size, dim)
         self.layers = []
         for _ in range(cfg.n_layers):
-            self.layers.append(dict(
+            lw = dict(
                 attn_norm=torch.ones(dim, dtype=BF, device=dev), ffn_norm=torch.ones(dim, dtype=BF, device=dev),
                 wqkv=rnd(g, (self.Hq + 2 * self.Hkv) * D, dim), wo=rnd(g, dim, self.Hq * D),
                 gate_w=rnd(g_rep, self.E, dim, scale=0.05),
                 # experts stacked like fused_experts expects: w1 = [gate ; up] (merge_gate_up), w2 = down
-                w1=rnd(g, self.E, 2 * self.F, dim), w2=rnd(g, self.E, dim, self.F)))
+                w1=rnd(g, self.E, 2 * self.F, dim), w2=rnd(g, self.E, dim, self.F))
+            if weight_format == "w4a16":
+                from .quantize.w4a16 import quantize_rtn
+                lw["wqkv"], lw["wo"] = quantize_rtn(lw["wqkv"], BF), quantize_rtn(lw["wo"], BF)
+                lw["w1"], lw["w2"] = _quantize_experts(lw["w1"]), _quantize_experts(lw["w2"])
+            self.layers.append(lw)
         self.norm = torch.ones(dim, dtype=BF, device=dev)
         self.head = rnd(g, cfg.vocab_size // T, dim)
         nblk = self.max_blocks * max_reqs
@@ -102,7 +125,7 @@ class MixtralDecodeEngine(DecodeEngine):
             if self.capture_h is not None:
                 self.capture_h.append(h.clone())
             next_norm = self.layers[li + 1]["attn_norm"] if li + 1 < n_layers else self.norm
-            self._linear(self.xn, lw["wqkv"], self.qkv, B)
+            self._layer_linear(self.xn, lw, "wqkv", self.qkv, B)
             q = self.qkv[:, : self.Hq * D]
             k = self.qkv[:, self.Hq * D: (self.Hq + self.Hkv) * D]
             v_view = self.qkv[:, (self.Hq + self.Hkv) * D:]
@@ -116,7 +139,7 @@ class MixtralDecodeEngine(DecodeEngine):
                 self.Hkv * D, qkv_w, ptr(self.seq_lens), ptr(self.block_table), self.max_blocks, B, self.Hq, self.Hkv, D,
                 self.page, self.max_seq_len, 1.0 / math.sqrt(D), ptr(self.attn_out), ptr(self.attn_ws),
                 self.attn_ws.numel(), _lib.CB_BF16, st), "gqa_paged_decode")
-            self._row_parallel(lambda out, res: self._linear(self.attn_out, lw["wo"], out, B, residual=res),
+            self._row_parallel(lambda out, res: self._layer_linear(self.attn_out, lw, "wo", out, B, residual=res),
                                lambda: self.comm.linear_push(self.attn_out, lw["wo"], B, self.lin_ws),
                                h, h2, lw["ffn_norm"], y=self.xn)
             # ---- sparse MoE block (model_hf_mixtral.py:51-96) through the fused experts ----
@@ -124,10 +147,7 @@ class MixtralDecodeEngine(DecodeEngine):
                                           1.0, ptr(self.gate_w_all[li]), ptr(self.gate_i_all[li]), self.topk,
                                           ptr(self.gate_ws), self.gate_ws.numel(), st), "moe_gate")
             self._row_parallel(
-                lambda out, res: check(lib.chitu_b200_fused_experts(
-                    ptr(self.xn), ptr(lw["w1"]), ptr(lw["w2"]), None, None, ptr(self.gate_w_all[li]), _lib.CB_BF16,
-                    ptr(self.gate_i_all[li]), _lib.CB_I64, B, self.topk, self.E, 2 * self.F, cfg.dim, 0, ptr(out), ptr(res),
-                    ptr(self.moe_ws), self.moe_ws.numel(), st), "fused_experts"),
+                lambda out, res: self._experts(li, lw, out, res),
                 lambda: self.comm.experts_push(self.xn, lw["w1"], lw["w2"], None, None, self.gate_w_all[li], _lib.CB_BF16,
                                                self.gate_i_all[li], _lib.CB_I64, B, self.topk, self.E, 2 * self.F, cfg.dim, 0,
                                                self.moe_ws),
@@ -135,15 +155,36 @@ class MixtralDecodeEngine(DecodeEngine):
         if self.capture_h is not None:
             self.capture_h.append(h.clone())
 
+    def _experts(self, li, lw, out, res):
+        """out = the fused experts of layer li on self.xn (+ res) in the engine's weight format."""
+        lib, B, st = self.lib, self.B, current_stream()
+        route = (ptr(self.gate_w_all[li]), _lib.CB_BF16, ptr(self.gate_i_all[li]), _lib.CB_I64, B, self.topk, self.E,
+                 2 * self.F, self.cfg.dim)
+        tail = (ptr(out), ptr(res), ptr(self.moe_ws), self.moe_ws.numel(), st)
+        if self.weight_format == "bf16":
+            check(lib.chitu_b200_fused_experts(ptr(self.xn), ptr(lw["w1"]), ptr(lw["w2"]), None, None, *route, 0, *tail),
+                  "fused_experts")
+        else:
+            (q1, s1, z1), (q2, s2, z2) = lw["w1"], lw["w2"]
+            check(lib.chitu_b200_fused_experts_w4a16(ptr(self.xn), ptr(q1), ptr(s1), ptr(z1), ptr(q2), ptr(s2), ptr(z2),
+                                                     *route, *tail), "fused_experts_w4a16")
+
+    def ref_layers(self):
+        """The layer weights as the reference multiplies them (the 4-bit ones dequantised) for the oracle side of the
+        tests."""
+        return [self._dequantized(lw) for lw in self.layers]
+
     def distinct_experts_per_layer(self) -> float:
         ids = self.gate_i_all.cpu()
         return float(sum(len(torch.unique(ids[l])) for l in range(ids.shape[0])) / ids.shape[0])
 
     def algorithmic_bytes(self, seq_len: int, distinct: float) -> int:
-        """SURVEY §8d: every attention weight byte once, each DISTINCT expert once, KV rows once, bf16 head + router."""
+        """SURVEY §8d: every attention weight byte once, each DISTINCT expert once, KV rows once, bf16 head + router.
+        4-bit weights count the packed weight, its bf16 scales and its uint8 zeros."""
         c, D = self.cfg, self.D
-        attn = ((self.Hq + 2 * self.Hkv) * D * c.dim + c.dim * self.Hq * D) * 2
-        expert = 3 * self.F * c.dim * 2
+        wbytes = (lambda n: n // 2 + n // 128 * 3) if self.weight_format == "w4a16" else (lambda n: n * 2)
+        attn = wbytes((self.Hq + 2 * self.Hkv) * D * c.dim) + wbytes(c.dim * self.Hq * D)
+        expert = wbytes(3 * self.F * c.dim)
         kv = self.B * (seq_len + 1) * 2 * self.Hkv * D * 2
         return int(c.n_layers * (attn + distinct * expert + kv + self.E * c.dim * 2) + self.head.numel() * 2)
 

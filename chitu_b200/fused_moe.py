@@ -137,11 +137,19 @@ def fused_experts(hidden_states: torch.Tensor, w1: torch.Tensor, w2: torch.Tenso
                   a1_scale: Optional[torch.Tensor] = None, a2_scale: Optional[torch.Tensor] = None,
                   block_shape: Optional[List[int]] = None, soft_fp8: bool = False) -> torch.Tensor:
     """fused_moe.py:1060-1307 — same signature.  Quantisation flags that are outside the
-    north-star path are accepted and rejected with NotImplementedError (SURVEY §8b)."""
-    if use_int8_w8a16 or use_int4_w4a16:
-        raise NotImplementedError("int8_w8a16 / int4_w4a16 expert weights are outside the hot path of this library")
+    north-star path are accepted and rejected with NotImplementedError (SURVEY §8b).
+
+    use_int4_w4a16=True: 4-bit weights in groups of 128 along K (GPTQ / AWQ after `quantize.w4a16.pack_experts`; vLLM's
+    int4 MoE layout): w1 uint8 [E, N1, K1/2] and w2 uint8 [E, K1, N1/4] (element k of a row in byte k/2, low nibble for
+    even k), w1_scale / w2_scale bf16 [E, N, K/128], w1_zp / w2_zp uint8 [E, N, K/128] with one zero (0..15) per byte,
+    or None for zeros of 8; block_shape None or [0, 128]; bf16 hidden states.  Weight element = bf16((q - z) * s)."""
+    if use_int8_w8a16:
+        raise NotImplementedError("int8_w8a16 expert weights are outside the hot path of this library")
     if activation != "silu":
         raise ValueError(f"Unsupported FusedMoe activation: {activation}")
+    if use_int4_w4a16:
+        return _fused_experts_w4a16(hidden_states, w1, w2, topk_weights, topk_ids, inplace, expert_map, w1_scale,
+                                    w2_scale, w1_zp, w2_zp, a1_scale, a2_scale, block_shape)
     if a1_scale is not None or a2_scale is not None or w1_zp is not None or w2_zp is not None:
         raise NotImplementedError("static activation scales / zero points are not used by the reference callers")
     assert hidden_states.shape[1] == w1.shape[2], "Hidden size mismatch"
@@ -162,6 +170,20 @@ def fused_experts(hidden_states: torch.Tensor, w1: torch.Tensor, w2: torch.Tenso
     else:
         assert w1.dtype == torch.bfloat16 and w2.dtype == torch.bfloat16
         wmode, w1_s, w2_s = 0, None, None
+    ids, tw = _routing(topk_ids, topk_weights, expert_map)
+    out = hidden_states if inplace else torch.empty_like(hidden_states)
+    lib = _lib.load()
+    for t0, t1, ws in _chunks(lib, T, topk, E, N1, K1, hidden_states.device):
+        check(lib.chitu_b200_fused_experts(
+            ptr(hidden_states[t0:t1]), ptr(w1), ptr(w2), ptr(w1_s), ptr(w2_s), ptr(tw[t0:t1]), dtype_code(tw.dtype),
+            ptr(ids[t0:t1]), dtype_code(ids.dtype), t1 - t0, topk, E, N1, K1, wmode, ptr(out[t0:t1]), None, ptr(ws),
+            ws.numel(), current_stream()), "fused_experts")
+    return out
+
+
+def _routing(topk_ids, topk_weights, expert_map):
+    """The ids (int32 / int64, local expert numbers, -1 = not on this rank) and routed weights (bf16 / fp32) the C entries
+    take."""
     ids = topk_ids.contiguous()
     if expert_map is not None:  # expert parallelism: global -> local id, -1 = not on this rank
         ids = expert_map[ids.long()].to(torch.int32).contiguous()
@@ -170,17 +192,64 @@ def fused_experts(hidden_states: torch.Tensor, w1: torch.Tensor, w2: torch.Tenso
     tw = topk_weights.contiguous()
     if tw.dtype not in (torch.bfloat16, torch.float32):
         tw = tw.float()
-    out = hidden_states if inplace else torch.empty_like(hidden_states)
-    lib = _lib.load()
-    # (token, slot) pairs per launch: <= 8192 keeps every chunk on the grouped wgmma path (each distinct expert streamed
-    # once per chunk); the C side accepts up to 65535 pairs (SIMT fallback above 8192)
+    return ids, tw
+
+
+def _chunks(lib, T, topk, E, N1, K1, device):
+    """(t0, t1, workspace) of each C call: (token, slot) pairs per launch <= 8192 keeps every chunk on the grouped wgmma
+    path (each distinct expert streamed once per chunk); the C side accepts up to 65535 pairs (SIMT fallback above 8192)."""
     CHUNK = max(1, 8192 // max(topk, 1))
     for t0 in range(0, T, CHUNK):
         t1 = min(T, t0 + CHUNK)
-        n = lib.chitu_b200_moe_workspace_bytes(t1 - t0, topk, E, N1, K1)
-        ws = workspace.get("moe", n, hidden_states.device)
-        check(lib.chitu_b200_fused_experts(
-            ptr(hidden_states[t0:t1]), ptr(w1), ptr(w2), ptr(w1_s), ptr(w2_s), ptr(tw[t0:t1]), dtype_code(tw.dtype),
-            ptr(ids[t0:t1]), dtype_code(ids.dtype), t1 - t0, topk, E, N1, K1, wmode, ptr(out[t0:t1]), None, ptr(ws),
-            ws.numel(), current_stream()), "fused_experts")
+        yield t0, t1, workspace.get("moe", lib.chitu_b200_moe_workspace_bytes(t1 - t0, topk, E, N1, K1), device)
+
+
+def _w4_operand(name, t, dtype, shape):
+    if t is None:
+        raise ValueError(f"use_int4_w4a16 needs {name}")
+    if t.dtype != dtype or tuple(t.shape) != tuple(shape):
+        raise ValueError(f"use_int4_w4a16: {name} must be {dtype} {list(shape)}, not {t.dtype} {list(t.shape)}")
+    return t.contiguous()
+
+
+def _fused_experts_w4a16(hidden_states, w1, w2, topk_weights, topk_ids, inplace, expert_map, w1_scale, w2_scale, w1_zp,
+                         w2_zp, a1_scale, a2_scale, block_shape):
+    """fused_experts over 4-bit expert weights (see fused_experts); every check is made before anything runs."""
+    if a1_scale is not None or a2_scale is not None:
+        raise ValueError("use_int4_w4a16 takes no activation scales (the activations stay bf16)")
+    if block_shape is not None and list(block_shape) != [0, 128]:
+        raise ValueError(f"use_int4_w4a16 is built for groups of 128 along K (block_shape [0, 128]), not {block_shape}")
+    if hidden_states.dtype != torch.bfloat16:
+        raise ValueError(f"use_int4_w4a16 computes in bf16, not {hidden_states.dtype}")
+    if hidden_states.dim() != 2 or w1.dim() != 3 or w2.dim() != 3:
+        raise ValueError("use_int4_w4a16: hidden_states [T, K1], w1 [E, N1, K1/2] and w2 [E, K1, N1/4]")
+    T, K1 = hidden_states.shape
+    E, N1 = w1.shape[0], w1.shape[1]
+    G1, G2 = K1 // 128, N1 // 2 // 128
+    if K1 % 128 != 0 or N1 % 256 != 0:
+        raise ValueError(f"use_int4_w4a16 needs K1 % 128 == 0 and N1 % 256 == 0 (K1 = {K1}, N1 = {N1})")
+    w1 = _w4_operand("w1", w1, torch.uint8, (E, N1, K1 // 2))
+    w2 = _w4_operand("w2", w2, torch.uint8, (E, K1, N1 // 4))
+    w1_s = _w4_operand("w1_scale", w1_scale, torch.bfloat16, (E, N1, G1))
+    w2_s = _w4_operand("w2_scale", w2_scale, torch.bfloat16, (E, K1, G2))
+    zps = []
+    for name, zp, N, G in (("w1_zp", w1_zp, N1, G1), ("w2_zp", w2_zp, K1, G2)):
+        if zp is not None and zp.dim() == 3 and tuple(zp.shape) == (E, N // 2, G):
+            raise ValueError(f"use_int4_w4a16: {name} {list(zp.shape)} holds two packed zero points per byte (vLLM's "
+                             f"layout); give one zero per byte, [E, N, K/128] — quantize.w4a16.pack_experts builds it")
+        zps.append(None if zp is None else _w4_operand(name, zp, torch.uint8, (E, N, G)))
+    if topk_weights.shape != topk_ids.shape or topk_ids.dim() != 2 or topk_ids.shape[0] != T:
+        raise ValueError("use_int4_w4a16: topk_weights and topk_ids must both be [T, topk]")
+    if not hidden_states.is_contiguous():
+        raise ValueError("use_int4_w4a16: hidden_states must be contiguous")
+    require_cuda(hidden_states, w1, w2, w1_s, w2_s, *zps, topk_weights, topk_ids)
+    topk = topk_ids.shape[1]
+    ids, tw = _routing(topk_ids, topk_weights, expert_map)
+    out = hidden_states if inplace else torch.empty_like(hidden_states)
+    lib = _lib.load()
+    for t0, t1, ws in _chunks(lib, T, topk, E, N1, K1, hidden_states.device):
+        check(lib.chitu_b200_fused_experts_w4a16(
+            ptr(hidden_states[t0:t1]), ptr(w1), ptr(w1_s), ptr(zps[0]), ptr(w2), ptr(w2_s), ptr(zps[1]), ptr(tw[t0:t1]),
+            dtype_code(tw.dtype), ptr(ids[t0:t1]), dtype_code(ids.dtype), t1 - t0, topk, E, N1, K1, ptr(out[t0:t1]), None,
+            ptr(ws), ws.numel(), current_stream()), "fused_experts_w4a16")
     return out

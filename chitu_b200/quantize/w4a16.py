@@ -6,7 +6,8 @@ The device layout of a weight W[N, K] (include/chitu_b200.h, chitu_b200_w4a16_ge
 The weight element is io((q - z) * s), one rounding; the GEMM accumulates in fp32 and rounds once to the io dtype.
 
 `from_gptq` / `from_awq` repack the two checkpoint layouts into it and `from_float` quantises a float weight; all three
-are host torch, run once at load time.  `forward` runs the sm_90a kernel; there is no other path."""
+are host torch, run once at load time.  `forward` runs the sm_90a kernel; there is no other path.  `pack_experts` stacks
+per-expert modules into the layout of `fused_moe.fused_experts(use_int4_w4a16=True)`."""
 from __future__ import annotations
 
 import torch
@@ -36,17 +37,18 @@ def pack_rows(q):
 
 
 def unpack_rows(qweight):
-    """The device's uint8 [N, K/2] -> q [N, K] (uint8, 0..15)."""
+    """The device's uint8 [..., N, K/2] -> q [..., N, K] (uint8, 0..15)."""
     lo, hi = qweight & 0xF, qweight >> 4
-    return torch.stack((lo, hi), dim=-1).reshape(qweight.shape[0], -1)
+    return torch.stack((lo, hi), dim=-1).reshape(*qweight.shape[:-1], -1)
 
 
 def dequantize(qweight, scales, zeros):
-    """The element values the kernel multiplies: io((q - z) * s) [N, K] in scales' dtype.  (q - z) * s is exact in fp32
-    (a 5-bit integer times a 16-bit float), so the cast is the one rounding."""
+    """The element values the kernel multiplies: io((q - z) * s) [..., N, K] in scales' dtype (leading dims: a stack of
+    experts; zeros None: every zero is 8).  (q - z) * s is exact in fp32 (a 5-bit integer times a 16-bit float), so the
+    cast is the one rounding."""
     q = unpack_rows(qweight).float()
-    z = zeros.float().repeat_interleave(GROUP, dim=1)
-    s = scales.float().repeat_interleave(GROUP, dim=1)
+    z = 8.0 if zeros is None else zeros.float().repeat_interleave(GROUP, dim=-1)
+    s = scales.float().repeat_interleave(GROUP, dim=-1)
     return ((q - z) * s).to(scales.dtype)
 
 
@@ -161,3 +163,31 @@ class W4A16Linear(nn.Module):
 
     def extra_repr(self):
         return f"{self.in_features}, {self.out_features}, bias={self.bias is not None}, dtype={self.dtype}"
+
+
+@torch.no_grad()
+def pack_experts(gate, up, down):
+    """Stack per-expert W4A16Linear modules (from `from_gptq` / `from_awq` / `from_float`) into the expert layout of
+    `fused_moe.fused_experts(use_int4_w4a16=True)`: gate / up / down are lists of E modules (Mixtral's w1 / w3 / w2), and
+    the result is (w1, w1_scale, w1_zp, w2, w2_scale, w2_zp) with
+      w1 uint8 [E, 2F, K/2] = each expert's [gate ; up] rows,  w2 uint8 [E, K, F/2] = down,
+      w*_scale bf16 [E, N, K/128],  w*_zp uint8 [E, N, K/128].
+    The MoE path computes in bf16, so the scales are cast to bf16.  GPTQ and AWQ store fp16 scales: that cast is one
+    rounding of each scale that the fp16 checkpoint does not have (about 2^-9 relative).  Biases are not carried (the
+    expert linears of Mixtral have none); a module with a bias is refused."""
+    if not (len(gate) == len(up) == len(down)) or not gate:
+        raise ValueError(f"pack_experts needs the same number (> 0) of gate, up and down modules, not "
+                         f"{len(gate)}, {len(up)}, {len(down)}")
+    if any(m.bias is not None for m in (*gate, *up, *down)):
+        raise ValueError("pack_experts: the fused experts take no bias")
+
+    def stack(mods):
+        return tuple(torch.stack([getattr(m, name) for m in mods]).contiguous() for name in ("qweight", "scales", "zeros"))
+
+    w1 = [torch.cat(pair, dim=1) for pair in zip(stack(gate), stack(up))]
+    w2 = list(stack(down))
+    if w1[0].shape[-1] * 2 != w2[0].shape[1] or w2[0].shape[-1] * 4 != w1[0].shape[1]:
+        raise ValueError(f"pack_experts: gate / up [{w1[0].shape[1] // 2}, {w1[0].shape[-1] * 2}] and down "
+                         f"[{w2[0].shape[1]}, {w2[0].shape[-1] * 2}] do not chain")
+    w1[1], w2[1] = w1[1].to(torch.bfloat16), w2[1].to(torch.bfloat16)
+    return w1[0], w1[1], w1[2], w2[0], w2[1], w2[2]

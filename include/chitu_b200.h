@@ -480,6 +480,17 @@ int chitu_b200_fused_experts(const void* x, const void* w1, const void* w2, cons
                              int K1, int wmode, void* out,
                              const void* residual /* [T,K1] bf16 added to the rounded result, or NULL */,
                              void* workspace, int64_t workspace_bytes, void* stream);
+/* fused_experts over 4-bit weights (W4A16, groups of 128 along K; vLLM's use_int4_w4a16 with block_shape [0, 128]):
+ * w1 uint8 [E, N1, K1/2], w2 uint8 [E, K1, N1/4]: element k of a weight row in byte k/2, low nibble for even k
+ * (quantize/w4a16.py); w*_scales bf16 [E, N, K/128]; w*_zeros uint8 [E, N, K/128], 0..15, or NULL: every zero is 8.
+ * The weight element is bf16((q - z) * s); x, topk_w, topk_ids, out, residual and the workspace
+ * (chitu_b200_moe_workspace_bytes) as in chitu_b200_fused_experts with wmode 0.  Runs on the grouped wgmma path only:
+ * N1 % 256 == 0, K1 % 128 == 0, (N1/2) % 128 == 0, T * topk <= 8192 and E <= 1024, otherwise -2 before any launch. */
+int chitu_b200_fused_experts_w4a16(const void* x, const void* w1, const void* w1_scales, const uint8_t* w1_zeros,
+                                   const void* w2, const void* w2_scales, const uint8_t* w2_zeros, const void* topk_w,
+                                   int topk_w_dtype, const void* topk_ids, int ids_dtype, int T, int topk, int E, int N1,
+                                   int K1, void* out, const void* residual, void* workspace, int64_t workspace_bytes,
+                                   void* stream);
 
 /* ---- tensor-parallel collective fused with what follows it ------------------------------------------ */
 /* Replaces `all_reduce` of RowParallelLinear.forward (tensor_parallel.py:157-169) / MoEDeepSeekV3
