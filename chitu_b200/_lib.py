@@ -48,6 +48,8 @@ SIGNATURES = {
     "chitu_b200_silu_and_mul": (I, [P, P, L, I, I, P]),
     "chitu_b200_act_quant_fp8": (I, [P, P, P, L, I, I, I, F, I, P]),
     "chitu_b200_quant_act_int8": (I, [P, P, P, L, I, I, P]),
+    "chitu_b200_quant_fp8_rowwise": (I, [P, P, P, L, I, P, P, P]),
+    "chitu_b200_rmsnorm_quant_fp8_rowwise": (I, [P, P, P, P, P, I, I, F, P]),
     "chitu_b200_weight_dequant_fp8": (I, [P, P, P, I, I, I, I, I, P]),
     "chitu_b200_linear_workspace_bytes": (L, [I, I]),
     "chitu_b200_linear_bf16": (I, [P, P, P, P, P, I, I, I, I, P, L, I, P]),
@@ -57,6 +59,8 @@ SIGNATURES = {
     "chitu_b200_w8a8_gemm": (I, [P, P, P, P, P, P, I, I, I, P, L, I, P]),
     "chitu_b200_w4a16_gemm": (I, [P, P, P, P, P, P, I, I, I, I, P, L, P]),
     "chitu_b200_w4a16_gemm_silu_pairs": (I, [P, P, P, P, P, I, I, I, I, P, L, P]),
+    "chitu_b200_fp8_rowwise_gemm": (I, [P, P, P, P, P, P, P, I, I, I, P, L, P]),
+    "chitu_b200_fp8_rowwise_gemm_silu_pairs": (I, [P, P, P, P, P, I, I, I, P, L, P]),
     "chitu_b200_attn_workspace_bytes": (L, [I, I, I, I]),
     "chitu_b200_gqa_paged_decode": (I, [P, P, P, P, P, L, L, P, P, I, I, I, I, I, I, I, F, P, P, L, I, P]),
     "chitu_b200_gqa_paged_decode_rope": (I, [P, L, P, P, P, P, L, L, P, P, P, P, I, I, I, I, I, I, I, F, P, P, L, I, P]),

@@ -298,6 +298,142 @@ extern "C" int chitu_b200_rmsnorm_quant_fp8(const void* x, const void* w, void* 
 }
 
 // ============================================================================================
+// Per-token e4m3 quantisation, vLLM QuantFP8(GroupShape.PER_TOKEN).forward_native
+// (model_executor/layers/quantization/input_quant_fp8.py): dynamic s = max(min(amax, ub) / 448, 1 / (448 * 512)) in
+// fp32, or the static s given; q = e4m3_rn(clamp(fp32(x) * rcp_rn(s), +-448)).  One CTA of 256 threads per row.
+// ============================================================================================
+__device__ __forceinline__ float e4m3_row_scale(float amax, const float* scale, const float* scale_ub) {
+  if (scale) return *scale;
+  if (scale_ub) amax = fminf(amax, *scale_ub);
+  return fmaxf(__fdiv_rn(amax, 448.f), 1.f / (448.f * 512.f));
+}
+__device__ __forceinline__ uint8_t e4m3_rowwise(float v, float rcp) {
+  return float_to_fp8(fminf(fmaxf(__fmul_rn(v, rcp), -448.f), 448.f));
+}
+// the maximum over the 256 threads of the CTA, on every thread
+__device__ __forceinline__ float block_max256(float v) {
+  __shared__ float red[8];
+  v = warp_max(v);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  float m = red[0];
+#pragma unroll
+  for (int i = 1; i < 8; ++i) m = fmaxf(m, red[i]);
+  return m;
+}
+
+// RMSNorm + the dynamic per-token quantisation.  The sum of squares runs in rmsnorm_kernel's order (thread t: elements
+// t, t + 256, ...; then the warps, then the 8 warp sums in order) and y is rounded as there, so q and s are bit for bit
+// chitu_b200_rmsnorm followed by chitu_b200_quant_fp8_rowwise.  The row stays in registers: dim <= 8192.
+__global__ void __launch_bounds__(256) rmsnorm_quant_rowwise_kernel(const __nv_bfloat16* __restrict__ x,
+                                                                    const __nv_bfloat16* __restrict__ w,
+                                                                    __nv_bfloat16* __restrict__ y,
+                                                                    uint8_t* __restrict__ q, float* __restrict__ qs,
+                                                                    int dim, float eps) {
+  cb::pdl_prologue();
+  constexpr int kMaxIt = 32;                       // 32 x 256 threads = 8192
+  const int64_t row = blockIdx.x;
+  const __nv_bfloat16* xr = x + row * dim;
+  float v[kMaxIt];
+  float ss = 0.f;
+#pragma unroll
+  for (int j = 0; j < kMaxIt; ++j) {
+    const int i = threadIdx.x + 256 * j;
+    v[j] = 0.f;
+    if (i < dim) {
+      v[j] = __bfloat162float(xr[i]);
+      ss += v[j] * v[j];
+    }
+  }
+  __shared__ float red[8];
+  ss = warp_sum(ss);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = ss;
+  __syncthreads();
+  float tot = 0.f;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) tot += red[i];
+  const float r = rsqrtf(tot / (float)dim + eps);
+  float amax = 0.f;
+#pragma unroll
+  for (int j = 0; j < kMaxIt; ++j) {
+    const int i = threadIdx.x + 256 * j;
+    if (i < dim) {
+      const __nv_bfloat16 o = __float2bfloat16_rn(v[j] * r * __bfloat162float(w[i]));
+      if (y) y[row * dim + i] = o;
+      v[j] = __bfloat162float(o);
+      amax = fmaxf(amax, fabsf(v[j]));
+    }
+  }
+  const float sc = e4m3_row_scale(block_max256(amax), nullptr, nullptr);
+  const float rcp = __frcp_rn(sc);
+#pragma unroll
+  for (int j = 0; j < kMaxIt; ++j) {
+    const int i = threadIdx.x + 256 * j;
+    if (i < dim) q[row * dim + i] = e4m3_rowwise(v[j], rcp);
+  }
+  if (threadIdx.x == 0) qs[row] = sc;
+}
+
+extern "C" int chitu_b200_rmsnorm_quant_fp8_rowwise(const void* x, const void* w, void* y, void* q, float* q_scales,
+                                                    int rows, int dim, float eps, void* stream) {
+  CB_ARG(x && w && q && q_scales && rows >= 0 && dim > 0 && dim <= 8192);
+  CB_ARG(((uintptr_t)x | (uintptr_t)w | (uintptr_t)y) % 2 == 0);
+  if (rows == 0) return 0;
+  cb::launch_k(rmsnorm_quant_rowwise_kernel, dim3(rows), dim3(256), 0, (cudaStream_t)stream, (const __nv_bfloat16*)x,
+               (const __nv_bfloat16*)w, (__nv_bfloat16*)y, (uint8_t*)q, q_scales, dim, eps);
+  CB_LAUNCHED(1);
+  return 0;
+}
+
+// The standalone quantiser: 8 elements per thread and pass; the second pass re-reads the row from L1 / L2.
+__global__ void __launch_bounds__(256) quant_fp8_rowwise_kernel(const __nv_bfloat16* __restrict__ x,
+                                                                uint8_t* __restrict__ q, float* __restrict__ qs, int K,
+                                                                const float* __restrict__ scale,
+                                                                const float* __restrict__ scale_ub) {
+  cb::pdl_prologue();
+  const int64_t row = blockIdx.x;
+  const __nv_bfloat16* xr = x + row * K;
+  auto unpack = [](const uint4 raw, float (&f)[8]) {
+    const uint32_t u[4] = {raw.x, raw.y, raw.z, raw.w};
+#pragma unroll
+    for (int i = 0; i < 4; ++i) { f[2 * i] = bf16lo(u[i]); f[2 * i + 1] = bf16hi(u[i]); }
+  };
+  float amax = 0.f;
+  if (!scale) {
+    for (int e = threadIdx.x * 8; e < K; e += 256 * 8) {
+      float f[8];
+      unpack(*reinterpret_cast<const uint4*>(xr + e), f);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) amax = fmaxf(amax, fabsf(f[i]));
+    }
+    amax = block_max256(amax);
+  }
+  const float sc = e4m3_row_scale(amax, scale, scale_ub);
+  const float rcp = __frcp_rn(sc);
+  for (int e = threadIdx.x * 8; e < K; e += 256 * 8) {
+    float f[8];
+    unpack(*reinterpret_cast<const uint4*>(xr + e), f);
+    uint32_t b[2] = {0, 0};
+#pragma unroll
+    for (int i = 0; i < 8; ++i) b[i >> 2] |= (uint32_t)e4m3_rowwise(f[i], rcp) << (8 * (i & 3));
+    *reinterpret_cast<uint2*>(q + row * K + e) = make_uint2(b[0], b[1]);
+  }
+  if (threadIdx.x == 0) qs[row] = sc;
+}
+
+extern "C" int chitu_b200_quant_fp8_rowwise(const void* x, void* q, float* q_scales, int64_t rows, int K,
+                                            const float* scale, const float* scale_ub, void* stream) {
+  CB_ARG(x && q && q_scales && rows >= 0 && rows <= INT32_MAX && K > 0 && K % 16 == 0);
+  CB_ARG(!(scale && scale_ub));                                   // an upper bound belongs to the dynamic mode
+  CB_ARG(((uintptr_t)x | (uintptr_t)q) % 16 == 0);
+  if (rows == 0) return 0;
+  cb::launch_k(quant_fp8_rowwise_kernel, dim3((unsigned)rows), dim3(256), 0, (cudaStream_t)stream,
+               (const __nv_bfloat16*)x, (uint8_t*)q, q_scales, K, scale, scale_ub);
+  CB_LAUNCHED(1);
+  return 0;
+}
+
+// ============================================================================================
 // Fused SiluAndMul + act_quant (dense FFN: linear_deepseek_v3 of w2 quantises silu(w1 x)*w3 x,
 // model_deepseek_v3.py:755-771): x [rows, 2F] bf16 -> fp8 [rows, F] + scales [rows, F/128] (mode 0: no eps)
 // ============================================================================================

@@ -24,6 +24,8 @@
 //   kind 1: fp8_gemm_deepseek_v3 (ops.py:452-483, triton_kernels.py:303-365)
 //   kind 2: w8a8gemm.mm / w8a8gemv.mv (quantize/w8a8.py:105,120,125)
 //   kind 4: W4A16, group 128 (GPTQ / AWQ weights after quantize/w4a16.py's repack): w = io((q - z) * s)
+//   kind 5: FP8 W8A8 with rowwise scales (vLLM Fp8LinearMethod / torch._scaled_mm, scale_a [M, 1], scale_b [1, N]):
+//           y = bf16((sum_k qx qw) * a_s[m] * b_s[n] (+ bias)); each 128-K stage is promoted into fp32 registers
 #include <cuda.h>
 
 #include <mutex>
@@ -65,8 +67,8 @@ struct Params {
   int act_pairs;            // kind 0: weight rows (2i, 2i+1) = (gate_i, up_i); out[m, i] = SiluAndMul -> [M, N/2]
   int has_push;             // row-parallel linear of a tensor-parallel layer: the bf16 result is stored into every rank's
   PushDev push;             // push area instead of `out`, as epoch-tagged words (comm.cu allreduce_consume_kernel)
-  const float* a_s;         // fp8: [M, kblocks]         i8: a_scales [M]
-  const float* b_s;         // fp8: [ceil(N/128), kblocks] i8: b_scales [N]
+  const float* a_s;         // fp8: [M, kblocks]         i8, fp8r: a_scales [M]
+  const float* b_s;         // fp8: [ceil(N/128), kblocks] i8, fp8r: b_scales [N]
   const void* bias;         // [N] (io dtype; i8: fp16) or null
   const void* residual;     // [M, N] io dtype or null (kind 0 only)
   void* out;                // [M, N]
@@ -147,7 +149,7 @@ enum { EPI_PLAIN = 0, EPI_PAIRS = 1, EPI_PUSH = 2, EPI_ROWS = 3 };   // ROWS: Pa
 // (KIND_16 and KIND_W4 multiply fp16 operands when `f16`, bf16 otherwise)
 template <int KIND, int BN, typename Acc>
 __device__ __forceinline__ void mma_k(Acc (&d)[BN / 2], uint64_t a, uint64_t b, int accumulate, bool f16) {
-  if constexpr (KIND == KIND_FP8) WgmmaN<BN>::e4m3(d, a, b, accumulate);
+  if constexpr (KIND == KIND_FP8 || KIND == KIND_FP8R) WgmmaN<BN>::e4m3(d, a, b, accumulate);
   else if constexpr (KIND == KIND_I8) WgmmaN<BN>::s8(d, a, b, accumulate);
   else if constexpr (KIND == KIND_SOFT) WgmmaN<BN>::template bf16<0>(d, a, b, accumulate);
   else if (f16) WgmmaN<BN>::template f16<0>(d, a, b, accumulate);
@@ -422,6 +424,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
         reinterpret_cast<__half*>(p.out)[o] = h;
       } else if (p.out_dtype == CB_BF16) {
         float v = v_f;
+        if constexpr (KIND == KIND_FP8R) v = __fmul_rn(__fmul_rn(v, p.a_s[m]), p.b_s[n]);   // unfused: (acc a_s) b_s
         if (p.g_row_scale) v *= p.g_row_scale[m];
         if (p.bias) v += __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(p.bias)[n]);
         if (p.residual) v = __bfloat162float(__float2bfloat16_rn(v)) + __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(p.residual)[o]);
@@ -500,7 +503,8 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
           else if (have_next) fetch_scales(gn, ii.item().s_lo, bsc_n, av_n);
         }
         mbar_wait(&full_bar[s], (it / C::kStages) & 1);
-        const int first = KIND == KIND_FP8 || st == w.s_lo;     // fp8: a fresh accumulator per K block
+        // fp8, fp8r: a fresh accumulator per K block (the e4m3 wgmma does not accumulate in full fp32)
+        const int first = KIND == KIND_FP8 || KIND == KIND_FP8R || st == w.s_lo;
         wgmma_fence();
         if constexpr (C::kCvt) {
           // A = the 16-bit tile the converter warps produced from this stage's fp8 / 4-bit weights (two 64-element atoms)
@@ -536,11 +540,15 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
             acc[e] = fmaf(d[e] * as, bsc, acc[e]);
           }
         }
+        if constexpr (KIND == KIND_FP8R) {     // the stage's promotion; the scales wait for the epilogue
+#pragma unroll
+          for (int e = 0; e < NR; ++e) acc[e] += d[e];
+        }
       }
       float vals[NR];                             // i8: raw int32 bits kept in the float register
 #pragma unroll
       for (int e = 0; e < NR; ++e) {
-        if constexpr (KIND == KIND_FP8) vals[e] = acc[e];
+        if constexpr (KIND == KIND_FP8 || KIND == KIND_FP8R) vals[e] = acc[e];
         else if constexpr (KIND == KIND_I8) vals[e] = __int_as_float(d[e]);
         else vals[e] = d[e];
       }
@@ -583,7 +591,16 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
         }
       };
       auto emit = [&](const float (&v)[NR]) {
-        if constexpr (kPairs) {
+        if constexpr (kPairs && KIND == KIND_FP8R) {
+          // g and u each scaled by their own row's scale (rows past N or tokens past cnt: never written)
+          float sv[NR];
+#pragma unroll
+          for (int e = 0; e < NR; ++e) {
+            const int n = ge.ocol0 + row_of(e), j = col_of(e);
+            sv[e] = n_ok(e) && j < cnt ? __fmul_rn(__fmul_rn(v[e], p.a_s[m0 + j]), p.b_s[n]) : 0.f;
+          }
+          emit_pairs(sv);
+        } else if constexpr (kPairs) {
           emit_pairs(v);
         } else if constexpr (kPush) {
           emit_push(v);
@@ -722,7 +739,7 @@ Operands operands(int kind, int dtype) {
   if (kind == KIND_16) return {2, io, 2, io};
   if (kind == KIND_SOFT) return {1, u8, 2, bf16};
   if (kind == KIND_W4) return {1, u8, 2, io};
-  return {1, u8, 1, u8};                              // fp8, int8
+  return {1, u8, 1, u8};                              // fp8, int8, fp8r
 }
 
 int pick_bn(int M) { return M <= 16 ? 16 : M <= 32 ? 32 : M <= 64 ? 64 : 128; }
@@ -759,16 +776,18 @@ int launch_epi(const CUtensorMap& mw, const CUtensorMap& mx, Params& p, int grid
 template <int KIND, int BN>
 int launch(const CUtensorMap& mw, const CUtensorMap& mx, Params& p, int grid, cudaStream_t st) {
   if (p.act_pairs) {
-    if constexpr (KIND == KIND_16 || KIND == KIND_W4) return launch_epi<KIND, BN, EPI_PAIRS>(mw, mx, p, grid, st);
-    else return fail(-2, "tc gemm: the SiluAndMul epilogue is built for bf16 and 4-bit weights only");
+    if constexpr (KIND == KIND_16 || KIND == KIND_W4 || KIND == KIND_FP8R)
+      return launch_epi<KIND, BN, EPI_PAIRS>(mw, mx, p, grid, st);
+    else return fail(-2, "tc gemm: the SiluAndMul epilogue is built for bf16, 4-bit and rowwise fp8 weights only");
   }
   if (p.has_push) {
     if constexpr (KIND == KIND_16 || KIND == KIND_FP8) return launch_epi<KIND, BN, EPI_PUSH>(mw, mx, p, grid, st);
     else return fail(-2, "tc gemm: the push epilogue is built for bf16 and fp8 weights only");
   }
   if (p.g_out_rows) {
-    if constexpr (KIND != KIND_I8 && KIND != KIND_W4) return launch_epi<KIND, BN, EPI_ROWS>(mw, mx, p, grid, st);
-    else return fail(-2, "tc gemm: output-row indirection is not built for int8 or 4-bit weights");
+    if constexpr (KIND != KIND_I8 && KIND != KIND_W4 && KIND != KIND_FP8R)
+      return launch_epi<KIND, BN, EPI_ROWS>(mw, mx, p, grid, st);
+    else return fail(-2, "tc gemm: output-row indirection is not built for int8, 4-bit or rowwise fp8 weights");
   }
   return launch_epi<KIND, BN, EPI_PLAIN>(mw, mx, p, grid, st);
 }
@@ -798,6 +817,7 @@ int launch_kind(int kind, const void* x, int64_t x_rows, const void* w, int64_t 
   if (kind == KIND_FP8) return dispatch_bn<KIND_FP8>(BN, mw, mx, p, grid, st);
   if (kind == KIND_SOFT) return dispatch_bn<KIND_SOFT>(BN, mw, mx, p, grid, st);
   if (kind == KIND_W4) return dispatch_bn<KIND_W4>(BN, mw, mx, p, grid, st);
+  if (kind == KIND_FP8R) return dispatch_bn<KIND_FP8R>(BN, mw, mx, p, grid, st);
   return dispatch_bn<KIND_I8>(BN, mw, mx, p, grid, st);
 }
 
@@ -928,6 +948,18 @@ int tc_w4a16(const void* x, const void* qweight, const void* scales, const uint8
   p.out_dtype = dtype; p.residual = residual; p.out = y; p.act_pairs = pairs ? 1 : 0;
   p.w4_s = (const uint16_t*)scales; p.w4_z = zeros;
   return run(KIND_W4, x, qweight, p, ws, ws_bytes, st);
+}
+
+// FP8 W8A8, rowwise scales: y[M, N] = bf16((a . b^T) * a_s[m] * b_s[n] (+ bias[n])) (+ residual, one more rounding);
+// pairs: y[M, N/2] = SiluAndMul of the interleaved gate / up rows
+int tc_fp8_rowwise_gemm(const void* a, const float* a_s, const void* b, const float* b_s, const void* bias,
+                        const void* residual, void* y, int M, int N, int K, bool pairs, void* ws, int64_t ws_bytes,
+                        cudaStream_t st) {
+  Params p{};
+  p.M = M; p.N = N; p.K = K;
+  p.out_dtype = CB_BF16; p.a_s = a_s; p.b_s = b_s; p.bias = bias; p.residual = residual; p.out = y;
+  p.act_pairs = pairs ? 1 : 0;
+  return run(KIND_FP8R, a, b, p, ws, ws_bytes, st);
 }
 
 int tc_w8a8_gemm(void* out, const int8_t* a, const int8_t* b, const float* a_scales, const float* b_scales,

@@ -133,4 +133,35 @@ extern "C" int chitu_b200_w4a16_gemm_silu_pairs(const void* x, const void* qweig
                stream);
 }
 
+// FP8 W8A8 with rowwise scales, the Fp8LinearMethod / torch._scaled_mm(a, b.T, scale_a [M, 1], scale_b [1, N],
+// bias, out_dtype=bf16) interface of vLLM's per-channel FP8 checkpoints: e4m3 x e4m3 on the tensor cores, every 128-K
+// stage promoted into fp32, the two scales applied in the epilogue.  wgmma only; refusals name the entry and launch
+// nothing.
+static int fp8_rowwise(const char* entry, const void* a, const float* a_s, const void* b, const float* b_s,
+                       const void* bias, const void* residual, void* y, int M, int N, int K, bool pairs, void* workspace,
+                       int64_t workspace_bytes, void* stream) {
+  CB_ARG_AS(entry, a && a_s && b && b_s && y && M >= 0 && N > 0 && K > 0);
+  CB_ARG_AS(entry, ((uintptr_t)a | (uintptr_t)a_s | (uintptr_t)b | (uintptr_t)b_s | (uintptr_t)bias |
+                    (uintptr_t)residual | (uintptr_t)y) % 16 == 0);
+  CB_ARG_AS(entry, K % 16 == 0);
+  CB_ARG_AS(entry, !pairs || N % 2 == 0);
+  if (M == 0) return 0;
+  const int path = linear_path(entry, KIND_FP8R, 2, CB_BF16, M, N, K, workspace, workspace_bytes);
+  if (path != kWgmma) return path;
+  return tc_fp8_rowwise_gemm(a, a_s, b, b_s, bias, residual, y, M, N, K, pairs, workspace, workspace_bytes,
+                             (cudaStream_t)stream);
+}
+
+extern "C" int chitu_b200_fp8_rowwise_gemm(const void* a, const float* a_s, const void* b, const float* b_s,
+                                           const void* bias, const void* residual, void* y, int M, int N, int K,
+                                           void* workspace, int64_t workspace_bytes, void* stream) {
+  return fp8_rowwise(__func__, a, a_s, b, b_s, bias, residual, y, M, N, K, false, workspace, workspace_bytes, stream);
+}
+
+extern "C" int chitu_b200_fp8_rowwise_gemm_silu_pairs(const void* a, const float* a_s, const void* b, const float* b_s,
+                                                      void* y, int M, int N, int K, void* workspace,
+                                                      int64_t workspace_bytes, void* stream) {
+  return fp8_rowwise(__func__, a, a_s, b, b_s, nullptr, nullptr, y, M, N, K, true, workspace, workspace_bytes, stream);
+}
+
 CB_DEFINE_TL_SETTER(linear)

@@ -72,7 +72,8 @@ class DecodeEngine:
 
     linear_impl = 0          # `impl` of the bf16 linear entries: 0 = auto
     # "w4a16": the subclass's W4_LINEARS hold (qweight, scales, zeros) in quantize/w4a16.py's layout (stacked per expert
-    # for the MoE weights) and run on the 4-bit GEMMs
+    # for the MoE weights) and run on the 4-bit GEMMs; "fp8": they hold (weight e4m3, weight_scale fp32 [N]) in
+    # quantize/fp8.py's layout and run on the rowwise FP8 GEMMs
     weight_format = "bf16"
     W4_LINEARS = ()
 
@@ -116,20 +117,21 @@ class DecodeEngine:
         # only, never under a graph)
         self.capture_h = None
 
-    def _set_weight_format(self, weight_format: str, tp_size: int, process_group):
-        if weight_format not in ("bf16", "w4a16"):
-            raise ValueError(f"weight_format must be 'bf16' or 'w4a16', not {weight_format!r}")
-        if weight_format == "w4a16" and process_group is not None and tp_size > 1:
-            raise ValueError("weight_format='w4a16' runs on one GPU or one shard: the 4-bit GEMM has no push epilogue "
-                             "for the tensor-parallel all-reduce")
+    def _set_weight_format(self, weight_format: str, tp_size: int, process_group, formats=("bf16", "w4a16")):
+        if weight_format not in formats:
+            raise ValueError(f"weight_format must be one of {formats}, not {weight_format!r}")
+        if weight_format != "bf16" and process_group is not None and tp_size > 1:
+            raise ValueError(f"weight_format={weight_format!r} runs on one GPU or one shard: its GEMM has no push "
+                             "epilogue for the tensor-parallel all-reduce")
         self.weight_format = weight_format
 
     def _dequantized(self, lw: dict) -> dict:
-        """A copy of the layer's weights with the 4-bit ones as the bf16 values the kernels multiply (the oracle side of
-        the tests)."""
-        from .quantize.w4a16 import dequantize
+        """A copy of the layer's weights with the quantised ones as the values the kernels multiply (the oracle side of
+        the tests): bf16 for 4-bit weights, fp32 q * s for fp8 ones."""
+        from .quantize import fp8, w4a16
         d = dict(lw)
-        if self.weight_format == "w4a16":
+        if self.weight_format != "bf16":
+            dequantize = w4a16.dequantize if self.weight_format == "w4a16" else fp8.dequantize
             d.update({name: dequantize(*lw[name]) for name in self.W4_LINEARS})
         return d
 
@@ -165,16 +167,28 @@ class DecodeEngine:
                                               current_stream()), "linear_bf16")
 
     def _layer_linear(self, x, lw, name, y, M, residual=None):
-        """y = x . lw[name]^T (+ residual) in the engine's weight format."""
+        """y = x . lw[name]^T (+ residual) in the engine's weight format; fp8: x is the e4m3 self.xq with the per-token
+        scales in self.xs."""
         if self.weight_format == "bf16":
             return self._linear(x, lw[name], y, M, residual=residual)
+        if self.weight_format == "fp8":
+            q, s = lw[name]
+            check(self.lib.chitu_b200_fp8_rowwise_gemm(ptr(x), ptr(self.xs), ptr(q), ptr(s), None, ptr(residual), ptr(y),
+                                                       M, q.shape[0], q.shape[1], ptr(self.lin_ws), self.lin_ws.numel(),
+                                                       current_stream()), f"fp8 {name}")
+            return
         q, s, z = lw[name]
         check(self.lib.chitu_b200_w4a16_gemm(ptr(x), ptr(q), ptr(s), ptr(z), ptr(residual), ptr(y), M, q.shape[0],
                                              2 * q.shape[1], _lib.CB_BF16, ptr(self.lin_ws), self.lin_ws.numel(),
                                              current_stream()), f"w4a16 {name}")
 
     def _norm(self, x, w, y, q=None, qs=None):
-        assert q is None and qs is None, "this engine has no fp8 norm output"
+        """RMSNorm into bf16 `y`; with `q`, into the e4m3 `q` and per-token scales `qs` as well (y may then be None)."""
+        if q is not None:
+            check(self.lib.chitu_b200_rmsnorm_quant_fp8_rowwise(ptr(x), ptr(w), ptr(y), ptr(q), ptr(qs), self.B,
+                                                                self.cfg.dim, self.cfg.norm_eps, current_stream()),
+                  "rmsnorm_quant_fp8_rowwise")
+            return
         check(self.lib.chitu_b200_rmsnorm(ptr(x), ptr(w), ptr(y), self.B, self.cfg.dim, self.cfg.norm_eps, _lib.CB_BF16,
                                           current_stream()), "rmsnorm")
 
@@ -275,7 +289,13 @@ class LlamaDecodeEngine(DecodeEngine):
 
     weight_format="w4a16" holds qkv, o, w13 and w2 as 4-bit groups of 128 (quantize/w4a16.py's round-to-nearest rule
     applied to the same synthetic weights) and runs them through chitu_b200_w4a16_gemm[_silu_pairs]; embedding, head,
-    norms, rotary and attention stay bf16.  The W4 GEMM has no push epilogue, so it runs on one GPU or in shard mode."""
+    norms, rotary and attention stay bf16.  The W4 GEMM has no push epilogue, so it runs on one GPU or in shard mode.
+
+    weight_format="fp8" holds the same four linears as e4m3 with per-channel scales (quantize/fp8.py's rule applied to
+    the same synthetic weights) and runs them through chitu_b200_fp8_rowwise_gemm[_silu_pairs] on per-token e4m3
+    activations: the RMSNorms before qkv and w13 emit them (chitu_b200_rmsnorm_quant_fp8_rowwise), and the attention
+    output and the SiLU product are quantised by chitu_b200_quant_fp8_rowwise before wo and w2.  Embedding, head,
+    rotary, attention and the KV cache stay as in bf16; one GPU or shard mode, as for W4."""
 
     W4_LINEARS = ("wqkv", "wo", "w13", "w2")
 
@@ -283,9 +303,10 @@ class LlamaDecodeEngine(DecodeEngine):
                  seed: int = 0, tp_rank: int = 0, tp_size: int = 1, process_group=None, linear_impl: int = 0,
                  use_fused_allreduce: bool = True, kv_dtype: torch.dtype = BF, weight_format: str = "bf16"):
         D = cfg.head_dim
-        self._set_weight_format(weight_format, tp_size, process_group)
-        if weight_format == "w4a16" and linear_impl == 1:
-            raise ValueError("weight_format='w4a16' runs on the wgmma GEMM only (linear_impl=1 selects the SIMT GEMV)")
+        self._set_weight_format(weight_format, tp_size, process_group, formats=("bf16", "w4a16", "fp8"))
+        if weight_format != "bf16" and linear_impl == 1:
+            raise ValueError(f"weight_format={weight_format!r} runs on the wgmma GEMM only (linear_impl=1 selects the "
+                             "SIMT GEMV)")
         assert cfg.n_heads % tp_size == 0 and cfg.n_kv_heads % tp_size == 0
         self.Hq, self.Hkv, self.D = cfg.n_heads // tp_size, cfg.n_kv_heads // tp_size, D
         self.F = cfg.ffn_dim // tp_size
@@ -343,6 +364,15 @@ class LlamaDecodeEngine(DecodeEngine):
             for lw in self.layers:
                 for name in self.W4_LINEARS:
                     lw[name] = quantize_rtn(lw[name], BF)
+        if weight_format == "fp8":
+            # per-channel scales: w13's interleaved rows carry their own; the e4m3 activations and their per-token
+            # scales of whichever linear runs next
+            from .quantize.fp8 import quantize_weight
+            for lw in self.layers:
+                for name in self.W4_LINEARS:
+                    lw[name] = quantize_weight(lw[name])
+            self.xq = torch.zeros(B, max(dim, self.Hq * D, self.F), dtype=torch.float8_e4m3fn, device=dev)
+            self.xs = torch.zeros(B, dtype=torch.float32, device=dev)
         # rotary fused into the tensor-core decode kernel (head dim 128, power-of-two pages)
         self.fuse_rope = D == 128 and (page_size & (page_size - 1)) == 0 and self.Hq // self.Hkv in (1, 2, 4, 8)
         if self.kv_fp8 and not (self.fuse_rope and page_size % 64 == 0):
@@ -359,18 +389,30 @@ class LlamaDecodeEngine(DecodeEngine):
             out.append(d)
         return out
 
+    def _quant(self, x):
+        """The input of the linear that reads x: fp8 quantises x per token into self.xq / self.xs."""
+        if self.weight_format != "fp8":
+            return x
+        check(self.lib.chitu_b200_quant_fp8_rowwise(ptr(x), ptr(self.xq), ptr(self.xs), self.B, x.shape[1], None, None,
+                                                    current_stream()), "quant_fp8_rowwise")
+        return self.xq
+
     def _decode_layers(self):
         lib, B, D = self.lib, self.B, self.D
         st = current_stream()
         h, h2 = self.h, self.h2
         qkv_w = (self.Hq + 2 * self.Hkv) * D
         n_layers = len(self.layers)
-        self._norm(h, self.layers[0]["attn_norm"], self.xn)
+        # what the norms before qkv and w13 write, and what those linears read
+        fp8 = self.weight_format == "fp8"
+        norm_out, x_in = (dict(y=None, q=self.xq, qs=self.xs), self.xq) if fp8 else (dict(y=self.xn), self.xn)
+        self._norm(h, self.layers[0]["attn_norm"], **norm_out)
         for li, lw in enumerate(self.layers):
             if self.capture_h is not None:
                 self.capture_h.append(h.clone())
-            next_norm = self.layers[li + 1]["attn_norm"] if li + 1 < n_layers else self.norm
-            self._layer_linear(self.xn, lw, "wqkv", self.qkv, B)
+            last = li + 1 == n_layers
+            next_norm = self.norm if last else self.layers[li + 1]["attn_norm"]
+            self._layer_linear(x_in, lw, "wqkv", self.qkv, B)
             q_view, k_view = self.qkv, self.qkv[:, self.Hq * D:]
             v_view = self.qkv[:, (self.Hq + self.Hkv) * D:]
             if self.kv_fp8:
@@ -397,10 +439,17 @@ class LlamaDecodeEngine(DecodeEngine):
                     self.Hkv, D, self.page, self.max_seq_len, 1.0 / math.sqrt(D), ptr(self.attn_out), ptr(self.attn_ws),
                     self.attn_ws.numel(), _lib.CB_BF16, st), "gqa_paged_decode")
             # h2 = wo(o) + h
-            self._row_parallel(lambda out, res: self._layer_linear(self.attn_out, lw, "wo", out, B, residual=res),
+            self._row_parallel(lambda out, res: self._layer_linear(self._quant(self.attn_out), lw, "wo", out, B,
+                                                                   residual=res),
                                lambda: self.comm.linear_push(self.attn_out, lw["wo"], B, self.lin_ws),
-                               h, h2, lw["ffn_norm"], y=self.xn)
-            if self.weight_format == "w4a16":
+                               h, h2, lw["ffn_norm"], **norm_out)
+            if fp8:
+                q, s = lw["w13"]
+                check(lib.chitu_b200_fp8_rowwise_gemm_silu_pairs(ptr(self.xq), ptr(self.xs), ptr(q), ptr(s),
+                                                                 ptr(self.act), B, 2 * self.F, self.cfg.dim,
+                                                                 ptr(self.lin_ws), self.lin_ws.numel(), st),
+                      "fp8 w13 + silu")
+            elif self.weight_format == "w4a16":
                 q, s, z = lw["w13"]
                 check(lib.chitu_b200_w4a16_gemm_silu_pairs(ptr(self.xn), ptr(q), ptr(s), ptr(z), ptr(self.act), B,
                                                            2 * self.F, self.cfg.dim, _lib.CB_BF16, ptr(self.lin_ws),
@@ -412,9 +461,10 @@ class LlamaDecodeEngine(DecodeEngine):
             else:
                 self._linear(self.xn, lw["w13"], self.gate_up, B)
                 check(lib.chitu_b200_silu_and_mul(ptr(self.gate_up), ptr(self.act), B, self.F, _lib.CB_BF16, st), "silu")
-            # h = w2(act) + h2
-            self._row_parallel(lambda out, res: self._layer_linear(self.act, lw, "w2", out, B, residual=res),
+            # h = w2(act) + h2; the head reads the final norm in bf16
+            self._row_parallel(lambda out, res: self._layer_linear(self._quant(self.act), lw, "w2", out, B,
+                                                                   residual=res),
                                lambda: self.comm.linear_push(self.act, lw["w2"], B, self.lin_ws),
-                               h2, h, next_norm, y=self.xn)
+                               h2, h, next_norm, **(dict(y=self.xn) if last else norm_out))
         if self.capture_h is not None:
             self.capture_h.append(h.clone())

@@ -152,6 +152,18 @@ int chitu_b200_act_quant_fp8(const void* x, void* y, float* s, int64_t rows, int
  * q = int8(round_half_even(x/scale)). x is fp16 or bf16. */
 int chitu_b200_quant_act_int8(const void* x, int8_t* q, float* scales, int64_t rows, int K,
                               int dtype, void* stream);
+/* Per-token e4m3 quantisation of bf16 rows, the rule of vLLM's QuantFP8(GroupShape.PER_TOKEN).forward_native:
+ * dynamic (scale == NULL): s[r] = max(min(max_k |x[r,k]|, *scale_ub) / 448, 1 / (448*512)) in fp32, the upper bound
+ * only when scale_ub != NULL; static: s[r] = *scale for every row.  q = e4m3_rn(clamp(fp32(x) * rcp_rn(s[r]), +-448)).
+ * x [rows, K] bf16, q [rows, K] e4m3, q_scales [rows] fp32; scale and scale_ub are fp32 device scalars.  K % 16 == 0,
+ * x and q 16-byte aligned; a static scale with an upper bound is refused. */
+int chitu_b200_quant_fp8_rowwise(const void* x, void* q, float* q_scales, int64_t rows, int K, const float* scale,
+                                 const float* scale_ub, void* stream);
+/* RMSNorm followed by the dynamic per-token quantisation above, in one launch and bit for bit chitu_b200_rmsnorm and
+ * chitu_b200_quant_fp8_rowwise in sequence: q [rows, dim] e4m3 and q_scales [rows] from the bf16-rounded norm output,
+ * which is also written to y unless y is NULL.  bf16, dim <= 8192. */
+int chitu_b200_rmsnorm_quant_fp8_rowwise(const void* x, const void* w, void* y, void* q, float* q_scales, int rows,
+                                         int dim, float eps, void* stream);
 /* weight_dequant_deepseek_v3 / weight_dequant_soft_fp8_deepseek_v3 (ops.py:356-449):
  * y[b,m,n] = fp8(x[b,m,n]) * s[b, m/128, n/128]  -> bf16.  soft != 0 reproduces the
  * bit-trick path ((x&0x80)<<24 | (x&0x7f)<<20) * (s * 2^120).  The kernel does not let the next kernel of the stream
@@ -220,6 +232,24 @@ int chitu_b200_w4a16_gemm(const void* x, const void* qweight, const void* scales
 int chitu_b200_w4a16_gemm_silu_pairs(const void* x, const void* qweight, const void* scales, const uint8_t* zeros,
                                      void* y, int M, int N, int K, int dtype, void* workspace, int64_t workspace_bytes,
                                      void* stream);
+
+/* FP8 W8A8 with rowwise scales (vLLM Fp8LinearMethod for compressed-tensors FP8 / FP8_DYNAMIC and fbgemm rowwise
+ * checkpoints; torch._scaled_mm(a, b.T, scale_a [M,1], scale_b [1,N], bias, out_dtype=bf16)):
+ *   y[m,n] = bf16((sum_k a[m,k] b[n,k]) * a_s[m] * b_s[n] (+ bias[n])), residual [M,N] (or NULL) added after that
+ *   rounding; a [M,K] and b [N,K] e4m3, a_s [M] and b_s [N] fp32, bias [N] bf16 or NULL.
+ * Every 128 K-elements are summed by the tensor cores and then added into an fp32 accumulator; the scales are applied
+ * once, (acc * a_s) * b_s.  wgmma path only, sharing chitu_b200_linear_workspace_bytes: where it cannot run (shape or
+ * workspace) the entries return -2 and launch nothing.  Refused before any launch, under the entry's name: a NULL
+ * operand, a base that is not 16-byte aligned, K % 16 != 0, an odd N for the pairs entry.  M == 0 launches nothing.
+ * b and b_s are weights under the weight contract above; a_s is read after griddepcontrol.wait, so the quantiser that
+ * writes a and a_s may directly precede the GEMM. */
+int chitu_b200_fp8_rowwise_gemm(const void* a, const float* a_s, const void* b, const float* b_s, const void* bias,
+                                const void* residual, void* y, int M, int N, int K, void* workspace,
+                                int64_t workspace_bytes, void* stream);
+/* The gate_up linear + SiluAndMul of chitu_b200_linear_bf16_silu_pairs on rowwise fp8 weights: rows 2i / 2i+1 of b
+ * (each with its own b_s) are gate_i / up_i; y [M, N/2] bf16 with the roundings of the two separate ops. */
+int chitu_b200_fp8_rowwise_gemm_silu_pairs(const void* a, const float* a_s, const void* b, const float* b_s, void* y,
+                                           int M, int N, int K, void* workspace, int64_t workspace_bytes, void* stream);
 
 /* ---- decode attention -------------------------------------------------------------------- */
 /* Workspace sizing for split-KV partials. */
