@@ -164,7 +164,42 @@ __global__ void __launch_bounds__(kThreads) sample_kernel(const T* __restrict__ 
   }
 }
 
+// Greedy acceptance of k draft tokens per request, one thread per request.  It writes seq_lens, which the decode kernels
+// read before their griddepcontrol.wait, so it waits for its predecessor and never lets its dependents start early
+// (the rule of decode_prepare_kernel).
+__global__ void spec_accept_greedy_kernel(const int64_t* __restrict__ target, const int64_t* __restrict__ drafts,
+                                          const int32_t* __restrict__ n_draft, int32_t* __restrict__ seq_lens,
+                                          int64_t* __restrict__ out_tokens, int32_t* __restrict__ accepted,
+                                          int64_t* __restrict__ next_tokens, int B, int k) {
+  cb::pdl_wait();
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  const int64_t* t = target + (int64_t)b * (k + 1);
+  const int64_t* d = drafts + (int64_t)b * k;
+  const int n = min(max(n_draft[b], 0), k);
+  int a = 0;
+  while (a < n && d[a] == t[a]) ++a;
+  int64_t* o = out_tokens + (int64_t)b * (k + 1);
+  for (int i = 0; i <= k; ++i) o[i] = i <= a ? t[i] : -1;
+  accepted[b] = a;
+  next_tokens[b] = t[a];
+  seq_lens[b] += a + 1;
+}
+
 }  // namespace
+
+// target int64 [B, k + 1], drafts int64 [B, k], n_draft int32 [B] (clamped to 0..k), seq_lens int32 [B] (in place);
+// out_tokens int64 [B, k + 1], accepted int32 [B], next_tokens int64 [B].
+extern "C" int chitu_b200_spec_accept_greedy(const int64_t* target, const int64_t* drafts, const int32_t* n_draft,
+                                             int32_t* seq_lens, int64_t* out_tokens, int32_t* accepted,
+                                             int64_t* next_tokens, int B, int k, void* stream) {
+  CB_ARG(target && drafts && n_draft && seq_lens && out_tokens && accepted && next_tokens && B >= 0 && k >= 1);
+  if (B == 0) return 0;
+  cb::launch_k(spec_accept_greedy_kernel, dim3(cb::cdiv(B, 128)), dim3(128), 0, (cudaStream_t)stream, target, drafts,
+               n_draft, seq_lens, out_tokens, accepted, next_tokens, B, k);
+  CB_LAUNCHED(1);
+  return 0;
+}
 
 // logits [B, V] (row stride in elements), bf16 / fp16 / fp32; temperatures, top_ps, uniforms fp32 [B]; top_ks int32 [B]
 // (<= 0: no top-k); out_tokens int64 [B]; out_kept / out_mass (optional, diagnostics): size and mass of the kept set.

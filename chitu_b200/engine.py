@@ -78,10 +78,13 @@ class DecodeEngine:
     W4_LINEARS = ()
 
     def __init__(self, cfg, max_reqs: int, max_seq_len: int, device, page_size: int, seed: int, tp_rank: int,
-                 tp_size: int, process_group, use_fused_allreduce: bool, attn_ws: tuple, lin_n: int):
+                 tp_size: int, process_group, use_fused_allreduce: bool, attn_ws: tuple, lin_n: int, max_draft: int = 0):
         """attn_ws: (heads, head_dim_v, max_splits) the attention workspace is sized for; lin_n: the widest N the
-        linear workspace is sized for."""
+        linear workspace is sized for; max_draft: the draft tokens per request a verify step checks (0: none), which
+        sizes the row buffers for max_reqs * (max_draft + 1) rows."""
         self.cfg, self.B, self.device = cfg, max_reqs, torch.device(device)
+        self.max_draft = max_draft
+        rows = max_reqs * (max_draft + 1)         # rows of the widest step: the decode step's B, or a verify step's
         self.tp_rank, self.tp_size, self.pg = tp_rank, tp_size, process_group
         self.tp_on = process_group is not None and tp_size > 1
         self.lib = _lib.load()
@@ -95,14 +98,14 @@ class DecodeEngine:
         self.seq_lens = torch.zeros(max_reqs, dtype=torch.int32, device=dev)
         # persistent step I/O and residual stream (CUDA-graph safe)
         self.tokens = torch.zeros(B, dtype=torch.int64, device=dev)
-        self.h, self.h2, self.xn = (torch.zeros(B, dim, dtype=BF, device=dev) for _ in range(3))
-        self.logits = torch.zeros(B, cfg.vocab_size // tp_size, dtype=BF, device=dev)
+        self.h, self.h2, self.xn = (torch.zeros(rows, dim, dtype=BF, device=dev) for _ in range(3))
+        self.logits = torch.zeros(rows, cfg.vocab_size // tp_size, dtype=BF, device=dev)
         self.next_tokens = torch.zeros(B, dtype=torch.int64, device=dev)
         self.tp_gather = torch.empty(tp_size, B, 2, dtype=torch.float32, device=dev) if self.tp_on else None
         heads, head_dim_v, max_splits = attn_ws
         self.attn_ws = torch.zeros(self.lib.chitu_b200_attn_workspace_bytes(B, heads, head_dim_v, max_splits),
                                    dtype=torch.uint8, device=dev)
-        self.lin_ws = torch.zeros(max(self.lib.chitu_b200_linear_workspace_bytes(B, lin_n), 256), dtype=torch.uint8,
+        self.lin_ws = torch.zeros(max(self.lib.chitu_b200_linear_workspace_bytes(rows, lin_n), 256), dtype=torch.uint8,
                                   device=dev)                    # split-K tickets start at 0
         # push mode: the row-parallel GEMM's epilogue starts the all-reduce; "0" selects the pull kernel
         self.ar_push = os.environ.get("CHITU_B200_AR_PUSH", "1") != "0"
@@ -110,7 +113,7 @@ class DecodeEngine:
         self.comm = None
         if self.tp_on and use_fused_allreduce:
             from .comm import FusedAllReduce
-            self.comm = FusedAllReduce(process_group, max_reqs, dim, dev)
+            self.comm = FusedAllReduce(process_group, rows, dim, dev)
         self.graph = None
         self.launches_per_step = 0
         # set to [] to record the residual stream entering every layer, and the last layer's output (tests; eager steps
@@ -182,32 +185,34 @@ class DecodeEngine:
                                              2 * q.shape[1], _lib.CB_BF16, ptr(self.lin_ws), self.lin_ws.numel(),
                                              current_stream()), f"w4a16 {name}")
 
-    def _norm(self, x, w, y, q=None, qs=None):
-        """RMSNorm into bf16 `y`; with `q`, into the e4m3 `q` and per-token scales `qs` as well (y may then be None)."""
+    def _norm(self, x, w, y, q=None, qs=None, rows=None):
+        """RMSNorm of `rows` rows (default B) into bf16 `y`; with `q`, into the e4m3 `q` and per-token scales `qs` as
+        well (y may then be None)."""
+        M = self.B if rows is None else rows
         if q is not None:
-            check(self.lib.chitu_b200_rmsnorm_quant_fp8_rowwise(ptr(x), ptr(w), ptr(y), ptr(q), ptr(qs), self.B,
+            check(self.lib.chitu_b200_rmsnorm_quant_fp8_rowwise(ptr(x), ptr(w), ptr(y), ptr(q), ptr(qs), M,
                                                                 self.cfg.dim, self.cfg.norm_eps, current_stream()),
                   "rmsnorm_quant_fp8_rowwise")
             return
-        check(self.lib.chitu_b200_rmsnorm(ptr(x), ptr(w), ptr(y), self.B, self.cfg.dim, self.cfg.norm_eps, _lib.CB_BF16,
+        check(self.lib.chitu_b200_rmsnorm(ptr(x), ptr(w), ptr(y), M, self.cfg.dim, self.cfg.norm_eps, _lib.CB_BF16,
                                           current_stream()), "rmsnorm")
 
     def _allreduce(self, t):
         if self.tp_on:
             torch.distributed.all_reduce(t, group=self.pg)
 
-    def _row_parallel(self, gemm, push, residual, h_out, norm_w, y=None, q=None, qs=None, partial=None):
+    def _row_parallel(self, gemm, push, residual, h_out, norm_w, y=None, q=None, qs=None, partial=None, rows=None):
         """h_out = residual + the sum over ranks of a row-parallel product, then RMSNorm(h_out) * norm_w into the
-        wanted outputs (bf16 `y`, fp8 `q` + scales `qs`).
+        wanted outputs (bf16 `y`, fp8 `q` + scales `qs`), over `rows` rows (default B).
 
         `gemm(out, residual)` writes this rank's product into `out`, adding `residual` when it is given; `push()` is the
         same product with the epilogue that starts the fused all-reduce.  Single GPU (and shard mode) fuses the residual
         into the GEMM; tensor parallel reduces by push + consume, by the fused pull kernel, or by NCCL + add + norm,
         with this rank's product in `partial` (default: `h_out`)."""
-        B, dim, eps = self.B, self.cfg.dim, self.cfg.norm_eps
+        B, dim, eps = self.B if rows is None else rows, self.cfg.dim, self.cfg.norm_eps
         if not self.tp_on:
             gemm(h_out, residual)
-            self._norm(h_out, norm_w, y, q, qs)
+            self._norm(h_out, norm_w, y, q, qs, rows=B)
         elif self.comm is not None and self.ar_push:
             push()
             self.comm.consume(residual, h_out, norm_w, y, q, qs, B, dim, eps)
@@ -220,7 +225,7 @@ class DecodeEngine:
                 self._allreduce(partial)
                 check(self.lib.chitu_b200_add(ptr(partial), ptr(residual), ptr(h_out), B * dim, _lib.CB_BF16,
                                               current_stream()), "add")
-                self._norm(h_out, norm_w, y, q, qs)
+                self._norm(h_out, norm_w, y, q, qs, rows=B)
 
     def _step_body(self):
         lib, B, cfg = self.lib, self.B, self.cfg
@@ -239,29 +244,34 @@ class DecodeEngine:
         if self.tp_on:
             # vocab-parallel head: the reference all-gathers the logits shards before sampling
             # (tensor_parallel.py:94-102); the same token from a (max, index) all-gather of B*8 bytes per rank
-            self.next_tokens.copy_(global_argmax(self.logits, self.next_tokens, self.tp_rank, vocab_local, self.pg,
+            self.next_tokens.copy_(global_argmax(self.logits[:B], self.next_tokens, self.tp_rank, vocab_local, self.pg,
                                                  self.tp_gather))
         self.seq_lens.add_(1)     # finalize_cache_single_decode (cache_manager.py)
 
-    def capture(self):
-        """Capture the decode step in a CUDA graph (models/model.py:572-611)."""
+    def _capture(self, body):
+        """(a CUDA graph of `body`, the launches it holds); seq_lens is restored after the warm-up and the capture."""
         torch.cuda.synchronize(self.device)
         saved = self.seq_lens.clone()
         s = torch.cuda.Stream(device=self.device)
         s.wait_stream(torch.cuda.current_stream(self.device))
         with torch.cuda.stream(s):
             for _ in range(2):
-                self._step_body()         # warm-up outside capture
+                body()                    # warm-up outside capture
         torch.cuda.current_stream(self.device).wait_stream(s)
         torch.cuda.synchronize(self.device)
         self.seq_lens.copy_(saved)
         before = _lib.launch_count()
-        self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph):
-            self._step_body()
-        self.launches_per_step = _lib.launch_count() - before
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph):
+            body()
+        launches = _lib.launch_count() - before
         self.seq_lens.copy_(saved)
         torch.cuda.synchronize(self.device)
+        return graph, launches
+
+    def capture(self):
+        """Capture the decode step in a CUDA graph (models/model.py:572-611)."""
+        self.graph, self.launches_per_step = self._capture(self._step_body)
 
     def step(self):
         """One decode step over the persistent buffers (tokens in self.tokens)."""
@@ -295,13 +305,19 @@ class LlamaDecodeEngine(DecodeEngine):
     the same synthetic weights) and runs them through chitu_b200_fp8_rowwise_gemm[_silu_pairs] on per-token e4m3
     activations: the RMSNorms before qkv and w13 emit them (chitu_b200_rmsnorm_quant_fp8_rowwise), and the attention
     output and the SiLU product are quantised by chitu_b200_quant_fp8_rowwise before wo and w2.  Embedding, head,
-    rotary, attention and the KV cache stay as in bf16; one GPU or shard mode, as for W4."""
+    rotary, attention and the KV cache stay as in bf16; one GPU or shard mode, as for W4.
+
+    max_draft=k > 0 adds a speculative verify step (`verify`, `capture_verify`): every request's token and up to k draft
+    tokens run through the model as B * (k + 1) rows with causal attention over the cache, and the greedy acceptance
+    kernel advances `seq_lens` on the device.  The row buffers are then sized for B * (k + 1) rows; the decode step is
+    unchanged."""
 
     W4_LINEARS = ("wqkv", "wo", "w13", "w2")
 
     def __init__(self, cfg: LlamaConfig, max_reqs: int, max_seq_len: int, device="cuda:0", page_size: int = 256,
                  seed: int = 0, tp_rank: int = 0, tp_size: int = 1, process_group=None, linear_impl: int = 0,
-                 use_fused_allreduce: bool = True, kv_dtype: torch.dtype = BF, weight_format: str = "bf16"):
+                 use_fused_allreduce: bool = True, kv_dtype: torch.dtype = BF, weight_format: str = "bf16",
+                 max_draft: int = 0):
         D = cfg.head_dim
         self._set_weight_format(weight_format, tp_size, process_group, formats=("bf16", "w4a16", "fp8"))
         if weight_format != "bf16" and linear_impl == 1:
@@ -311,9 +327,22 @@ class LlamaDecodeEngine(DecodeEngine):
         self.Hq, self.Hkv, self.D = cfg.n_heads // tp_size, cfg.n_kv_heads // tp_size, D
         self.F = cfg.ffn_dim // tp_size
         self.linear_impl = linear_impl
+        if max_draft < 0:
+            raise ValueError(f"max_draft must be >= 0, not {max_draft}")
+        if max_draft > 0:
+            # what the multi-token attention kernels are built for, and the rows one GEMM token tile set and the
+            # all-reduce kernels take
+            if linear_impl == 1:
+                raise ValueError("the verify step runs on the wgmma GEMMs (linear_impl=1 selects the SIMT GEMV)")
+            if D != 128 or page_size % 64 != 0 or self.Hq // self.Hkv not in (1, 2, 4, 8):
+                raise ValueError("the verify step needs head dim 128, Hq / Hkv in {1, 2, 4, 8} and a page that is a "
+                                 f"multiple of 64 (head dim {D}, page {page_size})")
+            if max_reqs * (max_draft + 1) > 256:
+                raise ValueError(f"the verify step runs at most 256 rows: max_reqs * (max_draft + 1) = "
+                                 f"{max_reqs * (max_draft + 1)}")
         super().__init__(cfg, max_reqs, max_seq_len, device, page_size, seed, tp_rank, tp_size, process_group,
                          use_fused_allreduce, attn_ws=(self.Hq, D, 64),
-                         lin_n=max(2 * self.F, cfg.vocab_size // tp_size))
+                         lin_n=max(2 * self.F, cfg.vocab_size // tp_size), max_draft=max_draft)
         dev, g, dim = self.device, self.g, cfg.dim
 
         def rnd(*shape, scale=0.02):
@@ -343,13 +372,32 @@ class LlamaDecodeEngine(DecodeEngine):
         # precompute_freqs_cis (models/model.py:81-89) as cos/sin tables
         freqs = 1.0 / (cfg.rope_theta ** (torch.arange(0, D, 2)[: D // 2].float() / D))
         self._rope_tables(torch.outer(torch.arange(max_seq_len * 2, dtype=torch.float32), freqs))
-        B = max_reqs
+        B = max_reqs * (max_draft + 1)                     # rows of the widest step
         self.qkv = torch.zeros(B, (self.Hq + 2 * self.Hkv) * D, dtype=BF, device=dev)
         self.q_rot = torch.zeros(B, self.Hq, D, dtype=BF, device=dev)
         self.k_rot = torch.zeros(B, self.Hkv, D, dtype=BF, device=dev)
         self.attn_out = torch.zeros(B, self.Hq * D, dtype=BF, device=dev)
         self.gate_up = torch.zeros(B, 2 * self.F, dtype=BF, device=dev)
         self.act = torch.zeros(B, self.F, dtype=BF, device=dev)
+        self.verify_graph = None
+        self.launches_per_verify = 0
+        if max_draft > 0:
+            # verify step I/O: [tokens | drafts] per request, the positions and rotary rows of its B * (k + 1) rows, the
+            # argmax at each row, the acceptance outputs; its attention workspace splits B * (k + 1) query rows
+            k, R = max_draft, B
+            self.draft_tokens = torch.zeros(max_reqs, k, dtype=torch.int64, device=dev)
+            self.n_draft = torch.zeros(max_reqs, dtype=torch.int32, device=dev)
+            self.verify_tokens = torch.zeros(max_reqs, k + 1, dtype=torch.int64, device=dev)
+            self.verify_offsets = torch.arange(k + 1, dtype=torch.int32, device=dev)
+            self.verify_pos = torch.zeros(max_reqs, k + 1, dtype=torch.int32, device=dev)
+            self.verify_cos = torch.zeros(R, D // 2, dtype=torch.float32, device=dev)
+            self.verify_sin = torch.zeros_like(self.verify_cos)
+            self.target = torch.zeros(max_reqs, k + 1, dtype=torch.int64, device=dev)
+            self.out_tokens = torch.zeros(max_reqs, k + 1, dtype=torch.int64, device=dev)
+            self.accepted = torch.zeros(max_reqs, dtype=torch.int32, device=dev)
+            self.verify_gather = torch.empty(tp_size, R, 2, dtype=torch.float32, device=dev) if self.tp_on else None
+            self.verify_attn_ws = torch.zeros(self.lib.chitu_b200_attn_workspace_bytes(R, self.Hq, D, 64),
+                                              dtype=torch.uint8, device=dev)
         # SiluAndMul inside the w13 GEMM epilogue: the merged gate/up weight is stored with its rows interleaved
         # (row 2i = gate_i, row 2i+1 = up_i) — a load-time permutation of the reference's merged tensor.
         # It and push mode need the wgmma GEMM, which linear_impl=1 (the SIMT GEMV) turns off.
@@ -389,16 +437,41 @@ class LlamaDecodeEngine(DecodeEngine):
             out.append(d)
         return out
 
-    def _quant(self, x):
-        """The input of the linear that reads x: fp8 quantises x per token into self.xq / self.xs."""
+    def _quant(self, x, rows):
+        """The input of the linear that reads the first `rows` rows of x: fp8 quantises them per token into self.xq /
+        self.xs."""
         if self.weight_format != "fp8":
             return x
-        check(self.lib.chitu_b200_quant_fp8_rowwise(ptr(x), ptr(self.xq), ptr(self.xs), self.B, x.shape[1], None, None,
+        check(self.lib.chitu_b200_quant_fp8_rowwise(ptr(x), ptr(self.xq), ptr(self.xs), rows, x.shape[1], None, None,
                                                     current_stream()), "quant_fp8_rowwise")
         return self.xq
 
-    def _decode_layers(self):
-        lib, B, D = self.lib, self.B, self.D
+    def _verify_attention(self, li, sq):
+        """Rotary over the B * sq rows, then causal attention of each request's sq queries over its cache and its sq
+        new K / V rows, which are appended at seq_lens[b] .. seq_lens[b] + sq - 1."""
+        lib, B, D, st = self.lib, self.B, self.D, current_stream()
+        qkv_w = (self.Hq + 2 * self.Hkv) * D
+        M = B * sq
+        check(lib.chitu_b200_rotary_interleaved(ptr(self.qkv), ptr(self.qkv[:, self.Hq * D:]), ptr(self.q_rot),
+                                                ptr(self.k_rot), ptr(self.verify_cos), ptr(self.verify_sin), M, self.Hq,
+                                                self.Hkv, D, qkv_w, D, qkv_w, D, _lib.CB_BF16, st), "rotary")
+        v_view = self.qkv[:, (self.Hq + self.Hkv) * D:]
+        kv_strides = (sq * self.Hkv * D, self.Hkv * D, sq * qkv_w, qkv_w)
+        tail = (ptr(self.seq_lens), ptr(self.block_table), self.max_blocks, B, sq, self.Hq, self.Hkv, D, self.page,
+                self.k_cache.shape[1], self.max_seq_len, 1, 1.0 / math.sqrt(D), ptr(self.attn_out),
+                ptr(self.verify_attn_ws), self.verify_attn_ws.numel(), _lib.CB_BF16, st)
+        if self.kv_fp8:
+            check(lib.chitu_b200_gqa_paged_attn_fp8kv(ptr(self.q_rot), sq * self.Hq * D, ptr(self.k_cache[li]),
+                                                      ptr(self.v_cache[li]), ptr(self.k_rot), ptr(v_view), *kv_strides,
+                                                      None, None, *tail), "gqa_paged_attn_fp8kv")
+        else:
+            check(lib.chitu_b200_gqa_paged_prefill(ptr(self.q_rot), ptr(self.k_cache[li]), ptr(self.v_cache[li]),
+                                                   ptr(self.k_rot), ptr(v_view), *kv_strides, *tail),
+                  "gqa_paged_prefill")
+
+    def _decode_layers(self, sq=1):
+        """The layers over B * sq rows: the decode step (sq = 1) or the verify step (sq = max_draft + 1)."""
+        lib, B, D = self.lib, self.B * sq, self.D
         st = current_stream()
         h, h2 = self.h, self.h2
         qkv_w = (self.Hq + 2 * self.Hkv) * D
@@ -406,7 +479,7 @@ class LlamaDecodeEngine(DecodeEngine):
         # what the norms before qkv and w13 write, and what those linears read
         fp8 = self.weight_format == "fp8"
         norm_out, x_in = (dict(y=None, q=self.xq, qs=self.xs), self.xq) if fp8 else (dict(y=self.xn), self.xn)
-        self._norm(h, self.layers[0]["attn_norm"], **norm_out)
+        self._norm(h, self.layers[0]["attn_norm"], **norm_out, rows=B)
         for li, lw in enumerate(self.layers):
             if self.capture_h is not None:
                 self.capture_h.append(h.clone())
@@ -415,7 +488,9 @@ class LlamaDecodeEngine(DecodeEngine):
             self._layer_linear(x_in, lw, "wqkv", self.qkv, B)
             q_view, k_view = self.qkv, self.qkv[:, self.Hq * D:]
             v_view = self.qkv[:, (self.Hq + self.Hkv) * D:]
-            if self.kv_fp8:
+            if sq > 1:
+                self._verify_attention(li, sq)
+            elif self.kv_fp8:
                 # the same fused rotary over the e4m3 caches; the new k / v rows are rounded to e4m3 as they are stored
                 check(lib.chitu_b200_gqa_paged_attn_fp8kv(
                     ptr(q_view), qkv_w, ptr(self.k_cache[li]), ptr(self.v_cache[li]), ptr(k_view), ptr(v_view), qkv_w, 0,
@@ -439,10 +514,10 @@ class LlamaDecodeEngine(DecodeEngine):
                     self.Hkv, D, self.page, self.max_seq_len, 1.0 / math.sqrt(D), ptr(self.attn_out), ptr(self.attn_ws),
                     self.attn_ws.numel(), _lib.CB_BF16, st), "gqa_paged_decode")
             # h2 = wo(o) + h
-            self._row_parallel(lambda out, res: self._layer_linear(self._quant(self.attn_out), lw, "wo", out, B,
+            self._row_parallel(lambda out, res: self._layer_linear(self._quant(self.attn_out, B), lw, "wo", out, B,
                                                                    residual=res),
                                lambda: self.comm.linear_push(self.attn_out, lw["wo"], B, self.lin_ws),
-                               h, h2, lw["ffn_norm"], **norm_out)
+                               h, h2, lw["ffn_norm"], **norm_out, rows=B)
             if fp8:
                 q, s = lw["w13"]
                 check(lib.chitu_b200_fp8_rowwise_gemm_silu_pairs(ptr(self.xq), ptr(self.xs), ptr(q), ptr(s),
@@ -462,9 +537,83 @@ class LlamaDecodeEngine(DecodeEngine):
                 self._linear(self.xn, lw["w13"], self.gate_up, B)
                 check(lib.chitu_b200_silu_and_mul(ptr(self.gate_up), ptr(self.act), B, self.F, _lib.CB_BF16, st), "silu")
             # h = w2(act) + h2; the head reads the final norm in bf16
-            self._row_parallel(lambda out, res: self._layer_linear(self._quant(self.act), lw, "w2", out, B,
+            self._row_parallel(lambda out, res: self._layer_linear(self._quant(self.act, B), lw, "w2", out, B,
                                                                    residual=res),
                                lambda: self.comm.linear_push(self.act, lw["w2"], B, self.lin_ws),
-                               h2, h, next_norm, **(dict(y=self.xn) if last else norm_out))
+                               h2, h, next_norm, **(dict(y=self.xn) if last else norm_out), rows=B)
         if self.capture_h is not None:
             self.capture_h.append(h.clone())
+
+    # ---- speculative verify step ------------------------------------------------------------------
+    def _verify_body(self):
+        lib, B, k, cfg = self.lib, self.B, self.max_draft, self.cfg
+        M, st = B * (k + 1), current_stream()
+        self.verify_tokens[:, 0].copy_(self.tokens)
+        self.verify_tokens[:, 1:].copy_(self.draft_tokens)
+        # row b * (k + 1) + i sits at position seq_lens[b] + i
+        torch.add(self.seq_lens.view(B, 1), self.verify_offsets, out=self.verify_pos)
+        torch.index_select(self.cos_table, 0, self.verify_pos.view(-1), out=self.verify_cos)
+        torch.index_select(self.sin_table, 0, self.verify_pos.view(-1), out=self.verify_sin)
+        check(lib.chitu_b200_embedding(ptr(self.verify_tokens), ptr(self.embed), ptr(self.h), M, cfg.dim, 0,
+                                       cfg.vocab_size, _lib.CB_BF16, st), "embedding")
+        self._decode_layers(sq=k + 1)
+        self._linear(self.xn, self.head, self.logits, M)
+        vocab_local = self.head.shape[0]
+        check(lib.chitu_b200_argmax(ptr(self.logits), ptr(self.target), M, vocab_local, _lib.CB_BF16, st), "argmax")
+        if self.tp_on:
+            self.target.view(-1).copy_(global_argmax(self.logits, self.target.view(-1), self.tp_rank, vocab_local,
+                                                     self.pg, self.verify_gather))
+        check(lib.chitu_b200_spec_accept_greedy(ptr(self.target), ptr(self.draft_tokens), ptr(self.n_draft),
+                                                ptr(self.seq_lens), ptr(self.out_tokens), ptr(self.accepted),
+                                                ptr(self.next_tokens), B, k, st), "spec_accept_greedy")
+
+    def _need_verify(self):
+        if self.max_draft == 0:
+            raise ValueError("this engine has no verify step: build it with max_draft > 0")
+
+    def capture_verify(self):
+        """Capture the verify step in a CUDA graph of its own (the decode step's graph is separate)."""
+        self._need_verify()
+        self.verify_graph, self.launches_per_verify = self._capture(self._verify_body)
+
+    def verify_step(self):
+        """One verify step over the persistent buffers (tokens in self.tokens, drafts in self.draft_tokens / n_draft)."""
+        self._need_verify()
+        if self.verify_graph is not None:
+            self.verify_graph.replay()
+        else:
+            before = _lib.launch_count()
+            self._verify_body()
+            self.launches_per_verify = _lib.launch_count() - before
+
+    def verify(self, tokens_host: torch.Tensor, drafts_host: torch.Tensor, n_draft_host: torch.Tensor):
+        """Greedy speculative verification.  tokens_host int64 [B]: each request's last token (what `decode` takes);
+        drafts_host int64 [B, k'] with k' <= max_draft: the proposed continuations; n_draft_host int32 [B] in 0..k':
+        how many of a request's drafts to check.  One step runs every request's token and drafts through the model
+        (positions seq_lens[b] .. seq_lens[b] + max_draft), accepts the leading drafts equal to the model's greedy
+        choice and advances seq_lens by the accepted count + 1 on the device.
+
+        Returns host (out_tokens int64 [B, max_draft + 1]: the accepted drafts then the model's next token, -1 after;
+        accepted int32 [B]).  self.next_tokens holds each request's last emitted token, the input of the next step.
+        K / V rows are written for all max_draft + 1 positions; those past the accepted ones stay beyond seq_lens and are
+        overwritten by later steps.  The caller keeps seq_lens[b] + max_draft + 1 <= max_seq_len, and the cache pages
+        for those positions in the block table."""
+        self._need_verify()
+        B, k = self.B, self.max_draft
+        drafts_host = torch.as_tensor(drafts_host)
+        n_draft_host = torch.as_tensor(n_draft_host)
+        if tuple(torch.as_tensor(tokens_host).shape) != (B,):
+            raise ValueError(f"tokens must be [{B}], not {tuple(torch.as_tensor(tokens_host).shape)}")
+        if drafts_host.dim() != 2 or drafts_host.shape[0] != B or drafts_host.shape[1] > k:
+            raise ValueError(f"drafts must be [{B}, k'] with k' <= max_draft = {k}, not {tuple(drafts_host.shape)}")
+        if tuple(n_draft_host.shape) != (B,):
+            raise ValueError(f"n_draft must be [{B}], not {tuple(n_draft_host.shape)}")
+        if bool(((n_draft_host < 0) | (n_draft_host > drafts_host.shape[1])).any()):
+            raise ValueError(f"n_draft must lie in 0..{drafts_host.shape[1]}")
+        self.tokens.copy_(tokens_host, non_blocking=True)
+        if drafts_host.shape[1] < k:       # the step always runs max_draft rows per request; pad with token 0
+            drafts_host = torch.cat([drafts_host, drafts_host.new_zeros(B, k - drafts_host.shape[1])], dim=1)
+        self.draft_tokens.copy_(drafts_host, non_blocking=True)
+        self.n_draft.copy_(n_draft_host, non_blocking=True)
+        self.verify_step()
+        return self.out_tokens.cpu(), self.accepted.cpu()

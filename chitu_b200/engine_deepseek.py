@@ -213,10 +213,12 @@ class DeepSeekDecodeEngine(DecodeEngine):
         check(self.lib.chitu_b200_rmsnorm_quant_fp8(ptr(x), ptr(w), ptr(y), ptr(self.xq), ptr(self.xs), rows, dim,
                                                     xs or dim, dim, self.cfg.norm_eps, current_stream()), "rmsnorm_quant")
 
-    def _norm(self, x, w, y=None, q=None, qs=None):
-        """RMSNorm of the residual stream into bf16 `y` and / or the fp8 activations `q` + scales `qs`."""
+    def _norm(self, x, w, y=None, q=None, qs=None, rows=None):
+        """RMSNorm of the residual stream into bf16 `y` and / or the fp8 activations `q` + scales `qs` (`rows`
+        rows, default B)."""
         c = self.cfg
-        check(self.lib.chitu_b200_rmsnorm_quant_fp8(ptr(x), ptr(w), ptr(y), ptr(q), ptr(qs), self.B, c.dim, c.dim, c.dim,
+        M = self.B if rows is None else rows
+        check(self.lib.chitu_b200_rmsnorm_quant_fp8(ptr(x), ptr(w), ptr(y), ptr(q), ptr(qs), M, c.dim, c.dim, c.dim,
                                                     c.norm_eps, current_stream()), "rmsnorm_quant")
 
     def _norm_out(self, bf16: bool):

@@ -27,6 +27,7 @@ __all__ = [
     "silu_and_mul",
     "linear",
     "sample_top_k_top_p",
+    "accept_draft_tokens_greedy",
 ]
 
 # impl selector for the linears: 0 auto, 1 SIMT, 2 wgmma (tests flip this)
@@ -404,3 +405,38 @@ def sample_top_k_top_p(logits: torch.Tensor, temperatures: torch.Tensor, top_ks:
                                                     ptr(top_ps.float().contiguous()), ptr(uniforms.float().contiguous()), ptr(tok),
                                                     ptr(kept), ptr(mass), current_stream()), "sample_top_k_top_p")
     return (tok, kept, mass) if return_stats else tok
+
+
+def accept_draft_tokens_greedy(target: torch.Tensor, drafts: torch.Tensor, n_draft: torch.Tensor,
+                               seq_lens: torch.Tensor):
+    """Greedy acceptance of speculative drafts after a verify step over k + 1 positions per request, in one launch.
+    target int64 [B, k + 1] (the argmax at each verified position), drafts int64 [B, k], n_draft int32 [B] (each
+    request's draft length, 0..k) and seq_lens int32 [B], all contiguous on one CUDA device.  Request b accepts the
+    a_b leading drafts that equal the target (i < n_draft[b]) and emits target[b, :a_b + 1]; seq_lens[b] grows by
+    a_b + 1 in place.  Returns (out_tokens int64 [B, k + 1] with -1 after the emitted tokens, accepted int32 [B],
+    next_tokens int64 [B] = target[b, a_b]).  No host synchronisation (capturable)."""
+    def refuse(why):
+        raise ValueError(f"accept_draft_tokens_greedy: {why}")
+
+    ts = (target, drafts, n_draft, seq_lens)
+    if not all(isinstance(t, torch.Tensor) for t in ts):
+        refuse("every argument must be a tensor")
+    if not all(t.is_cuda for t in ts) or any(t.device != target.device for t in ts):
+        refuse("every tensor must be on the same CUDA device")
+    if (target.dtype, drafts.dtype, n_draft.dtype, seq_lens.dtype) != (torch.int64, torch.int64, torch.int32,
+                                                                       torch.int32):
+        refuse("target and drafts must be int64, n_draft and seq_lens int32")
+    if target.dim() != 2 or target.shape[1] < 2:
+        refuse(f"target must be [B, k + 1] with k >= 1, not {tuple(target.shape)}")
+    B, k = target.shape[0], target.shape[1] - 1
+    if tuple(drafts.shape) != (B, k) or tuple(n_draft.shape) != (B,) or tuple(seq_lens.shape) != (B,):
+        refuse(f"drafts must be [{B}, {k}], n_draft and seq_lens [{B}]")
+    if not all(t.is_contiguous() for t in ts):
+        refuse("every tensor must be contiguous")
+    out = torch.empty(B, k + 1, dtype=torch.int64, device=target.device)
+    accepted = torch.empty(B, dtype=torch.int32, device=target.device)
+    nxt = torch.empty(B, dtype=torch.int64, device=target.device)
+    check(_lib.load().chitu_b200_spec_accept_greedy(ptr(target), ptr(drafts), ptr(n_draft), ptr(seq_lens), ptr(out),
+                                                    ptr(accepted), ptr(nxt), B, k, current_stream()),
+          "spec_accept_greedy")
+    return out, accepted, nxt

@@ -442,6 +442,17 @@ int chitu_b200_sample_top_k_top_p(const void* logits, int64_t row_stride, int B,
                                   const float* temperatures, const int32_t* top_ks, const float* top_ps,
                                   const float* uniforms, int64_t* out_tokens, int32_t* out_kept, float* out_mass,
                                   void* stream);
+/* Greedy acceptance of speculative drafts after a verify step over k + 1 positions per request.  target int64
+ * [B, k + 1]: the argmax at each verified position; drafts int64 [B, k]; n_draft int32 [B]: each request's draft length
+ * (clamped to 0..k); seq_lens int32 [B], updated in place.  a_b = the number of leading i < n_draft[b] with
+ * drafts[b, i] == target[b, i]; request b emits target[b, 0..a_b] into out_tokens int64 [B, k + 1] (the rest of the row
+ * is -1), accepted int32 [B] = a_b, next_tokens int64 [B] = target[b, a_b], seq_lens[b] += a_b + 1.
+ * One launch, no host synchronisation, capturable.  It writes seq_lens, which the decode kernels read before their
+ * griddepcontrol.wait, so it waits for its predecessor and never triggers its dependents early.  Null pointers, B < 0
+ * or k < 1 return a negative status before any launch; B == 0 launches nothing. */
+int chitu_b200_spec_accept_greedy(const int64_t* target, const int64_t* drafts, const int32_t* n_draft,
+                                  int32_t* seq_lens, int64_t* out_tokens, int32_t* accepted, int64_t* next_tokens,
+                                  int B, int k, void* stream);
 
 /* ---- dev tool: in-graph kernel timeline (see csrc/common.cuh) ------------------------------------------------ */
 int chitu_b200_debug_timeline(void* buf /* uint64 [2 + capacity] on the device, or NULL to disarm */);
