@@ -98,6 +98,8 @@ SIGNATURES = {
     "chitu_b200_allreduce_residual_rmsnorm": (I, [P, P, P, P, P, P, P, P, I, I, F, P]),
     "chitu_b200_sample_top_k_top_p": (I, [P, L, I, I, I, P, P, P, P, P, P, P, P]),
     "chitu_b200_spec_accept_greedy": (I, [P, P, P, P, P, P, P, I, I, P]),
+    "chitu_b200_spec_accept_sampled_workspace_bytes": (L, [I, I]),
+    "chitu_b200_spec_accept_sampled": (I, [P, L, I, I, P, P, P, P, P, P, L, P, P, P, P, P, P, I, I, P, L, P]),
     "chitu_b200_embedding": (I, [P, P, P, I, I, L, L, I, P]),
     "chitu_b200_add": (I, [P, P, P, L, I, P]),
     "chitu_b200_argmax": (I, [P, P, I, L, I, P]),

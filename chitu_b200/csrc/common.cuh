@@ -366,6 +366,33 @@ __device__ __forceinline__ float warp_max(float v) {
   return v;
 }
 
+// The first maximal index of row[0 .. V) (NaN never wins; index 0 when nothing beats -inf), by a block of 1024
+// threads; sv / si: 1024 entries of shared memory each.  Every thread gets the result.
+template <typename T>
+__device__ __forceinline__ int64_t block_argmax_1024(const T* row, int64_t V, float* sv, int64_t* si) {
+  float best = -INFINITY;
+  int64_t bi = 0;
+  for (int64_t i = threadIdx.x; i < V; i += 1024) {
+    float v = io<T>::to_f(row[i]);
+    if (v > best) { best = v; bi = i; }   // ascending i per thread -> first max wins
+  }
+  sv[threadIdx.x] = best;
+  si[threadIdx.x] = bi;
+  __syncthreads();
+  for (int o = 512; o > 0; o >>= 1) {
+    if (threadIdx.x < o) {
+      float v2 = sv[threadIdx.x + o];
+      int64_t i2 = si[threadIdx.x + o];
+      if (v2 > sv[threadIdx.x] || (v2 == sv[threadIdx.x] && i2 < si[threadIdx.x])) {
+        sv[threadIdx.x] = v2;
+        si[threadIdx.x] = i2;
+      }
+    }
+    __syncthreads();
+  }
+  return si[0];
+}
+
 // ---- e4m3 group quantisation: one warp per 128-element group, 4 consecutive elements per lane ---------------------
 // scale = amax / 448 and q = v / scale, both divided as torch divides (__fdiv_rn), bit-exact with one of two references:
 // kActQuant (act_quant_deepseek_v3) takes amax as is and leaves q unclamped; kPerTokenGroup (per_token_group_quant_fp8)

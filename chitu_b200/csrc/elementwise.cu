@@ -701,30 +701,10 @@ extern "C" int chitu_b200_add(const void* a, const void* b, void* y, int64_t n, 
 template <typename T>
 __global__ void __launch_bounds__(1024) argmax_kernel(const T* __restrict__ logits, int64_t* __restrict__ out, int64_t V) {
   cb::pdl_prologue();
-  const T* row = logits + (int64_t)blockIdx.x * V;
-  float best = -INFINITY;
-  int64_t bi = 0;
-  for (int64_t i = threadIdx.x; i < V; i += 1024) {
-    float v = io<T>::to_f(row[i]);
-    if (v > best) { best = v; bi = i; }   // ascending i per thread -> first max wins
-  }
   __shared__ float sv[1024];
   __shared__ int64_t si[1024];
-  sv[threadIdx.x] = best;
-  si[threadIdx.x] = bi;
-  __syncthreads();
-  for (int o = 512; o > 0; o >>= 1) {
-    if (threadIdx.x < o) {
-      float v2 = sv[threadIdx.x + o];
-      int64_t i2 = si[threadIdx.x + o];
-      if (v2 > sv[threadIdx.x] || (v2 == sv[threadIdx.x] && i2 < si[threadIdx.x])) {
-        sv[threadIdx.x] = v2;
-        si[threadIdx.x] = i2;
-      }
-    }
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) out[blockIdx.x] = si[0];
+  const int64_t best = block_argmax_1024(logits + (int64_t)blockIdx.x * V, V, sv, si);
+  if (threadIdx.x == 0) out[blockIdx.x] = best;
 }
 
 extern "C" int chitu_b200_argmax(const void* logits, int64_t* out, int T, int64_t V, int dtype, void* stream) {

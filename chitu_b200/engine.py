@@ -248,8 +248,9 @@ class DecodeEngine:
                                                  self.tp_gather))
         self.seq_lens.add_(1)     # finalize_cache_single_decode (cache_manager.py)
 
-    def _capture(self, body):
-        """(a CUDA graph of `body`, the launches it holds); seq_lens is restored after the warm-up and the capture."""
+    def _capture(self, body, generators=()):
+        """(a CUDA graph of `body`, the launches it holds); seq_lens is restored after the warm-up and the capture.
+        `generators`: the torch generators `body` draws from, registered with the graph so each replay draws anew."""
         torch.cuda.synchronize(self.device)
         saved = self.seq_lens.clone()
         s = torch.cuda.Stream(device=self.device)
@@ -262,6 +263,8 @@ class DecodeEngine:
         self.seq_lens.copy_(saved)
         before = _lib.launch_count()
         graph = torch.cuda.CUDAGraph()
+        for gen in generators:
+            graph.register_generator_state(gen)
         with torch.cuda.graph(graph):
             body()
         launches = _lib.launch_count() - before
@@ -310,14 +313,21 @@ class LlamaDecodeEngine(DecodeEngine):
     max_draft=k > 0 adds a speculative verify step (`verify`, `capture_verify`): every request's token and up to k draft
     tokens run through the model as B * (k + 1) rows with causal attention over the cache, and the greedy acceptance
     kernel advances `seq_lens` on the device.  The row buffers are then sized for B * (k + 1) rows; the decode step is
-    unchanged."""
+    unchanged.
+
+    sampled_verify=True verifies under each request's temperature / top_k / top_p instead (speculative sampling,
+    chitu_b200_spec_accept_sampled): the emitted tokens have the distribution of sampling the model one token at a
+    time, and T = 0 requests are accepted greedily as before.  Its uniforms are drawn on the device inside the verify
+    step from an engine-owned generator (`sample_generator`, seeded from `seed`).  draft_probs=True also takes the
+    drafter's distributions [B, k', V] (a draft model's); without it the drafts are token-only (q one-hot).  One GPU
+    only: the vocab-parallel head leaves each rank a vocabulary shard."""
 
     W4_LINEARS = ("wqkv", "wo", "w13", "w2")
 
     def __init__(self, cfg: LlamaConfig, max_reqs: int, max_seq_len: int, device="cuda:0", page_size: int = 256,
                  seed: int = 0, tp_rank: int = 0, tp_size: int = 1, process_group=None, linear_impl: int = 0,
                  use_fused_allreduce: bool = True, kv_dtype: torch.dtype = BF, weight_format: str = "bf16",
-                 max_draft: int = 0):
+                 max_draft: int = 0, sampled_verify: bool = False, draft_probs: bool = False):
         D = cfg.head_dim
         self._set_weight_format(weight_format, tp_size, process_group, formats=("bf16", "w4a16", "fp8"))
         if weight_format != "bf16" and linear_impl == 1:
@@ -340,6 +350,14 @@ class LlamaDecodeEngine(DecodeEngine):
             if max_reqs * (max_draft + 1) > 256:
                 raise ValueError(f"the verify step runs at most 256 rows: max_reqs * (max_draft + 1) = "
                                  f"{max_reqs * (max_draft + 1)}")
+        if sampled_verify and max_draft == 0:
+            raise ValueError("sampled_verify needs a verify step: build the engine with max_draft > 0")
+        if draft_probs and not sampled_verify:
+            raise ValueError("draft_probs are read by the sampled verify step only: build with sampled_verify=True")
+        if sampled_verify and tp_size > 1:
+            raise ValueError("sampled_verify runs on one GPU: under tensor parallelism each rank's head holds a "
+                             "vocabulary shard")
+        self.sampled_verify = sampled_verify
         super().__init__(cfg, max_reqs, max_seq_len, device, page_size, seed, tp_rank, tp_size, process_group,
                          use_fused_allreduce, attn_ws=(self.Hq, D, 64),
                          lin_n=max(2 * self.F, cfg.vocab_size // tp_size), max_draft=max_draft)
@@ -398,6 +416,19 @@ class LlamaDecodeEngine(DecodeEngine):
             self.verify_gather = torch.empty(tp_size, R, 2, dtype=torch.float32, device=dev) if self.tp_on else None
             self.verify_attn_ws = torch.zeros(self.lib.chitu_b200_attn_workspace_bytes(R, self.Hq, D, 64),
                                               dtype=torch.uint8, device=dev)
+        if sampled_verify:
+            # each request's sampling parameters; the uniforms of one step: u_accept [B, k] then u_draw [B]
+            self.temperatures = torch.zeros(max_reqs, dtype=torch.float32, device=dev)
+            self.top_ks = torch.zeros(max_reqs, dtype=torch.int32, device=dev)
+            self.top_ps = torch.ones(max_reqs, dtype=torch.float32, device=dev)
+            self.uniforms = torch.zeros(max_reqs * (max_draft + 1), dtype=torch.float32, device=dev)
+            self.u_accept = self.uniforms[:max_reqs * max_draft].view(max_reqs, max_draft)
+            self.u_draw = self.uniforms[max_reqs * max_draft:]
+            self.sample_generator = torch.Generator(device=dev).manual_seed(seed + 13)
+            self.spec_ws = torch.zeros(self.lib.chitu_b200_spec_accept_sampled_workspace_bytes(max_reqs, max_draft),
+                                       dtype=torch.uint8, device=dev)
+            self.draft_probs = (torch.zeros(max_reqs, max_draft, cfg.vocab_size, dtype=torch.float32, device=dev)
+                                if draft_probs else None)
         # SiluAndMul inside the w13 GEMM epilogue: the merged gate/up weight is stored with its rows interleaved
         # (row 2i = gate_i, row 2i+1 = up_i) — a load-time permutation of the reference's merged tensor.
         # It and push mode need the wgmma GEMM, which linear_impl=1 (the SIMT GEMV) turns off.
@@ -559,6 +590,17 @@ class LlamaDecodeEngine(DecodeEngine):
         self._decode_layers(sq=k + 1)
         self._linear(self.xn, self.head, self.logits, M)
         vocab_local = self.head.shape[0]
+        if self.sampled_verify:
+            torch.rand(self.uniforms.shape, generator=self.sample_generator, out=self.uniforms)
+            dp = self.draft_probs
+            check(lib.chitu_b200_spec_accept_sampled(ptr(self.logits), self.logits.stride(0), vocab_local, _lib.CB_BF16,
+                                                     ptr(self.temperatures), ptr(self.top_ks), ptr(self.top_ps),
+                                                     ptr(self.draft_tokens), ptr(self.n_draft), ptr(dp),
+                                                     0 if dp is None else dp.stride(1), ptr(self.u_accept),
+                                                     ptr(self.u_draw), ptr(self.seq_lens), ptr(self.out_tokens),
+                                                     ptr(self.accepted), ptr(self.next_tokens), B, k, ptr(self.spec_ws),
+                                                     self.spec_ws.numel(), st), "spec_accept_sampled")
+            return
         check(lib.chitu_b200_argmax(ptr(self.logits), ptr(self.target), M, vocab_local, _lib.CB_BF16, st), "argmax")
         if self.tp_on:
             self.target.view(-1).copy_(global_argmax(self.logits, self.target.view(-1), self.tp_rank, vocab_local,
@@ -574,7 +616,8 @@ class LlamaDecodeEngine(DecodeEngine):
     def capture_verify(self):
         """Capture the verify step in a CUDA graph of its own (the decode step's graph is separate)."""
         self._need_verify()
-        self.verify_graph, self.launches_per_verify = self._capture(self._verify_body)
+        self.verify_graph, self.launches_per_verify = self._capture(
+            self._verify_body, generators=(self.sample_generator,) if self.sampled_verify else ())
 
     def verify_step(self):
         """One verify step over the persistent buffers (tokens in self.tokens, drafts in self.draft_tokens / n_draft)."""
@@ -586,8 +629,9 @@ class LlamaDecodeEngine(DecodeEngine):
             self._verify_body()
             self.launches_per_verify = _lib.launch_count() - before
 
-    def verify(self, tokens_host: torch.Tensor, drafts_host: torch.Tensor, n_draft_host: torch.Tensor):
-        """Greedy speculative verification.  tokens_host int64 [B]: each request's last token (what `decode` takes);
+    def verify(self, tokens_host: torch.Tensor, drafts_host: torch.Tensor, n_draft_host: torch.Tensor,
+               temperature=None, top_k=None, top_p=None, draft_probs=None):
+        """Speculative verification, greedy (or sampled: below).  tokens_host int64 [B]: each request's last token (what `decode` takes);
         drafts_host int64 [B, k'] with k' <= max_draft: the proposed continuations; n_draft_host int32 [B] in 0..k':
         how many of a request's drafts to check.  One step runs every request's token and drafts through the model
         (positions seq_lens[b] .. seq_lens[b] + max_draft), accepts the leading drafts equal to the model's greedy
@@ -597,7 +641,12 @@ class LlamaDecodeEngine(DecodeEngine):
         accepted int32 [B]).  self.next_tokens holds each request's last emitted token, the input of the next step.
         K / V rows are written for all max_draft + 1 positions; those past the accepted ones stay beyond seq_lens and are
         overwritten by later steps.  The caller keeps seq_lens[b] + max_draft + 1 <= max_seq_len, and the cache pages
-        for those positions in the block table."""
+        for those positions in the block table.
+
+        An engine built with sampled_verify=True takes each request's temperature fp32 [B] (finite; <= 0: greedy),
+        top_k int32 [B] (<= 0: no top-k) and top_p fp32 [B] (in (0, 1]) on the host, and accepts by speculative
+        sampling; with draft_probs=True also draft_probs fp32 [B, k', V], the drafter's distribution at each draft.
+        A greedy engine takes none of them."""
         self._need_verify()
         B, k = self.B, self.max_draft
         drafts_host = torch.as_tensor(drafts_host)
@@ -610,10 +659,53 @@ class LlamaDecodeEngine(DecodeEngine):
             raise ValueError(f"n_draft must be [{B}], not {tuple(n_draft_host.shape)}")
         if bool(((n_draft_host < 0) | (n_draft_host > drafts_host.shape[1])).any()):
             raise ValueError(f"n_draft must lie in 0..{drafts_host.shape[1]}")
+        sampling = self._sampling_args(temperature, top_k, top_p, draft_probs, drafts_host.shape[1])
         self.tokens.copy_(tokens_host, non_blocking=True)
+        if sampling is not None:
+            temperature, top_k, top_p, draft_probs = sampling
+            self.temperatures.copy_(temperature, non_blocking=True)
+            self.top_ks.copy_(top_k, non_blocking=True)
+            self.top_ps.copy_(top_p, non_blocking=True)
+            if draft_probs is not None:
+                self.draft_probs[:, :draft_probs.shape[1]].copy_(draft_probs, non_blocking=True)
         if drafts_host.shape[1] < k:       # the step always runs max_draft rows per request; pad with token 0
             drafts_host = torch.cat([drafts_host, drafts_host.new_zeros(B, k - drafts_host.shape[1])], dim=1)
         self.draft_tokens.copy_(drafts_host, non_blocking=True)
         self.n_draft.copy_(n_draft_host, non_blocking=True)
         self.verify_step()
         return self.out_tokens.cpu(), self.accepted.cpu()
+
+    def _sampling_args(self, temperature, top_k, top_p, draft_probs, k_in):
+        """The host-side checks of verify's sampling arguments: None on a greedy engine, else them as host tensors of
+        the buffers' dtypes."""
+        given = [x is not None for x in (temperature, top_k, top_p)]
+        if not self.sampled_verify:
+            if any(given) or draft_probs is not None:
+                raise ValueError("temperature / top_k / top_p / draft_probs need an engine built with "
+                                 "sampled_verify=True")
+            return None
+        if not all(given):
+            raise ValueError("a sampled verify step needs temperature, top_k and top_p for every request")
+        B = self.B
+        temperature = torch.as_tensor(temperature).to(torch.float32)
+        top_k = torch.as_tensor(top_k).to(torch.int32)
+        top_p = torch.as_tensor(top_p).to(torch.float32)
+        for name, t in (("temperature", temperature), ("top_k", top_k), ("top_p", top_p)):
+            if t.is_cuda or tuple(t.shape) != (B,):
+                raise ValueError(f"{name} must be a host tensor [{B}], not {tuple(t.shape)} on {t.device}")
+        if not bool(torch.isfinite(temperature).all()):
+            raise ValueError("temperature must be finite")
+        if not bool(((top_p > 0) & (top_p <= 1)).all()):
+            raise ValueError("top_p must lie in (0, 1]")
+        if self.draft_probs is None:
+            if draft_probs is not None:
+                raise ValueError("draft_probs need an engine built with draft_probs=True")
+        else:
+            if draft_probs is None:
+                raise ValueError("this engine verifies draft-model drafts: pass draft_probs")
+            draft_probs = torch.as_tensor(draft_probs)
+            V = self.draft_probs.shape[2]
+            if draft_probs.is_cuda or draft_probs.dtype != torch.float32 or tuple(draft_probs.shape) != (B, k_in, V):
+                raise ValueError(f"draft_probs must be a host fp32 tensor [{B}, {k_in}, {V}], not {draft_probs.dtype} "
+                                 f"{tuple(draft_probs.shape)} on {draft_probs.device}")
+        return temperature, top_k, top_p, draft_probs

@@ -28,6 +28,7 @@ __all__ = [
     "linear",
     "sample_top_k_top_p",
     "accept_draft_tokens_greedy",
+    "accept_draft_tokens_sampled",
 ]
 
 # impl selector for the linears: 0 auto, 1 SIMT, 2 wgmma (tests flip this)
@@ -439,4 +440,70 @@ def accept_draft_tokens_greedy(target: torch.Tensor, drafts: torch.Tensor, n_dra
     check(_lib.load().chitu_b200_spec_accept_greedy(ptr(target), ptr(drafts), ptr(n_draft), ptr(seq_lens), ptr(out),
                                                     ptr(accepted), ptr(nxt), B, k, current_stream()),
           "spec_accept_greedy")
+    return out, accepted, nxt
+
+
+def accept_draft_tokens_sampled(logits: torch.Tensor, drafts: torch.Tensor, n_draft: torch.Tensor,
+                                seq_lens: torch.Tensor, temperatures: torch.Tensor, top_ks: torch.Tensor,
+                                top_ps: torch.Tensor, u_accept: torch.Tensor, u_draw: torch.Tensor,
+                                draft_probs: Optional[torch.Tensor] = None):
+    """Speculative sampling of k drafts per request after a verify step, in two launches: the emitted tokens have the
+    distribution of sampling the target one token at a time with each request's temperature / top_k / top_p (the rule
+    of `sample_top_k_top_p`; T <= 0 is greedy, as `accept_draft_tokens_greedy` on the first maximal index).
+
+    logits [B * (k + 1), V] bf16 / fp16 / fp32 with unit column stride (row b * (k + 1) + i: request b's position i);
+    drafts int64 [B, k]; n_draft int32 [B] (0..k); seq_lens int32 [B], advanced in place; temperatures, top_ps fp32 [B];
+    top_ks int32 [B] (<= 0: no top-k); u_accept fp32 [B, k] and u_draw fp32 [B], uniforms in [0, 1); draft_probs: fp32
+    [B, k, V] with unit last stride, the drafter's distributions (None: token-only drafts, q one-hot at the draft).
+    Draft i is accepted iff u_accept[b, i] * q_i(d_i) < p_i(d_i); at the first rejection the token is drawn from
+    max(p - q, 0), after n accepted drafts from p_n.  Returns (out_tokens int64 [B, k + 1] with -1 after the emitted
+    tokens, accepted int32 [B], next_tokens int64 [B]).  No host synchronisation (capturable)."""
+    def refuse(why):
+        raise ValueError(f"accept_draft_tokens_sampled: {why}")
+
+    ts = (logits, drafts, n_draft, seq_lens, temperatures, top_ks, top_ps, u_accept, u_draw)
+    if not all(isinstance(t, torch.Tensor) for t in ts) or not (draft_probs is None or
+                                                                isinstance(draft_probs, torch.Tensor)):
+        refuse("every argument must be a tensor")
+    every = ts + (() if draft_probs is None else (draft_probs,))
+    if not all(t.is_cuda for t in every) or any(t.device != logits.device for t in every):
+        refuse("every tensor must be on the same CUDA device")
+    if logits.dtype not in (torch.bfloat16, torch.float16, torch.float32):
+        refuse(f"logits must be bf16, fp16 or fp32, not {logits.dtype}")
+    if (drafts.dtype, n_draft.dtype, seq_lens.dtype, top_ks.dtype) != (torch.int64, torch.int32, torch.int32,
+                                                                       torch.int32):
+        refuse("drafts must be int64, n_draft, seq_lens and top_ks int32")
+    if any(t.dtype != torch.float32 for t in (temperatures, top_ps, u_accept, u_draw)):
+        refuse("temperatures, top_ps, u_accept and u_draw must be fp32")
+    if drafts.dim() != 2 or drafts.shape[1] < 1:
+        refuse(f"drafts must be [B, k] with k >= 1, not {tuple(drafts.shape)}")
+    B, k = drafts.shape
+    if logits.dim() != 2 or logits.shape[0] != B * (k + 1) or logits.shape[1] < 1 or logits.stride(1) != 1:
+        refuse(f"logits must be [{B * (k + 1)}, V] with unit column stride, not {tuple(logits.shape)} "
+               f"(strides {logits.stride()})")
+    V = logits.shape[1]
+    if any(tuple(t.shape) != (B,) for t in (n_draft, seq_lens, temperatures, top_ks, top_ps, u_draw)):
+        refuse(f"n_draft, seq_lens, temperatures, top_ks, top_ps and u_draw must be [{B}]")
+    if tuple(u_accept.shape) != (B, k):
+        refuse(f"u_accept must be [{B}, {k}], not {tuple(u_accept.shape)}")
+    if not all(t.is_contiguous() for t in ts[1:]):
+        refuse("every tensor but logits and draft_probs must be contiguous")
+    q_stride = 0
+    if draft_probs is not None:
+        if draft_probs.dtype != torch.float32 or tuple(draft_probs.shape) != (B, k, V):
+            refuse(f"draft_probs must be fp32 [{B}, {k}, {V}], not {draft_probs.dtype} {tuple(draft_probs.shape)}")
+        q_stride = draft_probs.stride(1)
+        if draft_probs.stride(2) != 1 or draft_probs.stride(0) != k * q_stride:
+            refuse(f"draft_probs must have unit last stride and rows at a fixed stride, not {draft_probs.stride()}")
+    lib = _lib.load()
+    dev = logits.device
+    ws = torch.empty(lib.chitu_b200_spec_accept_sampled_workspace_bytes(B, k), dtype=torch.uint8, device=dev)
+    out = torch.empty(B, k + 1, dtype=torch.int64, device=dev)
+    accepted = torch.empty(B, dtype=torch.int32, device=dev)
+    nxt = torch.empty(B, dtype=torch.int64, device=dev)
+    check(lib.chitu_b200_spec_accept_sampled(ptr(logits), logits.stride(0), V, dtype_code(logits.dtype),
+                                             ptr(temperatures), ptr(top_ks), ptr(top_ps), ptr(drafts), ptr(n_draft),
+                                             ptr(draft_probs), q_stride, ptr(u_accept), ptr(u_draw), ptr(seq_lens),
+                                             ptr(out), ptr(accepted), ptr(nxt), B, k, ptr(ws), ws.numel(),
+                                             current_stream()), "spec_accept_sampled")
     return out, accepted, nxt

@@ -453,6 +453,25 @@ int chitu_b200_sample_top_k_top_p(const void* logits, int64_t row_stride, int B,
 int chitu_b200_spec_accept_greedy(const int64_t* target, const int64_t* drafts, const int32_t* n_draft,
                                   int32_t* seq_lens, int64_t* out_tokens, int32_t* accepted, int64_t* next_tokens,
                                   int B, int k, void* stream);
+/* Speculative sampling (rejection sampling) of k draft tokens per request after a verify step: the emitted tokens have
+ * the distribution of sampling the target one token at a time.  logits [B * (k + 1), V] (row stride in elements; row
+ * b * (k + 1) + i is request b's position i), bf16 / fp16 / fp32.  p_i: softmax(l / T) over the kept set of
+ * chitu_b200_sample_top_k_top_p with the request's temperatures / top_ks / top_ps [B] (T <= 0: greedy, the rule of
+ * chitu_b200_spec_accept_greedy on the first maximal index; top_k <= 0: no top-k).  q_i: fp32 row draft_probs
+ * + (b * k + i) * draft_probs_stride, or one-hot at drafts[b, i] when draft_probs is NULL.  Draft i is accepted iff
+ * u_accept[b, i] * q_i(d_i) < p_i(d_i) (never outside the kept set); a_b = the leading accepted count (<= n_draft[b],
+ * clamped to 0..k).  The drawn token comes from max(p_a - q_a, 0) when a_b < n_draft[b] (from p_a when that has no mass),
+ * from p_n otherwise: inverse CDF in vocabulary order at u_draw[b] times the mass.  Outputs as the greedy entry:
+ * out_tokens int64 [B, k + 1] (drafts 0..a_b - 1, the drawn token, then -1), accepted int32 [B] = a_b, next_tokens
+ * int64 [B] = the drawn token, seq_lens int32 [B] += a_b + 1.  workspace: at least
+ * chitu_b200_spec_accept_sampled_workspace_bytes(B, k) bytes.  Two launches, no host synchronisation. */
+int64_t chitu_b200_spec_accept_sampled_workspace_bytes(int B, int k);
+int chitu_b200_spec_accept_sampled(const void* logits, int64_t row_stride, int V, int dtype, const float* temperatures,
+                                   const int32_t* top_ks, const float* top_ps, const int64_t* drafts,
+                                   const int32_t* n_draft, const float* draft_probs, int64_t draft_probs_stride,
+                                   const float* u_accept, const float* u_draw, int32_t* seq_lens, int64_t* out_tokens,
+                                   int32_t* accepted, int64_t* next_tokens, int B, int k, void* workspace,
+                                   int64_t workspace_bytes, void* stream);
 
 /* ---- dev tool: in-graph kernel timeline (see csrc/common.cuh) ------------------------------------------------ */
 int chitu_b200_debug_timeline(void* buf /* uint64 [2 + capacity] on the device, or NULL to disarm */);
