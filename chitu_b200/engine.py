@@ -22,9 +22,17 @@ import torch
 
 from . import _lib
 from ._lib import check, current_stream, ptr
+from .quantize import fp8, w4a16
 from .tensor_parallel import global_argmax
 
 BF = torch.bfloat16
+
+# quantised weight format -> (the quantiser of one float weight [N, K] into the tensors the format's GEMMs read, the
+# dequantiser of those tensors into the values the GEMMs multiply: bf16 for 4-bit weights, fp32 q * s for fp8 ones)
+QUANT_FORMATS = {
+    "w4a16": (lambda w: w4a16.quantize_rtn(w, BF), w4a16.dequantize),
+    "fp8": (fp8.quantize_weight, fp8.dequantize),
+}
 
 
 @dataclass
@@ -71,11 +79,12 @@ class DecodeEngine:
     configuration measured on one GPU)."""
 
     linear_impl = 0          # `impl` of the bf16 linear entries: 0 = auto
-    # "w4a16": the subclass's W4_LINEARS hold (qweight, scales, zeros) in quantize/w4a16.py's layout (stacked per expert
-    # for the MoE weights) and run on the 4-bit GEMMs; "fp8": they hold (weight e4m3, weight_scale fp32 [N]) in
-    # quantize/fp8.py's layout and run on the rowwise FP8 GEMMs
+    # "w4a16": the subclass's QUANT_LINEARS hold (qweight, scales, zeros) in quantize/w4a16.py's layout (stacked per
+    # expert for the MoE weights) and run on the 4-bit GEMMs; "fp8": they hold (weight e4m3, weight_scale fp32 [N]) in
+    # quantize/fp8.py's layout and run on the rowwise FP8 GEMMs.  WEIGHT_FORMATS: the formats the subclass accepts
     weight_format = "bf16"
-    W4_LINEARS = ()
+    WEIGHT_FORMATS = ("bf16",)
+    QUANT_LINEARS = ()
 
     def __init__(self, cfg, max_reqs: int, max_seq_len: int, device, page_size: int, seed: int, tp_rank: int,
                  tp_size: int, process_group, use_fused_allreduce: bool, attn_ws: tuple, lin_n: int, max_draft: int = 0):
@@ -120,22 +129,31 @@ class DecodeEngine:
         # only, never under a graph)
         self.capture_h = None
 
-    def _set_weight_format(self, weight_format: str, tp_size: int, process_group, formats=("bf16", "w4a16")):
-        if weight_format not in formats:
-            raise ValueError(f"weight_format must be one of {formats}, not {weight_format!r}")
+    def _set_weight_format(self, weight_format: str, tp_size: int, process_group):
+        if weight_format not in self.WEIGHT_FORMATS:
+            raise ValueError(f"weight_format must be one of {self.WEIGHT_FORMATS}, not {weight_format!r}")
         if weight_format != "bf16" and process_group is not None and tp_size > 1:
             raise ValueError(f"weight_format={weight_format!r} runs on one GPU or one shard: its GEMM has no push "
                              "epilogue for the tensor-parallel all-reduce")
         self.weight_format = weight_format
 
+    def _quantized(self, lw: dict) -> dict:
+        """The layer's weights `lw`, with its QUANT_LINEARS quantised in place into the engine's weight format; a stack
+        of expert weights [E, N, K] is quantised one expert at a time and restacked."""
+        if self.weight_format != "bf16":
+            quantize, _ = QUANT_FORMATS[self.weight_format]
+            for name in self.QUANT_LINEARS:
+                w = lw[name]
+                lw[name] = quantize(w) if w.dim() == 2 else tuple(torch.stack(t) for t in zip(*map(quantize, w)))
+        return lw
+
     def _dequantized(self, lw: dict) -> dict:
         """A copy of the layer's weights with the quantised ones as the values the kernels multiply (the oracle side of
-        the tests): bf16 for 4-bit weights, fp32 q * s for fp8 ones."""
-        from .quantize import fp8, w4a16
+        the tests)."""
         d = dict(lw)
         if self.weight_format != "bf16":
-            dequantize = w4a16.dequantize if self.weight_format == "w4a16" else fp8.dequantize
-            d.update({name: dequantize(*lw[name]) for name in self.W4_LINEARS})
+            _, dequantize = QUANT_FORMATS[self.weight_format]
+            d.update({name: dequantize(*lw[name]) for name in self.QUANT_LINEARS})
         return d
 
     def _rope_tables(self, ang: torch.Tensor, dtype=torch.float32):
@@ -169,21 +187,30 @@ class DecodeEngine:
                                               ptr(self.lin_ws), self.lin_ws.numel(), self.linear_impl,
                                               current_stream()), "linear_bf16")
 
-    def _layer_linear(self, x, lw, name, y, M, residual=None):
-        """y = x . lw[name]^T (+ residual) in the engine's weight format; fp8: x is the e4m3 self.xq with the per-token
-        scales in self.xs."""
-        if self.weight_format == "bf16":
-            return self._linear(x, lw[name], y, M, residual=residual)
-        if self.weight_format == "fp8":
-            q, s = lw[name]
-            check(self.lib.chitu_b200_fp8_rowwise_gemm(ptr(x), ptr(self.xs), ptr(q), ptr(s), None, ptr(residual), ptr(y),
-                                                       M, q.shape[0], q.shape[1], ptr(self.lin_ws), self.lin_ws.numel(),
-                                                       current_stream()), f"fp8 {name}")
-            return
-        q, s, z = lw[name]
-        check(self.lib.chitu_b200_w4a16_gemm(ptr(x), ptr(q), ptr(s), ptr(z), ptr(residual), ptr(y), M, q.shape[0],
-                                             2 * q.shape[1], _lib.CB_BF16, ptr(self.lin_ws), self.lin_ws.numel(),
-                                             current_stream()), f"w4a16 {name}")
+    def _layer_linear(self, x, lw, name, y, M, residual=None, silu_pairs=False):
+        """y = x . lw[name]^T (+ residual) in the engine's weight format; silu_pairs: y = SiluAndMul of that product,
+        whose rows hold interleaved gate / up pairs (no residual).  fp8: x is the e4m3 self.xq with the per-token scales
+        in self.xs."""
+        fmt, lib, w = self.weight_format, self.lib, lw[name]
+        if fmt == "bf16" and not silu_pairs:
+            return self._linear(x, w, y, M, residual=residual)
+        ws = (ptr(self.lin_ws), self.lin_ws.numel(), current_stream())
+        if fmt == "bf16":
+            N, K = w.shape
+            rc = lib.chitu_b200_linear_bf16_silu_pairs(ptr(x), ptr(w), ptr(y), M, N, K, *ws)
+        elif fmt == "fp8":
+            q, s = w
+            N, K = q.shape
+            operands = (ptr(x), ptr(self.xs), ptr(q), ptr(s))
+            rc = (lib.chitu_b200_fp8_rowwise_gemm_silu_pairs(*operands, ptr(y), M, N, K, *ws) if silu_pairs else
+                  lib.chitu_b200_fp8_rowwise_gemm(*operands, None, ptr(residual), ptr(y), M, N, K, *ws))
+        else:
+            q, s, z = w
+            N, K = q.shape[0], 2 * q.shape[1]
+            operands = (ptr(x), ptr(q), ptr(s), ptr(z))
+            rc = (lib.chitu_b200_w4a16_gemm_silu_pairs(*operands, ptr(y), M, N, K, _lib.CB_BF16, *ws) if silu_pairs else
+                  lib.chitu_b200_w4a16_gemm(*operands, ptr(residual), ptr(y), M, N, K, _lib.CB_BF16, *ws))
+        check(rc, f"{fmt} {name}" + (" + silu" if silu_pairs else ""))
 
     def _norm(self, x, w, y, q=None, qs=None, rows=None):
         """RMSNorm of `rows` rows (default B) into bf16 `y`; with `q`, into the e4m3 `q` and per-token scales `qs` as
@@ -322,14 +349,15 @@ class LlamaDecodeEngine(DecodeEngine):
     drafter's distributions [B, k', V] (a draft model's); without it the drafts are token-only (q one-hot).  One GPU
     only: the vocab-parallel head leaves each rank a vocabulary shard."""
 
-    W4_LINEARS = ("wqkv", "wo", "w13", "w2")
+    WEIGHT_FORMATS = ("bf16", "w4a16", "fp8")
+    QUANT_LINEARS = ("wqkv", "wo", "w13", "w2")
 
     def __init__(self, cfg: LlamaConfig, max_reqs: int, max_seq_len: int, device="cuda:0", page_size: int = 256,
                  seed: int = 0, tp_rank: int = 0, tp_size: int = 1, process_group=None, linear_impl: int = 0,
                  use_fused_allreduce: bool = True, kv_dtype: torch.dtype = BF, weight_format: str = "bf16",
                  max_draft: int = 0, sampled_verify: bool = False, draft_probs: bool = False):
         D = cfg.head_dim
-        self._set_weight_format(weight_format, tp_size, process_group, formats=("bf16", "w4a16", "fp8"))
+        self._set_weight_format(weight_format, tp_size, process_group)
         if weight_format != "bf16" and linear_impl == 1:
             raise ValueError(f"weight_format={weight_format!r} runs on the wgmma GEMM only (linear_impl=1 selects the "
                              "SIMT GEMV)")
@@ -366,18 +394,27 @@ class LlamaDecodeEngine(DecodeEngine):
         def rnd(*shape, scale=0.02):
             return (torch.randn(*shape, generator=g, dtype=torch.float32, device=dev) * scale).to(BF)
 
+        # SiluAndMul inside the w13 GEMM epilogue: the merged gate/up weight is stored with its rows interleaved
+        # (row 2i = gate_i, row 2i+1 = up_i) — a load-time permutation of the reference's merged tensor.
+        # It and push mode need the wgmma GEMM, which linear_impl=1 (the SIMT GEMV) turns off.
+        self.fuse_silu = linear_impl != 1
+        self.ar_push = self.ar_push and linear_impl != 1
         self.embed = (torch.randn(cfg.vocab_size, dim, generator=self.g_rep, dtype=torch.float32, device=dev) * 0.02).to(BF)
         self.layers = []
         for _ in range(cfg.n_layers):
-            self.layers.append(dict(
+            lw = dict(
                 attn_norm=torch.ones(dim, dtype=BF, device=dev),
                 ffn_norm=torch.ones(dim, dtype=BF, device=dev),
                 # column-parallel wq|wk|wv merged along N (shards of each concatenated); row-parallel wo
                 wqkv=rnd((self.Hq + 2 * self.Hkv) * D, dim),
                 wo=rnd(dim, self.Hq * D),
-                w13=rnd(2 * self.F, dim),          # [w1 (gate) ; w3 (up)]  (interleaved below when the epilogue fuses SiLU)
+                w13=rnd(2 * self.F, dim),          # [w1 (gate) ; w3 (up)]
                 w2=rnd(dim, self.F),
-            ))
+            )
+            if self.fuse_silu:
+                lw["w13"] = lw["w13"].view(2, self.F, dim).transpose(0, 1).reshape(2 * self.F, dim).contiguous()
+            # quantised per row after the interleave: w13's interleaved rows carry their own scales (and zeros)
+            self.layers.append(self._quantized(lw))
         self.norm = torch.ones(dim, dtype=BF, device=dev)
         self.head = rnd(cfg.vocab_size // tp_size, dim)
         nblk = self.max_blocks * max_reqs
@@ -429,27 +466,8 @@ class LlamaDecodeEngine(DecodeEngine):
                                        dtype=torch.uint8, device=dev)
             self.draft_probs = (torch.zeros(max_reqs, max_draft, cfg.vocab_size, dtype=torch.float32, device=dev)
                                 if draft_probs else None)
-        # SiluAndMul inside the w13 GEMM epilogue: the merged gate/up weight is stored with its rows interleaved
-        # (row 2i = gate_i, row 2i+1 = up_i) — a load-time permutation of the reference's merged tensor.
-        # It and push mode need the wgmma GEMM, which linear_impl=1 (the SIMT GEMV) turns off.
-        self.fuse_silu = linear_impl != 1
-        self.ar_push = self.ar_push and linear_impl != 1
-        if self.fuse_silu:
-            for lw in self.layers:
-                lw["w13"] = lw["w13"].view(2, self.F, dim).transpose(0, 1).reshape(2 * self.F, dim).contiguous()
-        if weight_format == "w4a16":
-            # per-row quantisation: w13's interleaved rows carry their own scales and zeros
-            from .quantize.w4a16 import quantize_rtn
-            for lw in self.layers:
-                for name in self.W4_LINEARS:
-                    lw[name] = quantize_rtn(lw[name], BF)
         if weight_format == "fp8":
-            # per-channel scales: w13's interleaved rows carry their own; the e4m3 activations and their per-token
-            # scales of whichever linear runs next
-            from .quantize.fp8 import quantize_weight
-            for lw in self.layers:
-                for name in self.W4_LINEARS:
-                    lw[name] = quantize_weight(lw[name])
+            # the e4m3 activations and their per-token scales of whichever linear runs next
             self.xq = torch.zeros(B, max(dim, self.Hq * D, self.F), dtype=torch.float8_e4m3fn, device=dev)
             self.xs = torch.zeros(B, dtype=torch.float32, device=dev)
         # rotary fused into the tensor-core decode kernel (head dim 128, power-of-two pages)
@@ -549,22 +567,9 @@ class LlamaDecodeEngine(DecodeEngine):
                                                                    residual=res),
                                lambda: self.comm.linear_push(self.attn_out, lw["wo"], B, self.lin_ws),
                                h, h2, lw["ffn_norm"], **norm_out, rows=B)
-            if fp8:
-                q, s = lw["w13"]
-                check(lib.chitu_b200_fp8_rowwise_gemm_silu_pairs(ptr(self.xq), ptr(self.xs), ptr(q), ptr(s),
-                                                                 ptr(self.act), B, 2 * self.F, self.cfg.dim,
-                                                                 ptr(self.lin_ws), self.lin_ws.numel(), st),
-                      "fp8 w13 + silu")
-            elif self.weight_format == "w4a16":
-                q, s, z = lw["w13"]
-                check(lib.chitu_b200_w4a16_gemm_silu_pairs(ptr(self.xn), ptr(q), ptr(s), ptr(z), ptr(self.act), B,
-                                                           2 * self.F, self.cfg.dim, _lib.CB_BF16, ptr(self.lin_ws),
-                                                           self.lin_ws.numel(), st), "w4a16 w13 + silu")
-            elif self.fuse_silu:
-                check(lib.chitu_b200_linear_bf16_silu_pairs(ptr(self.xn), ptr(lw["w13"]), ptr(self.act), B, 2 * self.F,
-                                                            self.cfg.dim, ptr(self.lin_ws), self.lin_ws.numel(), st),
-                      "w13 + silu")
-            else:
+            if self.fuse_silu:
+                self._layer_linear(x_in, lw, "w13", self.act, B, silu_pairs=True)
+            else:                          # linear_impl=1, bf16 only: the SIMT GEMV, then SiluAndMul
                 self._linear(self.xn, lw["w13"], self.gate_up, B)
                 check(lib.chitu_b200_silu_and_mul(ptr(self.gate_up), ptr(self.act), B, self.F, _lib.CB_BF16, st), "silu")
             # h = w2(act) + h2; the head reads the final norm in bf16

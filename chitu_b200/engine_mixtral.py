@@ -49,16 +49,9 @@ class MixtralConfig:
 MIXTRAL_8X7B = MixtralConfig()
 
 
-def _quantize_experts(w):
-    """Stacked expert weights [E, N, K] -> (qweight [E, N, K/2], scales [E, N, K/128], zeros [E, N, K/128]) by
-    quantize_rtn, one expert at a time."""
-    from .quantize.w4a16 import quantize_rtn
-    parts = [quantize_rtn(w[e], BF) for e in range(w.shape[0])]
-    return tuple(torch.stack(t) for t in zip(*parts))
-
-
 class MixtralDecodeEngine(DecodeEngine):
-    W4_LINEARS = ("wqkv", "wo", "w1", "w2")
+    WEIGHT_FORMATS = ("bf16", "w4a16")
+    QUANT_LINEARS = ("wqkv", "wo", "w1", "w2")
 
     def __init__(self, cfg: MixtralConfig, max_reqs: int, max_seq_len: int, device="cuda:0", page_size: int = 256,
                  seed: int = 0, tp_rank: int = 0, tp_size: int = 4, process_group=None, use_fused_allreduce: bool = True,
@@ -87,11 +80,7 @@ class MixtralDecodeEngine(DecodeEngine):
                 gate_w=rnd(g_rep, self.E, dim, scale=0.05),
                 # experts stacked like fused_experts expects: w1 = [gate ; up] (merge_gate_up), w2 = down
                 w1=rnd(g, self.E, 2 * self.F, dim), w2=rnd(g, self.E, dim, self.F))
-            if weight_format == "w4a16":
-                from .quantize.w4a16 import quantize_rtn
-                lw["wqkv"], lw["wo"] = quantize_rtn(lw["wqkv"], BF), quantize_rtn(lw["wo"], BF)
-                lw["w1"], lw["w2"] = _quantize_experts(lw["w1"]), _quantize_experts(lw["w2"])
-            self.layers.append(lw)
+            self.layers.append(self._quantized(lw))
         self.norm = torch.ones(dim, dtype=BF, device=dev)
         self.head = rnd(g, cfg.vocab_size // T, dim)
         nblk = self.max_blocks * max_reqs
@@ -180,11 +169,16 @@ class MixtralDecodeEngine(DecodeEngine):
 
     def algorithmic_bytes(self, seq_len: int, distinct: float) -> int:
         """SURVEY §8d: every attention weight byte once, each DISTINCT expert once, KV rows once, bf16 head + router.
-        4-bit weights count the packed weight, its bf16 scales and its uint8 zeros."""
-        c, D = self.cfg, self.D
-        wbytes = (lambda n: n // 2 + n // 128 * 3) if self.weight_format == "w4a16" else (lambda n: n * 2)
-        attn = wbytes((self.Hq + 2 * self.Hkv) * D * c.dim) + wbytes(c.dim * self.Hq * D)
-        expert = wbytes(3 * self.F * c.dim)
+        The weights count the bytes of the tensors the engine holds (4-bit ones: the packed weight, its bf16 scales and
+        its uint8 zeros)."""
+        c, D, lw = self.cfg, self.D, self.layers[0]
+
+        def nbytes(name):
+            w = lw[name]
+            return sum(t.nbytes for t in w) if isinstance(w, tuple) else w.nbytes
+
+        attn = nbytes("wqkv") + nbytes("wo")
+        expert = (nbytes("w1") + nbytes("w2")) // self.E
         kv = self.B * (seq_len + 1) * 2 * self.Hkv * D * 2
         return int(c.n_layers * (attn + distinct * expert + kv + self.E * c.dim * 2) + self.head.numel() * 2)
 

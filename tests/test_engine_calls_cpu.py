@@ -1,9 +1,10 @@
-"""The library calls of one decode step of every engine, in every mode, pinned without a GPU.
+"""The library calls of one decode or verify step of every engine, in every mode, pinned without a GPU.
 
 Each engine is built at toy sizes on the CPU with a recording stand-in for libchitu_b200, a fake fused all-reduce and
-recording `torch.distributed` collectives, and one `_step_body()` runs.  Every call is recorded with its arguments; a
-pointer becomes (buffer number, byte offset), with buffers numbered in order of first appearance, so the trace changes
-when a launch reads or writes a different buffer but not when an attribute is renamed.  The traces are compared with
+recording `torch.distributed` collectives, and one `_step_body()` (or LLaMA's `_verify_body()`) runs.  Every call is
+recorded with its arguments; a pointer becomes (buffer number, byte offset), with buffers numbered in order of first
+appearance, so the trace changes when a launch reads or writes a different buffer but not when an attribute is
+renamed.  The traces are compared with
 tests/golden/engine_calls.json: a change to the engines that should not alter what runs on the GPU must leave them
 equal.  `python tests/test_engine_calls_cpu.py --write` regenerates the file after an intended change; its diff then
 shows which launches changed."""
@@ -140,31 +141,49 @@ def _mixtral(**kw):
 
 
 _TP = dict(tp_size=2, process_group=PG, use_fused_allreduce=False)
+_E4M3 = dict(kv_dtype=torch.float8_e4m3fn)
+_VERIFY = dict(max_draft=3)
+_SAMPLED = dict(max_draft=3, sampled_verify=True)
+STEP, VERIFY = "_step_body", "_verify_body"
 
-# mode -> (engine factory, reduce mode under tensor parallelism: "push" / "pull" (fake comm) / "nccl" (no comm), traced)
+# mode -> (engine factory, reduce mode under tensor parallelism: "push" / "pull" (fake comm) / "nccl" (no comm), traced,
+#          the engine method that runs the step: the decode step or the speculative verify step)
 MODES = {
-    "llama_single_rope": (lambda: _llama(128), None, False),
-    "llama_single_unfused_rope": (lambda: _llama(64), None, False),
-    "llama_linear_impl1": (lambda: _llama(128, linear_impl=1), None, False),
-    "llama_tp_push": (lambda: _llama(128, **_TP), "push", False),
-    "llama_tp_pull": (lambda: _llama(128, **_TP), "pull", False),
-    "llama_tp_nccl": (lambda: _llama(128, **_TP), "nccl", False),
-    "deepseek_single": (lambda: _deepseek(tp_size=1), None, False),
-    "deepseek_shard": (lambda: _deepseek(tp_size=2), None, False),
-    "deepseek_tp_push": (lambda: _deepseek(**_TP), "push", False),
-    "deepseek_tp_pull": (lambda: _deepseek(**_TP), "pull", False),
-    "deepseek_tp_nccl": (lambda: _deepseek(**_TP), "nccl", False),
-    "deepseek_traced_single": (lambda: _deepseek(tp_size=1), None, True),
-    "deepseek_traced_tp": (lambda: _deepseek(**_TP), "nccl", True),
-    "mixtral_shard": (lambda: _mixtral(tp_size=2), None, False),
-    "mixtral_tp_push": (lambda: _mixtral(**_TP), "push", False),
-    "mixtral_tp_pull": (lambda: _mixtral(**_TP), "pull", False),
-    "mixtral_tp_nccl": (lambda: _mixtral(**_TP), "nccl", False),
+    "llama_single_rope": (lambda: _llama(128), None, False, STEP),
+    "llama_single_unfused_rope": (lambda: _llama(64), None, False, STEP),
+    "llama_linear_impl1": (lambda: _llama(128, linear_impl=1), None, False, STEP),
+    "llama_tp_push": (lambda: _llama(128, **_TP), "push", False, STEP),
+    "llama_tp_pull": (lambda: _llama(128, **_TP), "pull", False, STEP),
+    "llama_tp_nccl": (lambda: _llama(128, **_TP), "nccl", False, STEP),
+    "deepseek_single": (lambda: _deepseek(tp_size=1), None, False, STEP),
+    "deepseek_shard": (lambda: _deepseek(tp_size=2), None, False, STEP),
+    "deepseek_tp_push": (lambda: _deepseek(**_TP), "push", False, STEP),
+    "deepseek_tp_pull": (lambda: _deepseek(**_TP), "pull", False, STEP),
+    "deepseek_tp_nccl": (lambda: _deepseek(**_TP), "nccl", False, STEP),
+    "deepseek_traced_single": (lambda: _deepseek(tp_size=1), None, True, STEP),
+    "deepseek_traced_tp": (lambda: _deepseek(**_TP), "nccl", True, STEP),
+    "mixtral_shard": (lambda: _mixtral(tp_size=2), None, False, STEP),
+    "mixtral_tp_push": (lambda: _mixtral(**_TP), "push", False, STEP),
+    "mixtral_tp_pull": (lambda: _mixtral(**_TP), "pull", False, STEP),
+    "mixtral_tp_nccl": (lambda: _mixtral(**_TP), "nccl", False, STEP),
+    "llama_w4a16": (lambda: _llama(128, weight_format="w4a16"), None, False, STEP),
+    "llama_w4a16_shard": (lambda: _llama(128, tp_size=2, weight_format="w4a16"), None, False, STEP),
+    "llama_fp8": (lambda: _llama(128, weight_format="fp8"), None, False, STEP),
+    "llama_fp8_e4m3_kv": (lambda: _llama(128, weight_format="fp8", **_E4M3), None, False, STEP),
+    "mixtral_w4a16": (lambda: _mixtral(tp_size=1, weight_format="w4a16"), None, False, STEP),
+    "mixtral_w4a16_shard": (lambda: _mixtral(tp_size=2, weight_format="w4a16"), None, False, STEP),
+    "llama_verify": (lambda: _llama(128, **_VERIFY), None, False, VERIFY),
+    "llama_verify_tp_push": (lambda: _llama(128, **_VERIFY, **_TP), "push", False, VERIFY),
+    "llama_verify_w4a16": (lambda: _llama(128, **_VERIFY, weight_format="w4a16"), None, False, VERIFY),
+    "llama_verify_fp8_e4m3_kv": (lambda: _llama(128, **_VERIFY, weight_format="fp8", **_E4M3), None, False, VERIFY),
+    "llama_verify_sampled_fp8_draft_probs": (lambda: _llama(128, **_SAMPLED, weight_format="fp8", draft_probs=True),
+                                             None, False, VERIFY),
+    "llama_verify_sampled": (lambda: _llama(128, **_SAMPLED), None, False, VERIFY),
 }
 
 
 def trace(mode):
-    make, reduce, traced = MODES[mode]
+    make, reduce, traced, body = MODES[mode]
     rec = Recorder()
     with _patched(rec):
         eng = make()
@@ -174,7 +193,7 @@ def trace(mode):
         if traced:
             eng.trace = []
         rec.watch(eng)
-        eng._step_body()
+        getattr(eng, body)()
     return json.loads(json.dumps(rec.calls))
 
 
