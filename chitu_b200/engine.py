@@ -156,6 +156,10 @@ class DecodeEngine:
             d.update({name: dequantize(*lw[name]) for name in self.QUANT_LINEARS})
         return d
 
+    def _rnd(self, gen, *shape, scale=0.02, dtype=BF):
+        """A synthetic weight: normal(0, scale) drawn in fp32 from `gen`, then cast to `dtype`."""
+        return (torch.randn(*shape, generator=gen, dtype=torch.float32, device=self.device) * scale).to(dtype)
+
     def _rope_tables(self, ang: torch.Tensor, dtype=torch.float32):
         """cos / sin tables from the rotary angles [positions, rot_dim / 2], and the per-step buffers that
         `_step_body` gathers them into by position."""
@@ -254,6 +258,92 @@ class DecodeEngine:
                                               current_stream()), "add")
                 self._norm(h_out, norm_w, y, q, qs, rows=B)
 
+    # ---- GQA attention over the paged K / V caches (LLaMA, Mixtral) ----------------------------------
+    def _gqa_buffers(self, kv_dtype, rows: int):
+        """The paged K / V caches [L, blocks, page, Hkv, D] in kv_dtype, and the attention's buffers for `rows` rows: the
+        merged qkv projection, the rotated q / k and the attention output."""
+        dev, D, Hq, Hkv = self.device, self.D, self.Hq, self.Hkv
+        self.k_cache = torch.zeros(self.cfg.n_layers, self.max_blocks * self.B, self.page, Hkv, D, dtype=kv_dtype,
+                                   device=dev)
+        self.v_cache = torch.zeros_like(self.k_cache)
+        self.caches = (self.k_cache, self.v_cache)
+        self.qkv = torch.zeros(rows, (Hq + 2 * Hkv) * D, dtype=BF, device=dev)
+        self.q_rot = torch.zeros(rows, Hq, D, dtype=BF, device=dev)
+        self.k_rot = torch.zeros(rows, Hkv, D, dtype=BF, device=dev)
+        self.attn_out = torch.zeros(rows, Hq * D, dtype=BF, device=dev)
+
+    def _gqa_decode(self, li):
+        """Paged GQA decode of layer li over the bf16 caches: q / k rotated in q_rot / k_rot, v in the qkv output; the
+        new k / v rows are appended at seq_lens."""
+        D, qkv_w = self.D, self.qkv.shape[1]
+        v = self.qkv[:, (self.Hq + self.Hkv) * D:]
+        check(self.lib.chitu_b200_gqa_paged_decode(
+            ptr(self.q_rot), ptr(self.k_cache[li]), ptr(self.v_cache[li]), ptr(self.k_rot), ptr(v), self.Hkv * D, qkv_w,
+            ptr(self.seq_lens), ptr(self.block_table), self.max_blocks, self.B, self.Hq, self.Hkv, D, self.page,
+            self.max_seq_len, 1.0 / math.sqrt(D), ptr(self.attn_out), ptr(self.attn_ws), self.attn_ws.numel(),
+            _lib.CB_BF16, current_stream()), "gqa_paged_decode")
+
+    # ---- the MoE block (Mixtral, DeepSeek) ------------------------------------------------------------
+    def _init_moe(self, n_routed: int, topk: int, slots: int, n_stacked: int, n1: int, score_mode: int,
+                  route_scale: float = 1.0, groups=(1, 1), bias: bool = False, first_layer: int = 0,
+                  weights=("w1", "w2", None, None), wmode: int = 0):
+        """The engine's routing, stated once.  The gate (chitu_b200_moe_gate, `score_mode`) scores `n_routed` experts,
+        within the best `groups[1]` of `groups[0]` groups, with the layer's fp32 bias `gate_b` when `bias`, and picks
+        `topk` of them into `slots` slots per token (the engine fills the slots past topk).  Layers from `first_layer` on
+        are MoE layers; each holds its `n_stacked` experts stacked, as the layer entries `weights` (w1 [n_stacked, n1,
+        dim], w2, and their scales for wmode 1) in chitu_b200_fused_experts' `wmode`, or as (qweight, scales, zeros)
+        under weight_format "w4a16".  Allocates every layer's routing results (resident: bench.py counts the distinct
+        experts per layer), the workspaces and `y`, this rank's expert sum under tensor parallelism."""
+        B, dev, dim = self.B, self.device, self.cfg.dim
+        self.gate_w_all = torch.zeros(self.cfg.n_layers, B, slots, dtype=BF, device=dev)
+        self.gate_i_all = torch.zeros(self.cfg.n_layers, B, slots, dtype=torch.int64, device=dev)
+        self.moe_ws = torch.zeros(self.lib.chitu_b200_moe_workspace_bytes(B, slots, n_stacked, n1, dim), dtype=torch.uint8,
+                                  device=dev)
+        self.gate_ws = torch.zeros(self.lib.chitu_b200_moe_gate_workspace_bytes(B, n_routed), dtype=torch.uint8,
+                                   device=dev)
+        self.y = torch.zeros(B, dim, dtype=BF, device=dev)
+        self._gate = (n_routed, *groups, topk, score_mode, float(route_scale))       # chitu_b200_moe_gate's E .. scale
+        self._moe = dict(topk=topk, bias=bias, first_layer=first_layer, weights=weights, wmode=wmode,
+                         stack=(slots, n_stacked, n1))
+
+    def _moe_gate(self, li):
+        """Route every token of layer li on self.xn into gate_w_all[li] / gate_i_all[li]."""
+        lw = self.layers[li]
+        bias = lw["gate_b"] if self._moe["bias"] else None
+        check(self.lib.chitu_b200_moe_gate(ptr(self.xn), ptr(lw["gate_w"]), ptr(bias), 0 if bias is None else _lib.CB_F32,
+                                           self.B, self.cfg.dim, *self._gate, ptr(self.gate_w_all[li]),
+                                           ptr(self.gate_i_all[li]), self.gate_w_all.shape[2], ptr(self.gate_ws),
+                                           self.gate_ws.numel(), current_stream()), "moe_gate")
+
+    def _moe_block(self, li, residual, h_out, norm_w, **norm_out):
+        """Layer li's MoE block on self.xn: the gate, then h_out = residual + the experts' sum over ranks, and its
+        RMSNorm by norm_w into `norm_out` (`_row_parallel`)."""
+        self._moe_gate(li)
+        lw, (slots, n_stacked, n1) = self.layers[li], self._moe["stack"]
+        w1, w2, s1, s2 = (lw[n] if n else None for n in self._moe["weights"])
+        # the arguments up to the output, as tensors: the local call passes their pointers, the push epilogue takes them
+        route = (self.gate_w_all[li], _lib.CB_BF16, self.gate_i_all[li], _lib.CB_I64, self.B, slots, n_stacked, n1,
+                 self.cfg.dim)
+        if self.weight_format == "w4a16":
+            fn, name, args = self.lib.chitu_b200_fused_experts_w4a16, "fused_experts_w4a16", (self.xn, *w1, *w2, *route)
+        else:
+            fn, name, args = (self.lib.chitu_b200_fused_experts, "fused_experts",
+                              (self.xn, w1, w2, s1, s2, *route, self._moe["wmode"]))
+
+        def local(out, res):
+            check(fn(*(ptr(a) if isinstance(a, torch.Tensor) else a for a in args), ptr(out), ptr(res), ptr(self.moe_ws),
+                     self.moe_ws.numel(), current_stream()), name)
+
+        self._row_parallel(local, lambda: self.comm.experts_push(*args, self.moe_ws), residual, h_out, norm_w,
+                           partial=self.y, **norm_out)
+
+    def distinct_experts_per_layer(self) -> float:
+        """Mean number of distinct routed experts per MoE layer in the last step."""
+        ids = self.gate_i_all[self._moe["first_layer"]:, :, :self._moe["topk"]].cpu()
+        if ids.numel() == 0:
+            return 0.0
+        return float(sum(len(torch.unique(ids[l])) for l in range(ids.shape[0])) / ids.shape[0])
+
     def _step_body(self):
         lib, B, cfg = self.lib, self.B, self.cfg
         st = current_stream()
@@ -303,14 +393,20 @@ class DecodeEngine:
         """Capture the decode step in a CUDA graph (models/model.py:572-611)."""
         self.graph, self.launches_per_step = self._capture(self._step_body)
 
+    @staticmethod
+    def _run(graph, body, launches):
+        """Replay `graph`, or run `body` eagerly when it has not been captured; returns the launches of one step
+        (`launches`, what the capture counted, on a replay)."""
+        if graph is not None:
+            graph.replay()
+            return launches
+        before = _lib.launch_count()
+        body()
+        return _lib.launch_count() - before
+
     def step(self):
         """One decode step over the persistent buffers (tokens in self.tokens)."""
-        if self.graph is not None:
-            self.graph.replay()
-        else:
-            before = _lib.launch_count()
-            self._step_body()
-            self.launches_per_step = _lib.launch_count() - before
+        self.launches_per_step = self._run(self.graph, self._step_body, self.launches_per_step)
 
     def decode(self, tokens_host: torch.Tensor) -> torch.Tensor:
         """Public API: host tokens [B] int64 (pinned) -> host next tokens [B] (greedy).
@@ -389,49 +485,38 @@ class LlamaDecodeEngine(DecodeEngine):
         super().__init__(cfg, max_reqs, max_seq_len, device, page_size, seed, tp_rank, tp_size, process_group,
                          use_fused_allreduce, attn_ws=(self.Hq, D, 64),
                          lin_n=max(2 * self.F, cfg.vocab_size // tp_size), max_draft=max_draft)
-        dev, g, dim = self.device, self.g, cfg.dim
-
-        def rnd(*shape, scale=0.02):
-            return (torch.randn(*shape, generator=g, dtype=torch.float32, device=dev) * scale).to(BF)
-
+        dev, g, dim, rnd = self.device, self.g, cfg.dim, self._rnd
         # SiluAndMul inside the w13 GEMM epilogue: the merged gate/up weight is stored with its rows interleaved
         # (row 2i = gate_i, row 2i+1 = up_i) — a load-time permutation of the reference's merged tensor.
         # It and push mode need the wgmma GEMM, which linear_impl=1 (the SIMT GEMV) turns off.
         self.fuse_silu = linear_impl != 1
         self.ar_push = self.ar_push and linear_impl != 1
-        self.embed = (torch.randn(cfg.vocab_size, dim, generator=self.g_rep, dtype=torch.float32, device=dev) * 0.02).to(BF)
+        self.embed = rnd(self.g_rep, cfg.vocab_size, dim)
         self.layers = []
         for _ in range(cfg.n_layers):
             lw = dict(
                 attn_norm=torch.ones(dim, dtype=BF, device=dev),
                 ffn_norm=torch.ones(dim, dtype=BF, device=dev),
                 # column-parallel wq|wk|wv merged along N (shards of each concatenated); row-parallel wo
-                wqkv=rnd((self.Hq + 2 * self.Hkv) * D, dim),
-                wo=rnd(dim, self.Hq * D),
-                w13=rnd(2 * self.F, dim),          # [w1 (gate) ; w3 (up)]
-                w2=rnd(dim, self.F),
+                wqkv=rnd(g, (self.Hq + 2 * self.Hkv) * D, dim),
+                wo=rnd(g, dim, self.Hq * D),
+                w13=rnd(g, 2 * self.F, dim),          # [w1 (gate) ; w3 (up)]
+                w2=rnd(g, dim, self.F),
             )
             if self.fuse_silu:
                 lw["w13"] = lw["w13"].view(2, self.F, dim).transpose(0, 1).reshape(2 * self.F, dim).contiguous()
             # quantised per row after the interleave: w13's interleaved rows carry their own scales (and zeros)
             self.layers.append(self._quantized(lw))
         self.norm = torch.ones(dim, dtype=BF, device=dev)
-        self.head = rnd(cfg.vocab_size // tp_size, dim)
-        nblk = self.max_blocks * max_reqs
+        self.head = rnd(g, cfg.vocab_size // tp_size, dim)
         if kv_dtype not in (BF, torch.float8_e4m3fn):
             raise ValueError(f"kv_dtype must be torch.bfloat16 or torch.float8_e4m3fn, not {kv_dtype}")
         self.kv_fp8 = kv_dtype == torch.float8_e4m3fn
-        self.k_cache = torch.zeros(cfg.n_layers, nblk, page_size, self.Hkv, D, dtype=kv_dtype, device=dev)
-        self.v_cache = torch.zeros_like(self.k_cache)
-        self.caches = (self.k_cache, self.v_cache)
+        B = max_reqs * (max_draft + 1)                     # rows of the widest step
+        self._gqa_buffers(kv_dtype, B)
         # precompute_freqs_cis (models/model.py:81-89) as cos/sin tables
         freqs = 1.0 / (cfg.rope_theta ** (torch.arange(0, D, 2)[: D // 2].float() / D))
         self._rope_tables(torch.outer(torch.arange(max_seq_len * 2, dtype=torch.float32), freqs))
-        B = max_reqs * (max_draft + 1)                     # rows of the widest step
-        self.qkv = torch.zeros(B, (self.Hq + 2 * self.Hkv) * D, dtype=BF, device=dev)
-        self.q_rot = torch.zeros(B, self.Hq, D, dtype=BF, device=dev)
-        self.k_rot = torch.zeros(B, self.Hkv, D, dtype=BF, device=dev)
-        self.attn_out = torch.zeros(B, self.Hq * D, dtype=BF, device=dev)
         self.gate_up = torch.zeros(B, 2 * self.F, dtype=BF, device=dev)
         self.act = torch.zeros(B, self.F, dtype=BF, device=dev)
         self.verify_graph = None
@@ -557,11 +642,7 @@ class LlamaDecodeEngine(DecodeEngine):
                 check(lib.chitu_b200_rotary_interleaved(ptr(q_view), ptr(k_view), ptr(self.q_rot), ptr(self.k_rot),
                                                         ptr(self.cos), ptr(self.sin), B, self.Hq, self.Hkv, D, qkv_w, D,
                                                         qkv_w, D, _lib.CB_BF16, st), "rotary")
-                check(lib.chitu_b200_gqa_paged_decode(
-                    ptr(self.q_rot), ptr(self.k_cache[li]), ptr(self.v_cache[li]), ptr(self.k_rot), ptr(v_view),
-                    self.Hkv * D, qkv_w, ptr(self.seq_lens), ptr(self.block_table), self.max_blocks, B, self.Hq,
-                    self.Hkv, D, self.page, self.max_seq_len, 1.0 / math.sqrt(D), ptr(self.attn_out), ptr(self.attn_ws),
-                    self.attn_ws.numel(), _lib.CB_BF16, st), "gqa_paged_decode")
+                self._gqa_decode(li)
             # h2 = wo(o) + h
             self._row_parallel(lambda out, res: self._layer_linear(self._quant(self.attn_out, B), lw, "wo", out, B,
                                                                    residual=res),
@@ -627,12 +708,7 @@ class LlamaDecodeEngine(DecodeEngine):
     def verify_step(self):
         """One verify step over the persistent buffers (tokens in self.tokens, drafts in self.draft_tokens / n_draft)."""
         self._need_verify()
-        if self.verify_graph is not None:
-            self.verify_graph.replay()
-        else:
-            before = _lib.launch_count()
-            self._verify_body()
-            self.launches_per_verify = _lib.launch_count() - before
+        self.launches_per_verify = self._run(self.verify_graph, self._verify_body, self.launches_per_verify)
 
     def verify(self, tokens_host: torch.Tensor, drafts_host: torch.Tensor, n_draft_host: torch.Tensor,
                temperature=None, top_k=None, top_p=None, draft_probs=None):

@@ -18,7 +18,6 @@ from typing import Optional
 
 import torch
 
-from . import _lib
 from ._lib import check, current_stream, ptr
 from .engine import DecodeEngine
 
@@ -118,23 +117,20 @@ class DeepSeekDecodeEngine(DecodeEngine):
         self.F_moe = c.moe_inter_dim // T
         super().__init__(cfg, max_reqs, max_seq_len, device, page_size, seed, tp_rank, tp_size, process_group,
                          use_fused_allreduce, attn_ws=(self.H, self.C, 128), lin_n=max(c.vocab_size // T, c.dim))
-        dev, g, g_rep = self.device, self.g, self.g_rep
-
-        def rnd(gen, *shape, scale=0.02):
-            return torch.randn(*shape, generator=gen, dtype=torch.float32, device=dev) * scale
+        dev, g, g_rep, rnd = self.device, self.g, self.g_rep, self._rnd
 
         def fp8(gen, *shape):
             # quantise in slabs to bound the fp32 temporaries for the [E, N, K] expert tensors
             if len(shape) == 3:
                 qs, ss = [], []
                 for e0 in range(0, shape[0], 32):
-                    q, s = quantize_fp8_block(rnd(gen, min(32, shape[0] - e0), *shape[1:]))
+                    q, s = quantize_fp8_block(rnd(gen, min(32, shape[0] - e0), *shape[1:], dtype=torch.float32))
                     qs.append(q), ss.append(s)
                 return torch.cat(qs), torch.cat(ss)
-            return quantize_fp8_block(rnd(gen, *shape))
+            return quantize_fp8_block(rnd(gen, *shape, dtype=torch.float32))
 
         dim = c.dim
-        self.embed = rnd(g_rep, c.vocab_size, dim).to(BF)
+        self.embed = rnd(g_rep, c.vocab_size, dim)
         self.layers = []
         for li in range(c.n_layers):
             L = dict(attn_norm=torch.ones(dim, dtype=BF, device=dev), ffn_norm=torch.ones(dim, dtype=BF, device=dev),
@@ -148,8 +144,8 @@ class DeepSeekDecodeEngine(DecodeEngine):
                 L["w13"], L["w13_s"] = fp8(g, 2 * self.F_dense, dim)
                 L["w2"], L["w2_s"] = fp8(g, dim, self.F_dense)
             else:
-                L["gate_w"] = rnd(g_rep, c.n_routed_experts, dim).to(BF)
-                L["gate_b"] = rnd(g_rep, c.n_routed_experts, scale=0.01)                       # fp32 bias
+                L["gate_w"] = rnd(g_rep, c.n_routed_experts, dim)
+                L["gate_b"] = rnd(g_rep, c.n_routed_experts, scale=0.01, dtype=torch.float32)      # fp32 bias
                 # routed experts + the shared expert stored as expert index n_routed_experts, exactly like the
                 # reference's stacked w1w3 / w2 tensors (model_deepseek_v3.py:1167-1191: `weight[-1]` is shared)
                 assert c.n_shared_experts == 1
@@ -161,7 +157,7 @@ class DeepSeekDecodeEngine(DecodeEngine):
             L["wkv_b_bf16"] = self._dequant(L["wkv_b"], L["wkv_b_s"])
             self.layers.append(L)
         self.norm = torch.ones(dim, dtype=BF, device=dev)
-        self.head = rnd(g, c.vocab_size // T, dim).to(BF)
+        self.head = rnd(g, c.vocab_size // T, dim)
         # paged MLA cache: [L, num_blocks, 64, 576], replicated on every rank (cache_manager.py:71-76)
         nblk = self.max_blocks * max_reqs
         self.kv_cache = torch.zeros(c.n_layers, nblk, page_size, self.C + self.R, dtype=kv_dtype, device=dev)
@@ -173,29 +169,21 @@ class DeepSeekDecodeEngine(DecodeEngine):
         self.xq = torch.zeros(B, kmax, dtype=F8, device=dev)
         self.xs = z(B, kmax // 128 + 1, dt=torch.float32)
         self.qkv_a = z(B, c.q_lora_rank + self.C + self.R)
-        self.qa_n = z(B, c.q_lora_rank)
         self.q = z(B, self.H, self.qk_head)
         self.q_pe = z(B, self.H, self.R)
         self.q_abs = z(B, self.H, self.C)
         self.new_kv = z(B, self.C + self.R)
-        self.o_lat = z(B, self.H, self.C)
-        self.o = z(B, self.H * c.v_head_dim)
         self.ff = z(B, 2 * max(self.F_dense, self.F_moe))
-        self.act = z(B, max(self.F_dense, self.F_moe))
-        self.y = z(B, dim)
-        # routing results of every layer stay resident (bench.py counts the distinct experts per layer)
-        # one extra slot per token = the shared expert (id n_routed_experts, weight 1): it rides through the
-        # grouped expert GEMM instead of five separate launches
-        self.topk1 = c.n_activated_experts + 1
-        self.gate_w_all = z(c.n_layers, B, self.topk1)
-        self.gate_i_all = torch.zeros(c.n_layers, B, self.topk1, dtype=torch.int64, device=dev)
+        # the routed experts of the MoE layers (fp8 block-scaled w8a8, wmode 1), plus one slot per token for the shared
+        # expert (id n_routed_experts, weight 1): it rides through the grouped expert GEMM instead of five separate
+        # launches
+        E = c.n_routed_experts
+        self._init_moe(n_routed=E, topk=c.n_activated_experts, slots=c.n_activated_experts + 1, n_stacked=E + 1,
+                       n1=2 * self.F_moe, score_mode=1 if c.score_func == "sigmoid" else 0, route_scale=c.route_scale,
+                       groups=(c.n_expert_groups, c.n_limited_groups), bias=True, first_layer=c.n_dense_layers,
+                       weights=("we1", "we2", "we1_s", "we2_s"), wmode=1)
         self.gate_w_all[..., -1] = 1.0
-        self.gate_i_all[..., -1] = c.n_routed_experts
-        lib = self.lib
-        self.moe_ws = torch.zeros(lib.chitu_b200_moe_workspace_bytes(B, self.topk1, c.n_routed_experts + 1,
-                                                                     2 * self.F_moe, dim), dtype=torch.uint8, device=dev)
-        self.gate_ws = torch.zeros(lib.chitu_b200_moe_gate_workspace_bytes(B, c.n_routed_experts), dtype=torch.uint8, device=dev)
-        self.trace = None          # set to [] to record per-layer intermediates (tests; not under CUDA graphs)
+        self.gate_i_all[..., -1] = E
 
     # ---- helpers -----------------------------------------------------------------------------------
     def _dequant(self, w, s):
@@ -203,15 +191,6 @@ class DeepSeekDecodeEngine(DecodeEngine):
         check(self.lib.chitu_b200_weight_dequant_fp8(ptr(w), ptr(s), ptr(y), 1, w.shape[0], w.shape[1], 128, 0,
                                                      current_stream()), "weight_dequant")
         return y
-
-    def _rms(self, x, w, y, rows, dim, xs=None, ys=None):
-        check(self.lib.chitu_b200_rmsnorm_strided(ptr(x), ptr(w), ptr(y), rows, dim, xs or dim, ys or dim,
-                                                  self.cfg.norm_eps, _lib.CB_BF16, current_stream()), "rmsnorm")
-
-    def _rms_quant(self, x, w, dim, rows, xs=None, y=None):
-        """RMSNorm fused with act_quant_deepseek_v3: fp8 payload -> self.xq / self.xs (and bf16 -> y)."""
-        check(self.lib.chitu_b200_rmsnorm_quant_fp8(ptr(x), ptr(w), ptr(y), ptr(self.xq), ptr(self.xs), rows, dim,
-                                                    xs or dim, dim, self.cfg.norm_eps, current_stream()), "rmsnorm_quant")
 
     def _norm(self, x, w, y=None, q=None, qs=None, rows=None):
         """RMSNorm of the residual stream into bf16 `y` and / or the fp8 activations `q` + scales `qs` (`rows`
@@ -231,28 +210,6 @@ class DeepSeekDecodeEngine(DecodeEngine):
         check(self.lib.chitu_b200_fp8_gemm(ptr(self.xq), ptr(self.xs), ptr(w), ptr(w_s), ptr(y), M, N, K, ptr(residual),
                                            ptr(self.lin_ws), self.lin_ws.numel(), 0, current_stream()), "fp8_gemm")
 
-    def _add(self, a, b, y):
-        check(self.lib.chitu_b200_add(ptr(a), ptr(b), ptr(y), a.numel(), _lib.CB_BF16, current_stream()), "add")
-
-    def _moe_gate(self, li):
-        c, L = self.cfg, self.layers[li]
-        check(self.lib.chitu_b200_moe_gate(ptr(self.xn), ptr(L["gate_w"]), ptr(L["gate_b"]), _lib.CB_F32, self.B, c.dim,
-                                           c.n_routed_experts, c.n_expert_groups, c.n_limited_groups,
-                                           c.n_activated_experts, 1 if c.score_func == "sigmoid" else 0,
-                                           float(c.route_scale), ptr(self.gate_w_all[li]), ptr(self.gate_i_all[li]),
-                                           self.topk1, ptr(self.gate_ws), self.gate_ws.numel(), current_stream()),
-              "moe_gate")
-
-    def _fused_experts(self, li, out, residual):
-        """shared expert (model_deepseek_v3.py:936-949) + routed experts (fused_experts, :995-1009) in ONE grouped fp8
-        GEMM pass: the shared expert is slot `topk` of every token with weight 1"""
-        c, L = self.cfg, self.layers[li]
-        check(self.lib.chitu_b200_fused_experts(
-            ptr(self.xn), ptr(L["we1"]), ptr(L["we2"]), ptr(L["we1_s"]), ptr(L["we2_s"]), ptr(self.gate_w_all[li]),
-            _lib.CB_BF16, ptr(self.gate_i_all[li]), _lib.CB_I64, self.B, self.topk1, c.n_routed_experts + 1,
-            2 * self.F_moe, c.dim, 1, ptr(out), ptr(residual), ptr(self.moe_ws), self.moe_ws.numel(), current_stream()),
-            "fused_experts")
-
     def _mla_prep(self, li):
         """rotary(q_pe, k_pe) + kv_norm + cat + W_UK absorption in one launch"""
         c, L = self.cfg, self.layers[li]
@@ -262,32 +219,26 @@ class DeepSeekDecodeEngine(DecodeEngine):
                                            c.qk_nope_head_dim, c.v_head_dim, self.C, self.R, c.norm_eps, current_stream()),
               "mla_prep")
 
-    def _mla_decode(self, li, out):
-        """paged absorbed-MLA decode, appending new_kv; out = None leaves the split-KV partials in the workspace"""
+    def _mla_decode(self, li):
+        """paged absorbed-MLA decode, appending new_kv; the split-KV partials stay in the workspace"""
         if self.kv_cache.dtype == F8:
             check(self.lib.chitu_b200_mla_attn_fp8kv(
                 ptr(self.q_abs), ptr(self.q_pe), ptr(self.kv_cache[li]), ptr(self.new_kv), ptr(self.seq_lens),
                 ptr(self.block_table), self.max_blocks, self.B, 1, self.H, self.C, self.R, self.page,
-                self.kv_cache.shape[1], self.max_seq_len, 1, float(self.cfg.softmax_scale), ptr(out), ptr(self.attn_ws),
+                self.kv_cache.shape[1], self.max_seq_len, 1, float(self.cfg.softmax_scale), None, ptr(self.attn_ws),
                 self.attn_ws.numel(), current_stream()), "mla_attn_fp8kv")
             return
         check(self.lib.chitu_b200_mla_decode(ptr(self.q_abs), ptr(self.q_pe), ptr(self.kv_cache[li]), ptr(self.new_kv),
                                              ptr(self.seq_lens), ptr(self.block_table), self.max_blocks, self.B, self.H,
                                              self.C, self.R, self.page, self.kv_cache.shape[1], self.max_seq_len,
-                                             float(self.cfg.softmax_scale), ptr(out), ptr(self.attn_ws),
+                                             float(self.cfg.softmax_scale), None, ptr(self.attn_ws),
                                              self.attn_ws.numel(), current_stream()), "mla_decode")
 
     # ---- one decode step ---------------------------------------------------------------------------
     def _decode_layers(self):
-        if self.trace is None:
-            self._layers_fast()
-        else:
-            self._layers_traced()
-
-    def _layers_fast(self):
-        """Production flow: every RMSNorm is fused either into the collective that precedes it (tensor parallel:
-        all-reduce + residual + norm + quant in one kernel) or into a norm+quant kernel; residual adds ride in
-        the GEMM / expert-combine epilogues.  Arithmetic is identical to `_layers_traced`."""
+        """Every RMSNorm is fused either into the collective that precedes it (tensor parallel: all-reduce + residual +
+        norm + quant in one kernel) or into a norm+quant kernel; residual adds ride in the GEMM / expert-combine
+        epilogues."""
         lib, B, c = self.lib, self.B, self.cfg
         st = current_stream()
         h, h2 = self.h, self.h2
@@ -301,11 +252,14 @@ class DeepSeekDecodeEngine(DecodeEngine):
             is_moe = li >= c.n_dense_layers
             # ---------------- attention ----------------
             self._fp8_gemm(L["wqkv_a"], L["wqkv_a_s"], self.qkv_a, B)
-            self._rms_quant(self.qkv_a, L["q_norm"], c.q_lora_rank, B, xs=c.q_lora_rank + self.C + self.R)
+            # q_norm fused with the act_quant of wq_b's input
+            check(lib.chitu_b200_rmsnorm_quant_fp8(ptr(self.qkv_a), ptr(L["q_norm"]), None, ptr(self.xq), ptr(self.xs), B,
+                                                   c.q_lora_rank, c.q_lora_rank + self.C + self.R, c.q_lora_rank,
+                                                   c.norm_eps, st), "rmsnorm_quant")
             self._fp8_gemm(L["wq_b"], L["wq_b_s"], self.q, B)
             self._mla_prep(li)
             # split-KV partials stay in the workspace; the LSE merge happens inside the absorb-o kernel
-            self._mla_decode(li, None)
+            self._mla_decode(li)
             check(lib.chitu_b200_mla_absorb_o_merge_quant(ptr(self.attn_ws), self.attn_ws.numel(), self.max_seq_len,
                                                           ptr(L["wkv_b_bf16"]), None, None, ptr(self.xq), ptr(self.xs),
                                                           B, self.H, c.qk_nope_head_dim, c.v_head_dim, self.C, st),
@@ -323,92 +277,32 @@ class DeepSeekDecodeEngine(DecodeEngine):
                                    lambda: self.comm.fp8_gemm_push(self.xq, self.xs, L["w2"], L["w2_s"], B, self.lin_ws),
                                    h2, h, next_norm, partial=self.y, **self._norm_out(last))
             else:
-                self._moe_gate(li)
-                self._row_parallel(lambda out, res: self._fused_experts(li, out, res),
-                                   lambda: self.comm.experts_push(self.xn, L["we1"], L["we2"], L["we1_s"], L["we2_s"],
-                                                                  self.gate_w_all[li], _lib.CB_BF16, self.gate_i_all[li],
-                                                                  _lib.CB_I64, B, self.topk1, c.n_routed_experts + 1,
-                                                                  2 * self.F_moe, c.dim, 1, self.moe_ws),
-                                   h2, h, next_norm, partial=self.y, **self._norm_out(last))
+                # shared expert (model_deepseek_v3.py:936-949) + routed experts (fused_experts, :995-1009) in ONE
+                # grouped fp8 GEMM pass: the shared expert is slot `topk` of every token with weight 1
+                self._moe_block(li, h2, h, next_norm, **self._norm_out(last))
         if self.capture_h is not None:
             self.capture_h.append(h.clone())
 
-    def _layers_traced(self):
-        """The unfused flow, recording the intermediates of every layer into a new dict in self.trace (the
-        stage-by-stage test compares each with the oracle): the attention output lands in o_lat before absorb-o, an
-        extra SiLU launch exposes the dense FFN activation, and the residual adds and all-reduces run outside the GEMMs."""
-        lib, B, c = self.lib, self.B, self.cfg
-        st = current_stream()
-        h, h2 = self.h, self.h2
-        for li, L in enumerate(self.layers):
-            tr = {"h_in": h.clone()}
-            self.trace.append(tr)
-            # ---------------- attention (decode_forward_paged, :672-699) ----------------
-            self._rms_quant(h, L["attn_norm"], c.dim, B, y=self.xn)
-            tr["xn_attn"] = self.xn.clone()
-            self._fp8_gemm(L["wqkv_a"], L["wqkv_a_s"], self.qkv_a, B)
-            tr["qkv_a"] = self.qkv_a.clone()
-            self._rms_quant(self.qkv_a, L["q_norm"], c.q_lora_rank, B, xs=c.q_lora_rank + self.C + self.R, y=self.qa_n)
-            tr["qa_n"] = self.qa_n.clone()
-            self._fp8_gemm(L["wq_b"], L["wq_b_s"], self.q, B)
-            tr["q"] = self.q.clone()
-            self._mla_prep(li)
-            tr["q_pe"], tr["q_abs"], tr["new_kv"] = self.q_pe.clone(), self.q_abs.clone(), self.new_kv.clone()
-            tr["cache_before"], tr["lens"] = self.kv_cache[li].clone(), self.seq_lens.clone()
-            self._mla_decode(li, self.o_lat)
-            # absorb_o fused with the act_quant of the `wo` linear (one head = one 128-wide group)
-            check(lib.chitu_b200_mla_absorb_o_quant(ptr(self.o_lat), ptr(L["wkv_b_bf16"]), ptr(self.o), ptr(self.xq),
-                                                    ptr(self.xs), B, self.H, c.qk_nope_head_dim, c.v_head_dim, self.C, st),
-                  "absorb_o")
-            tr["o_lat"], tr["o"] = self.o_lat.clone(), self.o.clone()
-            self._fp8_gemm(L["wo"], L["wo_s"], h2, B)
-            tr["attn_out"] = h2.clone()
-            self._allreduce(h2)
-            self._add(h2, h, h2)                                # x = x + attn(...)
-            tr["h_mid"] = h2.clone()
-            # ---------------- FFN ----------------
-            self._rms_quant(h2, L["ffn_norm"], c.dim, B, y=self.xn)         # bf16 copy feeds the gate / experts
-            tr["xn_ffn"] = self.xn.clone()
-            if li < c.n_dense_layers:
-                self._fp8_gemm(L["w13"], L["w13_s"], self.ff, B)
-                check(lib.chitu_b200_silu_and_mul(ptr(self.ff), ptr(self.act), B, self.F_dense, _lib.CB_BF16, st), "silu")
-                tr["ff"], tr["act"] = self.ff.clone(), self.act.clone()
-                check(lib.chitu_b200_silu_mul_quant_fp8(ptr(self.ff), ptr(self.xq), ptr(self.xs), B, self.F_dense, st),
-                      "silu_quant")
-                self._fp8_gemm(L["w2"], L["w2_s"], self.y, B)
-            else:
-                self._moe_gate(li)
-                self._fused_experts(li, self.y, None)
-            tr["y"] = self.y.clone()
-            self._allreduce(self.y)
-            self._add(self.y, h2, h)                            # x = x + ffn(...)
-            tr["h_out"] = h.clone()
-        self._rms(h, self.norm, self.xn, B, c.dim)
-
-    def distinct_experts_per_layer(self) -> float:
-        """Mean number of distinct routed experts per MoE layer in the last step."""
-        c = self.cfg
-        ids = self.gate_i_all[c.n_dense_layers:, :, : c.n_activated_experts].cpu()
-        if ids.numel() == 0:
-            return 0.0
-        return float(sum(len(torch.unique(ids[l])) for l in range(ids.shape[0])) / ids.shape[0])
-
     # ---- algorithmic bytes of one step on this rank (SURVEY §8d formula) ---------------------------
     def algorithmic_bytes(self, seq_len: int, distinct_experts_per_layer: Optional[float] = None) -> int:
+        """Every attention and dense-FFN weight byte once, the router, the shared expert and each DISTINCT routed
+        expert once, KV rows once, the bf16 head.  The weights count the bytes of the tensors the engine holds: fp8
+        weights with their block scales (wkv_b, not its dequantised copy), the bf16 router without its bias."""
         c = self.cfg
-
-        def fp8_bytes(n, k):
-            return n * k + ((n + 127) // 128) * ((k + 127) // 128) * 4
-
-        attn = (fp8_bytes(c.q_lora_rank + self.C + self.R, c.dim) + fp8_bytes(self.H * self.qk_head, c.q_lora_rank)
-                + fp8_bytes(self.H * (c.qk_nope_head_dim + c.v_head_dim), self.C) + fp8_bytes(c.dim, self.H * c.v_head_dim))
-        dense = fp8_bytes(2 * self.F_dense, c.dim) + fp8_bytes(c.dim, self.F_dense)
-        expert = fp8_bytes(2 * self.F_moe, c.dim) + fp8_bytes(c.dim, self.F_moe)
-        if distinct_experts_per_layer is None:
-            distinct_experts_per_layer = c.n_routed_experts * (1 - (1 - c.n_activated_experts / c.n_routed_experts) ** self.B)
-        moe = c.n_routed_experts * c.dim * 2 + (c.n_shared_experts + distinct_experts_per_layer) * expert
-        kv = self.B * (seq_len + 1) * (self.C + self.R) * self.kv_cache.element_size()
-        n_moe = max(c.n_layers - c.n_dense_layers, 0)
         n_dense = min(c.n_layers, c.n_dense_layers)
-        head = self.head.numel() * 2
-        return int(c.n_layers * (attn + kv) + n_dense * dense + n_moe * moe + head)
+        n_moe = c.n_layers - n_dense
+
+        def nbytes(li, *names):
+            return sum(self.layers[li][n].nbytes for n in names)
+
+        attn = nbytes(0, "wqkv_a", "wqkv_a_s", "wq_b", "wq_b_s", "wkv_b", "wkv_b_s", "wo", "wo_s")
+        dense = nbytes(0, "w13", "w13_s", "w2", "w2_s") if n_dense else 0
+        moe = 0
+        if n_moe:
+            if distinct_experts_per_layer is None:
+                distinct_experts_per_layer = c.n_routed_experts * (1 - (1 - c.n_activated_experts / c.n_routed_experts)
+                                                                   ** self.B)
+            expert = nbytes(-1, "we1", "we1_s", "we2", "we2_s") // (c.n_routed_experts + 1)
+            moe = nbytes(-1, "gate_w") + (c.n_shared_experts + distinct_experts_per_layer) * expert
+        kv = self.B * (seq_len + 1) * (self.C + self.R) * self.kv_cache.element_size()
+        return int(c.n_layers * (attn + kv) + n_dense * dense + n_moe * moe + self.head.nbytes)

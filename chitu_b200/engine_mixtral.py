@@ -15,7 +15,6 @@ push epilogue, so it runs on one GPU or in shard mode.
 """
 from __future__ import annotations
 
-import math
 from dataclasses import dataclass
 
 import torch
@@ -65,11 +64,7 @@ class MixtralDecodeEngine(DecodeEngine):
         self.E, self.topk = cfg.num_local_experts, cfg.num_experts_per_tok
         super().__init__(cfg, max_reqs, max_seq_len, device, page_size, seed, tp_rank, tp_size, process_group,
                          use_fused_allreduce, attn_ws=(self.Hq, D, 64), lin_n=max(cfg.vocab_size // T, cfg.dim))
-        dev, g, g_rep = self.device, self.g, self.g_rep
-
-        def rnd(gen, *shape, scale=0.02):
-            return (torch.randn(*shape, generator=gen, dtype=torch.float32, device=dev) * scale).to(BF)
-
+        dev, g, g_rep, rnd = self.device, self.g, self.g_rep, self._rnd
         dim = cfg.dim
         self.embed = rnd(g_rep, cfg.vocab_size, dim)
         self.layers = []
@@ -83,28 +78,15 @@ class MixtralDecodeEngine(DecodeEngine):
             self.layers.append(self._quantized(lw))
         self.norm = torch.ones(dim, dtype=BF, device=dev)
         self.head = rnd(g, cfg.vocab_size // T, dim)
-        nblk = self.max_blocks * max_reqs
-        self.k_cache = torch.zeros(cfg.n_layers, nblk, page_size, self.Hkv, D, dtype=BF, device=dev)
-        self.v_cache = torch.zeros_like(self.k_cache)
-        self.caches = (self.k_cache, self.v_cache)
+        self._gqa_buffers(BF, max_reqs)
         # hf rotary: cos/sin [pos, D/2] in the model dtype, half-split layout (ops.py:243-308 "hf-llama")
         freqs = 1.0 / (cfg.rope_theta ** (torch.arange(0, D, 2).float() / D))
         self._rope_tables(torch.outer(torch.arange(max_seq_len * 2, dtype=torch.float32), freqs), BF)
-        B = max_reqs
-        z = lambda *s, dt=BF: torch.zeros(*s, dtype=dt, device=dev)
-        self.y = z(B, dim)
-        self.qkv = z(B, (self.Hq + 2 * self.Hkv) * D)
-        self.q_rot, self.k_rot = z(B, self.Hq, D), z(B, self.Hkv, D)
-        self.attn_out = z(B, self.Hq * D)
-        self.gate_w_all = z(cfg.n_layers, B, self.topk)
-        self.gate_i_all = torch.zeros(cfg.n_layers, B, self.topk, dtype=torch.int64, device=dev)
-        lib = self.lib
-        self.moe_ws = torch.zeros(lib.chitu_b200_moe_workspace_bytes(B, self.topk, self.E, 2 * self.F, dim), dtype=torch.uint8,
-                                  device=dev)
-        self.gate_ws = torch.zeros(lib.chitu_b200_moe_gate_workspace_bytes(B, self.E), dtype=torch.uint8, device=dev)
+        # softmax over the E experts -> top-2 -> renormalise (model_hf_mixtral.py:57-64)
+        self._init_moe(n_routed=self.E, topk=self.topk, slots=self.topk, n_stacked=self.E, n1=2 * self.F, score_mode=2)
 
     def _decode_layers(self):
-        lib, B, D, cfg = self.lib, self.B, self.D, self.cfg
+        lib, B, D = self.lib, self.B, self.D
         st = current_stream()
         h, h2 = self.h, self.h2
         qkv_w = (self.Hq + 2 * self.Hkv) * D
@@ -117,55 +99,24 @@ class MixtralDecodeEngine(DecodeEngine):
             self._layer_linear(self.xn, lw, "wqkv", self.qkv, B)
             q = self.qkv[:, : self.Hq * D]
             k = self.qkv[:, self.Hq * D: (self.Hq + self.Hkv) * D]
-            v_view = self.qkv[:, (self.Hq + self.Hkv) * D:]
             # apply_rotary_pos_emb(..., "hf-llama") on the q / k views of the merged qkv output
             check(lib.chitu_b200_rotary_half_strided(ptr(q), qkv_w, ptr(self.q_rot), ptr(self.cos), ptr(self.sin), B, self.Hq, D,
                                                      _lib.CB_BF16, st), "rotary_half q")
             check(lib.chitu_b200_rotary_half_strided(ptr(k), qkv_w, ptr(self.k_rot), ptr(self.cos), ptr(self.sin), B, self.Hkv, D,
                                                      _lib.CB_BF16, st), "rotary_half k")
-            check(lib.chitu_b200_gqa_paged_decode(
-                ptr(self.q_rot), ptr(self.k_cache[li]), ptr(self.v_cache[li]), ptr(self.k_rot), ptr(v_view),
-                self.Hkv * D, qkv_w, ptr(self.seq_lens), ptr(self.block_table), self.max_blocks, B, self.Hq, self.Hkv, D,
-                self.page, self.max_seq_len, 1.0 / math.sqrt(D), ptr(self.attn_out), ptr(self.attn_ws),
-                self.attn_ws.numel(), _lib.CB_BF16, st), "gqa_paged_decode")
+            self._gqa_decode(li)
             self._row_parallel(lambda out, res: self._layer_linear(self.attn_out, lw, "wo", out, B, residual=res),
                                lambda: self.comm.linear_push(self.attn_out, lw["wo"], B, self.lin_ws),
                                h, h2, lw["ffn_norm"], y=self.xn)
             # ---- sparse MoE block (model_hf_mixtral.py:51-96) through the fused experts ----
-            check(lib.chitu_b200_moe_gate(ptr(self.xn), ptr(lw["gate_w"]), None, 0, B, cfg.dim, self.E, 1, 1, self.topk, 2,
-                                          1.0, ptr(self.gate_w_all[li]), ptr(self.gate_i_all[li]), self.topk,
-                                          ptr(self.gate_ws), self.gate_ws.numel(), st), "moe_gate")
-            self._row_parallel(
-                lambda out, res: self._experts(li, lw, out, res),
-                lambda: self.comm.experts_push(self.xn, lw["w1"], lw["w2"], None, None, self.gate_w_all[li], _lib.CB_BF16,
-                                               self.gate_i_all[li], _lib.CB_I64, B, self.topk, self.E, 2 * self.F, cfg.dim, 0,
-                                               self.moe_ws),
-                h2, h, next_norm, y=self.xn, partial=self.y)
+            self._moe_block(li, h2, h, next_norm, y=self.xn)
         if self.capture_h is not None:
             self.capture_h.append(h.clone())
-
-    def _experts(self, li, lw, out, res):
-        """out = the fused experts of layer li on self.xn (+ res) in the engine's weight format."""
-        lib, B, st = self.lib, self.B, current_stream()
-        route = (ptr(self.gate_w_all[li]), _lib.CB_BF16, ptr(self.gate_i_all[li]), _lib.CB_I64, B, self.topk, self.E,
-                 2 * self.F, self.cfg.dim)
-        tail = (ptr(out), ptr(res), ptr(self.moe_ws), self.moe_ws.numel(), st)
-        if self.weight_format == "bf16":
-            check(lib.chitu_b200_fused_experts(ptr(self.xn), ptr(lw["w1"]), ptr(lw["w2"]), None, None, *route, 0, *tail),
-                  "fused_experts")
-        else:
-            (q1, s1, z1), (q2, s2, z2) = lw["w1"], lw["w2"]
-            check(lib.chitu_b200_fused_experts_w4a16(ptr(self.xn), ptr(q1), ptr(s1), ptr(z1), ptr(q2), ptr(s2), ptr(z2),
-                                                     *route, *tail), "fused_experts_w4a16")
 
     def ref_layers(self):
         """The layer weights as the reference multiplies them (the 4-bit ones dequantised) for the oracle side of the
         tests."""
         return [self._dequantized(lw) for lw in self.layers]
-
-    def distinct_experts_per_layer(self) -> float:
-        ids = self.gate_i_all.cpu()
-        return float(sum(len(torch.unique(ids[l])) for l in range(ids.shape[0])) / ids.shape[0])
 
     def algorithmic_bytes(self, seq_len: int, distinct: float) -> int:
         """SURVEY §8d: every attention weight byte once, each DISTINCT expert once, KV rows once, bf16 head + router.

@@ -146,52 +146,48 @@ _VERIFY = dict(max_draft=3)
 _SAMPLED = dict(max_draft=3, sampled_verify=True)
 STEP, VERIFY = "_step_body", "_verify_body"
 
-# mode -> (engine factory, reduce mode under tensor parallelism: "push" / "pull" (fake comm) / "nccl" (no comm), traced,
+# mode -> (engine factory, reduce mode under tensor parallelism: "push" / "pull" (fake comm) / "nccl" (no comm),
 #          the engine method that runs the step: the decode step or the speculative verify step)
 MODES = {
-    "llama_single_rope": (lambda: _llama(128), None, False, STEP),
-    "llama_single_unfused_rope": (lambda: _llama(64), None, False, STEP),
-    "llama_linear_impl1": (lambda: _llama(128, linear_impl=1), None, False, STEP),
-    "llama_tp_push": (lambda: _llama(128, **_TP), "push", False, STEP),
-    "llama_tp_pull": (lambda: _llama(128, **_TP), "pull", False, STEP),
-    "llama_tp_nccl": (lambda: _llama(128, **_TP), "nccl", False, STEP),
-    "deepseek_single": (lambda: _deepseek(tp_size=1), None, False, STEP),
-    "deepseek_shard": (lambda: _deepseek(tp_size=2), None, False, STEP),
-    "deepseek_tp_push": (lambda: _deepseek(**_TP), "push", False, STEP),
-    "deepseek_tp_pull": (lambda: _deepseek(**_TP), "pull", False, STEP),
-    "deepseek_tp_nccl": (lambda: _deepseek(**_TP), "nccl", False, STEP),
-    "deepseek_traced_single": (lambda: _deepseek(tp_size=1), None, True, STEP),
-    "deepseek_traced_tp": (lambda: _deepseek(**_TP), "nccl", True, STEP),
-    "mixtral_shard": (lambda: _mixtral(tp_size=2), None, False, STEP),
-    "mixtral_tp_push": (lambda: _mixtral(**_TP), "push", False, STEP),
-    "mixtral_tp_pull": (lambda: _mixtral(**_TP), "pull", False, STEP),
-    "mixtral_tp_nccl": (lambda: _mixtral(**_TP), "nccl", False, STEP),
-    "llama_w4a16": (lambda: _llama(128, weight_format="w4a16"), None, False, STEP),
-    "llama_w4a16_shard": (lambda: _llama(128, tp_size=2, weight_format="w4a16"), None, False, STEP),
-    "llama_fp8": (lambda: _llama(128, weight_format="fp8"), None, False, STEP),
-    "llama_fp8_e4m3_kv": (lambda: _llama(128, weight_format="fp8", **_E4M3), None, False, STEP),
-    "mixtral_w4a16": (lambda: _mixtral(tp_size=1, weight_format="w4a16"), None, False, STEP),
-    "mixtral_w4a16_shard": (lambda: _mixtral(tp_size=2, weight_format="w4a16"), None, False, STEP),
-    "llama_verify": (lambda: _llama(128, **_VERIFY), None, False, VERIFY),
-    "llama_verify_tp_push": (lambda: _llama(128, **_VERIFY, **_TP), "push", False, VERIFY),
-    "llama_verify_w4a16": (lambda: _llama(128, **_VERIFY, weight_format="w4a16"), None, False, VERIFY),
-    "llama_verify_fp8_e4m3_kv": (lambda: _llama(128, **_VERIFY, weight_format="fp8", **_E4M3), None, False, VERIFY),
+    "llama_single_rope": (lambda: _llama(128), None, STEP),
+    "llama_single_unfused_rope": (lambda: _llama(64), None, STEP),
+    "llama_linear_impl1": (lambda: _llama(128, linear_impl=1), None, STEP),
+    "llama_tp_push": (lambda: _llama(128, **_TP), "push", STEP),
+    "llama_tp_pull": (lambda: _llama(128, **_TP), "pull", STEP),
+    "llama_tp_nccl": (lambda: _llama(128, **_TP), "nccl", STEP),
+    "deepseek_single": (lambda: _deepseek(tp_size=1), None, STEP),
+    "deepseek_shard": (lambda: _deepseek(tp_size=2), None, STEP),
+    "deepseek_tp_push": (lambda: _deepseek(**_TP), "push", STEP),
+    "deepseek_tp_pull": (lambda: _deepseek(**_TP), "pull", STEP),
+    "deepseek_tp_nccl": (lambda: _deepseek(**_TP), "nccl", STEP),
+    "mixtral_shard": (lambda: _mixtral(tp_size=2), None, STEP),
+    "mixtral_tp_push": (lambda: _mixtral(**_TP), "push", STEP),
+    "mixtral_tp_pull": (lambda: _mixtral(**_TP), "pull", STEP),
+    "mixtral_tp_nccl": (lambda: _mixtral(**_TP), "nccl", STEP),
+    "llama_w4a16": (lambda: _llama(128, weight_format="w4a16"), None, STEP),
+    "llama_w4a16_shard": (lambda: _llama(128, tp_size=2, weight_format="w4a16"), None, STEP),
+    "llama_fp8": (lambda: _llama(128, weight_format="fp8"), None, STEP),
+    "llama_fp8_e4m3_kv": (lambda: _llama(128, weight_format="fp8", **_E4M3), None, STEP),
+    "mixtral_w4a16": (lambda: _mixtral(tp_size=1, weight_format="w4a16"), None, STEP),
+    "mixtral_w4a16_shard": (lambda: _mixtral(tp_size=2, weight_format="w4a16"), None, STEP),
+    "llama_verify": (lambda: _llama(128, **_VERIFY), None, VERIFY),
+    "llama_verify_tp_push": (lambda: _llama(128, **_VERIFY, **_TP), "push", VERIFY),
+    "llama_verify_w4a16": (lambda: _llama(128, **_VERIFY, weight_format="w4a16"), None, VERIFY),
+    "llama_verify_fp8_e4m3_kv": (lambda: _llama(128, **_VERIFY, weight_format="fp8", **_E4M3), None, VERIFY),
     "llama_verify_sampled_fp8_draft_probs": (lambda: _llama(128, **_SAMPLED, weight_format="fp8", draft_probs=True),
-                                             None, False, VERIFY),
-    "llama_verify_sampled": (lambda: _llama(128, **_SAMPLED), None, False, VERIFY),
+                                             None, VERIFY),
+    "llama_verify_sampled": (lambda: _llama(128, **_SAMPLED), None, VERIFY),
 }
 
 
 def trace(mode):
-    make, reduce, traced, body = MODES[mode]
+    make, reduce, body = MODES[mode]
     rec = Recorder()
     with _patched(rec):
         eng = make()
         if reduce is not None:
             eng.comm = None if reduce == "nccl" else FakeComm(rec)
             eng.ar_push = reduce == "push"
-        if traced:
-            eng.trace = []
         rec.watch(eng)
         getattr(eng, body)()
     return json.loads(json.dumps(rec.calls))

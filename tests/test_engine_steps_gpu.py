@@ -86,7 +86,7 @@ VARIANTS = {
     "llama_e4m3_kv": Variant("llama", (("kv_dtype", F8),)),                   # gqa_paged_attn_fp8kv
     "llama_tp2_shard": Variant("llama", (("tp_size", 2),)),                   # per-rank heads, vocabulary shard
     "mixtral_tp2_shard": Variant("mixtral", (("tp_size", 2),)),               # rotary_half_strided, bf16 experts
-    "deepseek_tp2_shard": Variant("deepseek", (("tp_size", 2),)),             # _layers_fast over a bf16 latent cache
+    "deepseek_tp2_shard": Variant("deepseek", (("tp_size", 2),)),             # mla_decode over a bf16 latent cache
     "deepseek_tp2_e4m3": Variant("deepseek", (("tp_size", 2), ("kv_dtype", F8))),   # mla_attn_fp8kv
 }
 
@@ -281,6 +281,10 @@ def test_engine_steps(name):
                 "rewound replay changed the caches"
         assert torch.equal(A.seq_lens, lens + 1)
         assert torch.equal(A.next_tokens, A.logits.float().argmax(dim=-1)), "next token is not the first maximal index"
+        if v.family == "deepseek":        # the shared expert: the last routing slot of every MoE token, weight 1
+            nd = A.cfg.n_dense_layers
+            assert bool((A.gate_i_all[nd:, :, -1] == A.cfg.n_routed_experts).all())
+            assert bool((A.gate_w_all[nd:, :, -1] == 1).all())
         for li in range(n_layers):
             caches, routes = [c.clone() for c in before[li]], []
             ref = m.layer(li, hs[li], caches, lens, routes=routes)

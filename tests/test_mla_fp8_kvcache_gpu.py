@@ -331,8 +331,6 @@ def test_prefill_scatter_stores_by_the_clamp_rule():
 
 @gpu
 def test_deepseek_engine_fp8_cache():
-    from chitu_b200 import _lib
-    from chitu_b200._lib import current_stream, ptr
     from chitu_b200.engine_deepseek import DeepSeekConfig, DeepSeekDecodeEngine
     cfg = DeepSeekConfig(vocab_size=1024, dim=512, inter_dim=1024, moe_inter_dim=256, n_layers=2, n_dense_layers=1,
                          n_heads=4, n_routed_experts=16, n_activated_experts=4, n_expert_groups=4, n_limited_groups=2,
@@ -347,27 +345,8 @@ def test_deepseek_engine_fp8_cache():
     eb.block_table.copy_(e8.block_table)
     eb.seq_lens.copy_(lens)
     eb.kv_cache.copy_(e8.kv_cache.float().bfloat16())
-    cache0 = e8.kv_cache.clone()
     eb.decode(tokens.pin_memory())
     e8.decode(tokens.pin_memory())
     torch.cuda.synchronize()
     got, want = e8.logits.float().cpu(), eb.logits.float().cpu()
     assert cos_diff(got, want) < 1e-2 and max_rel(got, want) < 0.15
-    # stage by stage: each layer's attention output equals the bf16 kernel on the decoded cache with the rounded row
-    e8.kv_cache.copy_(cache0)
-    e8.seq_lens.copy_(lens)
-    e8.trace = []
-    e8.decode(tokens.pin_memory())
-    torch.cuda.synchronize()
-    lib = _lib.load()
-    for li, tr in enumerate(e8.trace):
-        dec = tr["cache_before"].float().bfloat16()
-        nk = quant(tr["new_kv"]).float().bfloat16()
-        o = torch.empty_like(tr["o_lat"])
-        assert lib.chitu_b200_mla_decode(ptr(tr["q_abs"]), ptr(tr["q_pe"]), ptr(dec), ptr(nk), ptr(tr["lens"]),
-                                         ptr(e8.block_table), e8.max_blocks, B, e8.H, e8.C, e8.R, PAGE, dec.shape[0],
-                                         e8.max_seq_len, float(cfg.softmax_scale), ptr(o), ptr(e8.attn_ws),
-                                         e8.attn_ws.numel(), current_stream()) == 0
-        torch.cuda.synchronize()
-        assert _same_bits(o, tr["o_lat"]), li
-        assert _same_bits(e8.kv_cache[li].float().bfloat16(), dec)           # the twin's append stored the same row
