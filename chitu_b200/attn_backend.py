@@ -20,7 +20,7 @@ import torch
 from . import _lib, workspace
 from ._lib import check, current_stream, dtype_code, ptr, require_cuda
 
-__all__ = ["AttnBackend", "B200AttnBackend"]
+__all__ = ["AttnBackend", "B200AttnBackend", "gqa_paged_attention", "mla_paged_attention"]
 
 _MLA_QK, _MLA_V = 576, 512          # absorbed MLA: kv_lora_rank + qk_rope_head_dim, kv_lora_rank
 
@@ -216,7 +216,7 @@ class B200AttnBackend(AttnBackend):
         Built for D == 128, Hq / Hkv in {1, 2, 4, 8} and a power-of-two page that is a multiple of 64; no host
         synchronisation, capturable in a CUDA graph, deterministic."""
         B, sq, Hq, D = q.shape
-        num_blocks, page, Hkv, Dk = k_cache.shape
+        _, page, Hkv, Dk = k_cache.shape
         assert Dk == D and v_cache.shape == k_cache.shape
         if fp8:
             assert q.dtype in (torch.bfloat16, torch.float16)
@@ -227,23 +227,9 @@ class B200AttnBackend(AttnBackend):
         cache_seqlens = self._seqlens(q, cache_seqlens)
         strides, scale, hint = self._kv_args(q, k, v, Hkv, cache_seqlens, softmax_scale, block_table.shape[1] * page)
         out = torch.empty_like(q)
-        ws, wsn = self._ws(B, Hq, D, q.device)
-        lib, bt = _lib.load(), (ptr(block_table), block_table.stride(0))
-        if fp8:
-            check(lib.chitu_b200_gqa_paged_attn_fp8kv(
-                ptr(q), sq * Hq * D, ptr(k_cache), ptr(v_cache), ptr(k), ptr(v), *strides, None, None,
-                ptr(cache_seqlens), *bt, B, sq, Hq, Hkv, D, page, num_blocks, hint, int(bool(causal)), scale, ptr(out),
-                ptr(ws), wsn, dtype_code(q.dtype), current_stream()), "gqa_paged_attn_fp8kv")
-        elif sq == 1:
-            check(lib.chitu_b200_gqa_paged_decode(
-                ptr(q), ptr(k_cache), ptr(v_cache), ptr(k), ptr(v), strides[0], strides[2], ptr(cache_seqlens), *bt, B,
-                Hq, Hkv, D, page, hint, scale, ptr(out), ptr(ws), wsn, dtype_code(q.dtype), current_stream()),
-                "gqa_paged_decode")
-        else:
-            check(lib.chitu_b200_gqa_paged_prefill(
-                ptr(q), ptr(k_cache), ptr(v_cache), ptr(k), ptr(v), *strides, ptr(cache_seqlens), *bt, B, sq, Hq, Hkv,
-                D, page, num_blocks, hint, int(bool(causal)), scale, ptr(out), ptr(ws), wsn, dtype_code(q.dtype),
-                current_stream()), "gqa_paged_prefill")
+        ws, _ = self._ws(B, Hq, D, q.device)
+        gqa_paged_attention(q, sq * Hq * D, k_cache, v_cache, k, v, strides, None, cache_seqlens, block_table, B, sq, Hq,
+                            hint, causal, scale, out, ws)
         return out
 
     def _contiguous(self, q, k_cache, v_cache, k, v, cache_seqlens, cache_leftpad, causal, window_size, softcap,
@@ -277,91 +263,28 @@ class B200AttnBackend(AttnBackend):
                               cache_seqlens_incl_this_decode: Union[int, torch.Tensor],
                               block_table: torch.Tensor, causal=True, window_size=(-1, -1), softcap=0.0,
                               softmax_scale=None):
-        """Absorbed-MLA attention over the paged latent cache.  q_nope [B, H, C] (or [B, 1, H, C]): one decode token
-        per request with the fused append of `kv` (chitu_b200_mla_decode), returned as [B, 1, H, C].
-        q_nope [B, sq, H, C] with sq > 1: multi-token-prediction verification or chunked prefill, see
-        `_mla_paged_prefill`.  A kv_cache in torch.float8_e4m3fn takes both call shapes through `_mla_fp8kv`."""
-        require_cuda(q_nope, q_pe, kv_cache, block_table)
-        if kv_cache.dtype == torch.float8_e4m3fn:
-            return self._mla_fp8kv(q_nope, q_pe, kv_cache, kv, cache_seqlens_excl_this_decode, block_table, causal,
-                                   window_size, softcap, softmax_scale)
-        if q_nope.dim() == 4:
-            B, sq, H, C = q_nope.shape
-            if sq > 1:
-                return self._mla_paged_prefill(q_nope, q_pe, kv_cache, kv, cache_seqlens_excl_this_decode, block_table,
-                                               causal, window_size, softcap, softmax_scale)
-            q_nope, q_pe = q_nope.view(B, H, C), q_pe.view(B, H, q_pe.shape[-1])
-        assert kv_cache.ndim == 3  # (num_blocks, block_size, dim)
-        B, H, C = q_nope.shape
-        R = q_pe.shape[-1]
-        page = kv_cache.size(1)
-        assert kv_cache.size(2) == C + R
-        assert q_nope.is_contiguous() and q_pe.is_contiguous() and kv_cache.is_contiguous()
-        assert q_nope.dtype == torch.bfloat16 and kv_cache.dtype == torch.bfloat16
-        assert block_table.dtype == torch.int32 and block_table.stride(-1) == 1
+        """Absorbed-MLA attention over the paged latent cache kv_cache [num_blocks, 64, C + R], bf16 q / kv / output.
+        q_nope [B, H, C] (or [B, 1, H, C]): one decode token per request with the fused append of `kv` and the device
+        split plan of prepare_metadata_for_decode, returned as [B, 1, H, C].  q_nope [B, sq, H, C] with sq > 1:
+        multi-token-prediction verification or chunked prefill; the B * sq rows of `kv` ([B, sq, C + R] in any
+        contiguous shape, or None) are appended at seq_excl[b] + i, then query i attends to the first seq_excl[b] + sq
+        keys (without kv: seq_excl[b]), bottom-right causal when `causal`; returns [B, sq, H, C].  softmax_scale=None
+        means 1 / sqrt(qk_rope_head_dim + qk_nope_head_dim); window_size and softcap are not built.
+        A kv_cache in torch.float8_e4m3fn takes both call shapes with the same semantics, each new kv element stored as
+        x.float().clamp(-448, 448).to(float8_e4m3fn) and each cache element decoded exactly to bf16 before the unchanged
+        arithmetic; the appended rows are attended in their stored form.  No host synchronisation, capturable in a CUDA
+        graph, deterministic."""
         seq_excl = cache_seqlens_excl_this_decode
-        assert seq_excl.dtype == torch.int32 and seq_excl.is_contiguous()
-        new_kv = None
-        if kv is not None:
-            new_kv = kv.reshape(B, C + R)
-            assert new_kv.is_contiguous()
-        if softmax_scale is None:
-            softmax_scale = 1.0 / ((self.qk_rope_head_dim + self.qk_nope_head_dim) ** 0.5)
-        o = torch.empty(B, H, C, dtype=q_nope.dtype, device=q_nope.device)
-        ws, wsn = self._ws(B, H, C, q_nope.device)
-        hint = self.max_seq_len if self.max_seq_len else block_table.shape[1] * page
-        check(_lib.load().chitu_b200_mla_decode(
-            ptr(q_nope), ptr(q_pe), ptr(kv_cache), ptr(new_kv), ptr(seq_excl), ptr(block_table),
-            block_table.stride(0), B, H, C, R, page, kv_cache.size(0), int(hint), float(softmax_scale), ptr(o), ptr(ws), wsn,
-            current_stream()), "mla_decode")
-        return o.view(B, 1, H, -1)
-
-    def _mla_paged_prefill(self, q_nope, q_pe, kv_cache, kv, seq_excl, block_table, causal, window_size, softcap,
-                           softmax_scale):
-        """sq > 1 query tokens per request (chitu_b200_mla_paged_prefill): the B * sq rows of `kv` ([B, sq, C + R] in
-        any contiguous shape, or None) are appended at seq_excl[b] + i, then query i attends to the first
-        seq_excl[b] + sq keys (without kv: seq_excl[b]), bottom-right causal when `causal`.  The decode arithmetic and
-        default scale; returns [B, sq, H, C] bf16.  No host synchronisation, capturable in a CUDA graph, deterministic."""
+        require_cuda(q_nope, q_pe, kv_cache, block_table, seq_excl, kv)
         if tuple(window_size) != (-1, -1) or softcap != 0.0:
-            raise RuntimeError("mla_paged_prefill: window_size and softcap are not built")
-        B, sq, H, C = q_nope.shape
-        R = q_pe.shape[-1]
-        assert kv_cache.ndim == 3 and kv_cache.size(2) == C + R and q_pe.shape == (B, sq, H, R)
-        assert q_nope.is_contiguous() and q_pe.is_contiguous() and kv_cache.is_contiguous()
-        assert q_nope.dtype == q_pe.dtype == kv_cache.dtype == torch.bfloat16
-        assert block_table.dtype == torch.int32 and block_table.stride(-1) == 1
-        assert seq_excl.dtype == torch.int32 and seq_excl.is_contiguous()
-        if kv is not None:
-            assert kv.dtype == torch.bfloat16 and kv.is_contiguous() and kv.numel() == B * sq * (C + R)
-        if softmax_scale is None:
-            softmax_scale = 1.0 / ((self.qk_rope_head_dim + self.qk_nope_head_dim) ** 0.5)
-        page = kv_cache.size(1)
-        o = torch.empty(B, sq, H, C, dtype=q_nope.dtype, device=q_nope.device)
-        ws, wsn = self._ws(B, H, C, q_nope.device)
-        hint = self.max_seq_len if self.max_seq_len else block_table.shape[1] * page
-        check(_lib.load().chitu_b200_mla_paged_prefill(
-            ptr(q_nope), ptr(q_pe), ptr(kv_cache), ptr(kv), ptr(seq_excl), ptr(block_table), block_table.stride(0), B, sq,
-            H, C, R, page, kv_cache.size(0), int(hint), int(bool(causal)), float(softmax_scale), ptr(o), ptr(ws), wsn,
-            current_stream()), "mla_paged_prefill")
-        return o
-
-    def _mla_fp8kv(self, q_nope, q_pe, kv_cache, kv, seq_excl, block_table, causal, window_size, softcap,
-                   softmax_scale):
-        """The e4m3 latent cache [num_blocks, 64, C + R] (chitu_b200_mla_attn_fp8kv), both call shapes: q_nope
-        [B, H, C] or [B, sq, H, C], bf16 q / kv / output.  The semantics of the bf16 cache, with each new kv element
-        stored as x.float().clamp(-448, 448).to(float8_e4m3fn) and each cache element decoded exactly to bf16 before
-        the unchanged arithmetic; the appended rows are attended in their stored form.  sq == 1 is the decode with the
-        fused append and the device split plan of prepare_metadata_for_decode; returns [B, sq, H, C].  No host
-        synchronisation, capturable in a CUDA graph, deterministic."""
-        if tuple(window_size) != (-1, -1) or softcap != 0.0:
-            raise RuntimeError("mla_attn_fp8kv: window_size and softcap are not built")
-        if q_nope.dtype != torch.bfloat16 or q_pe.dtype != torch.bfloat16 or (kv is not None and kv.dtype != torch.bfloat16):
-            raise RuntimeError("mla_attn_fp8kv: q_nope, q_pe and kv must be bfloat16 (only the cache is fp8)")
-        require_cuda(seq_excl, kv)
+            raise RuntimeError("mla_attn_with_kvcache: window_size and softcap are not built")
+        if any(t is not None and t.dtype != torch.bfloat16 for t in (q_nope, q_pe, kv)):
+            raise RuntimeError("mla_attn_with_kvcache: q_nope, q_pe and kv must be bfloat16 (the cache may be fp8)")
         if q_nope.dim() == 3:
             q_nope, q_pe = q_nope.unsqueeze(1), q_pe.unsqueeze(1)
         B, sq, H, C = q_nope.shape
         R = q_pe.shape[-1]
+        assert kv_cache.dtype in (torch.bfloat16, torch.float8_e4m3fn)
         assert kv_cache.ndim == 3 and kv_cache.size(2) == C + R and q_pe.shape == (B, sq, H, R)
         assert q_nope.is_contiguous() and q_pe.is_contiguous() and kv_cache.is_contiguous()
         assert block_table.dtype == torch.int32 and block_table.stride(-1) == 1
@@ -370,12 +293,72 @@ class B200AttnBackend(AttnBackend):
             assert kv.is_contiguous() and kv.numel() == B * sq * (C + R)
         if softmax_scale is None:
             softmax_scale = 1.0 / ((self.qk_rope_head_dim + self.qk_nope_head_dim) ** 0.5)
-        page = kv_cache.size(1)
         o = torch.empty(B, sq, H, C, dtype=q_nope.dtype, device=q_nope.device)
-        ws, wsn = self._ws(B, H, C, q_nope.device)
-        hint = self.max_seq_len if self.max_seq_len else block_table.shape[1] * page
-        check(_lib.load().chitu_b200_mla_attn_fp8kv(
-            ptr(q_nope), ptr(q_pe), ptr(kv_cache), ptr(kv), ptr(seq_excl), ptr(block_table), block_table.stride(0), B, sq,
-            H, C, R, page, kv_cache.size(0), int(hint), int(bool(causal)), float(softmax_scale), ptr(o), ptr(ws), wsn,
-            current_stream()), "mla_attn_fp8kv")
+        ws, _ = self._ws(B, H, C, q_nope.device)
+        hint = self.max_seq_len if self.max_seq_len else block_table.shape[1] * kv_cache.size(1)
+        mla_paged_attention(q_nope, q_pe, kv_cache, kv, seq_excl, block_table, hint, causal, softmax_scale, o, ws)
         return o
+
+
+def gqa_paged_attention(q, q_sb, k_cache, v_cache, k_new, v_new, kv_strides, rope, cache_seqlens, block_table, B, sq,
+                        Hq, max_seqlen_hint, causal, softmax_scale, out, workspace):
+    """GQA attention over the paged caches k_cache / v_cache [num_blocks, page, Hkv, D] as one C call, the entry picked
+    from the cache dtype, sq and the query layout:
+      - an e4m3 cache: chitu_b200_gqa_paged_attn_fp8kv, any sq;
+      - sq > 1: chitu_b200_gqa_paged_prefill;
+      - sq == 1 with `rope` or a strided q (q_sb != Hq * D): chitu_b200_gqa_paged_decode_rope;
+      - otherwise chitu_b200_gqa_paged_decode.
+    q: B * sq query rows, batch stride q_sb elements; k_new / v_new: the new rows or None, with strides
+    kv_strides = (k_sb, k_st, v_sb, v_st) in elements (the decode entries read only the batch strides); rope: the fp32
+    (cos, sin) [B, D / 2] of the rotary fused at sq == 1, or None; workspace: the split-KV workspace (uint8).  The entries
+    and their arguments are described in include/chitu_b200.h; the caller checks the tensors."""
+    lib = _lib.load()
+    num_blocks, page, Hkv, D = k_cache.shape
+    cos, sin = rope if rope is not None else (None, None)
+    k_sb, _, v_sb, _ = kv_strides
+    caches = (ptr(k_cache), ptr(v_cache), ptr(k_new), ptr(v_new))
+    pages = (ptr(cache_seqlens), ptr(block_table), block_table.stride(0), B)
+    hint, causal, scale = int(max_seqlen_hint), int(bool(causal)), float(softmax_scale)
+    tail = (ptr(out), ptr(workspace), workspace.numel(), dtype_code(q.dtype), current_stream())
+    if k_cache.dtype == torch.float8_e4m3fn:
+        check(lib.chitu_b200_gqa_paged_attn_fp8kv(ptr(q), q_sb, *caches, *kv_strides, ptr(cos), ptr(sin), *pages, sq, Hq,
+                                                  Hkv, D, page, num_blocks, hint, causal, scale, *tail),
+              "gqa_paged_attn_fp8kv")
+    elif sq > 1:
+        assert rope is None and q_sb == sq * Hq * D
+        check(lib.chitu_b200_gqa_paged_prefill(ptr(q), *caches, *kv_strides, *pages, sq, Hq, Hkv, D, page, num_blocks,
+                                               hint, causal, scale, *tail), "gqa_paged_prefill")
+    elif rope is not None or q_sb != Hq * D:
+        check(lib.chitu_b200_gqa_paged_decode_rope(ptr(q), q_sb, *caches, k_sb, v_sb, ptr(cos), ptr(sin), *pages, Hq,
+                                                   Hkv, D, page, hint, scale, *tail), "gqa_paged_decode_rope")
+    else:
+        check(lib.chitu_b200_gqa_paged_decode(ptr(q), *caches, k_sb, v_sb, *pages, Hq, Hkv, D, page, hint, scale,
+                                              *tail), "gqa_paged_decode")
+
+
+def mla_paged_attention(q_nope, q_pe, kv_cache, new_kv, seqlens_excl, block_table, max_seqlen_hint, causal,
+                        softmax_scale, out, workspace):
+    """Absorbed-MLA attention over the paged latent cache kv_cache [num_blocks, page, C + R] as one C call, the entry
+    picked from the cache dtype and sq:
+      - an e4m3 cache: chitu_b200_mla_attn_fp8kv, any sq;
+      - sq == 1: chitu_b200_mla_decode (the one query row sees every key: it takes no `causal`);
+      - sq > 1: chitu_b200_mla_paged_prefill.
+    q_nope [B, H, C] (sq = 1) or [B, sq, H, C], q_pe the same with R; new_kv: the B * sq new rows or None; out None
+    (sq == 1): the split merge is left to chitu_b200_mla_absorb_o_merge_quant.  The entries and their arguments are
+    described in include/chitu_b200.h; the caller checks the tensors."""
+    lib = _lib.load()
+    B, H, C, R = q_nope.shape[0], q_nope.shape[-2], q_nope.shape[-1], q_pe.shape[-1]
+    sq = q_nope.shape[1] if q_nope.dim() == 4 else 1
+    num_blocks, page, _ = kv_cache.shape
+    head = (ptr(q_nope), ptr(q_pe), ptr(kv_cache), ptr(new_kv), ptr(seqlens_excl), ptr(block_table),
+            block_table.stride(0), B)
+    hint, scale = int(max_seqlen_hint), float(softmax_scale)
+    tail = (ptr(out), ptr(workspace), workspace.numel(), current_stream())
+    if kv_cache.dtype == torch.float8_e4m3fn:
+        fn, name = lib.chitu_b200_mla_attn_fp8kv, "mla_attn_fp8kv"
+    elif sq == 1:
+        check(lib.chitu_b200_mla_decode(*head, H, C, R, page, num_blocks, hint, scale, *tail), "mla_decode")
+        return
+    else:
+        fn, name = lib.chitu_b200_mla_paged_prefill, "mla_paged_prefill"
+    check(fn(*head, sq, H, C, R, page, num_blocks, hint, int(bool(causal)), scale, *tail), name)

@@ -22,6 +22,7 @@ import torch
 
 from . import _lib
 from ._lib import check, current_stream, ptr
+from .attn_backend import gqa_paged_attention
 from .quantize import fp8, w4a16
 from .tensor_parallel import global_argmax
 
@@ -272,16 +273,18 @@ class DecodeEngine:
         self.k_rot = torch.zeros(rows, Hkv, D, dtype=BF, device=dev)
         self.attn_out = torch.zeros(rows, Hq * D, dtype=BF, device=dev)
 
-    def _gqa_decode(self, li):
-        """Paged GQA decode of layer li over the bf16 caches: q / k rotated in q_rot / k_rot, v in the qkv output; the
-        new k / v rows are appended at seq_lens."""
-        D, qkv_w = self.D, self.qkv.shape[1]
+    def _gqa_attention(self, li, q, k, sq=1, rope=None):
+        """Paged GQA attention of layer li into attn_out: sq query rows per request (row b * sq + i is token i of
+        request b), q and the new k rows as given (any row stride), v in the qkv output.  The new k / v rows are
+        appended at seq_lens[b] + i and query i attends causally.  rope: the (cos, sin) rows that rotate q and k inside
+        the kernel (sq == 1); without it they are rotated already."""
+        D = self.D
         v = self.qkv[:, (self.Hq + self.Hkv) * D:]
-        check(self.lib.chitu_b200_gqa_paged_decode(
-            ptr(self.q_rot), ptr(self.k_cache[li]), ptr(self.v_cache[li]), ptr(self.k_rot), ptr(v), self.Hkv * D, qkv_w,
-            ptr(self.seq_lens), ptr(self.block_table), self.max_blocks, self.B, self.Hq, self.Hkv, D, self.page,
-            self.max_seq_len, 1.0 / math.sqrt(D), ptr(self.attn_out), ptr(self.attn_ws), self.attn_ws.numel(),
-            _lib.CB_BF16, current_stream()), "gqa_paged_decode")
+        kv_strides = (sq * k.stride(0), k.stride(0) if sq > 1 else 0, sq * v.stride(0), v.stride(0) if sq > 1 else 0)
+        ws = self.attn_ws if sq == 1 else self.verify_attn_ws
+        gqa_paged_attention(q, sq * q.stride(0), self.k_cache[li], self.v_cache[li], k, v, kv_strides, rope,
+                            self.seq_lens, self.block_table, self.B, sq, self.Hq, self.max_seq_len, True,
+                            1.0 / math.sqrt(D), self.attn_out, ws)
 
     # ---- the MoE block (Mixtral, DeepSeek) ------------------------------------------------------------
     def _init_moe(self, n_routed: int, topk: int, slots: int, n_stacked: int, n1: int, score_mode: int,
@@ -580,29 +583,6 @@ class LlamaDecodeEngine(DecodeEngine):
                                                     current_stream()), "quant_fp8_rowwise")
         return self.xq
 
-    def _verify_attention(self, li, sq):
-        """Rotary over the B * sq rows, then causal attention of each request's sq queries over its cache and its sq
-        new K / V rows, which are appended at seq_lens[b] .. seq_lens[b] + sq - 1."""
-        lib, B, D, st = self.lib, self.B, self.D, current_stream()
-        qkv_w = (self.Hq + 2 * self.Hkv) * D
-        M = B * sq
-        check(lib.chitu_b200_rotary_interleaved(ptr(self.qkv), ptr(self.qkv[:, self.Hq * D:]), ptr(self.q_rot),
-                                                ptr(self.k_rot), ptr(self.verify_cos), ptr(self.verify_sin), M, self.Hq,
-                                                self.Hkv, D, qkv_w, D, qkv_w, D, _lib.CB_BF16, st), "rotary")
-        v_view = self.qkv[:, (self.Hq + self.Hkv) * D:]
-        kv_strides = (sq * self.Hkv * D, self.Hkv * D, sq * qkv_w, qkv_w)
-        tail = (ptr(self.seq_lens), ptr(self.block_table), self.max_blocks, B, sq, self.Hq, self.Hkv, D, self.page,
-                self.k_cache.shape[1], self.max_seq_len, 1, 1.0 / math.sqrt(D), ptr(self.attn_out),
-                ptr(self.verify_attn_ws), self.verify_attn_ws.numel(), _lib.CB_BF16, st)
-        if self.kv_fp8:
-            check(lib.chitu_b200_gqa_paged_attn_fp8kv(ptr(self.q_rot), sq * self.Hq * D, ptr(self.k_cache[li]),
-                                                      ptr(self.v_cache[li]), ptr(self.k_rot), ptr(v_view), *kv_strides,
-                                                      None, None, *tail), "gqa_paged_attn_fp8kv")
-        else:
-            check(lib.chitu_b200_gqa_paged_prefill(ptr(self.q_rot), ptr(self.k_cache[li]), ptr(self.v_cache[li]),
-                                                   ptr(self.k_rot), ptr(v_view), *kv_strides, *tail),
-                  "gqa_paged_prefill")
-
     def _decode_layers(self, sq=1):
         """The layers over B * sq rows: the decode step (sq = 1) or the verify step (sq = max_draft + 1)."""
         lib, B, D = self.lib, self.B * sq, self.D
@@ -620,29 +600,17 @@ class LlamaDecodeEngine(DecodeEngine):
             last = li + 1 == n_layers
             next_norm = self.norm if last else self.layers[li + 1]["attn_norm"]
             self._layer_linear(x_in, lw, "wqkv", self.qkv, B)
-            q_view, k_view = self.qkv, self.qkv[:, self.Hq * D:]
-            v_view = self.qkv[:, (self.Hq + self.Hkv) * D:]
-            if sq > 1:
-                self._verify_attention(li, sq)
-            elif self.kv_fp8:
-                # the same fused rotary over the e4m3 caches; the new k / v rows are rounded to e4m3 as they are stored
-                check(lib.chitu_b200_gqa_paged_attn_fp8kv(
-                    ptr(q_view), qkv_w, ptr(self.k_cache[li]), ptr(self.v_cache[li]), ptr(k_view), ptr(v_view), qkv_w, 0,
-                    qkv_w, 0, ptr(self.cos), ptr(self.sin), ptr(self.seq_lens), ptr(self.block_table), self.max_blocks, B,
-                    1, self.Hq, self.Hkv, D, self.page, self.k_cache.shape[1], self.max_seq_len, 1, 1.0 / math.sqrt(D),
-                    ptr(self.attn_out), ptr(self.attn_ws), self.attn_ws.numel(), _lib.CB_BF16, st), "gqa_paged_attn_fp8kv")
-            elif self.fuse_rope:
-                # rotary (q and the new k) inside the attention kernel: q / k / v are views of the qkv GEMM output
-                check(lib.chitu_b200_gqa_paged_decode_rope(
-                    ptr(q_view), qkv_w, ptr(self.k_cache[li]), ptr(self.v_cache[li]), ptr(k_view), ptr(v_view), qkv_w, qkv_w,
-                    ptr(self.cos), ptr(self.sin), ptr(self.seq_lens), ptr(self.block_table), self.max_blocks, B, self.Hq,
-                    self.Hkv, D, self.page, self.max_seq_len, 1.0 / math.sqrt(D), ptr(self.attn_out), ptr(self.attn_ws),
-                    self.attn_ws.numel(), _lib.CB_BF16, st), "gqa_paged_decode_rope")
+            k_view = self.qkv[:, self.Hq * D:]
+            if sq == 1 and self.fuse_rope:
+                # rotary (q and the new k) inside the attention kernel: q / k / v are views of the qkv GEMM output; an
+                # e4m3 cache (which implies fuse_rope) rounds the new k / v rows to e4m3 as they are stored
+                self._gqa_attention(li, self.qkv, k_view, rope=(self.cos, self.sin))
             else:
-                check(lib.chitu_b200_rotary_interleaved(ptr(q_view), ptr(k_view), ptr(self.q_rot), ptr(self.k_rot),
-                                                        ptr(self.cos), ptr(self.sin), B, self.Hq, self.Hkv, D, qkv_w, D,
-                                                        qkv_w, D, _lib.CB_BF16, st), "rotary")
-                self._gqa_decode(li)
+                cos, sin = (self.cos, self.sin) if sq == 1 else (self.verify_cos, self.verify_sin)
+                check(lib.chitu_b200_rotary_interleaved(ptr(self.qkv), ptr(k_view), ptr(self.q_rot), ptr(self.k_rot),
+                                                        ptr(cos), ptr(sin), B, self.Hq, self.Hkv, D, qkv_w, D, qkv_w, D,
+                                                        _lib.CB_BF16, st), "rotary")
+                self._gqa_attention(li, self.q_rot, self.k_rot, sq)
             # h2 = wo(o) + h
             self._row_parallel(lambda out, res: self._layer_linear(self._quant(self.attn_out, B), lw, "wo", out, B,
                                                                    residual=res),

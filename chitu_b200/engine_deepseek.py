@@ -19,6 +19,7 @@ from typing import Optional
 import torch
 
 from ._lib import check, current_stream, ptr
+from .attn_backend import mla_paged_attention
 from .engine import DecodeEngine
 
 BF = torch.bfloat16
@@ -221,18 +222,8 @@ class DeepSeekDecodeEngine(DecodeEngine):
 
     def _mla_decode(self, li):
         """paged absorbed-MLA decode, appending new_kv; the split-KV partials stay in the workspace"""
-        if self.kv_cache.dtype == F8:
-            check(self.lib.chitu_b200_mla_attn_fp8kv(
-                ptr(self.q_abs), ptr(self.q_pe), ptr(self.kv_cache[li]), ptr(self.new_kv), ptr(self.seq_lens),
-                ptr(self.block_table), self.max_blocks, self.B, 1, self.H, self.C, self.R, self.page,
-                self.kv_cache.shape[1], self.max_seq_len, 1, float(self.cfg.softmax_scale), None, ptr(self.attn_ws),
-                self.attn_ws.numel(), current_stream()), "mla_attn_fp8kv")
-            return
-        check(self.lib.chitu_b200_mla_decode(ptr(self.q_abs), ptr(self.q_pe), ptr(self.kv_cache[li]), ptr(self.new_kv),
-                                             ptr(self.seq_lens), ptr(self.block_table), self.max_blocks, self.B, self.H,
-                                             self.C, self.R, self.page, self.kv_cache.shape[1], self.max_seq_len,
-                                             float(self.cfg.softmax_scale), None, ptr(self.attn_ws),
-                                             self.attn_ws.numel(), current_stream()), "mla_decode")
+        mla_paged_attention(self.q_abs, self.q_pe, self.kv_cache[li], self.new_kv, self.seq_lens, self.block_table,
+                            self.max_seq_len, True, self.cfg.softmax_scale, None, self.attn_ws)
 
     # ---- one decode step ---------------------------------------------------------------------------
     def _decode_layers(self):

@@ -104,7 +104,7 @@ class MixtralDecodeEngine(DecodeEngine):
                                                      _lib.CB_BF16, st), "rotary_half q")
             check(lib.chitu_b200_rotary_half_strided(ptr(k), qkv_w, ptr(self.k_rot), ptr(self.cos), ptr(self.sin), B, self.Hkv, D,
                                                      _lib.CB_BF16, st), "rotary_half k")
-            self._gqa_decode(li)
+            self._gqa_attention(li, self.q_rot, self.k_rot)
             self._row_parallel(lambda out, res: self._layer_linear(self.attn_out, lw, "wo", out, B, residual=res),
                                lambda: self.comm.linear_push(self.attn_out, lw["wo"], B, self.lin_ws),
                                h, h2, lw["ffn_norm"], y=self.xn)

@@ -160,6 +160,7 @@ MODES = {
     "deepseek_tp_push": (lambda: _deepseek(**_TP), "push", STEP),
     "deepseek_tp_pull": (lambda: _deepseek(**_TP), "pull", STEP),
     "deepseek_tp_nccl": (lambda: _deepseek(**_TP), "nccl", STEP),
+    "deepseek_e4m3_kv": (lambda: _deepseek(tp_size=1, **_E4M3), None, STEP),
     "mixtral_shard": (lambda: _mixtral(tp_size=2), None, STEP),
     "mixtral_tp_push": (lambda: _mixtral(**_TP), "push", STEP),
     "mixtral_tp_pull": (lambda: _mixtral(**_TP), "pull", STEP),
@@ -167,6 +168,7 @@ MODES = {
     "llama_w4a16": (lambda: _llama(128, weight_format="w4a16"), None, STEP),
     "llama_w4a16_shard": (lambda: _llama(128, tp_size=2, weight_format="w4a16"), None, STEP),
     "llama_fp8": (lambda: _llama(128, weight_format="fp8"), None, STEP),
+    "llama_e4m3_kv": (lambda: _llama(128, **_E4M3), None, STEP),
     "llama_fp8_e4m3_kv": (lambda: _llama(128, weight_format="fp8", **_E4M3), None, STEP),
     "mixtral_w4a16": (lambda: _mixtral(tp_size=1, weight_format="w4a16"), None, STEP),
     "mixtral_w4a16_shard": (lambda: _mixtral(tp_size=2, weight_format="w4a16"), None, STEP),

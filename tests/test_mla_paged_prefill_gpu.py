@@ -128,6 +128,23 @@ def test_mla_attn_with_kvcache_multi_token_refuses_cpu_tensors():
         _call(_backend(), c)
 
 
+def test_mla_attn_with_kvcache_bf16_python_refusals():
+    be = _backend()
+    one = make_case(1, 1, 16, [10], True, device="cpu")
+    one = dict(one, q_nope=one["q_nope"][:, 0], q_pe=one["q_pe"][:, 0])        # the 3-D single-token q
+    cases = (one, make_case(1, 4, 16, [10], True, device="cpu"))
+    for c in cases:
+        with pytest.raises(RuntimeError):
+            _call(be, c)                                                        # CPU tensors
+    if not torch.cuda.is_available():
+        return
+    for c in cases:
+        g = {k: (v.cuda() if torch.is_tensor(v) else v) for k, v in c.items()}
+        for kw in (dict(window_size=(16, 0)), dict(softcap=30.0)):
+            with pytest.raises(RuntimeError):
+                _call(be, g, **kw)
+
+
 def test_reference_equals_oracle_decode_at_one_token():
     from oracle.chitu_oracle import mla_attn_with_kvcache, mla_decode
     c = make_case(3, 1, 16, [5, 300, 64], True, seed=1, device="cpu")
