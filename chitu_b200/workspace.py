@@ -19,6 +19,7 @@ from . import _lib
 
 _ws = {}
 _retired = []
+LINEAR_MAX_TILE_ROWS = 128     # pick_bn (csrc/gemm_tc.cu): chitu_b200_linear_workspace_bytes is the same for any M >= it
 
 
 def _round_up_pow2(n: int) -> int:
@@ -68,7 +69,9 @@ def reserve_decode(device, max_reqs: int, *, heads: int = 128, head_dim_v: int =
     lib = _lib.load()
     B = max(int(max_reqs), 1)
     reserve("attn", attn_bytes(B, heads, head_dim_v, attn_cap_bytes), device)
-    reserve("linear", lib.chitu_b200_linear_workspace_bytes(B, max_out_features), device)
+    # the linears' workspace stops growing at the GEMM's widest token tile, LINEAR_MAX_TILE_ROWS rows: reserving that
+    # covers the B * (k + 1) rows of a speculative verify step as well as B (about 18 MB on 132 SMs)
+    reserve("linear", lib.chitu_b200_linear_workspace_bytes(max(B, LINEAR_MAX_TILE_ROWS), max_out_features), device)
     reserve("moe", lib.chitu_b200_moe_workspace_bytes(B, topk, num_experts, expert_n1, expert_k), device)
     reserve("moe_gate", lib.chitu_b200_moe_gate_workspace_bytes(B, max(num_experts, 8)), device)
 
