@@ -1,8 +1,10 @@
 """One-shot all-reduce over NVLink peer memory fused with residual add + RMSNorm (+ FP8 quant).
 
 Host side only does the plumbing: create the symmetric buffer in the C library, exchange the CUDA IPC
-handles with `torch.distributed.all_gather_object`, connect.  The data path is the
-`allreduce_norm_kernel` of csrc/comm.cu (SURVEY §5.8: 122 latency-bound all-reduces per DeepSeek step)."""
+handles with `torch.distributed.all_gather_object`, connect.  The reduce runs in csrc/comm.cu (SURVEY §5.8: 122
+latency-bound all-reduces per DeepSeek step): `consume` after a product whose epilogue pushed its partial into every
+rank's push area (`fp8_gemm_push`, `linear_push`, `experts_push`), `__call__` (the pull kernel `allreduce_norm_kernel`)
+for a partial written by a product without that epilogue."""
 from __future__ import annotations
 
 import ctypes

@@ -1022,8 +1022,8 @@ __global__ void __launch_bounds__(256) mla_absorb_o_kernel(const __nv_bfloat16* 
         *reinterpret_cast<uint2*>(out + o) = make_uint2(pack2(v[0], v[1], tag), pack2(v[2], v[3], tag));
       }
       if (q_out) {
-        const E4m3Word g = e4m3_group_quant<E4m3Group::kActQuant>(v);
-        *reinterpret_cast<uint32_t*>(q_out + o) = g.bits;
+        const E4m3Word<4> g = e4m3_group_quant<E4m3Group::kActQuant>(v);
+        *reinterpret_cast<uint32_t*>(q_out + o) = g.bits[0];
         if (lane == 0) q_scales[((int64_t)(b0 + m) * H + h) * (dv / 128) + d0 / 128] = g.scale;
       }
     }

@@ -249,9 +249,13 @@ int gqa_prefill(const char* entry, const char* name, KvLayout layout, const void
                 int dtype, cudaStream_t st);
 
 #ifdef __CUDACC__
+// byte offset of source `src`'s words inside a push buffer of `world` sources, for the reduce after `calls`
+__device__ __forceinline__ int64_t push_area(uint32_t calls, int world, int src, int64_t ll_bytes) {
+  return ((int64_t)(calls & 1u) * world + src) * ll_bytes;
+}
 // byte offset of this rank's area inside every push buffer, for the reduce that is being produced
 __device__ __forceinline__ int64_t push_area(const PushDev& d, uint32_t calls) {
-  return ((int64_t)(calls & 1u) * d.world + d.rank) * d.ll_bytes;
+  return push_area(calls, d.world, d.rank, d.ll_bytes);
 }
 // one word to every rank: word_off = byte offset inside the area (k * 8)
 __device__ __forceinline__ void push_word(const PushDev& d, int64_t off, uint32_t two_bf16, uint32_t epoch) {
@@ -393,25 +397,43 @@ __device__ __forceinline__ int64_t block_argmax_1024(const T* row, int64_t V, fl
   return si[0];
 }
 
-// ---- e4m3 group quantisation: one warp per 128-element group, 4 consecutive elements per lane ---------------------
-// scale = amax / 448 and q = v / scale, both divided as torch divides (__fdiv_rn), bit-exact with one of two references:
-// kActQuant (act_quant_deepseek_v3) takes amax as is and leaves q unclamped; kPerTokenGroup (per_token_group_quant_fp8)
-// floors amax at 1e-10 and clamps q to +-448, which also turns a NaN q (kept as NaN by float_to_fp8) into -448.
+// ---- e4m3 group quantisation: 128-element groups over 128 / N aligned lanes, N = 4 (a warp) or 8 consecutive elements
+// per lane.  scale = amax / 448 and q = v / scale, both divided as torch divides (__fdiv_rn), bit-exact with one of two
+// references: kActQuant (act_quant_deepseek_v3) takes amax as is and leaves q unclamped; kPerTokenGroup
+// (per_token_group_quant_fp8) floors amax at 1e-10 and clamps q to +-448, which also turns a NaN q (kept as NaN by
+// float_to_fp8) into -448.
 enum class E4m3Group { kActQuant, kPerTokenGroup };
-struct E4m3Word { uint32_t bits; float scale; };    // the lane's element i in byte i; the group's scale, on every lane
-template <E4m3Group kRule>
-__device__ __forceinline__ E4m3Word e4m3_group_quant(const float (&v)[4]) {
-  float amax = warp_max(fmaxf(fmaxf(fabsf(v[0]), fabsf(v[1])), fmaxf(fabsf(v[2]), fabsf(v[3]))));
+// the lane's element i in byte i % 4 of bits[i / 4]; the group's scale, on every lane
+template <int N>
+struct E4m3Word { uint32_t bits[N / 4]; float scale; };
+// max |v[I .. I + N)| as the pairwise tree fmaxf(max of the first half, max of the second half)
+template <int I, int N>
+__device__ __forceinline__ float abs_max(const float* v) {
+  if constexpr (N == 1) return fabsf(v[I]);
+  else return fmaxf(abs_max<I, N / 2>(v), abs_max<I + N / 2, N / 2>(v));
+}
+template <E4m3Group kRule, int N>
+__device__ __forceinline__ E4m3Word<N> e4m3_group_quant(const float (&v)[N]) {
+  static_assert(N == 4 || N == 8, "a lane holds 4 or 8 elements of its group");
+  float amax = abs_max<0, N>(v);
+#pragma unroll
+  for (int o = 64 / N; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
   if constexpr (kRule == E4m3Group::kPerTokenGroup) amax = fmaxf(amax, 1e-10f);
   const float sc = __fdiv_rn(amax, 448.0f);
-  uint32_t bits = 0;
+  E4m3Word<N> w;
 #pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    float q = __fdiv_rn(v[i], sc);
-    if constexpr (kRule == E4m3Group::kPerTokenGroup) q = fminf(fmaxf(q, -448.f), 448.f);
-    bits |= (uint32_t)float_to_fp8(q) << (8 * i);
+  for (int k = 0; k < N / 4; ++k) {
+    uint32_t bits = 0;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      float q = __fdiv_rn(v[4 * k + i], sc);
+      if constexpr (kRule == E4m3Group::kPerTokenGroup) q = fminf(fmaxf(q, -448.f), 448.f);
+      bits |= (uint32_t)float_to_fp8(q) << (8 * i);
+    }
+    w.bits[k] = bits;
   }
-  return {bits, sc};
+  w.scale = sc;
+  return w;
 }
 
 }  // namespace cb

@@ -275,8 +275,8 @@ __global__ void __launch_bounds__(256) rmsnorm_quant_kernel(const __nv_bfloat16*
         *reinterpret_cast<uint2*>(y + row * y_stride + e) = make_uint2(pack2(o[0], o[1], tag), pack2(o[2], o[3], tag));
       }
       if (q) {                                      // a warp covers exactly one 128-element group
-        const E4m3Word g = e4m3_group_quant<E4m3Group::kActQuant>(o);
-        *reinterpret_cast<uint32_t*>(q + row * dim + e) = g.bits;
+        const E4m3Word<4> g = e4m3_group_quant<E4m3Group::kActQuant>(o);
+        *reinterpret_cast<uint32_t*>(q + row * dim + e) = g.bits[0];
         if (lane == 0) qs[row * (dim / 128) + (e >> 7)] = g.scale;
       }
     }
@@ -457,8 +457,8 @@ __global__ void silu_mul_quant_kernel(const __nv_bfloat16* __restrict__ x, uint8
     const float sl = __bfloat162float(__float2bfloat16_rn(gv[i] / (1.f + expf(-gv[i]))));
     v[i] = __bfloat162float(__float2bfloat16_rn(sl * uv[i]));
   }
-  const E4m3Word g = e4m3_group_quant<E4m3Group::kActQuant>(v);
-  *reinterpret_cast<uint32_t*>(q + r * F + gk * 128 + lane * 4) = g.bits;
+  const E4m3Word<4> g = e4m3_group_quant<E4m3Group::kActQuant>(v);
+  *reinterpret_cast<uint32_t*>(q + r * F + gk * 128 + lane * 4) = g.bits[0];
   if (lane == 0) qs[r * groups + gk] = g.scale;
 }
 

@@ -680,8 +680,8 @@ __global__ void moe_gather_quant_kernel(const __nv_bfloat16* __restrict__ x, con
     return;
   }
   const float v[4] = {bf16lo(raw.x), bf16hi(raw.x), bf16lo(raw.y), bf16hi(raw.y)};
-  const E4m3Word g = e4m3_group_quant<E4m3Group::kPerTokenGroup>(v);
-  *reinterpret_cast<uint32_t*>(xq + (int64_t)r * K + gk * 128 + lane * 4) = g.bits;
+  const E4m3Word<4> g = e4m3_group_quant<E4m3Group::kPerTokenGroup>(v);
+  *reinterpret_cast<uint32_t*>(xq + (int64_t)r * K + gk * 128 + lane * 4) = g.bits[0];
   if (lane == 0) xs[(int64_t)r * groups + gk] = g.scale;
 }
 
@@ -710,8 +710,8 @@ __global__ void moe_silu_quant_kernel(const __nv_bfloat16* __restrict__ c1, cons
     *reinterpret_cast<uint2*>(ab + (int64_t)r * F + gk * 128 + lane * 4) = o;
     return;
   }
-  const E4m3Word g = e4m3_group_quant<E4m3Group::kPerTokenGroup>(v);
-  *reinterpret_cast<uint32_t*>(aq + (int64_t)r * F + gk * 128 + lane * 4) = g.bits;
+  const E4m3Word<4> g = e4m3_group_quant<E4m3Group::kPerTokenGroup>(v);
+  *reinterpret_cast<uint32_t*>(aq + (int64_t)r * F + gk * 128 + lane * 4) = g.bits[0];
   if (lane == 0) as[(int64_t)r * groups + gk] = g.scale;
 }
 
@@ -966,8 +966,8 @@ __global__ void moe_rows_gather_kernel(const __nv_bfloat16* __restrict__ A, cons
     return;
   }
   const float v[4] = {bf16lo(raw.x), bf16hi(raw.x), bf16lo(raw.y), bf16hi(raw.y)};
-  const E4m3Word g = e4m3_group_quant<E4m3Group::kPerTokenGroup>(v);
-  *reinterpret_cast<uint32_t*>(xq + (int64_t)r * K + gk * 128 + lane * 4) = g.bits;
+  const E4m3Word<4> g = e4m3_group_quant<E4m3Group::kPerTokenGroup>(v);
+  *reinterpret_cast<uint32_t*>(xq + (int64_t)r * K + gk * 128 + lane * 4) = g.bits[0];
   if (lane == 0) xs[(int64_t)r * groups + gk] = g.scale;
 }
 

@@ -14,7 +14,6 @@ Mixtral (engine_mixtral.py) engines add their weights and their layers.
 from __future__ import annotations
 
 import math
-import os
 from dataclasses import dataclass
 from typing import Optional
 
@@ -117,8 +116,9 @@ class DecodeEngine:
                                    dtype=torch.uint8, device=dev)
         self.lin_ws = torch.zeros(max(self.lib.chitu_b200_linear_workspace_bytes(rows, lin_n), 256), dtype=torch.uint8,
                                   device=dev)                    # split-K tickets start at 0
-        # push mode: the row-parallel GEMM's epilogue starts the all-reduce; "0" selects the pull kernel
-        self.ar_push = os.environ.get("CHITU_B200_AR_PUSH", "1") != "0"
+        # push mode: the row-parallel product's epilogue starts the all-reduce (every product the base and the
+        # DeepSeek / Mixtral engines reduce has a push epilogue; the pull kernel reduces products without one)
+        self.ar_push = True
         # fused one-shot all-reduce + residual + RMSNorm(+quant) over NVLink peer memory (csrc/comm.cu); NCCL otherwise
         self.comm = None
         if self.tp_on and use_fused_allreduce:
@@ -493,7 +493,7 @@ class LlamaDecodeEngine(DecodeEngine):
         # (row 2i = gate_i, row 2i+1 = up_i) — a load-time permutation of the reference's merged tensor.
         # It and push mode need the wgmma GEMM, which linear_impl=1 (the SIMT GEMV) turns off.
         self.fuse_silu = linear_impl != 1
-        self.ar_push = self.ar_push and linear_impl != 1
+        self.ar_push = linear_impl != 1
         self.embed = rnd(self.g_rep, cfg.vocab_size, dim)
         self.layers = []
         for _ in range(cfg.n_layers):

@@ -389,6 +389,65 @@ def test_consumer_sums_the_sources_in_rank_order(world):
         comm.close()
 
 
+# ------------------------------------------------------------------------------------------ refusals of both reduces
+SHAPE_CHECK = "rows >= 0 && rows <= kMaxRows && dim > 0 && dim % 8 == 0 && dim <= 8192"
+# entry -> (its C name, its first check)
+REDUCE_ENTRIES = {"pull": ("chitu_b200_allreduce_residual_rmsnorm", "handle && partial && " + SHAPE_CHECK),
+                  "consume": ("chitu_b200_allreduce_consume", "handle && " + SHAPE_CHECK)}
+# (arguments changed from a valid 16 x 512 call with every output, the failed check; None: the entry's first check)
+REDUCE_REFUSALS = (
+    (dict(handle=None), None), (dict(partial=None), None), (dict(rows=-1), None), (dict(rows=257), None),
+    (dict(dim=0), None), (dict(dim=12), None), (dict(dim=8200), None),
+    (dict(h=None, norm_w=None, y=None, q=None, qs=None), "h_out || norm_w"),
+    (dict(qs=None), "(q == nullptr) == (q_scales == nullptr)"),
+    (dict(q=None), "(q == nullptr) == (q_scales == nullptr)"),
+    (dict(dim=264), "q == nullptr || (norm_w && dim % 256 == 0)"),
+    (dict(norm_w=None, y=None), "q == nullptr || (norm_w && dim % 256 == 0)"),
+    (dict(rows=17), "(int64_t)rows * dim * 2 <= c->slot_bytes"),
+)
+
+
+@pytest.mark.gpu
+def test_reduce_refusals_launch_nothing():
+    """Both reduce entries refuse each bad argument with -1 and the message of the check that failed, under the entry's
+    own name; nothing is launched or written, and the call counter stays.  rows = 0 returns 0 and launches nothing."""
+    from chitu_b200._lib import launch_count
+    lib = _lib()
+    comm = Comm(0, 1, 16 * 512 * 2)
+    try:
+        n = 257 * 8200                                           # elements of the widest refused shape
+        bufs = {k: torch.full((n,), -1, dtype=torch.int32, device=DEV) for k in ("partial", "res", "h", "norm_w", "y",
+                                                                                   "q", "qs")}
+        comm.area.fill_(POISON)
+        torch.cuda.synchronize()
+        before = launch_count()
+        for entry, (name, first) in REDUCE_ENTRIES.items():
+            for change, check in REDUCE_REFUSALS + ((dict(rows=0), 0),):
+                if entry == "consume" and "partial" in change:
+                    continue
+                a = dict(handle=comm.h, rows=16, dim=512, **{k: _ptr(t) for k, t in bufs.items()})
+                a.update(change)
+                if entry == "pull":
+                    rc = lib.chitu_b200_allreduce_residual_rmsnorm(a["handle"], a["partial"], a["res"], a["h"],
+                                                                   a["norm_w"], a["y"], a["q"], a["qs"], a["rows"],
+                                                                   a["dim"], EPS, _stream())
+                else:
+                    rc = lib.chitu_b200_allreduce_consume(a["handle"], a["res"], a["h"], a["norm_w"], a["y"], a["q"],
+                                                          a["qs"], a["rows"], a["dim"], EPS, _stream())
+                if check == 0:
+                    assert rc == 0, (entry, change, _last_error())
+                else:
+                    assert rc == -1, (entry, change, rc)
+                    want = f"{name}: argument check failed: {first if check is None else check}"
+                    assert _last_error() == want, (entry, change, _last_error())
+        torch.cuda.synchronize()
+        assert launch_count() == before
+        assert all(bool((t == -1).all()) for t in bufs.values())
+        assert bool((comm.area == POISON).all()) and comm.calls() == 0 and comm.status() == 0
+    finally:
+        comm.close()
+
+
 # --------------------------------------------------------------------------------------- GEMM push epilogues, W = 1
 def _push_gemm(call, comm, ws, nbytes=None):
     """the _ar entry of a G Call's operands (no bias, no residual)"""
